@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Headline benchmark: mel-frames/sec of the Grad-TTS reverse-diffusion sampler at N=50 steps.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One bench "step" = one full `Diffusion.forward(z, mask, mu, n_timesteps=50)` call on the workload
@@ -12,6 +12,10 @@ weak scaling: every rank samples its own 32 utterances, outputs all-gathered).  
   e2e          same metric through the host-buffer entry point (pinned host tensors in/out, copies timed)
   roofline     the dominant kernel class (3x3 conv implicit GEMMs), timed per launch with CUDA events
   cpu_baseline the CPU oracle (a port of the reference's PyTorch path) on a bounded sample, this box's cores
+
+--dump-outputs DIR writes the mel the last timed step returned (all ranks' utterances, gathered) as DIR/mel.npy (float32
+[world * B, 80, T]); the GPU arm only (the CPU arm's bounded sample is not the workload's output).  The inputs
+and weights are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -26,7 +30,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 WORKLOADS = {
-    # BASELINE.json configs[1]: Grad-TTS batch=32, T~512, N=50, fp32, 1xB200
+    # BASELINE.json configs[1]: Grad-TTS batch=32, T~512, N=50, fp32, one GPU
     "gradtts_b32_t512_n50": dict(B=32, T=512, N=50, n_spks=1),
     # BASELINE.json configs[4]'s per-GPU share (2048 utterances over 8 GPUs = 256 per GPU); not the default bench line:
     #   torchrun --nproc-per-node 8 bench.py --gpus 8 --workload gradtts_b256_t512_n50 --steps 2 --warmup 3 --no-fp32-leg
@@ -41,7 +45,7 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm_gbs=6650.0, bf16=1400.0, src="fallback")
+    return dict(hbm_gbs=3350.0, bf16=989.0, src="H100 SXM data-sheet")
 
 
 def measure_tf32_matmul_tflops(torch, dev, seconds=1.0):
@@ -74,7 +78,7 @@ def measure_tf32_matmul_tflops(torch, dev, seconds=1.0):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -244,28 +248,17 @@ def bench_config(args, wl, world, **extra):
 
 # per-mode arithmetic + the parity bound its tests hold it to (tests/test_fp32x3_gpu.py, tests/test_parity_gpu.py)
 MODES = {
-    "fp32x3": dict(dtype="f32", what="fp32-class on tcgen05: x*w = x_hi*w_hi (kind::tf32) + (x_lo*w + x*w_lo) as one kind::f16 MMA over packed "
+    "fp32x3": dict(dtype="f32", what="fp32-class on wgmma: x*w = x_hi*w_hi (tf32) + (x_lo*w + x*w_lo) as one f16 MMA over packed "
                                      "fp16 correction chunks, fp32 accumulate with runs folded in fp32; exact fp32 GN/Mish/softmax/Euler",
-                   tol="rel-L2 <= 1e-5 per estimator call vs the reference's fp32 CPU outputs (13 goldens; measured 2.2-2.9e-6), <= 2e-4 on N<=50 trajectories (measured 1.1-1.4e-6)",
+                   tol="rel-L2 <= 1e-5 per estimator call vs the reference's fp32 CPU outputs (13 goldens), <= 2e-4 on N<=50 trajectories",
                    mma_per_mac=2),
-    "tf32": dict(dtype="tf32", what="tcgen05 kind::tf32 operands (PyTorch's default GPU conv arithmetic), fp32 accumulate / GN / softmax / Euler",
-                 tol="rel-L2 <= 4e-3 per estimator call (measured 1.5e-3), <= 8e-3 on trajectories", mma_per_mac=1),
-    "bf16": dict(dtype="bf16", what="bf16 operand tensors + weights on tcgen05 kind::f16 (BASELINE config 3's arithmetic), fp32 accumulate / GN / state",
-                 tol="rel-L2 <= 2e-2 per estimator call (measured 1.1e-2), <= 1e-2 on trajectories", mma_per_mac=1),
+    "tf32": dict(dtype="tf32", what="wgmma tf32 operands (PyTorch's default GPU conv arithmetic), fp32 accumulate / GN / softmax / Euler",
+                 tol="rel-L2 <= 4e-3 per estimator call, <= 8e-3 on trajectories", mma_per_mac=1),
+    "bf16": dict(dtype="bf16", what="bf16 operand tensors + weights on wgmma bf16 (BASELINE config 3's arithmetic), fp32 accumulate / GN / state",
+                 tol="rel-L2 <= 2e-2 per estimator call, <= 1e-2 on trajectories", mma_per_mac=1),
     "fp32": dict(dtype="f32", what="CUDA-core FFMA implicit GEMM (the round-1 exact mode; kept as a second opinion)",
-                 tol="rel-L2 <= 1e-4 per estimator call (measured 0.6-2.6e-6)", mma_per_mac=0),
+                 tol="rel-L2 <= 1e-4 per estimator call", mma_per_mac=0),
 }
-
-
-def csrc_digest():
-    """sha256 over the kernel sources: ties measured side files (profiles/r2_traffic_*.json) to the binary being benched."""
-    import hashlib
-    h = hashlib.sha256()
-    d = os.path.join(ROOT, "speech-backbones_b200", "csrc")
-    for f in sorted(os.listdir(d)):
-        if f.endswith((".cu", ".h")):
-            h.update(open(os.path.join(d, f), "rb").read())
-    return h.hexdigest()[:16]
 
 
 def run_ours(args, wl):
@@ -354,6 +347,11 @@ def run_ours(args, wl):
     dec = make(args.precision)
     eng = dec.engine()
     head = time_mode(dec, args.steps, args.warmup, sample_clocks=True)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        # what a caller of the timed path receives: the all-gathered mel when world > 1
+        np.save(os.path.join(args.dump_outputs, "mel.npy"), (gathered if world > 1 else head["y"]).float().cpu().numpy())
     ms_step, value, launches, clk = head["ms_step"], head["value"], head["launches"], head["clocks"]
 
     # ---- end to end through the host-buffer entry point (pinned host memory in/out, copies inside the timed region)
@@ -435,19 +433,9 @@ def run_ours(args, wl):
              "attention" if (".2." in n or "mid_attn" in n) else "resample" if ".3." in n else
              "final_euler" if n == "estimator.out" else "resblock_tail")
         by_kind[k] = by_kind.get(k, 0.0) + ms
-    # DRAM bytes per launch of the same kernel class from an ncu capture OF THIS BINARY (scripts/ncu_traffic.py writes the
-    # csrc digest next to the bytes); a capture of other kernels is not reported
-    traffic, traffic_src = None, None
-    tpath = os.path.join(ROOT, "profiles", f"r2_traffic_conv3x3_{args.precision}.json")
-    if os.path.exists(tpath) and (B, T) == (32, 512):
-        tj = json.load(open(tpath))
-        if tj.get("csrc_digest") == csrc_digest():
-            traffic, traffic_src = tj["dram_bytes_per_launch"], f"profiles/{os.path.basename(tpath)} (ncu dram__bytes_read+write, {tj['launches']} launches, csrc {tj['csrc_digest']})"
-        else:
-            traffic_src = f"not reported: profiles/{os.path.basename(tpath)} was captured from other kernel sources (csrc {tj.get('csrc_digest')} != {csrc_digest()})"
     roofline = {
         "kernel": "conv3x3 implicit GEMM (25 launches/step)", "bound": "tensor", "achieved": achieved, "peak": tensor_peak,
-        "unit": "TFLOP/s", "frac": achieved / tensor_peak, "traffic": traffic, "traffic_source": traffic_src,
+        "unit": "TFLOP/s", "frac": achieved / tensor_peak,
         "algorithmic_bytes_per_launch": conv_by / max(1, len(conv)),
         "traffic_note": ("fp32x3 reads every conv input twice by design (the fp32 tensor + its 16-byte-per-4-channels correction "
                          "chunks): expected DRAM bytes = algorithmic (4 B in + 4 B out per element) + the input bytes once more"
@@ -485,7 +473,7 @@ def run_ours(args, wl):
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": mode["dtype"], "data": "synthetic",
         "config": bench_config(args, wl, world, precision_mode=args.precision, arithmetic=mode["what"], tolerance=mode["tol"],
-                               l2=f"per-step working set ({eng.workspace_bytes(B, T) / 1e9:.1f} GB of activations) exceeds the 126 MB L2; no flush needed",
+                               l2=f"per-step working set ({eng.workspace_bytes(B, T) / 1e9:.1f} GB of activations) exceeds the 50 MB L2; no flush needed",
                                weights="synthetic seeded (no checkpoints ship with the reference)",
                                weight_broadcast_s=round(bcast_s, 4)),
         "frame_steps_per_s": value * N,
@@ -517,7 +505,7 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="gradtts_b32_t512_n50", choices=sorted(WORKLOADS))
     ap.add_argument("--precision", default="fp32x3", choices=["fp32x3", "fp32", "tf32", "bf16"],
-                    help="fp32x3 (default, the headline: BASELINE config 2 is fp32): fp32-class arithmetic on tcgen05 (tf32 + fp16 correction); "
+                    help="fp32x3 (default, the headline: BASELINE config 2 is fp32): fp32-class arithmetic on wgmma (tf32 + fp16 correction); "
                          "tf32: plain tf32 operands (PyTorch's default GPU conv arithmetic); bf16: bf16 operand tensors "
                          "(BASELINE config 3's arithmetic); fp32: the CUDA-core FFMA path")
     ap.add_argument("--no-extra-legs", "--no-fp32-leg", dest="no_extra_legs", action="store_true",
@@ -527,12 +515,16 @@ def main():
     ap.add_argument("--batch", type=int, default=None, help="override B (debug only; not a valid bench line)")
     ap.add_argument("--frames", type=int, default=None, help="override T (debug only)")
     ap.add_argument("--n-timesteps", type=int, default=None, help="override N (debug only)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the output of the last timed step as DIR/mel.npy (float32)")
     args = ap.parse_args()
     wl = dict(WORKLOADS[args.workload])
     if args.batch: wl["B"] = args.batch
     if args.frames: wl["T"] = args.frames
     if args.n_timesteps: wl["N"] = args.n_timesteps
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs applies to the GPU arm (--impl ours)")
         run_reference(args, wl)
     else:
         run_ours(args, wl)

@@ -1,5 +1,5 @@
 /*
- * sbk.h - C ABI of the B200-native score-based mel sampler (libsbk.so).
+ * sbk.h - C ABI of the H100-native score-based mel sampler (libsbk.so).
  *
  * The reference (huawei-noah/Speech-Backbones) has no FFI layer: its boundary for this
  * path is the Python class `Diffusion` (Grad-TTS/model/diffusion.py:227-279) and its
@@ -30,13 +30,13 @@ enum { SBK_OK = 0, SBK_ERR_ARG = 1, SBK_ERR_CUDA = 2, SBK_ERR_STATE = 3, SBK_ERR
 
 /* arithmetic of the dense contractions (3x3/1x1 convs); GN / softmax / Mish / Euler are always fp32 */
 enum { SBK_PREC_FP32 = 0,   /* CUDA-core FFMA, fp32 operands (bit-faithful class of the CPU reference)   */
-       SBK_PREC_TF32 = 1,   /* tcgen05 kind::tf32, fp32 accumulate in TMEM (PyTorch's default GPU class) */
-       SBK_PREC_BF16 = 2,   /* tcgen05 kind::f16 on bf16 operand tensors (conv inputs + weights stored as bf16),
+       SBK_PREC_TF32 = 1,   /* wgmma tf32, fp32 accumulate in registers (PyTorch's default GPU class) */
+       SBK_PREC_BF16 = 2,   /* wgmma bf16 on bf16 operand tensors (conv inputs + weights stored as bf16),
                                fp32 accumulate; raw conv outputs, GN statistics, softmax, sampler state fp32
                                (BASELINE config 3); both models                                             */
-       SBK_PREC_FP32X3 = 3 };/* fp32-class arithmetic on tcgen05: x*w = x_hi*w_hi (kind::tf32, the tensor core reads
-                               the top 19 bits of x) + (x_lo*w + x*w_lo) as ONE kind::f16 MMA over packed fp16
-                               correction chunks - two MMAs per MAC; fp32 accumulation in TMEM, cut into short runs
+       SBK_PREC_FP32X3 = 3 };/* fp32-class arithmetic on wgmma: x*w = x_hi*w_hi (tf32, the tensor core reads
+                               the top 19 bits of x) + (x_lo*w + x*w_lo) as ONE f16 MMA over packed fp16
+                               correction chunks - two MMAs per MAC; fp32 accumulation in registers, cut into short runs
                                that are summed in round-to-nearest fp32 (the tensor core truncates its accumulator);
                                softmax / Mish / GN exact fp32.  The default of the drop-in modules: matches the
                                reference's fp32 CPU arithmetic to 2-3e-6 per estimator call                   */
@@ -109,7 +109,7 @@ int sbk_vc_reverse_diffusion(sbk_handle* h, const float* z, const float* mask, c
 
 /* The hoisted conditioning branch natively (tensor-core precision modes only): for every step i (t_i = 1 - i/N)
  * xt_ref = compute_diffused_mean(ref, ref_mask, mean_ref, t_i) (:151-155) -> RefBlock (modules.py:156-166: six
- * Conv3x3 + InstanceNorm2d + GLU on tcgen05, two time biases, 1x1 conv, masked mean) -> cond_block over
+ * Conv3x3 + InstanceNorm2d + GLU on wgmma, two time biases, 1x1 conv, masked mean) -> cond_block over
  * [sinusoid(t_i) | RefBlock | c] (:62-71).  ref, mean_ref: [B,n_feats,Tr]; ref_mask: [B,1,Tr]; c: [B,256];
  * cond_out: [N][B][dim_cond], ready for sbk_vc_reverse_diffusion.  Returns SBK_ERR_UNSUPPORTED in fp32 mode. */
 int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float* ref_mask, const float* mean_ref, const float* c,
@@ -179,7 +179,7 @@ const char* sbk_debug_name(const sbk_handle* h, int i);
  * called as `vocoder.forward(y_dec)` at Grad-TTS/inference.py:81 after `remove_weight_norm()` (:63).  The fields below are that
  * JSON's; weights are the generator's state_dict AFTER remove_weight_norm ("conv_pre.weight" [C0,num_mels,7],
  * "ups.i.weight" [Cin,Cout,k], "resblocks.n.convs{1,2}.j.weight" [C,C,k], "conv_post.weight" [1,C,7] and the biases).
- * Dense contractions run on tcgen05 with tf32 operands and fp32 accumulation; everything else is fp32. */
+ * Dense contractions run on wgmma with tf32 operands and fp32 accumulation; everything else is fp32. */
 typedef struct sbk_vocoder sbk_vocoder;
 typedef struct sbk_vocoder_config {
     int32_t device;

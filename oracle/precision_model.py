@@ -4,7 +4,7 @@ Runs oracle/gradtts_oracle.py with every tensor-core operand rounded where libsb
 
   tf32  conv / projection weights: round-to-nearest-away to 10 mantissa bits (host packers, cvt.rna);
         Block activations (the second conv's input): cvt.rna in k_gn_act; every other A operand (residual-stream
-        tensors, the softmax numerators P and V in the context product) is fp32 in memory and the tcgen05 kind::tf32
+        tensors, the softmax numerators P and V in the context product) is fp32 in memory and the tensor core's tf32
         datapath drops the low 13 mantissa bits (truncation);
   bf16  weights and every stored operand tensor (Block activations, ResnetBlock / attention / resample outputs = the
         residual stream) round-to-nearest-even to bf16; P and V as in tf32.
@@ -14,7 +14,7 @@ Runs oracle/gradtts_oracle.py with every tensor-core operand rounded where libsb
         float64 here, so the model isolates the OPERAND roundings of the mode from fp32 accumulation effects).
 
 It predicts the error of a precision mode from its rounding points alone, so tests can check that the error MEASURED on
-the GPU (profiles/r1_bf16_bringup.log) is explained by operand rounding and by nothing else.  It is a model, not a
+the GPU (scripts/gpu_vs_precision_model.py) is explained by operand rounding and by nothing else.  It is a model, not a
 bit-exact emulator: accumulation order, the folded attention matrix and the fast Mish are not modelled.
 """
 from __future__ import annotations
@@ -106,7 +106,7 @@ def operand_rounding(mode, p):
             return (T0.einsum(eq, ah.to(d), bh.to(d))
                     + T0.einsum(eq, round_f16_sat((a - ah) * 256.0).to(d), round_f16_sat(b / 256.0).to(d))
                     + T0.einsum(eq, round_f16_sat(a / 16.0).to(d), round_f16_sat((b - bh) * 16.0).to(d))).float()
-        if eq == "bhdn,bhen->bhde":                                            # context = P V^T on the tensor core (tf32, from TMEM)
+        if eq == "bhdn,bhen->bhde":                                            # context = P V^T on the tensor core (tf32, P from shared memory)
             return T0.einsum(eq, trunc_tf32(a), trunc_tf32(b))
         return T0.einsum(eq, a, b)
 

@@ -1,4 +1,4 @@
-"""BASELINE config 3: Grad-TTS batch=128, T=512, N=1000 long-horizon sampler, bf16, one B200.
+"""BASELINE config 3: Grad-TTS batch=128, T=512, N=1000 long-horizon sampler, bf16, one GPU.
 The drop-in module in precision="bf16" is called with bf16 tensors (z, mask, mu) and returns a bf16 tensor; the whole
 N=1000 call is CUDA-event timed after a short warm-up call (plan + graph already built).  Size-independent checks at
 the full size: finite output, padded frames exactly zero, batch entries independent (a 2-utterance slice re-run alone

@@ -1,4 +1,4 @@
-"""BASELINE config 4: DiffVC decoder fast-ML sampler, B=64, T=T_ref=256, N in {6, 30}, mode 'ml', one B200.
+"""BASELINE config 4: DiffVC decoder fast-ML sampler, B=64, T=T_ref=256, N in {6, 30}, mode 'ml', one GPU.
 Reports mel-frames/s for the whole `Diffusion.forward` (hoisted PyTorch conditioning + libsbk loop) and for the loop alone."""
 import json
 import os

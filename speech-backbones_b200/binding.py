@@ -37,7 +37,7 @@ def load_library() -> C.CDLL:
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH):
-        raise RuntimeError(f"{LIB_PATH} not found: build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+        raise RuntimeError(f"{LIB_PATH} not found: build it with `python __graft_entry__.py` (nvcc, sm_90a). "
                            "There is no CPU fallback for the sampler.")
     lib = C.CDLL(LIB_PATH)
     P, I, F = C.c_void_p, C.c_int, C.c_void_p

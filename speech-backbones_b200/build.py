@@ -1,4 +1,4 @@
-"""Build libsbk.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libsbk.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsbk.so")
 SOURCES = ["sbk_api.cu", "sbk_kernels.cu", "sbk_conv_tc.cu", "sbk_attn_x3.cu", "sbk_vocoder.cu", "sbk_textenc.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", *ARCH, "-lineinfo", "-Xcompiler", "-fPIC"]
 
 

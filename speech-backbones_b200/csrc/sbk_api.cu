@@ -226,7 +226,7 @@ static int64_t numel_of(const std::vector<int64_t>& s) { int64_t n = 1; for (aut
 // C ABI: lifecycle + strict loading
 // ------------------------------------------------------------------------------------------------
 extern "C" const char* sbk_last_error(void) { return g_err; }
-extern "C" const char* sbk_version(void) { return "sbk 0.1 (sm_100a)"; }
+extern "C" const char* sbk_version(void) { return "sbk 0.1 (sm_90a)"; }
 
 extern "C" int sbk_create(const sbk_config* cfg, sbk_handle** out) {
     if (!cfg || !out) return fail(SBK_ERR_ARG, "sbk_create: null argument");
@@ -307,15 +307,8 @@ static int repack(sbk_handle* h, const std::string& src, const std::string& key,
     return SBK_OK;
 }
 
-// k_attn_kv_x3: items (64 pixels) per chunk = per partial.  A constant, so that an utterance is cut at the same pixels
-// whatever batch it sits in (alone-vs-in-batch results stay at the rounding level of the partial merge), and short enough
-// that a single utterance still spreads over the GPU (B=1, T=512, level 0: 160 chunks for 148 SMs).
-static int attn_x3_chunk_items(int items_per_sample, int B) {
-    (void)items_per_sample; (void)B;
-    return 4;
-}
 
-// Pack a 3x3 conv weight [co][ci][3][3] into the tcgen05 kernel's per-stage shared-memory image
+// Pack a 3x3 conv weight [co][ci][3][3] into the tensor-core kernel's per-stage shared-memory image
 // [ntile][kstage][tap][16-byte chunk][co % NT][elements]: tf32-rounded fp32 (4 per chunk) or bf16 (8 per chunk).
 static uint32_t f32_to_tf32_rna(float x) {
     uint32_t u; memcpy(&u, &x, 4);
@@ -338,50 +331,14 @@ static uint16_t f32_to_bf16_rn(float x) {
 static int pack_tc_host(sbk_handle* h, const std::vector<float>& hs, const std::string& key, int cout, int cin, int geom, bool bf16, int nt_override = 0);
 // fp32x3 handles (and the CUDA-core fp32 handles' RefBlock branch) pack every tensor-core weight as (hi, lo) stage pairs
 static bool packs_x3(const sbk_handle* h) { return h->cfg.precision == SBK_PREC_FP32X3 || h->cfg.precision == SBK_PREC_FP32; }
-// Row-shared image of a 3x3 conv with 64-wide N tiles (sbk_conv_tc.cu, RS): per K stage (and hi | correction in fp32x3)
-// [column tap sx][16-byte chunk][kernel row 2 | 1 | 0][co % 64][elements] - one N = 128 instruction then reads the two kernel
-// rows an input row feeds as adjacent weight rows.
-static int pack_tc_rs(sbk_handle* h, const std::vector<float>& hs, const std::string& key, int cout, int cin, bool bf16) {
-    const bool x3 = !bf16 && packs_x3(h);
-    const int NT = 64, CPS = conv_tc_stage_channels(G_C3, bf16 ? 1 : 0), EPC = bf16 ? 8 : 4, KCHK = CPS / EPC, ksteps = cin / CPS;
-    const size_t esz = bf16 ? 2 : 4, img = (size_t)3 * KCHK * 3 * NT * EPC;          // elements of one stage image
-    std::vector<uint8_t> hd((size_t)cout * cin * 9 * esz * (x3 ? 2 : 1));
-    for (int nt = 0; nt < cout / NT; ++nt) for (int ks = 0; ks < ksteps; ++ks) for (int sx = 0; sx < 3; ++sx)
-        for (int k = 0; k < KCHK; ++k) for (int kr = 0; kr < 3; ++kr) for (int col = 0; col < NT; ++col) for (int e = 0; e < EPC; ++e) {
-            const int co = nt * NT + col, ci = ks * CPS + k * EPC + e;
-            const float w = hs[((size_t)co * cin + ci) * 9 + kr * 3 + sx];
-            const size_t in_img = ((((size_t)sx * KCHK + k) * 3 + (2 - kr)) * NT + col) * EPC + e;
-            const size_t stage = ((size_t)nt * ksteps + ks) * (x3 ? 2 : 1);
-            if (x3) {
-                const uint32_t uh = f32_to_tf32_rna(w);
-                float fh; memcpy(&fh, &uh, 4);
-                reinterpret_cast<uint32_t*>(hd.data())[stage * img + in_img] = uh;
-                uint16_t* cc = reinterpret_cast<uint16_t*>(hd.data()) + 2 * ((stage + 1) * img + in_img - e);
-                cc[e] = f32_to_f16_rn(w);
-                cc[4 + e] = f32_to_f16_rn((w - fh) * 4096.f);
-            } else if (bf16) {
-                reinterpret_cast<uint16_t*>(hd.data())[stage * img + in_img] = f32_to_bf16_rn(w);
-            } else {
-                reinterpret_cast<uint32_t*>(hd.data())[stage * img + in_img] = f32_to_tf32_rna(w);
-            }
-        }
-    float*& d = h->packed[key];
-    if (!d) { CU(cudaMalloc(&d, hd.size())); h->owned.push_back(d); }
-    CU(cudaMemcpy(d, hd.data(), hd.size(), cudaMemcpyHostToDevice));
-    return SBK_OK;
-}
 static int pack_tc(sbk_handle* h, const std::string& src, const std::string& key, int cout, int cin, int geom, bool bf16) {
     const int taps = conv_tc_taps(geom);
     std::vector<float> hs((size_t)cout * cin * taps);
     CU(cudaMemcpy(hs.data(), h->raw[src], hs.size() * sizeof(float), cudaMemcpyDeviceToHost));
     TRY_RC(pack_tc_host(h, hs, key, cout, cin, geom, bf16));
     // 3x3 convs with >= 128 output channels also get a 64-wide N-tile image: small batches have too few 128-wide tiles to
-    // fill 148 SMs (B=1, level 2: 20 tiles), so the planner switches those launches to twice as many half-width tiles
-    // ... and that half-width image is also what a CTA pair stages: each CTA of a cta_group::2 pair holds half of the N tile
-    // (sbk_conv_tc.cu, PAIR).  64-channel convs (level 0) get a 32-wide image for the same purpose.
+    // fill the GPU's SMs, so the planner switches those launches to twice as many half-width tiles
     if (geom == G_C3 && conv_tc_ntile(geom, cout) == 128) TRY_RC(pack_tc_host(h, hs, key + "64", cout, cin, geom, bf16, 64));
-    if (geom == G_C3 && conv_tc_ntile(geom, cout) == 64) TRY_RC(pack_tc_host(h, hs, key + "32", cout, cin, geom, bf16, 32));
-    if (geom == G_C3 && conv_tc_ntile(geom, cout) == 64) TRY_RC(pack_tc_rs(h, hs, key + "rs", cout, cin, bf16));
     return SBK_OK;
 }
 // k and v rows of to_qkv ('(qkv heads c)': k = rows 128.., v = rows 256..) in k_attn_kv's per-stage shared-memory image
@@ -449,7 +406,7 @@ static int pack_tc_host(sbk_handle* h, const std::vector<float>& hs, const std::
             if (x3) {
                 // [ntile][kstage][hi|correction][tap][chunk][co % NT][16 B]: the main image holds w_hi = tf32(w) (RNA), the
                 // correction image the fp16 chunk {w[c0..c3], (w - w_hi)[c0..c3] * 2^12} that pairs with the activations'
-                // {x_lo, x * 2^-12} chunk in one kind::f16 MMA (sbk_internal.h: corr_chunk)
+                // {x_lo, x * 2^-12} chunk in one f16 MMA (sbk_internal.h: corr_chunk)
                 const size_t ih = ((((((size_t)nt * ksteps + ks) * 2) * taps + tap) * KCHK + k) * NT + col) * EPC + e;
                 const uint32_t uh = f32_to_tf32_rna(w);
                 float fh; memcpy(&fh, &uh, 4);
@@ -610,15 +567,7 @@ static size_t layout(const sbk_handle* h, int B, int T, int tb_rows, Arena& ar, 
         b.D[l] = l > 0 ? fo((size_t)B * P[l] * C[l - 1]) : nullptr;
     }
     b.U1 = fo((size_t)B * P[1] * C[1]);
-    size_t mt0 = (P[0] + 127) / 128;
-    if (x3) {
-        mt0 = 0;                                    // the chunk length depends on the level's item count: take the largest chunk count
-        for (int l = 0; l < 3; ++l) {
-            const int items = (int)((P[l] + attn_kv_x3_item_pixels() - 1) / attn_kv_x3_item_pixels());
-            const int ci = attn_x3_chunk_items(items, B);
-            mt0 = std::max(mt0, (size_t)((items + ci - 1) / ci));
-        }
-    }
+    const size_t mt0 = (P[0] + attn_kv_tile_pixels() - 1) / attn_kv_tile_pixels();     // attention partials: level 0 has the most items
     b.kv_part = f((size_t)B * mt0 * kHeads * kKvPartFloats);
     b.ctx = f((size_t)B * kHeads * 1024);
     b.w_eff = f((size_t)B * C[2] * C[2] * (x3 ? 2 : 1));
@@ -707,7 +656,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
     const bool use_tc = c.precision != SBK_PREC_FP32;
     const bool x3 = c.precision == SBK_PREC_FP32X3;
     auto LO = [&](const void* q) -> float* { auto it = bf.lo.find(q); return it == bf.lo.end() ? nullptr : it->second; };
-    int num_sms = 148;
+    int num_sms = 132;
     cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, c.device);
     const bool b16 = c.precision == SBK_PREC_BF16;          // operand tensors in bf16 [B][H][C/8][W][8]
     const double osz = b16 ? 2.0 : 4.0;                     // bytes per operand-tensor element
@@ -753,32 +702,12 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         p.bf16 = b16 ? 1 : 0;
         if (x3) {
             p.x3 = 1; p.in0_lo = LO(in0); p.in1_lo = LO(in1); p.out_lo = geom != G_C3 ? LO(out) : nullptr;
-            static const int flush_env = getenv("SBK_X3_FLUSH") ? atoi(getenv("SBK_X3_FLUSH")) : 0;     // measurement knob
-            p.flush = flush_env;
         }
-        if (geom == G_C3 && conv_tc_ntile(geom, cout) == 128 && getenv("SBK_FORCE_PAIR") == nullptr) {
-            // tiles of 2 rows x 128 pixels x 128 channels; when they cannot fill half the SMs, use 64-wide N tiles instead
-            const long long tiles = (long long)B * ((Ws[lvl] + 127) / 128) * ((Hs[lvl] + 1) / 2) * (cout / 128);
+        if (geom == G_C3 && conv_tc_ntile(geom, cout) == 128) {
+            // tiles of one row x 128 pixels x 128 channels; when they cannot fill half the SMs, use 64-wide N tiles instead
+            const int rows = conv_tc_tile_rows();
+            const long long tiles = (long long)B * ((Ws[lvl] + 127) / 128) * ((Hs[lvl] + rows - 1) / rows) * (cout / 128);
             if (tiles * 2 <= num_sms && h->packed.count(wkey + "64")) { p.nt = 64; p.wpk = W(wkey + "64"); }
-        }
-        if (geom == G_C3 && conv_tc_ntile(geom, cout) == 64 && h->packed.count(wkey + "rs") && getenv("SBK_FORCE_PAIR") == nullptr &&
-            ((!x3 && getenv("SBK_NO_RS") == nullptr) || getenv("SBK_FORCE_RS") != nullptr)) {
-            // 64-channel convs (level 0), tf32 / bf16: row-shared issue order on single CTAs (measured 5 % / 3 % faster than the
-            // tap-by-tap kernels; in fp32x3 the CTA pairs are 3 % faster than this order and stay).  SBK_NO_RS=1 / SBK_FORCE_RS=1:
-            // measurement and test knobs, read when a plan is built.
-            p.rs = 1; p.wpk = W(wkey + "rs");
-        }
-        if (geom == G_C3 && !p.nt && !p.rs) {
-            // CTA pairs (cta_group::2) when there are enough 4-row pair tiles to fill every SM pair; the pair kernel reads the
-            // weight image packed for half-width N tiles.  SBK_NO_PAIR=1 keeps the single-CTA kernels (measurement knob).
-            // SBK_FORCE_PAIR=1 uses them for every shape (the parity tests run the small ragged goldens through the pair kernels).
-            // Both are read when a plan is built, so a test can switch them between engines.
-            const bool no_pair = getenv("SBK_NO_PAIR") != nullptr, force_pair = getenv("SBK_FORCE_PAIR") != nullptr;
-            const int ntile = conv_tc_ntile(geom, cout);
-            const std::string half = wkey + (ntile == 128 ? "64" : "32");
-            const long long ptiles = (long long)B * conv_tc_pair_tiles(Hs[lvl], Ws[lvl]) * (cout / ntile);
-            // (bf16 mode: measured 2 % slower on pairs - its MMAs are half as long, the pair's cross-CTA handshakes are not)
-            if (!no_pair && h->packed.count(half) && (force_pair || (!b16 && ptiles >= num_sms / 2))) { p.pair = 1; p.wpk = W(half); }
         }
         const double taps = geom == G_PW ? 1.0 : (geom == G_UP ? 4.0 : 9.0);
         op.flops = 2.0 * B * Hs[lvl] * Ws[lvl] * cout * (c0 + c1) * taps;
@@ -883,19 +812,17 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         int mt = igemm_mtiles(G_PW, Hs[lvl], Ws[lvl], Hs[lvl], Ws[lvl]);
         const bool tc_apply = use_tc && a.c % tc_cps1 == 0;
         if (tc_apply && x3) {
-            // fp32-class attention, fused (k_attn_kv_x3): k|v projection (tf32 + fp16 correction), online softmax over the
-            // items of a chunk, context partials - k and v never reach HBM.  One partial per chunk of `chunk_items` 64-pixel
-            // items; the chunk length keeps >= ~2 chunks per SM in flight for small batches.
+            // fp32-class attention, fused (k_attn_kv_x3): k|v projection (tf32 + fp16 correction), softmax, context
+            // partials - k and v never reach HBM.  One partial per item of attn_kv_tile_pixels() pixels: an utterance is cut
+            // at the same pixels whatever batch it sits in.
             Op op = tc_conv(a.prefix + ".kvpart", G_PW, a.prefix + ".kvx.wtc", "", lvl, x, a.c, nullptr, 0, 256, nullptr, nullptr);
-            const int items = (Hs[lvl] * Ws[lvl] + attn_kv_x3_item_pixels() - 1) / attn_kv_x3_item_pixels();
-            const int chunk_items = attn_x3_chunk_items(items, B);
-            mt = (items + chunk_items - 1) / chunk_items;
-            op.tc.epi = EPI_KV; op.tc.kv_part = bf.kv_part; op.tc.Ho = chunk_items; op.tc.Wo = mt;
+            mt = (Hs[lvl] * Ws[lvl] + attn_kv_tile_pixels() - 1) / attn_kv_tile_pixels();
+            op.tc.epi = EPI_KV; op.tc.kv_part = bf.kv_part;
             op.bytes = 8.0 * npix(lvl) * a.c;
             op.flops += 2.0 * npix(lvl) * 4096.0;
             push(op, nullptr, 0);
         } else if (tc_apply) {
-            // k/v projection + softmax partials on tensor cores (k_attn_kv): items of 128 pixels x 4 heads
+            // k/v projection + softmax partials on tensor cores (k_attn_kv): items of attn_kv_tile_pixels() pixels x 4 heads
             Op op = tc_conv(a.prefix + ".kvpart", G_PW, a.prefix + ".kv.wtc", "", lvl, x, a.c, nullptr, 0, 256, nullptr, nullptr);
             op.tc.epi = EPI_KV; op.tc.kv_part = bf.kv_part;
             op.bytes = osz * npix(lvl) * a.c;
@@ -925,7 +852,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             push(op, nullptr, 0);
         }
         if (tc_apply) {
-            // the per-sample (I + g P_b) matrix is written by k_attn_mix directly in the tcgen05 weight-stage layout
+            // the per-sample (I + g P_b) matrix is written by k_attn_mix directly in the tensor-core weight-stage layout
             Op op = tc_conv(a.prefix + ".out", G_PW, "", "", lvl, x, a.c, nullptr, 0, a.c, out, nullptr);
             op.tc.wpk = bf.w_eff; op.tc.w_bstride_bytes = (long long)a.c * a.c * (b16 ? 2 : (x3 ? 8 : 4)); op.tc.bias = bf.b_eff;
             op.tc.out_mask = 1; op.tc.addin = x;

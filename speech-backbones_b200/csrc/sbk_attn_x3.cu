@@ -1,31 +1,23 @@
-// fp32x3 mode, LinearAttention pass 1 fused (Grad-TTS/model/diffusion.py:93-96): k|v projection, softmax-over-pixels
-// statistics and the context partials S[d][e] = sum_px P[d,px] V[e,px] in ONE persistent tcgen05 kernel - k and v never
-// reach HBM.  (The first fp32-class version wrote the projection to HBM as a 256-channel fp32 tensor, 1.3 GB per call at
-// B=32 x T=512, and re-read it in a second kernel: 0.44 + 0.62 ms at level 0 for 0.2 ms of algorithmic work.)
+// LinearAttention pass 1 fused (Grad-TTS/model/diffusion.py:93-96): k|v projection, softmax-over-pixels statistics and
+// the context partials S[d][e] = sum_px P[d,px] V[e,px] in ONE persistent wgmma kernel - k and v never reach HBM.
 //
-// Roles are swapped relative to the convs, as in the tf32 kernel k_attn_kv (sbk_conv_tc.cu): the weights are the M operand,
-// so a TMEM lane is a k (or v) channel and a column is a pixel of the current 64-pixel ITEM:
-//     D1K[k row 32*head+d][px] = Wk X^T,   D1V[v row 32*head+e][px] = Wv X^T
-// Every product is fp32-class: each 32-channel K stage runs as a kind::f16 correction sub-stage on the packed fp16 chunks
-// ({x_lo, x*2^-12} x {w, w_lo*2^12}, sbk_internal.h: corr_chunk) followed by the kind::tf32 main sub-stage (x_hi * w_hi).
-// One softmax thread owns a k row and a v row over 16 pixels: running max m (online softmax across the items of a chunk),
-// P = exp(k - m) written back to TMEM in place (the A operand of the main context MMA; the tensor core reads P_hi), and the
-// three remaining operands to shared memory as K-major images [4-pixel chunk][row][16 B]:
-//     V^T (fp32; read as V_hi),   Pc = {P_lo*2^8, P*2^-4} and Vc = {V*2^-8, V_lo*2^4} (fp16).
-// The powers of two are exact and chosen so that neither the tiny softmax numerators nor V_lo fall into fp16's subnormals:
-//     S_item = P_hi V_hi^T  +  [ P_lo V^T + P V_lo^T ]   = 8 TS-form tf32 MMAs + 8 fp16 MMAs into a FRESH accumulator
-// (16 MMAs per run: the tensor core's truncating fp32 accumulate costs < 5e-7 here), and the head's 32x32 block is then
-// added into fp32 registers with the online-softmax rescale: acc = acc * e^(m_old - m_new) + S_item.  A CHUNK (up to
-// `chunk_items` consecutive items of one sample) produces one partial {max[32], sum[32], S[32][32]} per head in the
-// k_attn_kv format, merged by k_attn_ctx.
+// One ITEM = 64 consecutive pixels of one sample, all four heads.  The pixels are the M operand of the projection:
+//     warpgroup 0:  K^T[px][k row 32*head+d] = X Wk^T,     warpgroup 1:  V^T[px][v row 32*head+e] = X Wv^T
+// (one m64n128 wgmma per K step each, the same activation tile for both).  The two results go to shared memory as K-major
+// images [4-pixel chunk][row][16 B] - the operand layout of the context MMAs - and the softmax runs over those images,
+// one thread per (row, half of the item's pixels): P = exp(k - max) replaces K in place.  The context S = P V^T is a
+// second pair of wgmmas (warpgroup c: rows / columns 64c..64c+63, i.e. heads 2c and 2c+1; only the two diagonal 32 x 32
+// blocks are kept).  Per item and head one partial {max[32], sum[32], S[32][32]} is written, merged by k_attn_ctx.
 //
-// Pipeline (one CTA per SM, persistent over chunks): loader warp (cp.async.bulk, 3-stage ring of 40 KB sub-stages),
-// projection-MMA warp, context-MMA warp, 16 softmax warps.  Two TMEM slots of 256 columns (K then P 64 | V 64 | S 128):
-// S has its own columns, so a slot's K/V part is free again as soon as its context MMAs have completed - the projection
-// of item i+2 is gated on kvdone(i) alone and runs under the softmax of item i+1; the context MMAs of item i run under the
-// max/exp pass of item i+1, and their S block is read out just before the operand images are rewritten.  (With S stored
-// over V the slot was held until that read-out, which serialised projection and softmax: 7.7 k clocks per item against
-// 2.6 k of MMA work, profiles/r2_ncu_attn_x3.md.)
+// Precision modes.  tf32: tf32 projection, fp32 softmax, tf32 context (P and V fp32 in shared memory, read as tf32).
+// bf16: the activations and weights are bf16 (a stage carries 64 channels), the rest as tf32.  fp32x3: every product is
+// fp32-class: each 32-channel K stage runs as an f16 correction sub-stage on the packed fp16 chunks ({x_lo, x*2^-12} x
+// {w, w_lo*2^12}, sbk_internal.h: corr_chunk) followed by the tf32 main sub-stage (x_hi * w_hi), and the context adds
+//     [ P_lo V^T + P V_lo^T ]  from  Pc = {P_lo*2^8, P*2^-4},  Vc = {V*2^-8, V_lo*2^4}  (fp16 images)
+// to P_hi V_hi^T.  The powers of two are exact and keep neither the tiny softmax numerators nor V_lo in fp16's subnormals.
+//
+// Pipeline (one CTA per SM, persistent over items): loader warp (cp.async.bulk, STAGES-deep ring of 40 KB stages) and two
+// consumer warpgroups; the projection of item i+1 streams in while the softmax / context of item i run.
 #include "sbk_tc.cuh"
 
 #include <type_traits>
@@ -35,321 +27,223 @@ namespace sbk {
 using namespace tc;
 
 namespace kx3 {
-constexpr int PX = 64;                         // pixels per item: N of the projection, K extent of the context MMAs
-constexpr int KCH = 8;                         // 16-byte channel chunks per sub-stage (32 channels)
-constexpr int XS = KCH * PX * 16;              // activation sub-stage [chunk][pixel][16 B]
-constexpr int WS = 2 * KCH * 128 * 16;         // weight sub-stage     [k|v][chunk][row][16 B]
+constexpr int PX = 64;                         // pixels per item: M of the projection, K extent of the context MMAs
+constexpr int KCH = 8;                         // 16-byte channel chunks per stage
+constexpr int XS = KCH * PX * 16;              // activation stage [chunk][pixel][16 B]
+constexpr int WS = 2 * KCH * 128 * 16;         // weight stage     [k|v][chunk][row][16 B]
 constexpr int STAGE = XS + WS;
-constexpr int STAGES = 3;
+constexpr int STAGES = 2;
 constexpr int OPI = (PX / 4) * 128 * 16;       // one context operand image [pixel chunk][row][16 B]
-constexpr int NPART = 4;                       // pixel parts per item: 4 lane quarters x NPART = softmax warps
-constexpr int PCOLS = PX / NPART;              // columns (pixels) per softmax thread
-constexpr int EPW = 4 * NPART;                 // softmax warps
-constexpr int THREADS = (EPW + 3) * 32;        // + projection-MMA warp, loader warp, context-MMA warp
-constexpr int RED = 2 * 2 * NPART * 128 * 4;   // max | sum exchange between the pixel parts, double-buffered by slot
-constexpr int NSLOT = 2, SLOT_COLS = 256;      // K then P [0,64) | V [64,128) | S [128,256)
-constexpr int SCOL = 128;                      // first S column of a slot
-constexpr int NBARS = 2 * STAGES + 3 * NSLOT;
-constexpr size_t SMEM = (size_t)STAGES * STAGE + 3 * OPI + RED + NBARS * 8 + 16;
-static_assert(PCOLS == 16, "one 16-column TMEM load per operand and thread");
+constexpr int THREADS = 256 + 32;              // 2 consumer warpgroups + loader warp
+constexpr int NBARS = 2 * STAGES;
+constexpr size_t SMEM = (size_t)STAGES * STAGE + 4 * OPI + 4 * 128 * 4 + NBARS * 8 + 16;
 static_assert(SMEM <= 227 * 1024, "shared memory budget");
 }
 
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        :: "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-           "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-
-// p.in0 / p.in0_lo: x and its correction chunks ([B][H][C/4][W][4] / 16-byte chunks); p.c0 = C; p.wpk: the k|v rows of to_qkv
-// as [32-channel stage][hi | correction][k|v][chunk][row][16 B]; p.kv_part: [B][nchunks][4][kKvPartFloats];
-// p.Ho = chunk_items, p.Wo = chunks per sample (free fields of ConvTcParams for this launch)
-__global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_x3(const ConvTcParams p) {
+// MODE: 0 = tf32, 1 = bf16, 2 = fp32x3.  p.in0 (/ p.in0_lo): x (and its correction chunks); p.c0 = C; p.wpk: the k|v rows
+// of to_qkv as per-stage images [k|v][chunk][row][16 B] (fp32x3: [32-channel stage][hi | correction][k|v]...);
+// p.kv_part: [B][items per sample][4][kKvPartFloats]
+template <int MODE>
+__global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcParams p) {
     using namespace kx3;
+    constexpr bool X3 = MODE == 2;
+    constexpr int EPC = MODE == 1 ? 8 : 4;                         // channels per 16-byte chunk
+    constexpr int KMAIN = MODE == 1 ? K_BF16 : K_TF32;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* sS = smem;                                            // [STAGES][X | Wk | Wv]
-    uint8_t* vt = sS + STAGES * STAGE;                             // V^T fp32
-    uint8_t* vc = vt + OPI;                                        // Vc fp16 pairs
-    uint8_t* pc = vc + OPI;                                        // Pc fp16 pairs
-    float* s_mx = reinterpret_cast<float*>(pc + OPI);              // [2 slot][NPART][128]
-    float* s_z = s_mx + 2 * NPART * 128;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(s_z + 2 * NPART * 128);
-    uint32_t* s_tmem = reinterpret_cast<uint32_t*>(bars + NBARS);
+    uint8_t* kp = sS + STAGES * STAGE;                             // K, then P (fp32)
+    uint8_t* vt = kp + OPI;                                        // V (fp32)
+    uint8_t* pc = vt + OPI;                                        // Pc fp16 pairs (fp32x3)
+    uint8_t* vc = pc + OPI;                                        // Vc fp16 pairs (fp32x3)
+    float* s_mx = reinterpret_cast<float*>(vc + OPI);              // [2 halves][128 rows]
+    float* s_z = s_mx + 2 * 128;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(s_z + 2 * 128);
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;   // (warp-uniform, see sbk_conv_tc.cu)
     const int HW = p.H * p.W;
-    const int ksteps = p.c0 / (KCH * 4);
-    const int ksteps_t = 2 * ksteps;                               // correction + main sub-stage per 32 channels
+    const int ksteps = p.c0 / (KCH * EPC);
+    const int ksteps_t = X3 ? 2 * ksteps : ksteps;                 // fp32x3: correction + main sub-stage per 32 channels
     const int items = (HW + PX - 1) / PX;                          // items per sample
-    const int chunk_items = p.Ho, cps = p.Wo;                      // items per chunk, chunks per sample
-    const int total_chunks = p.B * cps;
+    const int total = p.B * items;
     const uint32_t bar0 = smem_u32(bars);
     auto full = [&](int s) { return bar0 + 8u * s; };
     auto empty = [&](int s) { return bar0 + 8u * (STAGES + s); };
-    auto tfull = [&](int a) { return bar0 + 8u * (2 * STAGES + a); };              // projection of the slot complete
-    auto pready = [&](int a) { return bar0 + 8u * (2 * STAGES + NSLOT + a); };     // P in TMEM + Pc, V^T, Vc in smem written
-    auto kvdone = [&](int a) { return bar0 + 8u * (2 * STAGES + 2 * NSLOT + a); }; // context MMAs complete: K/P and V columns free
 
     if (tid == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 1); }
-        for (int a = 0; a < NSLOT; ++a) {
-            mbar_init(tfull(a), 1); mbar_init(pready(a), EPW); mbar_init(kvdone(a), 1);
-        }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 8); }
         fence_barrier_init();
     }
-    if (warp == EPW) tmem_alloc(smem_u32(s_tmem), 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *s_tmem;
 
-    if (warp < EPW) {
-        // ---------------------------------------------------------------- softmax warps
-        const int q = warp & 3, part = warp >> 2;                  // TMEM lane quarter = head, pixel part
-        const int row = q * 32 + lane;
-        const int col0 = part * PCOLS;
-        const uint32_t lane_sel = (uint32_t)(q * 32) << 16;
-        float m_run = -INFINITY, z_run = 0.f;                      // online softmax state of the current chunk
-        float acc[32];                                             // part 0: S[d = lane][e] of head q, running
+    if (warp < 8) {
+        const int wg = warp >> 2, wt = tid & 127;
+        const int row = tid & 127, half = tid >> 7;                // softmax: one row, half of the item's pixels
+        constexpr uint32_t D_HI = desc_hi(128);
+        const uint32_t s0 = smem_u32(sS);
+        uint32_t it = 0;
+        for (int t = blockIdx.x; t < total; t += gridDim.x) {
+            const int b = t / items, mt = t - b * items;
+            // ---- projection: warpgroup 0 -> K^T, warpgroup 1 -> V^T  (64 pixels x 128 rows)
+            float acc[64];
+            for (int ks = 0; ks < ksteps_t; ++ks, ++it) {
+                const int s = it % STAGES;
+                mbar_wait(full(s), (it / STAGES) & 1);
+                const uint32_t xs = s0 + s * STAGE;
+                const uint32_t x_lo = desc_lo(xs, PX * 16), w_lo = desc_lo(xs + XS + wg * (KCH * 128 * 16), 128 * 16);
+                auto issue = [&](auto kind) {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) acc[i] = 0.f;
-        int tl = 0;                                                // item counter of this CTA (slot / phase)
-        bool pend = false, pend_last = false;                      // a finished-but-not-read-out item, and whether it closes a chunk
-        int pend_b = 0, pend_ci = 0; float pend_f = 0.f, pend_m = 0.f;
-        auto finish = [&](int ptl) {
-            const int pslot = ptl & 1;
-            mbar_wait(kvdone(pslot), (ptl >> 1) & 1);
-            tc_fence_after();
-            if (part == 0) {
-                float z = 0.f;
+                    for (int kk = 0; kk < KCH / 2; ++kk)
+                        wgmma<128, decltype(kind)::value>(acc, desc_pack(x_lo + (uint32_t)(kk * 2 * PX), D_HI),
+                                                          desc_pack(w_lo + (uint32_t)(kk * 2 * 128), D_HI), (ks | kk) != 0 ? 1u : 0u);
+                };
+                wg_fence();
+                if (X3 && (ks & 1) == 0) issue(std::integral_constant<int, K_F16>{});   // correction sub-stage (fp16 chunks)
+                else issue(std::integral_constant<int, KMAIN>{});
+                wg_commit();
+                wg_wait<0>();
+                wg_fence_regs(acc);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty(s));
+            }
+            // ---- K^T / V^T fragments -> [pixel chunk][row][16 B] images
+            {
+                uint8_t* img = wg == 0 ? kp : vt;
 #pragma unroll
-                for (int j = 0; j < NPART; ++j) z += s_z[(pslot * NPART + j) * 128 + row];
-                z_run = fmaf(z_run, pend_f, z);
-#pragma unroll
-                for (int hb = 0; hb < 32; hb += 16) {
-                    uint32_t r[16];
-                    tmem_ld16(tmem_base + pslot * SLOT_COLS + lane_sel + SCOL + q * 32 + hb, r);  // S[d = lane][e] of head q
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) acc[hb + i] = fmaf(acc[hb + i], pend_f, __uint_as_float(r[i]));
-                }
-                if (pend_last) {
-                    float* pt = p.kv_part + (((long long)pend_b * cps + pend_ci) * kHeads + q) * kKvPartFloats;
-                    pt[lane] = pend_m;
-                    pt[32 + lane] = z_run;
-#pragma unroll
-                    for (int i = 0; i < 32; i += 4)
-                        *reinterpret_cast<float4*>(&pt[64 + lane * 32 + i]) = make_float4(acc[i], acc[i + 1], acc[i + 2], acc[i + 3]);
+                for (int i = 0; i < 64; ++i) {
+                    const int px = frag_row(wt, i), r = frag_col(wt, i);
+                    *reinterpret_cast<float*>(img + ((size_t)(px / 4) * 128 + r) * 16 + (px % 4) * 4) = acc[i];
                 }
             }
-            tc_fence_before();
-        };
-        for (int c = blockIdx.x; c < total_chunks; c += gridDim.x) {
-            const int b = c / cps, ci = c - b * cps;
-            const int it_lo = ci * chunk_items, it_hi = min(items, it_lo + chunk_items);
-            m_run = -INFINITY;                                     // (acc / z_run restart through the rescale factor 0 of the first item)
-            for (int mt = it_lo; mt < it_hi; ++mt, ++tl) {
-                const int slot = tl & 1;
-                const uint32_t tq = tmem_base + slot * SLOT_COLS + lane_sel;
-                const int nvalid = min(PX, HW - mt * PX) - col0;   // valid columns of this thread's part (may be <= 0)
-                mbar_wait(tfull(slot), (tl >> 1) & 1);
-                tc_fence_after();
-                uint32_t kr[PCOLS];
-                tmem_ld16(tq + col0, kr);
-                float mx = -INFINITY;
-                const bool whole = nvalid >= PCOLS;               // (all but a ragged last item: no per-column predicates)
-                if (whole) {
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            // ---- softmax over the item's pixels: max, P = exp(k - max) in place, row sums
+            const int nvalid = min(PX, HW - mt * PX) - half * (PX / 2);   // valid pixels of this thread's half (may be <= 0)
+            float kr[PX / 2];
 #pragma unroll
-                    for (int i = 0; i < PCOLS; ++i) mx = fmaxf(mx, __uint_as_float(kr[i]));
-                } else {
+            for (int c = 0; c < PX / 8; ++c) {
+                const float4 q = *reinterpret_cast<const float4*>(kp + ((size_t)(half * (PX / 8) + c) * 128 + row) * 16);
+                kr[4 * c] = q.x; kr[4 * c + 1] = q.y; kr[4 * c + 2] = q.z; kr[4 * c + 3] = q.w;
+            }
+            float mx = -INFINITY;
 #pragma unroll
-                    for (int i = 0; i < PCOLS; ++i) mx = fmaxf(mx, i < nvalid ? __uint_as_float(kr[i]) : -INFINITY);
-                }
-                s_mx[(slot * NPART + part) * 128 + row] = mx;
-                asm volatile("bar.sync 1, %0;" ::"n"(EPW * 32) : "memory");
-                float md = s_mx[(slot * NPART) * 128 + row];
+            for (int i = 0; i < PX / 2; ++i) mx = fmaxf(mx, i < nvalid ? kr[i] : -INFINITY);
+            s_mx[half * 128 + row] = mx;
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            const float md = fmaxf(s_mx[row], s_mx[128 + row]);
+            float z0 = 0.f, z1 = 0.f;
 #pragma unroll
-                for (int j = 1; j < NPART; ++j) md = fmaxf(md, s_mx[(slot * NPART + j) * 128 + row]);
-                const float mn = fmaxf(m_run, md);
-                const float f = m_run == -INFINITY ? 0.f : expf(m_run - mn);
-                m_run = mn;
-                float z0 = 0.f, z1 = 0.f;
+            for (int i = 0; i < PX / 2; i += 2) {                  // (pixels past the image hold k = 0: finite, then selected away)
+                const float e0 = i < nvalid ? (X3 ? expf(kr[i] - md) : __expf(kr[i] - md)) : 0.f;
+                const float e1 = i + 1 < nvalid ? (X3 ? expf(kr[i + 1] - md) : __expf(kr[i + 1] - md)) : 0.f;
+                z0 += e0; z1 += e1;
+                kr[i] = e0; kr[i + 1] = e1;
+            }
+            s_z[half * 128 + row] = z0 + z1;
 #pragma unroll
-                for (int i = 0; i < PCOLS; i += 2) {              // (columns past the image hold k = 0: finite, then selected away)
-                    float e0 = expf(__uint_as_float(kr[i]) - mn), e1 = expf(__uint_as_float(kr[i + 1]) - mn);
-                    if (!whole) { e0 = i < nvalid ? e0 : 0.f; e1 = i + 1 < nvalid ? e1 : 0.f; }
-                    z0 += e0; z1 += e1;
-                    kr[i] = __float_as_uint(e0); kr[i + 1] = __float_as_uint(e1);
-                }
-                tmem_st16(tq + col0, kr);                          // P (fp32) in place: the A operand of the main context MMAs
-                s_z[(slot * NPART + part) * 128 + row] = z0 + z1;
-                // The context MMAs of the previous item have had the whole max/exp pass to finish; they must be complete
-                // before the operand images are overwritten.  Its S block is read out (and its slot released) here.
-                if (pend) finish(tl - 1);
-                // Pc = {P_lo * 2^8, P * 2^-4}: one 16-byte chunk per 4 pixels
-#pragma unroll
-                for (int i = 0; i < PCOLS; i += 4) {
-                    const float e0 = __uint_as_float(kr[i]), e1 = __uint_as_float(kr[i + 1]), e2 = __uint_as_float(kr[i + 2]), e3 = __uint_as_float(kr[i + 3]);
-                    *reinterpret_cast<uint4*>(pc + ((size_t)((col0 + i) / 4) * 128 + row) * 16) =
+            for (int c = 0; c < PX / 8; ++c) {
+                const size_t o = ((size_t)(half * (PX / 8) + c) * 128 + row) * 16;
+                const float e0 = kr[4 * c], e1 = kr[4 * c + 1], e2 = kr[4 * c + 2], e3 = kr[4 * c + 3];
+                *reinterpret_cast<float4*>(kp + o) = make_float4(e0, e1, e2, e3);
+                if constexpr (X3) {
+                    // Pc = {P_lo * 2^8, P * 2^-4},  Vc = {V * 2^-8, V_lo * 2^4}: one 16-byte chunk per 4 pixels
+                    *reinterpret_cast<uint4*>(pc + o) =
                         make_uint4(f16x2_sat(tf32_lo(e0) * 256.f, tf32_lo(e1) * 256.f), f16x2_sat(tf32_lo(e2) * 256.f, tf32_lo(e3) * 256.f),
                                    f16x2_sat(e0 * 0.0625f, e1 * 0.0625f), f16x2_sat(e2 * 0.0625f, e3 * 0.0625f));
-                }
-                // V: fp32 image (read as V_hi) and Vc = {V * 2^-8, V_lo * 2^4}
-                {
-                    uint32_t vr[PCOLS];
-                    tmem_ld16(tq + 64 + col0, vr);
-#pragma unroll
-                    for (int i = 0; i < PCOLS; i += 4) {
-                        const float v0 = __uint_as_float(vr[i]), v1 = __uint_as_float(vr[i + 1]), v2 = __uint_as_float(vr[i + 2]), v3 = __uint_as_float(vr[i + 3]);
-                        const size_t o = ((size_t)((col0 + i) / 4) * 128 + row) * 16;
-                        *reinterpret_cast<uint4*>(vt + o) = make_uint4(vr[i], vr[i + 1], vr[i + 2], vr[i + 3]);
-                        *reinterpret_cast<uint4*>(vc + o) =
-                            make_uint4(f16x2_sat(v0 * 0.00390625f, v1 * 0.00390625f), f16x2_sat(v2 * 0.00390625f, v3 * 0.00390625f),
-                                       f16x2_sat(tf32_lo(v0) * 16.f, tf32_lo(v1) * 16.f), f16x2_sat(tf32_lo(v2) * 16.f, tf32_lo(v3) * 16.f));
-                    }
-                }
-                tmem_wait_st();
-                fence_proxy_async();                               // operand images in smem -> visible to the tensor core
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(pready(slot));
-                pend = true; pend_last = mt == it_hi - 1; pend_b = b; pend_ci = ci; pend_f = f; pend_m = mn;
-            }
-        }
-        if (pend) finish(tl - 1);
-    } else if (warp == EPW) {
-        // ---------------------------------------------------------------- projection MMA issuer (whole warp + elect_one)
-        const uint32_t idesc_m = make_idesc_fmt(2u, 128, PX), idesc_c = make_idesc_fmt(0u, 128, PX);
-        const uint32_t s0 = smem_u32(sS);
-        constexpr uint32_t D_HI = desc_hi(128);
-        uint32_t it = 0;
-        int tl = 0;
-        for (int c = blockIdx.x; c < total_chunks; c += gridDim.x) {
-            const int ci = c % cps;
-            const int it_lo = ci * chunk_items, it_hi = min(items, it_lo + chunk_items);
-            for (int mt = it_lo; mt < it_hi; ++mt, ++tl) {
-                const int slot = tl & 1;
-                const uint32_t tslot = tmem_base + slot * SLOT_COLS;
-                if (tl >= 2) mbar_wait(kvdone(slot), ((tl >> 1) & 1) ^ 1);   // the slot's previous item: its P (A operand) and V are done with
-                tc_fence_after();
-                for (int ks = 0; ks < ksteps_t; ++ks, ++it) {
-                    const int s = it % STAGES;
-                    mbar_wait(full(s), (it / STAGES) & 1);
-                    tc_fence_after();
-                    const uint32_t xs = s0 + s * STAGE;
-                    const uint32_t x_lo = desc_lo(xs, PX * 16), k_lo = desc_lo(xs + XS, 128 * 16), v_lo = desc_lo(xs + XS + KCH * 128 * 16, 128 * 16);
-                    if (elect_one()) {
-                        auto issue = [&](auto kind16, const uint32_t idk) {
-#pragma unroll
-                            for (int kk = 0; kk < KCH / 2; ++kk) {
-                                const uint64_t xd = desc_pack(x_lo + (uint32_t)(kk * 2 * PX), D_HI);
-                                umma<decltype(kind16)::value>(tslot, desc_pack(k_lo + (uint32_t)(kk * 2 * 128), D_HI), xd, idk, (ks | kk) != 0 ? 1u : 0u);
-                                umma<decltype(kind16)::value>(tslot + 64, desc_pack(v_lo + (uint32_t)(kk * 2 * 128), D_HI), xd, idk, (ks | kk) != 0 ? 1u : 0u);
-                            }
-                        };
-                        if ((ks & 1) == 0) issue(std::true_type{}, idesc_c);     // correction sub-stage (fp16 chunks)
-                        else issue(std::false_type{}, idesc_m);                  // main sub-stage (tf32)
-                        umma_commit(empty(s));
-                        if (ks == ksteps_t - 1) umma_commit(tfull(slot));
-                    }
-                    __syncwarp();
+                    const float4 v = *reinterpret_cast<const float4*>(vt + o);
+                    *reinterpret_cast<uint4*>(vc + o) =
+                        make_uint4(f16x2_sat(v.x * 0.00390625f, v.y * 0.00390625f), f16x2_sat(v.z * 0.00390625f, v.w * 0.00390625f),
+                                   f16x2_sat(tf32_lo(v.x) * 16.f, tf32_lo(v.y) * 16.f), f16x2_sat(tf32_lo(v.z) * 16.f, tf32_lo(v.w) * 16.f));
                 }
             }
-        }
-    } else if (warp == EPW + 2) {
-        // ---------------------------------------------------------------- context MMA issuer: S = P V^T (fresh accumulator per item)
-        const uint32_t idesc_m = make_idesc_fmt(2u, 128, 128), idesc_c = make_idesc_fmt(0u, 128, 128);
-        const uint32_t vt_lo = desc_lo(smem_u32(vt), 128 * 16), vc_lo = desc_lo(smem_u32(vc), 128 * 16), pc_lo = desc_lo(smem_u32(pc), 128 * 16);
-        constexpr uint32_t D_HI = desc_hi(128);
-        int tl = 0;
-        for (int c = blockIdx.x; c < total_chunks; c += gridDim.x) {
-            const int ci = c % cps;
-            const int it_lo = ci * chunk_items, it_hi = min(items, it_lo + chunk_items);
-            for (int mt = it_lo; mt < it_hi; ++mt, ++tl) {
-                const int slot = tl & 1;
-                const uint32_t tslot = tmem_base + slot * SLOT_COLS;
-                mbar_wait(pready(slot), (tl >> 1) & 1);
-                tc_fence_after();
-                if (elect_one()) {
+            fence_proxy_async();                                   // operand images in smem -> visible to the tensor core
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            // ---- context: warpgroup wg, rows and columns 64 wg .. 64 wg + 63 (heads 2 wg, 2 wg + 1)
+            float sacc[32];
+            {
+                const uint32_t p_lo = desc_lo(smem_u32(kp) + 64 * wg * 16, 128 * 16), v_lo = desc_lo(smem_u32(vt) + 64 * wg * 16, 128 * 16);
+                const uint32_t pc_lo = desc_lo(smem_u32(pc) + 64 * wg * 16, 128 * 16), vc_lo = desc_lo(smem_u32(vc) + 64 * wg * 16, 128 * 16);
+                wg_fence();
+                if constexpr (X3) {
 #pragma unroll
-                    for (int kk = 0; kk < PX / 8; ++kk)                // correction: K = 16 fp16 = 8 pixels x {P_lo V, P V_lo}
-                        umma<true>(tslot + SCOL, desc_pack(pc_lo + (uint32_t)(kk * 2 * 128), D_HI), desc_pack(vc_lo + (uint32_t)(kk * 2 * 128), D_HI),
-                                   idesc_c, kk != 0 ? 1u : 0u);
-#pragma unroll
-                    for (int kk = 0; kk < PX / 8; ++kk)                // main: K = 8 pixels, A = P read from TMEM (tf32 truncation = P_hi)
-                        umma_ts_tf32(tslot + SCOL, tslot + kk * 8, desc_pack(vt_lo + (uint32_t)(kk * 2 * 128), D_HI), idesc_m, 1u);
-                    umma_commit(kvdone(slot));
+                    for (int kk = 0; kk < PX / 8; ++kk)            // correction: K = 16 fp16 = 8 pixels x {P_lo V, P V_lo}
+                        wgmma<64, K_F16>(sacc, desc_pack(pc_lo + (uint32_t)(kk * 2 * 128), D_HI), desc_pack(vc_lo + (uint32_t)(kk * 2 * 128), D_HI),
+                                         kk != 0 ? 1u : 0u);
                 }
-                __syncwarp();
+#pragma unroll
+                for (int kk = 0; kk < PX / 8; ++kk)                // main: K = 8 pixels, P and V read as tf32 (P_hi V_hi)
+                    wgmma<64, K_TF32>(sacc, desc_pack(p_lo + (uint32_t)(kk * 2 * 128), D_HI), desc_pack(v_lo + (uint32_t)(kk * 2 * 128), D_HI),
+                                      (X3 || kk != 0) ? 1u : 0u);
+                wg_commit();
+                wg_wait<0>();
+                wg_fence_regs(sacc);
             }
+            // ---- partials of this item: max, sum (softmax threads of the first half), diagonal S blocks (fragments)
+            float* pt0 = p.kv_part + ((long long)b * items + mt) * kHeads * kKvPartFloats;
+            if (half == 0) {
+                float* pt = pt0 + (row / 32) * kKvPartFloats;
+                pt[row % 32] = md;
+                pt[32 + row % 32] = s_z[row] + s_z[128 + row];
+            }
+#pragma unroll
+            for (int i = 0; i < 32; ++i) {
+                const int dl = frag_row(wt, i), el = frag_col(wt, i);
+                if ((dl >> 5) == (el >> 5)) {
+                    float* pt = pt0 + (2 * wg + (dl >> 5)) * kKvPartFloats;
+                    pt[64 + (dl & 31) * 32 + (el & 31)] = sacc[i];
+                }
+            }
+            asm volatile("bar.sync 1, 256;" ::: "memory");        // the images are rewritten by the next item
         }
     } else {
         // ---------------------------------------------------------------- loader warp: weights + activation runs (cp.async.bulk)
         // lane 0 owns the ring protocol and the weight copy; lanes 0-7 each issue the activation runs of one channel chunk
         uint32_t it = 0;
-        const int chs = p.c0 / 4;
-        for (int c = blockIdx.x; c < total_chunks; c += gridDim.x) {
-            const int b = c / cps, ci = c - b * cps;
-            const int it_lo = ci * chunk_items, it_hi = min(items, it_lo + chunk_items);
-            for (int mt = it_lo; mt < it_hi; ++mt) {
-                const int m0 = mt * PX, m_hi = m0 + PX < HW ? m0 + PX : HW;
-                const int hh0 = m0 / p.W, ww0 = m0 - hh0 * p.W;
-                for (int ks = 0; ks < ksteps_t; ++ks, ++it) {
-                    const int s = it % STAGES;
-                    const int kb = ks >> 1;
-                    const bool corr = (ks & 1) == 0;
-                    const uint32_t xs = smem_u32(sS) + s * STAGE;
-                    if (lane == 0) {
-                        mbar_wait(empty(s), ((it / STAGES) & 1) ^ 1);
-                        mbar_arrive_expect_tx(full(s), STAGE);
-                        bulk_g2s(xs + XS, reinterpret_cast<const uint8_t*>(p.wpk) + (size_t)(2 * kb + (corr ? 1 : 0)) * WS, WS, full(s));
+        const int chs = p.c0 / EPC;
+        for (int t = blockIdx.x; t < total; t += gridDim.x) {
+            const int b = t / items, mt = t - b * items;
+            const int m0 = mt * PX, m_hi = m0 + PX < HW ? m0 + PX : HW;
+            const int hh0 = m0 / p.W, ww0 = m0 - hh0 * p.W;
+            for (int ks = 0; ks < ksteps_t; ++ks, ++it) {
+                const int s = it % STAGES;
+                const int kb = X3 ? ks >> 1 : ks;
+                const bool corr = X3 && (ks & 1) == 0;
+                const uint32_t xs = smem_u32(sS) + s * STAGE;
+                if (lane == 0) {
+                    mbar_wait(empty(s), ((it / STAGES) & 1) ^ 1);
+                    mbar_arrive_expect_tx(full(s), STAGE);
+                    bulk_g2s(xs + XS, reinterpret_cast<const uint8_t*>(p.wpk) + (size_t)(X3 ? 2 * kb + (corr ? 1 : 0) : ks) * WS, WS, full(s));
+                }
+                __syncwarp();
+                if (lane < KCH) {
+                    const uint8_t* src = reinterpret_cast<const uint8_t*>(corr ? p.in0_lo : p.in0);
+                    const int k = lane, cl = kb * KCH + k;
+                    int m = m0, hh = hh0, ww = ww0, qx = 0;
+                    while (m < m_hi) {                             // split the flattened run at image-row boundaries
+                        const int n = (p.W - ww) < (m_hi - m) ? (p.W - ww) : (m_hi - m);
+                        bulk_g2s(xs + (k * PX + qx) * 16, src + (((long long)(b * p.H + hh) * chs + cl) * p.W + ww) * 16,
+                                 (uint32_t)n * 16u, full(s));
+                        m += n; qx += n; ++hh; ww = 0;
                     }
-                    __syncwarp();
-                    if (lane < KCH) {
-                        const uint8_t* src = reinterpret_cast<const uint8_t*>(corr ? p.in0_lo : p.in0);
-                        const int k = lane, cl = kb * KCH + k;
-                        int m = m0, hh = hh0, ww = ww0, qx = 0;
-                        while (m < m_hi) {                             // split the flattened run at image-row boundaries
-                            const int n = (p.W - ww) < (m_hi - m) ? (p.W - ww) : (m_hi - m);
-                            bulk_g2s(xs + (k * PX + qx) * 16, src + (((long long)(b * p.H + hh) * chs + cl) * p.W + ww) * 16,
-                                     (uint32_t)n * 16u, full(s));
-                            m += n; qx += n; ++hh; ww = 0;
-                        }
-                        if (qx < PX) bulk_g2s(xs + (k * PX + qx) * 16, p.zero_page, (uint32_t)(PX - qx) * 16u, full(s));
-                    }
+                    if (qx < PX) bulk_g2s(xs + (k * PX + qx) * 16, p.zero_page, (uint32_t)(PX - qx) * 16u, full(s));
                 }
             }
         }
     }
-    __syncthreads();
-    if (warp == EPW) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
-    }
 }
 
-int attn_kv_x3_item_pixels() { return kx3::PX; }
-
-int launch_attn_kv_x3(const ConvTcParams& p, cudaStream_t s) {
+template <int MODE>
+static int launch_kv(const ConvTcParams& p, cudaStream_t s) {
     static DevCache cache;
-    const int num_sms = cache.get(reinterpret_cast<const void*>(k_attn_kv_x3));
+    const int num_sms = cache.get(reinterpret_cast<const void*>(k_attn_kv_wg<MODE>));
     if (num_sms <= 0) return -1;
-    if (p.c0 % (kx3::KCH * 4) != 0 || p.Ho < 1 || p.Wo < 1) return -1;
-    const long long total = (long long)p.B * p.Wo;
+    if (p.c0 % (kx3::KCH * (MODE == 1 ? 8 : 4)) != 0) return -1;
+    const long long total = (long long)p.B * ((p.H * p.W + kx3::PX - 1) / kx3::PX);
     const int grid = (int)(total < num_sms ? total : num_sms);
-    k_attn_kv_x3<<<grid, kx3::THREADS, kx3::SMEM, s>>>(p);
+    k_attn_kv_wg<MODE><<<grid, kx3::THREADS, kx3::SMEM, s>>>(p);
     return 1;
 }
+
+int attn_kv_tile_pixels() { return kx3::PX; }
+int launch_attn_kv(const ConvTcParams& p, cudaStream_t s) { return p.bf16 ? launch_kv<1>(p, s) : launch_kv<0>(p, s); }
+int launch_attn_kv_x3(const ConvTcParams& p, cudaStream_t s) { return launch_kv<2>(p, s); }
 
 }  // namespace sbk

@@ -1,27 +1,27 @@
-// tcgen05 implicit-GEMM convolutions for sm_100a: the 3x3 Block convs (81.5 % of the step's MACs) and the 1x1
-// channel mixes (res_conv, attention apply).  tf32 (or bf16) operands, fp32 accumulation in TMEM.
+// Warpgroup-MMA (wgmma) implicit-GEMM convolutions for sm_90a: the 3x3 Block convs (81.5 % of the step's MACs), the
+// 1x1 channel mixes (res_conv, attention apply), Downsample / Upsample and the vocoder's dilated Conv1d.  tf32 (or bf16)
+// operands from shared memory, fp32 accumulation in registers.
 //
-//   D[pixel][cout] (fp32, TMEM) += A[pixel][tap, cin] (smem) * W[cout][tap, cin] (smem)
+//   D[pixel][cout] (fp32, registers) += A[pixel][tap, cin] (smem) * W[cout][tap, cin] (smem)
 //
-// Mapping.  One CTA owns ROWS=2 rows of 128 pixels x NT output channels of one sample.  Each row is one UMMA
-// (M=128, N=NT, K=32 bytes) per tap and K step; the two rows use two TMEM accumulators (2*NT columns) and share
-// every weight stage.  For the 3x3 conv a row is 128 consecutive frames of one mel bin; for 1x1 convs the image
-// is flattened and a row is any 128 consecutive pixels.
+// Mapping.  One CTA owns one row of TPX = 128 pixels x NT output channels of one sample; each of its two consumer
+// warpgroups owns 64 of the pixels (one m64nNT wgmma per tap and K step).  For the 3x3 conv a row is 128 consecutive
+// frames of one mel bin; for 1x1 convs the image is flattened and a row is any 128 consecutive pixels.  (A 128 x NT tile
+// per CTA keeps the accumulators - and in fp32x3 mode their running sums - in the register file.)
 //
-// A operand.  Conv inputs are stored in HBM already in operand form (masked; Block activations GroupNorm-ed,
-// Mish-ed and time-biased by k_gn_act, see sbk_kernels.cu), so producing the A tile is a pure copy: eight
-// producer warps issue 16-byte cp.async (LDGSTS, zero-fill outside the image = the conv's zero padding) straight
-// into the UMMA no-swizzle K-major layout [16 B channel chunk][halo row][pixel][16 B].  In that layout eight
-// consecutive pixels x 16 B are one core matrix, so EVERY one of the nine taps is only a different descriptor
-// start address into the same halo tile (start += (r*130 + s)*16 B): each input element is fetched once per CTA
-// and feeds nine MMAs.  (v1 of this kernel applied GN+Mish in the producers; the MUFU/ALU work made those convs
-// 3x slower than the copy-only ones - profiles/r1_ops_tf32_v1.txt - hence the separate elementwise pass.)
+// A operand.  Conv inputs are stored in HBM already in operand form (masked; Block activations GroupNorm-ed, Mish-ed
+// and time-biased by k_gn_act, see sbk_kernels.cu), so producing the A tile is a pure copy straight into the wgmma
+// no-swizzle K-major layout [16 B channel chunk][halo row][pixel][16 B].  In that layout eight consecutive pixels x 16 B
+// are one core matrix, so EVERY one of the nine taps is only a different descriptor start address into the same halo
+// tile (start += (r*130 + s)*16 B): each input element is fetched once per CTA and feeds nine MMAs.
 //
 // B operand.  Weights are packed on the host into exactly the per-stage shared-memory image
-// [tap][chunk][cout][16 B] and streamed with one cp.async.bulk (UBLKCP) per stage, mbarrier complete_tx.
+// [tap][chunk][cout][16 B] and streamed with one cp.async.bulk per stage, mbarrier complete_tx.
 //
-// Pipeline.  STAGES-deep ring with full_a / full_b / empty mbarriers; one thread issues tcgen05.mma and frees
-// stages with tcgen05.commit; the epilogue (the eight producer warps) reads the accumulators with tcgen05.ld.
+// Pipeline.  STAGES-deep ring with full_a / full_b / empty mbarriers; a loader warp fills it with bulk copies (the
+// Downsample gathers are cp.async issued by the consumers themselves) while the consumer warpgroups issue one stage's
+// MMAs back to back, wait for them and free the stage.  The epilogue stages the accumulators through shared
+// memory ([pixel][column]), so one thread owns one pixel and a contiguous run of output channels.
 // All waits are bounded spins that trap instead of hanging the GPU.
 #include "sbk_tc.cuh"
 
@@ -31,26 +31,26 @@ namespace sbk {
 
 namespace tc {
 
-constexpr int ROWS = 2;               // M=128 pixel rows per CTA (two TMEM accumulators share every weight stage)
-constexpr int TPX = 128;              // pixels per row (= UMMA M)
-constexpr int NPROD = 256;            // producer / epilogue threads (8 warps)
-constexpr int NTHREADS = NPROD + 64;  // + MMA warp + weight-loader warp
+constexpr int ROWS = 1;               // output rows of TPX pixels per tile
+constexpr int TPX = 128;              // pixels per row = 2 consumer warpgroups x wgmma M (64)
+constexpr int NCONS = 256;            // consumer threads (2 warpgroups): MMAs + epilogue (Downsample: + A gathers)
+constexpr int NTHREADS = NCONS + 32;  // + loader warp
 
 // geometry of the A tile in shared memory, [16-byte K chunk][row][pixel][16 B]
 template <int GEOM> struct Geo;
-template <> struct Geo<G_C3> { static constexpr int HR = ROWS + 2, PXP = TPX + 2, TAPS = 9, KCH = 2, NACC = ROWS; };   // 3x3: halo tile
-template <> struct Geo<G_PW> { static constexpr int HR = ROWS, PXP = TPX, TAPS = 1, KCH = 8, NACC = ROWS; };           // 1x1: plain tile
-// 3x3 stride 2 (Downsample): 5 input rows; input columns de-interleaved into an odd plane (129 px: 2*w0-1+2i) and
+template <> struct Geo<G_C3> { static constexpr int HR = ROWS + 2, PXP = TPX + 2, TAPS = 9, KCH = 2, NACC = 1; };   // 3x3: halo tile
+template <> struct Geo<G_PW> { static constexpr int HR = ROWS, PXP = TPX, TAPS = 1, KCH = 8, NACC = 1; };           // 1x1: plain tile
+// 3x3 stride 2 (Downsample): 3 input rows; input columns de-interleaved into an odd plane (129 px: 2*w0-1+2i) and
 // an even plane (2*w0+2i) so that consecutive OUTPUT pixels read consecutive smem pixels for every tap.
-template <> struct Geo<G_DOWN> { static constexpr int HR = 2 * ROWS + 1, PXP = 2 * (TPX + 1), TAPS = 9, KCH = 2, NACC = ROWS; };
+template <> struct Geo<G_DOWN> { static constexpr int HR = 2 * ROWS + 1, PXP = 2 * (TPX + 1), TAPS = 9, KCH = 2, NACC = 1; };
 // ConvTranspose2d(4,2,1) (Upsample): per output parity (ph,pw) a 2x2-tap conv over the same 3x3-style input halo;
-// all four phases are computed from one halo tile into 4*ROWS accumulators; the stage carries all 16 (kh,kw) taps.
-template <> struct Geo<G_UP> { static constexpr int HR = ROWS + 2, PXP = TPX + 2, TAPS = 16, KCH = 2, NACC = 4 * ROWS; };
+// all four phases are computed from one halo tile into 4 accumulators; the stage carries all 16 (kh,kw) taps.
+template <> struct Geo<G_UP> { static constexpr int HR = ROWS + 2, PXP = TPX + 2, TAPS = 16, KCH = 2, NACC = 4; };
 
 // Conv1d, K taps, runtime dilation d (HiFi-GAN: K in {3,7,11}, d in {1,3,5}; halo (K-1)*d <= 50 samples): ONE strip of
-// ROWS*TPX + 64 samples per channel chunk; the two M=128 accumulators are the two consecutive 128-sample halves of the strip
-// and tap t of half j is the descriptor start (j*128 + t*d) samples into it - each input sample is fetched once for all taps.
-template <int K> struct GeoC1 { static constexpr int HR = 1, PXP = ROWS * TPX + 64, TAPS = K, KCH = 2, NACC = ROWS; };
+// TPX + 64 samples per channel chunk; tap t is the descriptor start t*d samples into it - each input sample is fetched
+// once for all taps.
+template <int K> struct GeoC1 { static constexpr int HR = 1, PXP = ROWS * TPX + 64, TAPS = K, KCH = 2, NACC = 1; };
 template <> struct Geo<G_C1K3> : GeoC1<3> {};
 template <> struct Geo<G_C1K7> : GeoC1<7> {};
 template <> struct Geo<G_C1K11> : GeoC1<11> {};
@@ -60,93 +60,40 @@ template <> struct Geo<G_C1K11> : GeoC1<11> {};
 using namespace tc;
 
 
-// Residency / pipeline / accumulator configuration.
-//   * persistent CTAs: each CTA loops over output tiles (round-robin), every role keeps its own ring / slot counters;
-//   * NSLOT TMEM accumulator slots: with two slots the epilogue of tile i overlaps the loads + MMAs of tile i+1;
-//   * two CTAs per SM when smem (<= ~108 KB) and TMEM (<= 256 columns) allow, else one CTA with a deeper ring.
-constexpr int pow2_cols(int c) { return c <= 32 ? 32 : c <= 64 ? 64 : c <= 128 ? 128 : c <= 256 ? 256 : 512; }
-// X3 (fp32x3 mode), 3x3 and 1x1 convs (TMSUM): TMEM holds one accumulation-run slot per output row plus the running
-// fp32 sums of the tile, 4*NT columns in all (see conv_tc_body); Downsample keeps its running sums in registers
-// (one CTA per SM: 64 accumulators per thread); Upsample runs unchunked.
-// PAIR (3x3 convs only): the CTA is one half of a cta_group::2 pair - it stages its own two output rows' A tile and HALF of
-// the weight tile (NT/2 output channels); see conv_tc_body.
-template <int GEOM, int NT, bool X3 = false, bool PAIR = false> struct Depth {
-    static constexpr int NB = PAIR ? NT / 2 : NT;           // weight rows (output channels) staged by this CTA
-    static constexpr int STAGE_BYTES = Geo<GEOM>::KCH * Geo<GEOM>::HR * Geo<GEOM>::PXP * 16 + Geo<GEOM>::TAPS * Geo<GEOM>::KCH * NB * 16;
-    static constexpr int SLOT_COLS = Geo<GEOM>::NACC * NT;
-    static constexpr int FIT2 = (108 * 1024) / STAGE_BYTES;
-    static constexpr int FIT1 = (220 * 1024) / STAGE_BYTES;
-    static constexpr bool TMSUM = X3 && (GEOM == G_C3 || GEOM == G_PW);
-    // long-K 3x3 convs (NT = 128) are MMA-bound: one CTA, deep ring, two accumulator slots.  Everything else is
-    // epilogue/latency-bound: two CTAs per SM double the epilogue warps; slots as TMEM (256 columns per CTA) allows.
-    // (TMSUM: a run's FLUSH stages stay resident for both row passes, so two CTAs need at least 3 stages each.)
-    static constexpr bool TWO = X3 ? (TMSUM && 4 * NT <= 256 && FIT2 >= 3)
-                                   : (FIT2 >= 2 && SLOT_COLS <= 256 && !(GEOM == G_C3 && NT == 128));
-    static constexpr int NSLOT = TMSUM ? 2 : (TWO ? (2 * SLOT_COLS <= 256 ? 2 : 1) : (2 * SLOT_COLS <= 512 ? 2 : 1));
-    static constexpr int TMEM_COLS = TMSUM ? 4 * NT : pow2_cols(NSLOT * SLOT_COLS);
-    static constexpr int STAGES = TWO ? (FIT2 > 4 ? 4 : FIT2) : (FIT1 > 6 ? 6 : FIT1);
-    static constexpr int MINB = TWO ? 2 : 1;
-    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + (3 * STAGES + 2 * NSLOT + 2) * 8 + 128 * 4 + 16 + 3 * NT * 4 + 64;
+// Persistent CTAs (one per SM: each CTA loops over output tiles round-robin) with as deep a ring as shared memory
+// allows next to the epilogue's [TPX][NT + 4] fp32 staging tile.
+template <int GEOM, int NT> struct Depth {
+    static constexpr int STAGE_BYTES = Geo<GEOM>::KCH * Geo<GEOM>::HR * Geo<GEOM>::PXP * 16 + Geo<GEOM>::TAPS * Geo<GEOM>::KCH * NT * 16;
+    static constexpr int LDS = NT + 4;                       // staging row pitch (floats): conflict-free float4 reads
+    static constexpr int SD_BYTES = TPX * LDS * 4;
+    static constexpr int FIT = (220 * 1024 - SD_BYTES) / STAGE_BYTES;
+    static constexpr int STAGES = FIT > 6 ? 6 : FIT;
+    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + SD_BYTES + 3 * STAGES * 8 + 128 * 4 + 3 * NT * 4 + 64;
+    static_assert(STAGES >= 2, "need at least 2 stages");
+    static_assert(SMEM <= 227 * 1024, "shared memory budget");
 };
 
 // RES: ResnetBlock-tail epilogue (1x1 res_conv + Mish(GN(h2raw)) side input), compile-time so that the plain 1x1 /
 // 3x3 instantiations do not pay its registers.
 //
-// X3 (fp32x3 mode, p.x3): two sub-stages per K stage (the kind::f16 correction MMAs over the packed fp16 chunks, then the
-// kind::tf32 main MMAs - sbk_internal.h: corr_chunk) AND chunked accumulation.  Measured on the B200
-// (profiles/r2_fp32x3_v1_*): the tensor core TRUNCATES its fp32 accumulator on every MMA, a bias of ~2^-25 |acc| per
-// instruction towards zero, so a single accumulation run over the hundreds of MMAs of a 3x3 conv loses 4e-6 ... 3e-5
-// relative - 10-50x the fp32 rounding the reference's own fp32 sums have.  An accumulation run is therefore cut every
-// FLUSH sub-stages and the partial sums are added in round-to-nearest fp32 outside the MMA pipe (below: where they live).
-//
-// PAIR (cta_group::2, G_C3 only).  Every SS-form UMMA reads its A tile (4 KB) and its B tile (NT x 32 B) from shared
-// memory: at M = N = 128 that is 8 KB per 64-clock instruction, the SM's whole shared-memory bandwidth.  A CTA pair cuts
-// the weight side in half: the two CTAs of a 2-CTA cluster own the two halves of a 4-row tile (2 rows = 2 M = 128
-// row-tiles each) and each stages only HALF of the weight tile; one tcgen05.mma.cta_group::2 (M = 256) issued by the
-// leader CTA computes row j of both CTAs, reading each CTA's A tile locally and the B halves from both shared memories
-// (6 KB instead of 8 KB per instruction and SM, and half the weight bytes through L2 -> smem).  Measured: a pure MMA
-// stream runs 11 % faster on pairs, the whole conv 0-10 % (fp32x3 level 0: 0.426 -> 0.385 ms; profiles/r2_experiments.md, 3-4).
-// Protocol:
-//   * both loaders fill their own ring; the peer's MMA warp relays "my stage s is full" to the leader's full barrier
-//     (remote mbarrier arrive), so the leader's issuer waits on ONE barrier per stage (count 2: local expect_tx + relay);
-//   * tcgen05.commit.cta_group::2 multicasts stage-empty / accumulator-full arrivals to the same barrier in both CTAs;
-//   * the epilogue warps of both CTAs (each reads its own TMEM: its 128 pixel rows) arrive on the LEADER's tempty barrier.
-//
-// RS ("row-shared" issue order, 64-output-channel 3x3 convs = level 0).  An N = 64 instruction still reads its whole 4 KB A
-// tile for half the math of an N = 128 one: with one MMA per (tap, output row) the 18 instructions of a stage read 108 KB
-// of operands in 576 clocks = 187 B/clk against the SM's 128 - the level-0 convs were shared-memory bound (tensor pipe 47-61 %).
-// Input-stationary order instead: ONE MMA per (input halo row, column tap) updates every output row that input row feeds.
-// Input row i feeds output row i+1 through kernel row 0, row i through kernel row 1 and row i-1 through kernel row 2, and
-// the two output rows' accumulators are adjacent TMEM columns, so with the weights of a column tap packed as
-// [kr=2 | kr=1 | kr=0] x 64 channels the middle halo rows are single N = 128 instructions (B = [W1|W0] resp. [W2|W1], D = both
-// rows) and the outer halo rows N = 64 ones: 12 instructions per stage instead of 18, the same MMA time, 84 KB of operand
-// reads instead of 108.  (The two N = 64 instructions come first in a run: they are the ones that may start an accumulator.)
-template <int GEOM, bool BF16, int NT, bool RES, bool X3, bool PAIR = false, bool RS = false>
+// X3 (fp32x3 mode, p.x3): two sub-stages per K stage (the f16 correction MMAs over the packed fp16 chunks, then the tf32
+// main MMAs - sbk_internal.h: corr_chunk) AND chunked accumulation.  The tensor core truncates its fp32 accumulator on
+// every MMA (a bias of ~2^-25 |acc| per instruction towards zero), so a single accumulation run over the hundreds of MMAs
+// of a 3x3 conv would lose several 1e-6 relative - more than the fp32 rounding of the reference's own sums.  An
+// accumulation run is therefore cut every FLUSH sub-stages and the partial sums are added in round-to-nearest fp32 into a
+// second register array.  (Upsample runs unchunked: its runs are short, 4 taps per phase.)
+template <int GEOM, bool BF16, int NT, bool RES, bool X3>
 __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     static_assert(!(X3 && BF16), "fp32x3 runs on tf32 operands");
-    static_assert(!PAIR || (GEOM == G_C3 && !RES), "CTA pairs: 3x3 convs only");
-    static_assert(!RS || (GEOM == G_C3 && NT == 64 && !RES && !PAIR), "row-shared issue order: 64-channel 3x3 convs on single CTAs");
     using G = Geo<GEOM>;
-    using D = Depth<GEOM, NT, X3, PAIR>;
-    constexpr int NB = D::NB;
-    // Upsample keeps its 8 accumulators (4 phases x 2 rows x 64 columns = all of TMEM) in one run: 256 register
-    // accumulators per thread do not exist, and its runs are short (4 taps: 96-192 MMAs per accumulator)
-    // Two homes for the running sums of the accumulation runs:
-    //   CHUNKED (Downsample): registers of the epilogue warps (64 per thread, one CTA per SM), two whole-tile TMEM slots;
-    //   TMSUM (3x3 and 1x1): TMEM.  Columns [0,NT) / [NT,2NT) are the RUN slots of output rows 0 / 1, [2NT,4NT) the
-    //   running sums.  The four epilogue warps of a row fold that row's finished run into its sums (tcgen05.ld run + ld
-    //   sum, fp32 round-to-nearest add, tcgen05.st) while the issuer works on the other row / the next run (see the
-    //   issuer): N = 128 tiles and two CTAs per SM where they fit, which the register variant cannot do (128
-    //   accumulators per thread spill at the 168-register ceiling of a 10-warp CTA; the N = 64 UMMA shape it forces ran at
-    //   474 vs 780 TFLOP/s of MMA issue, profiles/r2_ops_fp32x3_v2_chunked_nt64.txt).
-    constexpr bool TMSUM = D::TMSUM;
-    constexpr bool CHUNKED = X3 && GEOM == G_DOWN;
-    // sub-stages per accumulation run (p.flush overrides): 6 = three K stages of correction + main sub-stage, 54 MMAs per
-    // accumulator for a 3x3 conv (~1e-6 of truncation bias; 4 gave 2.0-2.5e-6 per estimator call on the goldens, 6 gives 2.2-2.9e-6 and 2-5 % less time)
-    const int FLUSH = p.flush > 0 ? p.flush : 6;
-    constexpr int STAGES = D::STAGES, NSLOT = D::NSLOT, SLOT_COLS = D::SLOT_COLS;
+    using D = Depth<GEOM, NT>;
+    constexpr int NACC = G::NACC;
+    constexpr bool CHUNKED = X3 && GEOM != G_UP;
+    // sub-stages per accumulation run: 6 = three K stages of correction + main sub-stage, 54 MMAs per accumulator for a
+    // 3x3 conv
+    const int FLUSH = CHUNKED ? 6 : (1 << 30);
+    constexpr int STAGES = D::STAGES, LDS = D::LDS;
     constexpr int LAG = STAGES >= 3 ? STAGES - 2 : 0;      // G_DOWN only: cp.async groups in flight behind the newest
-    static_assert(STAGES >= 2, "need at least 2 stages");
     constexpr int HR = G::HR, PXP = G::PXP, TAPS = G::TAPS, KCH = G::KCH;
     constexpr int EPC = BF16 ? 8 : 4;                      // elements per 16-byte channel chunk
     constexpr int CPS = KCH * EPC;                         // input channels per stage
@@ -155,120 +102,80 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     constexpr bool OUT16 = BF16 && GEOM != G_C3;
     constexpr int PLANE = HR * PXP * 16;                   // bytes between K chunks of the A tile
     constexpr int A_STAGE_BYTES = KCH * PLANE;
-    constexpr int B_STAGE_BYTES = TAPS * KCH * NB * 16;
+    constexpr int B_STAGE_BYTES = TAPS * KCH * NT * 16;
     constexpr bool BULK = GEOM != G_DOWN;                  // A tile = contiguous runs -> cp.async.bulk (no LSU work)
     constexpr bool C1 = geom_is_c1(GEOM);                  // Conv1d strip geometry
-    constexpr int SPAN = C1 ? ROWS * TPX : TPX;            // output pixels per tile along W
+    constexpr int SPAN = TPX;                              // output pixels per tile along W
+    constexpr int FR = NT / 2;                             // accumulator registers per thread and accumulator
+    constexpr int KMAIN = BF16 ? K_BF16 : K_TF32;
 
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* sA = smem;                                            // [STAGES][KCH][HR][PXP][16]
     uint8_t* sB = sA + STAGES * A_STAGE_BYTES;                     // [STAGES][TAPS][KCH][NT][16]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sB + STAGES * B_STAGE_BYTES);   // full[S], empty[S], tfull[NSLOT], tempty[NSLOT], fa[S]*, kv
-    // GroupNorm partials of the current tile: one private slot row per epilogue warp (plain read-modify-write by lane 0,
+    float* sD = reinterpret_cast<float*>(sB + STAGES * B_STAGE_BYTES);            // [TPX][LDS] accumulator staging
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sD + TPX * LDS);                 // full_b[S], empty[S], full_a[S]
+    // GroupNorm partials of the current tile: one private slot row per consumer warp (plain read-modify-write by lane 0,
     // no atomics), summed in a fixed order at the end of the tile and flushed as fp64 -> the totals can only differ between
     // runs through the order of the fp64 global atomics (1e-16), so the fp32 mean / rstd - and the sampler - are reproducible.
-    // (fp32 smem atomics made the result depend on warp arrival order; fp64 smem atomics fixed that but cost 0.035 ms per
-    // level-0 conv in CAS contention: profiles/r1_ops_tf32_v24_fp64_smem_atomics.txt.)
-    float* s_st = reinterpret_cast<float*>(bars + 3 * STAGES + 2 * NSLOT + 2);   // [8 warps][8 groups][2]
-    uint32_t* s_tmem = reinterpret_cast<uint32_t*>(s_st + 128);
-    float* s_rg = reinterpret_cast<float*>(s_tmem + 4);                          // EPI_RES: mean|scale|beta [NT] each
+    float* s_st = reinterpret_cast<float*>(bars + 3 * STAGES);                    // [8 warps][8 groups][2]
+    float* s_rg = s_st + 128;                                                     // EPI_RES: mean|scale|beta [NT] each
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    // (the warp index is broadcast from lane 0 so that the compiler can prove the role branches warp-uniform: wgmma code
+    // under a branch it considers divergent is serialised)
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
     const int Cin = p.c0 + p.c1;
     const int HW = p.H * p.W;
     const int ksteps = Cin / CPS;
-    // fp32x3 mode: each K stage runs twice - the kind::f16 correction sub-stage (x_lo*w + x*w_lo from the packed fp16
-    // chunks, sbk_internal.h: corr_chunk) first, then the kind::tf32 main sub-stage (x_hi*w_hi): small terms first
+    // fp32x3 mode: each K stage runs twice - the f16 correction sub-stage (x_lo*w + x*w_lo from the packed fp16 chunks,
+    // sbk_internal.h: corr_chunk) first, then the tf32 main sub-stage (x_hi*w_hi): small terms first
     const int ksteps_t = X3 ? 2 * ksteps : ksteps;
-    const int nchunks = (CHUNKED || TMSUM) ? (ksteps_t + FLUSH - 1) / FLUSH : 1;     // accumulation runs per tile
     // ---- tile space: (sample, pixel tile, N tile), N tile fastest so neighbours in time share the A tile in L2
     const int wt_w = (GEOM == G_DOWN ? p.Wo : p.W), wt_h = (GEOM == G_DOWN ? p.Ho : p.H);
     const int wtiles = (wt_w + SPAN - 1) / SPAN;
-    constexpr int TROWS = PAIR ? 2 * ROWS : ROWS;           // output rows per (pair) tile
-    const int mtiles = GEOM == G_PW ? (HW + ROWS * TPX - 1) / (ROWS * TPX) : wtiles * ((wt_h + TROWS - 1) / TROWS);
+    const int mtiles = GEOM == G_PW ? (HW + TPX - 1) / TPX : wtiles * wt_h;
     const int ntn = p.Cout / NT;
     const int total_tiles = p.B * mtiles * ntn;
-    const uint32_t rank = PAIR ? cluster_ctarank() : 0u;   // PAIR: rank 0 = leader (issues the MMAs), rank 1 = peer
-    const int tile0 = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x, tstep = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-    auto decode = [&](int t, int& b, int& h0, int& w0, int& n0, int& mt) {
+    auto decode = [&](int t, int& b, int& h0, int& w0, int& n0) {
         const int nt = t % ntn; const int r = t / ntn;
-        mt = r % mtiles; b = r / mtiles; n0 = nt * NT;
-        if (GEOM == G_PW) { w0 = 0; h0 = mt * ROWS; }
-        else { w0 = (mt % wtiles) * SPAN; h0 = (mt / wtiles) * TROWS + (int)rank * ROWS; }
+        const int mt = r % mtiles; b = r / mtiles; n0 = nt * NT;
+        if (GEOM == G_PW) { w0 = 0; h0 = mt; }
+        else { w0 = (mt % wtiles) * SPAN; h0 = mt / wtiles; }
     };
 
     const uint32_t bar0 = smem_u32(bars);
     auto full_b = [&](int s) { return bar0 + 8u * s; };                       // weights (+ bulk A runs): tx-count
-    auto empty = [&](int s) { return bar0 + 8u * (STAGES + s); };
-    auto tfull = [&](int a) { return bar0 + 8u * (2 * STAGES + a); };         // accumulator slot complete
-    auto tempty = [&](int a) { return bar0 + 8u * (2 * STAGES + NSLOT + a); };// accumulator slot drained
-    auto full_a = [&](int s) { return bar0 + 8u * (2 * STAGES + 2 * NSLOT + s); };   // G_DOWN cp.async producers
-    const uint32_t kv_bar = bar0 + 8u * (3 * STAGES + 2 * NSLOT);
+    auto empty = [&](int s) { return bar0 + 8u * (STAGES + s); };             // every consumer warp done with the stage
+    auto full_a = [&](int s) { return bar0 + 8u * (2 * STAGES + s); };        // G_DOWN cp.async producers
 
     // ---- one-time setup
     if (tid == 0) {
-        // PAIR: the leader's full barrier also takes the peer's relay arrival; its tempty barriers take both CTAs' epilogue warps
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full_a(s), NPROD / 32); mbar_init(full_b(s), (PAIR && rank == 0) ? 2 : 1); mbar_init(empty(s), 1); }
-        // (TMSUM: slot a belongs to output row a and is drained by that row's four epilogue warps)
-        for (int a = 0; a < NSLOT; ++a) { mbar_init(tfull(a), 1); mbar_init(tempty(a), (TMSUM ? NPROD / 64 : NPROD / 32) * (PAIR ? 2 : 1)); }
-        mbar_init(kv_bar, 1);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(full_a(s), NCONS / 32); mbar_init(full_b(s), 1); mbar_init(empty(s), NCONS / 32); }
         fence_barrier_init();
     }
-    if (warp == NPROD / 32) { if constexpr (PAIR) tmem_alloc2(smem_u32(s_tmem), D::TMEM_COLS); else tmem_alloc(smem_u32(s_tmem), D::TMEM_COLS); }
     if (tid < 128) s_st[tid] = 0.f;
-    tc_fence_before();
-    if constexpr (PAIR) cluster_sync_all(); else __syncthreads();    // (pair: the peer's barriers must exist before any remote arrival)
-    tc_fence_after();
-    const uint32_t lead_bar0 = PAIR ? mapa_shared(bar0, 0u) : bar0;  // the leader CTA's barrier block (cluster address)
-    auto tempty_arrive = [&](int a) {                                 // one epilogue warp done with accumulator slot a
-        if constexpr (PAIR) mbar_arrive_cluster(lead_bar0 + 8u * (2 * STAGES + NSLOT + a));
-        else mbar_arrive(tempty(a));
-    };
-    const uint32_t tmem_base = *s_tmem;
+    __syncthreads();
 
-    if (warp < NPROD / 32) {
+    if (warp < NCONS / 32) {
         // =========================================================================================================
-        // warps 0-7: (G_DOWN: cp.async A producers, then) epilogue of every tile
+        // consumer warpgroups: (G_DOWN: cp.async A producers,) MMAs, epilogue of every tile
         // =========================================================================================================
-        uint32_t it = 0;      // G_DOWN producer ring counter
-        uint32_t ar = 0;      // accumulation-run counter (accumulator slot / phase); one run per tile unless CHUNKED
-        for (int t = tile0; t < total_tiles; t += tstep) {
-            int b, h0, w0, n0, mt;
-            decode(t, b, h0, w0, n0, mt);
-            // CHUNKED: accumulation runs of this tile are drained, in order, into register accumulators (round-to-nearest
-            // fp32 adds): this thread's TMEM lane (pixel) x the NT columns of its accumulator row
-            float accr[CHUNKED ? NT : 1];
-            int drained = 0;
-            auto drain_run = [&]() {
-                const int rs = ar % NSLOT;
-                mbar_wait(tfull(rs), (ar / NSLOT) & 1);
-                tc_fence_after();
-                const uint32_t ta = tmem_base + rs * SLOT_COLS + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)((warp >> 2) * NT);
-#pragma unroll
-                for (int cb = 0; cb < (CHUNKED ? NT : 0); cb += 32) {
-                    uint32_t r[32];
-                    tmem_ld32(ta + cb, r);
-                    if (drained == 0) {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) accr[cb + i] = __uint_as_float(r[i]);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) accr[cb + i] += __uint_as_float(r[i]);
-                    }
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) tempty_arrive(rs);
-                ++ar; ++drained;
-            };
-            if (!BULK) {
-                // ---- A producers (Downsample only): 16-byte cp.async gathers that de-interleave even/odd columns
-                constexpr int SLOTS = HR * PXP * KCH;
-                constexpr int PER = (SLOTS + NPROD - 1) / NPROD;
-                uint32_t sl_dst[PER]; long long sl_off[PER]; int sl_chunk[PER]; bool sl_ok[PER];
+        const int wg = warp >> 2, wt = tid & 127;                  // warpgroup = pixel half of the tile
+        uint32_t it = 0;                                           // ring counter (stages consumed by this CTA)
+        // ---- A producers (Downsample only): 16-byte cp.async gathers that de-interleave even/odd columns
+        constexpr int SLOTS = HR * PXP * KCH;
+        constexpr int PER = BULK ? 1 : (SLOTS + NCONS - 1) / NCONS;
+        uint32_t sl_dst[PER]; long long sl_off[PER]; int sl_chunk[PER]; bool sl_ok[PER];
+        const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
+        constexpr uint32_t D_HI = desc_hi(128);                    // SBO = 128 B for both operands
+        float acc[NACC][FR];
+        float sum[CHUNKED ? FR : 1];
+        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+            int b, h0, w0, n0;
+            decode(t, b, h0, w0, n0);
+            if constexpr (!BULK) {
 #pragma unroll
                 for (int j = 0; j < PER; ++j) {
-                    const int e = tid + j * NPROD;
+                    const int e = tid + j * NCONS;
                     const bool in = e < SLOTS;
                     const int k = in ? e / (HR * PXP) : 0, item = in ? e - k * (HR * PXP) : 0;     // pixel fastest
                     const int r = item / PXP, q = item - r * PXP;
@@ -279,55 +186,119 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                     sl_off[j] = (ok ? (long long)(b * p.H + hi) : 0) * 1048576 + (ok ? wi : 0);   // pack (row, w)
                     sl_dst[j] = in ? (uint32_t)(k * PLANE + (r * PXP + q) * 16) : 0xFFFFFFFFu;
                 }
-                const uint32_t a0 = smem_u32(sA);
-                for (int ks = 0; ks < ksteps_t + LAG; ++ks) {
-                    if (ks < ksteps_t) {
-                        const uint32_t g = it + ks;
-                        const int s = g % STAGES;
-                        mbar_wait(empty(s), ((g / STAGES) & 1) ^ 1);
-                        const int kb = X3 ? ks / 2 : ks;
-                        const bool lo = X3 && (ks & 1) == 0;
-                        const int ck = kb * KCH;
-                        const bool second = ck * EPC >= p.c0;
-                        const uint8_t* src = reinterpret_cast<const uint8_t*>(second ? (lo ? p.in1_lo : p.in1) : (lo ? p.in0_lo : p.in0));
-                        const int chs = (second ? p.c1 : p.c0) / EPC;
-                        const int c0k = second ? ck - p.c0 / EPC : ck;
+            }
+            auto produce = [&](int ks) {
+                const uint32_t g = it + ks;
+                const int s = g % STAGES;
+                mbar_wait(empty(s), ((g / STAGES) & 1) ^ 1);
+                const int kb = X3 ? ks / 2 : ks;
+                const bool lo = X3 && (ks & 1) == 0;
+                const int ck = kb * KCH;
+                const bool second = ck * EPC >= p.c0;
+                const uint8_t* src = reinterpret_cast<const uint8_t*>(second ? (lo ? p.in1_lo : p.in1) : (lo ? p.in0_lo : p.in0));
+                const int chs = (second ? p.c1 : p.c0) / EPC;
+                const int c0k = second ? ck - p.c0 / EPC : ck;
 #pragma unroll
-                        for (int j = 0; j < PER; ++j) {
-                            if (sl_dst[j] == 0xFFFFFFFFu) continue;
-                            const long long row = sl_off[j] / 1048576, wi = sl_off[j] % 1048576;
-                            const uint8_t* gp = src + ((row * chs + c0k + sl_chunk[j]) * p.W + wi) * 16;
-                            cp_async16(a0 + s * A_STAGE_BYTES + sl_dst[j], gp, sl_ok[j] ? 16u : 0u);
+                for (int j = 0; j < PER; ++j) {
+                    if (sl_dst[j] == 0xFFFFFFFFu) continue;
+                    const long long row = sl_off[j] / 1048576, wi = sl_off[j] % 1048576;
+                    const uint8_t* gp = src + ((row * chs + c0k + sl_chunk[j]) * p.W + wi) * 16;
+                    cp_async16(a0 + s * A_STAGE_BYTES + sl_dst[j], gp, sl_ok[j] ? 16u : 0u);
+                }
+            };
+            auto release = [&](uint32_t g) {                        // this warp's MMAs of stage g have completed
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty(g % STAGES));
+            };
+            // MMAs of K sub-stage ks; keeps one stage of MMAs in flight, folds a finished accumulation run (CHUNKED)
+            // (kind: the MMA kind of sub-stage ks as a compile-time constant, so no branch separates the wgmmas of a run)
+            auto compute = [&](int ks, auto kind) {
+                const uint32_t g = it + ks;
+                const int s = g % STAGES;
+                const uint32_t ph = (g / STAGES) & 1;
+                if (!BULK) mbar_wait(full_a(s), ph);
+                mbar_wait(full_b(s), ph);                  // weights (+ the A runs when they are bulk copies)
+                const int run_lo = CHUNKED ? ks - ks % FLUSH : 0;
+                const bool last = ks == ksteps_t - 1 || (CHUNKED && ks - run_lo == FLUSH - 1);
+                const uint32_t a_lo = desc_lo(a0 + s * A_STAGE_BYTES, PLANE) + (uint32_t)(64 * wg);   // this warpgroup's 64 pixels
+                const uint32_t b_lo = desc_lo(b0 + s * B_STAGE_BYTES, NT * 16);
+                const uint32_t dil = C1 ? (uint32_t)p.dil : 0u;
+                auto issue = [&](auto kind) {
+                    constexpr int KD = decltype(kind)::value;
+#pragma unroll
+                    for (int kk = 0; kk < KCH / 2; ++kk) {
+                        const uint32_t a_k = a_lo + (uint32_t)(kk * 2 * (PLANE / 16)), b_k = b_lo + (uint32_t)(kk * 2 * NT);
+                        if (GEOM == G_UP) {
+                            // ho = 2*hi - 1 + kh: parity ph uses (kh=1,dh=0),(kh=3,dh=-1) if ph=0 and (kh=0,dh=+1),(kh=2,dh=0) if ph=1
+#pragma unroll
+                            for (int phase = 0; phase < 4; ++phase) {
+                                const int pph = phase >> 1, pw = phase & 1;
+#pragma unroll
+                                for (int t2 = 0; t2 < 4; ++t2) {
+                                    const int a = t2 >> 1, bb = t2 & 1;
+                                    const int kh = pph ? (a ? 2 : 0) : (a ? 3 : 1), kw = pw ? (bb ? 2 : 0) : (bb ? 3 : 1);
+                                    const int dh = pph ? (a ? 0 : 1) : (a ? -1 : 0), dw = pw ? (bb ? 0 : 1) : (bb ? -1 : 0);
+                                    wgmma<NT, KD>(acc[GEOM == G_UP ? phase : 0], desc_pack(a_k + (uint32_t)((1 + dh) * PXP + 1 + dw), D_HI),
+                                                  desc_pack(b_k + (uint32_t)((kh * 4 + kw) * KCH * NT), D_HI),
+                                                  ((ks - run_lo) | kk | t2) != 0 ? 1u : 0u);
+                                }
+                            }
+                        } else {
+#pragma unroll
+                            for (int tap = 0; tap < TAPS; ++tap) {
+                                const int r = TAPS == 9 ? tap / 3 : 0, sx = TAPS == 9 ? tap % 3 : 0;
+                                // DOWN: input row r; column tap s reads the odd plane at x (s=0) / x+1 (s=2), the even plane at x (s=1)
+                                const uint32_t aoff = GEOM == G_DOWN ? (uint32_t)(r * PXP + (sx == 1 ? TPX + 1 : (sx == 2 ? 1 : 0)))
+                                                    : C1 ? (uint32_t)tap * dil
+                                                         : (uint32_t)(r * PXP + sx);
+                                wgmma<NT, KD>(acc[0], desc_pack(a_k + aoff, D_HI), desc_pack(b_k + (uint32_t)(tap * KCH * NT), D_HI),
+                                              ((ks - run_lo) | kk | tap) != 0 ? 1u : 0u);
+                            }
                         }
                     }
+                };
+                wg_fence();
+                issue(kind);
+                wg_commit();
+                // The stage's MMAs run back to back; the wait sits on the uniform path after them (the loader keeps the
+                // next stages in flight meanwhile), and a finished accumulation run is folded branch-free.
+                wg_wait<0>();
+#pragma unroll
+                for (int a = 0; a < NACC; ++a) wg_fence_regs(acc[a]);
+                release(g);
+                if constexpr (CHUNKED) {
+                    const bool first = run_lo == 0;
+#pragma unroll
+                    for (int i = 0; i < FR; ++i) sum[i] = last ? (first ? acc[0][i] : sum[i] + acc[0][i]) : sum[i];
+                }
+            };
+            constexpr auto kind_c = std::integral_constant<int, K_F16>{};     // fp32x3 correction sub-stage (even ks)
+            constexpr auto kind_m = std::integral_constant<int, KMAIN>{};
+            if constexpr (BULK && X3) {
+                for (int ks = 0; ks < ksteps_t; ks += 2) { compute(ks, kind_c); compute(ks + 1, kind_m); }
+            } else if constexpr (BULK) {
+                for (int ks = 0; ks < ksteps_t; ++ks) compute(ks, kind_m);
+            } else {
+                for (int ks = 0; ks < ksteps_t + LAG; ++ks) {
+                    if (ks < ksteps_t) produce(ks);
                     cp_async_commit();                       // (empty groups past the last stage keep the accounting uniform)
                     if (ks >= LAG) {
                         cp_async_wait<LAG>();                // this thread's copies of stage ks-LAG have landed
                         fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor core
                         __syncwarp();
                         if (lane == 0) mbar_arrive(full_a((it + ks - LAG) % STAGES));
-                        if constexpr (CHUNKED) {
-                            // These warps are also the ones that drain the accumulation runs: a run whose last stage has
-                            // been handed to the MMA issuer completes without further production, so it is drained here -
-                            // otherwise the issuer would wait for a free TMEM slot while we wait for a free smem stage.
-                            while (drained < nchunks) {
-                                const int last = (drained + 1) * FLUSH < ksteps_t ? (drained + 1) * FLUSH - 1 : ksteps_t - 1;
-                                if (last > ks - LAG) break;
-                                drain_run();
-                            }
-                        }
+                        if (X3 && ((ks - LAG) & 1) == 0) compute(ks - LAG, kind_c);
+                        else compute(ks - LAG, kind_m);
                     }
                 }
-                it += ksteps_t;
             }
+            it += ksteps_t;
 
             // ---- epilogue of tile t
-            const int slot = ar % NSLOT;                           // (!CHUNKED: the slot of this tile's only run)
-            const uint32_t tslot = tmem_base + slot * SLOT_COLS;
             if constexpr (RES) {
                 asm volatile("bar.sync 1, 256;" ::: "memory");        // previous tile's readers of s_rg are done
                 const int cpg = p.Cout / kGroups;
-                for (int i = tid; i < NT; i += NPROD) {
+                for (int i = tid; i < NT; i += NCONS) {
                     const int c = n0 + i, g = c / cpg;
                     const double sm_ = p.rgn.stats[(b * kGroups + g) * 2], ss = p.rgn.stats[(b * kGroups + g) * 2 + 1];
                     const double m = sm_ * (double)p.rgn.inv_count;
@@ -339,415 +310,187 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 }
                 asm volatile("bar.sync 1, 256;" ::: "memory");
             }
-            bool acc_ready = false;                                // the tfull wait is taken after the epilogue's own loads are in flight
-            const int q4 = warp & 3, jrow = warp >> 2;            // TMEM lane quarter / accumulator (output row)
-            const int px = q4 * 32 + lane;
+            // one thread = one pixel x a contiguous half of the NT columns (NT = 32: the first 128 threads, all columns)
+            const int px = tid & 127, chalf = tid >> 7;
+            const int cb_lo = NT >= 64 ? chalf * (NT / 2) : 0, cb_hi = NT >= 64 ? cb_lo + NT / 2 : (chalf == 0 ? NT : 0);
             const int Ho = (GEOM == G_DOWN || GEOM == G_UP) ? p.Ho : p.H, Wo = (GEOM == G_DOWN || GEOM == G_UP) ? p.Wo : p.W;
             const int CHo = p.Cout / 4;                            // 16-byte channel chunks of the output tensor
             int ho, wo; bool valid;
             if (GEOM == G_C3 || GEOM == G_DOWN) {
-                ho = h0 + jrow; wo = w0 + px;
+                ho = h0; wo = w0 + px;
                 valid = ho < Ho && wo < Wo;
             } else if (C1) {
-                ho = 0; wo = w0 + jrow * TPX + px;
+                ho = 0; wo = w0 + px;
                 valid = wo < Wo;
             } else if (GEOM == G_UP) {
-                valid = (h0 + jrow) < p.H && (w0 + px) < p.W;          // per-phase coordinates are formed below
-                ho = 2 * (h0 + jrow); wo = 2 * (w0 + px);
+                valid = h0 < p.H && (w0 + px) < p.W;                 // per-phase coordinates are formed below
+                ho = 2 * h0; wo = 2 * (w0 + px);
             } else {
-                const long long m = (long long)(h0 + jrow) * TPX + px;
+                const long long m = (long long)h0 * TPX + px;
                 valid = m < HW;
                 ho = valid ? (int)(m / p.W) : 0;
                 wo = valid ? (int)(m - (long long)ho * p.W) : 0;
             }
             if (!valid) { ho = 0; wo = 0; }
-        {
-        const int cpg = p.Cout / kGroups;
-        const float* bp = p.bias ? p.bias + (long long)b * p.bias_bstride + n0 : nullptr;
-        constexpr int NPH = GEOM == G_UP ? 4 : 1;
-#pragma unroll 1
-        for (int phase = 0; phase < NPH; ++phase) {
-        const int ho_p = GEOM == G_UP ? ho + (phase >> 1) : ho;
-        const int wo_p = GEOM == G_UP ? wo + (phase & 1) : wo;
-        const int acc = GEOM == G_UP ? phase * ROWS + jrow : jrow;
-        const float mo = (p.out_mask || RES) ? __ldg(p.mask + (long long)b * p.T + ((long long)wo_p << p.lvl)) : 1.f;
-        // element (b, ho, chunk, wo) of a [B][H][C/4][W][4] tensor; consecutive lanes = consecutive pixels = 16 B apart
-        const long long obase = (((long long)(b * Ho + ho_p) * CHo + n0 / 4) * Wo + wo_p) * 4;
-        const long long cstride = (long long)Wo * 4;           // floats between consecutive channel chunks
-        // bf16 outputs: index of the 16-byte chunk (b, ho, n0/8, wo) in a [B][H][C/8][W] grid of chunks; the chunks of one
-        // pixel are Wo apart, consecutive lanes (pixels) are adjacent: a warp store is again 512 contiguous bytes
-        const long long ochunk = OUT16 ? (((long long)(b * Ho + ho_p) * (p.Cout / 8) + n0 / 8) * Wo + wo_p) : 0;
-        // ResnetBlock tail: the h2raw side input does not depend on the accumulators, so chunk block 0 is requested before
-        // the tfull wait and block cb+32 as soon as block cb has been consumed: the global latency hides under the TMEM
-        // load, the Mish math and the stores.  (The attention apply's residual read is a plain streaming add; prefetching
-        // it only cost registers.)
-        constexpr bool SIDE = GEOM == G_PW;                     // the 1x1 convs never carry GN statistics
-        const float* pre_src = RES ? p.rraw : nullptr;
-        const bool pre_on = RES && valid && mo != 0.f;
-        float4 pre[RES ? 8 : 1];
-        if constexpr (RES) {
+            const int cpg = p.Cout / kGroups;
+            const float* bp = p.bias ? p.bias + (long long)b * p.bias_bstride + n0 : nullptr;
 #pragma unroll
-            for (int i = 0; i < 8; ++i)
-                pre[i] = pre_on ? __ldg(reinterpret_cast<const float4*>(pre_src + obase + i * cstride)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-        if constexpr (CHUNKED) {
-            while (drained < nchunks) drain_run();
-            acc_ready = true;
-        }
-        if constexpr (TMSUM) {
-            // fold every accumulation run of this row into the running sums in TMEM (this thread's lane x NT columns)
-            const uint32_t trun = tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(jrow * NT);
-            const uint32_t tsum = trun + 2 * NT;
-            for (int c = 0; c < nchunks; ++c, ++ar) {
-                mbar_wait(tfull(jrow), ar & 1);
-                tc_fence_after();
-#pragma unroll 1
-                for (int cb = 0; cb < NT; cb += 32) {
-                    uint32_t r[32];
-                    tmem_ld32(trun + cb, r);
-                    if (c > 0) {
-                        uint32_t q[32];
-                        tmem_ld32(tsum + cb, q);
+            for (int phase = 0; phase < NACC; ++phase) {
+            // accumulators -> staging tile [pixel][column]
+            asm volatile("bar.sync 2, 256;" ::: "memory");            // previous readers of the staging tile are done
+            {
+                auto stage_out = [&](const float (&res)[FR]) {
 #pragma unroll
-                        for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) + __uint_as_float(q[i]));
-                    }
-                    tmem_st32(tsum + cb, r);
-                }
-                tmem_wait_st();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) tempty_arrive(jrow);
+                    for (int i = 0; i < FR; i += 2)
+                        *reinterpret_cast<float2*>(&sD[(64 * wg + frag_row(wt, i)) * LDS + frag_col(wt, i)]) = make_float2(res[i], res[i + 1]);
+                };
+                if constexpr (CHUNKED) stage_out(sum);
+                else stage_out(acc[phase]);
             }
-            acc_ready = true;
-        }
-#pragma unroll (CHUNKED ? NT / 32 : 1)
-        for (int cb = 0; cb < NT; cb += 32) {
-            if (!acc_ready) {
-                mbar_wait(tfull(slot), (ar / NSLOT) & 1);
-                tc_fence_after();
-                acc_ready = true;
-            }
-            uint32_t r[32];
-            if constexpr (CHUNKED) {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(accr[cb + i]);
-            } else if constexpr (TMSUM) {
-                tmem_ld32(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(2 * NT + acc * NT + cb), r);
-            } else {
-                tmem_ld32(tslot + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(acc * NT + cb), r);
-            }
-            float v[32];
-#pragma unroll
-            for (int i = 0; i < 32; i += 4) {
-                const float4 bb = bp ? __ldg(reinterpret_cast<const float4*>(bp + cb + i)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                v[i] = __uint_as_float(r[i]) + bb.x; v[i + 1] = __uint_as_float(r[i + 1]) + bb.y;
-                v[i + 2] = __uint_as_float(r[i + 2]) + bb.z; v[i + 3] = __uint_as_float(r[i + 3]) + bb.w;
-            }
+            asm volatile("bar.sync 2, 256;" ::: "memory");
+            const int ho_p = GEOM == G_UP ? ho + (phase >> 1) : ho;
+            const int wo_p = GEOM == G_UP ? wo + (phase & 1) : wo;
+            const float mo = (p.out_mask || RES) ? __ldg(p.mask + (long long)b * p.T + ((long long)wo_p << p.lvl)) : 1.f;
+            // element (b, ho, chunk, wo) of a [B][H][C/4][W][4] tensor; consecutive threads = consecutive pixels = 16 B apart
+            const long long obase = (((long long)(b * Ho + ho_p) * CHo + n0 / 4) * Wo + wo_p) * 4;
+            const long long cstride = (long long)Wo * 4;           // floats between consecutive channel chunks
+            // bf16 outputs: index of the 16-byte chunk (b, ho, n0/8, wo) in a [B][H][C/8][W] grid of chunks; the chunks of one
+            // pixel are Wo apart, consecutive threads (pixels) are adjacent: a warp store is again 512 contiguous bytes
+            const long long ochunk = OUT16 ? (((long long)(b * Ho + ho_p) * (p.Cout / 8) + n0 / 8) * Wo + wo_p) : 0;
+            // ResnetBlock tail: the h2raw side input does not depend on the accumulators, so the first 32-column block is
+            // requested before the staging-tile reads and block cb+32 as soon as block cb has been consumed
+            constexpr bool SIDE = GEOM == G_PW;                     // the 1x1 convs never carry GN statistics
+            const float* pre_src = RES ? p.rraw : nullptr;
+            const bool pre_on = RES && valid && mo != 0.f;
+            float4 pre[RES ? 8 : 1];
             if constexpr (RES) {
-                // ResnetBlock tail: + Mish(GN(h2raw)) * mask  (diffusion.py:77-78)
-                if (pre_on) {
 #pragma unroll
-                    for (int i = 0; i < 32; i += 4) {
-                        const float rr[4] = {pre[i / 4].x, pre[i / 4].y, pre[i / 4].z, pre[i / 4].w};
+                for (int i = 0; i < 8; ++i)
+                    pre[i] = pre_on && cb_lo < cb_hi ? __ldg(reinterpret_cast<const float4*>(pre_src + obase + (cb_lo / 4 + i) * cstride))
+                                                     : make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+#pragma unroll 1
+            for (int cb = cb_lo; cb < cb_hi; cb += 32) {
+                float v[32];
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const int cl = cb + i + e;
-                            const float xn = (rr[e] - s_rg[cl]) * s_rg[NT + cl] + s_rg[2 * NT + cl];
-                            v[i + e] += X3 ? mish_exact(xn) : mish_fast(xn);
-                        }
-                    }
-                    if (cb + 32 < NT) {
-#pragma unroll
-                        for (int i = 0; i < 8; ++i)
-                            pre[i] = __ldg(reinterpret_cast<const float4*>(pre_src + obase + ((cb + 32) / 4 + i) * cstride));
-                    }
+                for (int i = 0; i < 32; i += 4) {
+                    const float4 r = *reinterpret_cast<const float4*>(&sD[px * LDS + cb + i]);
+                    const float4 bb = bp ? __ldg(reinterpret_cast<const float4*>(bp + cb + i)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                    v[i] = r.x + bb.x; v[i + 1] = r.y + bb.y; v[i + 2] = r.z + bb.z; v[i + 3] = r.w + bb.w;
                 }
-            } else if (p.addin && valid) {
-                // fp32-exact residual (attention: x + g*P x): the tensor core only carries the small g*P x term
-                if constexpr (OUT16) {
-                    const uint4* ap = reinterpret_cast<const uint4*>(p.addin) + ochunk + (long long)(cb / 8) * Wo;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const uint4 a = __ldg(ap + (long long)j * Wo);
-                        v[8 * j + 0] += bf16_lo(a.x); v[8 * j + 1] += bf16_hi(a.x); v[8 * j + 2] += bf16_lo(a.y); v[8 * j + 3] += bf16_hi(a.y);
-                        v[8 * j + 4] += bf16_lo(a.z); v[8 * j + 5] += bf16_hi(a.z); v[8 * j + 6] += bf16_lo(a.w); v[8 * j + 7] += bf16_hi(a.w);
-                    }
-                } else {
-                    const float* ap = p.addin + obase + (cb / 4) * cstride;
-#pragma unroll
-                    for (int i = 0; i < 32; i += 4) {
-                        const float4 av = __ldg(reinterpret_cast<const float4*>(ap + (i / 4) * cstride));
-                        v[i] += av.x; v[i + 1] += av.y; v[i + 2] += av.z; v[i + 3] += av.w;
-                    }
-                }
-            }
-            if (p.out_mask) {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) v[i] *= mo;
-            }
-            if (C1 && p.act_out) {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) v[i] = v[i] > 0.f ? v[i] : v[i] * p.slope;
-            }
-            if (valid) {
-                if constexpr (OUT16) {
-                    uint4* op = reinterpret_cast<uint4*>(p.out) + ochunk + (long long)(cb / 8) * Wo;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j)
-                        op[(long long)j * Wo] = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
-                                                           pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
-                } else {
-                    float* op = p.out + obase + (cb / 4) * cstride;
-#pragma unroll
-                    for (int i = 0; i < 32; i += 4) *reinterpret_cast<float4*>(op + (i / 4) * cstride) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-                    if (GEOM != G_C3 && p.out_lo) {
-                        float* lp = p.out_lo + obase + (cb / 4) * cstride;
+                if constexpr (RES) {
+                    // ResnetBlock tail: + Mish(GN(h2raw)) * mask  (diffusion.py:77-78)
+                    if (pre_on) {
 #pragma unroll
                         for (int i = 0; i < 32; i += 4) {
-                            if (C1 && p.act_out2) {
-                                const float sl = p.slope;
-                                *reinterpret_cast<float4*>(lp + (i / 4) * cstride) =
-                                    make_float4(v[i] > 0.f ? v[i] : v[i] * sl, v[i + 1] > 0.f ? v[i + 1] : v[i + 1] * sl,
-                                                v[i + 2] > 0.f ? v[i + 2] : v[i + 2] * sl, v[i + 3] > 0.f ? v[i + 3] : v[i + 3] * sl);
-                            } else {
-                                *reinterpret_cast<float4*>(lp + (i / 4) * cstride) = corr_chunk(v[i], v[i + 1], v[i + 2], v[i + 3]);
+                            const float rr[4] = {pre[i / 4].x, pre[i / 4].y, pre[i / 4].z, pre[i / 4].w};
+#pragma unroll
+                            for (int e = 0; e < 4; ++e) {
+                                const int cl = cb + i + e;
+                                const float xn = (rr[e] - s_rg[cl]) * s_rg[NT + cl] + s_rg[2 * NT + cl];
+                                v[i + e] += X3 ? mish_exact(xn) : mish_fast(xn);
+                            }
+                        }
+                        if (cb + 32 < cb_hi) {
+#pragma unroll
+                            for (int i = 0; i < 8; ++i)
+                                pre[i] = __ldg(reinterpret_cast<const float4*>(pre_src + obase + ((cb + 32) / 4 + i) * cstride));
+                        }
+                    }
+                } else if (p.addin && valid) {
+                    // fp32-exact residual (attention: x + g*P x): the tensor core only carries the small g*P x term
+                    if constexpr (OUT16) {
+                        const uint4* ap = reinterpret_cast<const uint4*>(p.addin) + ochunk + (long long)(cb / 8) * Wo;
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {
+                            const uint4 a = __ldg(ap + (long long)j * Wo);
+                            v[8 * j + 0] += bf16_lo(a.x); v[8 * j + 1] += bf16_hi(a.x); v[8 * j + 2] += bf16_lo(a.y); v[8 * j + 3] += bf16_hi(a.y);
+                            v[8 * j + 4] += bf16_lo(a.z); v[8 * j + 5] += bf16_hi(a.z); v[8 * j + 6] += bf16_lo(a.w); v[8 * j + 7] += bf16_hi(a.w);
+                        }
+                    } else {
+                        const float* ap = p.addin + obase + (cb / 4) * cstride;
+#pragma unroll
+                        for (int i = 0; i < 32; i += 4) {
+                            const float4 av = __ldg(reinterpret_cast<const float4*>(ap + (i / 4) * cstride));
+                            v[i] += av.x; v[i + 1] += av.y; v[i + 2] += av.z; v[i + 3] += av.w;
+                        }
+                    }
+                }
+                if (p.out_mask) {
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) v[i] *= mo;
+                }
+                if (C1 && p.act_out) {
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) v[i] = v[i] > 0.f ? v[i] : v[i] * p.slope;
+                }
+                if (valid) {
+                    if constexpr (OUT16) {
+                        uint4* op = reinterpret_cast<uint4*>(p.out) + ochunk + (long long)(cb / 8) * Wo;
+#pragma unroll
+                        for (int j = 0; j < 4; ++j)
+                            op[(long long)j * Wo] = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
+                                                               pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
+                    } else {
+                        float* op = p.out + obase + (cb / 4) * cstride;
+#pragma unroll
+                        for (int i = 0; i < 32; i += 4) *reinterpret_cast<float4*>(op + (i / 4) * cstride) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
+                        if (GEOM != G_C3 && p.out_lo) {
+                            float* lp = p.out_lo + obase + (cb / 4) * cstride;
+#pragma unroll
+                            for (int i = 0; i < 32; i += 4) {
+                                if (C1 && p.act_out2) {
+                                    const float sl = p.slope;
+                                    *reinterpret_cast<float4*>(lp + (i / 4) * cstride) =
+                                        make_float4(v[i] > 0.f ? v[i] : v[i] * sl, v[i + 1] > 0.f ? v[i + 1] : v[i + 1] * sl,
+                                                    v[i + 2] > 0.f ? v[i + 2] : v[i + 2] * sl, v[i + 3] > 0.f ? v[i + 3] : v[i + 3] * sl);
+                                } else {
+                                    *reinterpret_cast<float4*>(lp + (i / 4) * cstride) = corr_chunk(v[i], v[i + 1], v[i + 2], v[i + 3]);
+                                }
+                            }
+                        }
+                    }
+                }
+                if (!SIDE && p.ostats) {
+                    // GroupNorm partials of this 32-column chunk: 8-channel sub-sums first (static register indexing),
+                    // then merged to the group width cpg (8 -> 4 groups, 16 -> 2 groups, >= 32 -> 1 group)
+                    float s8[4], q8[4];
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        float s = 0.f, q = 0.f;
+#pragma unroll
+                        for (int i = 0; i < 8; ++i) { const float x = valid ? v[8 * k + i] : 0.f; s += x; q = fmaf(x, x, q); }
+                        s8[k] = s; q8[k] = q;
+                    }
+                    const int ngrp = cpg == 8 ? 4 : (cpg == 16 ? 2 : 1);
+                    if (ngrp == 2) { s8[0] += s8[1]; q8[0] += q8[1]; s8[1] = s8[2] + s8[3]; q8[1] = q8[2] + q8[3]; }
+                    if (ngrp == 1) { s8[0] += s8[1] + s8[2] + s8[3]; q8[0] += q8[1] + q8[2] + q8[3]; }
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        if (k < ngrp) {
+                            float s = s8[k], q = q8[k];
+#pragma unroll
+                            for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); q += __shfl_xor_sync(0xffffffffu, q, o); }
+                            if (lane == 0) {
+                                const int gl = (n0 + cb + k * (32 / ngrp)) / cpg - n0 / cpg;
+                                s_st[(warp * 8 + gl) * 2] += s;
+                                s_st[(warp * 8 + gl) * 2 + 1] += q;
                             }
                         }
                     }
                 }
             }
-            if (!SIDE && p.ostats) {
-                // GroupNorm partials of this 32-column chunk: 8-channel sub-sums first (static register indexing),
-                // then merged to the group width cpg (8 -> 4 groups, 16 -> 2 groups, >= 32 -> 1 group)
-                float s8[4], q8[4];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    float s = 0.f, q = 0.f;
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) { const float x = valid ? v[8 * k + i] : 0.f; s += x; q = fmaf(x, x, q); }
-                    s8[k] = s; q8[k] = q;
-                }
-                const int ngrp = cpg == 8 ? 4 : (cpg == 16 ? 2 : 1);
-                if (ngrp == 2) { s8[0] += s8[1]; q8[0] += q8[1]; s8[1] = s8[2] + s8[3]; q8[1] = q8[2] + q8[3]; }
-                if (ngrp == 1) { s8[0] += s8[1] + s8[2] + s8[3]; q8[0] += q8[1] + q8[2] + q8[3]; }
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    if (k < ngrp) {
-                        float s = s8[k], q = q8[k];
-#pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); q += __shfl_xor_sync(0xffffffffu, q, o); }
-                        if (lane == 0) {
-                            const int gl = (n0 + cb + k * (32 / ngrp)) / cpg - n0 / cpg;
-                            s_st[(warp * 8 + gl) * 2] += s;
-                            s_st[(warp * 8 + gl) * 2 + 1] += q;
-                        }
-                    }
-                }
-            }
-        }
-        }
-        }
-            // accumulator slot drained: hand it back to the MMA issuer (CHUNKED: every run was handed back as it was drained)
-            if constexpr (!CHUNKED && !TMSUM) {
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) tempty_arrive(slot);
-                ++ar;
             }
             if (GEOM != G_PW && p.ostats) {
                 asm volatile("bar.sync 1, 256;" ::: "memory");
-                const int cpg = p.Cout / kGroups, gb = n0 / cpg, ng = (NT + cpg - 1) / cpg;
+                const int gb = n0 / cpg, ng = (NT + cpg - 1) / cpg;
                 if (tid < ng * 2) {
                     double tot = 0.0;
 #pragma unroll
-                    for (int w8 = 0; w8 < NPROD / 32; ++w8) { tot += (double)s_st[w8 * 16 + tid]; s_st[w8 * 16 + tid] = 0.f; }
+                    for (int w8 = 0; w8 < NCONS / 32; ++w8) { tot += (double)s_st[w8 * 16 + tid]; s_st[w8 * 16 + tid] = 0.f; }
                     atomicAdd(&p.ostats[((long long)b * kGroups + gb + (tid >> 1)) * 2 + (tid & 1)], tot);
                 }
                 asm volatile("bar.sync 1, 256;" ::: "memory");
-            }
-        }
-    } else if (warp == NPROD / 32) {
-        // =========================================================================================================
-        // MMA issuer: the whole warp runs the loops and the barrier waits; one elected lane issues (see elect_one)
-        // =========================================================================================================
-        if (PAIR && rank != 0) {
-            // peer CTA of a pair: no MMAs to issue - relay "stage s of MY ring is full" to the leader's full barrier, in ring order
-            const uint32_t lead_full0 = lead_bar0;                       // full_b(s) = bar0 + 8 s
-            uint32_t it = 0;
-            for (int t = tile0; t < total_tiles; t += tstep)
-                for (int ks = 0; ks < ksteps_t; ++ks, ++it) {
-                    const int s = it % STAGES;
-                    mbar_wait(full_b(s), (it / STAGES) & 1);
-                    if (lane == 0) mbar_arrive_cluster(lead_full0 + 8u * s);
-                    __syncwarp();
-                }
-        } else {
-            const uint32_t idesc = make_idesc<BF16>(PAIR ? 2 * TPX : TPX, NT);
-            const uint32_t idesc_c = make_idesc_fmt(0u, PAIR ? 2 * TPX : TPX, NT);   // fp32x3 correction sub-stages: fp16 operands
-            const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
-            constexpr uint32_t D_HI = desc_hi(128);                      // SBO = 128 B for both operands
-            auto mma = [&](auto kind16, uint32_t d, uint64_t ad, uint64_t bd, uint32_t idk, uint32_t acc) {
-                if constexpr (PAIR) umma2<decltype(kind16)::value>(d, ad, bd, idk, acc);
-                else umma<decltype(kind16)::value>(d, ad, bd, idk, acc);
-            };
-            auto commit = [&](uint32_t bar) { if constexpr (PAIR) umma_commit2(bar); else umma_commit(bar); };
-            auto wait_full = [&](uint32_t bar, uint32_t ph) { if constexpr (PAIR) mbar_wait_cluster(bar, ph); else mbar_wait(bar, ph); };
-            // RS: the 12 MMAs of one (sub-)stage into the two adjacent row accumulators at tbase / tbase + NT; `first` = this stage
-            // starts an accumulation run.  Weight stage image: [column tap sx][chunk][kr=2 | kr=1 | kr=0][NT rows][16 B].
-            auto issue_rs = [&](auto kind16, const uint32_t id64, const uint32_t id128, const uint32_t tbase, const uint32_t a_st, const uint32_t b_st, const bool first) {
-                constexpr uint32_t BL = 3 * NT;                                 // weight rows per (sx, chunk)
-#pragma unroll
-                for (int sx = 0; sx < 3; ++sx) {
-                    const uint32_t bs = b_st + (uint32_t)(sx * KCH) * BL;       // (KCH = 2: one K step of two chunks per stage)
-                    const uint32_t acc0 = (first && sx == 0) ? 0u : 1u;
-                    // halo row 0 (input h0-1) -> output row 0 through kernel row 0;  halo row 3 (input h0+2) -> output row 1 through kr 2
-                    mma(kind16, tbase, desc_pack(a_st + (uint32_t)(0 * PXP + sx), D_HI), desc_pack(bs + 2 * NT, D_HI), id64, acc0);
-                    mma(kind16, tbase + NT, desc_pack(a_st + (uint32_t)(3 * PXP + sx), D_HI), desc_pack(bs, D_HI), id64, acc0);
-                    // halo row 1 (input h0): [W1 | W0] -> rows 0, 1;  halo row 2 (input h0+1): [W2 | W1] -> rows 0, 1
-                    mma(kind16, tbase, desc_pack(a_st + (uint32_t)(1 * PXP + sx), D_HI), desc_pack(bs + NT, D_HI), id128, 1u);
-                    mma(kind16, tbase, desc_pack(a_st + (uint32_t)(2 * PXP + sx), D_HI), desc_pack(bs, D_HI), id128, 1u);
-                }
-            };
-            const uint32_t idesc_w = make_idesc<BF16>(TPX, 2 * NT), idesc_cw = make_idesc_fmt(0u, TPX, 2 * NT);   // RS: the N = 128 instructions
-            uint32_t it = 0;
-            uint32_t ar = 0;                                             // accumulation-run counter (see the epilogue warps)
-            if constexpr (TMSUM) {
-                // Both rows advance together through the sub-stages of a run - row 0's taps, then row 1's, on every stage - so a
-                // stage is released as soon as both rows have read it (18 MMAs), and each row's run is committed separately:
-                // row 0's fold into the running sums overlaps row 1's last stage, row 1's fold overlaps row 0's first stage
-                // of the next run (whose MMAs only wait for row 0's fold).  (The first version walked a run row by row over
-                // RESIDENT stages so that one row's fold hid under the other row's whole run; holding 3 of the 4 stages for
-                // two passes left the ring one stage of prefetch, and the activation loads - ~2 us from HBM - were exposed:
-                // 39 % of the conv time, profiles/r2_experiments.md, 4-5.)
-                for (int t = tile0; t < total_tiles; t += tstep) {
-                    for (int c = 0; c < nchunks; ++c, ++ar) {
-                        const int ks_lo = c * FLUSH, ks_hi = ks_lo + FLUSH < ksteps_t ? ks_lo + FLUSH : ksteps_t;
-                        for (int ks = ks_lo; ks < ks_hi; ++ks, ++it) {
-                            const int s = it % STAGES;
-                            wait_full(full_b(s), (it / STAGES) & 1);
-                            tc_fence_after();
-                            if constexpr (RS) {
-                                if (ks == ks_lo) {                              // both rows' previous runs folded (every MMA may touch both)
-                                    wait_full(tempty(0), (ar & 1) ^ 1);
-                                    wait_full(tempty(1), (ar & 1) ^ 1);
-                                    tc_fence_after();
-                                }
-                                const uint32_t a_st = desc_lo(a0 + s * A_STAGE_BYTES, PLANE), b_st = desc_lo(b0 + s * B_STAGE_BYTES, 3 * NT * 16);
-                                if (elect_one()) {
-                                    if ((ks & 1) == 0) issue_rs(std::true_type{}, idesc_c, idesc_cw, tmem_base, a_st, b_st, ks == ks_lo);
-                                    else issue_rs(std::false_type{}, idesc, idesc_w, tmem_base, a_st, b_st, ks == ks_lo);
-                                    commit(empty(s));
-                                    if (ks == ks_hi - 1) { commit(tfull(0)); commit(tfull(1)); }
-                                }
-                                __syncwarp();
-                                continue;
-                            }
-                            const uint32_t b_lo = desc_lo(b0 + s * B_STAGE_BYTES, NB * 16);
-#pragma unroll
-                            for (int j = 0; j < ROWS; ++j) {
-                                if (ks == ks_lo) {
-                                    wait_full(tempty(j), (ar & 1) ^ 1);     // this row's previous run has been folded into the sums
-                                    tc_fence_after();
-                                }
-                                const uint32_t tslot = tmem_base + j * NT;
-                                const uint32_t a_lo = desc_lo(a0 + s * A_STAGE_BYTES + (j * PXP) * 16, PLANE);
-                                if (elect_one()) {
-                                    auto issue = [&](auto kind16, const uint32_t idk) {
-#pragma unroll
-                                        for (int kk = 0; kk < KCH / 2; ++kk) {
-#pragma unroll
-                                            for (int tap = 0; tap < TAPS; ++tap) {
-                                                const int r = TAPS == 9 ? tap / 3 : 0, sx = TAPS == 9 ? tap % 3 : 0;
-                                                mma(kind16, tslot, desc_pack(a_lo + (uint32_t)(kk * 2 * (PLANE / 16) + r * PXP + sx), D_HI),
-                                                    desc_pack(b_lo + (uint32_t)((kk * 2 + tap * KCH) * NB), D_HI), idk,
-                                                    ((ks - ks_lo) | kk | tap) != 0 ? 1u : 0u);
-                                            }
-                                        }
-                                    };
-                                    if ((ks & 1) == 0) issue(std::true_type{}, idesc_c);      // correction sub-stage: kind::f16 on the fp16 chunks
-                                    else issue(std::false_type{}, idesc);                     // main sub-stage: kind::tf32
-                                    if (j == ROWS - 1) commit(empty(s));        // frees the stage: both rows have read it
-                                    if (ks == ks_hi - 1) commit(tfull(j));      // this row's run is complete
-                                }
-                                __syncwarp();
-                            }
-                        }
-                    }
-                }
-            } else
-            for (int t = tile0; t < total_tiles; t += tstep) {
-              for (int c = 0; c < nchunks; ++c, ++ar) {
-                const int slot = ar % NSLOT;
-                const uint32_t tslot = tmem_base + slot * SLOT_COLS;
-                wait_full(tempty(slot), ((ar / NSLOT) & 1) ^ 1);        // epilogue has drained this slot
-                tc_fence_after();
-                const int ks_lo = CHUNKED ? c * FLUSH : 0, ks_hi = CHUNKED ? (ks_lo + FLUSH < ksteps_t ? ks_lo + FLUSH : ksteps_t) : ksteps_t;
-                for (int ks = ks_lo; ks < ks_hi; ++ks, ++it) {
-                    const int s = it % STAGES;
-                    const uint32_t ph = (it / STAGES) & 1;
-                    if (!BULK) mbar_wait(full_a(s), ph);
-                    wait_full(full_b(s), ph);               // weights (+ the A runs when they are bulk copies)
-                    tc_fence_after();
-                    if constexpr (RS) {
-                        const uint32_t a_st = desc_lo(a0 + s * A_STAGE_BYTES, PLANE), b_st = desc_lo(b0 + s * B_STAGE_BYTES, 3 * NT * 16);
-                        if (elect_one()) {
-                            issue_rs(std::integral_constant<bool, BF16>{}, idesc, idesc_w, tslot, a_st, b_st, ks == ks_lo);
-                            commit(empty(s));
-                            if (ks == ks_hi - 1) commit(tfull(slot));
-                        }
-                        __syncwarp();
-                        continue;
-                    }
-                    const uint32_t a_lo = desc_lo(a0 + s * A_STAGE_BYTES, PLANE);
-                    const uint32_t b_lo = desc_lo(b0 + s * B_STAGE_BYTES, NB * 16);
-                    const uint32_t dil = C1 ? (uint32_t)p.dil : 0u;
-                    if (elect_one()) {
-                      auto issue = [&](auto kind16, const uint32_t idk) {
-#pragma unroll
-                        for (int kk = 0; kk < KCH / 2; ++kk) {
-                            const uint32_t a_k = a_lo + (uint32_t)(kk * 2 * (PLANE / 16)), b_k = b_lo + (uint32_t)(kk * 2 * NB);
-                            if (GEOM == G_UP) {
-                                // ho = 2*hi - 1 + kh: parity ph uses (kh=1,dh=0),(kh=3,dh=-1) if ph=0 and (kh=0,dh=+1),(kh=2,dh=0) if ph=1
-#pragma unroll
-                                for (int phase = 0; phase < 4; ++phase) {
-                                    const int pph = phase >> 1, pw = phase & 1;
-#pragma unroll
-                                    for (int t2 = 0; t2 < 4; ++t2) {
-                                        const int a = t2 >> 1, bb = t2 & 1;
-                                        const int kh = pph ? (a ? 2 : 0) : (a ? 3 : 1), kw = pw ? (bb ? 2 : 0) : (bb ? 3 : 1);
-                                        const int dh = pph ? (a ? 0 : 1) : (a ? -1 : 0), dw = pw ? (bb ? 0 : 1) : (bb ? -1 : 0);
-                                        const uint64_t bd = desc_pack(b_k + (uint32_t)((kh * 4 + kw) * KCH * NB), D_HI);
-#pragma unroll
-                                        for (int j = 0; j < ROWS; ++j)
-                                            mma(kind16, tslot + (phase * ROWS + j) * NT, desc_pack(a_k + (uint32_t)((1 + j + dh) * PXP + 1 + dw), D_HI), bd,
-                                                idk, ((ks - ks_lo) | kk | t2) != 0 ? 1u : 0u);
-                                    }
-                                }
-                            } else {
-#pragma unroll
-                                for (int tap = 0; tap < TAPS; ++tap) {
-                                    const int r = TAPS == 9 ? tap / 3 : 0, sx = TAPS == 9 ? tap % 3 : 0;
-                                    const uint64_t bd = desc_pack(b_k + (uint32_t)(tap * KCH * NB), D_HI);
-#pragma unroll
-                                    for (int j = 0; j < ROWS; ++j) {
-                                        // DOWN: input row 2j+r; column tap s reads the odd plane at x (s=0) / x+1 (s=2), the even plane at x (s=1)
-                                        const uint32_t aoff = GEOM == G_DOWN ? (uint32_t)((2 * j + r) * PXP + (sx == 1 ? TPX + 1 : (sx == 2 ? 1 : 0)))
-                                                            : C1 ? (uint32_t)(j * TPX) + (uint32_t)tap * dil
-                                                                 : (uint32_t)((r + j) * PXP + sx);
-                                        mma(kind16, tslot + j * NT, desc_pack(a_k + aoff, D_HI), bd, idk, ((ks - ks_lo) | kk | tap) != 0 ? 1u : 0u);
-                                    }
-                                }
-                            }
-                        }
-                      };
-                        if (X3 && (ks & 1) == 0) issue(std::true_type{}, idesc_c);          // fp32x3 correction sub-stage: kind::f16
-                        else issue(std::integral_constant<bool, BF16>{}, idesc);
-                        commit(empty(s));                       // frees the stage when these MMAs have read it
-                        if (ks == ks_hi - 1) commit(tfull(slot));        // this run's accumulators are complete
-                    }
-                    __syncwarp();
-                }
-              }
             }
         }
     } else {
@@ -756,458 +499,132 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
         // out-of-image rows / columns (the conv's zero padding, the ragged last 1x1 tile) come from a zero page.
         // =========================================================================================================
         // Lane 0 owns the ring protocol, the border bookkeeping and the weight copy; the (chunk, row) activation runs of a
-        // stage are issued by KCH*HR lanes in parallel (one thread issuing ~10-20 copies + address math per stage was
-        // a measurable part of the pipeline latency).
-        {
-            uint32_t it = 0;
-            const float* zero = p.zero_page;
-            uint32_t stage_pat[STAGES];
+        // stage are issued by KCH*HR lanes in parallel.
+        uint32_t it = 0;
+        const float* zero = p.zero_page;
+        uint32_t stage_pat[STAGES];
 #pragma unroll
-            for (int i = 0; i < STAGES; ++i) stage_pat[i] = 0xFFFFFFFFu;
-            for (int t = tile0; t < total_tiles; t += tstep) {
-                int b, h0, w0, n0, mt;
-                decode(t, b, h0, w0, n0, mt);
-                // weight image: [ntile][kstage][tap][chunk][NT][16 B]; fp32x3: [ntile][kstage][hi|correction][tap][chunk][NT][16 B]
-                // (PAIR: the image is packed for NT/2-wide tiles; this CTA stages half `rank` of the N tile)
-                const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.wpk) + (size_t)b * p.w_bstride_bytes +
-                                      (size_t)(PAIR ? 2 * (n0 / NT) + (int)rank : n0 / NT) * ksteps * (X3 ? 2 : 1) * B_STAGE_BYTES;
-                for (int ks = 0; ks < ksteps_t; ++ks, ++it) {
-                    const int s = it % STAGES;
-                    const int kb = X3 ? ks / 2 : ks, var = X3 ? (ks & 1) : 1;          // 0: correction (fp16 chunks), 1: main (x, w_hi)
-                    if (lane == 0) {
-                        mbar_wait(empty(s), ((it / STAGES) & 1) ^ 1);
-                        uint32_t a_tx = BULK ? A_STAGE_BYTES : 0;
-                        if (BULK && GEOM != G_PW) {
-                            // Image-border columns (the conv's zero padding) are never written by the row copies, so they only
-                            // need zeroing when this stage buffer last served a tile with a different border pattern.  With
-                            // the round-robin tile order a CTA normally keeps one pattern, so this (and its proxy fence,
-                            // which would otherwise serialise against the bulk copies in flight) runs a handful of times.
-                            const int pad = C1 ? p.pad : 1;             // Conv1d: (K-1)*dil/2 samples of halo on each side
-                            const int wlo = w0 - pad < 0 ? 0 : w0 - pad, whi = w0 + SPAN + pad > p.W ? p.W : w0 + SPAN + pad;
-                            const int qlo = wlo - (w0 - pad), qhi = qlo + (whi - wlo);
-                            const uint32_t pat = (uint32_t)qlo | ((uint32_t)qhi << 16);
-                            if (stage_pat[s] != pat) {
-                                stage_pat[s] = pat;
-                                if (qlo > 0 || qhi < PXP) {
-                                    uint8_t* st = sA + s * A_STAGE_BYTES;
-                                    for (int k = 0; k < KCH; ++k)
-                                        for (int r = 0; r < HR; ++r) {
-                                            uint4* rowp = reinterpret_cast<uint4*>(st + k * PLANE + (r * PXP) * 16);
-                                            for (int q = 0; q < qlo; ++q) rowp[q] = make_uint4(0u, 0u, 0u, 0u);
-                                            for (int q = qhi; q < PXP; ++q) rowp[q] = make_uint4(0u, 0u, 0u, 0u);
-                                        }
-                                    fence_proxy_async();
-                                }
+        for (int i = 0; i < STAGES; ++i) stage_pat[i] = 0xFFFFFFFFu;
+        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+            int b, h0, w0, n0;
+            decode(t, b, h0, w0, n0);
+            // weight image: [ntile][kstage][tap][chunk][NT][16 B]; fp32x3: [ntile][kstage][hi|correction][tap][chunk][NT][16 B]
+            const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.wpk) + (size_t)b * p.w_bstride_bytes +
+                                  (size_t)(n0 / NT) * ksteps * (X3 ? 2 : 1) * B_STAGE_BYTES;
+            for (int ks = 0; ks < ksteps_t; ++ks, ++it) {
+                const int s = it % STAGES;
+                const int kb = X3 ? ks / 2 : ks, var = X3 ? (ks & 1) : 1;          // 0: correction (fp16 chunks), 1: main (x, w_hi)
+                if (lane == 0) {
+                    mbar_wait(empty(s), ((it / STAGES) & 1) ^ 1);
+                    uint32_t a_tx = BULK ? A_STAGE_BYTES : 0;
+                    if (BULK && GEOM != G_PW) {
+                        // Image-border columns (the conv's zero padding) are never written by the row copies, so they only
+                        // need zeroing when this stage buffer last served a tile with a different border pattern.  With
+                        // the round-robin tile order a CTA normally keeps one pattern, so this (and its proxy fence,
+                        // which would otherwise serialise against the bulk copies in flight) runs a handful of times.
+                        const int pad = C1 ? p.pad : 1;             // Conv1d: (K-1)*dil/2 samples of halo on each side
+                        const int wlo = w0 - pad < 0 ? 0 : w0 - pad, whi = w0 + SPAN + pad > p.W ? p.W : w0 + SPAN + pad;
+                        const int qlo = wlo - (w0 - pad), qhi = qlo + (whi - wlo);
+                        const uint32_t pat = (uint32_t)qlo | ((uint32_t)qhi << 16);
+                        if (stage_pat[s] != pat) {
+                            stage_pat[s] = pat;
+                            if (qlo > 0 || qhi < PXP) {
+                                uint8_t* st = sA + s * A_STAGE_BYTES;
+                                for (int k = 0; k < KCH; ++k)
+                                    for (int r = 0; r < HR; ++r) {
+                                        uint4* rowp = reinterpret_cast<uint4*>(st + k * PLANE + (r * PXP) * 16);
+                                        for (int q = 0; q < qlo; ++q) rowp[q] = make_uint4(0u, 0u, 0u, 0u);
+                                        for (int q = qhi; q < PXP; ++q) rowp[q] = make_uint4(0u, 0u, 0u, 0u);
+                                    }
+                                fence_proxy_async();
                             }
-                            int vrows = 0;
-                            for (int r = 0; r < HR; ++r) { const int hi = C1 ? 0 : h0 - 1 + r; vrows += (hi >= 0 && hi < p.H) ? 1 : 0; }
-                            a_tx -= (uint32_t)(KCH * vrows * (PXP - (qhi - qlo))) * 16u;
                         }
-                        mbar_arrive_expect_tx(full_b(s), B_STAGE_BYTES + a_tx);
-                        bulk_g2s(smem_u32(sB + s * B_STAGE_BYTES), wsrc + (size_t)(X3 ? 2 * kb + (var == 0) : ks) * B_STAGE_BYTES,
-                                 B_STAGE_BYTES, full_b(s));
+                        int vrows = 0;
+                        for (int r = 0; r < HR; ++r) { const int hi = C1 ? 0 : h0 - 1 + r; vrows += (hi >= 0 && hi < p.H) ? 1 : 0; }
+                        a_tx -= (uint32_t)(KCH * vrows * (PXP - (qhi - qlo))) * 16u;
                     }
-                    __syncwarp();
-                    if (BULK && lane < KCH * HR) {
-                        const uint32_t a_s = smem_u32(sA) + s * A_STAGE_BYTES;
-                        const int k = lane / HR, r = lane - k * HR;
-                        const int ck = kb * KCH + k;                     // 16-byte channel chunk index over the concat
-                        const bool second = ck * EPC >= p.c0;
-                        const uint8_t* src = reinterpret_cast<const uint8_t*>(var == 0 ? (second ? p.in1_lo : p.in0_lo) : (second ? p.in1 : p.in0));
-                        const int chs = (second ? p.c1 : p.c0) / EPC;
-                        const int cl = second ? ck - p.c0 / EPC : ck;
-                        if (GEOM == G_PW) {
-                            long long m = (long long)(h0 + r) * TPX;
-                            const long long m_hi = m >= HW ? m : (m + TPX < HW ? m + TPX : HW);
-                            int q = 0;
-                            if (m < m_hi) {
-                                int hh = (int)(m / p.W), ww = (int)(m - (long long)hh * p.W);
-                                while (m < m_hi) {                     // split the flattened run at image-row boundaries
-                                    const int n = (int)((p.W - ww) < (m_hi - m) ? (p.W - ww) : (m_hi - m));
-                                    bulk_g2s(a_s + k * PLANE + (r * PXP + q) * 16,
-                                             src + (((long long)(b * p.H + hh) * chs + cl) * p.W + ww) * 16, (uint32_t)n * 16u, full_b(s));
-                                    m += n; q += n; ++hh; ww = 0;
-                                }
+                    mbar_arrive_expect_tx(full_b(s), B_STAGE_BYTES + a_tx);
+                    bulk_g2s(smem_u32(sB + s * B_STAGE_BYTES), wsrc + (size_t)(X3 ? 2 * kb + (var == 0) : ks) * B_STAGE_BYTES,
+                             B_STAGE_BYTES, full_b(s));
+                }
+                __syncwarp();
+                if (BULK && lane < KCH * HR) {
+                    const uint32_t a_s = smem_u32(sA) + s * A_STAGE_BYTES;
+                    const int k = lane / HR, r = lane - k * HR;
+                    const int ck = kb * KCH + k;                     // 16-byte channel chunk index over the concat
+                    const bool second = ck * EPC >= p.c0;
+                    const uint8_t* src = reinterpret_cast<const uint8_t*>(var == 0 ? (second ? p.in1_lo : p.in0_lo) : (second ? p.in1 : p.in0));
+                    const int chs = (second ? p.c1 : p.c0) / EPC;
+                    const int cl = second ? ck - p.c0 / EPC : ck;
+                    if (GEOM == G_PW) {
+                        long long m = (long long)(h0 + r) * TPX;
+                        const long long m_hi = m >= HW ? m : (m + TPX < HW ? m + TPX : HW);
+                        int q = 0;
+                        if (m < m_hi) {
+                            int hh = (int)(m / p.W), ww = (int)(m - (long long)hh * p.W);
+                            while (m < m_hi) {                     // split the flattened run at image-row boundaries
+                                const int n = (int)((p.W - ww) < (m_hi - m) ? (p.W - ww) : (m_hi - m));
+                                bulk_g2s(a_s + k * PLANE + (r * PXP + q) * 16,
+                                         src + (((long long)(b * p.H + hh) * chs + cl) * p.W + ww) * 16, (uint32_t)n * 16u, full_b(s));
+                                m += n; q += n; ++hh; ww = 0;
                             }
-                            if (q < PXP) bulk_g2s(a_s + k * PLANE + (r * PXP + q) * 16, zero, (uint32_t)(PXP - q) * 16u, full_b(s));
-                        } else {
-                            const int pad = C1 ? p.pad : 1;
-                            const int wlo = w0 - pad < 0 ? 0 : w0 - pad, whi = w0 + SPAN + pad > p.W ? p.W : w0 + SPAN + pad;
-                            const int qlo = wlo - (w0 - pad);
-                            const int hi = C1 ? 0 : h0 - 1 + r;
-                            const uint32_t row_s = a_s + k * PLANE + (r * PXP) * 16;
-                            if (hi < 0 || hi >= p.H) bulk_g2s(row_s, zero, PXP * 16u, full_b(s));
-                            else bulk_g2s(row_s + qlo * 16, src + (((long long)(b * p.H + hi) * chs + cl) * p.W + wlo) * 16,
-                                          (uint32_t)(whi - wlo) * 16u, full_b(s));
                         }
+                        if (q < PXP) bulk_g2s(a_s + k * PLANE + (r * PXP + q) * 16, zero, (uint32_t)(PXP - q) * 16u, full_b(s));
+                    } else {
+                        const int pad = C1 ? p.pad : 1;
+                        const int wlo = w0 - pad < 0 ? 0 : w0 - pad, whi = w0 + SPAN + pad > p.W ? p.W : w0 + SPAN + pad;
+                        const int qlo = wlo - (w0 - pad);
+                        const int hi = C1 ? 0 : h0 - 1 + r;
+                        const uint32_t row_s = a_s + k * PLANE + (r * PXP) * 16;
+                        if (hi < 0 || hi >= p.H) bulk_g2s(row_s, zero, PXP * 16u, full_b(s));
+                        else bulk_g2s(row_s + qlo * 16, src + (((long long)(b * p.H + hi) * chs + cl) * p.W + wlo) * 16,
+                                      (uint32_t)(whi - wlo) * 16u, full_b(s));
                     }
                 }
             }
         }
-    }
-
-    if constexpr (PAIR) cluster_sync_all(); else __syncthreads();    // (pair: neither CTA may exit or free TMEM while the other still uses it)
-    if (warp == NPROD / 32) {
-        tc_fence_after();
-        if constexpr (PAIR) tmem_dealloc2(tmem_base, D::TMEM_COLS); else tmem_dealloc(tmem_base, D::TMEM_COLS);
     }
 }
 
 template <int GEOM, bool BF16, int NT, bool RES = false>
-__global__ void __launch_bounds__(NTHREADS, Depth<GEOM, NT, false>::MINB) k_conv_tc(const ConvTcParams p) {
+__global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc(const ConvTcParams p) {
     conv_tc_body<GEOM, BF16, NT, RES, false>(p);
 }
-// fp32x3 instantiations.  (Warps are allocated four at a time, so a 10-warp CTA is sized as 384 threads: the ceiling is
-// 65536 / 384 = 168 registers per thread at one CTA per SM - a __maxnreg__(200) build fails to launch with "too many
-// resources requested".  That is why the running sums of the 3x3 / 1x1 convs live in TMEM, not in registers.)
 template <int GEOM, int NT, bool RES = false>
-__global__ void __launch_bounds__(NTHREADS, Depth<GEOM, NT, true>::MINB) k_conv_tc_x3(const ConvTcParams p) {
+__global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc_x3(const ConvTcParams p) {
     conv_tc_body<GEOM, false, NT, RES, true>(p);
 }
-// row-shared issue order (64-channel 3x3 convs, single CTAs)
-template <bool BF16>
-__global__ void __launch_bounds__(NTHREADS, Depth<G_C3, 64, false>::MINB) k_conv_tc_rs(const ConvTcParams p) {
-    conv_tc_body<G_C3, BF16, 64, false, false, false, true>(p);
-}
-__global__ void __launch_bounds__(NTHREADS, Depth<G_C3, 64, true>::MINB) k_conv_tc_x3_rs(const ConvTcParams p) {
-    conv_tc_body<G_C3, false, 64, false, true, false, true>(p);
-}
-// CTA-pair instantiations (3x3 convs; launched as 2-CTA clusters)
-template <bool BF16, int NT>
-__global__ void __launch_bounds__(NTHREADS, Depth<G_C3, NT, false, true>::MINB) k_conv_tc_pair(const ConvTcParams p) {
-    conv_tc_body<G_C3, BF16, NT, false, false, true>(p);
-}
-template <int NT>
-__global__ void __launch_bounds__(NTHREADS, Depth<G_C3, NT, true, true>::MINB) k_conv_tc_x3_pair(const ConvTcParams p) {
-    conv_tc_body<G_C3, false, NT, false, true, true>(p);
-}
 
-template <int GEOM, bool BF16, int NT, bool RES = false, bool X3 = false, bool RS = false>
+template <int GEOM, bool BF16, int NT, bool RES = false, bool X3 = false>
 static int launch_tc(const ConvTcParams& p, cudaStream_t s) {
-    using D = Depth<GEOM, NT, X3>;
+    using D = Depth<GEOM, NT>;
     // the dynamic-shared-memory opt-in is a per-device function attribute and the persistent grid is sized from the
     // current device's SM count: both are cached per device ordinal (a process may drive several GPUs through several handles)
     static DevCache cache;
     const void* fn;
-    if constexpr (RS && X3) fn = reinterpret_cast<const void*>(k_conv_tc_x3_rs);
-    else if constexpr (RS) fn = reinterpret_cast<const void*>(k_conv_tc_rs<BF16>);
-    else if constexpr (X3) fn = reinterpret_cast<const void*>(k_conv_tc_x3<GEOM, NT, RES>);
+    if constexpr (X3) fn = reinterpret_cast<const void*>(k_conv_tc_x3<GEOM, NT, RES>);
     else fn = reinterpret_cast<const void*>(k_conv_tc<GEOM, BF16, NT, RES>);
     const int num_sms = cache.get(fn);
     if (num_sms <= 0) return -1;
     int mt;
-    if (geom_is_c1(GEOM)) mt = (p.W + ROWS * TPX - 1) / (ROWS * TPX);
-    else if (GEOM == G_C3 || GEOM == G_UP) mt = ((p.W + TPX - 1) / TPX) * ((p.H + ROWS - 1) / ROWS);
-    else if (GEOM == G_DOWN) mt = ((p.Wo + TPX - 1) / TPX) * ((p.Ho + ROWS - 1) / ROWS);
-    else mt = (p.H * p.W + ROWS * TPX - 1) / (ROWS * TPX);
+    if (geom_is_c1(GEOM)) mt = (p.W + TPX - 1) / TPX;
+    else if (GEOM == G_C3 || GEOM == G_UP) mt = ((p.W + TPX - 1) / TPX) * p.H;
+    else if (GEOM == G_DOWN) mt = ((p.Wo + TPX - 1) / TPX) * p.Ho;
+    else mt = (p.H * p.W + TPX - 1) / TPX;
     const long long total = (long long)mt * (p.Cout / NT) * p.B;
-    const long long cap = (long long)num_sms * D::MINB;             // persistent: one wave of resident CTAs
-    const int grid = (int)(total < cap ? total : cap);
-    if constexpr (RS && X3) k_conv_tc_x3_rs<<<grid, NTHREADS, D::SMEM, s>>>(p);
-    else if constexpr (RS) k_conv_tc_rs<BF16><<<grid, NTHREADS, D::SMEM, s>>>(p);
-    else if constexpr (X3) k_conv_tc_x3<GEOM, NT, RES><<<grid, NTHREADS, D::SMEM, s>>>(p);
+    const int grid = (int)(total < num_sms ? total : num_sms);       // persistent: one wave of resident CTAs
+    if constexpr (X3) k_conv_tc_x3<GEOM, NT, RES><<<grid, NTHREADS, D::SMEM, s>>>(p);
     else k_conv_tc<GEOM, BF16, NT, RES><<<grid, NTHREADS, D::SMEM, s>>>(p);
     return 1;
 }
 
-// 3x3 conv on CTA pairs: persistent grid of 2-CTA clusters, one pair tile = 4 rows x 128 pixels x NT channels
-template <bool BF16, int NT, bool X3>
-static int launch_tc_pair(const ConvTcParams& p, cudaStream_t s) {
-    using D = Depth<G_C3, NT, X3, true>;
-    static DevCache cache;
-    const void* fn;
-    if constexpr (X3) fn = reinterpret_cast<const void*>(k_conv_tc_x3_pair<NT>);
-    else fn = reinterpret_cast<const void*>(k_conv_tc_pair<BF16, NT>);
-    const int num_sms = cache.get(fn);
-    if (num_sms <= 0) return -1;
-    const long long total = (long long)conv_tc_pair_tiles(p.H, p.W) * (p.Cout / NT) * p.B;
-    const long long cap = (long long)(num_sms / 2) * D::MINB;       // clusters resident at once
-    const unsigned clusters = (unsigned)(total < cap ? total : cap);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * clusters, 1, 1); cfg.blockDim = dim3(NTHREADS, 1, 1); cfg.dynamicSmemBytes = D::SMEM; cfg.stream = s;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    cudaError_t e;
-    if constexpr (X3) e = cudaLaunchKernelEx(&cfg, k_conv_tc_x3_pair<NT>, p);
-    else e = cudaLaunchKernelEx(&cfg, k_conv_tc_pair<BF16, NT>, p);
-    return e == cudaSuccess ? 1 : -1;
-}
-
-// =================================================================================================================
-// LinearAttention pass 1 (diffusion.py:93-96): k/v projection + softmax-over-pixels partials, one 128-pixel item at a
-// time, all four heads per item.  Roles are swapped relative to the convs: the weights are the M operand, so a TMEM
-// lane is a k (or v) channel and a column is a pixel:
-//     D1K[k channel 32*head+d][px] = Wk * X^T ,   D1V[v channel 32*head+e][px] = Wv * X^T      (two UMMAs per K step)
-// One thread therefore owns one k row AND one v row over 64 pixels: the softmax max / sum are private reductions
-// over its own TMEM columns (held in registers between the max and the exp pass), P = exp(k - max) goes back to TMEM
-// in place, V^T goes to shared memory as a K-major operand, and S[d][e] = sum_px P[d,px] V[e,px] is a second UMMA
-// with A = P read from TMEM, accumulated into the (already drained) D1V columns.  k and v never reach HBM; per item
-// only (max, sum, S) partials of the four 32x32 diagonal blocks are written, merged by k_attn_ctx.
-// Pipeline: two 256-column TMEM slots, so the projection of item i+1 runs under the softmax of item i; the context
-// UMMA of item i (issued by its own warp) runs under the max/exp pass of item i+1: its read-out is deferred until just
-// before V^T is rewritten.  One named barrier per item; everything else is mbarrier hand-offs.
-// =================================================================================================================
-namespace kvk {
-constexpr int PX = 128;                        // pixels per item: N of the projection, K extent of the context UMMA
-constexpr int KCH = 8;                         // 16-byte channel chunks per stage (32 channels)
-constexpr int XS = KCH * PX * 16;              // activation stage  [chunk][pixel][16 B]
-constexpr int WS = 2 * KCH * 128 * 16;         // weight stage      [k|v][chunk][row][16 B]
-constexpr int STAGE = XS + WS;
-constexpr int STAGES = 3;
-constexpr int VT = (PX / 4) * 128 * 16;        // V^T operand       [pixel chunk][v row][16 B]
-constexpr int NPART = 4;                       // pixel parts: 4 lane quarters x NPART = softmax warps
-constexpr int PCOLS = PX / NPART;              // columns (pixels) per thread
-constexpr int EPW = 4 * NPART;                 // softmax warps
-constexpr int THREADS = (EPW + 3) * 32;        // + projection-UMMA warp, loader warp, context-UMMA warp
-constexpr int RED = 2 * 2 * NPART * 128 * 4;   // max | sum exchange between the pixel parts, double-buffered
-constexpr int NSLOT = 2, SLOT_COLS = 256;
-constexpr int NBARS = 2 * STAGES + 4 * NSLOT;
-constexpr size_t SMEM = (size_t)STAGES * STAGE + VT + RED + NBARS * 8 + 16;
-static_assert(PCOLS == 32 || PCOLS == 64, "one or two 32-column TMEM loads per thread");
-}
-
-// BF16: x is a bf16 operand tensor [B][H][C/8][W][8] and the projection runs as kind::f16 (a stage then carries 64
-// channels); P and V stay fp32 in TMEM / shared memory, so the context UMMA is tf32 in both modes.
-template <bool BF16>
-__global__ void __launch_bounds__(kvk::THREADS, 1) k_attn_kv(const ConvTcParams p) {
-    using namespace kvk;
-    constexpr int EPC = BF16 ? 8 : 4;                              // channels per 16-byte chunk
-    extern __shared__ __align__(1024) uint8_t smem[];
-    uint8_t* sS = smem;                                            // [STAGES][X | Wk | Wv]
-    uint8_t* vt = sS + STAGES * STAGE;
-    float* s_mx = reinterpret_cast<float*>(vt + VT);               // [2 parity][NPART][128]
-    float* s_z = s_mx + 2 * NPART * 128;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(s_z + 2 * NPART * 128);
-    uint32_t* s_tmem = reinterpret_cast<uint32_t*>(bars + NBARS);
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int HW = p.H * p.W;
-    const int ksteps = p.c0 / (KCH * EPC);
-    const int mtiles = (HW + PX - 1) / PX;
-    const int total = p.B * mtiles;
-    const uint32_t bar0 = smem_u32(bars);
-    auto full = [&](int s) { return bar0 + 8u * s; };
-    auto empty = [&](int s) { return bar0 + 8u * (STAGES + s); };
-    auto tfull = [&](int a) { return bar0 + 8u * (2 * STAGES + a); };              // projection of the slot complete
-    auto tempty = [&](int a) { return bar0 + 8u * (2 * STAGES + NSLOT + a); };     // slot drained
-    auto pready = [&](int a) { return bar0 + 8u * (2 * STAGES + 2 * NSLOT + a); }; // P in TMEM + V^T in smem written
-    auto kvdone = [&](int a) { return bar0 + 8u * (2 * STAGES + 3 * NSLOT + a); }; // context UMMA complete
-
-    if (tid == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 1); }
-        for (int a = 0; a < NSLOT; ++a) {
-            mbar_init(tfull(a), 1); mbar_init(tempty(a), EPW); mbar_init(pready(a), EPW); mbar_init(kvdone(a), 1);
-        }
-        fence_barrier_init();
-    }
-    if (warp == EPW) tmem_alloc(smem_u32(s_tmem), 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *s_tmem;
-
-    if (warp < EPW) {
-        // ---------------------------------------------------------------- softmax warps
-        const int q = warp & 3, part = warp >> 2;                  // TMEM lane quarter = head, pixel part
-        const int row = q * 32 + lane;
-        const int col0 = part * PCOLS;
-        const uint32_t lane_sel = (uint32_t)(q * 32) << 16;
-        int tl = 0;
-        int pb = 0, pmt = 0; float pmd = 0.f;                      // previous item (deferred read-out)
-        auto finish = [&](int ptl) {
-            const int pslot = ptl & 1;
-            mbar_wait(kvdone(pslot), (ptl >> 1) & 1);
-            tc_fence_after();
-            if (part == 0) {
-                uint32_t r[32];
-                tmem_ld32(tmem_base + pslot * SLOT_COLS + lane_sel + 128 + q * 32, r);     // S[d = lane][e] of head q
-                float* pt = p.kv_part + (((long long)pb * mtiles + pmt) * kHeads + q) * kKvPartFloats;
-                float z = 0.f;
-#pragma unroll
-                for (int j = 0; j < NPART; ++j) z += s_z[(pslot * NPART + j) * 128 + row];
-                pt[lane] = pmd;
-                pt[32 + lane] = z;
-#pragma unroll
-                for (int i = 0; i < 32; i += 4)
-                    *reinterpret_cast<float4*>(&pt[64 + lane * 32 + i]) =
-                        make_float4(__uint_as_float(r[i]), __uint_as_float(r[i + 1]), __uint_as_float(r[i + 2]), __uint_as_float(r[i + 3]));
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty(pslot));
-        };
-        for (int t = blockIdx.x; t < total; t += gridDim.x, ++tl) {
-            const int b = t / mtiles, mt = t - b * mtiles;
-            const int slot = tl & 1;
-            const uint32_t tq = tmem_base + slot * SLOT_COLS + lane_sel;
-            const int nvalid = min(PX, HW - mt * PX) - col0;       // valid columns of this thread's part (may be <= 0)
-            mbar_wait(tfull(slot), (tl >> 1) & 1);
-            tc_fence_after();
-            uint32_t kr[PCOLS / 32][32];
-            float mx = -INFINITY;
-#pragma unroll
-            for (int c = 0; c < PCOLS / 32; ++c) {
-                tmem_ld32(tq + col0 + c * 32, kr[c]);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) if (c * 32 + i < nvalid) mx = fmaxf(mx, __uint_as_float(kr[c][i]));
-            }
-            s_mx[(slot * NPART + part) * 128 + row] = mx;
-            asm volatile("bar.sync 1, %0;" ::"n"(EPW * 32) : "memory");
-            float md = s_mx[(slot * NPART) * 128 + row];
-#pragma unroll
-            for (int j = 1; j < NPART; ++j) md = fmaxf(md, s_mx[(slot * NPART + j) * 128 + row]);
-            float z0 = 0.f, z1 = 0.f, z2 = 0.f, z3 = 0.f;
-#pragma unroll
-            for (int c = 0; c < PCOLS / 32; ++c) {
-#pragma unroll
-                for (int i = 0; i < 32; i += 4) {
-                    const float e0 = c * 32 + i < nvalid ? __expf(__uint_as_float(kr[c][i]) - md) : 0.f;
-                    const float e1 = c * 32 + i + 1 < nvalid ? __expf(__uint_as_float(kr[c][i + 1]) - md) : 0.f;
-                    const float e2 = c * 32 + i + 2 < nvalid ? __expf(__uint_as_float(kr[c][i + 2]) - md) : 0.f;
-                    const float e3 = c * 32 + i + 3 < nvalid ? __expf(__uint_as_float(kr[c][i + 3]) - md) : 0.f;
-                    z0 += e0; z1 += e1; z2 += e2; z3 += e3;
-                    kr[c][i] = __float_as_uint(e0); kr[c][i + 1] = __float_as_uint(e1);
-                    kr[c][i + 2] = __float_as_uint(e2); kr[c][i + 3] = __float_as_uint(e3);
-                }
-                tmem_st32(tq + col0 + c * 32, kr[c]);
-            }
-            s_z[(slot * NPART + part) * 128 + row] = (z0 + z1) + (z2 + z3);
-            // The context UMMA of the previous item has had the whole max/exp pass to finish; it must be complete before
-            // V^T is overwritten.  Its S block is read out (and its slot released) here.
-            if (tl > 0) finish(tl - 1);
-#pragma unroll
-            for (int c = 0; c < PCOLS; c += 32) {
-                uint32_t r[32];
-                tmem_ld32(tq + 128 + col0 + c, r);
-#pragma unroll
-                for (int i = 0; i < 32; i += 4)
-                    *reinterpret_cast<uint4*>(vt + ((size_t)((col0 + c + i) / 4) * 128 + row) * 16) = make_uint4(r[i], r[i + 1], r[i + 2], r[i + 3]);
-            }
-            tmem_wait_st();
-            fence_proxy_async();                                   // V^T smem writes -> visible to the tensor core
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(pready(slot));
-            pb = b; pmt = mt; pmd = md;
-        }
-        if (tl > 0) finish(tl - 1);
-    } else if (warp == EPW) {
-        // ---------------------------------------------------------------- projection UMMA issuer (whole warp + elect_one)
-        {
-            const uint32_t idesc = make_idesc<BF16>(128, PX);
-            const uint32_t s0 = smem_u32(sS);
-            constexpr uint32_t D_HI = desc_hi(128);
-            uint32_t it = 0;
-            int tl = 0;
-            for (int t = blockIdx.x; t < total; t += gridDim.x, ++tl) {
-                const int slot = tl & 1;
-                const uint32_t tslot = tmem_base + slot * SLOT_COLS;
-                mbar_wait(tempty(slot), ((tl >> 1) & 1) ^ 1);
-                tc_fence_after();
-                for (int ks = 0; ks < ksteps; ++ks, ++it) {
-                    const int s = it % STAGES;
-                    mbar_wait(full(s), (it / STAGES) & 1);
-                    tc_fence_after();
-                    const uint32_t xs = s0 + s * STAGE;
-                    const uint32_t x_lo = desc_lo(xs, PX * 16), k_lo = desc_lo(xs + XS, 128 * 16), v_lo = desc_lo(xs + XS + KCH * 128 * 16, 128 * 16);
-                    if (elect_one()) {
-#pragma unroll
-                        for (int kk = 0; kk < KCH / 2; ++kk) {
-                            const uint64_t xd = desc_pack(x_lo + (uint32_t)(kk * 2 * PX), D_HI);
-                            umma<BF16>(tslot, desc_pack(k_lo + (uint32_t)(kk * 2 * 128), D_HI), xd, idesc, (ks | kk) != 0 ? 1u : 0u);
-                            umma<BF16>(tslot + 128, desc_pack(v_lo + (uint32_t)(kk * 2 * 128), D_HI), xd, idesc, (ks | kk) != 0 ? 1u : 0u);
-                        }
-                        umma_commit(empty(s));
-                        if (ks == ksteps - 1) umma_commit(tfull(slot));
-                    }
-                    __syncwarp();
-                }
-            }
-        }
-    } else if (warp == EPW + 2) {
-        // ---------------------------------------------------------------- context UMMA issuer: S = P * V^T
-        {
-            const uint32_t idesc2 = make_idesc<false>(128, 128);
-            const uint32_t v_lo = desc_lo(smem_u32(vt), 128 * 16);
-            constexpr uint32_t D_HI = desc_hi(128);
-            int tl = 0;
-            for (int t = blockIdx.x; t < total; t += gridDim.x, ++tl) {
-                const int slot = tl & 1;
-                const uint32_t tslot = tmem_base + slot * SLOT_COLS;
-                mbar_wait(pready(slot), (tl >> 1) & 1);
-                tc_fence_after();
-                if (elect_one()) {
-#pragma unroll
-                    for (int kk = 0; kk < PX / 8; ++kk)                // K = 8 pixels (32 bytes) per UMMA
-                        umma_ts_tf32(tslot + 128, tslot + kk * 8, desc_pack(v_lo + (uint32_t)(kk * 2 * 128), D_HI), idesc2, kk != 0 ? 1u : 0u);
-                    umma_commit(kvdone(slot));
-                }
-                __syncwarp();
-            }
-        }
-    } else {
-        // ---------------------------------------------------------------- loader warp: weights + activation runs (cp.async.bulk)
-        // lane 0 owns the ring protocol and the weight copy; lanes 0-7 each issue the activation runs of one channel chunk
-        // (a single issuing thread was the bottleneck of this kernel: ~20 copies + address math per 48 KB stage).
-        uint32_t it = 0;
-        const int chs = p.c0 / EPC;
-        const uint8_t* src = reinterpret_cast<const uint8_t*>(p.in0);
-        for (int t = blockIdx.x; t < total; t += gridDim.x) {
-            const int b = t / mtiles, mt = t - b * mtiles;
-            const int m0 = mt * PX, m_hi = m0 + PX < HW ? m0 + PX : HW;
-            const int hh0 = m0 / p.W, ww0 = m0 - hh0 * p.W;
-            for (int ks = 0; ks < ksteps; ++ks, ++it) {
-                const int s = it % STAGES;
-                const uint32_t xs = smem_u32(sS) + s * STAGE;
-                if (lane == 0) {
-                    mbar_wait(empty(s), ((it / STAGES) & 1) ^ 1);
-                    mbar_arrive_expect_tx(full(s), STAGE);
-                    bulk_g2s(xs + XS, reinterpret_cast<const uint8_t*>(p.wpk) + (size_t)ks * WS, WS, full(s));
-                }
-                __syncwarp();
-                if (lane < KCH) {
-                    const int k = lane, cl = ks * KCH + k;
-                    int m = m0, hh = hh0, ww = ww0, qx = 0;
-                    while (m < m_hi) {                             // split the flattened run at image-row boundaries
-                        const int n = (p.W - ww) < (m_hi - m) ? (p.W - ww) : (m_hi - m);
-                        bulk_g2s(xs + (k * PX + qx) * 16, src + (((long long)(b * p.H + hh) * chs + cl) * p.W + ww) * 16,
-                                 (uint32_t)n * 16u, full(s));
-                        m += n; qx += n; ++hh; ww = 0;
-                    }
-                    if (qx < PX) bulk_g2s(xs + (k * PX + qx) * 16, p.zero_page, (uint32_t)(PX - qx) * 16u, full(s));
-                }
-            }
-        }
-    }
-    __syncthreads();
-    if (warp == EPW) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
-    }
-}
-
-template <bool BF16>
-static int launch_attn_kv(const ConvTcParams& p, cudaStream_t s) {
-    static DevCache cache;
-    const int num_sms = cache.get(reinterpret_cast<const void*>(k_attn_kv<BF16>));
-    if (num_sms <= 0) return -1;
-    const long long total = (long long)p.B * ((p.H * p.W + kvk::PX - 1) / kvk::PX);
-    const int grid = (int)(total < num_sms ? total : num_sms);
-    k_attn_kv<BF16><<<grid, kvk::THREADS, kvk::SMEM, s>>>(p);
-    return 1;
-}
-int attn_kv_tile_pixels() { return kvk::PX; }
-
-// N tile per geometry: UP needs 8 accumulators (8*64 = all 512 TMEM columns), DOWN's de-interleaved A tile is large
+// N tile per geometry: Upsample keeps 4 phase accumulators per thread, so its tiles are 64 channels wide
 int conv_tc_ntile(int geom, int Cout) {
     if (geom == G_UP || geom == G_DOWN) return 64;
     if (geom_is_c1(geom)) return Cout % 128 == 0 ? 128 : (Cout % 64 == 0 ? 64 : 32);
     return Cout % 128 == 0 ? 128 : 64;
 }
-// pair tiles (4 rows x 128 pixels) of one sample's grid
-int conv_tc_pair_tiles(int H, int W) { return ((W + TPX - 1) / TPX) * ((H + 2 * ROWS - 1) / (2 * ROWS)); }
-int conv_tc_ntile_x3(int geom, int Cout) { return conv_tc_ntile(geom, Cout); }     // (the running sums live in TMEM: same N tiles as tf32)
+int conv_tc_ntile_x3(int geom, int Cout) { return conv_tc_ntile(geom, Cout); }     // (the running sums live in registers next to the accumulators)
 int conv_tc_taps(int geom) {
     switch (geom) {
         case G_PW: return 1;
@@ -1222,17 +639,16 @@ int conv_tc_stage_channels(int geom, int bf16) {
     const int epc = bf16 ? 8 : 4;
     return (geom == G_PW ? Geo<G_PW>::KCH : Geo<G_C3>::KCH) * epc;
 }
+int conv_tc_tile_rows() { return ROWS; }
 
 template <bool BF16>
 static int dispatch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
     const int nt = (p.nt == 64 && p.geom == G_C3) ? 64 : conv_tc_ntile(p.geom, p.Cout);
     switch (p.geom) {
         case G_C3:
-            if (p.rs) return nt == 64 ? launch_tc<G_C3, BF16, 64, false, false, true>(p, s) : -1;
-            if (p.pair) return nt == 128 ? launch_tc_pair<BF16, 128, false>(p, s) : launch_tc_pair<BF16, 64, false>(p, s);
             return nt == 128 ? launch_tc<G_C3, BF16, 128>(p, s) : launch_tc<G_C3, BF16, 64>(p, s);
         case G_PW:
-            if (p.epi == EPI_KV) return launch_attn_kv<BF16>(p, s);
+            if (p.epi == EPI_KV) return launch_attn_kv(p, s);
             if (p.epi == EPI_RES) return nt == 128 ? launch_tc<G_PW, BF16, 128, true>(p, s) : launch_tc<G_PW, BF16, 64, true>(p, s);
             return nt == 128 ? launch_tc<G_PW, BF16, 128>(p, s) : launch_tc<G_PW, BF16, 64>(p, s);
         case G_DOWN: return launch_tc<G_DOWN, BF16, 64>(p, s);
@@ -1257,8 +673,6 @@ static int dispatch_conv_tc_x3(const ConvTcParams& p, cudaStream_t s) {
     const int nt = (p.nt == 64 && p.geom == G_C3) ? 64 : conv_tc_ntile(p.geom, p.Cout);
     switch (p.geom) {
         case G_C3:
-            if (p.rs) return nt == 64 ? launch_tc<G_C3, false, 64, false, true, true>(p, s) : -1;
-            if (p.pair) return nt == 128 ? launch_tc_pair<false, 128, true>(p, s) : launch_tc_pair<false, 64, true>(p, s);
             return nt == 128 ? launch_tc<G_C3, false, 128, false, true>(p, s) : launch_tc<G_C3, false, 64, false, true>(p, s);
         case G_PW:
             if (p.epi == EPI_KV) return launch_attn_kv_x3(p, s);      // fused projection + softmax + context (sbk_attn_x3.cu)

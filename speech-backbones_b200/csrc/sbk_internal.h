@@ -49,7 +49,7 @@ struct IgemmParams {
     int out_mask;                                 // multiply the stored output by mask[b][wo << out_lvl]
 };
 
-// tcgen05 convolution (sbk_conv_tc.cu).  Inputs are operand-form tensors: already masked / activated, so the
+// Tensor-core (wgmma) convolution (sbk_conv_tc.cu).  Inputs are operand-form tensors: already masked / activated, so the
 // kernel's A path is a pure copy.  geom = G_C3 (3x3, pad 1) or G_PW (1x1 over the flattened image).
 struct ConvTcParams {
     int geom;
@@ -65,7 +65,7 @@ struct ConvTcParams {
     double* ostats;                                 // EPI_PLAIN: GroupNorm statistics of the raw output (nullable)
     const float* mask; int T; int lvl; int out_mask;   // out_mask: multiply the stored output by mask[b][wo << lvl]
     const float* rraw; GnRef rgn;                   // EPI_RES: out = acc + bias + Mish(GN(rraw))*mask
-    float* kv_part;                                 // EPI_KV (1x1, NT=128): [B][ceil(HW/256)][4][kKvPartFloats]
+    float* kv_part;                                 // EPI_KV: [B][ceil(HW/attn_kv_tile_pixels())][4][kKvPartFloats]
     const float* addin;                             // EPI_PLAIN: out += addin (same shape/layout/dtype as out): residual added in fp32
     const float* zero_page;                         // >= 4 KB of zeros in global memory (out-of-image parts of A tiles)
     int bf16;
@@ -76,12 +76,9 @@ struct ConvTcParams {
     int dil, pad; float slope; int act_out, act_out2;
     // fp32-class mode (SBK_PREC_FP32X3): every operand x is carried as the pair (x, correction chunks - see corr_chunk
     // below); the tensor core reads the top 19 bits of x (= x_hi) by itself.  Weights are packed as (w_hi, correction)
-    // stage pairs and each K stage is issued twice into the same fp32 TMEM accumulator: the kind::f16 correction MMAs
-    // (x_lo*w + x*w_lo) first, then the kind::tf32 main MMAs (x_hi*w_hi).
-    int rs;                                         // G_C3, 64 output channels: row-shared issue order; wpk is then the [sx][chunk][kr2|kr1|kr0] image
-    int pair;                                       // G_C3: run on CTA pairs (cta_group::2); wpk is then the image packed for NT/2-wide tiles
+    // stage pairs and each K stage is issued twice into the same fp32 register accumulator: the f16 correction MMAs
+    // (x_lo*w + x*w_lo) first, then the tf32 main MMAs (x_hi*w_hi).
     int x3;
-    int flush;                                      // sub-stages per accumulation run (0 = default); SBK_X3_FLUSH overrides it (measurement knob)
     const void* in0_lo; const void* in1_lo;         // the correction tensors, same chunk layout as in0 / in1
     float* out_lo;                                  // operand-form outputs (non-3x3 geometries): also write the correction chunks
 };
@@ -139,7 +136,7 @@ struct AttnMixParams {          // A_b = I + g * Wout * blockdiag(ctx^T) * Wq ; 
     float* b_eff;               // [C]
     int B, C;
     int tc_nt, tc_cps;          // != 0: write g*P only (the identity/residual is added in fp32 by the conv epilogue),
-                                // in the tcgen05 1x1 weight-stage layout, tf32-rounded
+                                // in the tensor-core 1x1 weight-stage layout, tf32-rounded
     int tc_bf16;                // ... as bf16, 8 input channels per 16-byte chunk (tc_cps = 64)
     int tc_x3;                  // fp32x3 mode: (hi, lo) stage pairs [ntile][kstage][hi|lo][chunk][cout % NT][4]
 };
@@ -240,30 +237,31 @@ int launch_first_conv(const FirstConvParams& p, cudaStream_t s);
 int launch_conv_tc(const ConvTcParams& p, cudaStream_t s);
 int conv_tc_ntile(int geom, int Cout);
 int conv_tc_ntile_x3(int geom, int Cout);
-int conv_tc_pair_tiles(int H, int W);
+int conv_tc_tile_rows();
 int conv_tc_taps(int geom);
 int conv_tc_stage_channels(int geom, int bf16);
 int launch_gn_act(const GnActParams& p, cudaStream_t s);
 int launch_resfinal(const ResFinalParams& p, cudaStream_t s);
 int launch_attn_ctx(const AttnCtxParams& p, cudaStream_t s);
+// fused k|v projection + softmax + context partials (sbk_attn_x3.cu), one partial per item of attn_kv_tile_pixels() pixels:
+// p.kv_part = [B][items per sample][4][kKvPartFloats]; tf32 / bf16 operands, or fp32-class (fp32x3 mode)
 int attn_kv_tile_pixels();
-// fp32x3 mode: fused k|v projection + online softmax + context partials (sbk_attn_x3.cu); p.Ho = items per chunk, p.Wo = chunks
-// per sample, p.kv_part = [B][chunks per sample][4][kKvPartFloats]
+int launch_attn_kv(const ConvTcParams& p, cudaStream_t s);
 int launch_attn_kv_x3(const ConvTcParams& p, cudaStream_t s);
-int attn_kv_x3_item_pixels();
 int launch_attn_mix(const AttnMixParams& p, cudaStream_t s);
 int launch_final(const FinalParams& p, cudaStream_t s);
 int launch_time_table(const TimeTableParams& p, cudaStream_t s);
 int launch_spk(const SpkParams& p, cudaStream_t s);
 int launch_step_begin(const StepBeginParams& p, cudaStream_t s);
+int device_sm_count();      // SMs of the current device (grid caps of the grid-stride kernels)
 int launch_scale_mask(const float* z, const float* mask, float* out, long long n_per_b_row, int B, int H, int T, cudaStream_t s);
 
 // the part of an fp32 value the tensor core's tf32 operand path drops (low 13 mantissa bits): exact in fp32
 __device__ __forceinline__ float tf32_lo(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
 // ---- fp32x3 mode: the correction operand ------------------------------------------------------------------------------
-// x*w = x_hi*w_hi + (x_lo*w + x*w_lo) + O(2^-23): the first product runs on kind::tf32 from the fp32 tensor itself (the
-// tensor core reads the top 19 bits = x_hi), the bracket is ONE kind::f16 MMA over a packed correction operand.  For every
+// x*w = x_hi*w_hi + (x_lo*w + x*w_lo) + O(2^-23): the first product runs as a tf32 MMA on the fp32 tensor itself (the
+// tensor core reads the top 19 bits = x_hi), the bracket is ONE f16 MMA over a packed correction operand.  For every
 // 16-byte chunk of 4 channels the producers write, next to the fp32 chunk, a second 16-byte chunk of eight fp16 values
 //     { x_lo[c0..c3] , x[c0..c3] * 2^-12 }            with x_lo = x - trunc_tf32(x)  (|x_lo| <= 2^-10 |x|)
 // and the weight packers write the matching K order { w[c0..c3] , w_lo[c0..c3] * 2^12 } (w_lo = w - tf32(w)), so one

@@ -1,4 +1,4 @@
-// sm_100a kernels of the score U-Net step (fp32 CUDA-core path + all fused glue kernels).
+// sm_90a kernels of the score U-Net step (fp32 CUDA-core path + all fused glue kernels).
 //
 // Data layout: every activation is NHWC fp32, [B][H][W][C] with H = mel bins (80/40/20),
 // W = frames (T, T/2, T/4), C innermost so that one pixel's channels are one contiguous
@@ -835,7 +835,6 @@ __device__ __forceinline__ float bf16_hi_f(uint32_t u) { return __uint_as_float(
 // Thread mapping of the two kernels below: a LANE PAIR owns one frame - lane half h handles the fp32 chunk 2*ch+h
 // (4 channels: the same register footprint as the fp32 kernels, so the same 4 CTAs/SM) and writes its 8-byte half of
 // the 16-byte bf16 chunk: loads are two interleaved 256-byte runs per warp, stores one contiguous 256-byte run.
-// (First version: one thread per 8-channel chunk = 92-128 registers, 2 CTAs/SM, 2.8-3.7 TB/s; profiles/r1_ops_bf16_v2.txt.)
 __global__ void __launch_bounds__(256) k_gn_act_bf16(const GnActParams p) {
     extern __shared__ __align__(16) float sm[];
     float* mean = sm; float* scale = mean + p.C; float* beta = scale + p.C; float* tbv = beta + p.C;
@@ -1154,7 +1153,7 @@ __global__ void __launch_bounds__(256) k_attn_mix(const AttnMixParams p) {
             acc[4] = fmaf(m1.x, wq, acc[4]); acc[5] = fmaf(m1.y, wq, acc[5]); acc[6] = fmaf(m1.z, wq, acc[6]); acc[7] = fmaf(m1.w, wq, acc[7]);
         }
         if (p.tc_nt) {
-            // tcgen05 1x1 weight image: [ntile][kstage][chunk][cout % NT][4 cin], tf32 (RNA); g*P only (see AttnMixParams)
+            // tensor-core 1x1 weight image: [ntile][kstage][chunk][cout % NT][4 cin], tf32 (RNA); g*P only (see AttnMixParams)
             // (bf16 mode: 8 cin per 16-byte chunk, stored as bf16)
             const int epc = p.tc_bf16 ? 8 : 4;
             const int NT = p.tc_nt, kch = p.tc_cps / epc, ksteps = C / p.tc_cps;
@@ -1165,7 +1164,7 @@ __global__ void __launch_bounds__(256) k_attn_mix(const AttnMixParams p) {
                 float v = g * acc[i];
                 if (p.tc_x3) {
                     // fp32x3: (w_hi, correction) stage pair - tf32 (RNA) main image and the fp16 chunk {w[c0..c3], w_lo[c0..c3] * 2^12}
-                    // of the kind::f16 correction MMA (sbk_internal.h: corr_chunk)
+                    // of the f16 correction MMA (sbk_internal.h: corr_chunk)
                     const long long ih = (((((long long)(co / NT) * ksteps + ks) * 2) * kch + kc) * NT + (co % NT)) * 4 + e;
                     uint32_t uh;
                     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(uh) : "f"(v));

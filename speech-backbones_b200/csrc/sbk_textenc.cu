@@ -453,7 +453,7 @@ static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths
         conv(mel, c.n_feats, nullptr, 0, "init_proj", "init_proj.bias", 1, C, 1, 0, 0, nullptr, 0, "", 0, 0, h0, 0, 1);
     } else {
         k_te_mask<<<(B * Tx + 255) / 256, 256, 0, s>>>(reinterpret_cast<const long long*>(x_lengths), x_mask, B, Tx); ++n;
-        k_te_embed<<<(int)std::min<size_t>((ntok * (C / 4) + 255) / 256, 148 * 8), 256, 0, s>>>(reinterpret_cast<const long long*>(x), W("emb.weight"), h0, (int)ntok, C, c.n_vocab, sqrtf((float)C)); ++n;
+        k_te_embed<<<(int)std::min<size_t>((ntok * (C / 4) + 255) / 256, 8 * (size_t)sbk::device_sm_count()), 256, 0, s>>>(reinterpret_cast<const long long*>(x), W("emb.weight"), h0, (int)ntok, C, c.n_vocab, sqrtf((float)C)); ++n;
     }
     // ---- prenet (ConvReluNorm, :57-64): x = relu(LN(conv5(x * mask))) x3; x = (x_org + proj(x)) * mask
     const float* cur = h0; float* pp[2] = {h1, h2};
@@ -469,7 +469,7 @@ static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths
     if (c.n_spks > 1) {
         float* hc = (hx == h1) ? h2 : h1;
         // h0 is free now but sized for Ce as well: concatenate into it
-        k_te_concat_spk<<<(int)std::min<size_t>((ntok * Ce + 255) / 256, 148 * 8), 256, 0, s>>>(hx, spk, h0, B, Tx, C, c.spk_emb_dim); ++n;
+        k_te_concat_spk<<<(int)std::min<size_t>((ntok * Ce + 255) / 256, 8 * (size_t)sbk::device_sm_count()), 256, 0, s>>>(hx, spk, h0, B, Tx, C, c.spk_emb_dim); ++n;
         h = h0; (void)hc;
     }
     float* other[2];

@@ -1,9 +1,9 @@
 // HiFi-GAN generator (mel -> waveform), the step immediately after the sampler: Grad-TTS/hifi-gan/models.py:77-128 (Generator),
 // :13-49 (ResBlock1), called at Grad-TTS/inference.py:81.  SURVEY.md 8(f) rank 3.
 //
-// Mapping onto the sampler's tcgen05 kernels (sbk_conv_tc.cu), all activations fp32 [B][C/4][L][4] (the 2-D layout with H = 1):
-//   * Conv1d(K in {3,7,11}, dilation d)   -> k_conv_tc<G_C1K*>: one strip of 256 + 64 samples per channel chunk in shared memory,
-//                                            tap t of the UMMA A operand = descriptor start + t*d samples; bias, LeakyReLU and
+// Mapping onto the sampler's wgmma kernels (sbk_conv_tc.cu), all activations fp32 [B][C/4][L][4] (the 2-D layout with H = 1):
+//   * Conv1d(K in {3,7,11}, dilation d)   -> k_conv_tc<G_C1K*>: one strip of 128 + 64 samples per channel chunk in shared memory,
+//                                            tap t of the wgmma A operand = descriptor start + t*d samples; bias, LeakyReLU and
 //                                            the ResBlock residual (x + conv2(...), models.py:47) live in its epilogue, which
 //                                            also writes lrelu(x) - the next conv's operand - so no activation pass exists;
 //   * ConvTranspose1d(k = 2u, stride u)   -> ONE 1x1 GEMM (k_conv_tc<G_PW>) to k*Cout channels, Z[i][t][co] = sum_ci x[i][ci] w[ci][co][t],
@@ -27,6 +27,12 @@
 #include <vector>
 
 using namespace sbk;
+
+int sbk::device_sm_count() {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
+    return n;
+}
 
 int sbk_set_error(int code, const char* fmt, ...);     // sbk_api.cu: fills the thread-local error text
 
@@ -116,7 +122,11 @@ __global__ void __launch_bounds__(256) k_voc_post(const float* a, const float* w
     }
 }
 
-int ew_grid(long long n) { long long g = (n + 255) / 256; return (int)(g < 1 ? 1 : (g > 148 * 16 ? 148 * 16 : g)); }
+// grid-stride elementwise kernels: 256-thread blocks, at most 16 blocks per SM
+int ew_grid(long long n) {
+    const long long g = (n + 255) / 256, cap = 16LL * device_sm_count();
+    return (int)(g < 1 ? 1 : (g > cap ? cap : g));
+}
 
 uint32_t f32_to_tf32_rna(float x) {
     uint32_t u; memcpy(&u, &x, 4);
@@ -132,7 +142,7 @@ struct sbk_vocoder {
     sbk_vocoder_config cfg;
     std::vector<VWSpec> spec;
     std::map<std::string, float*> raw;       // device copies, reference layout (after remove_weight_norm)
-    std::map<std::string, float*> packed;    // tcgen05 stage images
+    std::map<std::string, float*> packed;    // tensor-core stage images
     float* zero = nullptr;
     void* mem = nullptr; size_t cap = 0;
     bool is_packed = false;

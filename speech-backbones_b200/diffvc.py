@@ -53,7 +53,7 @@ class GradLogPEstimator(BaseModule):
     def __init__(self, dim_base, dim_cond, use_ref_t, dim_mults=(1, 2, 4)):
         super().__init__()
         if tuple(dim_mults) != (1, 2, 4):
-            raise ValueError("the sm_100a engine is built for dim_mults=(1,2,4)")
+            raise ValueError("the sm_90a engine is built for dim_mults=(1,2,4)")
         self.use_ref_t, self.dim_base, self.dim_cond = use_ref_t, dim_base, dim_cond
         chans = [2 + dim_cond] + [dim_base * m for m in dim_mults]
         pairs = list(zip(chans[:-1], chans[1:]))
@@ -140,7 +140,7 @@ class Diffusion(BaseModule):
     def engine(self) -> Engine:
         dev = next(self.parameters()).device
         if dev.type != "cuda":
-            raise RuntimeError("DiffVC sampling runs only on a CUDA device (sm_100a); move the module with .cuda() "
+            raise RuntimeError("DiffVC sampling runs only on a CUDA device (sm_90a); move the module with .cuda() "
                                "first - there is no CPU fallback")
         sig = (dev.index,) + tuple((p.data_ptr(), p._version) for p in self.estimator.parameters())
         if self._engine is None or self._engine.device != dev.index:
@@ -160,7 +160,7 @@ class Diffusion(BaseModule):
     @torch.no_grad()
     def conditioning_table(self, ref, ref_mask, mean_ref, c, n_timesteps):
         """cond[i] for every step i (t_i = 1 - i/N): the hoisted conditioning branch, native in every precision
-        (libsbk `sbk_vc_conditioning`: RefBlock convs on tcgen05 - tf32 + fp16 correction for the fp32-class modes - plus the
+        (libsbk `sbk_vc_conditioning`: RefBlock convs on wgmma - tf32 + fp16 correction for the fp32-class modes - plus the
         InstanceNorm / GLU / cond_block kernels).  There is no PyTorch fallback."""
         with torch.cuda.device(ref.device):
             return self.engine().vc_conditioning(ref, ref_mask, mean_ref, c, n_timesteps)

@@ -3,7 +3,7 @@
 Same constructor, same parameter names/shapes under `estimator.*` (so
 `GradTTS.load_state_dict(strict=True)`, inference.py:53, keeps working) and the same
 `forward(z, mask, mu, n_timesteps, stoc=False, spk=None)` surface called from
-`GradTTS.forward` (tts.py:96).  Sampling runs in libsbk.so (hand-written sm_100a CUDA,
+`GradTTS.forward` (tts.py:96).  Sampling runs in libsbk.so (hand-written sm_90a CUDA,
 CUDA-graph replay of the Euler loop); there is NO CPU or eager-PyTorch sampling path -
 calling `forward` with CPU tensors raises.  The training-time methods
 (`forward_diffusion`, `loss_t`, `compute_loss`; diffusion.py:244-252,281-294) stay plain
@@ -125,7 +125,7 @@ class GradLogPEstimator2d(BaseModule):
     def __init__(self, dim, dim_mults=(1, 2, 4), groups=8, n_spks=None, spk_emb_dim=64, n_feats=80, pe_scale=1000):
         super().__init__()
         if tuple(dim_mults) != (1, 2, 4) or groups != 8:
-            raise ValueError("the sm_100a engine is built for dim_mults=(1,2,4), groups=8 (the reference defaults)")
+            raise ValueError("the sm_90a engine is built for dim_mults=(1,2,4), groups=8 (the reference defaults)")
         self.dim, self.dim_mults, self.groups = dim, dim_mults, groups
         self.n_spks = 1 if n_spks is None else n_spks
         self.spk_emb_dim, self.pe_scale, self.n_feats = spk_emb_dim, pe_scale, n_feats
@@ -211,7 +211,7 @@ class Diffusion(BaseModule):
         """The libsbk handle for the module's current device/weights (re-packed when weights change)."""
         dev = next(self.parameters()).device
         if dev.type != "cuda":
-            raise RuntimeError("Diffusion sampling runs only on a CUDA device (sm_100a); move the module with "
+            raise RuntimeError("Diffusion sampling runs only on a CUDA device (sm_90a); move the module with "
                                ".cuda() first - there is no CPU fallback")
         sig = self._weights_signature(dev)
         if self._engine is None or self._engine.device != dev.index:
@@ -326,7 +326,7 @@ def synthesize_from_encoder(decoder, mu_x, logw, x_mask, n_timesteps, temperatur
     the reference's own call on a tensor with the reference's strides (`reference_order_noise`), so with the same
     generator state z equals the reference's z bit for bit.  Returns (encoder_outputs, decoder_outputs, attn) like the reference."""
     if not mu_x.is_cuda:
-        raise RuntimeError("synthesize_from_encoder runs only on a CUDA device (sm_100a); there is no CPU fallback")
+        raise RuntimeError("synthesize_from_encoder runs only on a CUDA device (sm_90a); there is no CPU fallback")
     B, Fm, Tx = mu_x.shape
     w = torch.exp(logw) * x_mask                                                   # :77
     w_ceil = torch.ceil(w) * length_scale                                          # :78

@@ -10,7 +10,7 @@
 Same constructor argument, same parameter names (`conv_pre.weight_g/_v`, `ups.i.*`, `resblocks.n.convs{1,2}.j.*`, `conv_post.*`,
 and the plain `.weight` names after `remove_weight_norm()`), so the reference checkpoint loads with `strict=True`.  The modules
 below are parameter containers only: `forward` runs in libsbk.so (`sbk_vocoder_forward`: dilated Conv1d and the transposed
-convs on tcgen05, see csrc/sbk_vocoder.cu).  There is no CPU or eager-PyTorch path: calling `forward` with CPU tensors raises.
+convs on wgmma, see csrc/sbk_vocoder.cu).  There is no CPU or eager-PyTorch path: calling `forward` with CPU tensors raises.
 """
 from __future__ import annotations
 
@@ -189,7 +189,7 @@ class Generator(nn.Module):
     def engine(self) -> VocoderEngine:
         dev = next(self.parameters()).device
         if dev.type != "cuda":
-            raise RuntimeError("the HiFi-GAN generator runs only on a CUDA device (sm_100a); move the module with .cuda() "
+            raise RuntimeError("the HiFi-GAN generator runs only on a CUDA device (sm_90a); move the module with .cuda() "
                                "first - there is no CPU fallback")
         sig = (dev.index,) + tuple((n, p.data_ptr(), p._version) for n, p in self.named_parameters())
         if self._engine is None or self._engine.device != dev.index:

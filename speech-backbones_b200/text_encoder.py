@@ -171,7 +171,7 @@ class MelEncoder(BaseModule):
     def __init__(self, n_feats, channels, filters, heads, layers, kernel, dropout, window_size=None):
         super().__init__()
         if window_size is None:
-            raise ValueError("the sm_100a mel encoder implements relative-position attention (DiffVC uses window_size=4)")
+            raise ValueError("the sm_90a mel encoder implements relative-position attention (DiffVC uses window_size=4)")
         self.n_feats, self.channels, self.filters, self.heads, self.layers = n_feats, channels, filters, heads, layers
         self.kernel, self.dropout, self.window_size = kernel, dropout, window_size
         # the engine reads the text encoder's attribute names
@@ -187,7 +187,7 @@ class MelEncoder(BaseModule):
     def engine(self) -> TextEncEngine:
         dev = next(self.parameters()).device
         if dev.type != "cuda":
-            raise RuntimeError("the mel encoder runs only on a CUDA device (sm_100a); move the module with .cuda() first - "
+            raise RuntimeError("the mel encoder runs only on a CUDA device (sm_90a); move the module with .cuda() first - "
                                "there is no CPU fallback")
         sig = (dev.index,) + tuple((p.data_ptr(), p._version) for p in self.parameters())
         if self._engine is None or self._engine.device != dev.index:
@@ -211,7 +211,7 @@ class TextEncoder(BaseModule):
                  p_dropout, window_size=None, spk_emb_dim=64, n_spks=1):
         super().__init__()
         if window_size is None:
-            raise ValueError("the sm_100a text encoder implements the relative-position attention Grad-TTS uses (window_size=4)")
+            raise ValueError("the sm_90a text encoder implements the relative-position attention Grad-TTS uses (window_size=4)")
         self.n_vocab, self.n_feats, self.n_channels = n_vocab, n_feats, n_channels
         self.filter_channels, self.filter_channels_dp = filter_channels, filter_channels_dp
         self.n_heads, self.n_layers, self.kernel_size = n_heads, n_layers, kernel_size
@@ -229,7 +229,7 @@ class TextEncoder(BaseModule):
     def engine(self) -> TextEncEngine:
         dev = next(self.parameters()).device
         if dev.type != "cuda":
-            raise RuntimeError("the text encoder runs only on a CUDA device (sm_100a); move the module with .cuda() first - "
+            raise RuntimeError("the text encoder runs only on a CUDA device (sm_90a); move the module with .cuda() first - "
                                "there is no CPU fallback")
         sig = (dev.index,) + tuple((p.data_ptr(), p._version) for p in self.parameters())
         if self._engine is None or self._engine.device != dev.index:

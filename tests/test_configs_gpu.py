@@ -77,10 +77,9 @@ def test_config4_diffvc_ml_n6_t256_vs_oracle(sbk_lib):
 @pytest.mark.parametrize("precision", ["fp32x3", "tf32", "bf16"])
 def test_alone_vs_in_batch_at_config_shapes(sbk_lib, precision):
     """scripts/gpu_config3.py's probe as a test: rows 5..6 of a B=8, T=512 ragged batch re-run alone (same padded T) for
-    N = 20 steps reproduce their rows: bit for bit in the tf32 / bf16 modes (fp64 GroupNorm statistics, one TMEM
+    N = 20 steps reproduce their rows: bit for bit in the tf32 / bf16 modes (fp64 GroupNorm statistics, one
     accumulation run per output whatever the tiling), to fp32 rounding in the fp32x3 mode (a 2-utterance batch takes the
-    64-wide N tiles, whose accumulation runs are cut every 2 sub-stages instead of 3: same sums, different fp32 rounding
-    points - measured 2.5e-7 after 20 steps)."""
+    64-wide N tiles: same sums, different fp32 rounding points)."""
     from speech_backbones_b200.binding import Engine
     cfg = UNetConfig()
     eng = Engine(precision=precision)

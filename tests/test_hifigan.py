@@ -2,7 +2,7 @@
 
 CPU: the module's parameter tree is the reference's (weight-norm names before, plain names after `remove_weight_norm()`), the
 effective weights it hands to libsbk equal what `remove_weight_norm()` produces, and the C ABI exports the vocoder symbols.
-GPU: `sbk_vocoder_forward` (dilated Conv1d + transposed-conv GEMMs on tcgen05, tf32 operands) against the committed outputs of
+GPU: `sbk_vocoder_forward` (dilated Conv1d + transposed-conv GEMMs on wgmma, tf32 operands) against the committed outputs of
 the UNMODIFIED reference generator (tests/golden/hifigan_golden.pt) and against the CPU oracle at a ragged size.
 
 Tolerance: tf32 operands through a 15-conv-deep residual stack per stage (the arithmetic PyTorch's own GPU convs use by

@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a path (through the C ABI / the drop-in module) vs the CPU oracle and the
+"""GPU parity tests: the sm_90a path (through the C ABI / the drop-in module) vs the CPU oracle and the
 committed reference goldens.  Tolerances (fp32 CUDA-core path): rel-L2 <= 1e-4 per estimator call and per
 intermediate, <= 2e-3 on trajectories (the random-weight reverse SDE is expansive, SURVEY.md 8c)."""
 import pytest
@@ -201,12 +201,12 @@ def test_config2_shape_properties(engines):
     assert torch.isfinite(out).all() and (out * (1 - mask)).abs().max().item() == 0.0
 
 
-# ---- tensor-core precision modes (tcgen05 kind::tf32 / kind::f16-bf16 operands, fp32 accumulate in TMEM) ----
+# ---- tensor-core precision modes (wgmma tf32 / bf16 operands, fp32 accumulate in registers) ----
 # Tolerances follow the operand rounding (SURVEY.md 8c, measured by emulation on the reference):
 # tf32 (10-bit mantissa) ~1e-3 per estimator call, bf16 (8-bit) ~9e-3; GN/softmax/Mish/Euler stay fp32.
 # bf16 mode: conv inputs AND the residual stream are stored as bf16 (8-bit mantissa, 2^-9 relative rounding per store),
-# accumulation / GN statistics / raw conv outputs / sampler state fp32.  Measured on B200: 1.07-1.27e-2 per estimator call,
-# <= 1.2e-2 per stage, 3.1-5.5e-3 on trajectories, 3.7e-2 on the |xt| x100 stress case (SURVEY 8c predicted 9e-3 / 3-5e-3).
+# accumulation / GN statistics / raw conv outputs / sampler state fp32 (SURVEY 8c predicted 9e-3 per call, 3-5e-3 on
+# trajectories).
 TC_TOL = {"tf32": (4e-3, 8e-3), "bf16": (2e-2, 1e-2)}       # (per estimator call / stage, trajectory)
 # The |xt| x100 stress case drives the attention logits k to O(100): softmax turns the tf32 operand rounding of the
 # k projection (|k| * 2^-11 absolute) into a relative error of the same size in p = exp(k - max), so this one case
@@ -289,9 +289,8 @@ def test_bf16_tracks_tf32_at_config_shapes(engines):
 @pytest.mark.parametrize("precision", ["fp32", "tf32", "bf16"])
 def test_reproducible_and_batch_independent(engines, precision):
     """Same call twice -> same result; an utterance alone -> the same rows as inside a batch.  GroupNorm statistics are
-    accumulated in fp64 (smem + global atomics), so the summation order cannot move the fp32 mean / rstd: before that
-    change the 1e-8 order noise was amplified by operand-rounding flips through this random-weight U-Net to 6e-4 (tf32)
-    and 7e-3 (bf16) per call (profiles/r1_batch_dep_before.log)."""
+    accumulated in fp64 (smem + global atomics), so the summation order cannot move the fp32 mean / rstd (1e-8 of order noise would be amplified by
+    operand-rounding flips through this random-weight U-Net to visible per-call differences)."""
     z, mask, mu, _, _ = synthetic_inputs(3, 512, ragged=True)
     t = torch.tensor([0.9, 0.5, 0.1])
     eng = engines(1, True, 1234, precision)

@@ -1,9 +1,9 @@
-"""CPU: the operand-rounding model of the tensor-core modes (oracle/precision_model.py) vs the errors MEASURED on the B200.
+"""CPU: the operand-rounding model of the tensor-core modes (oracle/precision_model.py) vs the errors MEASURED on the H100.
 
 The model runs the pinned CPU oracle with tf32 / bf16 rounding applied exactly where libsbk rounds operands and nowhere
 else.  If the GPU paths had any error source beyond operand rounding (a wrong tap, a dropped border, a mis-scaled GN), the
 measured rel-L2 against the fp32 reference would exceed the model's prediction; it does not: the measured per-call errors
-(profiles/r1_bf16_bringup.log, golden `est` cases, single-speaker) sit within a few percent of the prediction."""
+(scripts/gpu_vs_precision_model.py, golden `est` cases, single-speaker) sit within a few percent of the prediction."""
 import pytest
 import torch
 
@@ -11,14 +11,14 @@ from helpers import case_id, case_inputs, rel_l2
 from oracle import gradtts_oracle as O
 from oracle.precision_model import operand_rounding, round_bf16, round_tf32_rna, trunc_tf32
 
-# rel-L2 of one estimator call vs the reference, measured on the GPU (profiles/r1_bf16_bringup.log), keyed by case id
+# rel-L2 of one estimator call vs the reference, measured on an H100 (scripts/gpu_vs_precision_model.py), keyed by case id
 MEASURED = {
-    "kindest-n_spks1-B2-T32-raggedTrue-t[0.995, 0.5]-scale1.0": dict(tf32=1.559e-3, bf16=1.118e-2),
-    "kindest-n_spks1-B1-T64-raggedFalse-t[0.005]-scale1.0": dict(tf32=1.489e-3, bf16=1.070e-2),
-    "kindest-n_spks1-B2-T32-raggedTrue-t[0.3, 0.7]-scale100.0": dict(tf32=4.615e-3, bf16=3.713e-2),
-    "kindest-n_spks1-B3-T100-raggedTrue-t[0.9, 0.1, 0.5]-scale1.0": dict(tf32=1.541e-3, bf16=1.111e-2),
-    "kindest-n_spks1-B1-T4-raggedFalse-t[0.5]-scale1.0": dict(tf32=1.507e-3, bf16=1.266e-2),
-    "kindest-n_spks1-B1-T256-raggedFalse-t[0.5]-scale1.0": dict(tf32=1.524e-3, bf16=1.107e-2),
+    "kindest-n_spks1-B2-T32-raggedTrue-t[0.995, 0.5]-scale1.0": dict(tf32=1.545e-03, bf16=1.109e-02),
+    "kindest-n_spks1-B1-T64-raggedFalse-t[0.005]-scale1.0": dict(tf32=1.489e-03, bf16=1.067e-02),
+    "kindest-n_spks1-B2-T32-raggedTrue-t[0.3, 0.7]-scale100.0": dict(tf32=4.477e-03, bf16=3.754e-02),
+    "kindest-n_spks1-B3-T100-raggedTrue-t[0.9, 0.1, 0.5]-scale1.0": dict(tf32=1.545e-03, bf16=1.114e-02),
+    "kindest-n_spks1-B1-T4-raggedFalse-t[0.5]-scale1.0": dict(tf32=1.462e-03, bf16=1.169e-02),
+    "kindest-n_spks1-B1-T256-raggedFalse-t[0.5]-scale1.0": dict(tf32=1.516e-03, bf16=1.100e-02),
 }
 
 
@@ -47,12 +47,12 @@ def test_measured_gpu_error_is_explained_by_operand_rounding(golden, mode):
     assert seen == len(MEASURED)
 
 
-# rel-L2 of whole trajectories (N reverse steps) vs the reference, measured on the GPU (same log)
+# rel-L2 of whole trajectories (N reverse steps) vs the reference, measured on the H100 (same script)
 MEASURED_TRAJ = {
-    "kindtraj-n_spks1-B2-T32-raggedTrue-N1-stocFalse": dict(tf32=7.011e-4, bf16=4.932e-3),
-    "kindtraj-n_spks1-B2-T32-raggedTrue-N10-stocFalse": dict(tf32=6.490e-4, bf16=4.127e-3),
-    "kindtraj-n_spks1-B2-T32-raggedTrue-N5-stocTrue": dict(tf32=8.297e-4, bf16=5.483e-3),
-    "kindtraj-n_spks1-B1-T128-raggedFalse-N10-stocFalse": dict(tf32=5.761e-4, bf16=3.568e-3),
+    "kindtraj-n_spks1-B2-T32-raggedTrue-N1-stocFalse": dict(tf32=6.958e-04, bf16=4.832e-03),
+    "kindtraj-n_spks1-B2-T32-raggedTrue-N10-stocFalse": dict(tf32=6.422e-04, bf16=4.113e-03),
+    "kindtraj-n_spks1-B2-T32-raggedTrue-N5-stocTrue": dict(tf32=8.220e-04, bf16=5.441e-03),
+    "kindtraj-n_spks1-B1-T128-raggedFalse-N10-stocFalse": dict(tf32=5.726e-04, bf16=3.591e-03),
 }
 
 
@@ -74,10 +74,10 @@ def test_measured_trajectory_error_is_explained_by_operand_rounding(golden, mode
     assert seen == len(MEASURED_TRAJ)
 
 
-@pytest.mark.parametrize("mode,measured", [("tf32", 5.854e-4), ("bf16", 3.720e-3)])
+@pytest.mark.parametrize("mode,measured", [("tf32", 5.842e-4), ("bf16", 3.721e-3)], ids=["tf32", "bf16"])   # (ids: not the measured data)
 def test_config1_end_to_end_error_was_predicted(mode, measured):
     """BASELINE config 1 end to end (tests/test_zz_config1_e2e.py): the model's prediction (5.82e-4 / 3.71e-3) was computed
-    before the case first ran on the B200; the measured values are the ones printed by that GPU test."""
+    before the case first ran on a GPU; the measured values are the ones that GPU test printed on an H100."""
     import os
     from speech_backbones_b200 import UNetConfig, synthetic_state_dict
     from speech_backbones_b200.gradtts import reference_order_noise
@@ -95,13 +95,13 @@ def test_config1_end_to_end_error_was_predicted(mode, measured):
     assert abs(measured / predicted - 1.0) <= 0.05
 
 
-# fp32x3 (tests/test_fp32x3_gpu.py on the B200, final round-2 kernels): rel-L2 of one estimator call vs the reference
+# fp32x3 (scripts/gpu_vs_precision_model.py on an H100): rel-L2 of one estimator call vs the reference
 MEASURED_X3 = {
-    "kindest-n_spks1-B1-T64-raggedFalse-t[0.005]-scale1.0": 2.788e-6,
-    "kindest-n_spks1-B2-T32-raggedTrue-t[0.3, 0.7]-scale100.0": 5.520e-6,
-    "kindest-n_spks1-B3-T100-raggedTrue-t[0.9, 0.1, 0.5]-scale1.0": 2.874e-6,
-    "kindest-n_spks1-B1-T4-raggedFalse-t[0.5]-scale1.0": 2.167e-6,
-    "kindest-n_spks1-B1-T256-raggedFalse-t[0.5]-scale1.0": 2.839e-6,
+    "kindest-n_spks1-B1-T64-raggedFalse-t[0.005]-scale1.0": 2.787e-06,
+    "kindest-n_spks1-B2-T32-raggedTrue-t[0.3, 0.7]-scale100.0": 4.796e-06,
+    "kindest-n_spks1-B3-T100-raggedTrue-t[0.9, 0.1, 0.5]-scale1.0": 2.878e-06,
+    "kindest-n_spks1-B1-T4-raggedFalse-t[0.5]-scale1.0": 2.082e-06,
+    "kindest-n_spks1-B1-T256-raggedFalse-t[0.5]-scale1.0": 2.841e-06,
 }
 
 
