@@ -233,6 +233,38 @@ int sbk_textenc_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengt
 int sbk_melenc_forward(sbk_textenc* e, const float* x, const float* x_mask, float* out, int B, int T, void* stream);
 int64_t sbk_textenc_last_launch_count(const sbk_textenc* e);
 
+/* ---- DiffVC's PostNet: the second half of the "average voice" encoder --------------------------------------------------
+ * FwdDiffusion (DiffVC/model/vc.py:19-48) is MelEncoder (above, kind = 1) followed by PostNet (DiffVC/model/postnet.py:40-53):
+ * init_conv 1x1 (1 -> dim), a ResnetBlock of two Block(7x7 Conv2d(dim, dim, padding 3), GroupNorm(groups, dim), Mish) plus a
+ * 1x1 residual conv (postnet.py:15-37), final_conv 1x1 (dim -> 1), over the [n_feats, T] mel grid as a one-channel image.
+ * The 7x7 convs run on wgmma (tf32 operands, or the fp32x3 split); GroupNorm statistics cover the whole grid, padded columns
+ * included, as the reference's do. */
+typedef struct sbk_postnet sbk_postnet;
+typedef struct sbk_postnet_config {
+    int32_t device;
+    int32_t dim;          /* PostNet(dim) (vc.py:34; DiffVC enc_dim = 128): 64, 128 or a multiple of 256                  */
+    int32_t groups;       /* GroupNorm groups (postnet.py:16,27,41, default 8): must be 8                                       */
+    int32_t precision;    /* SBK_PREC_*: FP32X3 and FP32 run the fp32x3 split, TF32 and BF16 run tf32 operands            */
+} sbk_postnet_config;
+/* PostNet.__init__ (postnet.py:41-45).  SBK_ERR_UNSUPPORTED for any other dim / groups. */
+int sbk_postnet_create(const sbk_postnet_config* cfg, sbk_postnet** out);
+void sbk_postnet_destroy(sbk_postnet* p);
+/* the 14 tensors of PostNet.state_dict() (init_conv.*, res_block.block{1,2}.block.{0,1}.*, res_block.res.*, final_conv.*):
+ * count / name of the i-th one (host logic; no GPU work) */
+int sbk_postnet_num_weights(const sbk_postnet* p);
+const char* sbk_postnet_weight_name(const sbk_postnet* p, int i);
+/* load_state_dict(strict) (vc.py:77-79 loads the encoder's checkpoint): one call per tensor, host or device fp32; then pack */
+int sbk_postnet_set_weight(sbk_postnet* p, const char* name, const void* data, const int64_t* shape, int ndim);
+int sbk_postnet_pack(sbk_postnet* p);
+/* device workspace of a (B, n_feats, T) call (allocated by sbk_postnet_forward, grow-only) */
+size_t sbk_postnet_workspace_bytes(const sbk_postnet* p, int B, int n_feats, int T);
+/* PostNet.forward(x, mask) (postnet.py:47-53, called at vc.py:40,46): x [B,n_feats,T], mask [B,1,T] in {0,1} -> out
+ * [B,n_feats,T].  The output is not masked, as in the reference: a padded column equals final_conv.bias.  Device pointers,
+ * asynchronous on `stream`; a refused kernel launch fails the call. */
+int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* mask, float* out, int B, int n_feats, int T, void* stream);
+/* kernel launches (and memsets) the last sbk_postnet_forward enqueued */
+int64_t sbk_postnet_last_launch_count(const sbk_postnet* p);
+
 const char* sbk_last_error(void);
 const char* sbk_version(void);
 

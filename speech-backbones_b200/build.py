@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsbk.so")
-SOURCES = ["sbk_api.cu", "sbk_kernels.cu", "sbk_conv_tc.cu", "sbk_attn_x3.cu", "sbk_vocoder.cu", "sbk_textenc.cu"]
+SOURCES = ["sbk_api.cu", "sbk_kernels.cu", "sbk_conv_tc.cu", "sbk_attn_x3.cu", "sbk_vocoder.cu", "sbk_textenc.cu", "sbk_postnet.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", *ARCH, "-lineinfo", "-Xcompiler", "-fPIC"]
 

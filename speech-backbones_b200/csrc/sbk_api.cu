@@ -392,34 +392,44 @@ static int pack_tc_up(sbk_handle* h, const std::string& src, const std::string& 
         m[((size_t)co * C + ci) * 16 + t] = w[((size_t)ci * C + co) * 16 + t];
     return pack_tc_host(h, m, key, C, C, G_UP, bf16);
 }
-static int pack_tc_host(sbk_handle* h, const std::vector<float>& hs, const std::string& key, int cout, int cin, int geom, bool bf16, int nt_override) {
-    const int taps = conv_tc_taps(geom);
-    const bool x3 = !bf16 && packs_x3(h);
+// The 7x7 geometry streams one kernel row per stage: weight stage ks = (K step ks / 7, kernel row ks % 7) holds the 7 taps
+// of that row, so with `rows` stages per K step a stage carries taps / rows taps, stage tap s being tap (ks % rows) * (taps
+// / rows) + s of the kernel.  rows = 1 for every other geometry.
+size_t sbk::conv_tc_pack_image(const float* hs, int cout, int cin, int geom, bool bf16, bool x3, int nt_override, uint8_t* dst) {
+    const int taps = conv_tc_taps(geom), rows = conv_tc_stage_rows(geom), tps = taps / rows;
     const int NT = nt_override ? nt_override : (x3 ? conv_tc_ntile_x3(geom, cout) : conv_tc_ntile(geom, cout)), CPS = conv_tc_stage_channels(geom, bf16 ? 1 : 0), EPC = bf16 ? 8 : 4, KCHK = CPS / EPC;
-    const int ksteps = cin / CPS;
+    const int ksteps = cin / CPS * rows;
     const size_t esz = bf16 ? 2 : 4;
-    std::vector<uint8_t> hd((size_t)cout * cin * taps * esz * (x3 ? 2 : 1));
-    for (int nt = 0; nt < cout / NT; ++nt) for (int ks = 0; ks < ksteps; ++ks) for (int tap = 0; tap < taps; ++tap)
+    const size_t bytes = (size_t)cout * cin * taps * esz * (x3 ? 2 : 1);
+    if (!dst) return bytes;
+    uint8_t* hd = dst;
+    for (int nt = 0; nt < cout / NT; ++nt) for (int ks = 0; ks < ksteps; ++ks) for (int tap = 0; tap < tps; ++tap)
         for (int k = 0; k < KCHK; ++k) for (int col = 0; col < NT; ++col) for (int e = 0; e < EPC; ++e) {
-            const int co = nt * NT + col, ci = ks * CPS + k * EPC + e;
-            const float w = hs[((size_t)co * cin + ci) * taps + tap];
+            const int co = nt * NT + col, ci = (ks / rows) * CPS + k * EPC + e;
+            const float w = hs[((size_t)co * cin + ci) * taps + (ks % rows) * tps + tap];
             if (x3) {
                 // [ntile][kstage][hi|correction][tap][chunk][co % NT][16 B]: the main image holds w_hi = tf32(w) (RNA), the
                 // correction image the fp16 chunk {w[c0..c3], (w - w_hi)[c0..c3] * 2^12} that pairs with the activations'
                 // {x_lo, x * 2^-12} chunk in one f16 MMA (sbk_internal.h: corr_chunk)
-                const size_t ih = ((((((size_t)nt * ksteps + ks) * 2) * taps + tap) * KCHK + k) * NT + col) * EPC + e;
+                const size_t ih = ((((((size_t)nt * ksteps + ks) * 2) * tps + tap) * KCHK + k) * NT + col) * EPC + e;
                 const uint32_t uh = f32_to_tf32_rna(w);
                 float fh; memcpy(&fh, &uh, 4);
-                reinterpret_cast<uint32_t*>(hd.data())[ih] = uh;
-                uint16_t* cc = reinterpret_cast<uint16_t*>(hd.data()) + 2 * ((ih - e) + (size_t)taps * KCHK * NT * EPC);   // this (chunk, co)'s 8 halfs
+                reinterpret_cast<uint32_t*>(hd)[ih] = uh;
+                uint16_t* cc = reinterpret_cast<uint16_t*>(hd) + 2 * ((ih - e) + (size_t)tps * KCHK * NT * EPC);   // this (chunk, co)'s 8 halfs
                 cc[e] = f32_to_f16_rn(w);
                 cc[4 + e] = f32_to_f16_rn((w - fh) * 4096.f);
                 continue;
             }
-            const size_t idx = (((((size_t)nt * ksteps + ks) * taps + tap) * KCHK + k) * NT + col) * EPC + e;
-            if (bf16) reinterpret_cast<uint16_t*>(hd.data())[idx] = f32_to_bf16_rn(w);
-            else reinterpret_cast<uint32_t*>(hd.data())[idx] = f32_to_tf32_rna(w);
+            const size_t idx = (((((size_t)nt * ksteps + ks) * tps + tap) * KCHK + k) * NT + col) * EPC + e;
+            if (bf16) reinterpret_cast<uint16_t*>(hd)[idx] = f32_to_bf16_rn(w);
+            else reinterpret_cast<uint32_t*>(hd)[idx] = f32_to_tf32_rna(w);
         }
+    return bytes;
+}
+static int pack_tc_host(sbk_handle* h, const std::vector<float>& hs, const std::string& key, int cout, int cin, int geom, bool bf16, int nt_override) {
+    const bool x3 = !bf16 && packs_x3(h);
+    std::vector<uint8_t> hd(conv_tc_pack_image(hs.data(), cout, cin, geom, bf16, x3, nt_override, nullptr));
+    conv_tc_pack_image(hs.data(), cout, cin, geom, bf16, x3, nt_override, hd.data());
     float*& d = h->packed[key];
     if (!d) { CU(cudaMalloc(&d, hd.size())); h->owned.push_back(d); }
     CU(cudaMemcpy(d, hd.data(), hd.size(), cudaMemcpyHostToDevice));

@@ -1,5 +1,6 @@
 // Warpgroup-MMA (wgmma) implicit-GEMM convolutions for sm_90a: the 3x3 Block convs (81.5 % of the step's MACs), the
-// 1x1 channel mixes (res_conv, attention apply), Downsample / Upsample and the vocoder's dilated Conv1d.  tf32 (or bf16)
+// 1x1 channel mixes (res_conv, attention apply), Downsample / Upsample, the vocoder's dilated Conv1d and the 7x7 convs of
+// DiffVC's PostNet (G_C7: one kernel row per ring stage, see Geo<G_C7>).  tf32 (or bf16)
 // operands from shared memory, fp32 accumulation in registers.
 //
 //   D[pixel][cout] (fp32, registers) += A[pixel][tap, cin] (smem) * W[cout][tap, cin] (smem)
@@ -55,6 +56,15 @@ template <> struct Geo<G_C1K3> : GeoC1<3> {};
 template <> struct Geo<G_C1K7> : GeoC1<7> {};
 template <> struct Geo<G_C1K11> : GeoC1<11> {};
 
+// 7x7, pad 3 (PostNet): a 3x3-style stage (halo tile + all taps of one 8-channel K step) would carry 49 x 2 x NT x 16 B
+// of weights - 200 KB at NT = 128 - and leave no room for a second stage.  A K step is therefore split by kernel row:
+// stage (K step, kernel row r) holds ONE input row of TPX + 6 pixels per channel chunk (4.3 KB) and the 7 taps of row r
+// (28 KB at NT = 128); tap s is the descriptor start s pixels into the row, as in the 3x3 halo tile.  Every input row is
+// fetched by up to 7 stages of a tile (from L2 after the first), ~15 % of the weight bytes.
+template <> struct Geo<G_C7> { static constexpr int HR = 1, PXP = TPX + 6, TAPS = 7, KCH = 2, NACC = 1; };
+// stages per K step (kernel rows streamed one stage at a time)
+template <int GEOM> constexpr int kRows = GEOM == G_C7 ? 7 : 1;
+
 }  // namespace tc
 
 using namespace tc;
@@ -90,7 +100,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     constexpr int NACC = G::NACC;
     constexpr bool CHUNKED = X3 && GEOM != G_UP;
     // sub-stages per accumulation run: 6 = three K stages of correction + main sub-stage, 54 MMAs per accumulator for a
-    // 3x3 conv
+    // 3x3 conv (7x7: three (K step, kernel row) stages, 42 MMAs)
     const int FLUSH = CHUNKED ? 6 : (1 << 30);
     constexpr int STAGES = D::STAGES, LDS = D::LDS;
     constexpr int LAG = STAGES >= 3 ? STAGES - 2 : 0;      // G_DOWN only: cp.async groups in flight behind the newest
@@ -125,7 +135,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
     const int Cin = p.c0 + p.c1;
     const int HW = p.H * p.W;
-    const int ksteps = Cin / CPS;
+    const int ksteps = Cin / CPS * kRows<GEOM>;            // ring stages per tile (7x7: one per K step and kernel row)
     // fp32x3 mode: each K stage runs twice - the f16 correction sub-stage (x_lo*w + x*w_lo from the packed fp16 chunks,
     // sbk_internal.h: corr_chunk) first, then the tf32 main sub-stage (x_hi*w_hi): small terms first
     const int ksteps_t = X3 ? 2 * ksteps : ksteps;
@@ -246,7 +256,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         } else {
 #pragma unroll
                             for (int tap = 0; tap < TAPS; ++tap) {
-                                const int r = TAPS == 9 ? tap / 3 : 0, sx = TAPS == 9 ? tap % 3 : 0;
+                                const int r = TAPS == 9 ? tap / 3 : 0, sx = TAPS == 9 ? tap % 3 : (GEOM == G_C7 ? tap : 0);
                                 // DOWN: input row r; column tap s reads the odd plane at x (s=0) / x+1 (s=2), the even plane at x (s=1)
                                 const uint32_t aoff = GEOM == G_DOWN ? (uint32_t)(r * PXP + (sx == 1 ? TPX + 1 : (sx == 2 ? 1 : 0)))
                                                     : C1 ? (uint32_t)tap * dil
@@ -316,7 +326,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
             const int Ho = (GEOM == G_DOWN || GEOM == G_UP) ? p.Ho : p.H, Wo = (GEOM == G_DOWN || GEOM == G_UP) ? p.Wo : p.W;
             const int CHo = p.Cout / 4;                            // 16-byte channel chunks of the output tensor
             int ho, wo; bool valid;
-            if (GEOM == G_C3 || GEOM == G_DOWN) {
+            if (GEOM == G_C3 || GEOM == G_C7 || GEOM == G_DOWN) {
                 ho = h0; wo = w0 + px;
                 valid = ho < Ho && wo < Wo;
             } else if (C1) {
@@ -435,7 +445,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         float* op = p.out + obase + (cb / 4) * cstride;
 #pragma unroll
                         for (int i = 0; i < 32; i += 4) *reinterpret_cast<float4*>(op + (i / 4) * cstride) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-                        if (GEOM != G_C3 && p.out_lo) {
+                        if (GEOM != G_C3 && GEOM != G_C7 && p.out_lo) {
                             float* lp = p.out_lo + obase + (cb / 4) * cstride;
 #pragma unroll
                             for (int i = 0; i < 32; i += 4) {
@@ -511,9 +521,12 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
             // weight image: [ntile][kstage][tap][chunk][NT][16 B]; fp32x3: [ntile][kstage][hi|correction][tap][chunk][NT][16 B]
             const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.wpk) + (size_t)b * p.w_bstride_bytes +
                                   (size_t)(n0 / NT) * ksteps * (X3 ? 2 : 1) * B_STAGE_BYTES;
+            // 3x3 / 7x7 halo: input row of halo row r of a stage is h0 - PADK + krow + r
+            constexpr int PADK = GEOM == G_C7 ? 3 : 1;
             for (int ks = 0; ks < ksteps_t; ++ks, ++it) {
                 const int s = it % STAGES;
-                const int kb = X3 ? ks / 2 : ks, var = X3 ? (ks & 1) : 1;          // 0: correction (fp16 chunks), 1: main (x, w_hi)
+                const int st = X3 ? ks / 2 : ks, var = X3 ? (ks & 1) : 1;          // 0: correction (fp16 chunks), 1: main (x, w_hi)
+                const int kb = st / kRows<GEOM>, krow = st - kb * kRows<GEOM>;     // K step, kernel row (7x7) of weight stage st
                 if (lane == 0) {
                     mbar_wait(empty(s), ((it / STAGES) & 1) ^ 1);
                     uint32_t a_tx = BULK ? A_STAGE_BYTES : 0;
@@ -522,7 +535,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         // need zeroing when this stage buffer last served a tile with a different border pattern.  With
                         // the round-robin tile order a CTA normally keeps one pattern, so this (and its proxy fence,
                         // which would otherwise serialise against the bulk copies in flight) runs a handful of times.
-                        const int pad = C1 ? p.pad : 1;             // Conv1d: (K-1)*dil/2 samples of halo on each side
+                        const int pad = C1 ? p.pad : PADK;          // Conv1d: (K-1)*dil/2 samples of halo on each side
                         const int wlo = w0 - pad < 0 ? 0 : w0 - pad, whi = w0 + SPAN + pad > p.W ? p.W : w0 + SPAN + pad;
                         const int qlo = wlo - (w0 - pad), qhi = qlo + (whi - wlo);
                         const uint32_t pat = (uint32_t)qlo | ((uint32_t)qhi << 16);
@@ -540,11 +553,11 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                             }
                         }
                         int vrows = 0;
-                        for (int r = 0; r < HR; ++r) { const int hi = C1 ? 0 : h0 - 1 + r; vrows += (hi >= 0 && hi < p.H) ? 1 : 0; }
+                        for (int r = 0; r < HR; ++r) { const int hi = C1 ? 0 : h0 - PADK + krow + r; vrows += (hi >= 0 && hi < p.H) ? 1 : 0; }
                         a_tx -= (uint32_t)(KCH * vrows * (PXP - (qhi - qlo))) * 16u;
                     }
                     mbar_arrive_expect_tx(full_b(s), B_STAGE_BYTES + a_tx);
-                    bulk_g2s(smem_u32(sB + s * B_STAGE_BYTES), wsrc + (size_t)(X3 ? 2 * kb + (var == 0) : ks) * B_STAGE_BYTES,
+                    bulk_g2s(smem_u32(sB + s * B_STAGE_BYTES), wsrc + (size_t)(X3 ? 2 * st + (var == 0) : ks) * B_STAGE_BYTES,
                              B_STAGE_BYTES, full_b(s));
                 }
                 __syncwarp();
@@ -571,10 +584,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         }
                         if (q < PXP) bulk_g2s(a_s + k * PLANE + (r * PXP + q) * 16, zero, (uint32_t)(PXP - q) * 16u, full_b(s));
                     } else {
-                        const int pad = C1 ? p.pad : 1;
+                        const int pad = C1 ? p.pad : PADK;
                         const int wlo = w0 - pad < 0 ? 0 : w0 - pad, whi = w0 + SPAN + pad > p.W ? p.W : w0 + SPAN + pad;
                         const int qlo = wlo - (w0 - pad);
-                        const int hi = C1 ? 0 : h0 - 1 + r;
+                        const int hi = C1 ? 0 : h0 - PADK + krow + r;
                         const uint32_t row_s = a_s + k * PLANE + (r * PXP) * 16;
                         if (hi < 0 || hi >= p.H) bulk_g2s(row_s, zero, PXP * 16u, full_b(s));
                         else bulk_g2s(row_s + qlo * 16, src + (((long long)(b * p.H + hi) * chs + cl) * p.W + wlo) * 16,
@@ -608,7 +621,7 @@ static int launch_tc(const ConvTcParams& p, cudaStream_t s) {
     if (num_sms <= 0) return -1;
     int mt;
     if (geom_is_c1(GEOM)) mt = (p.W + TPX - 1) / TPX;
-    else if (GEOM == G_C3 || GEOM == G_UP) mt = ((p.W + TPX - 1) / TPX) * p.H;
+    else if (GEOM == G_C3 || GEOM == G_C7 || GEOM == G_UP) mt = ((p.W + TPX - 1) / TPX) * p.H;
     else if (GEOM == G_DOWN) mt = ((p.Wo + TPX - 1) / TPX) * p.Ho;
     else mt = (p.H * p.W + TPX - 1) / TPX;
     const long long total = (long long)mt * (p.Cout / NT) * p.B;
@@ -624,7 +637,8 @@ int conv_tc_ntile(int geom, int Cout) {
     if (geom_is_c1(geom)) return Cout % 128 == 0 ? 128 : (Cout % 64 == 0 ? 64 : 32);
     return Cout % 128 == 0 ? 128 : 64;
 }
-int conv_tc_ntile_x3(int geom, int Cout) { return conv_tc_ntile(geom, Cout); }     // (the running sums live in registers next to the accumulators)
+// (the running sums live in registers next to the accumulators; the 7x7 conv's 128-wide variant would spill them)
+int conv_tc_ntile_x3(int geom, int Cout) { return geom == G_C7 ? 64 : conv_tc_ntile(geom, Cout); }
 int conv_tc_taps(int geom) {
     switch (geom) {
         case G_PW: return 1;
@@ -632,12 +646,14 @@ int conv_tc_taps(int geom) {
         case G_C1K3: return 3;
         case G_C1K7: return 7;
         case G_C1K11: return 11;
+        case G_C7: return 49;
         default: return 9;
     }
 }
+int conv_tc_stage_rows(int geom) { return geom == G_C7 ? kRows<G_C7> : 1; }
 int conv_tc_stage_channels(int geom, int bf16) {
     const int epc = bf16 ? 8 : 4;
-    return (geom == G_PW ? Geo<G_PW>::KCH : Geo<G_C3>::KCH) * epc;
+    return (geom == G_PW ? Geo<G_PW>::KCH : geom == G_C7 ? Geo<G_C7>::KCH : Geo<G_C3>::KCH) * epc;
 }
 int conv_tc_tile_rows() { return ROWS; }
 
@@ -653,6 +669,9 @@ static int dispatch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
             return nt == 128 ? launch_tc<G_PW, BF16, 128>(p, s) : launch_tc<G_PW, BF16, 64>(p, s);
         case G_DOWN: return launch_tc<G_DOWN, BF16, 64>(p, s);
         case G_UP:   return launch_tc<G_UP, BF16, 64>(p, s);
+        case G_C7:                                                    // tf32 only
+            if constexpr (BF16) return -1;
+            else return nt == 128 ? launch_tc<G_C7, false, 128>(p, s) : launch_tc<G_C7, false, 64>(p, s);
         default:     return -1;
     }
 }
@@ -679,6 +698,7 @@ static int dispatch_conv_tc_x3(const ConvTcParams& p, cudaStream_t s) {
             if (p.epi == EPI_RES) return nt == 128 ? launch_tc<G_PW, false, 128, true, true>(p, s) : launch_tc<G_PW, false, 64, true, true>(p, s);
             return nt == 128 ? launch_tc<G_PW, false, 128, false, true>(p, s) : launch_tc<G_PW, false, 64, false, true>(p, s);
         case G_DOWN: return launch_tc<G_DOWN, false, 64, false, true>(p, s);
+        case G_C7:   return launch_tc<G_C7, false, 64, false, true>(p, s);          // conv_tc_ntile_x3
         default:     return launch_tc<G_UP, false, 64, false, true>(p, s);
     }
 }

@@ -12,8 +12,9 @@ constexpr int kAttnHidden = 128;  // heads * dim_head
 constexpr int kKvPartFloats = 32 + 32 + 32 * 32;   // per (tile, head): max[32], sum[32], S[32][32]
 
 // G_C1K*: Conv1d with K taps and a runtime dilation over [B][1][C/4][L][4] tensors (the HiFi-GAN vocoder, sbk_vocoder.cu)
-enum Geom { G_PW = 0, G_C3 = 1, G_DOWN = 2, G_UP = 3, G_C1K3 = 4, G_C1K7 = 5, G_C1K11 = 6 };
-__host__ __device__ constexpr bool geom_is_c1(int g) { return g >= G_C1K3; }
+// G_C7: 7x7 conv, pad 3, stride 1 (DiffVC's PostNet Block, sbk_postnet.cu): tf32 operands or fp32x3, EPI_PLAIN output
+enum Geom { G_PW = 0, G_C3 = 1, G_DOWN = 2, G_UP = 3, G_C1K3 = 4, G_C1K7 = 5, G_C1K11 = 6, G_C7 = 7 };
+__host__ __device__ constexpr bool geom_is_c1(int g) { return g >= G_C1K3 && g <= G_C1K11; }
 enum Pro { PRO_NONE = 0, PRO_MASK = 1, PRO_GN = 2 };
 enum Epi { EPI_PLAIN = 0, EPI_RES = 1, EPI_KV = 2 };
 
@@ -239,7 +240,11 @@ int conv_tc_ntile(int geom, int Cout);
 int conv_tc_ntile_x3(int geom, int Cout);
 int conv_tc_tile_rows();
 int conv_tc_taps(int geom);
+int conv_tc_stage_rows(int geom);       // weight stages per K step: 7 for G_C7 (one per kernel row), else 1
 int conv_tc_stage_channels(int geom, int bf16);
+// host: logical weights [cout][cin][taps] -> the conv kernel's per-stage shared-memory image (sbk_api.cu); nt = 0 picks
+// conv_tc_ntile.  Returns the image size in bytes; dst may be null to query it.
+size_t conv_tc_pack_image(const float* w, int cout, int cin, int geom, bool bf16, bool x3, int nt, uint8_t* dst);
 int launch_gn_act(const GnActParams& p, cudaStream_t s);
 int launch_resfinal(const ResFinalParams& p, cudaStream_t s);
 int launch_attn_ctx(const AttnCtxParams& p, cudaStream_t s);

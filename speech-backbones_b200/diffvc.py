@@ -1,6 +1,7 @@
-"""Drop-in `Diffusion` for DiffVC (replaces DiffVC/model/diffusion.py:109-222).
+"""Drop-in `Diffusion`, `FwdDiffusion` and `DiffVC` for DiffVC (replace DiffVC/model/diffusion.py:109-222 and
+DiffVC/model/vc.py:19-144; `DiffVC` and `FwdDiffusion` are at the end of this file).
 
-Same constructor `(n_feats, dim_unet, dim_spk, use_ref_t, beta_min, beta_max)`, the same 206 parameter
+`Diffusion` has the same constructor `(n_feats, dim_unet, dim_spk, use_ref_t, beta_min, beta_max)`, the same 206 parameter
 names/shapes under `estimator.*` (so `DiffVC.load_state_dict` / `vc_*.pt` checkpoints load unchanged) and the same
 `forward(z, mask, mean, ref, ref_mask, mean_ref, c, n_timesteps, mode)` surface called from `DiffVC.forward`
 (DiffVC/model/vc.py:125), including the reference's behaviour for an invalid mode (prints and returns `z`, :201-203).
@@ -22,6 +23,8 @@ import torch.nn.functional as F
 
 from .binding import Engine
 from .gradtts import (BaseModule, Mish, SinusoidalPosEmb, _ConvGNMish, _Gate, _LinAttn, _Resample, _Skip, _TimeResBlock)
+from .postnet import PostNet
+from .text_encoder import MelEncoder
 
 
 class RefBlock(BaseModule):
@@ -241,3 +244,70 @@ def convert_from_encoder(decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_re
     z += torch.randn_like(mean_x_new, device=mean_x_new.device)                    # :122-123
     y = decoder(z, x_mask_new, mean_new, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode)     # :125
     return mean_x, y[:, :, :max_length]
+
+
+# ---- the whole model: DiffVC/model/vc.py:19-144 ------------------------------------------------------------------------------
+def sequence_mask(length, max_length=None):
+    """DiffVC/model/utils.py (same helper as Grad-TTS/model/utils.py:6-10)."""
+    if max_length is None:
+        max_length = length.max()
+    x = torch.arange(int(max_length), dtype=length.dtype, device=length.device)
+    return x.unsqueeze(0) < length.unsqueeze(1)
+
+
+class FwdDiffusion(BaseModule):
+    """Drop-in for DiffVC's "average voice" encoder (vc.py:19-48): `MelEncoder` (text_encoder.py) followed by `PostNet`
+    (postnet.py), the reference's constructor and state_dict (`encoder.*`, `postnet.*`: 8,464,529 parameters at
+    DiffVC's configuration).  `forward(x, mask)` runs both halves in libsbk; `precision` selects the PostNet's arithmetic
+    (the mel encoder is exact fp32 on CUDA cores).  Training (`compute_loss`, :43-48) is not implemented here."""
+
+    def __init__(self, n_feats, channels, filters, heads, layers, kernel, dropout, window_size, dim, *, precision="fp32x3"):
+        super().__init__()
+        self.n_feats, self.channels, self.filters, self.heads, self.layers = n_feats, channels, filters, heads, layers
+        self.kernel, self.dropout, self.window_size, self.dim = kernel, dropout, window_size, dim
+        self.encoder = MelEncoder(n_feats, channels, filters, heads, layers, kernel, dropout, window_size)
+        self.postnet = PostNet(dim, precision=precision)
+
+    @torch.no_grad()
+    def forward(self, x, mask):                                                     # :37-41
+        x, mask = self.relocate_input([x, mask])
+        z = self.encoder(x, mask)
+        return self.postnet(z, mask)
+
+
+class DiffVC(BaseModule):
+    """Drop-in for `model.vc.DiffVC` (vc.py:52-144): the same constructor, the same 346-tensor state_dict (`encoder.*` of
+    `FwdDiffusion`, `decoder.*` of `Diffusion`; 126,259,128 parameters at the notebook's configuration, so `vc_*.pt`
+    checkpoints load strictly) and the same `forward(x, x_lengths, x_ref, x_ref_lengths, c, n_timesteps, mode)` ->
+    (mean_x, y).  Encoder, PostNet and decoder run in libsbk; the random draws are the reference's, in its order."""
+
+    def __init__(self, n_feats, channels, filters, heads, layers, kernel, dropout, window_size, enc_dim, spk_dim, use_ref_t,
+                 dec_dim, beta_min, beta_max, *, precision="fp32x3"):
+        super().__init__()
+        self.n_feats, self.channels, self.filters, self.heads, self.layers = n_feats, channels, filters, heads, layers
+        self.kernel, self.dropout, self.window_size, self.enc_dim, self.spk_dim = kernel, dropout, window_size, enc_dim, spk_dim
+        self.use_ref_t, self.dec_dim, self.beta_min, self.beta_max = use_ref_t, dec_dim, beta_min, beta_max
+        self.encoder = FwdDiffusion(n_feats, channels, filters, heads, layers, kernel, dropout, window_size, enc_dim,
+                                    precision=precision)
+        self.decoder = Diffusion(n_feats, dec_dim, spk_dim, use_ref_t, beta_min, beta_max, precision=precision)
+
+    def load_encoder(self, enc_path):                                               # :77-79
+        enc_dict = torch.load(enc_path, map_location=lambda loc, storage: loc)
+        self.encoder.load_state_dict(enc_dict, strict=False)
+
+    @torch.no_grad()
+    def forward(self, x, x_lengths, x_ref, x_ref_lengths, c, n_timesteps, mode="ml"):   # :82-127
+        x, x_lengths = self.relocate_input([x, x_lengths])
+        x_ref, x_ref_lengths, c = self.relocate_input([x_ref, x_ref_lengths, c])
+        x_mask = sequence_mask(x_lengths).unsqueeze(1).to(x.dtype)
+        x_ref_mask = sequence_mask(x_ref_lengths).unsqueeze(1).to(x_ref.dtype)
+        mean = self.encoder(x, x_mask)
+        mean_ref = self.encoder(x_ref, x_ref_mask)
+        return convert_from_encoder(self.decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode)
+
+    def compute_loss(self, x, x_lengths, x_ref, c):                                 # :129-144
+        x, x_lengths, x_ref, c = self.relocate_input([x, x_lengths, x_ref, c])
+        x_mask = sequence_mask(x_lengths).unsqueeze(1).to(x.dtype)
+        mean = self.encoder(x, x_mask).detach()
+        mean_ref = self.encoder(x_ref, x_mask).detach()                            # the reference uses x_mask here (:142)
+        return self.decoder.compute_loss(x, x_mask, mean, x_ref, mean_ref, c)

@@ -367,3 +367,67 @@ def synthetic_diffvc_inputs(B: int, T: int, T_ref: int, n_feats: int = 80, seed:
     mask = (torch.arange(T)[None, :] < lens("vc_len", T)[:, None]).to(torch.float32)[:, None, :]
     ref_mask = (torch.arange(T_ref)[None, :] < lens("vc_reflen", T_ref)[:, None]).to(torch.float32)[:, None, :]
     return z, mask, mean, ref, ref_mask, mean_ref, c
+
+
+# ---------------------------------------------------------------------------------------------
+# DiffVC encoder side: FwdDiffusion = MelEncoder + PostNet (DiffVC/model/vc.py:19-48, postnet.py:15-53)
+# ---------------------------------------------------------------------------------------------
+def postnet_param_spec(dim: int = 128, prefix: str = ""):
+    """Ordered {name: shape} of PostNet(dim).state_dict() (DiffVC/model/postnet.py:40-45): 14 tensors."""
+    spec = {f"{prefix}init_conv.weight": (dim, 1, 1, 1), f"{prefix}init_conv.bias": (dim,)}
+    for blk in ("block1", "block2"):
+        q = f"{prefix}res_block.{blk}.block"
+        spec.update({f"{q}.0.weight": (dim, dim, 7, 7), f"{q}.0.bias": (dim,), f"{q}.1.weight": (dim,), f"{q}.1.bias": (dim,)})
+    spec.update({f"{prefix}res_block.res.weight": (dim, dim, 1, 1), f"{prefix}res_block.res.bias": (dim,),
+                 f"{prefix}final_conv.weight": (1, dim, 1, 1), f"{prefix}final_conv.bias": (1,)})
+    return spec
+
+
+def synthetic_postnet_state_dict(dim: int = 128, seed: int = 1234, prefix: str = ""):
+    """Seeded PostNet weights at PyTorch's default init scale (conv weights and biases uniform +-1/sqrt(fan_in)); the
+    GroupNorm affine is perturbed away from (1, 0) so that gamma / beta handling is exercised."""
+    sd = {}
+    for name, shape in postnet_param_spec(dim, prefix).items():
+        if ".block.1." in name:
+            sd[name] = (1.0 if name.endswith("weight") else 0.0) + 0.1 * synthetic_tensor(seed, "postnet/" + name, shape)
+        else:
+            wshape = postnet_param_spec(dim, prefix)[name[:-len("bias")] + "weight"] if name.endswith("bias") else shape
+            fan_in = int(math.prod(wshape[1:]))
+            sd[name] = synthetic_tensor(seed, "postnet/" + name, shape, "uniform") / math.sqrt(fan_in)
+    return sd
+
+
+DIFFVC_MODEL_ARGS = (80, 192, 768, 2, 6, 3, 0.1, 4, 128, 128, True, 256, 0.05, 20.0)   # DiffVC/inference.ipynb, params.py
+
+
+def mel_encoder_param_spec(n_feats=80, ch=192, filt=768, n_heads=2, n_layers=6, kernel=3, window=4, prefix=""):
+    """Ordered {name: shape} of DiffVC's MelEncoder.state_dict() (DiffVC/model/encoder.py:258-277)."""
+    s = {f"{prefix}init_proj.weight": (ch, n_feats, 1), f"{prefix}init_proj.bias": (ch,)}
+    for i in range(3):
+        q = f"{prefix}prenet"
+        s.update({f"{q}.conv_layers.{i}.weight": (ch, ch, 5), f"{q}.conv_layers.{i}.bias": (ch,),
+                  f"{q}.norm_layers.{i}.gamma": (ch,), f"{q}.norm_layers.{i}.beta": (ch,)})
+    s.update({f"{prefix}prenet.proj.weight": (ch, ch, 1), f"{prefix}prenet.proj.bias": (ch,)})
+    for i in range(n_layers):
+        a = f"{prefix}encoder.attn_layers.{i}"
+        s.update({f"{a}.emb_rel_k": (1, 2 * window + 1, ch // n_heads), f"{a}.emb_rel_v": (1, 2 * window + 1, ch // n_heads)})
+        for c in ("conv_q", "conv_k", "conv_v", "conv_o"):
+            s.update({f"{a}.{c}.weight": (ch, ch, 1), f"{a}.{c}.bias": (ch,)})
+        e = f"{prefix}encoder"
+        s.update({f"{e}.norm_layers_1.{i}.gamma": (ch,), f"{e}.norm_layers_1.{i}.beta": (ch,),
+                  f"{e}.ffn_layers.{i}.conv_1.weight": (filt, ch, kernel), f"{e}.ffn_layers.{i}.conv_1.bias": (filt,),
+                  f"{e}.ffn_layers.{i}.conv_2.weight": (ch, filt, kernel), f"{e}.ffn_layers.{i}.conv_2.bias": (ch,),
+                  f"{e}.norm_layers_2.{i}.gamma": (ch,), f"{e}.norm_layers_2.{i}.beta": (ch,)})
+    s.update({f"{prefix}term_proj.weight": (n_feats, ch, 1), f"{prefix}term_proj.bias": (n_feats,)})
+    return s
+
+
+def diffvc_model_param_spec(args=DIFFVC_MODEL_ARGS):
+    """Ordered {name: shape} of the whole DiffVC(*args).state_dict() (DiffVC/model/vc.py:52-75): `encoder.encoder.*`
+    (MelEncoder), `encoder.postnet.*` (PostNet), `decoder.estimator.*` - 346 tensors, 126,259,128 parameters."""
+    n_feats, ch, filt, heads, layers, kernel, _, window, enc_dim, spk_dim, use_ref_t, dec_dim, bmin, bmax = args
+    spec = mel_encoder_param_spec(n_feats, ch, filt, heads, layers, kernel, window, prefix="encoder.encoder.")
+    spec.update(postnet_param_spec(enc_dim, prefix="encoder.postnet."))
+    dec = diffvc_param_spec(DiffVCConfig(n_feats, dec_dim, spk_dim, use_ref_t, bmin, bmax))
+    spec.update({"decoder." + k: v for k, v in dec.items()})
+    return spec
