@@ -89,6 +89,13 @@ def test_unsupported_postnet_configs_are_rejected(sbk_lib, dim, groups):
         PostNet(dim, groups)
 
 
+@pytest.mark.parametrize("dim", [64, 128, 256, 512])
+def test_supported_postnet_dims_are_accepted(sbk_lib, dim):
+    """dim 64, 128 or a multiple of 256 (8 GroupNorm groups of 8, 16 or a multiple of 32 channels) creates a handle."""
+    from speech_backbones_b200.postnet import PostNet
+    assert PostNet(dim).dim == dim
+
+
 def test_cpu_tensors_raise(sbk_lib):
     from speech_backbones_b200.diffvc import FwdDiffusion
     from speech_backbones_b200.postnet import PostNet
