@@ -204,6 +204,15 @@ size_t sbk_vocoder_workspace_bytes(const sbk_vocoder* v, int B, int T);
  * asynchronous on `stream`. */
 int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav, int B, int T, void* stream);
 int64_t sbk_vocoder_last_launch_count(const sbk_vocoder* v);
+/* test hook: when on, sbk_vocoder_forward copies every tensor it writes right after the launch that wrote it (the workspace
+ * buffers are reused within a call) into a per-name device buffer; the copies do not count as launches.  Names in launch
+ * order: mel_in, conv_pre, ups.i.{z,x,a}, resblocks.n.convs1.d, resblocks.n.convs2.d.x (and .a for d < 2), mrf.i, wav.
+ * Activations keep the kernel layout [B][C/4][L][4]; wav is [B][1][L]. */
+int sbk_vocoder_debug_capture(sbk_vocoder* v, int on);
+int sbk_vocoder_debug_num(const sbk_vocoder* v);                                  /* names captured by the last forward */
+const char* sbk_vocoder_debug_name(const sbk_vocoder* v, int i);
+/* copy a captured tensor to `dst` (host or device); returns its element count through *numel; dst may be NULL to query it */
+int sbk_vocoder_debug_read(sbk_vocoder* v, const char* name, float* dst, int64_t* numel);
 
 /* ---- the module in front of the glue (SURVEY.md 8f rank 4): the Grad-TTS text encoder -------------------------------
  * TextEncoder (Grad-TTS/model/text_encoder.py:281-326): embedding, ConvReluNorm prenet, relative-position transformer

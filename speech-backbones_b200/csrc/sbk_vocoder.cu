@@ -147,6 +147,10 @@ struct sbk_vocoder {
     void* mem = nullptr; size_t cap = 0;
     bool is_packed = false;
     int64_t last_launches = 0;
+    // test hook (sbk_vocoder_debug_*): per-name snapshots of the last forward's intermediates, in launch order
+    struct Snap { std::string name; float* buf; size_t cap, numel; };
+    bool capture = false;
+    std::vector<Snap> snaps;
     int n_res() const { return cfg.n_kernels; }
 };
 
@@ -202,6 +206,7 @@ extern "C" void sbk_vocoder_destroy(sbk_vocoder* v) {
     for (auto& kv : v->packed) cudaFree(kv.second);
     if (v->zero) cudaFree(v->zero);
     if (v->mem) cudaFree(v->mem);
+    for (auto& sn : v->snaps) cudaFree(sn.buf);
     delete v;
 }
 
@@ -328,40 +333,101 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
         const int k = launch_conv_tc(p, s);
         if (k < 0) rcl = -1; else n += k;
     };
+    // debug capture: the workspace buffers are overwritten within the call, so each written tensor is copied (stream-ordered)
+    // right after its launch into a per-name buffer.  The copies are not launches and do not count in last_launches.
+    size_t nsnap = 0;
+    cudaError_t snap_err = cudaSuccess;
+    // (the name is pre + suf, put together only when capturing)
+    auto snap = [&](const std::string& pre, const char* suf, const float* src, size_t numel) {
+        if (!v->capture || snap_err != cudaSuccess) return;
+        if (nsnap == v->snaps.size()) v->snaps.push_back({std::string(), nullptr, 0, 0});
+        sbk_vocoder::Snap& sn = v->snaps[nsnap++];
+        sn.name = pre + suf; sn.numel = numel;
+        if (numel > sn.cap) {
+            cudaFree(sn.buf); sn.buf = nullptr; sn.cap = 0;
+            if ((snap_err = cudaMalloc(&sn.buf, numel * sizeof(float))) != cudaSuccess) { sn.buf = nullptr; sn.numel = 0; return; }
+            sn.cap = numel;
+        }
+        snap_err = cudaMemcpyAsync(sn.buf, src, numel * sizeof(float), cudaMemcpyDeviceToDevice, s);
+    };
+    const size_t bn = (size_t)B;
     k_voc_mel_in<<<ew_grid((long long)B * (c.num_mels / 4) * T), 256, 0, s>>>(mel, melc, B, c.num_mels, T); ++n;
+    snap("mel_in", "", melc, bn * c.num_mels * T);
     int ch = c.upsample_initial_channel; int L = T;
     // conv_pre + the first stage's leaky_relu (models.py:105,107)
     conv(G_C1K7, "conv_pre", melc, c.num_mels, ch, L, 1, SA, 1, nullptr, nullptr);
+    snap("conv_pre", "", SA, bn * ch * L);
     int rb = 0;
     for (int i = 0; i < c.n_ups; ++i) {
         const int u = c.upsample_rates[i], k = c.upsample_kernel_sizes[i], co = ch / 2;
         const std::string up = "ups." + std::to_string(i);
         conv(G_PW, up, SA, ch, k * co, L, 1, Z, 0, nullptr, nullptr);                           // Z[i][t*co + c] (models.py:108)
+        snap(up, ".z", Z, bn * k * co * L);
         const int Lo = L * u;
         k_voc_ct_fold<<<ew_grid((long long)B * (co / 4) * Lo), 256, 0, s>>>(Z, W(up + ".bias"), X0, A0, B, co, L, u, kSlope); ++n;
+        snap(up, ".x", X0, bn * co * Lo); snap(up, ".a", A0, bn * co * Lo);
         ch = co; L = Lo;
+        const size_t na = bn * ch * L;
         for (int j = 0; j < 3; ++j, ++rb) {
             const int geom = voc_geom(c.resblock_kernel_sizes[j]);
             const std::string rp = "resblocks." + std::to_string(rb);
             // per dilation d: xt = conv2(lrelu(conv1_d(lrelu(x)))); x = xt + x   (models.py:42-47)
             conv(geom, rp + ".convs1.0", A0, ch, ch, L, c.resblock_dilations[j][0], Hb, 1, nullptr, nullptr);
+            snap(rp, ".convs1.0", Hb, na);
             conv(geom, rp + ".convs2.0", Hb, ch, ch, L, 1, X1, 0, X0, A1);
+            snap(rp, ".convs2.0.x", X1, na); snap(rp, ".convs2.0.a", A1, na);
             conv(geom, rp + ".convs1.1", A1, ch, ch, L, c.resblock_dilations[j][1], Hb, 1, nullptr, nullptr);
+            snap(rp, ".convs1.1", Hb, na);
             conv(geom, rp + ".convs2.1", Hb, ch, ch, L, 1, X2, 0, X1, A2);
+            snap(rp, ".convs2.1.x", X2, na); snap(rp, ".convs2.1.a", A2, na);
             conv(geom, rp + ".convs1.2", A2, ch, ch, L, c.resblock_dilations[j][2], Hb, 1, nullptr, nullptr);
+            snap(rp, ".convs1.2", Hb, na);
             conv(geom, rp + ".convs2.2", Hb, ch, ch, L, 1, R[j], 0, X2, nullptr);
+            snap(rp, ".convs2.2.x", R[j], na);
         }
         // x = xs / num_kernels, then the next consumer's leaky_relu: LRELU_SLOPE before the next ups, torch's default 0.01
         // before conv_post (models.py:107,114-115).  SA is free again: its only reader was this stage's GEMM.
         const long long n4 = (long long)B * (ch / 4) * L;
         k_voc_mrf<<<ew_grid(n4), 256, 0, s>>>(reinterpret_cast<const float4*>(R[0]), reinterpret_cast<const float4*>(R[1]), reinterpret_cast<const float4*>(R[2]),
                                                reinterpret_cast<float4*>(SA), n4, 1.0f / 3.0f, i + 1 < c.n_ups ? kSlope : 0.01f); ++n;
+        if (v->capture) snap("mrf." + std::to_string(i), "", SA, na);
     }
     k_voc_post<<<ew_grid((long long)B * L), 256, 7 * ch * sizeof(float), s>>>(SA, W("conv_post.weight"), W("conv_post.bias"), wav, B, ch, L); ++n;
+    snap("wav", "", wav, bn * L);
+    if (v->capture) {
+        for (size_t i = nsnap; i < v->snaps.size(); ++i) cudaFree(v->snaps[i].buf);
+        v->snaps.resize(nsnap);
+    }
     if (rcl < 0) return sbk_set_error(SBK_ERR_CUDA, "sbk_vocoder_forward: a tensor-core launch was refused (device attribute / geometry)");
+    if (snap_err != cudaSuccess) return sbk_set_error(SBK_ERR_CUDA, "sbk_vocoder_forward: debug capture failed: %s", cudaGetErrorString(snap_err));
     VCU(cudaGetLastError());
     v->last_launches = n;
     return SBK_OK;
 }
 
 extern "C" int64_t sbk_vocoder_last_launch_count(const sbk_vocoder* v) { return v ? v->last_launches : 0; }
+
+extern "C" int sbk_vocoder_debug_capture(sbk_vocoder* v, int on) {
+    if (!v) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_debug_capture: null handle");
+    v->capture = on != 0;
+    return SBK_OK;
+}
+extern "C" int sbk_vocoder_debug_num(const sbk_vocoder* v) { return v ? (int)v->snaps.size() : 0; }
+extern "C" const char* sbk_vocoder_debug_name(const sbk_vocoder* v, int i) {
+    if (!v || i < 0 || i >= (int)v->snaps.size()) return nullptr;
+    return v->snaps[i].name.c_str();
+}
+extern "C" int sbk_vocoder_debug_read(sbk_vocoder* v, const char* name, float* dst, int64_t* numel) {
+    if (!v || !name) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_debug_read: null argument");
+    for (auto& sn : v->snaps) {
+        if (sn.name != name) continue;
+        if (numel) *numel = (int64_t)sn.numel;
+        if (dst && sn.numel > 0) {
+            VCU(cudaSetDevice(v->cfg.device));
+            VCU(cudaDeviceSynchronize());
+            VCU(cudaMemcpy(dst, sn.buf, sn.numel * sizeof(float), cudaMemcpyDefault));
+        }
+        return SBK_OK;
+    }
+    return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_debug_read: no intermediate named '%s'", name);
+}

@@ -67,6 +67,11 @@ class VocoderEngine:
         self.lib.sbk_vocoder_forward.argtypes = [P, P, P, I, I, P]
         self.lib.sbk_vocoder_last_launch_count.argtypes = [P]
         self.lib.sbk_vocoder_last_launch_count.restype = C.c_int64
+        self.lib.sbk_vocoder_debug_capture.argtypes = [P, I]
+        self.lib.sbk_vocoder_debug_num.argtypes = [P]
+        self.lib.sbk_vocoder_debug_name.argtypes = [P, I]
+        self.lib.sbk_vocoder_debug_name.restype = C.c_char_p
+        self.lib.sbk_vocoder_debug_read.argtypes = [P, C.c_char_p, P, C.POINTER(C.c_int64)]
         rates, ks = list(_get(h, "upsample_rates")), list(_get(h, "upsample_kernel_sizes"))
         rk, rd = list(_get(h, "resblock_kernel_sizes")), [list(d) for d in _get(h, "resblock_dilation_sizes")]
         if str(_get(h, "resblock", "1")) != "1":
@@ -86,9 +91,11 @@ class VocoderEngine:
         _check(self.lib.sbk_vocoder_create(C.byref(cfg), C.byref(self.h)), "sbk_vocoder_create")
         self.device = device
         self.num_mels = cfg.num_mels
+        self.rates = rates
         self.hop = 1
         for u in rates:
             self.hop *= u
+        self._last_bt = None
 
     def close(self):
         if getattr(self, "h", None) and self.h.value:
@@ -135,10 +142,45 @@ class VocoderEngine:
                 torch.cuda.empty_cache()
                 rc = self.lib.sbk_vocoder_forward(self.h, _ptr(mel), _ptr(wav), B, T, stream)
             _check(rc, "sbk_vocoder_forward")
+        self._last_bt = (B, T)
         return wav
 
     def last_launch_count(self):
         return int(self.lib.sbk_vocoder_last_launch_count(self.h))
+
+    # ---- test hooks: the intermediates of the last forward run with capture on (sbk_vocoder_debug_*)
+    def debug_capture(self, on=True):
+        _check(self.lib.sbk_vocoder_debug_capture(self.h, 1 if on else 0), "sbk_vocoder_debug_capture")
+
+    def debug_names(self):
+        return [self.lib.sbk_vocoder_debug_name(self.h, i).decode() for i in range(self.lib.sbk_vocoder_debug_num(self.h))]
+
+    def _debug_len(self, name):
+        """signal length of a captured tensor: T before the first transposed conv, times each rate after it"""
+        B, T = self._last_bt
+        parts = name.split(".")
+        if parts[0] in ("mel_in", "conv_pre"):
+            return T
+        if parts[0] == "wav":
+            return T * self.hop
+        stage = int(parts[1]) // 3 if parts[0] == "resblocks" else int(parts[1])
+        done = stage if (parts[0] == "ups" and parts[2] == "z") else stage + 1
+        L = T
+        for u in self.rates[:done]:
+            L *= u
+        return L
+
+    def debug_read(self, name):
+        """captured tensor `name` as a [B, C, L] fp32 CUDA tensor (wav: [B, 1, L])"""
+        n = C.c_int64(0)
+        _check(self.lib.sbk_vocoder_debug_read(self.h, name.encode(), None, C.byref(n)), "sbk_vocoder_debug_read")
+        flat = torch.empty(n.value, dtype=torch.float32, device=f"cuda:{self.device}")
+        _check(self.lib.sbk_vocoder_debug_read(self.h, name.encode(), _ptr(flat), C.byref(n)), "sbk_vocoder_debug_read")
+        B, L = self._last_bt[0], self._debug_len(name)
+        if name == "wav":
+            return flat.view(B, 1, L)
+        Ch = n.value // (B * L)
+        return flat.view(B, Ch // 4, L, 4).permute(0, 1, 3, 2).reshape(B, Ch, L)
 
 
 class Generator(nn.Module):

@@ -233,13 +233,13 @@ def hifigan_param_spec(h=None):
     return spec + [("conv_post.weight", (1, ch, 7)), ("conv_post.bias", (1,))]
 
 
-def synthetic_hifigan_state_dict(seed: int = 1234):
-    """Seeded weights for the HiFi-GAN V1 generator after remove_weight_norm: the reference ships no vocoder checkpoint.
-    He-style scales (std = 1/sqrt(fan_in)) keep the activations O(1) through the 15-conv-deep residual stacks, so the tanh
-    output is neither saturated nor vanishing."""
+def synthetic_hifigan_state_dict(seed: int = 1234, h=None):
+    """Seeded weights for a HiFi-GAN generator (`h`, default V1) after remove_weight_norm: the reference ships no vocoder
+    checkpoint.  He-style scales (std = 1/sqrt(fan_in)) keep the activations O(1) through the 15-conv-deep residual stacks,
+    so the tanh output is neither saturated nor vanishing."""
     import math
     sd = {}
-    for name, shape in hifigan_param_spec():
+    for name, shape in hifigan_param_spec(h):
         g = torch.Generator().manual_seed(_key_seed(seed, "hifigan/" + name))
         if name.endswith(".bias"):
             sd[name] = torch.randn(shape, generator=g) * 0.02

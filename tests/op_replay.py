@@ -14,6 +14,10 @@ For every linear op the replay also computes the magnitude companion A: the same
 
 Rounding noise is nearly the same in every group (each column has C*H samples), so a defect at one tile seam, one halo row
 or one N tile stands out by orders of magnitude even where check 1's worst-case bound is loose (tf32, bf16, fp32x3).
+
+`VocoderReplay` does the same for one HiFi-GAN vocoder call (oracle/hifigan_oracle.py semantics): its [B, C, L] signals
+are grouped by sample, 128-sample tile, within-tile phase and N-tile block (`uniformity1d`), and its elementwise kernels
+(mel layout, transposed-conv fold, LeakyReLU second outputs, MRF mean) must reproduce their fp32 arithmetic bit for bit.
 """
 from __future__ import annotations
 
@@ -138,23 +142,82 @@ def uniformity(err, A, Alin=None, min_group=MIN_GROUP, valid=None):
             ok = full & (classes[name] == cls)
             if ok.sum() < 2:
                 continue
-            e = (en[ok] / an[ok]).double()
-            i = int(e.argmax())
-            med = torch.cat([e[:i], e[i + 1:]]).median().item()
-            emax = e[i].item()
-            r = 0.0 if emax == 0.0 else (math.inf if med == 0.0 else emax / med)
+            r, i = _max_over_median((en[ok] / an[ok]).double())
             if r > worst:
                 worst, where = r, f"{name}[{int(ok.nonzero()[i])}]"
     return worst, where
 
 
-def check(got, ref, A, kap, floor=0.0, Alin=None, groups=True, min_group=MIN_GROUP):
-    """-> (elem, unif, where): elem = max |err| / (kappa A + floor) (<= 1 passes), unif = worst max/median group ratio."""
+def _max_over_median(e):
+    """-> (max e / median of the others, index of the max)"""
+    i = int(e.argmax())
+    med = torch.cat([e[:i], e[i + 1:]]).median().item()
+    emax = e[i].item()
+    return (0.0 if emax == 0.0 else (math.inf if med == 0.0 else emax / med)), i
+
+
+# ---- check 2 on 1-D signals [B, C, L] (the vocoder's Conv1d, GEMM and fold outputs) -------------------------------------
+# The Conv1d / 1x1 wgmma kernels tile a signal into TPX = 128-sample strips per N-tile block of output channels
+# (sbk_conv_tc.cu).  A defect at a strip seam, in a halo, in one warpgroup half or descriptor offset, or in one N tile shows
+# up in one of these groups.  e_g = ||err_g|| / ||Alin_g||: the rounding error scales with the op's own products, while the
+# bias and the ResBlock residual that A also carries vary between samples without adding error beyond one fp32 rounding.
+# Samples within `pad` of either end see zero-padding taps (a different mix of terms); they are left out here and held to
+# check 1, which a stale or non-zero padding value fails many times over.  The same R_UNIFORM applies: on an H100 the
+# vocoder's worst ratio was 2.6 (per-sample groups of the 32-channel last stage, the smallest groups), while one dropped
+# tap term of a K = 704 Conv1d gives ~80 (test_op_replay.py).
+TPX = 128
+
+
+def groupings1d(x, pad, ntile):
+    """[B,C,L] -> {name: fn}: each sample (b, w) over its channels, each 128-sample tile (b, w // 128), each within-tile
+    phase w % 128 over the full interior tiles (a defect that repeats in every tile), each `ntile`-channel block."""
+    B, C, L = x.shape
+    nt = (L + TPX - 1) // TPX
+
+    def tiles(t):
+        return F.pad(t, (0, nt * TPX - L)).view(B, C, nt, TPX)
+    out = {"sample": lambda t: _group_norms(t, (1,)), "tile": lambda t: _group_norms(tiles(t), (1, 3))}
+    inner = [j for j in range(nt) if j * TPX >= pad and (j + 1) * TPX <= L - pad]
+    if inner:
+        lo, hi = inner[0], inner[-1] + 1
+        out["phase"] = lambda t: _group_norms(tiles(t)[:, :, lo:hi], (0, 1, 2))
+    if C % ntile == 0 and C // ntile > 1:
+        out["ntile"] = lambda t: _group_norms(t.reshape(B, C // ntile, ntile, L), (0, 2, 3))
+    return out
+
+
+def uniformity1d(err, Alin, pad=0, ntile=128, min_group=MIN_GROUP):
+    """max over the 1-D groupings of  max_g e_g / median of the other groups' e_g, edge samples left out."""
+    B, C, L = err.shape
+    valid = torch.zeros(L, dtype=torch.float64, device=err.device)
+    valid[pad:max(pad, L - pad)] = 1.0
+    valid = valid.expand(B, C, L)
+    err, Alin = err * valid, Alin.double() * valid
+    worst, where = 0.0, ""
+    for name, fn in groupings1d(err, pad, ntile).items():
+        en, ln, cnt = fn(err), fn(Alin), fn(valid).pow(2).round()
+        ok = (cnt >= min_group) & (ln > 0)
+        if ok.sum() < 2:
+            continue
+        r, i = _max_over_median((en[ok] / ln[ok]).double())
+        if r > worst:
+            worst, where = r, f"{name}[{int(ok.nonzero()[i])}]"
+    return worst, where
+
+
+def check(got, ref, A, kap, floor=0.0, Alin=None, groups=True, min_group=MIN_GROUP, pad=0, ntile=128):
+    """-> (elem, unif, where): elem = max |err| / (kappa A + floor) (<= 1 passes), unif = worst max/median group ratio.
+    4-D [B,C,H,W] tensors are grouped as images; 3-D [B,C,L] tensors as 1-D signals (`pad`, `ntile`: uniformity1d)."""
     got, ref, A = got.double(), ref.double(), A.double()
     err = (got - ref).abs()
     tiny = torch.finfo(torch.float32).tiny
     elem = (err / (kap * A + floor + tiny)).max().item()
-    unif, where = uniformity(err, A, Alin, min_group) if groups and err.dim() == 4 else (0.0, "")
+    if groups and err.dim() == 4:
+        unif, where = uniformity(err, A, Alin, min_group)
+    elif groups and err.dim() == 3:
+        unif, where = uniformity1d(err, A if Alin is None else Alin, pad, ntile, min_group)
+    else:
+        unif, where = 0.0, ""
     return elem, unif, where
 
 
@@ -484,4 +547,207 @@ class Replay:
             elem, unif, where = check(got, ref, A, k, floor, Alin, groups=Alin is not False)
             rows.append((name, elem, unif, where))
         assert any(r[0] == "estimator.out" for r in rows), "the plan no longer names estimator.out"
+        return rows
+
+
+# ---- the HiFi-GAN vocoder (csrc/sbk_vocoder.cu), replayed op by op -------------------------------------------------------
+# Every Conv1d, the transposed-conv GEMMs and conv_post are recomputed in float64 from the GPU's captured inputs with the
+# semantics of oracle/hifigan_oracle.py.  The Conv1d kernels (k_conv_tc<G_C1K*>) and the GEMMs (k_conv_tc<G_PW>) run tf32
+# operands with fp32 accumulation: kappa("tf32", K) with K = Cin * taps.  Their epilogue then adds the fp32 bias (and the
+# ResBlock residual) and applies LeakyReLU: each add is one fp32 rounding of <= 2^-24 of a value bounded by A, and x * 0.1f
+# one more; LeakyReLU is 1-Lipschitz, so it does not enlarge the error it receives.
+EPS_ADD = 2 ** -24
+# conv_post + tanh (k_voc_post) runs on CUDA cores: a chain of 7 * C fmaf from the bias, gamma_K = K * 2^-24 of A.  tanh is
+# 1-Lipschitz, so that bound carries through it; tanhf adds its own error, at most 2 ulp (CUDA C Programming Guide,
+# "Mathematical Functions": tanhf, maximum ulp error 2), and one ulp of y is at most 2^-23 |y|.
+TANHF_ULP = 2
+VOC_SLOPE = 0.1                         # LRELU_SLOPE (models.py:10); 0.01 (torch's default) before conv_post
+
+
+def conv1d_ntile(C):
+    """N-tile width of k_conv_tc for a Conv1d with C output channels (sbk_conv_tc.cu conv_tc_ntile)"""
+    return 128 if C % 128 == 0 else (64 if C % 64 == 0 else 32)
+
+
+def gemm_ntile(C):
+    return 128 if C % 128 == 0 else 64
+
+
+def lrelu_f32(x, slope):
+    """the kernels' LeakyReLU, bit for bit: x > 0 ? x : x * slope (fp32)"""
+    x = x.float()
+    return torch.where(x > 0, x, x * torch.tensor(slope, dtype=torch.float32, device=x.device))
+
+
+def ct_fold(z, bias, u):
+    """k_voc_ct_fold in fp32: ConvTranspose1d(k = 2u, stride u, padding u/2) as a 2-tap overlap-add of the GEMM output
+    z [B, 2u*C, Lin] (channel t*C + c).  Output o (o + u/2 = u*i1 + t1) is (bias + z[t1, i1]) + z[t1 + u, i1 - 1], each
+    tap skipped where its input sample lies outside the signal."""
+    B, KC, Lin = z.shape
+    Cc, p = KC // (2 * u), u // 2
+    zz = z.float().view(B, 2 * u, Cc, Lin).permute(0, 2, 1, 3)              # [B, C, tap, Lin]
+    o = torch.arange(Lin * u, device=z.device)
+    i1, t1 = (o + p) // u, (o + p) % u
+    x = bias.float()[None, :, None].expand(B, Cc, Lin * u).clone()
+    m = i1 < Lin
+    x[:, :, m] = x[:, :, m] + zz[:, :, t1[m], i1[m]]
+    m = i1 >= 1
+    x[:, :, m] = x[:, :, m] + zz[:, :, t1[m] + u, i1[m] - 1]
+    return x
+
+
+def _bitwise(got, ref):
+    """(elem, unif, where) of an op that must reproduce `ref` bit for bit: elem 0 when equal, else inf"""
+    same = got.shape == ref.shape and torch.equal(got.float(), ref.float())
+    return (0.0 if same else math.inf), 0.0, "bitwise"
+
+
+class VocoderReplay:
+    """Run one vocoder call with debug capture and judge every captured op against its float64 (or bitwise) replay.
+    `sd` holds the effective weights the engine was loaded with; `h` its config (oracle/hifigan_oracle.py keys)."""
+
+    def __init__(self, eng, sd, h, mel, dev="cuda"):
+        self.eng, self.h, self.dev = eng, h, dev
+        self.p = {k: v.to(dev, torch.float64) for k, v in sd.items()}
+        self.mel = mel.to(dev, torch.float32).contiguous()
+        eng.debug_capture(True)
+        try:
+            self.wav = eng.forward(self.mel)
+            torch.cuda.synchronize()
+        finally:
+            eng.debug_capture(False)
+        self.names = eng.debug_names()
+        self.cap = {}
+
+    def got(self, name):
+        if name not in self.cap:
+            assert name in self.names, f"{name}: the vocoder did not capture it"
+            self.cap[name] = self.eng.debug_read(name)
+        return self.cap[name]
+
+    def stage_input(self, i):
+        """the activation operand a stage's transposed conv reads: lrelu(conv_pre) or lrelu(the previous MRF mean)"""
+        return self.got("conv_pre" if i == 0 else f"mrf.{i - 1}")
+
+    def _conv(self, x, w, b, dil, addin=None):
+        """(ref, A, Alin, floor): Conv1d 'same' padding + bias (+ residual) on float64 copies, and its magnitude companions"""
+        x = x.double()
+        pad = (w.shape[2] - 1) * dil // 2
+        ref = F.conv1d(x, w, b, padding=pad, dilation=dil)
+        Alin = F.conv1d(x.abs(), w.abs(), None, padding=pad, dilation=dil)
+        A = Alin + b.abs()[None, :, None]
+        if addin is not None:
+            ref, A = ref + addin.double(), A + addin.double().abs()
+        return ref, A, Alin, FLOOR_PER_W * w.abs().flatten(1).sum(1).max().item()
+
+    def conv_op(self, name):
+        """conv_pre, resblocks.n.convs1.d (-> lrelu), resblocks.n.convs2.d.x (+ residual): the Conv1d kernels"""
+        p, h = self.p, self.h
+        if name == "conv_pre":
+            x, w, b, dil, addin, act = self.got("mel_in"), p["conv_pre.weight"], p["conv_pre.bias"], 1, None, True
+        else:
+            _, n, grp, d = name.split(".")[:4]
+            n, d = int(n), int(d)
+            st, j = n // 3, n % 3
+            pre = f"resblocks.{n}"
+            w, b = p[f"{pre}.{grp}.{d}.weight"], p[f"{pre}.{grp}.{d}.bias"]
+            if grp == "convs1":
+                # input lrelu(x): the fold's second output, then each convs2's
+                x = self.got(f"ups.{st}.a" if d == 0 else f"{pre}.convs2.{d - 1}.a")
+                dil, addin, act = h["resblock_dilation_sizes"][j][d], None, True
+            else:
+                x, dil, act = self.got(f"{pre}.convs1.{d}"), 1, False
+                addin = self.got(f"ups.{st}.x" if d == 0 else f"{pre}.convs2.{d - 1}.x")
+        ref, A, Alin, floor = self._conv(x, w, b, dil, addin)
+        if act:
+            ref = F.leaky_relu(ref, VOC_SLOPE)
+        K = w.shape[1] * w.shape[2]
+        # bias add (+ residual add) + LeakyReLU's product, one fp32 rounding each
+        k = kappa("tf32", K, extra=EPS_ADD * (1 + (addin is not None) + act))
+        pad = (w.shape[2] - 1) * dil // 2
+        return self.got(name), ref, A, k, floor, Alin, pad, conv1d_ntile(w.shape[0])
+
+    def gemm_op(self, i):
+        """ups.i.z: the transposed conv's 1x1 GEMM to k*co channels, channel t*co + c (sbk_vocoder_pack)"""
+        w = self.p[f"ups.{i}.weight"]                                       # [ci, co, k]
+        ci, co, k = w.shape
+        g = w.permute(2, 1, 0).reshape(k * co, ci, 1)                       # [t*co + c][ci]
+        x = self.stage_input(i).double()
+        ref, Alin = F.conv1d(x, g), F.conv1d(x.abs(), g.abs())
+        floor = FLOOR_PER_W * g.abs().flatten(1).sum(1).max().item()
+        return self.got(f"ups.{i}.z"), ref, Alin, kappa("tf32", ci), floor, Alin, 0, gemm_ntile(k * co)
+
+    def fold_vs_convt(self, i):
+        """ups.i.x against torch's ConvTranspose1d (models.py:108) on the captured GEMM input: the GEMM's bound plus the
+        fold's two fp32 adds"""
+        u, k = self.h["upsample_rates"][i], self.h["upsample_kernel_sizes"][i]
+        w, b = self.p[f"ups.{i}.weight"], self.p[f"ups.{i}.bias"]
+        x = self.stage_input(i).double()
+        ref = F.conv_transpose1d(x, w, b, stride=u, padding=(k - u) // 2)
+        Alin = F.conv_transpose1d(x.abs(), w.abs(), None, stride=u, padding=(k - u) // 2)
+        floor = 2 * FLOOR_PER_W * w.abs().sum(dim=(0, 2)).max().item()
+        # the first / last u/2 samples receive one tap instead of two; the fold is elementwise (no N tiles of its own)
+        return (self.got(f"ups.{i}.x"), ref, Alin + b.abs()[None, :, None], kappa("tf32", w.shape[0], extra=2 * EPS_ADD),
+                floor, Alin, u // 2, w.shape[1])
+
+    def wav_op(self):
+        nu = len(self.h["upsample_rates"])
+        x = self.got(f"mrf.{nu - 1}").double()
+        w, b = self.p["conv_post.weight"], self.p["conv_post.bias"]
+        pre = F.conv1d(x, w, b, padding=3)
+        A = F.conv1d(x.abs(), w.abs(), b.abs(), padding=3)
+        kA = w.shape[1] * w.shape[2] * 2 ** -24 * A
+        ref = torch.tanh(pre)
+        # per element: the FMA chain's bound through tanh, plus tanhf's 2 ulp of a result no larger than |ref| + kappa A
+        bound = kA + TANHF_ULP * 2 ** -23 * (ref.abs() + kA) + torch.finfo(torch.float32).tiny
+        return self.got("wav"), ref, bound
+
+    def run(self):
+        """-> rows (name, elem, unif, where); raises on a captured name this replay does not know"""
+        rows = []
+        nu = len(self.h["upsample_rates"])
+        for name in self.names:
+            parts = name.split(".")
+            if name == "mel_in":
+                rows.append((name,) + _bitwise(self.got(name), self.mel))
+                continue
+            if name == "wav":
+                got, ref, bound = self.wav_op()
+                # CUDA-core chain, no tiles; tanhf's ulp error is not proportional to A, so check 1 only
+                rows.append((name,) + check(got, ref, bound, 1.0, groups=False))
+                continue
+            if parts[0] == "mrf" and len(parts) == 2:
+                i = int(parts[1])
+                r = [self.got(f"resblocks.{3 * i + j}.convs2.2.x").float() for j in range(3)]
+                inv = torch.tensor(1.0 / 3.0, dtype=torch.float32, device=r[0].device)
+                ref = lrelu_f32(((r[0] + r[1]) + r[2]) * inv, VOC_SLOPE if i + 1 < nu else 0.01)
+                rows.append((name,) + _bitwise(self.got(name), ref))
+                continue
+            if parts[0] == "ups" and len(parts) == 3 and parts[2] in ("z", "x", "a"):
+                i = int(parts[1])
+                if parts[2] == "z":
+                    r = self.gemm_op(i)
+                elif parts[2] == "a":
+                    rows.append((name,) + _bitwise(self.got(name), lrelu_f32(self.got(f"ups.{i}.x"), VOC_SLOPE)))
+                    continue
+                else:
+                    u = self.h["upsample_rates"][i]
+                    ref = ct_fold(self.got(f"ups.{i}.z"), self.p[f"ups.{i}.bias"].float(), u)
+                    rows.append((name,) + _bitwise(self.got(name), ref))
+                    got, ref, A, k, floor, Alin, pad, nt = self.fold_vs_convt(i)
+                    rows.append((name + "~convT",) + check(got, ref, A, k, floor, Alin, pad=pad, ntile=nt))
+                    continue
+            elif name == "conv_pre" or (parts[0] == "resblocks" and len(parts) >= 4 and (
+                    (parts[2] == "convs1" and len(parts) == 4) or (parts[2] == "convs2" and parts[4:] == ["x"]))):
+                r = self.conv_op(name)
+            elif parts[0] == "resblocks" and parts[2:3] == ["convs2"] and parts[4:] == ["a"] and int(parts[3]) < 2:
+                x = self.got(name[:-2] + ".x")
+                rows.append((name,) + _bitwise(self.got(name), lrelu_f32(x, VOC_SLOPE)))
+                continue
+            else:
+                raise AssertionError(f"unknown vocoder op '{name}': add a replay for it")
+            got, ref, A, k, floor, Alin, pad, nt = r
+            assert got.shape == ref.shape, f"{name}: captured {tuple(got.shape)} vs replay {tuple(ref.shape)}"
+            rows.append((name,) + check(got, ref, A, k, floor, Alin, pad=pad, ntile=nt))
+        assert rows and rows[-1][0] == "wav", "the vocoder no longer captures wav last"
         return rows

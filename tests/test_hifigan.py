@@ -49,7 +49,8 @@ def test_parameter_tree_matches_reference_names():
 def test_vocoder_symbols_exported(sbk_lib):
     for sym in ("sbk_vocoder_create", "sbk_vocoder_destroy", "sbk_vocoder_num_weights", "sbk_vocoder_weight_name",
                 "sbk_vocoder_set_weight", "sbk_vocoder_pack", "sbk_vocoder_workspace_bytes", "sbk_vocoder_forward",
-                "sbk_vocoder_last_launch_count"):
+                "sbk_vocoder_last_launch_count", "sbk_vocoder_debug_capture", "sbk_vocoder_debug_num", "sbk_vocoder_debug_name",
+                "sbk_vocoder_debug_read"):
         assert hasattr(sbk_lib, sym), sym
 
 
@@ -106,3 +107,71 @@ def test_vocoder_weight_norm_checkpoint_path(hg_golden):
     g.remove_weight_norm()
     b = g(mel)
     assert torch.isfinite(a).all() and rel_l2(b.cpu(), a.cpu()) <= VOC_TOL
+
+
+# A generator valid for HiFi-GAN and accepted by sbk_vocoder_create that reaches the Conv1d strip's limits, which V1 does
+# not: K=3, d=32 gives a 64-sample halo (pad 32: an interior strip fills all 128 + 64 columns), K=7, d=10 and K=11, d=6 a
+# 60-sample one; stride-4 transposed convs (k = 8: 2-tap folds with u = 4, GEMMs to 8 * co channels).
+HIFIGAN_EDGE = dict(HIFIGAN_V1, upsample_rates=[4, 4, 4, 4], upsample_kernel_sizes=[8, 8, 8, 8],
+                    resblock_dilation_sizes=[[1, 8, 32], [1, 5, 10], [1, 3, 6]])
+
+
+def _voc_create_rc(lib, h):
+    import ctypes as C
+    from speech_backbones_b200.hifigan import SbkVocoderConfig
+    lib.sbk_vocoder_create.argtypes = [C.POINTER(SbkVocoderConfig), C.POINTER(C.c_void_p)]
+    lib.sbk_vocoder_destroy.argtypes = [C.c_void_p]
+    lib.sbk_vocoder_destroy.restype = None
+    cfg = SbkVocoderConfig()
+    cfg.device, cfg.num_mels, cfg.upsample_initial_channel = 0, h["num_mels"], h["upsample_initial_channel"]
+    cfg.n_ups, cfg.n_kernels = len(h["upsample_rates"]), 3
+    for i, (u, k) in enumerate(zip(h["upsample_rates"], h["upsample_kernel_sizes"])):
+        cfg.upsample_rates[i], cfg.upsample_kernel_sizes[i] = u, k
+    for j in range(3):
+        cfg.resblock_kernel_sizes[j] = h["resblock_kernel_sizes"][j]
+        for d in range(3):
+            cfg.resblock_dilations[j][d] = h["resblock_dilation_sizes"][j][d]
+    v = C.c_void_p()
+    rc = lib.sbk_vocoder_create(C.byref(cfg), C.byref(v))
+    if rc == 0:
+        lib.sbk_vocoder_destroy(v)
+    return rc
+
+
+def test_vocoder_create_accepts_and_rejects_at_the_strip_limits(sbk_lib):
+    """sbk_vocoder_create touches no device.  A halo (K-1)*d of 64 samples (the strip's capacity) is accepted and 66 is
+    not; so are a transposed conv with k != 2u, an odd stride, and a stage whose channels are not a multiple of 32."""
+    SBK_ERR_UNSUPPORTED = 4
+    assert _voc_create_rc(sbk_lib, HIFIGAN_V1) == 0
+    assert _voc_create_rc(sbk_lib, HIFIGAN_EDGE) == 0
+    assert _voc_create_rc(sbk_lib, dict(HIFIGAN_V1, resblock_dilation_sizes=[[1, 3, 32], [1, 3, 5], [1, 3, 5]])) == 0
+    rejected = {
+        "halo 66 (K=3, d=33)": dict(HIFIGAN_V1, resblock_dilation_sizes=[[1, 3, 33], [1, 3, 5], [1, 3, 5]]),
+        "halo 70 (K=11, d=7)": dict(HIFIGAN_V1, resblock_dilation_sizes=[[1, 3, 5], [1, 3, 5], [1, 3, 7]]),
+        "k != 2u": dict(HIFIGAN_V1, upsample_kernel_sizes=[15, 16, 4, 4]),
+        "odd u": dict(HIFIGAN_V1, upsample_rates=[8, 8, 3, 2], upsample_kernel_sizes=[16, 16, 6, 4]),
+        "48 channels": dict(HIFIGAN_V1, upsample_initial_channel=192, upsample_rates=[8, 8],
+                            upsample_kernel_sizes=[16, 16]),
+    }
+    for what, h in rejected.items():
+        assert _voc_create_rc(sbk_lib, h) == SBK_ERR_UNSUPPORTED, what
+
+
+@pytest.mark.gpu
+def test_vocoder_edge_config_vs_oracle():
+    """The strip-limit config end to end against the CPU oracle, at a ragged and at a one-frame input."""
+    from speech_backbones_b200.hifigan import VocoderEngine
+    sd = synthetic_hifigan_state_dict(1234, HIFIGAN_EDGE)
+    eng = VocoderEngine(HIFIGAN_EDGE, 0)
+    try:
+        eng.load_state_dict(sd)
+        for B, T in ((2, 17), (1, 1)):
+            mel = torch.randn(B, 80, T, generator=torch.Generator().manual_seed(B * 100 + T))
+            with torch.no_grad():
+                ref = H.generator(sd, mel, HIFIGAN_EDGE)
+            y = eng.forward(mel.cuda()).cpu()
+            err = rel_l2(y, ref)
+            print("vocoder edge config B=%d T=%d rel_l2 %.3e" % (B, T, err))
+            assert y.shape == ref.shape and err <= VOC_TOL
+    finally:
+        eng.close()
