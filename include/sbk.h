@@ -179,7 +179,13 @@ const char* sbk_debug_name(const sbk_handle* h, int i);
  * called as `vocoder.forward(y_dec)` at Grad-TTS/inference.py:81 after `remove_weight_norm()` (:63).  The fields below are that
  * JSON's; weights are the generator's state_dict AFTER remove_weight_norm ("conv_pre.weight" [C0,num_mels,7],
  * "ups.i.weight" [Cin,Cout,k], "resblocks.n.convs{1,2}.j.weight" [C,C,k], "conv_post.weight" [1,C,7] and the biases).
- * Dense contractions run on wgmma with tf32 operands and fp32 accumulation; everything else is fp32. */
+ * Dense contractions run on wgmma, by default with tf32 operands and fp32 accumulation; everything else is fp32.
+ * sbk_vocoder_set_precision selects the operand arithmetic of the convs and transposed convs:
+ *   SBK_PREC_TF32 (a fresh handle)  tf32 operands;
+ *   SBK_PREC_FP32X3 (and FP32, which maps to it)  fp32-class: x*w = x_hi*w_hi + one f16 correction MMA, chunked accumulation;
+ *   SBK_PREC_BF16  bf16 weights and bf16 conv inputs (the LeakyReLU operands); the residual stream stays fp32.
+ * In every mode conv_post + tanh, the transposed convs' overlap-add, the MRF mean and the waveform are fp32, and the forward
+ * makes the same launches. */
 typedef struct sbk_vocoder sbk_vocoder;
 typedef struct sbk_vocoder_config {
     int32_t device;
@@ -199,6 +205,11 @@ const char* sbk_vocoder_weight_name(const sbk_vocoder* v, int i);
 /* load_state_dict(strict) + remove_weight_norm (inference.py:61-63): one call per effective tensor, host or device fp32 */
 int sbk_vocoder_set_weight(sbk_vocoder* v, const char* name, const void* data, const int64_t* shape, int ndim);
 int sbk_vocoder_pack(sbk_vocoder* v);
+/* SBK_PREC_* (host logic only, no device work).  Drops the packed weights: sbk_vocoder_forward returns SBK_ERR_STATE until
+ * sbk_vocoder_pack runs again.  SBK_ERR_UNSUPPORTED for a configuration the mode cannot tile (bf16: num_mels a multiple of
+ * 16); the handle then keeps its previous precision. */
+int sbk_vocoder_set_precision(sbk_vocoder* v, int32_t precision);
+/* device bytes of one forward at (B, T) in the current precision */
 size_t sbk_vocoder_workspace_bytes(const sbk_vocoder* v, int B, int T);
 /* Generator.forward (models.py:104-119): mel [B,num_mels,T] -> wav [B,1,T*prod(upsample_rates)] in (-1,1).  Device pointers,
  * asynchronous on `stream`. */
@@ -207,12 +218,17 @@ int64_t sbk_vocoder_last_launch_count(const sbk_vocoder* v);
 /* test hook: when on, sbk_vocoder_forward copies every tensor it writes right after the launch that wrote it (the workspace
  * buffers are reused within a call) into a per-name device buffer; the copies do not count as launches.  Names in launch
  * order: mel_in, conv_pre, ups.i.{z,x,a}, resblocks.n.convs1.d, resblocks.n.convs2.d.x (and .a for d < 2), mrf.i, wav.
- * Activations keep the kernel layout [B][C/4][L][4]; wav is [B][1][L]. */
+ * Activations keep the kernel layout (sbk_vocoder_debug_op_layout); wav is [B][1][L].  The fp32x3 correction chunks are not
+ * captured: they are a function of the fp32 tensor they accompany. */
 int sbk_vocoder_debug_capture(sbk_vocoder* v, int on);
 int sbk_vocoder_debug_num(const sbk_vocoder* v);                                  /* names captured by the last forward */
 const char* sbk_vocoder_debug_name(const sbk_vocoder* v, int i);
-/* copy a captured tensor to `dst` (host or device); returns its element count through *numel; dst may be NULL to query it */
+/* copy a captured tensor to `dst` (host or device) as fp32, bf16 snapshots widened exactly, element order unchanged; returns
+ * its element count through *numel; dst may be NULL to query it */
 int sbk_vocoder_debug_read(sbk_vocoder* v, const char* name, float* dst, int64_t* numel);
+/* layout of a captured tensor: 1 = fp32 [B][C/4][L][4] (wav: [B][1][L]), 2 = bf16 [B][C/8][L][8] (the conv inputs in the bf16
+ * mode), -1 = no such name */
+int sbk_vocoder_debug_op_layout(const sbk_vocoder* v, const char* name);
 
 /* ---- the module in front of the glue (SURVEY.md 8f rank 4): the Grad-TTS text encoder -------------------------------
  * TextEncoder (Grad-TTS/model/text_encoder.py:281-326): embedding, ConvReluNorm prenet, relative-position transformer

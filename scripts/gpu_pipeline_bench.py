@@ -1,14 +1,17 @@
 """The whole of inference.py's GPU work in libsbk: text encoder -> durations / alignment / prior (sbk_prior_expand) -> N-step
-sampler -> HiFi-GAN vocoder, timed stage by stage with CUDA events (median of 5 after 2 warm-ups).
+sampler -> HiFi-GAN vocoder, timed stage by stage with CUDA events (median of 5 after 2 warm-ups).  The vocoder runs in the
+decoder's precision (fp32x3, tf32 or bf16); the bf16 rows hand it the mel as bfloat16, as a pipeline that keeps its tensors
+in bf16 would.
 
     python scripts/gpu_pipeline_bench.py            # config 1's shape (B=1, 221 tokens, N=10) and a batch (B=32, N=50)
 
-Prints one JSON line per configuration: ms per stage, kernel launches per stage, mel-frames/s of the sampler and the vocoder,
+Prints one JSON line per configuration (with the card's name and power limit): ms per stage, kernel launches per stage, mel-frames/s of the sampler and the vocoder,
 the vocoder's achieved TFLOP/s (307.3 MMAC per mel frame, oracle/hifigan_oracle.py:macs_per_mel_frame) against the measured
 tf32 tensor rate, and the real-time factor at 22.05 kHz (hop 256)."""
 import json
 import os
 import statistics
+import subprocess
 import sys
 
 import torch
@@ -29,11 +32,19 @@ dev = torch.device("cuda", 0)
 enc = TextEncoder(149, 80, 192, 768, 256, 2, 6, 3, 0.1, window_size=4).eval()
 enc.load_state_dict(T.synthetic_weights(1234), strict=True)
 enc = enc.to(dev)
-voc = Generator(HIFIGAN_V1).eval()
-voc.remove_weight_norm()
-voc.load_state_dict(synthetic_hifigan_state_dict(2468), strict=True)
-voc = voc.to(dev)
-decs = {}
+decs, vocs = {}, {}
+q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                   capture_output=True, text=True)
+CARD = {"gpu": torch.cuda.get_device_name(dev), "nvidia_smi": q.stdout.strip()}
+
+
+def vocoder(precision):
+    if precision not in vocs:
+        v = Generator(HIFIGAN_V1, precision=precision).eval()
+        v.remove_weight_norm()
+        v.load_state_dict(synthetic_hifigan_state_dict(2468), strict=True)
+        vocs[precision] = v.to(dev)
+    return vocs[precision]
 
 
 def decoder(precision):
@@ -63,6 +74,7 @@ def run(B, Tx, N, precision):
     x = torch.randint(0, 148, (B, Tx), generator=g).to(dev)
     x_lengths = torch.full((B,), Tx, dtype=torch.long, device=dev)
     dec = decoder(precision)
+    voc = vocoder(precision)
     ms_enc, (mu_x, logw, x_mask) = timed(lambda: enc(x, x_lengths))
     # synthetic durations with the reference's scale: the random-weight duration predictor is not trained, so logw is replaced
     # by log(2.3 frames per token) to give config 1's utterance length (221 tokens -> ~512 frames)
@@ -74,10 +86,11 @@ def run(B, Tx, N, precision):
     if T4 != T_y:
         z, mask, muy = (torch.nn.functional.pad(v, (0, T4 - T_y)) for v in (z, mask, muy))
     ms_dec, _ = timed(lambda: dec(z.contiguous(), mask.contiguous(), muy.contiguous(), N))
-    ms_voc, wav = timed(lambda: voc(y.contiguous()))
+    mel = y.contiguous().to(torch.bfloat16 if precision == "bf16" else torch.float32)
+    ms_voc, wav = timed(lambda: voc(mel))
     frames = B * T_y
     voc_flops = 2.0 * H.macs_per_mel_frame() * frames
-    out = {"case": f"B={B} tokens={Tx} N={N} decoder precision {precision}", "frames_per_utterance": T_y,
+    out = {"case": f"B={B} tokens={Tx} N={N} decoder and vocoder precision {precision}", "frames_per_utterance": T_y, **CARD,
            "ms": {"text_encoder": round(ms_enc, 3), "glue+sampler": round(ms_all, 3), "sampler_alone": round(ms_dec, 3),
                   "vocoder": round(ms_voc, 3), "total": round(ms_enc + ms_all + ms_voc, 3)},
            "launches": {"text_encoder": enc.engine().last_launch_count(), "sampler": dec.engine().last_launch_count(),
@@ -89,5 +102,6 @@ def run(B, Tx, N, precision):
     print(json.dumps(out), flush=True)
 
 
-for B, Tx, N, prec in ((1, 221, 10, "fp32x3"), (1, 221, 10, "tf32"), (32, 221, 50, "fp32x3"), (32, 221, 50, "tf32")):
+for B, Tx, N, prec in ((1, 221, 10, "fp32x3"), (1, 221, 10, "tf32"), (1, 221, 10, "bf16"),
+                       (32, 221, 50, "fp32x3"), (32, 221, 50, "tf32"), (32, 221, 50, "bf16")):
     run(B, Tx, N, prec)

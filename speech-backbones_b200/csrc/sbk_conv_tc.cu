@@ -92,7 +92,11 @@ template <int GEOM, int NT> struct Depth {
 // of a 3x3 conv would lose several 1e-6 relative - more than the fp32 rounding of the reference's own sums.  An
 // accumulation run is therefore cut every FLUSH sub-stages and the partial sums are added in round-to-nearest fp32 into a
 // second register array.  (Upsample runs unchunked: its runs are short, 4 taps per phase.)
-template <int GEOM, bool BF16, int NT, bool RES, bool X3>
+//
+// VOC: the vocoder's output forms (ConvTcParams::voc) on a 1x1 GEMM; the Conv1d geometries always use them.  They only
+// differ from the sampler's in the bf16 mode (an output is bf16 only when it is an activated operand) and, for fp32x3,
+// in the correction chunks of the second output (out_corr).
+template <int GEOM, bool BF16, int NT, bool RES, bool X3, bool VOC = false>
 __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     static_assert(!(X3 && BF16), "fp32x3 runs on tf32 operands");
     using G = Geo<GEOM>;
@@ -107,14 +111,16 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     constexpr int HR = G::HR, PXP = G::PXP, TAPS = G::TAPS, KCH = G::KCH;
     constexpr int EPC = BF16 ? 8 : 4;                      // elements per 16-byte channel chunk
     constexpr int CPS = KCH * EPC;                         // input channels per stage
+    constexpr bool C1 = geom_is_c1(GEOM);                  // Conv1d strip geometry
     // bf16 mode: the raw Block-conv outputs (GroupNorm inputs) stay fp32 [C/4]; every other output is an operand tensor
-    // of a later tensor-core kernel and is written as bf16 [B][H][C/8][W][8]
-    constexpr bool OUT16 = BF16 && GEOM != G_C3;
+    // of a later tensor-core kernel and is written as bf16 [B][H][C/8][W][8].  The vocoder's forms (VF16) instead pick
+    // the dtype per output: bf16 for an activated output (act_out) and the act_out2 output, fp32 for the others.
+    constexpr bool VF16 = BF16 && (C1 || VOC);
+    constexpr bool OUT16 = BF16 && GEOM != G_C3 && !VF16;
     constexpr int PLANE = HR * PXP * 16;                   // bytes between K chunks of the A tile
     constexpr int A_STAGE_BYTES = KCH * PLANE;
     constexpr int B_STAGE_BYTES = TAPS * KCH * NT * 16;
     constexpr bool BULK = GEOM != G_DOWN;                  // A tile = contiguous runs -> cp.async.bulk (no LSU work)
-    constexpr bool C1 = geom_is_c1(GEOM);                  // Conv1d strip geometry
     constexpr int SPAN = TPX;                              // output pixels per tile along W
     constexpr int FR = NT / 2;                             // accumulator registers per thread and accumulator
     constexpr int KMAIN = BF16 ? K_BF16 : K_TF32;
@@ -366,7 +372,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
             const long long cstride = (long long)Wo * 4;           // floats between consecutive channel chunks
             // bf16 outputs: index of the 16-byte chunk (b, ho, n0/8, wo) in a [B][H][C/8][W] grid of chunks; the chunks of one
             // pixel are Wo apart, consecutive threads (pixels) are adjacent: a warp store is again 512 contiguous bytes
-            const long long ochunk = OUT16 ? (((long long)(b * Ho + ho_p) * (p.Cout / 8) + n0 / 8) * Wo + wo_p) : 0;
+            const long long ochunk = (OUT16 || VF16) ? (((long long)(b * Ho + ho_p) * (p.Cout / 8) + n0 / 8) * Wo + wo_p) : 0;
             // ResnetBlock tail: the h2raw side input does not depend on the accumulators, so the first 32-column block is
             // requested before the staging-tile reads and block cb+32 as soon as block cb has been consumed
             constexpr bool SIDE = GEOM == G_PW;                     // the 1x1 convs never carry GN statistics
@@ -441,6 +447,26 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         for (int j = 0; j < 4; ++j)
                             op[(long long)j * Wo] = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
                                                                pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
+                    } else if constexpr (VF16) {
+                        // bf16 [C/8] chunks of the activated operand (out, or lrelu(out) through out_lo); fp32 x / Z otherwise
+                        auto st16 = [&](void* base, float sl) {
+                            uint4* op = reinterpret_cast<uint4*>(base) + ochunk + (long long)(cb / 8) * Wo;
+                            float a[32];
+#pragma unroll
+                            for (int i = 0; i < 32; ++i) a[i] = v[i] > 0.f ? v[i] : v[i] * sl;
+#pragma unroll
+                            for (int j = 0; j < 4; ++j)
+                                op[(long long)j * Wo] = make_uint4(pack_bf16x2(a[8 * j], a[8 * j + 1]), pack_bf16x2(a[8 * j + 2], a[8 * j + 3]),
+                                                                   pack_bf16x2(a[8 * j + 4], a[8 * j + 5]), pack_bf16x2(a[8 * j + 6], a[8 * j + 7]));
+                        };
+                        if (p.act_out) {
+                            st16(p.out, 1.f);                       // v is already lrelu(acc + bias)
+                        } else {
+                            float* op = p.out + obase + (cb / 4) * cstride;
+#pragma unroll
+                            for (int i = 0; i < 32; i += 4) *reinterpret_cast<float4*>(op + (i / 4) * cstride) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
+                            if (C1 && p.out_lo) st16(p.out_lo, p.slope);
+                        }
                     } else {
                         float* op = p.out + obase + (cb / 4) * cstride;
 #pragma unroll
@@ -451,9 +477,14 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                             for (int i = 0; i < 32; i += 4) {
                                 if (C1 && p.act_out2) {
                                     const float sl = p.slope;
-                                    *reinterpret_cast<float4*>(lp + (i / 4) * cstride) =
-                                        make_float4(v[i] > 0.f ? v[i] : v[i] * sl, v[i + 1] > 0.f ? v[i + 1] : v[i + 1] * sl,
-                                                    v[i + 2] > 0.f ? v[i + 2] : v[i + 2] * sl, v[i + 3] > 0.f ? v[i + 3] : v[i + 3] * sl);
+                                    const float4 a = make_float4(v[i] > 0.f ? v[i] : v[i] * sl, v[i + 1] > 0.f ? v[i + 1] : v[i + 1] * sl,
+                                                                 v[i + 2] > 0.f ? v[i + 2] : v[i + 2] * sl, v[i + 3] > 0.f ? v[i + 3] : v[i + 3] * sl);
+                                    *reinterpret_cast<float4*>(lp + (i / 4) * cstride) = a;
+                                    if constexpr (X3 && C1) {
+                                        // fp32x3 vocoder: x, lrelu(x) and the correction chunks of lrelu(x)
+                                        if (p.out_corr)
+                                            *reinterpret_cast<float4*>(p.out_corr + obase + (cb / 4) * cstride + (i / 4) * cstride) = corr_chunk(a.x, a.y, a.z, a.w);
+                                    }
                                 } else {
                                     *reinterpret_cast<float4*>(lp + (i / 4) * cstride) = corr_chunk(v[i], v[i + 1], v[i + 2], v[i + 3]);
                                 }
@@ -607,15 +638,22 @@ template <int GEOM, int NT, bool RES = false>
 __global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc_x3(const ConvTcParams p) {
     conv_tc_body<GEOM, false, NT, RES, true>(p);
 }
+// the vocoder's transposed-conv GEMM in bf16 mode: bf16 operands, fp32 output Z (ConvTcParams::voc)
+template <int NT>
+__global__ void __launch_bounds__(NTHREADS, 1) k_gemm_voc_bf16(const ConvTcParams p) {
+    conv_tc_body<G_PW, true, NT, false, false, true>(p);
+}
 
-template <int GEOM, bool BF16, int NT, bool RES = false, bool X3 = false>
+template <int GEOM, bool BF16, int NT, bool RES = false, bool X3 = false, bool VOC = false>
 static int launch_tc(const ConvTcParams& p, cudaStream_t s) {
     using D = Depth<GEOM, NT>;
+    static_assert(!VOC || (GEOM == G_PW && BF16 && !RES && !X3), "VOC selects the bf16 GEMM with fp32 output");
     // the dynamic-shared-memory opt-in is a per-device function attribute and the persistent grid is sized from the
     // current device's SM count: both are cached per device ordinal (a process may drive several GPUs through several handles)
     static DevCache cache;
     const void* fn;
-    if constexpr (X3) fn = reinterpret_cast<const void*>(k_conv_tc_x3<GEOM, NT, RES>);
+    if constexpr (VOC) fn = reinterpret_cast<const void*>(k_gemm_voc_bf16<NT>);
+    else if constexpr (X3) fn = reinterpret_cast<const void*>(k_conv_tc_x3<GEOM, NT, RES>);
     else fn = reinterpret_cast<const void*>(k_conv_tc<GEOM, BF16, NT, RES>);
     const int num_sms = cache.get(fn);
     if (num_sms <= 0) return -1;
@@ -626,7 +664,8 @@ static int launch_tc(const ConvTcParams& p, cudaStream_t s) {
     else mt = (p.H * p.W + TPX - 1) / TPX;
     const long long total = (long long)mt * (p.Cout / NT) * p.B;
     const int grid = (int)(total < num_sms ? total : num_sms);       // persistent: one wave of resident CTAs
-    if constexpr (X3) k_conv_tc_x3<GEOM, NT, RES><<<grid, NTHREADS, D::SMEM, s>>>(p);
+    if constexpr (VOC) k_gemm_voc_bf16<NT><<<grid, NTHREADS, D::SMEM, s>>>(p);
+    else if constexpr (X3) k_conv_tc_x3<GEOM, NT, RES><<<grid, NTHREADS, D::SMEM, s>>>(p);
     else k_conv_tc<GEOM, BF16, NT, RES><<<grid, NTHREADS, D::SMEM, s>>>(p);
     return 1;
 }
@@ -637,8 +676,13 @@ int conv_tc_ntile(int geom, int Cout) {
     if (geom_is_c1(geom)) return Cout % 128 == 0 ? 128 : (Cout % 64 == 0 ? 64 : 32);
     return Cout % 128 == 0 ? 128 : 64;
 }
-// (the running sums live in registers next to the accumulators; the 7x7 conv's 128-wide variant would spill them)
-int conv_tc_ntile_x3(int geom, int Cout) { return geom == G_C7 ? 64 : conv_tc_ntile(geom, Cout); }
+// (the running sums live in registers next to the accumulators; the 128-wide variants of the 7x7 conv and of the Conv1d
+// would spill them)
+int conv_tc_ntile_x3(int geom, int Cout) {
+    if (geom == G_C7) return 64;
+    if (geom_is_c1(geom)) return Cout % 64 == 0 ? 64 : 32;
+    return conv_tc_ntile(geom, Cout);
+}
 int conv_tc_taps(int geom) {
     switch (geom) {
         case G_PW: return 1;
@@ -676,15 +720,23 @@ static int dispatch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
     }
 }
 
-// Conv1d (vocoder): tf32 operands
+// Conv1d (vocoder): tf32 operands, bf16 operands, or fp32x3 (the N tile of conv_tc_ntile_x3, as the weights are packed)
+template <int GEOM, bool BF16, bool X3>
+static int launch_conv1d(const ConvTcParams& p, cudaStream_t s, int nt) {
+    switch (nt) {
+        case 128:
+            if constexpr (X3) return -1;                               // conv_tc_ntile_x3: at most 64 wide
+            else return launch_tc<GEOM, BF16, 128, false, X3>(p, s);
+        case 64:  return launch_tc<GEOM, BF16, 64, false, X3>(p, s);
+        default:  return p.Cout % 32 == 0 ? launch_tc<GEOM, BF16, 32, false, X3>(p, s) : -1;
+    }
+}
 template <int GEOM>
 static int dispatch_conv1d(const ConvTcParams& p, cudaStream_t s) {
     if (p.dil < 1 || p.pad < 0 || 2 * p.pad > 64) return -1;      // the strip carries at most 64 halo samples
-    switch (conv_tc_ntile(p.geom, p.Cout)) {
-        case 128: return launch_tc<GEOM, false, 128>(p, s);
-        case 64:  return launch_tc<GEOM, false, 64>(p, s);
-        default:  return p.Cout % 32 == 0 ? launch_tc<GEOM, false, 32>(p, s) : -1;
-    }
+    if (p.x3) return launch_conv1d<GEOM, false, true>(p, s, conv_tc_ntile_x3(p.geom, p.Cout));
+    if (p.bf16) return launch_conv1d<GEOM, true, false>(p, s, conv_tc_ntile(p.geom, p.Cout));
+    return launch_conv1d<GEOM, false, false>(p, s, conv_tc_ntile(p.geom, p.Cout));
 }
 
 // fp32x3 mode (p.x3): correction + main sub-stages, chunked accumulation
@@ -704,11 +756,15 @@ static int dispatch_conv_tc_x3(const ConvTcParams& p, cudaStream_t s) {
 }
 
 int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
-    if (geom_is_c1(p.geom)) {
-        if (p.x3 || p.bf16) return -1;
+    if (p.x3 && p.bf16) return -1;
+    if (geom_is_c1(p.geom))
         return p.geom == G_C1K3 ? dispatch_conv1d<G_C1K3>(p, s) : p.geom == G_C1K7 ? dispatch_conv1d<G_C1K7>(p, s) : dispatch_conv1d<G_C1K11>(p, s);
+    if (p.voc && p.bf16) {                                            // the vocoder's GEMM: fp32 Z from bf16 operands
+        if (p.geom != G_PW || p.epi != EPI_PLAIN) return -1;
+        return conv_tc_ntile(G_PW, p.Cout) == 128 ? launch_tc<G_PW, true, 128, false, false, true>(p, s)
+                                                  : launch_tc<G_PW, true, 64, false, false, true>(p, s);
     }
-    if (p.x3) return p.bf16 ? -1 : dispatch_conv_tc_x3(p, s);
+    if (p.x3) return dispatch_conv_tc_x3(p, s);
     return p.bf16 ? dispatch_conv_tc<true>(p, s) : dispatch_conv_tc<false>(p, s);
 }
 

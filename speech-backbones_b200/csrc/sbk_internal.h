@@ -82,6 +82,13 @@ struct ConvTcParams {
     int x3;
     const void* in0_lo; const void* in1_lo;         // the correction tensors, same chunk layout as in0 / in1
     float* out_lo;                                  // operand-form outputs (non-3x3 geometries): also write the correction chunks
+    // The vocoder's output forms (Conv1d geometries, and the transposed convs' 1x1 GEMM when voc = 1).  The output dtype is
+    // per output, not per mode: an activated output (act_out) is the next conv's operand and takes the mode's operand form
+    // (bf16 mode: bf16 [B][C/8][L][8]); every other output (the residual stream x, the GEMM output Z) stays fp32, with a
+    // fp32 addin; the act_out2 output lrelu(out) is an operand again (bf16 in bf16 mode).  fp32x3: out_corr receives the
+    // correction chunks of the act_out2 output (those of an act_out output go through out_lo, see above).
+    int voc;
+    float* out_corr;
 };
 
 // Block activation between the two convs of a ResnetBlock, written once in operand form (diffusion.py:57,76):

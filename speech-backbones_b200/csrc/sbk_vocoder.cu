@@ -11,8 +11,14 @@
 //                                            bias and the LeakyReLU.  (A transposed conv with k = 2u is exactly a 2-tap overlap-add.)
 //   * MRF mean (xs / num_kernels, :112)   -> k_mrf: (r0 + r1 + r2) / 3 and the next stage's LeakyReLU in one pass;
 //   * conv_post (C -> 1, K = 7) + tanh    -> k_post on CUDA cores (224 MACs per sample).
-// tf32 operands (weights rounded to nearest at pack time, activations truncated by the tensor core), fp32 accumulation and
-// fp32 everywhere else - the arithmetic PyTorch's own GPU convs use by default.
+// Precision (sbk_vocoder_set_precision), the same launches in every mode:
+//   tf32 (default)  tf32 operands (weights rounded to nearest at pack time, activations truncated by the tensor core), fp32
+//                   accumulation and fp32 everywhere else - the arithmetic PyTorch's own GPU convs use by default;
+//   fp32x3 (and fp32)  x*w = x_hi*w_hi + one f16 correction MMA (sbk_internal.h: corr_chunk), chunked accumulation: every
+//                   conv input (mel_in, SA, A0, A1, A2, Hb) carries a correction twin, written by its producer in the same pass;
+//   bf16            bf16 weights, and the conv inputs (the LeakyReLU operands mel_in, SA, A0, A1, A2, Hb) stored as bf16
+//                   [B][C/8][L][8]; the residual stream x (X0, X1, X2, R[j]), the GEMM output Z and conv_post's input stay fp32.
+// conv_post, tanh, the folds and the MRF mean are fp32 in every mode.
 #include "../../include/sbk.h"
 #include "sbk_internal.h"
 
@@ -47,22 +53,43 @@ namespace {
 
 constexpr float kSlope = 0.1f;        // LRELU_SLOPE, models.py:10
 
-// mel [B][F][T] (the reference's planar layout) -> [B][F/4][T][4]
-__global__ void k_voc_mel_in(const float* mel, float* out, int B, int F, int T) {
+// An activation operand (a conv input) in the mode's form.  The 4 channels v of element i = bc*L + l of a [B][C/4][L][4]
+// tensor (bc = b*C/4 + channel chunk) go to
+//   bf16 = 0: out[i] fp32 and, when out_lo is set (fp32x3), out_lo[i] = their correction chunk (sbk_internal.h: corr_chunk);
+//   bf16 = 1: half of the 16-byte chunk (b, c/8, l) of a bf16 [B][C/8][L][8] tensor (C/4 even), round to nearest even.
+__device__ __forceinline__ void store_operand(float4 v, long long bc, long long l, long long L, void* out, float* out_lo, int bf16) {
+    if (bf16) {
+        uint32_t lo, hi;
+        asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(v.y), "f"(v.x));
+        asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(v.w), "f"(v.z));
+        reinterpret_cast<uint2*>(out)[((bc >> 1) * L + l) * 2 + (bc & 1)] = make_uint2(lo, hi);
+    } else {
+        reinterpret_cast<float4*>(out)[bc * L + l] = v;
+        if (out_lo) reinterpret_cast<float4*>(out_lo)[bc * L + l] = corr_chunk(v.x, v.y, v.z, v.w);
+    }
+}
+
+__device__ __forceinline__ float4 lrelu4(float4 v, float slope) {
+    return make_float4(v.x > 0.f ? v.x : v.x * slope, v.y > 0.f ? v.y : v.y * slope, v.z > 0.f ? v.z : v.z * slope, v.w > 0.f ? v.w : v.w * slope);
+}
+
+// mel [B][F][T] (the reference's planar layout) -> the operand [B][F/4][T][4] (+ correction chunks), or bf16 [B][F/8][T][8]
+__global__ void k_voc_mel_in(const float* mel, void* out, float* out_lo, int B, int F, int T, int bf16) {
     const long long n = (long long)B * (F / 4) * T;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         const int t = (int)(i % T);
         const long long bc = i / T;
         const int ch = (int)(bc % (F / 4)); const long long b = bc / (F / 4);
         const float* src = mel + ((b * F + ch * 4) * T) + t;
-        reinterpret_cast<float4*>(out)[i] = make_float4(src[0], src[T], src[2 * (long long)T], src[3 * (long long)T]);
+        store_operand(make_float4(src[0], src[T], src[2 * (long long)T], src[3 * (long long)T]), bc, t, T, out, out_lo, bf16);
     }
 }
 
 // ConvTranspose1d(k = 2u, stride u, padding u/2) overlap-add (models.py:108): output sample o = u*q + r receives tap
 // t1 = (o + p) mod u of input i1 = (o + p) / u and tap t1 + u of input i1 - 1 (p = u/2).
-//   z: [B][(2u*C)/4][Lin][4], channel index t*C + co;  x (raw) and a = lrelu(x): [B][C/4][Lin*u][4]
-__global__ void k_voc_ct_fold(const float* z, const float* bias, float* x, float* a, int B, int C, int Lin, int u, float slope) {
+//   z: [B][(2u*C)/4][Lin][4], channel index t*C + co;  x (raw): [B][C/4][Lin*u][4];  a = lrelu(x) in operand form (store_operand)
+__global__ void k_voc_ct_fold(const float* z, const float* bias, float* x, void* a, float* a_lo, int B, int C, int Lin, int u, float slope,
+                              int bf16) {
     const int Lout = Lin * u, c4n = C / 4, p = u / 2;
     const long long n = (long long)B * c4n * Lout;
     const long long zc = (long long)Lin * 4;                       // floats between consecutive channel chunks of z
@@ -82,17 +109,19 @@ __global__ void k_voc_ct_fold(const float* z, const float* bias, float* x, float
             v.x += w.x; v.y += w.y; v.z += w.z; v.w += w.w;
         }
         reinterpret_cast<float4*>(x)[i] = v;
-        reinterpret_cast<float4*>(a)[i] = make_float4(v.x > 0.f ? v.x : v.x * slope, v.y > 0.f ? v.y : v.y * slope,
-                                                      v.z > 0.f ? v.z : v.z * slope, v.w > 0.f ? v.w : v.w * slope);
+        store_operand(lrelu4(v, slope), bc, o, Lout, a, a_lo, bf16);
     }
 }
 
 // Multi-receptive-field fusion (models.py:109-114): x = ((r0 + r1) + r2) / 3, written as the next consumer's operand lrelu(x)
-__global__ void k_voc_mrf(const float4* r0, const float4* r1, const float4* r2, float4* a, long long n4, float inv, float slope) {
+// (store_operand over [B][C/4][L][4] chunks, i = bc*L + l; conv_post's input is plain fp32: bf16 = 0, a_lo = null)
+__global__ void k_voc_mrf(const float4* r0, const float4* r1, const float4* r2, void* a, float* a_lo, long long n4, int L, float inv,
+                          float slope, int bf16) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
         const float4 p = __ldg(r0 + i), q = __ldg(r1 + i), r = __ldg(r2 + i);
         float4 v = make_float4(((p.x + q.x) + r.x) * inv, ((p.y + q.y) + r.y) * inv, ((p.z + q.z) + r.z) * inv, ((p.w + q.w) + r.w) * inv);
-        a[i] = make_float4(v.x > 0.f ? v.x : v.x * slope, v.y > 0.f ? v.y : v.y * slope, v.z > 0.f ? v.z : v.z * slope, v.w > 0.f ? v.w : v.w * slope);
+        const long long bc = bf16 ? i / L : 0;
+        store_operand(lrelu4(v, slope), bc, bf16 ? i - bc * L : i, L, a, a_lo, bf16);
     }
 }
 
@@ -128,30 +157,33 @@ int ew_grid(long long n) {
     return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
-uint32_t f32_to_tf32_rna(float x) {
-    uint32_t u; memcpy(&u, &x, 4);
-    if ((u & 0x7F800000u) != 0x7F800000u) u += 0x1000u;
-    return u & 0xFFFFE000u;
-}
-
 struct VWSpec { std::string name; std::vector<int64_t> shape; };
+
+// the tensor-core form of each mode: fp32 and fp32x3 run the fp32x3 split, bf16 its bf16 operands, tf32 tf32 operands
+bool prec_x3(int precision) { return precision == SBK_PREC_FP32X3 || precision == SBK_PREC_FP32; }
+bool prec_bf16(int precision) { return precision == SBK_PREC_BF16; }
 
 }  // namespace
 
 struct sbk_vocoder {
     sbk_vocoder_config cfg;
+    int precision = SBK_PREC_TF32;
     std::vector<VWSpec> spec;
     std::map<std::string, float*> raw;       // device copies, reference layout (after remove_weight_norm)
-    std::map<std::string, float*> packed;    // tensor-core stage images
+    std::map<std::string, void*> packed;     // tensor-core stage images
+    std::map<std::string, size_t> packed_bytes;
     float* zero = nullptr;
     void* mem = nullptr; size_t cap = 0;
     bool is_packed = false;
     int64_t last_launches = 0;
-    // test hook (sbk_vocoder_debug_*): per-name snapshots of the last forward's intermediates, in launch order
-    struct Snap { std::string name; float* buf; size_t cap, numel; };
+    // test hook (sbk_vocoder_debug_*): per-name snapshots of the last forward's intermediates, in launch order; fmt 1 = fp32
+    // [B][C/4][L][4] (wav: [B][1][L]), 2 = bf16 [B][C/8][L][8]
+    struct Snap { std::string name; void* buf; size_t cap, numel; int fmt; };
     bool capture = false;
     std::vector<Snap> snaps;
     int n_res() const { return cfg.n_kernels; }
+    bool x3() const { return prec_x3(precision); }
+    bool bf16() const { return prec_bf16(precision); }
 };
 
 static int voc_geom(int k) { return k == 3 ? G_C1K3 : (k == 7 ? G_C1K7 : (k == 11 ? G_C1K11 : -1)); }
@@ -210,6 +242,22 @@ extern "C" void sbk_vocoder_destroy(sbk_vocoder* v) {
     delete v;
 }
 
+// Host logic only (no device work): the mode's tiling rules, then the packed state is dropped.
+extern "C" int sbk_vocoder_set_precision(sbk_vocoder* v, int32_t precision) {
+    if (!v) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_set_precision: null handle");
+    if (precision < SBK_PREC_FP32 || precision > SBK_PREC_FP32X3) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_set_precision: unknown precision %d", precision);
+    if (prec_bf16(precision)) {
+        // bf16 K stages hold 16 input channels (Conv1d) and 64 (GEMM, sbk_conv_tc.cu conv_tc_stage_channels).  Every stage
+        // has a multiple of 32 channels (sbk_vocoder_create), so its GEMM reads a multiple of 64: only conv_pre can fail.
+        const int c1 = conv_tc_stage_channels(G_C1K3, 1);
+        if (v->cfg.num_mels % c1 != 0)
+            return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_vocoder_set_precision: bf16 needs num_mels to be a multiple of %d, got %d", c1, v->cfg.num_mels);
+    }
+    v->precision = precision;
+    v->is_packed = false;
+    return SBK_OK;
+}
+
 extern "C" int sbk_vocoder_num_weights(const sbk_vocoder* v) { return v ? (int)v->spec.size() : 0; }
 extern "C" const char* sbk_vocoder_weight_name(const sbk_vocoder* v, int i) {
     if (!v || i < 0 || i >= (int)v->spec.size()) return nullptr;
@@ -235,20 +283,19 @@ extern "C" int sbk_vocoder_set_weight(sbk_vocoder* v, const char* name, const vo
     return SBK_OK;
 }
 
-// logical [co][ci][taps] -> the conv kernel's per-stage shared-memory image [ntile][kstage][tap][16 B chunk][co % NT][4], tf32 (RNA)
+// logical [co][ci][taps] -> the conv kernel's per-stage shared-memory image in the handle's mode (conv_tc_pack_image: tf32
+// RNA, bf16 RNE, or fp32x3 (w_hi, correction) stage pairs)
 static int voc_pack(sbk_vocoder* v, const std::vector<float>& w, const std::string& key, int cout, int cin, int geom) {
-    const int taps = conv_tc_taps(geom), NT = conv_tc_ntile(geom, cout), CPS = conv_tc_stage_channels(geom, 0), KCHK = CPS / 4;
+    const bool bf = v->bf16(), x3 = v->x3();
+    const int NT = x3 ? conv_tc_ntile_x3(geom, cout) : conv_tc_ntile(geom, cout), CPS = conv_tc_stage_channels(geom, bf ? 1 : 0);
     if (cin % CPS != 0 || cout % NT != 0) return sbk_set_error(SBK_ERR_UNSUPPORTED, "vocoder pack '%s': %d -> %d channels do not tile (K stage %d, N tile %d)", key.c_str(), cin, cout, CPS, NT);
-    const int ksteps = cin / CPS;
-    std::vector<uint32_t> img((size_t)cout * cin * taps);
-    for (int nt = 0; nt < cout / NT; ++nt) for (int ks = 0; ks < ksteps; ++ks) for (int tap = 0; tap < taps; ++tap)
-        for (int k = 0; k < KCHK; ++k) for (int col = 0; col < NT; ++col) for (int e = 0; e < 4; ++e) {
-            const int co = nt * NT + col, ci = ks * CPS + k * 4 + e;
-            img[(((((size_t)nt * ksteps + ks) * taps + tap) * KCHK + k) * NT + col) * 4 + e] = f32_to_tf32_rna(w[((size_t)co * cin + ci) * taps + tap]);
-        }
-    float*& d = v->packed[key];
-    if (!d) VCU(cudaMalloc(&d, img.size() * 4));
-    VCU(cudaMemcpy(d, img.data(), img.size() * 4, cudaMemcpyHostToDevice));
+    std::vector<uint8_t> img(conv_tc_pack_image(w.data(), cout, cin, geom, bf, x3, 0, nullptr));
+    conv_tc_pack_image(w.data(), cout, cin, geom, bf, x3, 0, img.data());
+    void*& d = v->packed[key];
+    size_t& have = v->packed_bytes[key];
+    if (d && have != img.size()) { VCU(cudaFree(d)); d = nullptr; }     // another mode's image
+    if (!d) { VCU(cudaMalloc(&d, img.size())); have = img.size(); }
+    VCU(cudaMemcpy(d, img.data(), img.size(), cudaMemcpyHostToDevice));
     return SBK_OK;
 }
 
@@ -256,6 +303,7 @@ extern "C" int sbk_vocoder_pack(sbk_vocoder* v) {
     if (!v) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_pack: null handle");
     for (auto& s : v->spec) if (!v->raw.count(s.name)) return sbk_set_error(SBK_ERR_STATE, "sbk_vocoder_pack: missing key '%s' (strict)", s.name.c_str());
     VCU(cudaSetDevice(v->cfg.device));
+    v->is_packed = false;
     for (auto& s : v->spec) {
         if (s.name.size() < 7 || s.name.compare(s.name.size() - 7, 7, ".weight") != 0 || s.name == "conv_post.weight") continue;
         size_t numel = 1; for (auto d : s.shape) numel *= (size_t)d;
@@ -280,23 +328,54 @@ extern "C" int sbk_vocoder_pack(sbk_vocoder* v) {
     return SBK_OK;
 }
 
-extern "C" size_t sbk_vocoder_workspace_bytes(const sbk_vocoder* v, int B, int T) {
-    if (!v || B <= 0 || T <= 0) return 0;
+namespace {
+
+// The workspace of one (B, T) in the handle's mode: 11 activation buffers of the largest stage, the transposed-conv GEMM
+// output and the re-laid-out mel.  SA, A0, A1, A2, Hb and the mel are conv inputs: bf16 in the bf16 mode, and with a
+// correction twin each in fp32x3.  With base = null only the size is computed.
+struct VocBufs {
+    void* melc; float* melc_lo; float* Z;
+    void *SA, *A0, *A1, *A2, *Hb;
+    float *SA_lo, *A0_lo, *A1_lo, *A2_lo, *Hb_lo;
+    float *X0, *X1, *X2, *R[3];
+};
+
+size_t voc_carve(const sbk_vocoder* v, int B, int T, char* base, VocBufs* o) {
     const sbk_vocoder_config& c = v->cfg;
     size_t big = 0, zmax = 0;
-    long long L = T; int ch = c.upsample_initial_channel;
-    big = (size_t)B * ch * L;
-    for (int i = 0; i < c.n_ups; ++i) {
-        zmax = std::max<size_t>(zmax, (size_t)B * c.upsample_kernel_sizes[i] * (ch / 2) * L);
-        L *= c.upsample_rates[i]; ch /= 2;
-        big = std::max<size_t>(big, (size_t)B * ch * L);
+    { long long L = T; int ch = c.upsample_initial_channel; big = (size_t)B * ch * L;
+      for (int i = 0; i < c.n_ups; ++i) { zmax = std::max<size_t>(zmax, (size_t)B * c.upsample_kernel_sizes[i] * (ch / 2) * L); L *= c.upsample_rates[i]; ch /= 2; big = std::max<size_t>(big, (size_t)B * ch * L); } }
+    const size_t ob = v->bf16() ? 2 : 4;            // bytes per element of an operand tensor
+    const bool x3 = v->x3();
+    size_t off = 0;
+    auto take = [&](size_t bytes) -> char* { off = (off + 255) & ~size_t(255); char* r = base ? base + off : nullptr; off += bytes; return r; };
+    VocBufs b{};
+    b.melc = take((size_t)B * c.num_mels * T * ob);
+    b.Z = (float*)take(zmax * 4);
+    // SA: the stage input lrelu(x) (conv_pre / MRF output);  X0|A0: the stage's x after the transposed conv and lrelu(x);
+    // X1|A1, X2|A2: the running x of a ResBlock after its first / second dilation;  Hb: lrelu(conv1(.));  R[j]: ResBlock outputs
+    b.SA = take(big * ob); b.X0 = (float*)take(big * 4); b.A0 = take(big * ob); b.X1 = (float*)take(big * 4); b.A1 = take(big * ob);
+    b.X2 = (float*)take(big * 4); b.A2 = take(big * ob); b.Hb = take(big * ob);
+    for (int j = 0; j < 3; ++j) b.R[j] = (float*)take(big * 4);
+    if (x3) {
+        b.melc_lo = (float*)take((size_t)B * c.num_mels * T * 4);
+        b.SA_lo = (float*)take(big * 4); b.A0_lo = (float*)take(big * 4); b.A1_lo = (float*)take(big * 4);
+        b.A2_lo = (float*)take(big * 4); b.Hb_lo = (float*)take(big * 4);
     }
-    return (11 * big + zmax + (size_t)B * c.num_mels * T) * sizeof(float) + 16 * 256;
+    if (o) *o = b;
+    return off + 256;
+}
+
+}  // namespace
+
+extern "C" size_t sbk_vocoder_workspace_bytes(const sbk_vocoder* v, int B, int T) {
+    if (!v || B <= 0 || T <= 0) return 0;
+    return voc_carve(v, B, T, nullptr, nullptr);
 }
 
 extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav, int B, int T, void* stream) {
     if (!v || !mel || !wav) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_forward: null argument");
-    if (!v->is_packed) return sbk_set_error(SBK_ERR_STATE, "sbk_vocoder_forward: weights not packed (sbk_vocoder_set_weight for every key, then sbk_vocoder_pack)");
+    if (!v->is_packed) return sbk_set_error(SBK_ERR_STATE, "sbk_vocoder_forward: weights not packed for the current precision (sbk_vocoder_set_weight for every key, then sbk_vocoder_pack)");
     if (B <= 0 || T <= 0) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_forward: B and T must be positive (got %d, %d)", B, T);
     VCU(cudaSetDevice(v->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
@@ -308,28 +387,28 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
         if (e != cudaSuccess) { v->mem = nullptr; cudaGetLastError(); return sbk_set_error(SBK_ERR_CUDA, "out of memory: the vocoder workspace for (B=%d, T=%d) needs %zu bytes", B, T, need); }
         v->cap = need;
     }
-    // ---- carve: 10 activation buffers of the largest stage + the transposed-conv GEMM output + the re-laid-out mel
-    size_t big = 0, zmax = 0;
-    { long long L = T; int ch = c.upsample_initial_channel; big = (size_t)B * ch * L;
-      for (int i = 0; i < c.n_ups; ++i) { zmax = std::max<size_t>(zmax, (size_t)B * c.upsample_kernel_sizes[i] * (ch / 2) * L); L *= c.upsample_rates[i]; ch /= 2; big = std::max<size_t>(big, (size_t)B * ch * L); } }
-    char* base = (char*)v->mem; size_t off = 0;
-    auto take = [&](size_t floats) { off = (off + 255) & ~size_t(255); float* r = (float*)(base + off); off += floats * sizeof(float); return r; };
-    float* melc = take((size_t)B * c.num_mels * T);
-    float* Z = take(zmax);
-    // SA: the stage input lrelu(x) (conv_pre / MRF output);  X0|A0: the stage's x after the transposed conv and lrelu(x);
-    // X1|A1, X2|A2: the running x of a ResBlock after its first / second dilation;  Hb: lrelu(conv1(.));  R[j]: ResBlock outputs
-    float *SA = take(big), *X0 = take(big), *A0 = take(big), *X1 = take(big), *A1 = take(big), *X2 = take(big), *A2 = take(big), *Hb = take(big);
-    float* R[3] = {take(big), take(big), take(big)};
-    auto W = [&](const std::string& k) -> const float* { auto it = v->packed.find(k); if (it != v->packed.end()) return it->second; auto i2 = v->raw.find(k); return i2 != v->raw.end() ? i2->second : nullptr; };
+    VocBufs wb;
+    voc_carve(v, B, T, (char*)v->mem, &wb);
+    const bool x3 = v->x3(), bf = v->bf16();
+    const int ofmt = bf ? 2 : 1;                     // debug layout of the operand tensors
+    void *melc = wb.melc, *SA = wb.SA, *A0 = wb.A0, *A1 = wb.A1, *A2 = wb.A2, *Hb = wb.Hb;
+    float *Z = wb.Z, *X0 = wb.X0, *X1 = wb.X1, *X2 = wb.X2, **R = wb.R;
+    auto W = [&](const std::string& k) -> const void* { auto it = v->packed.find(k); if (it != v->packed.end()) return it->second; auto i2 = v->raw.find(k); return i2 != v->raw.end() ? i2->second : nullptr; };
+    auto Wf = [&](const std::string& k) { return (const float*)W(k); };
     int64_t n = 0;
     int rcl = 0;
-    auto conv = [&](int geom, const std::string& pre, const float* in, int cin, int cout, int L, int dil, float* out, int act_out,
-                    const float* addin, float* out2) {
+    // act_out: out = lrelu(conv + bias), the next conv's operand (fp32x3: a_corr = its correction chunks); otherwise
+    // out = conv + bias (+ addin) in fp32 and a_out = lrelu(out) in operand form (+ a_corr)
+    auto conv = [&](int geom, const std::string& pre, const void* in, const void* in_lo, int cin, int cout, int L, int dil, void* out,
+                    int act_out, const float* addin, void* a_out, float* a_corr) {
         ConvTcParams p; memset(&p, 0, sizeof(p));
         p.geom = geom; p.in0 = in; p.c0 = cin; p.H = 1; p.W = L; p.B = B; p.Ho = 1; p.Wo = L;
-        p.wpk = W(pre + ".wtc"); p.bias = geom == G_PW ? nullptr : W(pre + ".bias"); p.out = out; p.Cout = cout; p.epi = EPI_PLAIN;
+        p.wpk = W(pre + ".wtc"); p.bias = geom == G_PW ? nullptr : Wf(pre + ".bias"); p.out = (float*)out; p.Cout = cout; p.epi = EPI_PLAIN;
         p.zero_page = v->zero; p.dil = dil; p.pad = geom == G_PW ? 0 : (conv_tc_taps(geom) - 1) * dil / 2;
-        p.slope = kSlope; p.act_out = act_out; p.addin = addin; p.out_lo = out2; p.act_out2 = out2 ? 1 : 0;
+        p.slope = kSlope; p.act_out = act_out; p.addin = addin;
+        if (act_out) { p.out_lo = a_corr; p.act_out2 = 0; }
+        else { p.out_lo = (float*)a_out; p.act_out2 = a_out ? 1 : 0; p.out_corr = a_corr; }
+        p.x3 = x3 ? 1 : 0; p.in0_lo = in_lo; p.bf16 = bf ? 1 : 0; p.voc = 1;
         const int k = launch_conv_tc(p, s);
         if (k < 0) rcl = -1; else n += k;
     };
@@ -338,62 +417,68 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
     size_t nsnap = 0;
     cudaError_t snap_err = cudaSuccess;
     // (the name is pre + suf, put together only when capturing)
-    auto snap = [&](const std::string& pre, const char* suf, const float* src, size_t numel) {
+    auto snap = [&](const std::string& pre, const char* suf, const void* src, size_t numel, int fmt) {
         if (!v->capture || snap_err != cudaSuccess) return;
-        if (nsnap == v->snaps.size()) v->snaps.push_back({std::string(), nullptr, 0, 0});
+        if (nsnap == v->snaps.size()) v->snaps.push_back({std::string(), nullptr, 0, 0, 1});
         sbk_vocoder::Snap& sn = v->snaps[nsnap++];
-        sn.name = pre + suf; sn.numel = numel;
-        if (numel > sn.cap) {
+        const size_t bytes = numel * (fmt == 2 ? 2 : 4);
+        sn.name = pre + suf; sn.numel = numel; sn.fmt = fmt;
+        if (bytes > sn.cap) {
             cudaFree(sn.buf); sn.buf = nullptr; sn.cap = 0;
-            if ((snap_err = cudaMalloc(&sn.buf, numel * sizeof(float))) != cudaSuccess) { sn.buf = nullptr; sn.numel = 0; return; }
-            sn.cap = numel;
+            if ((snap_err = cudaMalloc(&sn.buf, bytes)) != cudaSuccess) { sn.buf = nullptr; sn.numel = 0; return; }
+            sn.cap = bytes;
         }
-        snap_err = cudaMemcpyAsync(sn.buf, src, numel * sizeof(float), cudaMemcpyDeviceToDevice, s);
+        snap_err = cudaMemcpyAsync(sn.buf, src, bytes, cudaMemcpyDeviceToDevice, s);
     };
     const size_t bn = (size_t)B;
-    k_voc_mel_in<<<ew_grid((long long)B * (c.num_mels / 4) * T), 256, 0, s>>>(mel, melc, B, c.num_mels, T); ++n;
-    snap("mel_in", "", melc, bn * c.num_mels * T);
+    k_voc_mel_in<<<ew_grid((long long)B * (c.num_mels / 4) * T), 256, 0, s>>>(mel, melc, wb.melc_lo, B, c.num_mels, T, bf ? 1 : 0); ++n;
+    snap("mel_in", "", melc, bn * c.num_mels * T, ofmt);
     int ch = c.upsample_initial_channel; int L = T;
     // conv_pre + the first stage's leaky_relu (models.py:105,107)
-    conv(G_C1K7, "conv_pre", melc, c.num_mels, ch, L, 1, SA, 1, nullptr, nullptr);
-    snap("conv_pre", "", SA, bn * ch * L);
+    conv(G_C1K7, "conv_pre", melc, wb.melc_lo, c.num_mels, ch, L, 1, SA, 1, nullptr, nullptr, wb.SA_lo);
+    snap("conv_pre", "", SA, bn * ch * L, ofmt);
     int rb = 0;
+    const float* post_in = nullptr;
     for (int i = 0; i < c.n_ups; ++i) {
         const int u = c.upsample_rates[i], k = c.upsample_kernel_sizes[i], co = ch / 2;
         const std::string up = "ups." + std::to_string(i);
-        conv(G_PW, up, SA, ch, k * co, L, 1, Z, 0, nullptr, nullptr);                           // Z[i][t*co + c] (models.py:108)
-        snap(up, ".z", Z, bn * k * co * L);
+        conv(G_PW, up, SA, wb.SA_lo, ch, k * co, L, 1, Z, 0, nullptr, nullptr, nullptr);    // Z[i][t*co + c] (models.py:108)
+        snap(up, ".z", Z, bn * k * co * L, 1);
         const int Lo = L * u;
-        k_voc_ct_fold<<<ew_grid((long long)B * (co / 4) * Lo), 256, 0, s>>>(Z, W(up + ".bias"), X0, A0, B, co, L, u, kSlope); ++n;
-        snap(up, ".x", X0, bn * co * Lo); snap(up, ".a", A0, bn * co * Lo);
+        k_voc_ct_fold<<<ew_grid((long long)B * (co / 4) * Lo), 256, 0, s>>>(Z, Wf(up + ".bias"), X0, A0, wb.A0_lo, B, co, L, u, kSlope, bf ? 1 : 0); ++n;
+        snap(up, ".x", X0, bn * co * Lo, 1); snap(up, ".a", A0, bn * co * Lo, ofmt);
         ch = co; L = Lo;
         const size_t na = bn * ch * L;
         for (int j = 0; j < 3; ++j, ++rb) {
             const int geom = voc_geom(c.resblock_kernel_sizes[j]);
             const std::string rp = "resblocks." + std::to_string(rb);
             // per dilation d: xt = conv2(lrelu(conv1_d(lrelu(x)))); x = xt + x   (models.py:42-47)
-            conv(geom, rp + ".convs1.0", A0, ch, ch, L, c.resblock_dilations[j][0], Hb, 1, nullptr, nullptr);
-            snap(rp, ".convs1.0", Hb, na);
-            conv(geom, rp + ".convs2.0", Hb, ch, ch, L, 1, X1, 0, X0, A1);
-            snap(rp, ".convs2.0.x", X1, na); snap(rp, ".convs2.0.a", A1, na);
-            conv(geom, rp + ".convs1.1", A1, ch, ch, L, c.resblock_dilations[j][1], Hb, 1, nullptr, nullptr);
-            snap(rp, ".convs1.1", Hb, na);
-            conv(geom, rp + ".convs2.1", Hb, ch, ch, L, 1, X2, 0, X1, A2);
-            snap(rp, ".convs2.1.x", X2, na); snap(rp, ".convs2.1.a", A2, na);
-            conv(geom, rp + ".convs1.2", A2, ch, ch, L, c.resblock_dilations[j][2], Hb, 1, nullptr, nullptr);
-            snap(rp, ".convs1.2", Hb, na);
-            conv(geom, rp + ".convs2.2", Hb, ch, ch, L, 1, R[j], 0, X2, nullptr);
-            snap(rp, ".convs2.2.x", R[j], na);
+            conv(geom, rp + ".convs1.0", A0, wb.A0_lo, ch, ch, L, c.resblock_dilations[j][0], Hb, 1, nullptr, nullptr, wb.Hb_lo);
+            snap(rp, ".convs1.0", Hb, na, ofmt);
+            conv(geom, rp + ".convs2.0", Hb, wb.Hb_lo, ch, ch, L, 1, X1, 0, X0, A1, wb.A1_lo);
+            snap(rp, ".convs2.0.x", X1, na, 1); snap(rp, ".convs2.0.a", A1, na, ofmt);
+            conv(geom, rp + ".convs1.1", A1, wb.A1_lo, ch, ch, L, c.resblock_dilations[j][1], Hb, 1, nullptr, nullptr, wb.Hb_lo);
+            snap(rp, ".convs1.1", Hb, na, ofmt);
+            conv(geom, rp + ".convs2.1", Hb, wb.Hb_lo, ch, ch, L, 1, X2, 0, X1, A2, wb.A2_lo);
+            snap(rp, ".convs2.1.x", X2, na, 1); snap(rp, ".convs2.1.a", A2, na, ofmt);
+            conv(geom, rp + ".convs1.2", A2, wb.A2_lo, ch, ch, L, c.resblock_dilations[j][2], Hb, 1, nullptr, nullptr, wb.Hb_lo);
+            snap(rp, ".convs1.2", Hb, na, ofmt);
+            conv(geom, rp + ".convs2.2", Hb, wb.Hb_lo, ch, ch, L, 1, R[j], 0, X2, nullptr, nullptr);
+            snap(rp, ".convs2.2.x", R[j], na, 1);
         }
         // x = xs / num_kernels, then the next consumer's leaky_relu: LRELU_SLOPE before the next ups, torch's default 0.01
-        // before conv_post (models.py:107,114-115).  SA is free again: its only reader was this stage's GEMM.
+        // before conv_post (models.py:107,114-115).  SA is free again: its only reader was this stage's GEMM.  conv_post's
+        // input is fp32 in every mode and goes to X0 (its last reader, this stage's first convs2, is done).
         const long long n4 = (long long)B * (ch / 4) * L;
+        const bool last = i + 1 == c.n_ups;
+        void* mo = last ? (void*)X0 : SA;
         k_voc_mrf<<<ew_grid(n4), 256, 0, s>>>(reinterpret_cast<const float4*>(R[0]), reinterpret_cast<const float4*>(R[1]), reinterpret_cast<const float4*>(R[2]),
-                                               reinterpret_cast<float4*>(SA), n4, 1.0f / 3.0f, i + 1 < c.n_ups ? kSlope : 0.01f); ++n;
-        if (v->capture) snap("mrf." + std::to_string(i), "", SA, na);
+                                               mo, last ? nullptr : wb.SA_lo, n4, L, 1.0f / 3.0f, last ? 0.01f : kSlope, (bf && !last) ? 1 : 0); ++n;
+        if (v->capture) snap("mrf." + std::to_string(i), "", mo, na, last ? 1 : ofmt);
+        if (last) post_in = X0;
     }
-    k_voc_post<<<ew_grid((long long)B * L), 256, 7 * ch * sizeof(float), s>>>(SA, W("conv_post.weight"), W("conv_post.bias"), wav, B, ch, L); ++n;
-    snap("wav", "", wav, bn * L);
+    k_voc_post<<<ew_grid((long long)B * L), 256, 7 * ch * sizeof(float), s>>>(post_in, Wf("conv_post.weight"), Wf("conv_post.bias"), wav, B, ch, L); ++n;
+    snap("wav", "", wav, bn * L, 1);
     if (v->capture) {
         for (size_t i = nsnap; i < v->snaps.size(); ++i) cudaFree(v->snaps[i].buf);
         v->snaps.resize(nsnap);
@@ -417,6 +502,11 @@ extern "C" const char* sbk_vocoder_debug_name(const sbk_vocoder* v, int i) {
     if (!v || i < 0 || i >= (int)v->snaps.size()) return nullptr;
     return v->snaps[i].name.c_str();
 }
+extern "C" int sbk_vocoder_debug_op_layout(const sbk_vocoder* v, const char* name) {
+    if (!v || !name) return -1;
+    for (auto& sn : v->snaps) if (sn.name == name) return sn.fmt;
+    return -1;
+}
 extern "C" int sbk_vocoder_debug_read(sbk_vocoder* v, const char* name, float* dst, int64_t* numel) {
     if (!v || !name) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_debug_read: null argument");
     for (auto& sn : v->snaps) {
@@ -425,7 +515,16 @@ extern "C" int sbk_vocoder_debug_read(sbk_vocoder* v, const char* name, float* d
         if (dst && sn.numel > 0) {
             VCU(cudaSetDevice(v->cfg.device));
             VCU(cudaDeviceSynchronize());
-            VCU(cudaMemcpy(dst, sn.buf, sn.numel * sizeof(float), cudaMemcpyDefault));
+            if (sn.fmt == 2) {
+                // bf16 snapshot: widened to fp32 on the host (exact), element order unchanged; dst may be host or device memory
+                std::vector<uint16_t> h16(sn.numel);
+                VCU(cudaMemcpy(h16.data(), sn.buf, sn.numel * 2, cudaMemcpyDeviceToHost));
+                std::vector<float> h32(sn.numel);
+                for (size_t i = 0; i < sn.numel; ++i) { const uint32_t u = (uint32_t)h16[i] << 16; memcpy(&h32[i], &u, 4); }
+                VCU(cudaMemcpy(dst, h32.data(), sn.numel * sizeof(float), cudaMemcpyDefault));
+            } else {
+                VCU(cudaMemcpy(dst, sn.buf, sn.numel * sizeof(float), cudaMemcpyDefault));
+            }
         }
         return SBK_OK;
     }

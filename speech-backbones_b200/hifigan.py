@@ -11,6 +11,10 @@ Same constructor argument, same parameter names (`conv_pre.weight_g/_v`, `ups.i.
 and the plain `.weight` names after `remove_weight_norm()`), so the reference checkpoint loads with `strict=True`.  The modules
 below are parameter containers only: `forward` runs in libsbk.so (`sbk_vocoder_forward`: dilated Conv1d and the transposed
 convs on wgmma, see csrc/sbk_vocoder.cu).  There is no CPU or eager-PyTorch path: calling `forward` with CPU tensors raises.
+
+`Generator(h, precision=...)` picks the operand arithmetic of those convs (the binding's PREC names): "tf32" (the default),
+"fp32x3" ("fp32" maps to it: fp32-class results on the tensor cores) or "bf16".  In the bf16 mode `forward` also takes a
+bfloat16 mel (widened to float32 first); the waveform is float32 in every mode.
 """
 from __future__ import annotations
 
@@ -20,7 +24,7 @@ import torch
 import torch.nn as nn
 from torch.nn.utils import remove_weight_norm, weight_norm
 
-from .binding import _check, _ptr, load_library
+from .binding import PREC, _check, _ptr, load_library
 
 
 class SbkVocoderConfig(C.Structure):
@@ -48,10 +52,17 @@ class _ResBlock1(nn.Module):                                   # reference name:
             remove_weight_norm(l)
 
 
-class VocoderEngine:
-    """One sbk_vocoder handle (device + packed weights + workspace)."""
+def _check_precision(precision):
+    if precision not in PREC:
+        raise ValueError(f"precision must be one of {sorted(PREC)}, got {precision!r}")
+    return precision
 
-    def __init__(self, h, device):
+
+class VocoderEngine:
+    """One sbk_vocoder handle (device + packed weights + workspace) in one precision mode."""
+
+    def __init__(self, h, device, precision="tf32"):
+        self.precision = _check_precision(precision)
         self.lib = load_library()
         P, I = C.c_void_p, C.c_int
         self.lib.sbk_vocoder_create.argtypes = [C.POINTER(SbkVocoderConfig), C.POINTER(P)]
@@ -62,6 +73,8 @@ class VocoderEngine:
         self.lib.sbk_vocoder_weight_name.restype = C.c_char_p
         self.lib.sbk_vocoder_set_weight.argtypes = [P, C.c_char_p, P, C.POINTER(C.c_int64), I]
         self.lib.sbk_vocoder_pack.argtypes = [P]
+        self.lib.sbk_vocoder_set_precision.argtypes = [P, C.c_int32]
+        self.lib.sbk_vocoder_debug_op_layout.argtypes = [P, C.c_char_p]
         self.lib.sbk_vocoder_workspace_bytes.argtypes = [P, I, I]
         self.lib.sbk_vocoder_workspace_bytes.restype = C.c_size_t
         self.lib.sbk_vocoder_forward.argtypes = [P, P, P, I, I, P]
@@ -89,6 +102,10 @@ class VocoderEngine:
                 cfg.resblock_dilations[j][d] = rd[j][d]
         self.h = C.c_void_p()
         _check(self.lib.sbk_vocoder_create(C.byref(cfg), C.byref(self.h)), "sbk_vocoder_create")
+        rc = self.lib.sbk_vocoder_set_precision(self.h, PREC[precision])
+        if rc != 0:
+            self.close()
+            _check(rc, f"sbk_vocoder_set_precision({precision})")
         self.device = device
         self.num_mels = cfg.num_mels
         self.rates = rates
@@ -130,8 +147,11 @@ class VocoderEngine:
             raise RuntimeError(f"mel lives on {mel.device}; the vocoder runs only on cuda:{self.device} (no CPU path)")
         if mel.dim() != 3 or mel.shape[1] != self.num_mels:
             raise RuntimeError(f"mel shape {tuple(mel.shape)}: expected [B, {self.num_mels}, T]")
+        if mel.dtype == torch.bfloat16 and self.precision == "bf16":
+            mel = mel.float()                                   # exact; the mode stores the mel as bf16 operands anyway
         if mel.dtype != torch.float32:
-            raise RuntimeError(f"mel: expected float32, got {mel.dtype}")
+            extra = " (or bfloat16 in the bf16 mode)" if self.precision != "bf16" else " or bfloat16"
+            raise RuntimeError(f"mel: expected float32{extra}, got {mel.dtype} (precision={self.precision!r})")
         mel = mel.contiguous()
         B, _, T = mel.shape
         wav = torch.empty((B, 1, T * self.hop), dtype=torch.float32, device=mel.device)
@@ -170,6 +190,10 @@ class VocoderEngine:
             L *= u
         return L
 
+    def debug_op_layout(self, name):
+        """1: fp32 [B][C/4][L][4], 2: bf16 [B][C/8][L][8] (read back widened to fp32), -1: not captured"""
+        return int(self.lib.sbk_vocoder_debug_op_layout(self.h, name.encode()))
+
     def debug_read(self, name):
         """captured tensor `name` as a [B, C, L] fp32 CUDA tensor (wav: [B, 1, L])"""
         n = C.c_int64(0)
@@ -180,15 +204,18 @@ class VocoderEngine:
         if name == "wav":
             return flat.view(B, 1, L)
         Ch = n.value // (B * L)
-        return flat.view(B, Ch // 4, L, 4).permute(0, 1, 3, 2).reshape(B, Ch, L)
+        e = 8 if self.debug_op_layout(name) == 2 else 4                # channels per 16-byte chunk
+        return flat.view(B, Ch // e, L, e).permute(0, 1, 3, 2).reshape(B, Ch, L)
 
 
 class Generator(nn.Module):
-    """HiFi-GAN generator (models.py:77-128): parameter tree of the reference, forward in libsbk."""
+    """HiFi-GAN generator (models.py:77-128): parameter tree of the reference, forward in libsbk.  `precision`: the
+    convs' operand arithmetic, one of the binding's PREC names (module docstring)."""
 
-    def __init__(self, h):
+    def __init__(self, h, *, precision="tf32"):
         super().__init__()
         self.h = h
+        self.precision = _check_precision(precision)
         rates, ks = list(_get(h, "upsample_rates")), list(_get(h, "upsample_kernel_sizes"))
         rk, rd = list(_get(h, "resblock_kernel_sizes")), [list(d) for d in _get(h, "resblock_dilation_sizes")]
         c0 = int(_get(h, "upsample_initial_channel"))
@@ -237,7 +264,7 @@ class Generator(nn.Module):
         if self._engine is None or self._engine.device != dev.index:
             if self._engine is not None:
                 self._engine.close()
-            self._engine = VocoderEngine(self.h, dev.index)
+            self._engine = VocoderEngine(self.h, dev.index, self.precision)
             self._engine_sig = None
         if sig != self._engine_sig:
             with torch.cuda.device(dev):
