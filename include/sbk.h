@@ -107,13 +107,28 @@ int sbk_vc_estimator(sbk_handle* h, const float* x, const float* mask, const flo
 int sbk_vc_reverse_diffusion(sbk_handle* h, const float* z, const float* mask, const float* mean, const float* cond,
                              const float* noise, float* out, int B, int T, int n_timesteps, int mode, void* stream);
 
-/* The hoisted conditioning branch natively (tensor-core precision modes only): for every step i (t_i = 1 - i/N)
- * xt_ref = compute_diffused_mean(ref, ref_mask, mean_ref, t_i) (:151-155) -> RefBlock (modules.py:156-166: six
- * Conv3x3 + InstanceNorm2d + GLU on wgmma, two time biases, 1x1 conv, masked mean) -> cond_block over
- * [sinusoid(t_i) | RefBlock | c] (:62-71).  ref, mean_ref: [B,n_feats,Tr]; ref_mask: [B,1,Tr]; c: [B,256];
- * cond_out: [N][B][dim_cond], ready for sbk_vc_reverse_diffusion.  Returns SBK_ERR_UNSUPPORTED in fp32 mode. */
+/* The hoisted conditioning branch natively: for every step i (t_i = 1 - i/N)
+ * xt_ref = compute_diffused_mean(ref, ref_mask, mean_ref, t_i) (:151-155) -> RefBlock (modules.py:156-166: a CUDA-core
+ * first Conv3x3, five Conv3x3 on wgmma, each + InstanceNorm2d + GLU, two time biases, 1x1 conv, masked mean) -> cond_block
+ * over [sinusoid(t_i) | RefBlock | c] (:62-71).  ref, mean_ref: [B,n_feats,Tr]; ref_mask: [B,1,Tr]; c: [B,256];
+ * cond_out: [N][B][dim_cond], ready for sbk_vc_reverse_diffusion.  Every precision mode runs it: tf32 and bf16 handles
+ * with tf32 operands, fp32x3 and fp32 handles with the fp32x3 split (so each pair computes the same table).
+ * SBK_ERR_UNSUPPORTED if a RefBlock conv has no tensor-core kernel. */
 int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float* ref_mask, const float* mean_ref, const float* c,
                         float* cond_out, int B, int Tr, int n_timesteps, void* stream);
+/* test hook: with sbk_debug_capture on, sbk_vc_conditioning copies every tensor the RefBlock branch writes right after the
+ * launch that wrote it into a per-name device buffer (the copies do not count as launches).  Each step overwrites the
+ * previous step's copies, so they hold the LAST step (t = 1/N).  Names in launch order: ref_block.xt_ref [B][H][Tr];
+ * ref_block.tb (the step's time-bias row, [3 * dim_cond / 4]: mlp1 then mlp2); then per block11, block12, block21, block22,
+ * block31, block32: ref_block.<blk>.raw (conv output), .stats ([B][C][2] float64 sums of x and x^2), .act (InstanceNorm +
+ * GLU (+ time bias) * mask); last ref_block.ysum ([B][dim_cond][2] float64).  No names when use_ref_t is 0. */
+int sbk_vc_cond_debug_num(const sbk_handle* h);
+const char* sbk_vc_cond_debug_name(const sbk_handle* h, int i);
+/* 0 = fp32 array, 1 = fp32 [B][H][C/4][Tr][4], 3 = float64 array, -1 = no such name */
+int sbk_vc_cond_debug_op_layout(const sbk_handle* h, const char* name);
+/* copy a snapshot to `dst` (host or device) in its own dtype (float64 for layout 3, else fp32); returns its element count
+ * through *numel; dst may be NULL to query it */
+int sbk_vc_cond_debug_read(sbk_handle* h, const char* name, void* dst, int64_t* numel);
 
 /* The same loop in slices: runs steps [step_begin, step_end) of an n_timesteps-step trajectory in place
  * on xt (which must already hold z*mask at step 0, or the previous slice's result).  noise, when stoc,

@@ -78,8 +78,11 @@ def sinusoid(t, dim, scale):
     """SinusoidalPosEmb.forward, model/diffusion.py:118-125."""
     half = dim // 2
     f = math.log(10000) / (half - 1)
-    f = torch.exp(torch.arange(half, device=t.device).float() * -f)
-    e = scale * t[:, None] * f[None, :]
+    # the fp32 frequency table and the fp32 argument are evaluated on the CPU whatever t's device and dtype: at scale 1000 the
+    # argument reaches ~1000 rad, where one ulp of a frequency (a GPU expf may differ from the CPU's) or a float64 argument
+    # moves it by ~3e-5 (bit-identical to before for fp32 CPU t)
+    f = torch.exp(torch.arange(half).float() * -f)
+    e = ((scale * t.detach().cpu().float())[:, None] * f[None, :]).to(t.device, t.dtype)
     return torch.cat((e.sin(), e.cos()), dim=-1)
 
 

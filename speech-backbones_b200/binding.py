@@ -19,6 +19,7 @@ EXPORTS = [
     "sbk_reverse_diffusion_host", "sbk_last_launch_count", "sbk_debug_read", "sbk_debug_num",
     "sbk_debug_name", "sbk_last_error", "sbk_version", "sbk_profile_ops", "sbk_debug_capture", "sbk_debug_layout", "sbk_debug_op_layout", "sbk_vc_estimator", "sbk_vc_reverse_diffusion", "sbk_vc_conditioning",
     "sbk_prior_expand", "sbk_last_host_launches", "sbk_workspace_bytes_n",
+    "sbk_vc_cond_debug_num", "sbk_vc_cond_debug_name", "sbk_vc_cond_debug_op_layout", "sbk_vc_cond_debug_read",
 ]
 
 
@@ -71,6 +72,11 @@ def load_library() -> C.CDLL:
     lib.sbk_debug_op_layout.argtypes = [P, C.c_char_p]
     lib.sbk_debug_name.argtypes = [P, I]
     lib.sbk_debug_name.restype = C.c_char_p
+    lib.sbk_vc_cond_debug_num.argtypes = [P]
+    lib.sbk_vc_cond_debug_name.argtypes = [P, I]
+    lib.sbk_vc_cond_debug_name.restype = C.c_char_p
+    lib.sbk_vc_cond_debug_op_layout.argtypes = [P, C.c_char_p]
+    lib.sbk_vc_cond_debug_read.argtypes = [P, C.c_char_p, F, C.POINTER(C.c_int64)]
     lib.sbk_profile_ops.argtypes = [P, F, F, F, I, C.POINTER(C.c_int)]
     lib.sbk_last_error.restype = C.c_char_p
     lib.sbk_version.restype = C.c_char_p
@@ -286,7 +292,34 @@ class Engine:
         out = torch.empty((n_timesteps, B, self.dim_cond), dtype=torch.float32, device=ref.device)
         _check(self.lib.sbk_vc_conditioning(self.h, _ptr(ref), _ptr(ref_mask), _ptr(mean_ref), _ptr(c), _ptr(out), B, Tr,
                                             int(n_timesteps), self._stream()), "sbk_vc_conditioning")
+        self._vc_shape = (B, Tr)
         return out
+
+    def vc_cond_debug_names(self):
+        """Tensors the last vc_conditioning call captured (debug_capture on), in launch order; they hold its last step."""
+        return [self.lib.sbk_vc_cond_debug_name(self.h, i).decode() for i in range(self.lib.sbk_vc_cond_debug_num(self.h))]
+
+    def vc_cond_debug_read(self, name):
+        """One captured RefBlock tensor as a CPU float64 tensor: conv-shaped ones ([B][H][C/4][Tr][4] in the kernels) as NCHW
+        [B, C, H, Tr]; xt_ref as [B, H, Tr]; stats / ysum as [B, C, 2]; tb as the flat row."""
+        fmt = int(self.lib.sbk_vc_cond_debug_op_layout(self.h, name.encode()))
+        if fmt < 0:
+            raise RuntimeError(f"vc_cond_debug_read: no captured tensor named '{name}'")
+        n = C.c_int64(0)
+        _check(self.lib.sbk_vc_cond_debug_read(self.h, name.encode(), None, C.byref(n)), "sbk_vc_cond_debug_read")
+        out = torch.empty(n.value, dtype=torch.float64 if fmt == 3 else torch.float32)
+        _check(self.lib.sbk_vc_cond_debug_read(self.h, name.encode(), C.c_void_p(out.data_ptr()), C.byref(n)),
+               "sbk_vc_cond_debug_read")
+        B, Tr = self._vc_shape
+        H = self.n_feats
+        if fmt == 1:                                       # [B][H][C/4][Tr][4] -> [B, C, H, Tr]
+            Cc = n.value // (B * H * Tr)
+            out = out.view(B, H, Cc // 4, Tr, 4).permute(0, 2, 4, 1, 3).reshape(B, Cc, H, Tr)
+        elif fmt == 3:
+            out = out.view(B, -1, 2)
+        elif name.endswith(".xt_ref"):
+            out = out.view(B, H, Tr)
+        return out.double().contiguous()
 
     def vc_reverse_diffusion(self, z, mask, mean, cond, n_timesteps, mode, noise=None):
         B, T = self._check_inputs(z, mask, mean, None)

@@ -118,6 +118,9 @@ struct sbk_handle {
     int64_t last_launches = 0;
     int last_host_launches = 0;               // graph launches the host issued for the loop of the last sampler call
     bool capture = false;
+    // sbk_vc_conditioning's debug snapshots (names in launch order; fmt: 0 fp32 array, 1 fp32 [B][H][C/4][Tr][4], 3 float64)
+    struct VcSnap { std::string name; void* buf; size_t cap, numel; int fmt; };
+    std::vector<VcSnap> vc_snaps;
     int tb_off[16];
     int tb_total = 0;
 };
@@ -265,6 +268,7 @@ extern "C" void sbk_destroy(sbk_handle* h) {
     for (auto& kv : h->raw) cudaFree(kv.second);
     for (void* p : h->owned) cudaFree(p);
     if (h->ref_mem) cudaFree(h->ref_mem);
+    for (auto& sn : h->vc_snaps) cudaFree(sn.buf);
     if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
     delete h;
 }
@@ -1432,37 +1436,65 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
         if (x3) { p.x3 = 1; p.in0_lo = act_lo; }
         return launch_conv_tc(p, s);
     };
+    // debug capture: every step reuses the workspace, so each tensor the branch writes is copied (stream-ordered) right
+    // after the launch that wrote it into a per-name buffer; step i overwrites step i-1's copies, so the last step remains.
+    // The copies are not launches and do not count in last_launches.
+    size_t nsnap = 0;
+    cudaError_t snap_err = cudaSuccess;
+    auto snap = [&](const char* name, const char* suf, const void* src, size_t numel, int fmt) {
+        if (!h->capture || snap_err != cudaSuccess) return;
+        if (nsnap == h->vc_snaps.size()) h->vc_snaps.push_back({std::string(), nullptr, 0, 0, 0});
+        sbk_handle::VcSnap& sn = h->vc_snaps[nsnap++];
+        const size_t bytes = numel * (fmt == 3 ? sizeof(double) : sizeof(float));
+        sn.name = std::string("ref_block.") + name + suf; sn.numel = numel; sn.fmt = fmt;
+        if (bytes > sn.cap) {
+            cudaFree(sn.buf); sn.buf = nullptr; sn.cap = 0;
+            if ((snap_err = cudaMalloc(&sn.buf, bytes)) != cudaSuccess) { sn.buf = nullptr; sn.numel = 0; return; }
+            sn.cap = bytes;
+        }
+        snap_err = cudaMemcpyAsync(sn.buf, src, bytes, cudaMemcpyDeviceToDevice, s);
+    };
     auto norm_glu = [&](const char* name, int C, const float* tbias) {
         const std::string q = std::string("estimator.ref_block.") + name;
         ChanStatsParams cs{raw, st, B, H, Tr, C};
         int k = launch_chan_stats(cs, s);
+        snap(name, ".stats", st, (size_t)B * C * 2, 3);
         InGluParams g; memset(&g, 0, sizeof(g));
         g.raw = raw; g.stats = st; g.gamma = W(q + ".1.weight"); g.beta = W(q + ".1.bias"); g.tb = tbias;
         g.mask = ref_mask; g.T = Tr; g.out = act; g.out_lo = act_lo; g.B = B; g.H = H; g.W = Tr; g.C = C;
-        return k + launch_in_glu(g, s);
+        k += launch_in_glu(g, s);
+        snap(name, ".act", act, px * C / 2, 1);
+        return k;
     };
+    // the five wgmma convs, each followed by its InstanceNorm + GLU; tb_off: offset of the stage's time bias in a tb row
+    struct Stage { const char* name; int cin, cout, tb_off; };
+    const Stage stages[5] = {{"block12", base, 2 * base, 0}, {"block21", base, 4 * base, -1}, {"block22", 2 * base, 4 * base, base},
+                             {"block31", 2 * base, 8 * base, -1}, {"block32", 4 * base, 8 * base, -1}};
     for (int i = 0; i < N; ++i) {
+        nsnap = 0;
         if (cf.use_ref_t) {
+            const float* tb_row = tb + (size_t)i * 3 * base;
             DiffMeanParams dm{ref, mean_ref, ref_mask, xt_ref, (float)gamma0(1.0 - i * (1.0 / N)), B, H, Tr};
             n += launch_diff_mean(dm, s);
+            snap("xt_ref", "", xt_ref, px, 0);
+            snap("tb", "", tb_row, (size_t)3 * base, 0);
             FirstConvParams fc; memset(&fc, 0, sizeof(fc));
             fc.mu = xt_ref; fc.xt = xt_ref; fc.mask = ref_mask; fc.w = W("estimator.ref_block.block11.w");
             fc.bias = W("estimator.ref_block.block11.0.bias"); fc.out = raw; fc.ostats = nullptr;
             fc.B = B; fc.H = H; fc.T = Tr; fc.cin = 1; fc.C = 2 * base; fc.chw4 = 1;
             n += launch_first_conv(fc, s);
+            snap("block11", ".raw", raw, px * 2 * base, 1);
             n += norm_glu("block11", 2 * base, nullptr);
-            n += conv("block12", base, 2 * base);
-            n += norm_glu("block12", 2 * base, tb + (size_t)i * 3 * base);
-            n += conv("block21", base, 4 * base);
-            n += norm_glu("block21", 4 * base, nullptr);
-            n += conv("block22", 2 * base, 4 * base);
-            n += norm_glu("block22", 4 * base, tb + (size_t)i * 3 * base + base);
-            n += conv("block31", 2 * base, 8 * base);
-            n += norm_glu("block31", 8 * base, nullptr);
-            n += conv("block32", 4 * base, 8 * base);
-            n += norm_glu("block32", 8 * base, nullptr);
+            for (const Stage& sg : stages) {
+                const int k = conv(sg.name, sg.cin, sg.cout);
+                if (k < 0) return fail(SBK_ERR_UNSUPPORTED, "sbk_vc_conditioning: the tensor-core conv of %s was refused", sg.name);
+                n += k;
+                snap(sg.name, ".raw", raw, px * sg.cout, 1);
+                n += norm_glu(sg.name, sg.cout, sg.tb_off < 0 ? nullptr : tb_row + sg.tb_off);
+            }
             ChanStatsParams ysm{act, ys, B, H, Tr, 4 * base};
             n += launch_chan_stats(ysm, s);
+            snap("ysum", "", ys, (size_t)B * dc * 2, 3);
         }
         VcCondParams vp; memset(&vp, 0, sizeof(vp));
         vp.ysum = ys; vp.mask = ref_mask; vp.Tr = Tr; vp.H = H;
@@ -1473,9 +1505,39 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
         vp.out = cond_out + (size_t)i * B * dc; vp.B = B; vp.dc = dc; vp.use_ref = cf.use_ref_t ? 1 : 0;
         n += launch_vc_cond(vp, s);
     }
+    if (h->capture) {
+        for (size_t i = nsnap; i < h->vc_snaps.size(); ++i) cudaFree(h->vc_snaps[i].buf);
+        h->vc_snaps.resize(nsnap);
+    }
+    if (snap_err != cudaSuccess) return fail(SBK_ERR_CUDA, "sbk_vc_conditioning: debug capture failed: %s", cudaGetErrorString(snap_err));
     CU(cudaGetLastError());
     h->last_launches = n;
     return SBK_OK;
+}
+
+extern "C" int sbk_vc_cond_debug_num(const sbk_handle* h) { return h ? (int)h->vc_snaps.size() : 0; }
+extern "C" const char* sbk_vc_cond_debug_name(const sbk_handle* h, int i) {
+    if (!h || i < 0 || i >= (int)h->vc_snaps.size()) return nullptr;
+    return h->vc_snaps[i].name.c_str();
+}
+extern "C" int sbk_vc_cond_debug_op_layout(const sbk_handle* h, const char* name) {
+    if (!h || !name) return -1;
+    for (auto& sn : h->vc_snaps) if (sn.name == name) return sn.fmt;
+    return -1;
+}
+extern "C" int sbk_vc_cond_debug_read(sbk_handle* h, const char* name, void* dst, int64_t* numel) {
+    if (!h || !name) return fail(SBK_ERR_ARG, "sbk_vc_cond_debug_read: null argument");
+    for (auto& sn : h->vc_snaps) {
+        if (sn.name != name) continue;
+        if (numel) *numel = (int64_t)sn.numel;
+        if (dst && sn.numel > 0) {
+            CU(cudaSetDevice(h->cfg.device));
+            CU(cudaDeviceSynchronize());
+            CU(cudaMemcpy(dst, sn.buf, sn.numel * (sn.fmt == 3 ? sizeof(double) : sizeof(float)), cudaMemcpyDefault));
+        }
+        return SBK_OK;
+    }
+    return fail(SBK_ERR_ARG, "sbk_vc_cond_debug_read: no intermediate named '%s'", name);
 }
 
 extern "C" int sbk_prior_expand(const float* mu_x, const float* w_ceil, const float* x_mask, const int64_t* y_lengths,

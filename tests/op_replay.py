@@ -101,30 +101,42 @@ def _group_norms(t, dims):
     return t.pow(2).sum(dim=dims).sqrt().flatten()
 
 
-def groupings(x):
-    """[B,C,H,W] -> {name: (reduce dims or channel-block view)}: columns (b,w), rows (b,h), 64-channel N-tile blocks."""
+def groupings(x, ntile=64, period=None):
+    """[B,C,H,W] -> {name: (reduce dims or channel-block view)}: columns (b,w), rows (b,h), `ntile`-channel N-tile blocks,
+    and with `period`, the column phase w % period over the full period-wide tiles (the image's border columns left out)."""
     B, C, H, W = x.shape
-    nb = (C + 63) // 64
+    nb = (C + ntile - 1) // ntile
     out = {"col": lambda t: _group_norms(t, (1, 2)), "row": lambda t: _group_norms(t, (1, 3))}
     if nb > 1:
-        pad = nb * 64 - C
+        pad = nb * ntile - C
 
         def blk(t):
             t = F.pad(t, (0, 0, 0, 0, 0, pad)) if pad else t
-            return t.view(B, nb, 64, H, W).pow(2).sum(dim=(0, 2, 3, 4)).sqrt()
+            return t.view(B, nb, ntile, H, W).pow(2).sum(dim=(0, 2, 3, 4)).sqrt()
         out["ntile"] = blk
-    sizes = {"col": C * H, "row": C * W, "ntile": B * 64 * H * W}
+    sizes = {"col": C * H, "row": C * W, "ntile": B * ntile * H * W}
     # class of each group: 1 for the image's first / last column (row), 0 otherwise
     edge = lambda n: torch.tensor([i in (0, n - 1) for i in range(n)] * B, device=x.device)
     classes = {"col": edge(W), "row": edge(H), "ntile": torch.zeros(nb, dtype=torch.bool, device=x.device)}
+    nfull = W // period if period else 0
+    if nfull >= 1:
+        def phase(t):
+            t = t[..., :nfull * period].clone()
+            t[..., 0] = 0
+            if nfull * period == W:
+                t[..., W - 1] = 0
+            return t.reshape(B, C, H, nfull, period).pow(2).sum(dim=(0, 1, 2, 3)).sqrt()
+        out["phase"] = phase
+        sizes["phase"] = B * C * H * nfull
+        classes["phase"] = torch.zeros(period, dtype=torch.bool, device=x.device)
     return out, sizes, classes
 
 
-def uniformity(err, A, Alin=None, min_group=MIN_GROUP, valid=None):
+def uniformity(err, A, Alin=None, min_group=MIN_GROUP, valid=None, ntile=64, period=None):
     """max over groupings of  max_g e_g / median of the other groups' e_g  (0 when the error is zero everywhere).
     `valid` (0/1, the shape of err): groups with fewer than min_group valid elements are left out."""
     Alin = A if Alin is None else Alin
-    fns, sizes, classes = groupings(err)
+    fns, sizes, classes = groupings(err, ntile, period)
     worst, where = 0.0, ""
     for name, fn in fns.items():
         if sizes[name] < min_group:
@@ -205,17 +217,19 @@ def uniformity1d(err, Alin, pad=0, ntile=128, min_group=MIN_GROUP):
     return worst, where
 
 
-def check(got, ref, A, kap, floor=0.0, Alin=None, groups=True, min_group=MIN_GROUP, pad=0, ntile=128):
+def check(got, ref, A, kap, floor=0.0, Alin=None, groups=True, min_group=MIN_GROUP, pad=0, ntile=None, period=None,
+          valid=None):
     """-> (elem, unif, where): elem = max |err| / (kappa A + floor) (<= 1 passes), unif = worst max/median group ratio.
-    4-D [B,C,H,W] tensors are grouped as images; 3-D [B,C,L] tensors as 1-D signals (`pad`, `ntile`: uniformity1d)."""
+    4-D [B,C,H,W] tensors are grouped as images (`ntile`, default 64, `period` and `valid`: groupings / uniformity);
+    3-D [B,C,L] tensors as 1-D signals (`pad`, `ntile`, default 128: uniformity1d)."""
     got, ref, A = got.double(), ref.double(), A.double()
     err = (got - ref).abs()
     tiny = torch.finfo(torch.float32).tiny
     elem = (err / (kap * A + floor + tiny)).max().item()
     if groups and err.dim() == 4:
-        unif, where = uniformity(err, A, Alin, min_group)
+        unif, where = uniformity(err, A, Alin, min_group, valid, ntile=ntile or 64, period=period)
     elif groups and err.dim() == 3:
-        unif, where = uniformity1d(err, A if Alin is None else Alin, pad, ntile, min_group)
+        unif, where = uniformity1d(err, A if Alin is None else Alin, pad, ntile or 128, min_group)
     else:
         unif, where = 0.0, ""
     return elem, unif, where
@@ -750,4 +764,273 @@ class VocoderReplay:
             assert got.shape == ref.shape, f"{name}: captured {tuple(got.shape)} vs replay {tuple(ref.shape)}"
             rows.append((name,) + check(got, ref, A, k, floor, Alin, pad=pad, ntile=nt))
         assert rows and rows[-1][0] == "wav", "the vocoder no longer captures wav last"
+        return rows
+
+
+# ---- DiffVC's RefBlock conditioning branch (sbk_api.cu sbk_vc_conditioning), replayed op by op -----------------------------
+# One sbk_vc_conditioning call with capture on keeps the tensors of its last step (t = 1/N): the diffused reference, the
+# step's time-bias row, and per block the conv output (raw), the InstanceNorm sums (stats) and IN + GLU (+ bias) * mask (act),
+# then the masked-mean sums (ysum).  Each is recomputed in float64 from the GPU's own captured inputs with the semantics of
+# oracle/diffvc_oracle.py ref_block / conditioning.  The branch runs tf32 operands on tf32 / bf16 handles and the fp32x3
+# split on fp32x3 / fp32 handles.
+RB_BLOCKS = ("block11", "block12", "block21", "block22", "block31", "block32")
+RB_TBIAS = {"block12": (0, 1), "block22": (1, 3)}        # the block's slice of a tb row, in units of base = dim_cond / 4
+FIRST_CONV_TILE = 256                                    # k_first_conv: 256 frames of one row per CTA, 64 output channels
+TC_TILE = 128                                            # k_conv_tc<G_C3>: 128-pixel tiles of one row
+U32 = 2 ** -24
+# sinf / cosf: at most 2 ulp (CUDA C Programming Guide, "Mathematical Functions"), one ulp <= 2^-23 of the value
+SIN_ULP = 2 * 2 ** -23
+# k_in_glu, on top of the operand / activation roundings: fp32 (raw - mean), the fma with scale and beta, the mean and
+# rstd * gamma rounded to fp32 from statistics that may land one ulp away from the float64 ones, the sigmoid (2 ulp expf +
+# the division, or EPS_NL for __expf / __fdividef), the product with the value half and the time-bias add
+IN_GLU_ROUNDINGS = 10
+
+
+def rb_branch_mode(precision):
+    return "fp32x3" if precision in ("fp32", "fp32x3") else "tf32"
+
+
+def rb_ntile(cout):
+    """N tile of the RefBlock's wgmma convs (sbk_conv_tc.cu conv_tc_ntile(G_C3, Cout), no planner override)"""
+    return 128 if cout % 128 == 0 else 64
+
+
+def rb_chain(Tr):
+    """fp32 terms a k_chan_stats thread sums before it flushes to float64: 8 rows of ceil(Tr / 256) columns"""
+    return 8 * math.ceil(Tr / 256)
+
+
+def rb_conv(x, mask, w, b, got, mode, first=False):
+    """blockXY.raw: Conv3x3(x * mask) + bias (ref_block's cig).  block11 runs on CUDA cores (k_first_conv, a 9-term FFMA
+    chain from the bias); the others on wgmma (kappa(mode, 9 Cin)).  Uniformity over columns, rows, the conv's N tiles and
+    the phase within its pixel tile; the image's border and the columns past a mask edge are left to check 1."""
+    m4 = mask[:, None, None, :]
+    ref, A, floor, Alin = _lin(F.conv2d, x * m4, w, b, padding=1)
+    if first:
+        return check(got, ref, A, kappa("fp32", 9 * w.shape[1]), floor, Alin, ntile=64, period=FIRST_CONV_TILE)
+    return check(got, ref, A, kappa(mode, 9 * w.shape[1]), floor, Alin, ntile=rb_ntile(w.shape[0]), period=TC_TILE)
+
+
+def rb_stats(raw, got, Tr):
+    """[B,C,2] sums of x and x^2 over all H * Tr pixels (F.instance_norm normalises over the padded columns too).  Each
+    k_chan_stats thread runs fp32 chains of rb_chain(Tr) terms (<= that many roundings of 2^-24 of the sum of |terms|),
+    flushed into float64 (H * Tr more adds of 2^-53)."""
+    s, q = raw.sum((2, 3)), (raw * raw).sum((2, 3))
+    ref = torch.stack([s, q], -1)
+    A = torch.stack([raw.abs().sum((2, 3)), q], -1)
+    k = rb_chain(Tr) * U32 + raw.shape[2] * raw.shape[3] * 2 ** -53
+    return check(got, ref, A, k, groups=False)
+
+
+def rb_var_error(raw, got):
+    """worst relative error of the variance k_in_glu derives from the captured sums, against the float64 variance"""
+    n = raw.shape[2] * raw.shape[3]
+    m = got[..., 0] / n
+    var_gpu = (got[..., 1] / n - m * m).clamp_min(0.0)
+    var = raw.var(dim=(2, 3), unbiased=False)
+    return ((var_gpu - var).abs() / var.clamp_min(1e-300)).max().item()
+
+
+def in_glu(raw, gamma, beta, tb, mask, mode):
+    """k_in_glu on a captured raw [B,C,H,Tr]: InstanceNorm2d(affine) + GLU (+ time bias) * mask, float64 apart from the
+    kernel's own roundings: mean and rstd * gamma to fp32, and in the tf32 branch the output to tf32 (rna).
+    -> (ref, A): A bounds the magnitudes the rounding errors are relative to.  The reference does not mask the GLU output
+    (cig masks the next conv's input instead); the kernel writes zeros there, which the next conv reads."""
+    B, C, H, W = raw.shape
+    n = H * W
+    mean = raw.sum((2, 3)) / n
+    var = ((raw * raw).sum((2, 3)) / n - mean * mean).clamp_min(0.0)
+    mean_f = _f32(mean)[:, :, None, None]
+    scale = _f32(_f32(1.0 / torch.sqrt(var + 1e-5)) * _f32(gamma)[None])[:, :, None, None]
+    d = raw - mean_f
+    xn = d * scale + beta[None, :, None, None]
+    # companion of each normalised value: |raw - mean| |scale| + |beta|, plus |mean| |scale| for the mean's fp32 rounding
+    An = (d.abs() + mean_f.abs()) * scale.abs() + beta.abs()[None, :, None, None]
+    Ch = C // 2
+    xa, xg, Aa, Ag = xn[:, :Ch], xn[:, Ch:], An[:, :Ch], An[:, Ch:]
+    sig = torch.sigmoid(xg)
+    tbv = torch.zeros(Ch, dtype=raw.dtype, device=raw.device) if tb is None else tb
+    m4 = mask[:, None, None, :]
+    y = (xa * sig + tbv[None, :, None, None]) * m4
+    if mode == "tf32":
+        y = round_tf32_rna(y.float()).double()
+    # sigmoid' <= 1/4: an error in xg reaches the output as |xa| / 4 of it
+    A = (Aa + 0.25 * xa.abs() * Ag + tbv.abs()[None, :, None, None]) * m4
+    return y, A
+
+
+def rb_act(raw, gamma, beta, tb, mask, got, mode):
+    ref, A = in_glu(raw, gamma, beta, tb, mask, mode)
+    # tf32: the replay rounds its output as the kernel does, so most elements match exactly and the few whose fp32 value
+    # lies on the other side of a rounding boundary differ by one tf32 step (<= 2^-10 of the value); that sparse error has
+    # no meaningful group ratio (see RB_NO_UNIFORMITY)
+    k = IN_GLU_ROUNDINGS * U32 + (EPS_NL + 2 ** -10 if mode == "tf32" else 0.0)
+    # groups need RB_MIN_VALID unmasked elements: a row of a one-frame reference holds only C/2 values
+    valid = mask[:, None, None, :].expand_as(ref)
+    return check(got, ref, A, k, groups=mode != "tf32", min_group=RB_MIN_VALID, valid=valid)
+
+
+RB_MIN_VALID = 4 * MIN_GROUP
+
+
+RB_NO_UNIFORMITY = {
+    "xt_ref": "elementwise (k_diff_mean, no tiles); held to its per-element bound and to exact zeros past the mask",
+    "tb": "one vector per step (k_time_table); no columns or rows",
+    "stats": "one pair of sums per (sample, channel); no columns or rows",
+    "act.tf32": "the replay is rounded to tf32 as the kernel rounds, so the error is a sparse set of one-step differences",
+    "ysum": "one pair of sums per (sample, channel); no columns or rows",
+    "cond": "one vector per sample (k_vc_cond); no columns or rows",
+}
+
+
+def _libm_expf():
+    import ctypes
+    import ctypes.util
+    f = ctypes.CDLL(ctypes.util.find_library("m")).expf
+    f.argtypes, f.restype = [ctypes.c_float], ctypes.c_float
+    return f
+
+
+def host_freqs(dim):
+    """the sinusoid frequencies libsbk uploads (sbk_api.cu sbk_pack): expf((float)j * (float)(-log(10000) / (half - 1)))"""
+    import numpy as np
+    half = dim // 2
+    neg = float(np.float32(-(math.log(10000.0) / (half - 1))))
+    expf = _libm_expf()
+    return torch.tensor([expf(float(np.float32(np.float32(j) * np.float32(neg)))) for j in range(half)], dtype=torch.float64)
+
+
+def sinusoid_f32(t32, dim, dev):
+    """(emb, bound): [sin | cos] of the fp32 argument fp32(fp32(1000 t) * freq), as k_time_table / k_vc_cond form it"""
+    a = torch.tensor(1000.0, dtype=torch.float32) * torch.tensor(t32, dtype=torch.float32)
+    arg = (a * host_freqs(dim).float()).double().to(dev)
+    emb = torch.cat([arg.sin(), arg.cos()])
+    return emb, SIN_ULP * emb.abs() + 2 ** -149
+
+
+def ffma_layer(x, ex, w, b):
+    """y = b + W x as a fp32 FFMA chain of K = fan-in terms from the bias: (ref, bound) for inputs x with error bound ex"""
+    y = F.linear(x, w, b)
+    prop = F.linear(ex, w.abs())
+    A = F.linear(x.abs(), w.abs(), b.abs()) + prop
+    return y, prop + (w.shape[1] + 1) * U32 * A
+
+
+def mish_layer(h, eh):
+    """Mish (mish_f, the exact closed form) of a value with error bound eh: |Mish'| <= 1.1, plus EPS_NL of 1.1 |h|"""
+    return O.mish(h), 1.1 * eh + EPS_NL * 1.1 * (h.abs() + eh)
+
+
+class RefBlockReplay:
+    """Run one sbk_vc_conditioning call with debug capture and judge every op of its last step against a float64 replay.
+    `sd` is the state_dict the engine holds; ref / mean_ref [B,H,Tr], ref_mask [B,1,Tr], c [B,256] (CPU fp32)."""
+
+    def __init__(self, eng, sd, precision, cfg, ref, ref_mask, mean_ref, c, n_timesteps, dev="cuda"):
+        self.eng, self.cfg, self.dev, self.N = eng, cfg, dev, n_timesteps
+        self.mode = rb_branch_mode(precision)
+        eng.debug_capture(True)
+        try:
+            self.table = eng.vc_conditioning(ref.cuda(), ref_mask.cuda(), mean_ref.cuda(), c.cuda(), n_timesteps)
+            torch.cuda.synchronize()
+        finally:
+            eng.debug_capture(False)
+        self.names = eng.vc_cond_debug_names()
+        self.cap = {n: eng.vc_cond_debug_read(n).to(dev) for n in self.names}
+        d = torch.float64
+        self.p = {k: v.to(dev, d) for k, v in sd.items()}
+        self.ref, self.mean_ref, self.c = ref.to(dev, d), mean_ref.to(dev, d), c.to(dev, d)
+        self.mask = ref_mask[:, 0].to(dev, d)
+        self.B, self.H, self.Tr = ref.shape
+        # the host's scalars of the last step: t as fp32(1 - i / N), gamma(0, t) in double from the fp32 config betas
+        i = n_timesteps - 1
+        td = 1.0 - i * (1.0 / n_timesteps)
+        self.t32 = float(torch.tensor(td, dtype=torch.float32))
+        bmin, bmax = (float(torch.tensor(v, dtype=torch.float32)) for v in (cfg.beta_min, cfg.beta_max))
+        bi = bmin + 0.5 * (bmax - bmin) * td
+        bi *= td
+        self.g = float(torch.tensor(math.exp(-0.5 * bi), dtype=torch.float32))
+        self.base = cfg.dim_spk // 4
+
+    def _w(self, blk, part):
+        return self.p[f"estimator.ref_block.{blk}.{part}"]
+
+    def xt_ref(self):
+        g = self.g
+        m = self.mask[:, None, :]
+        ref = (self.ref * g + self.mean_ref * (1.0 - g)) * m
+        A = ((self.ref * g).abs() + (self.mean_ref * (1.0 - g)).abs()) * m
+        got = self.cap["ref_block.xt_ref"]
+        past = (m == 0).expand_as(got)
+        assert not past.any() or got[past].abs().max().item() == 0.0, "xt_ref: non-zero past the mask"
+        # ref * g, (1 - g), mean_ref * (1 - g) and the sum: four fp32 roundings
+        return check(got, ref, A, 4 * U32, groups=False)
+
+    def time_bias(self):
+        """tb: k_time_table's Linear(dim, 4 dim) -> Mish -> Linear(4 dim, dim) -> Mish -> mlp1 | mlp2 on this step's t"""
+        p = self.p
+        emb, e = sinusoid_f32(self.t32, self.cfg.dim_unet, self.dev)
+        h, e = ffma_layer(emb, e, p["estimator.mlp.0.weight"], p["estimator.mlp.0.bias"])
+        h, e = mish_layer(h, e)
+        h, e = ffma_layer(h, e, p["estimator.mlp.2.weight"], p["estimator.mlp.2.bias"])
+        h, e = mish_layer(h, e)
+        outs = [ffma_layer(h, e, p[f"estimator.ref_block.{m}.1.weight"], p[f"estimator.ref_block.{m}.1.bias"])
+                for m in ("mlp1", "mlp2")]
+        ref, bound = torch.cat([o[0] for o in outs]), torch.cat([o[1] for o in outs])
+        return check(self.cap["ref_block.tb"], ref, bound, 1.0, groups=False)
+
+    def cond(self):
+        """the step's cond row from the captured ysum: ybar = ysum / (sum(mask) H) rounded to fp32 as k_vc_cond rounds it,
+        final_conv, then cond_block over [sinusoid | final_conv(ybar) | c]"""
+        p, dev = self.p, self.dev
+        emb, e_emb = sinusoid_f32(self.t32, self.cfg.dim_unet, dev)
+        emb, e_emb = emb.expand(self.B, -1), e_emb.expand(self.B, -1)
+        parts, errs = [emb], [e_emb]
+        if self.cfg.use_ref_t:
+            den = self.mask.sum(1, keepdim=True) * self.H
+            ybar = _f32(self.cap["ref_block.ysum"][..., 0] / den)
+            y, e = ffma_layer(ybar, torch.zeros_like(ybar), p["estimator.ref_block.final_conv.weight"][:, :, 0, 0],
+                              p["estimator.ref_block.final_conv.bias"])
+            parts.append(y)
+            errs.append(e)
+        parts.append(self.c)
+        errs.append(torch.zeros_like(self.c))
+        h, e = ffma_layer(torch.cat(parts, 1), torch.cat(errs, 1), p["estimator.cond_block.0.weight"],
+                          p["estimator.cond_block.0.bias"])
+        h, e = mish_layer(h, e)
+        ref, bound = ffma_layer(h, e, p["estimator.cond_block.2.weight"], p["estimator.cond_block.2.bias"])
+        return check(self.table[-1].to(dev, torch.float64), ref, bound, 1.0, groups=False)
+
+    def run(self):
+        """-> rows (name, elem, unif, where); raises on a captured name this replay does not know, and on a non-zero act
+        past the mask.  Also -> self.var_err: {block: worst relative error of the variance from the captured sums}."""
+        rows, self.var_err = [], {}
+        known = {"ref_block.xt_ref", "ref_block.tb", "ref_block.ysum"}
+        known |= {f"ref_block.{b}.{s}" for b in RB_BLOCKS for s in ("raw", "stats", "act")}
+        for name in self.names:
+            assert name in known, f"unknown RefBlock op '{name}': add a replay for it"
+        if self.cfg.use_ref_t:
+            assert self.names[:2] == ["ref_block.xt_ref", "ref_block.tb"] and self.names[-1] == "ref_block.ysum", self.names
+            rows.append(("xt_ref",) + self.xt_ref())
+            rows.append(("tb",) + self.time_bias())
+            x = self.cap["ref_block.xt_ref"][:, None]
+            for blk in RB_BLOCKS:
+                raw = self.cap[f"ref_block.{blk}.raw"]
+                rows.append((f"{blk}.raw",) + rb_conv(x, self.mask, self._w(blk, "0.weight"), self._w(blk, "0.bias"), raw,
+                                                     self.mode, first=blk == "block11"))
+                st = self.cap[f"ref_block.{blk}.stats"]
+                rows.append((f"{blk}.stats",) + rb_stats(raw, st, self.Tr))
+                self.var_err[blk] = rb_var_error(raw, st)
+                tb = None
+                if blk in RB_TBIAS:
+                    lo, hi = RB_TBIAS[blk]
+                    tb = self.cap["ref_block.tb"][lo * self.base:hi * self.base]
+                x = self.cap[f"ref_block.{blk}.act"]
+                past = (self.mask == 0)[:, None, None, :].expand_as(x)
+                assert not past.any() or x[past].abs().max().item() == 0.0, f"{blk}.act: non-zero past the mask"
+                rows.append((f"{blk}.act",) + rb_act(raw, self._w(blk, "1.weight"), self._w(blk, "1.bias"), tb, self.mask, x,
+                                                     self.mode))
+            rows.append(("ysum",) + rb_stats(x, self.cap["ref_block.ysum"], self.Tr))
+        else:
+            assert not self.names, f"use_ref_t = False captured {self.names}"
+        rows.append(("cond",) + self.cond())
         return rows

@@ -9,7 +9,7 @@ import torch
 import torch.nn.functional as F
 
 from helpers import rel_l2
-from op_replay import FLOOR_PER_W, R_UNIFORM, check, ct_fold, kappa, passes
+from op_replay import FIRST_CONV_TILE, FLOOR_PER_W, R_UNIFORM, TC_TILE, check, ct_fold, kappa, passes, rb_act, rb_conv
 from oracle.precision_model import fp32x3_product, round_bf16, round_tf32_rna, trunc_tf32
 
 B, CIN, COUT, H, W = 1, 64, 128, 6, 260
@@ -257,3 +257,115 @@ def test_fold_wrong_tap_index_fails(convt):
     elem, unif, where = _judge_fold(y, convt)
     print(f"fold wrong tap index: |err|/(kappa A) max {elem:.3g}, uniformity {unif:.3g} at {where}")
     assert elem > 1.0 and unif > R_UNIFORM and not passes(elem, unif)
+
+
+# ---- one RefBlock stage (DiffVC's conditioning branch): tf32 3x3 conv + InstanceNorm + GLU + time bias, and the first conv ---
+# Tr = 300 (wgmma tiles 128 | 128 | 44, k_first_conv tiles 256 | 44) with a mask edge at frame 280.  The emulation follows
+# the kernels: k_conv_tc<G_C3> on tf32 operands (the activation is already in tf32 form), k_in_glu's fp32 arithmetic with
+# the fast sigmoid and an rna tf32 output, zero past the mask; k_first_conv as an fp32 conv of the one-channel xt_ref.
+RB_H, RB_TR, RB_LEN, RB_CIN, RB_COUT = 8, 300, 280, 32, 64
+
+
+@pytest.fixture(scope="module")
+def rb_stage():
+    g = torch.Generator().manual_seed(17)
+    mask = (torch.arange(RB_TR) < RB_LEN).double()[None]
+    x = round_tf32_rna(torch.randn(1, RB_CIN, RB_H, RB_TR, generator=g)).double() * mask[:, None, None, :]
+    w = (torch.rand(RB_COUT, RB_CIN, 3, 3, generator=g) * 2 - 1) / (RB_CIN * 9) ** 0.5
+    b = (torch.rand(RB_COUT, generator=g) * 2 - 1) / (RB_CIN * 9) ** 0.5
+    gamma = 1 + 0.1 * torch.randn(RB_COUT, generator=g)
+    beta = 0.1 * torch.randn(RB_COUT, generator=g)
+    tb = 0.5 * torch.randn(RB_COUT // 2, generator=g)
+    xt = torch.randn(1, 1, RB_H, RB_TR, generator=g).double() * mask[:, None, None, :]
+    w1 = (torch.rand(RB_COUT, 1, 3, 3, generator=g) * 2 - 1) / 3
+    b1 = (torch.rand(RB_COUT, generator=g) * 2 - 1) / 3
+    d = torch.float64
+    return dict(mask=mask, x=x, w=w.to(d), b=b.to(d), gamma=gamma.to(d), beta=beta.to(d), tb=tb.float().double(),
+                xt=xt, w1=w1.to(d), b1=b1.to(d))
+
+
+def rb_emulate_conv(s, x=None, w_only=None):
+    x = s["x"] if x is None else x
+    w = round_tf32_rna(s["w"].float()).double() if w_only is None else w_only
+    return F.conv2d(x, w, s["b"] if w_only is None else None, padding=1).float().double()
+
+
+def rb_emulate_in_glu(raw, s, cols=None, swap=False, tb_gate=False):
+    """k_in_glu in fp32: statistics over `cols` (default: every column), mean / rstd * gamma rounded to fp32"""
+    C = raw.shape[1]
+    r = raw if cols is None else raw[..., cols]
+    n = r.shape[2] * r.shape[3]
+    m = r.sum((2, 3)) / n
+    var = ((r * r).sum((2, 3)) / n - m * m).clamp_min(0)
+    mean = m.float()[:, :, None, None]
+    scale = ((1.0 / torch.sqrt(var + 1e-5)).float() * s["gamma"].float()[None])[:, :, None, None]
+    xn = (raw.float() - mean) * scale + s["beta"].float()[None, :, None, None]
+    a, gt = (xn[:, C // 2:], xn[:, :C // 2]) if swap else (xn[:, :C // 2], xn[:, C // 2:])
+    tb = s["tb"].float()[None, :, None, None]
+    y = a * torch.sigmoid(gt + tb) if tb_gate else a * torch.sigmoid(gt) + tb
+    return round_tf32_rna(y).double() * s["mask"][:, None, None, :]
+
+
+def rb_judge_conv(s, raw):
+    return rb_conv(s["x"], s["mask"], s["w"], s["b"], raw, "tf32")
+
+
+def rb_judge_act(s, raw, act):
+    return rb_act(raw, s["gamma"], s["beta"], s["tb"], s["mask"], act, "tf32")
+
+
+def rb_emulate_first(s, xt=None):
+    return F.conv2d(s["xt"] if xt is None else xt, s["w1"], s["b1"], padding=1).float().double()
+
+
+def test_refblock_clean_emulation_passes(rb_stage):
+    s = rb_stage
+    raw = rb_emulate_conv(s)
+    rows = {"raw": rb_judge_conv(s, raw), "act": rb_judge_act(s, raw, rb_emulate_in_glu(raw, s)),
+            "first": rb_conv(s["xt"], s["mask"], s["w1"], s["b1"], rb_emulate_first(s), "tf32", first=True)}
+    for k, (elem, unif, where) in rows.items():
+        print(f"refblock clean {k}: |err|/(kappa A) max {elem:.3f}, uniformity {unif:.2f} at {where}")
+        assert passes(elem, unif), (k, elem, unif, where)
+
+
+def test_refblock_dropped_tap_at_seam_fails(rb_stage):
+    """one of K = 288 terms (tap r=1, s=0 of input channel 0) lost in column 128"""
+    s = rb_stage
+    raw = rb_emulate_conv(s)
+    t = torch.zeros_like(s["w"])
+    t[:, 0, 1, 0] = round_tf32_rna(s["w"][:, 0, 1, 0].float()).double()
+    raw[..., TC_TILE] -= rb_emulate_conv(s, w_only=t)[..., TC_TILE]
+    elem, unif, where = rb_judge_conv(s, raw)
+    print(f"refblock dropped tap: |err|/(kappa A) max {elem:.3g}, uniformity {unif:.3g} at {where}")
+    assert unif > R_UNIFORM and where == f"col[{TC_TILE}]" and not passes(elem, unif)
+
+
+@pytest.mark.parametrize("name", ["stats_over_valid_columns", "glu_halves_swapped", "time_bias_on_gate", "nonzero_past_mask"])
+def test_refblock_in_glu_defect_fails(rb_stage, name):
+    s = rb_stage
+    raw = rb_emulate_conv(s)
+    if name == "stats_over_valid_columns":      # InstanceNorm over the valid frames only: not what F.instance_norm does
+        act = rb_emulate_in_glu(raw, s, cols=slice(0, RB_LEN))
+    elif name == "glu_halves_swapped":
+        act = rb_emulate_in_glu(raw, s, swap=True)
+    elif name == "time_bias_on_gate":
+        act = rb_emulate_in_glu(raw, s, tb_gate=True)
+    else:                                       # the first masked frame keeps its IN + GLU value
+        act = rb_emulate_in_glu(raw, s)
+        full = rb_emulate_in_glu(raw, dict(s, mask=torch.ones_like(s["mask"])))
+        act[..., RB_LEN] = full[..., RB_LEN]
+    elem, unif, where = rb_judge_act(s, raw, act)
+    print(f"refblock {name}: |err|/(kappa A) max {elem:.3g}")
+    assert elem > 10 and not passes(elem, unif)
+
+
+def test_refblock_stale_halo_at_first_conv_seam_fails(rb_stage):
+    """k_first_conv's second 256-frame tile reads its left halo (frame 255) from a stale shared-memory slot (frame 0)"""
+    s = rb_stage
+    raw = rb_emulate_first(s)
+    xs = s["xt"].clone()
+    xs[..., FIRST_CONV_TILE - 1] = xs[..., 0]
+    raw[..., FIRST_CONV_TILE] = rb_emulate_first(s, xs)[..., FIRST_CONV_TILE]
+    elem, unif, where = rb_conv(s["xt"], s["mask"], s["w1"], s["b1"], raw, "tf32", first=True)
+    print(f"refblock stale first-conv halo: |err|/(kappa A) max {elem:.3g}, uniformity {unif:.3g} at {where}")
+    assert elem > 10 and unif > R_UNIFORM and not passes(elem, unif)
