@@ -340,8 +340,9 @@ static int pack_tc(sbk_handle* h, const std::string& src, const std::string& key
     std::vector<float> hs((size_t)cout * cin * taps);
     CU(cudaMemcpy(hs.data(), h->raw[src], hs.size() * sizeof(float), cudaMemcpyDeviceToHost));
     TRY_RC(pack_tc_host(h, hs, key, cout, cin, geom, bf16));
-    // 3x3 convs with >= 128 output channels also get a 64-wide N-tile image: small batches have too few 128-wide tiles to
-    // fill the GPU's SMs, so the planner switches those launches to twice as many half-width tiles
+    // 3x3 convs with >= 128 output channels also get a 64-wide N-tile image: the two-row tiles run 64 channels wide, and
+    // small batches have too few 128-wide tiles to fill the GPU's SMs, so the planner switches those launches to twice as
+    // many half-width tiles
     if (geom == G_C3 && conv_tc_ntile(geom, cout) == 128) TRY_RC(pack_tc_host(h, hs, key + "64", cout, cin, geom, bf16, 64));
     return SBK_OK;
 }
@@ -672,6 +673,8 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
     auto LO = [&](const void* q) -> float* { auto it = bf.lo.find(q); return it == bf.lo.end() ? nullptr : it->second; };
     int num_sms = 132;
     cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, c.device);
+    const char* rows_env = getenv("SBK_CONV3_ROWS");
+    const int conv_rows_env = rows_env ? atoi(rows_env) : 0;
     const bool b16 = c.precision == SBK_PREC_BF16;          // operand tensors in bf16 [B][H][C/8][W][8]
     const double osz = b16 ? 2.0 : 4.0;                     // bytes per operand-tensor element
     const int fmt_raw = use_tc ? 1 : 0, fmt_opnd = b16 ? 2 : fmt_raw;
@@ -717,11 +720,24 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         if (x3) {
             p.x3 = 1; p.in0_lo = LO(in0); p.in1_lo = LO(in1); p.out_lo = geom != G_C3 ? LO(out) : nullptr;
         }
-        if (geom == G_C3 && conv_tc_ntile(geom, cout) == 128) {
-            // tiles of one row x 128 pixels x 128 channels; when they cannot fill half the SMs, use 64-wide N tiles instead
-            const int rows = conv_tc_tile_rows();
-            const long long tiles = (long long)B * ((Ws[lvl] + 127) / 128) * ((Hs[lvl] + rows - 1) / rows) * (cout / 128);
-            if (tiles * 2 <= num_sms && h->packed.count(wkey + "64")) { p.nt = 64; p.wpk = W(wkey + "64"); }
+        if (geom == G_C3) {
+            // Two-row tiles (2 rows x 128 pixels x 64 channels) bring a third less operand traffic from L2 per MAC than
+            // one-row tiles, but there are half as many per 64 channels.  A persistent grid runs ceil(tiles / SMs) waves,
+            // so they are used only from 4 waves on, where the last wave's round-up costs at most a quarter of a wave
+            // more than in the one-row layout.  SBK_CONV3_ROWS = 1 | 2 overrides the choice (A/B runs of one process).
+            const long long wt = (Ws[lvl] + 127) / 128;
+            const long long tiles2 = (long long)B * wt * ((Hs[lvl] + 1) / 2) * (cout / 64);
+            bool two = tiles2 >= 4LL * num_sms;
+            if (conv_rows_env == 1 || conv_rows_env == 2) two = conv_rows_env == 2;
+            const bool wide = conv_tc_ntile(geom, cout) == 128;
+            if (two && (!wide || h->packed.count(wkey + "64"))) {
+                p.rows = 2;
+                if (wide) { p.nt = 64; p.wpk = W(wkey + "64"); }
+            } else if (wide) {
+                // tiles of one row x 128 pixels x 128 channels; when they cannot fill half the SMs, use 64-wide N tiles instead
+                const long long tiles = (long long)B * wt * Hs[lvl] * (cout / 128);
+                if (tiles * 2 <= num_sms && h->packed.count(wkey + "64")) { p.nt = 64; p.wpk = W(wkey + "64"); }
+            }
         }
         const double taps = geom == G_PW ? 1.0 : (geom == G_UP ? 4.0 : 9.0);
         op.flops = 2.0 * B * Hs[lvl] * Ws[lvl] * cout * (c0 + c1) * taps;

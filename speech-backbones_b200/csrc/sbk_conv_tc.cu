@@ -7,8 +7,10 @@
 //
 // Mapping.  One CTA owns one row of TPX = 128 pixels x NT output channels of one sample; each of its two consumer
 // warpgroups owns 64 of the pixels (one m64nNT wgmma per tap and K step).  For the 3x3 conv a row is 128 consecutive
-// frames of one mel bin; for 1x1 convs the image is flattened and a row is any 128 consecutive pixels.  (A 128 x NT tile
-// per CTA keeps the accumulators - and in fp32x3 mode their running sums - in the register file.)
+// frames of one mel bin; for 1x1 convs the image is flattened and a row is any 128 consecutive pixels.  A 3x3 tile may
+// also be two rows x 128 pixels x 64 channels (Geo<G_C3, 2>): each consumer warpgroup owns one row, and every weight stage
+// feeds twice the pixels.  The consumers hold up to 128 accumulator registers (fp32x3: accumulators + running sums)
+// because the producer warpgroup hands its registers over (setmaxnreg).
 //
 // A operand.  Conv inputs are stored in HBM already in operand form (masked; Block activations GroupNorm-ed, Mish-ed
 // and time-biased by k_gn_act, see sbk_kernels.cu), so producing the A tile is a pure copy straight into the wgmma
@@ -19,7 +21,8 @@
 // B operand.  Weights are packed on the host into exactly the per-stage shared-memory image
 // [tap][chunk][cout][16 B] and streamed with one cp.async.bulk per stage, mbarrier complete_tx.
 //
-// Pipeline.  STAGES-deep ring with full_a / full_b / empty mbarriers; a loader warp fills it with bulk copies (the
+// Pipeline.  STAGES-deep ring with full_a / full_b / empty mbarriers; a loader warp (the first warp of the producer
+// warpgroup) fills it with bulk copies (the
 // Downsample gathers are cp.async issued by the consumers themselves) while the consumer warpgroups issue one stage's
 // MMAs back to back, wait for them and free the stage.  The epilogue stages the accumulators through shared
 // memory ([pixel][column]), so one thread owns one pixel and a contiguous run of output channels.
@@ -32,26 +35,36 @@ namespace sbk {
 
 namespace tc {
 
-constexpr int ROWS = 1;               // output rows of TPX pixels per tile
 constexpr int TPX = 128;              // pixels per row = 2 consumer warpgroups x wgmma M (64)
 constexpr int NCONS = 256;            // consumer threads (2 warpgroups): MMAs + epilogue (Downsample: + A gathers)
-constexpr int NTHREADS = NCONS + 32;  // + loader warp
+constexpr int NTHREADS = NCONS + 128; // + producer warpgroup (its first warp is the loader, the other three exit)
+// Register split (setmaxnreg): the CTA starts with 65536 / 384 registers per thread; the producer warpgroup gives most of
+// its share back so that the consumers can hold a 128-register accumulator tile (+ fp32x3 running sums) without spilling.
+constexpr int PROD_REGS = 40, CONS_REGS = 232;
+static_assert(128 * PROD_REGS + NCONS * CONS_REGS <= 65536, "register file");
 
-// geometry of the A tile in shared memory, [16-byte K chunk][row][pixel][16 B]
-template <int GEOM> struct Geo;
-template <> struct Geo<G_C3> { static constexpr int HR = ROWS + 2, PXP = TPX + 2, TAPS = 9, KCH = 2, NACC = 1; };   // 3x3: halo tile
-template <> struct Geo<G_PW> { static constexpr int HR = ROWS, PXP = TPX, TAPS = 1, KCH = 8, NACC = 1; };           // 1x1: plain tile
+// geometry of the A tile in shared memory, [16-byte K chunk][row][pixel][16 B]; ROWS output rows of TPX pixels per tile,
+// NACC accumulators per consumer thread
+template <int GEOM, int R = 1> struct Geo;
+// 3x3: halo tile of R + 2 input rows.  R = 1: consumer warpgroup w owns pixels 64w..64w+63 of the row.  R = 2: warpgroup w
+// owns output row h0 + w, i.e. two m64 pixel blocks (two accumulators) that share every weight descriptor - each weight
+// byte brought to shared memory feeds twice the pixels.
+template <int R> struct Geo<G_C3, R> {
+    static_assert(R == 1 || R == 2, "3x3 tiles are 1 or 2 rows");
+    static constexpr int ROWS = R, HR = R + 2, PXP = TPX + 2, TAPS = 9, KCH = 2, NACC = R;
+};
+template <> struct Geo<G_PW> { static constexpr int ROWS = 1, HR = 1, PXP = TPX, TAPS = 1, KCH = 8, NACC = 1; };           // 1x1: plain tile
 // 3x3 stride 2 (Downsample): 3 input rows; input columns de-interleaved into an odd plane (129 px: 2*w0-1+2i) and
 // an even plane (2*w0+2i) so that consecutive OUTPUT pixels read consecutive smem pixels for every tap.
-template <> struct Geo<G_DOWN> { static constexpr int HR = 2 * ROWS + 1, PXP = 2 * (TPX + 1), TAPS = 9, KCH = 2, NACC = 1; };
+template <> struct Geo<G_DOWN> { static constexpr int ROWS = 1, HR = 3, PXP = 2 * (TPX + 1), TAPS = 9, KCH = 2, NACC = 1; };
 // ConvTranspose2d(4,2,1) (Upsample): per output parity (ph,pw) a 2x2-tap conv over the same 3x3-style input halo;
 // all four phases are computed from one halo tile into 4 accumulators; the stage carries all 16 (kh,kw) taps.
-template <> struct Geo<G_UP> { static constexpr int HR = ROWS + 2, PXP = TPX + 2, TAPS = 16, KCH = 2, NACC = 4; };
+template <> struct Geo<G_UP> { static constexpr int ROWS = 1, HR = 3, PXP = TPX + 2, TAPS = 16, KCH = 2, NACC = 4; };
 
 // Conv1d, K taps, runtime dilation d (HiFi-GAN: K in {3,7,11}, d in {1,3,5}; halo (K-1)*d <= 50 samples): ONE strip of
 // TPX + 64 samples per channel chunk; tap t is the descriptor start t*d samples into it - each input sample is fetched
 // once for all taps.
-template <int K> struct GeoC1 { static constexpr int HR = 1, PXP = ROWS * TPX + 64, TAPS = K, KCH = 2, NACC = 1; };
+template <int K> struct GeoC1 { static constexpr int ROWS = 1, HR = 1, PXP = TPX + 64, TAPS = K, KCH = 2, NACC = 1; };
 template <> struct Geo<G_C1K3> : GeoC1<3> {};
 template <> struct Geo<G_C1K7> : GeoC1<7> {};
 template <> struct Geo<G_C1K11> : GeoC1<11> {};
@@ -61,7 +74,7 @@ template <> struct Geo<G_C1K11> : GeoC1<11> {};
 // stage (K step, kernel row r) holds ONE input row of TPX + 6 pixels per channel chunk (4.3 KB) and the 7 taps of row r
 // (28 KB at NT = 128); tap s is the descriptor start s pixels into the row, as in the 3x3 halo tile.  Every input row is
 // fetched by up to 7 stages of a tile (from L2 after the first), ~15 % of the weight bytes.
-template <> struct Geo<G_C7> { static constexpr int HR = 1, PXP = TPX + 6, TAPS = 7, KCH = 2, NACC = 1; };
+template <> struct Geo<G_C7> { static constexpr int ROWS = 1, HR = 1, PXP = TPX + 6, TAPS = 7, KCH = 2, NACC = 1; };
 // stages per K step (kernel rows streamed one stage at a time)
 template <int GEOM> constexpr int kRows = GEOM == G_C7 ? 7 : 1;
 
@@ -71,14 +84,15 @@ using namespace tc;
 
 
 // Persistent CTAs (one per SM: each CTA loops over output tiles round-robin) with as deep a ring as shared memory
-// allows next to the epilogue's [TPX][NT + 4] fp32 staging tile.
-template <int GEOM, int NT> struct Depth {
-    static constexpr int STAGE_BYTES = Geo<GEOM>::KCH * Geo<GEOM>::HR * Geo<GEOM>::PXP * 16 + Geo<GEOM>::TAPS * Geo<GEOM>::KCH * NT * 16;
+// allows next to the epilogue's [TPX][NT + 4] fp32 staging tile (a 2-row tile passes through it one m64 block pair at a time).
+template <int GEOM, int NT, int R = 1> struct Depth {
+    using G = Geo<GEOM, R>;
+    static constexpr int STAGE_BYTES = G::KCH * G::HR * G::PXP * 16 + G::TAPS * G::KCH * NT * 16;
     static constexpr int LDS = NT + 4;                       // staging row pitch (floats): conflict-free float4 reads
     static constexpr int SD_BYTES = TPX * LDS * 4;
     static constexpr int FIT = (220 * 1024 - SD_BYTES) / STAGE_BYTES;
     static constexpr int STAGES = FIT > 6 ? 6 : FIT;
-    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + SD_BYTES + 3 * STAGES * 8 + 128 * 4 + 3 * NT * 4 + 64;
+    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + SD_BYTES + 3 * STAGES * 8 + 128 * 4 * G::ROWS + 3 * NT * 4 + 64;
     static_assert(STAGES >= 2, "need at least 2 stages");
     static_assert(SMEM <= 227 * 1024, "shared memory budget");
 };
@@ -96,12 +110,13 @@ template <int GEOM, int NT> struct Depth {
 // VOC: the vocoder's output forms (ConvTcParams::voc) on a 1x1 GEMM; the Conv1d geometries always use them.  They only
 // differ from the sampler's in the bf16 mode (an output is bf16 only when it is an activated operand) and, for fp32x3,
 // in the correction chunks of the second output (out_corr).
-template <int GEOM, bool BF16, int NT, bool RES, bool X3, bool VOC = false>
+template <int GEOM, bool BF16, int NT, bool RES, bool X3, bool VOC = false, int R = 1>
 __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     static_assert(!(X3 && BF16), "fp32x3 runs on tf32 operands");
-    using G = Geo<GEOM>;
-    using D = Depth<GEOM, NT>;
-    constexpr int NACC = G::NACC;
+    using G = Geo<GEOM, R>;
+    using D = Depth<GEOM, NT, R>;
+    constexpr int NACC = G::NACC, ROWS = G::ROWS;
+    constexpr bool ROW2 = ROWS == 2;                       // 3x3, 2-row tile: accumulator a = pixel block a of the row
     constexpr bool CHUNKED = X3 && GEOM != G_UP;
     // sub-stages per accumulation run: 6 = three K stages of correction + main sub-stage, 54 MMAs per accumulator for a
     // 3x3 conv (7x7: three (K step, kernel row) stages, 42 MMAs)
@@ -133,8 +148,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     // GroupNorm partials of the current tile: one private slot row per consumer warp (plain read-modify-write by lane 0,
     // no atomics), summed in a fixed order at the end of the tile and flushed as fp64 -> the totals can only differ between
     // runs through the order of the fp64 global atomics (1e-16), so the fp32 mean / rstd - and the sampler - are reproducible.
-    float* s_st = reinterpret_cast<float*>(bars + 3 * STAGES);                    // [8 warps][8 groups][2]
-    float* s_rg = s_st + 128;                                                     // EPI_RES: mean|scale|beta [NT] each
+    // A 2-row tile keeps one slot set per output row, and a slot row is the warp that covers the same pixels in a 1-row tile,
+    // so every row's fp64 total receives exactly the fp32 partials a 1-row tile would flush.
+    float* s_st = reinterpret_cast<float*>(bars + 3 * STAGES);                    // [ROWS][8 warps][8 groups][2]
+    float* s_rg = s_st + 128 * ROWS;                                              // EPI_RES: mean|scale|beta [NT] each
 
     // (the warp index is broadcast from lane 0 so that the compiler can prove the role branches warp-uniform: wgmma code
     // under a branch it considers divergent is serialised)
@@ -148,14 +165,14 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     // ---- tile space: (sample, pixel tile, N tile), N tile fastest so neighbours in time share the A tile in L2
     const int wt_w = (GEOM == G_DOWN ? p.Wo : p.W), wt_h = (GEOM == G_DOWN ? p.Ho : p.H);
     const int wtiles = (wt_w + SPAN - 1) / SPAN;
-    const int mtiles = GEOM == G_PW ? (HW + TPX - 1) / TPX : wtiles * wt_h;
+    const int mtiles = GEOM == G_PW ? (HW + TPX - 1) / TPX : wtiles * ((wt_h + ROWS - 1) / ROWS);
     const int ntn = p.Cout / NT;
     const int total_tiles = p.B * mtiles * ntn;
     auto decode = [&](int t, int& b, int& h0, int& w0, int& n0) {
         const int nt = t % ntn; const int r = t / ntn;
         const int mt = r % mtiles; b = r / mtiles; n0 = nt * NT;
         if (GEOM == G_PW) { w0 = 0; h0 = mt; }
-        else { w0 = (mt % wtiles) * SPAN; h0 = mt / wtiles; }
+        else { w0 = (mt % wtiles) * SPAN; h0 = (mt / wtiles) * ROWS; }
     };
 
     const uint32_t bar0 = smem_u32(bars);
@@ -168,14 +185,15 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(full_a(s), NCONS / 32); mbar_init(full_b(s), 1); mbar_init(empty(s), NCONS / 32); }
         fence_barrier_init();
     }
-    if (tid < 128) s_st[tid] = 0.f;
+    if (tid < 128 * ROWS) s_st[tid] = 0.f;
     __syncthreads();
 
     if (warp < NCONS / 32) {
         // =========================================================================================================
         // consumer warpgroups: (G_DOWN: cp.async A producers,) MMAs, epilogue of every tile
         // =========================================================================================================
-        const int wg = warp >> 2, wt = tid & 127;                  // warpgroup = pixel half of the tile
+        setmaxnreg_inc<CONS_REGS>();
+        const int wg = warp >> 2, wt = tid & 127;                  // warpgroup = pixel half of the tile (2-row tile: its row)
         uint32_t it = 0;                                           // ring counter (stages consumed by this CTA)
         // ---- A producers (Downsample only): 16-byte cp.async gathers that de-interleave even/odd columns
         constexpr int SLOTS = HR * PXP * KCH;
@@ -184,7 +202,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
         const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
         constexpr uint32_t D_HI = desc_hi(128);                    // SBO = 128 B for both operands
         float acc[NACC][FR];
-        float sum[CHUNKED ? FR : 1];
+        float sum[CHUNKED ? NACC : 1][CHUNKED ? FR : 1];
         for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
             int b, h0, w0, n0;
             decode(t, b, h0, w0, n0);
@@ -236,7 +254,8 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 mbar_wait(full_b(s), ph);                  // weights (+ the A runs when they are bulk copies)
                 const int run_lo = CHUNKED ? ks - ks % FLUSH : 0;
                 const bool last = ks == ksteps_t - 1 || (CHUNKED && ks - run_lo == FLUSH - 1);
-                const uint32_t a_lo = desc_lo(a0 + s * A_STAGE_BYTES, PLANE) + (uint32_t)(64 * wg);   // this warpgroup's 64 pixels
+                // this warpgroup's 64 pixels (2-row tile: its halo row; block a of the row adds 64 a)
+                const uint32_t a_lo = desc_lo(a0 + s * A_STAGE_BYTES, PLANE) + (uint32_t)(ROW2 ? wg * PXP : 64 * wg);
                 const uint32_t b_lo = desc_lo(b0 + s * B_STAGE_BYTES, NT * 16);
                 const uint32_t dil = C1 ? (uint32_t)p.dil : 0u;
                 auto issue = [&](auto kind) {
@@ -267,8 +286,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                                 const uint32_t aoff = GEOM == G_DOWN ? (uint32_t)(r * PXP + (sx == 1 ? TPX + 1 : (sx == 2 ? 1 : 0)))
                                                     : C1 ? (uint32_t)tap * dil
                                                          : (uint32_t)(r * PXP + sx);
-                                wgmma<NT, KD>(acc[0], desc_pack(a_k + aoff, D_HI), desc_pack(b_k + (uint32_t)(tap * KCH * NT), D_HI),
-                                              ((ks - run_lo) | kk | tap) != 0 ? 1u : 0u);
+#pragma unroll
+                                for (int a = 0; a < NACC; ++a)
+                                    wgmma<NT, KD>(acc[a], desc_pack(a_k + aoff + (uint32_t)(64 * a), D_HI),
+                                                  desc_pack(b_k + (uint32_t)(tap * KCH * NT), D_HI), ((ks - run_lo) | kk | tap) != 0 ? 1u : 0u);
                             }
                         }
                     }
@@ -285,7 +306,9 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 if constexpr (CHUNKED) {
                     const bool first = run_lo == 0;
 #pragma unroll
-                    for (int i = 0; i < FR; ++i) sum[i] = last ? (first ? acc[0][i] : sum[i] + acc[0][i]) : sum[i];
+                    for (int a = 0; a < NACC; ++a)
+#pragma unroll
+                        for (int i = 0; i < FR; ++i) sum[a][i] = last ? (first ? acc[a][i] : sum[a][i] + acc[a][i]) : sum[a][i];
                 }
             };
             constexpr auto kind_c = std::integral_constant<int, K_F16>{};     // fp32x3 correction sub-stage (even ks)
@@ -352,6 +375,14 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
             const float* bp = p.bias ? p.bias + (long long)b * p.bias_bstride + n0 : nullptr;
 #pragma unroll
             for (int phase = 0; phase < NACC; ++phase) {
+            if constexpr (ROW2) {
+                // pass `phase` stages pixel block `phase` of both rows: staging pixel px is row px / 64, column 64 phase + px % 64
+                ho = h0 + (px >> 6); wo = w0 + 64 * phase + (px & 63);
+                valid = ho < Ho && wo < Wo;
+                if (!valid) { ho = 0; wo = 0; }
+            }
+            // GroupNorm slot row of this warp's 32 pixels (2-row tile: the row's slot set, the warp of the 1-row tile)
+            const int slot = ROW2 ? ((warp & 3) >> 1) * 64 + ((warp >> 2) * 4 + 2 * phase + (warp & 1)) * 8 : warp * 8;
             // accumulators -> staging tile [pixel][column]
             asm volatile("bar.sync 2, 256;" ::: "memory");            // previous readers of the staging tile are done
             {
@@ -360,7 +391,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                     for (int i = 0; i < FR; i += 2)
                         *reinterpret_cast<float2*>(&sD[(64 * wg + frag_row(wt, i)) * LDS + frag_col(wt, i)]) = make_float2(res[i], res[i + 1]);
                 };
-                if constexpr (CHUNKED) stage_out(sum);
+                if constexpr (CHUNKED) stage_out(sum[phase]);
                 else stage_out(acc[phase]);
             }
             asm volatile("bar.sync 2, 256;" ::: "memory");
@@ -514,8 +545,8 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                             for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); q += __shfl_xor_sync(0xffffffffu, q, o); }
                             if (lane == 0) {
                                 const int gl = (n0 + cb + k * (32 / ngrp)) / cpg - n0 / cpg;
-                                s_st[(warp * 8 + gl) * 2] += s;
-                                s_st[(warp * 8 + gl) * 2 + 1] += q;
+                                s_st[(slot + gl) * 2] += s;
+                                s_st[(slot + gl) * 2 + 1] += q;
                             }
                         }
                     }
@@ -525,16 +556,21 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
             if (GEOM != G_PW && p.ostats) {
                 asm volatile("bar.sync 1, 256;" ::: "memory");
                 const int gb = n0 / cpg, ng = (NT + cpg - 1) / cpg;
-                if (tid < ng * 2) {
+                const int r = tid / (ng * 2), e = tid - r * (ng * 2);       // output row of the tile, (group, sum | squares)
+                if (tid < ng * 2 * ROWS) {
                     double tot = 0.0;
+                    float* sl = s_st + r * 128 + e;
 #pragma unroll
-                    for (int w8 = 0; w8 < NCONS / 32; ++w8) { tot += (double)s_st[w8 * 16 + tid]; s_st[w8 * 16 + tid] = 0.f; }
-                    atomicAdd(&p.ostats[((long long)b * kGroups + gb + (tid >> 1)) * 2 + (tid & 1)], tot);
+                    for (int w8 = 0; w8 < NCONS / 32; ++w8) { tot += (double)sl[w8 * 16]; sl[w8 * 16] = 0.f; }
+                    if (!ROW2 || h0 + r < Ho)                          // (the missing second row of an odd H adds nothing)
+                        atomicAdd(&p.ostats[((long long)b * kGroups + gb + (e >> 1)) * 2 + (e & 1)], tot);
                 }
                 asm volatile("bar.sync 1, 256;" ::: "memory");
             }
         }
     } else {
+        setmaxnreg_dec<PROD_REGS>();
+        if (warp != NCONS / 32) return;
         // =========================================================================================================
         // loader warp: weights + A runs by cp.async.bulk.  Every byte of the A tile is written every stage:
         // out-of-image rows / columns (the conv's zero padding, the ragged last 1x1 tile) come from a zero page.
@@ -630,13 +666,13 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     }
 }
 
-template <int GEOM, bool BF16, int NT, bool RES = false>
+template <int GEOM, bool BF16, int NT, bool RES = false, int R = 1>
 __global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc(const ConvTcParams p) {
-    conv_tc_body<GEOM, BF16, NT, RES, false>(p);
+    conv_tc_body<GEOM, BF16, NT, RES, false, false, R>(p);
 }
-template <int GEOM, int NT, bool RES = false>
+template <int GEOM, int NT, bool RES = false, int R = 1>
 __global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc_x3(const ConvTcParams p) {
-    conv_tc_body<GEOM, false, NT, RES, true>(p);
+    conv_tc_body<GEOM, false, NT, RES, true, false, R>(p);
 }
 // the vocoder's transposed-conv GEMM in bf16 mode: bf16 operands, fp32 output Z (ConvTcParams::voc)
 template <int NT>
@@ -644,29 +680,29 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_gemm_voc_bf16(const ConvTcParam
     conv_tc_body<G_PW, true, NT, false, false, true>(p);
 }
 
-template <int GEOM, bool BF16, int NT, bool RES = false, bool X3 = false, bool VOC = false>
+template <int GEOM, bool BF16, int NT, bool RES = false, bool X3 = false, bool VOC = false, int R = 1>
 static int launch_tc(const ConvTcParams& p, cudaStream_t s) {
-    using D = Depth<GEOM, NT>;
+    using D = Depth<GEOM, NT, R>;
     static_assert(!VOC || (GEOM == G_PW && BF16 && !RES && !X3), "VOC selects the bf16 GEMM with fp32 output");
     // the dynamic-shared-memory opt-in is a per-device function attribute and the persistent grid is sized from the
     // current device's SM count: both are cached per device ordinal (a process may drive several GPUs through several handles)
     static DevCache cache;
     const void* fn;
     if constexpr (VOC) fn = reinterpret_cast<const void*>(k_gemm_voc_bf16<NT>);
-    else if constexpr (X3) fn = reinterpret_cast<const void*>(k_conv_tc_x3<GEOM, NT, RES>);
-    else fn = reinterpret_cast<const void*>(k_conv_tc<GEOM, BF16, NT, RES>);
+    else if constexpr (X3) fn = reinterpret_cast<const void*>(k_conv_tc_x3<GEOM, NT, RES, R>);
+    else fn = reinterpret_cast<const void*>(k_conv_tc<GEOM, BF16, NT, RES, R>);
     const int num_sms = cache.get(fn);
     if (num_sms <= 0) return -1;
     int mt;
     if (geom_is_c1(GEOM)) mt = (p.W + TPX - 1) / TPX;
-    else if (GEOM == G_C3 || GEOM == G_C7 || GEOM == G_UP) mt = ((p.W + TPX - 1) / TPX) * p.H;
+    else if (GEOM == G_C3 || GEOM == G_C7 || GEOM == G_UP) mt = ((p.W + TPX - 1) / TPX) * ((p.H + R - 1) / R);
     else if (GEOM == G_DOWN) mt = ((p.Wo + TPX - 1) / TPX) * p.Ho;
     else mt = (p.H * p.W + TPX - 1) / TPX;
     const long long total = (long long)mt * (p.Cout / NT) * p.B;
     const int grid = (int)(total < num_sms ? total : num_sms);       // persistent: one wave of resident CTAs
     if constexpr (VOC) k_gemm_voc_bf16<NT><<<grid, NTHREADS, D::SMEM, s>>>(p);
-    else if constexpr (X3) k_conv_tc_x3<GEOM, NT, RES><<<grid, NTHREADS, D::SMEM, s>>>(p);
-    else k_conv_tc<GEOM, BF16, NT, RES><<<grid, NTHREADS, D::SMEM, s>>>(p);
+    else if constexpr (X3) k_conv_tc_x3<GEOM, NT, RES, R><<<grid, NTHREADS, D::SMEM, s>>>(p);
+    else k_conv_tc<GEOM, BF16, NT, RES, R><<<grid, NTHREADS, D::SMEM, s>>>(p);
     return 1;
 }
 
@@ -699,13 +735,13 @@ int conv_tc_stage_channels(int geom, int bf16) {
     const int epc = bf16 ? 8 : 4;
     return (geom == G_PW ? Geo<G_PW>::KCH : geom == G_C7 ? Geo<G_C7>::KCH : Geo<G_C3>::KCH) * epc;
 }
-int conv_tc_tile_rows() { return ROWS; }
 
 template <bool BF16>
 static int dispatch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
     const int nt = (p.nt == 64 && p.geom == G_C3) ? 64 : conv_tc_ntile(p.geom, p.Cout);
     switch (p.geom) {
         case G_C3:
+            if (p.rows == 2) return nt == 64 ? launch_tc<G_C3, BF16, 64, false, false, false, 2>(p, s) : -1;
             return nt == 128 ? launch_tc<G_C3, BF16, 128>(p, s) : launch_tc<G_C3, BF16, 64>(p, s);
         case G_PW:
             if (p.epi == EPI_KV) return launch_attn_kv(p, s);
@@ -744,6 +780,7 @@ static int dispatch_conv_tc_x3(const ConvTcParams& p, cudaStream_t s) {
     const int nt = (p.nt == 64 && p.geom == G_C3) ? 64 : conv_tc_ntile(p.geom, p.Cout);
     switch (p.geom) {
         case G_C3:
+            if (p.rows == 2) return nt == 64 ? launch_tc<G_C3, false, 64, false, true, false, 2>(p, s) : -1;
             return nt == 128 ? launch_tc<G_C3, false, 128, false, true>(p, s) : launch_tc<G_C3, false, 64, false, true>(p, s);
         case G_PW:
             if (p.epi == EPI_KV) return launch_attn_kv_x3(p, s);      // fused projection + softmax + context (sbk_attn_x3.cu)

@@ -72,6 +72,7 @@ struct ConvTcParams {
     int bf16;
     int nt;                                         // N tile override (64) for launches with too few 128-wide tiles to fill the
                                                     // GPU (small batches); 0 = conv_tc_ntile(geom, Cout).  The weights must be packed for it.
+    int rows;                                       // G_C3: output rows per tile, 1 (0 = 1) or 2; 2 runs 64-wide N tiles (nt = 64)
     // Conv1d geometries: dilation and left padding ((K-1)*dil/2) in samples; output activation LeakyReLU(slope) on `out`
     // (act_out) and/or on the second output written through out_lo (act_out2: out_lo = lrelu(out) instead of the x_lo split)
     int dil, pad; float slope; int act_out, act_out2;
@@ -245,7 +246,6 @@ int launch_first_conv(const FirstConvParams& p, cudaStream_t s);
 int launch_conv_tc(const ConvTcParams& p, cudaStream_t s);
 int conv_tc_ntile(int geom, int Cout);
 int conv_tc_ntile_x3(int geom, int Cout);
-int conv_tc_tile_rows();
 int conv_tc_taps(int geom);
 int conv_tc_stage_rows(int geom);       // weight stages per K step: 7 for G_C7 (one per kernel row), else 1
 int conv_tc_stage_channels(int geom, int bf16);

@@ -132,6 +132,10 @@ template <> __device__ __forceinline__ void wgmma<128, K_BF16>(float (&d)[64], u
                  : "l"(a), "l"(b), "r"(acc));
 }
 
+// per-thread register budget of the calling warpgroup (warp-specialised kernels): every warp of the warpgroup executes it
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // fragment element i of a warpgroup accumulator -> (row, column) of the 64 x N tile
 __device__ __forceinline__ int frag_row(int t, int i) { return 16 * (t >> 5) + ((t & 31) >> 2) + ((i & 2) ? 8 : 0); }
 __device__ __forceinline__ int frag_col(int t, int i) { return 8 * (i >> 2) + 2 * (t & 3) + (i & 1); }
