@@ -42,14 +42,6 @@ def load_library() -> C.CDLL:
                            "There is no CPU fallback for the sampler.")
     lib = C.CDLL(LIB_PATH)
     P, I, F = C.c_void_p, C.c_int, C.c_void_p
-    lib.sbk_create.argtypes = [C.POINTER(SbkConfig), C.POINTER(P)]
-    lib.sbk_destroy.argtypes = [P]
-    lib.sbk_destroy.restype = None
-    lib.sbk_set_weight.argtypes = [P, C.c_char_p, F, C.POINTER(C.c_int64), I]
-    lib.sbk_pack.argtypes = [P]
-    lib.sbk_num_weights.argtypes = [P]
-    lib.sbk_weight_name.argtypes = [P, I]
-    lib.sbk_weight_name.restype = C.c_char_p
     lib.sbk_workspace_bytes.argtypes = [P, I, I]
     lib.sbk_workspace_bytes.restype = C.c_size_t
     lib.sbk_workspace_bytes_n.argtypes = [P, I, I, I]
@@ -62,8 +54,6 @@ def load_library() -> C.CDLL:
     lib.sbk_reverse_steps.argtypes = [P, F, F, F, F, F, I, I, I, I, I, I, P]
     lib.sbk_reverse_diffusion_host.argtypes = [P, F, F, F, F, F, F, I, I, I, I]
     lib.sbk_prior_expand.argtypes = [F, F, F, F, F, C.c_float, I, I, I, I, F, F, F, F, P]
-    lib.sbk_last_launch_count.argtypes = [P]
-    lib.sbk_last_launch_count.restype = C.c_int64
     lib.sbk_last_host_launches.argtypes = [P]
     lib.sbk_debug_read.argtypes = [P, C.c_char_p, F, C.POINTER(C.c_int64)]
     lib.sbk_debug_num.argtypes = [P]
@@ -91,6 +81,12 @@ def _check(rc: int, what: str):
 
 def _ptr(t):
     return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def _check_precision(precision):
+    if precision not in PREC:
+        raise ValueError(f"precision must be one of {sorted(PREC)}, got {precision!r}")
+    return precision
 
 
 def _f32c(t: torch.Tensor, name: str) -> torch.Tensor:
@@ -132,27 +128,38 @@ def prior_expand(mu_x, w_ceil, x_mask, y_lengths, Ty, noise_tf=None, temperature
     return mu_y, z, y_mask, attn
 
 
-class Engine:
-    """One sbk_handle: a (device, configuration) pair owning packed weights, workspace and graphs."""
+class _NativeHandle:
+    """One libsbk handle of the C prefix PREFIX ("sbk", "sbk_vocoder", "sbk_postnet", "sbk_textenc"): the entry points every
+    engine shares - create / destroy, the strict weight inventory and loader, the launch count - declared once here."""
+    PREFIX = "sbk"
+    STATE_DICT = "state_dict"           # how load_state_dict's missing-key error names the state dict
 
-    def __init__(self, n_feats=80, dim=64, n_spks=1, spk_emb_dim=64, beta_min=0.05, beta_max=20.0,
-                 pe_scale=1000.0, device=0, precision="fp32x3", use_graph=True, model="gradtts", dim_cond=0,
-                 use_ref_t=True):
+    def __init__(self):
         self.lib = load_library()
-        self.cfg = SbkConfig(MODEL[model], n_feats, dim, n_spks, spk_emb_dim, beta_min, beta_max, pe_scale,
-                             device, PREC[precision], 1 if use_graph else 0, dim_cond, 1 if use_ref_t else 0)
-        self.model = model
-        self.dim_cond = dim_cond
+        P, I = C.c_void_p, C.c_int
+        self._fn("destroy").argtypes = [P]
+        self._fn("destroy").restype = None
+        self._fn("num_weights").argtypes = [P]
+        self._fn("weight_name").argtypes = [P, I]
+        self._fn("weight_name").restype = C.c_char_p
+        self._fn("set_weight").argtypes = [P, C.c_char_p, P, C.POINTER(C.c_int64), I]
+        self._fn("pack").argtypes = [P]
+        self._fn("last_launch_count").argtypes = [P]
+        self._fn("last_launch_count").restype = C.c_int64
         self.h = C.c_void_p()
-        _check(self.lib.sbk_create(C.byref(self.cfg), C.byref(self.h)), "sbk_create")
-        self.device = device
-        self.n_feats = n_feats
-        self.n_spks = n_spks
-        self.spk_emb_dim = spk_emb_dim
+
+    def _fn(self, name):
+        return getattr(self.lib, f"{self.PREFIX}_{name}")
+
+    def _create(self, cfg):
+        """<prefix>_create(&cfg, &h); returns its status code"""
+        create = self._fn("create")
+        create.argtypes = [C.POINTER(type(cfg)), C.POINTER(C.c_void_p)]
+        return create(C.byref(cfg), C.byref(self.h))
 
     def close(self):
         if getattr(self, "h", None) and self.h.value:
-            self.lib.sbk_destroy(self.h)
+            self._fn("destroy")(self.h)
             self.h = C.c_void_p()
 
     def __del__(self):
@@ -161,36 +168,57 @@ class Engine:
         except Exception:
             pass
 
-    # ---- strict state_dict loading (Grad-TTS/inference.py:53)
     def weight_names(self):
-        return [self.lib.sbk_weight_name(self.h, i).decode() for i in range(self.lib.sbk_num_weights(self.h))]
+        return [self._fn("weight_name")(self.h, i).decode() for i in range(self._fn("num_weights")(self.h))]
 
     def load_state_dict(self, sd, prefix=""):
         """`sd` maps reference names (optionally under `prefix`, e.g. 'decoder.') to tensors (CPU or CUDA)."""
         for name in self.weight_names():
             key = prefix + name
             if key not in sd:
-                raise RuntimeError(f"missing key '{key}' in state_dict (strict)")
+                raise RuntimeError(f"missing key '{key}' in {self.STATE_DICT} (strict)")
             t = sd[key].detach().to(torch.float32).contiguous()
             shape = (C.c_int64 * t.dim())(*t.shape)
-            _check(self.lib.sbk_set_weight(self.h, name.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()),
-                   f"sbk_set_weight({name})")
-        _check(self.lib.sbk_pack(self.h), "sbk_pack")
+            _check(self._fn("set_weight")(self.h, name.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()),
+                   f"{self.PREFIX}_set_weight({name})")
+        _check(self._fn("pack")(self.h), f"{self.PREFIX}_pack")
 
     def _call(self, fn, what, *args):
-        """One libsbk call; if its workspace allocation ran out of memory while torch holds cached blocks (the arena is
-        raw cudaMalloc, outside torch's caching allocator), release them and retry once."""
+        """One libsbk call; if its workspace allocation ran out of memory while torch holds cached blocks (the workspace
+        is raw cudaMalloc, outside torch's caching allocator), release them and retry once."""
         rc = fn(*args)
         if rc != 0 and b"out of memory" in self.lib.sbk_last_error():
             torch.cuda.empty_cache()
             rc = fn(*args)
         _check(rc, what)
 
-    def workspace_bytes(self, B, T, n_timesteps=1024):
-        return int(self.lib.sbk_workspace_bytes_n(self.h, B, T, int(n_timesteps)))
-
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def last_launch_count(self):
+        return int(self._fn("last_launch_count")(self.h))
+
+
+class Engine(_NativeHandle):
+    """One sbk_handle: a (device, configuration) pair owning packed weights, workspace and graphs.  load_state_dict is the
+    strict loading of Grad-TTS/inference.py:53."""
+
+    def __init__(self, n_feats=80, dim=64, n_spks=1, spk_emb_dim=64, beta_min=0.05, beta_max=20.0,
+                 pe_scale=1000.0, device=0, precision="fp32x3", use_graph=True, model="gradtts", dim_cond=0,
+                 use_ref_t=True):
+        super().__init__()
+        self.cfg = SbkConfig(MODEL[model], n_feats, dim, n_spks, spk_emb_dim, beta_min, beta_max, pe_scale,
+                             device, PREC[precision], 1 if use_graph else 0, dim_cond, 1 if use_ref_t else 0)
+        self.model = model
+        self.dim_cond = dim_cond
+        _check(self._create(self.cfg), "sbk_create")
+        self.device = device
+        self.n_feats = n_feats
+        self.n_spks = n_spks
+        self.spk_emb_dim = spk_emb_dim
+
+    def workspace_bytes(self, B, T, n_timesteps=1024):
+        return int(self.lib.sbk_workspace_bytes_n(self.h, B, T, int(n_timesteps)))
 
     def _check_inputs(self, x, mask, mu, spk, t=None):
         for n, v in (("x", x), ("mask", mask), ("mu", mu)):
@@ -356,9 +384,6 @@ class Engine:
                                                    _ptr(out), B, T, int(n_timesteps), 1 if stoc else 0),
                "sbk_reverse_diffusion_host")
         return out
-
-    def last_launch_count(self):
-        return int(self.lib.sbk_last_launch_count(self.h))
 
     def last_host_launches(self):
         """Host launches the Euler loop of the last sampler call took (1 = the whole loop ran as one CUDA graph)."""

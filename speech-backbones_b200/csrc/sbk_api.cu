@@ -1,8 +1,7 @@
 // Host side of libsbk.so: strict weight loading + packing, workspace arena, the per-step launch
 // plan of the Grad-TTS score U-Net, CUDA-graph replay of the Euler(-Maruyama) loop, and the C ABI.
 // Mirrors Diffusion / GradLogPEstimator2d (Grad-TTS/model/diffusion.py:128-279); see include/sbk.h.
-#include "../../include/sbk.h"
-#include "sbk_internal.h"
+#include "sbk_host.h"
 
 #include <cuda_fp16.h>
 #include <math.h>
@@ -19,33 +18,16 @@
 using namespace sbk;
 
 static thread_local char g_err[1024] = "";
-static int fail(int code, const char* fmt, ...) {
+int sbk::fail(int code, const char* fmt, ...) {
     va_list ap;
     va_start(ap, fmt);
     vsnprintf(g_err, sizeof(g_err), fmt, ap);
     va_end(ap);
     return code;
 }
-// shared with the other translation units of the library (sbk_vocoder.cu ...): same thread-local error text
-int sbk_set_error(int code, const char* fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof(g_err), fmt, ap);
-    va_end(ap);
-    return code;
-}
-#define CU(x)                                                                                          \
-    do {                                                                                               \
-        cudaError_t e_ = (x);                                                                          \
-        if (e_ != cudaSuccess)                                                                         \
-            return fail(SBK_ERR_CUDA, "%s failed: %s (%s:%d)", #x, cudaGetErrorString(e_), __FILE__, __LINE__); \
-    } while (0)
-
-#define TRY_RC(x) do { int rc__ = (x); if (rc__ != SBK_OK) return rc__; } while (0)
 
 namespace {
 
-struct WSpec { std::string name; std::vector<int64_t> shape; };
 struct ResnetInfo { std::string prefix; int cin, cout; };
 struct AttnInfo { std::string prefix; int c; };
 
@@ -55,16 +37,6 @@ __global__ void k_set_ptr(const float** p, const float* v) { *p = v; }
 __global__ void k_loop_cond(cudaGraphConditionalHandle handle, const int* step_next, const int* step_end) {
     cudaGraphSetConditional(handle, *step_next < *step_end ? 1u : 0u);
 }
-
-struct Arena {
-    char* base = nullptr; size_t cap = 0, off = 0;
-    void* take(size_t bytes) {
-        off = (off + 255) & ~size_t(255);
-        void* r = base ? base + off : nullptr;
-        off += bytes;
-        return r;
-    }
-};
 
 enum OpKind { OP_FIRST, OP_IGEMM, OP_RESFINAL, OP_CTX, OP_MIX, OP_FINAL, OP_CONVTC, OP_GNACT };
 struct Op {
@@ -78,7 +50,6 @@ struct Op {
 
 struct Plan {
     int B = 0, T = 0, tb_rows = 0, noise_cap_steps = 0;
-    void* mem = nullptr; size_t bytes = 0, cap = 0;   // arena: grow-only (cap) across (B,T) changes, `bytes` in use
     std::vector<Op> ops;
     int final_op = -1;
     // owned buffers
@@ -103,24 +74,21 @@ struct Plan {
 
 struct sbk_handle {
     sbk_config cfg;
-    std::vector<WSpec> spec;
+    WeightSet w;
     std::vector<ResnetInfo> resnets;
     std::vector<AttnInfo> attns;
-    std::map<std::string, float*> raw;        // device copies, reference layout
-    std::map<std::string, float*> packed;     // kernel layouts
-    std::vector<void*> owned;
     float* d_freqs = nullptr;
     float* d_zero = nullptr;                  // zero page for the tensor-core kernels' border copies
-    void* ref_mem = nullptr; size_t ref_bytes = 0;   // DiffVC RefBlock workspace (grown on demand)
+    Workspace ws;                             // the plan's arena
+    Workspace ref_ws;                         // DiffVC RefBlock workspace
     bool is_packed = false;
     Plan plan;
     cudaStream_t cap_stream = nullptr;
     int64_t last_launches = 0;
     int last_host_launches = 0;               // graph launches the host issued for the loop of the last sampler call
     bool capture = false;
-    // sbk_vc_conditioning's debug snapshots (names in launch order; fmt: 0 fp32 array, 1 fp32 [B][H][C/4][Tr][4], 3 float64)
-    struct VcSnap { std::string name; void* buf; size_t cap, numel; int fmt; };
-    std::vector<VcSnap> vc_snaps;
+    // sbk_vc_conditioning's debug snapshots (fmt: 0 fp32 array, 1 fp32 [B][H][C/4][Tr][4], 3 float64)
+    Snapshots vc_snaps;
     int tb_off[16];
     int tb_total = 0;
 };
@@ -133,7 +101,7 @@ static void build_spec(sbk_handle* h) {
     const int dim = c.dim;
     const bool vc = c.model == SBK_MODEL_DIFFVC;
     const int d[4] = {vc ? 2 + c.dim_cond : 2 + (c.n_spks > 1 ? 1 : 0), dim, dim * 2, dim * 4};
-    auto add = [&](const std::string& n, std::vector<int64_t> s) { h->spec.push_back({n, s}); };
+    auto add = [&](const std::string& n, std::vector<int64_t> s) { h->w.add(n, std::move(s)); };
     auto resnet = [&](const std::string& p, int cin, int cout) {
         add(p + ".mlp.1.weight", {cout, dim});
         add(p + ".mlp.1.bias", {cout});
@@ -223,8 +191,6 @@ static void build_spec(sbk_handle* h) {
     h->tb_total = off;
 }
 
-static int64_t numel_of(const std::vector<int64_t>& s) { int64_t n = 1; for (auto v : s) n *= v; return n; }
-
 // ------------------------------------------------------------------------------------------------
 // C ABI: lifecycle + strict loading
 // ------------------------------------------------------------------------------------------------
@@ -249,49 +215,31 @@ extern "C" int sbk_create(const sbk_config* cfg, sbk_handle** out) {
     return SBK_OK;
 }
 
-// drop the launch plan and its graphs; the arena allocation survives unless `release_arena` (it is grow-only: a new
-// (B,T) whose layout fits the existing capacity is laid out inside it without a cudaFree/cudaMalloc pair)
-static void free_plan(sbk_handle* h, bool release_arena = true) {
+// drop the launch plan and its graphs (the arena h->ws is grow-only: a new (B,T) whose layout fits its capacity is laid out
+// inside it without a cudaFree/cudaMalloc pair)
+static void free_plan(sbk_handle* h) {
     Plan& p = h->plan;
     for (int i = 0; i < 4; ++i) if (p.gexec[i]) { cudaGraphExecDestroy(p.gexec[i]); p.gexec[i] = nullptr; }
     for (int i = 0; i < 4; ++i) if (p.gloop[i]) { cudaGraphExecDestroy(p.gloop[i]); p.gloop[i] = nullptr; }
     for (auto& op : p.ops) if (op.dbg_copy) cudaFree(op.dbg_copy);
-    void* mem = p.mem; const size_t cap = p.cap;
-    if (mem && release_arena) { cudaFree(mem); mem = nullptr; }
     p = Plan();
-    if (mem) { p.mem = mem; p.cap = cap; }
 }
 
 extern "C" void sbk_destroy(sbk_handle* h) {
     if (!h) return;
     free_plan(h);
-    for (auto& kv : h->raw) cudaFree(kv.second);
-    for (void* p : h->owned) cudaFree(p);
-    if (h->ref_mem) cudaFree(h->ref_mem);
-    for (auto& sn : h->vc_snaps) cudaFree(sn.buf);
+    cudaFree(h->d_freqs);
+    cudaFree(h->d_zero);
     if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
     delete h;
 }
 
-extern "C" int sbk_num_weights(const sbk_handle* h) { return h ? (int)h->spec.size() : 0; }
-extern "C" const char* sbk_weight_name(const sbk_handle* h, int i) {
-    if (!h || i < 0 || i >= (int)h->spec.size()) return nullptr;
-    return h->spec[i].name.c_str();
-}
+extern "C" int sbk_num_weights(const sbk_handle* h) { return h ? h->w.count() : 0; }
+extern "C" const char* sbk_weight_name(const sbk_handle* h, int i) { return h ? h->w.name(i) : nullptr; }
 
 extern "C" int sbk_set_weight(sbk_handle* h, const char* name, const void* data, const int64_t* shape, int ndim) {
     if (!h || !name || !data || !shape) return fail(SBK_ERR_ARG, "sbk_set_weight: null argument");
-    const WSpec* ws = nullptr;
-    for (auto& s : h->spec) if (s.name == name) { ws = &s; break; }
-    if (!ws) return fail(SBK_ERR_ARG, "sbk_set_weight: unexpected key '%s' (strict)", name);
-    if ((int)ws->shape.size() != ndim) return fail(SBK_ERR_ARG, "sbk_set_weight: '%s' rank %d, expected %d", name, ndim, (int)ws->shape.size());
-    for (int i = 0; i < ndim; ++i)
-        if (ws->shape[i] != shape[i]) return fail(SBK_ERR_ARG, "sbk_set_weight: '%s' dim %d is %lld, expected %lld", name, i, (long long)shape[i], (long long)ws->shape[i]);
-    CU(cudaSetDevice(h->cfg.device));
-    const size_t bytes = numel_of(ws->shape) * sizeof(float);
-    float*& dst = h->raw[name];
-    if (!dst) CU(cudaMalloc(&dst, bytes));
-    CU(cudaMemcpy(dst, data, bytes, cudaMemcpyDefault));
+    TRY(h->w.set(name, data, shape, ndim, h->cfg.device, "sbk_set_weight"));
     h->is_packed = false;
     return SBK_OK;
 }
@@ -299,16 +247,10 @@ extern "C" int sbk_set_weight(sbk_handle* h, const char* name, const void* data,
 // copy a raw tensor to the host, repack with `f(dst, src)`, upload under `key`
 template <class F>
 static int repack(sbk_handle* h, const std::string& src, const std::string& key, size_t out_floats, F f) {
-    const WSpec* ws = nullptr;
-    for (auto& s : h->spec) if (s.name == src) { ws = &s; break; }
-    if (!ws) return fail(SBK_ERR_STATE, "repack: no spec for %s", src.c_str());
-    std::vector<float> hs(numel_of(ws->shape)), hd(out_floats);
-    CU(cudaMemcpy(hs.data(), h->raw[src], hs.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    f(hd.data(), hs.data(), ws->shape);
-    float*& d = h->packed[key];
-    if (!d) { CU(cudaMalloc(&d, out_floats * sizeof(float))); h->owned.push_back(d); }
-    CU(cudaMemcpy(d, hd.data(), out_floats * sizeof(float), cudaMemcpyHostToDevice));
-    return SBK_OK;
+    std::vector<float> hs, hd(out_floats);
+    TRY(h->w.fetch(src, hs));
+    f(hd.data(), hs.data(), h->w.find(src)->shape);
+    return upload(h->w.packed, key, out_floats * sizeof(float), hd.data());
 }
 
 
@@ -333,25 +275,22 @@ static uint16_t f32_to_bf16_rn(float x) {
     return (uint16_t)(u >> 16);
 }
 static int pack_tc_host(sbk_handle* h, const std::vector<float>& hs, const std::string& key, int cout, int cin, int geom, bool bf16, int nt_override = 0);
-// fp32x3 handles (and the CUDA-core fp32 handles' RefBlock branch) pack every tensor-core weight as (hi, lo) stage pairs
-static bool packs_x3(const sbk_handle* h) { return h->cfg.precision == SBK_PREC_FP32X3 || h->cfg.precision == SBK_PREC_FP32; }
 static int pack_tc(sbk_handle* h, const std::string& src, const std::string& key, int cout, int cin, int geom, bool bf16) {
-    const int taps = conv_tc_taps(geom);
-    std::vector<float> hs((size_t)cout * cin * taps);
-    CU(cudaMemcpy(hs.data(), h->raw[src], hs.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    TRY_RC(pack_tc_host(h, hs, key, cout, cin, geom, bf16));
+    std::vector<float> hs;
+    TRY(h->w.fetch(src, hs));
+    TRY(pack_tc_host(h, hs, key, cout, cin, geom, bf16));
     // 3x3 convs with >= 128 output channels also get a 64-wide N-tile image: the two-row tiles run 64 channels wide, and
     // small batches have too few 128-wide tiles to fill the GPU's SMs, so the planner switches those launches to twice as
     // many half-width tiles
-    if (geom == G_C3 && conv_tc_ntile(geom, cout) == 128) TRY_RC(pack_tc_host(h, hs, key + "64", cout, cin, geom, bf16, 64));
+    if (geom == G_C3 && conv_tc_ntile(geom, cout) == 128) TRY(pack_tc_host(h, hs, key + "64", cout, cin, geom, bf16, 64));
     return SBK_OK;
 }
 // k and v rows of to_qkv ('(qkv heads c)': k = rows 128.., v = rows 256..) in k_attn_kv's per-stage shared-memory image
 // [32-channel stage][k|v][16-byte chunk][row = head*32 + c][4], tf32-rounded
 // (bf16: [64-channel stage][k|v][16-byte chunk][row][8] as bf16)
 static int pack_tc_kv(sbk_handle* h, const std::string& src, const std::string& key, int C, bool bf16) {
-    std::vector<float> q((size_t)384 * C);
-    CU(cudaMemcpy(q.data(), h->raw[src], q.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    std::vector<float> q;
+    TRY(h->w.fetch(src, q));
     const int EPC = bf16 ? 8 : 4, CPS = 8 * EPC;
     std::vector<uint8_t> m((size_t)256 * C * (bf16 ? 2 : 4));
     for (int ks = 0; ks < C / CPS; ++ks) for (int kv = 0; kv < 2; ++kv) for (int k = 0; k < 8; ++k)
@@ -361,16 +300,13 @@ static int pack_tc_kv(sbk_handle* h, const std::string& src, const std::string& 
             if (bf16) reinterpret_cast<uint16_t*>(m.data())[idx] = f32_to_bf16_rn(w);
             else reinterpret_cast<uint32_t*>(m.data())[idx] = f32_to_tf32_rna(w);
         }
-    float*& d = h->packed[key];
-    if (!d) { CU(cudaMalloc(&d, m.size())); h->owned.push_back(d); }
-    CU(cudaMemcpy(d, m.data(), m.size(), cudaMemcpyHostToDevice));
-    return SBK_OK;
+    return upload(h->w.packed, key, m.size(), m.data());
 }
 // fp32x3 mode: the same k and v rows for k_attn_kv_x3 (sbk_attn_x3.cu): per 32-channel stage a (w_hi, correction) pair of
 // images [k|v][16-byte chunk][row][16 B] - tf32 (RNA) w_hi, and the fp16 chunks {w[c0..c3], (w - w_hi)[c0..c3] * 2^12}
 static int pack_tc_kvx(sbk_handle* h, const std::string& src, const std::string& key, int C) {
-    std::vector<float> q((size_t)384 * C);
-    CU(cudaMemcpy(q.data(), h->raw[src], q.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    std::vector<float> q;
+    TRY(h->w.fetch(src, q));
     std::vector<uint8_t> m((size_t)2 * 256 * C * 4);
     for (int ks = 0; ks < C / 32; ++ks) for (int kv = 0; kv < 2; ++kv) for (int k = 0; k < 8; ++k)
         for (int row = 0; row < 128; ++row) for (int e = 0; e < 4; ++e) {
@@ -384,15 +320,12 @@ static int pack_tc_kvx(sbk_handle* h, const std::string& src, const std::string&
             cc[e] = f32_to_f16_rn(w);
             cc[4 + e] = f32_to_f16_rn((w - fh) * 4096.f);
         }
-    float*& d = h->packed[key];
-    if (!d) { CU(cudaMalloc(&d, m.size())); h->owned.push_back(d); }
-    CU(cudaMemcpy(d, m.data(), m.size(), cudaMemcpyHostToDevice));
-    return SBK_OK;
+    return upload(h->w.packed, key, m.size(), m.data());
 }
 // ConvTranspose2d weight [ci][co][4][4] -> logical [co][ci][kh*4+kw]
 static int pack_tc_up(sbk_handle* h, const std::string& src, const std::string& key, int C, bool bf16) {
-    std::vector<float> w((size_t)C * C * 16), m((size_t)C * C * 16);
-    CU(cudaMemcpy(w.data(), h->raw[src], w.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    std::vector<float> w, m((size_t)C * C * 16);
+    TRY(h->w.fetch(src, w));
     for (int ci = 0; ci < C; ++ci) for (int co = 0; co < C; ++co) for (int t = 0; t < 16; ++t)
         m[((size_t)co * C + ci) * 16 + t] = w[((size_t)ci * C + co) * 16 + t];
     return pack_tc_host(h, m, key, C, C, G_UP, bf16);
@@ -431,22 +364,17 @@ size_t sbk::conv_tc_pack_image(const float* hs, int cout, int cin, int geom, boo
         }
     return bytes;
 }
+// fp32x3 handles (and the CUDA-core fp32 handles' RefBlock branch) pack every tensor-core weight as (hi, lo) stage pairs
 static int pack_tc_host(sbk_handle* h, const std::vector<float>& hs, const std::string& key, int cout, int cin, int geom, bool bf16, int nt_override) {
-    const bool x3 = !bf16 && packs_x3(h);
+    const bool x3 = !bf16 && prec_runs_x3(h->cfg.precision);
     std::vector<uint8_t> hd(conv_tc_pack_image(hs.data(), cout, cin, geom, bf16, x3, nt_override, nullptr));
     conv_tc_pack_image(hs.data(), cout, cin, geom, bf16, x3, nt_override, hd.data());
-    float*& d = h->packed[key];
-    if (!d) { CU(cudaMalloc(&d, hd.size())); h->owned.push_back(d); }
-    CU(cudaMemcpy(d, hd.data(), hd.size(), cudaMemcpyHostToDevice));
-    return SBK_OK;
+    return upload(h->w.packed, key, hd.size(), hd.data());
 }
-
-#define TRY(x) do { int rc_ = (x); if (rc_ != SBK_OK) return rc_; } while (0)
 
 extern "C" int sbk_pack(sbk_handle* h) {
     if (!h) return fail(SBK_ERR_ARG, "sbk_pack: null handle");
-    for (auto& s : h->spec)
-        if (!h->raw.count(s.name)) return fail(SBK_ERR_STATE, "sbk_pack: missing key '%s' (strict)", s.name.c_str());
+    TRY(h->w.require_all("sbk_pack"));
     CU(cudaSetDevice(h->cfg.device));
     // conv KxK [co][ci][r][s] -> [r*K+s][ci][co]
     auto conv_pack = [](float* d, const float* s, const std::vector<int64_t>& sh) {
@@ -536,15 +464,14 @@ extern "C" int sbk_pack(sbk_handle* h) {
         std::vector<float> f(half);
         const float neg = (float)(-(log(10000.0) / (double)(half - 1)));
         for (int j = 0; j < half; ++j) f[j] = expf((float)j * neg);
-        if (!h->d_freqs) { CU(cudaMalloc(&h->d_freqs, half * sizeof(float))); h->owned.push_back(h->d_freqs); }
+        if (!h->d_freqs) CU(cudaMalloc(&h->d_freqs, half * sizeof(float)));
         CU(cudaMemcpy(h->d_freqs, f.data(), half * sizeof(float), cudaMemcpyHostToDevice));
     }
     if (!h->d_zero) {
         CU(cudaMalloc(&h->d_zero, 8192));
-        h->owned.push_back(h->d_zero);
         CU(cudaMemset(h->d_zero, 0, 8192));
     }
-    free_plan(h, false);   // packed pointers may have changed; the arena itself stays
+    free_plan(h);   // packed pointers may have changed; the arena itself stays
     h->is_packed = true;
     return SBK_OK;
 }
@@ -607,7 +534,7 @@ static size_t layout(const sbk_handle* h, int B, int T, int tb_rows, Arena& ar, 
         p.vc_wextra = f((size_t)tb_rows * B * 9 * dim);
         p.vc_rextra = f((size_t)tb_rows * B * dim);
     }
-    return ar.off + 256;
+    return ar.bytes();
 }
 
 // rows of the per-step tables (time projections, coefficients, DiffVC conditioning): the same rule ensure_plan uses
@@ -621,25 +548,15 @@ extern "C" size_t sbk_workspace_bytes_n(const sbk_handle* h, int B, int T, int n
 extern "C" size_t sbk_workspace_bytes(const sbk_handle* h, int B, int T) { return sbk_workspace_bytes_n(h, B, T, 1024); }
 
 static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
-    free_plan(h, false);
+    free_plan(h);
     Plan& pl = h->plan;
     const sbk_config& c = h->cfg;
     Arena probe;
     const size_t bytes = layout(h, B, T, tb_rows, probe, nullptr, nullptr);
-    if (bytes > pl.cap) {
-        // grow-only arena: utterance lengths change from call to call, and a cudaFree/cudaMalloc pair is a device-wide sync
-        if (pl.mem) { cudaFree(pl.mem); pl.mem = nullptr; pl.cap = 0; }
-        const cudaError_t e = cudaMalloc(&pl.mem, bytes);
-        if (e != cudaSuccess) {
-            pl.mem = nullptr;
-            cudaGetLastError();
-            return fail(SBK_ERR_CUDA, "out of memory: the (B=%d, T=%d) workspace needs %zu bytes (%s); free cached blocks "
-                                      "(torch.cuda.empty_cache()) or split the batch", B, T, bytes, cudaGetErrorString(e));
-        }
-        pl.cap = bytes;
-    }
-    pl.bytes = bytes;
-    Arena ar; ar.base = (char*)pl.mem; ar.cap = bytes;
+    if (const cudaError_t e = h->ws.reserve(bytes))
+        return fail(SBK_ERR_CUDA, "out of memory: the (B=%d, T=%d) workspace needs %zu bytes (%s); free cached blocks "
+                                  "(torch.cuda.empty_cache()) or split the batch", B, T, bytes, cudaGetErrorString(e));
+    Arena ar = h->ws.arena();
     Bufs bf;
     layout(h, B, T, tb_rows, ar, &bf, &pl);
     pl.B = B; pl.T = T; pl.tb_rows = tb_rows;
@@ -650,14 +567,8 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
     const int cin0 = vc ? 3 : 2 + (c.n_spks > 1 ? 1 : 0);     // DiffVC: {mean, xt, folded conditioning channel}
     int gn_slot = 0;
     auto stats_slot = [&]() { return pl.stats + (size_t)(gn_slot++) * B * kGroups * 2; };
-    auto W = [&](const std::string& k) -> const float* {
-        auto it = h->packed.find(k);
-        if (it != h->packed.end()) return it->second;
-        auto it2 = h->raw.find(k);
-        return it2 != h->raw.end() ? it2->second : nullptr;
-    };
     auto gnref = [&](const double* st, const std::string& blk, int C, int lvl) {
-        GnRef g; g.stats = st; g.gamma = W(blk + ".block.1.weight"); g.beta = W(blk + ".block.1.bias");
+        GnRef g; g.stats = st; g.gamma = h->w.get(blk + ".block.1.weight"); g.beta = h->w.get(blk + ".block.1.bias");
         g.inv_count = 1.0f / ((float)(C / kGroups) * (float)Hs[lvl] * (float)Ws[lvl]);
         return g;
     };
@@ -671,8 +582,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
     const bool use_tc = c.precision != SBK_PREC_FP32;
     const bool x3 = c.precision == SBK_PREC_FP32X3;
     auto LO = [&](const void* q) -> float* { auto it = bf.lo.find(q); return it == bf.lo.end() ? nullptr : it->second; };
-    int num_sms = 132;
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, c.device);
+    const int num_sms = device_sm_count();
     const char* rows_env = getenv("SBK_CONV3_ROWS");
     const int conv_rows_env = rows_env ? atoi(rows_env) : 0;
     const bool b16 = c.precision == SBK_PREC_BF16;          // operand tensors in bf16 [B][H][C/8][W][8]
@@ -714,7 +624,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         ConvTcParams& p = op.tc; memset(&p, 0, sizeof(p));
         p.geom = geom; p.in0 = in0; p.c0 = c0; p.in1 = in1; p.c1 = c1; p.H = Hs[lvl]; p.W = Ws[lvl]; p.B = B;
         p.Ho = p.H; p.Wo = p.W;
-        p.wpk = W(wkey); p.bias = bkey.empty() ? nullptr : W(bkey); p.out = out; p.Cout = cout;
+        p.wpk = h->w.get(wkey); p.bias = bkey.empty() ? nullptr : h->w.get(bkey); p.out = out; p.Cout = cout;
         p.epi = EPI_PLAIN; p.ostats = st; p.mask = pl.mask; p.T = T; p.lvl = lvl; p.zero_page = h->d_zero;
         p.bf16 = b16 ? 1 : 0;
         if (x3) {
@@ -730,13 +640,13 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             bool two = tiles2 >= 4LL * num_sms;
             if (conv_rows_env == 1 || conv_rows_env == 2) two = conv_rows_env == 2;
             const bool wide = conv_tc_ntile(geom, cout) == 128;
-            if (two && (!wide || h->packed.count(wkey + "64"))) {
+            if (two && (!wide || h->w.packed.count(wkey + "64"))) {
                 p.rows = 2;
-                if (wide) { p.nt = 64; p.wpk = W(wkey + "64"); }
+                if (wide) { p.nt = 64; p.wpk = h->w.get(wkey + "64"); }
             } else if (wide) {
                 // tiles of one row x 128 pixels x 128 channels; when they cannot fill half the SMs, use 64-wide N tiles instead
                 const long long tiles = (long long)B * wt * Hs[lvl] * (cout / 128);
-                if (tiles * 2 <= num_sms && h->packed.count(wkey + "64")) { p.nt = 64; p.wpk = W(wkey + "64"); }
+                if (tiles * 2 <= num_sms && h->w.packed.count(wkey + "64")) { p.nt = 64; p.wpk = h->w.get(wkey + "64"); }
             }
         }
         const double taps = geom == G_PW ? 1.0 : (geom == G_UP ? 4.0 : 9.0);
@@ -751,7 +661,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         Op op; op.name = name; op.kind = OP_IGEMM;
         op.ig = base_ig(G_C3, lvl, lvl);
         IgemmParams& p = op.ig;
-        p.in0 = in0; p.c0 = c0; p.in1 = in1; p.c1 = c1; p.w = W(wkey); p.bias = W(bkey);
+        p.in0 = in0; p.c0 = c0; p.in1 = in1; p.c1 = c1; p.w = h->w.get(wkey); p.bias = h->w.get(bkey);
         p.out = out; p.Cout = cout; p.pro = pro; p.epi = EPI_PLAIN; p.ostats = st;
         if (pgn) { p.pgn = *pgn; p.tb = pl.tb + h->tb_off[tb_k]; p.tb_stride = pl.tb_stride; }
         push(op, out, npix(lvl) * cout);
@@ -767,7 +677,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             Op op; op.kind = OP_FIRST; op.name = r.prefix + ".block1.raw";
             FirstConvParams& p = op.fc; memset(&p, 0, sizeof(p));
             p.mu = pl.mu; p.xt = pl.xt; p.spk_s = pl.spk_s; p.mask = pl.mask;
-            p.w = W(r.prefix + ".block1.w"); p.bias = W(r.prefix + ".block1.block.0.bias");
+            p.w = h->w.get(r.prefix + ".block1.w"); p.bias = h->w.get(r.prefix + ".block1.block.0.bias");
             p.out = A; p.ostats = st1; p.B = B; p.H = H0; p.T = T; p.cin = cin0; p.C = r.cout; p.chw4 = use_tc ? 1 : 0;
             if (vc) { p.w_extra = pl.vc_wextra; p.step = pl.step_cur; }
             pl.first_op = (int)pl.ops.size();
@@ -811,7 +721,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             p.out_mask = store_masked ? 1 : 0; p.chw4 = use_tc ? 1 : 0; p.bf16 = b16 ? 1 : 0; p.out_lo = LO(out);
             if (k == 0) {
                 p.x = nullptr; p.mu = pl.mu; p.xt = pl.xt; p.spk_s = pl.spk_s; p.cin = cin0;
-                p.wres = W(r.prefix + ".res.w"); p.bres = W(r.prefix + ".res_conv.bias");
+                p.wres = h->w.get(r.prefix + ".res.w"); p.bres = h->w.get(r.prefix + ".res_conv.bias");
                 if (vc) { p.r_extra = pl.vc_rextra; p.step = pl.step_cur; }
                 pl.first_res_op = (int)pl.ops.size();
             } else {
@@ -830,7 +740,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             op.ig = base_ig(G_PW, lvl, lvl);
             IgemmParams& p = op.ig;
             p.in0 = in0; p.c0 = c0; p.in1 = in1; p.c1 = c1;
-            p.w = W(r.prefix + ".res.w"); p.bias = W(r.prefix + ".res_conv.bias");
+            p.w = h->w.get(r.prefix + ".res.w"); p.bias = h->w.get(r.prefix + ".res_conv.bias");
             p.out = out; p.Cout = r.cout; p.pro = PRO_MASK; p.epi = EPI_RES;
             p.rraw = h2; p.rgn = g2; p.out_mask = store_masked ? 1 : 0;
             push(op, out, npix(lvl) * r.cout);
@@ -863,7 +773,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             Op op; op.kind = OP_IGEMM; op.name = a.prefix + ".kvpart";
             op.ig = base_ig(G_PW, lvl, lvl);
             IgemmParams& p = op.ig;
-            p.in0 = x; p.c0 = a.c; p.w = W(a.prefix + ".kv.w"); p.Cout = 256; p.pro = PRO_NONE; p.epi = EPI_KV;
+            p.in0 = x; p.c0 = a.c; p.w = h->w.get(a.prefix + ".kv.w"); p.Cout = 256; p.pro = PRO_NONE; p.epi = EPI_KV;
             p.kv_part = bf.kv_part; p.out = nullptr;
             push(op, nullptr, 0);
         }
@@ -875,8 +785,8 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         {
             Op op; op.kind = OP_MIX; op.name = a.prefix + ".mix";
             AttnMixParams& p = op.mx; memset(&p, 0, sizeof(p));
-            p.ctx = bf.ctx; p.wq = W(a.prefix + ".fn.fn.to_qkv.weight"); p.wout = W(a.prefix + ".fn.fn.to_out.weight");
-            p.bout = W(a.prefix + ".fn.fn.to_out.bias"); p.g = W(a.prefix + ".fn.g");
+            p.ctx = bf.ctx; p.wq = h->w.get(a.prefix + ".fn.fn.to_qkv.weight"); p.wout = h->w.get(a.prefix + ".fn.fn.to_out.weight");
+            p.bout = h->w.get(a.prefix + ".fn.fn.to_out.bias"); p.g = h->w.get(a.prefix + ".fn.g");
             p.w_eff = bf.w_eff; p.b_eff = bf.b_eff; p.B = B; p.C = a.c;
             if (tc_apply) { p.tc_nt = x3 ? conv_tc_ntile_x3(G_PW, a.c) : conv_tc_ntile(G_PW, a.c); p.tc_cps = tc_cps1; p.tc_bf16 = b16 ? 1 : 0; p.tc_x3 = x3 ? 1 : 0; }
             push(op, nullptr, 0);
@@ -909,7 +819,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         Op op; op.kind = OP_IGEMM; op.name = pre + ".out";
         op.ig = base_ig(geom, lvl_in, lvl_out);
         IgemmParams& p = op.ig;
-        p.in0 = x; p.c0 = C; p.w = W(pre + ".conv.w"); p.bias = W(pre + ".conv.bias");
+        p.in0 = x; p.c0 = C; p.w = h->w.get(pre + ".conv.w"); p.bias = h->w.get(pre + ".conv.bias");
         p.out = out; p.Cout = C; p.pro = PRO_MASK; p.epi = EPI_PLAIN; p.out_mask = use_tc ? 1 : 0;
         push(op, out, npix(lvl_out) * C);
     };
@@ -955,7 +865,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         Op op; op.kind = OP_FINAL; op.name = "estimator.out";
         FinalParams& p = op.fn; memset(&p, 0, sizeof(p));
         p.raw = bf.A[0]; p.gn = gnref(stf, "estimator.final_block", C1, 0);
-        p.wfin = W("estimator.final_conv.weight"); p.bfin = W("estimator.final_conv.bias");
+        p.wfin = h->w.get("estimator.final_conv.weight"); p.bfin = h->w.get("estimator.final_conv.bias");
         p.mask = pl.mask; p.mu = pl.mu; p.xt_in = pl.xt; p.xt_out = pl.xt;
         p.coef = pl.coef; p.step = pl.step_cur; p.B = B; p.H = H0; p.T = T; p.C = C1; p.chw4 = use_tc ? 1 : 0; p.exact = x3 ? 1 : 0;
         pl.final_op = (int)pl.ops.size();
@@ -990,7 +900,7 @@ static int run_ops(sbk_handle* h, cudaStream_t s) {
         if (k < 0) { fail(SBK_ERR_CUDA, "launch of '%s' was refused (device attribute / layout)", op.name.c_str()); return -1; }
         n += k;
         if (h->capture && op.dbg_ptr && op.dbg_numel > 0) {
-            const size_t esz = op.dbg_fmt == 2 ? 2 : 4;
+            const size_t esz = snap_elem_bytes(op.dbg_fmt);
             if (!op.dbg_copy) cudaMalloc(&op.dbg_copy, op.dbg_numel * esz);
             cudaMemcpyAsync(op.dbg_copy, op.dbg_ptr, op.dbg_numel * esz, cudaMemcpyDeviceToDevice, s);
         }
@@ -1003,9 +913,9 @@ static int ensure_plan(sbk_handle* h, int B, int T, int rows) {
     if (B <= 0 || T <= 0 || T % 4 != 0) return fail(SBK_ERR_ARG, "B must be > 0 and T a positive multiple of 4 (fix_len_compatibility), got B=%d T=%d", B, T);
     CU(cudaSetDevice(h->cfg.device));
     Plan& pl = h->plan;
-    if (pl.mem && pl.B == B && pl.T == T && pl.tb_rows >= rows) return SBK_OK;
+    if (pl.B == B && pl.T == T && pl.tb_rows >= rows) return SBK_OK;     // (a freed plan has B = 0)
     int cap = rows < 64 ? 64 : rows;
-    if (pl.mem && pl.B == B && pl.T == T && cap < pl.tb_rows) cap = pl.tb_rows;
+    if (pl.B == B && pl.T == T && cap < pl.tb_rows) cap = pl.tb_rows;
     return build_plan(h, B, T, cap);
 }
 
@@ -1013,12 +923,12 @@ static int time_table(sbk_handle* h, int rows, cudaStream_t s) {
     Plan& pl = h->plan;
     TimeTableParams p; memset(&p, 0, sizeof(p));
     p.t_rows = pl.t_rows; p.rows = rows; p.freqs = h->d_freqs; p.pe_scale = h->cfg.pe_scale; p.dim = h->cfg.dim;
-    p.w0 = h->raw["estimator.mlp.0.weight"]; p.b0 = h->raw["estimator.mlp.0.bias"];
-    p.w2 = h->raw["estimator.mlp.2.weight"]; p.b2 = h->raw["estimator.mlp.2.bias"];
+    p.w0 = h->w.get("estimator.mlp.0.weight"); p.b0 = h->w.get("estimator.mlp.0.bias");
+    p.w2 = h->w.get("estimator.mlp.2.weight"); p.b2 = h->w.get("estimator.mlp.2.bias");
     p.nproj = (int)h->resnets.size();
     for (int k = 0; k < p.nproj; ++k) {
-        p.pw[k] = h->raw[h->resnets[k].prefix + ".mlp.1.weight"];
-        p.pb[k] = h->raw[h->resnets[k].prefix + ".mlp.1.bias"];
+        p.pw[k] = h->w.get(h->resnets[k].prefix + ".mlp.1.weight");
+        p.pb[k] = h->w.get(h->resnets[k].prefix + ".mlp.1.bias");
         p.pc[k] = h->resnets[k].cout; p.poff[k] = h->tb_off[k];
     }
     p.tb = pl.tb; p.tb_stride = pl.tb_stride;
@@ -1029,8 +939,8 @@ static int speaker(sbk_handle* h, const float* spk, int B, cudaStream_t s) {
     if (h->cfg.n_spks < 2) return 0;
     Plan& pl = h->plan;
     SpkParams p; p.spk = spk; p.B = B; p.E = h->cfg.spk_emb_dim; p.n_feats = h->cfg.n_feats; p.out = pl.spk_s;
-    p.w0 = h->raw["estimator.spk_mlp.0.weight"]; p.b0 = h->raw["estimator.spk_mlp.0.bias"];
-    p.w2 = h->raw["estimator.spk_mlp.2.weight"]; p.b2 = h->raw["estimator.spk_mlp.2.bias"];
+    p.w0 = h->w.get("estimator.spk_mlp.0.weight"); p.b0 = h->w.get("estimator.spk_mlp.0.bias");
+    p.w2 = h->w.get("estimator.spk_mlp.2.weight"); p.b2 = h->w.get("estimator.spk_mlp.2.bias");
     return launch_spk(p, s);
 }
 
@@ -1321,8 +1231,8 @@ static int vc_fold(sbk_handle* h, const float* cond, int rows, int B, cudaStream
     const sbk_config& c = h->cfg;
     CU(cudaMemcpyAsync(pl.vc_cond, cond, (size_t)rows * B * c.dim_cond * sizeof(float), cudaMemcpyDeviceToDevice, s));
     CondFoldParams p;
-    p.cond = pl.vc_cond; p.w1 = h->raw["estimator.downs.0.0.block1.block.0.weight"];
-    p.wres = h->raw["estimator.downs.0.0.res_conv.weight"];
+    p.cond = pl.vc_cond; p.w1 = h->w.get("estimator.downs.0.0.block1.block.0.weight");
+    p.wres = h->w.get("estimator.downs.0.0.res_conv.weight");
     p.w_extra = pl.vc_wextra; p.r_extra = pl.vc_rextra; p.rows = rows; p.B = B; p.dc = c.dim_cond; p.C = c.dim;
     return launch_cond_fold(p, s);
 }
@@ -1385,7 +1295,7 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
     if (!h->is_packed) return fail(SBK_ERR_STATE, "sbk_vc_conditioning: weights not packed");
     if (h->cfg.use_ref_t && h->cfg.dim_cond % 128 != 0) return fail(SBK_ERR_ARG, "sbk_vc_conditioning: dim_cond must be a multiple of 128");
     // fp32-class handles (fp32x3 and the CUDA-core fp32 mode) run the RefBlock convs with the tf32 + fp16-correction split and exact IN / GLU
-    const bool x3 = packs_x3(h);
+    const bool x3 = prec_runs_x3(h->cfg.precision);
     if (B <= 0 || Tr <= 0 || n_timesteps < 1) return fail(SBK_ERR_ARG, "sbk_vc_conditioning: bad sizes");
     CU(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
@@ -1393,9 +1303,8 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
     const int H = cf.n_feats, dc = cf.dim_cond, base = dc / 4, N = n_timesteps, dim = cf.dim;
     const size_t px = (size_t)B * H * Tr;
     // ---- workspace
-    Arena probe;
-    float* act_lo = nullptr;
-    auto carve = [&](Arena& ar, float*& xt_ref, float*& raw, float*& act, double*& st, double*& ys, float*& tb, float*& trows) {
+    float *xt_ref, *raw, *act, *act_lo, *tb, *trows; double *st, *ys;
+    auto carve = [&](Arena& ar) {
         xt_ref = (float*)ar.take(px * sizeof(float));
         raw = (float*)ar.take(px * 8 * base * sizeof(float));
         act = (float*)ar.take(px * 4 * base * sizeof(float));
@@ -1405,17 +1314,12 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
         tb = (float*)ar.take((size_t)N * 3 * base * sizeof(float));
         trows = (float*)ar.take((size_t)N * sizeof(float));
     };
-    float *xt_ref, *raw, *act, *tb, *trows; double *st, *ys;
-    carve(probe, xt_ref, raw, act, st, ys, tb, trows);
-    const size_t need = probe.off + 256;
-    if (need > h->ref_bytes) {
-        if (h->ref_mem) CU(cudaFree(h->ref_mem));
-        h->ref_mem = nullptr; h->ref_bytes = 0;
-        CU(cudaMalloc(&h->ref_mem, need));
-        h->ref_bytes = need;
-    }
-    Arena ar; ar.base = (char*)h->ref_mem; ar.cap = h->ref_bytes;
-    carve(ar, xt_ref, raw, act, st, ys, tb, trows);
+    Arena probe;
+    carve(probe);
+    if (const cudaError_t e = h->ref_ws.reserve(probe.bytes()))
+        return fail(SBK_ERR_CUDA, "out of memory: the RefBlock workspace for (B=%d, Tr=%d) needs %zu bytes (%s)", B, Tr, probe.bytes(), cudaGetErrorString(e));
+    Arena ar = h->ref_ws.arena();
+    carve(ar);
     // ---- time values + the two RefBlock time biases (mlp1, mlp2: Mish -> Linear on the time-MLP output) for all steps
     std::vector<float> tr(N);
     for (int i = 0; i < N; ++i) tr[i] = (float)(1.0 - i * (1.0 / N));
@@ -1424,20 +1328,14 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
     if (cf.use_ref_t) {
         TimeTableParams tp; memset(&tp, 0, sizeof(tp));
         tp.t_rows = trows; tp.rows = N; tp.freqs = h->d_freqs; tp.pe_scale = 1000.0f; tp.dim = dim;
-        tp.w0 = h->raw["estimator.mlp.0.weight"]; tp.b0 = h->raw["estimator.mlp.0.bias"];
-        tp.w2 = h->raw["estimator.mlp.2.weight"]; tp.b2 = h->raw["estimator.mlp.2.bias"];
+        tp.w0 = h->w.get("estimator.mlp.0.weight"); tp.b0 = h->w.get("estimator.mlp.0.bias");
+        tp.w2 = h->w.get("estimator.mlp.2.weight"); tp.b2 = h->w.get("estimator.mlp.2.bias");
         tp.nproj = 2;
-        tp.pw[0] = h->raw["estimator.ref_block.mlp1.1.weight"]; tp.pb[0] = h->raw["estimator.ref_block.mlp1.1.bias"]; tp.pc[0] = base; tp.poff[0] = 0;
-        tp.pw[1] = h->raw["estimator.ref_block.mlp2.1.weight"]; tp.pb[1] = h->raw["estimator.ref_block.mlp2.1.bias"]; tp.pc[1] = 2 * base; tp.poff[1] = base;
+        tp.pw[0] = h->w.get("estimator.ref_block.mlp1.1.weight"); tp.pb[0] = h->w.get("estimator.ref_block.mlp1.1.bias"); tp.pc[0] = base; tp.poff[0] = 0;
+        tp.pw[1] = h->w.get("estimator.ref_block.mlp2.1.weight"); tp.pb[1] = h->w.get("estimator.ref_block.mlp2.1.bias"); tp.pc[1] = 2 * base; tp.poff[1] = base;
         tp.tb = tb; tp.tb_stride = 3 * base;
         n += launch_time_table(tp, s);
     }
-    auto W = [&](const std::string& k) -> const float* {
-        auto it = h->packed.find(k);
-        if (it != h->packed.end()) return it->second;
-        auto it2 = h->raw.find(k);
-        return it2 != h->raw.end() ? it2->second : nullptr;
-    };
     auto gamma0 = [&](double t) {       // get_gamma(0, t), diffusion.py:124-131
         double bi = cf.beta_min + 0.5 * ((double)cf.beta_max - cf.beta_min) * t;
         bi *= t;
@@ -1447,28 +1345,16 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
         ConvTcParams p; memset(&p, 0, sizeof(p));
         const std::string q = std::string("estimator.ref_block.") + name;
         p.geom = G_C3; p.in0 = act; p.c0 = cin; p.H = H; p.W = Tr; p.B = B; p.Ho = H; p.Wo = Tr;
-        p.wpk = W(q + ".wtc"); p.bias = W(q + ".0.bias"); p.out = raw; p.Cout = cout; p.epi = EPI_PLAIN;
+        p.wpk = h->w.get(q + ".wtc"); p.bias = h->w.get(q + ".0.bias"); p.out = raw; p.Cout = cout; p.epi = EPI_PLAIN;
         p.mask = ref_mask; p.T = Tr; p.zero_page = h->d_zero;
         if (x3) { p.x3 = 1; p.in0_lo = act_lo; }
         return launch_conv_tc(p, s);
     };
-    // debug capture: every step reuses the workspace, so each tensor the branch writes is copied (stream-ordered) right
-    // after the launch that wrote it into a per-name buffer; step i overwrites step i-1's copies, so the last step remains.
-    // The copies are not launches and do not count in last_launches.
-    size_t nsnap = 0;
-    cudaError_t snap_err = cudaSuccess;
+    // debug capture: every step writes the same workspace buffers, so the last step's tensors are recorded
+    h->vc_snaps.begin();
+    bool last_step = false;
     auto snap = [&](const char* name, const char* suf, const void* src, size_t numel, int fmt) {
-        if (!h->capture || snap_err != cudaSuccess) return;
-        if (nsnap == h->vc_snaps.size()) h->vc_snaps.push_back({std::string(), nullptr, 0, 0, 0});
-        sbk_handle::VcSnap& sn = h->vc_snaps[nsnap++];
-        const size_t bytes = numel * (fmt == 3 ? sizeof(double) : sizeof(float));
-        sn.name = std::string("ref_block.") + name + suf; sn.numel = numel; sn.fmt = fmt;
-        if (bytes > sn.cap) {
-            cudaFree(sn.buf); sn.buf = nullptr; sn.cap = 0;
-            if ((snap_err = cudaMalloc(&sn.buf, bytes)) != cudaSuccess) { sn.buf = nullptr; sn.numel = 0; return; }
-            sn.cap = bytes;
-        }
-        snap_err = cudaMemcpyAsync(sn.buf, src, bytes, cudaMemcpyDeviceToDevice, s);
+        if (h->vc_snaps.on && last_step) h->vc_snaps.record(std::string("ref_block.") + name + suf, src, numel, fmt, s);
     };
     auto norm_glu = [&](const char* name, int C, const float* tbias) {
         const std::string q = std::string("estimator.ref_block.") + name;
@@ -1476,7 +1362,7 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
         int k = launch_chan_stats(cs, s);
         snap(name, ".stats", st, (size_t)B * C * 2, 3);
         InGluParams g; memset(&g, 0, sizeof(g));
-        g.raw = raw; g.stats = st; g.gamma = W(q + ".1.weight"); g.beta = W(q + ".1.bias"); g.tb = tbias;
+        g.raw = raw; g.stats = st; g.gamma = h->w.get(q + ".1.weight"); g.beta = h->w.get(q + ".1.bias"); g.tb = tbias;
         g.mask = ref_mask; g.T = Tr; g.out = act; g.out_lo = act_lo; g.B = B; g.H = H; g.W = Tr; g.C = C;
         k += launch_in_glu(g, s);
         snap(name, ".act", act, px * C / 2, 1);
@@ -1487,7 +1373,7 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
     const Stage stages[5] = {{"block12", base, 2 * base, 0}, {"block21", base, 4 * base, -1}, {"block22", 2 * base, 4 * base, base},
                              {"block31", 2 * base, 8 * base, -1}, {"block32", 4 * base, 8 * base, -1}};
     for (int i = 0; i < N; ++i) {
-        nsnap = 0;
+        last_step = i + 1 == N;
         if (cf.use_ref_t) {
             const float* tb_row = tb + (size_t)i * 3 * base;
             DiffMeanParams dm{ref, mean_ref, ref_mask, xt_ref, (float)gamma0(1.0 - i * (1.0 / N)), B, H, Tr};
@@ -1495,8 +1381,8 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
             snap("xt_ref", "", xt_ref, px, 0);
             snap("tb", "", tb_row, (size_t)3 * base, 0);
             FirstConvParams fc; memset(&fc, 0, sizeof(fc));
-            fc.mu = xt_ref; fc.xt = xt_ref; fc.mask = ref_mask; fc.w = W("estimator.ref_block.block11.w");
-            fc.bias = W("estimator.ref_block.block11.0.bias"); fc.out = raw; fc.ostats = nullptr;
+            fc.mu = xt_ref; fc.xt = xt_ref; fc.mask = ref_mask; fc.w = h->w.get("estimator.ref_block.block11.w");
+            fc.bias = h->w.get("estimator.ref_block.block11.0.bias"); fc.out = raw; fc.ostats = nullptr;
             fc.B = B; fc.H = H; fc.T = Tr; fc.cin = 1; fc.C = 2 * base; fc.chw4 = 1;
             n += launch_first_conv(fc, s);
             snap("block11", ".raw", raw, px * 2 * base, 1);
@@ -1514,46 +1400,31 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
         }
         VcCondParams vp; memset(&vp, 0, sizeof(vp));
         vp.ysum = ys; vp.mask = ref_mask; vp.Tr = Tr; vp.H = H;
-        vp.wf = W("estimator.ref_block.final_conv.weight"); vp.bf = W("estimator.ref_block.final_conv.bias");
+        vp.wf = h->w.get("estimator.ref_block.final_conv.weight"); vp.bf = h->w.get("estimator.ref_block.final_conv.bias");
         vp.c = c; vp.freqs = h->d_freqs; vp.t = tr[i]; vp.dim = dim;
-        vp.w0 = W("estimator.cond_block.0.weight"); vp.b0 = W("estimator.cond_block.0.bias");
-        vp.w2 = W("estimator.cond_block.2.weight"); vp.b2 = W("estimator.cond_block.2.bias");
+        vp.w0 = h->w.get("estimator.cond_block.0.weight"); vp.b0 = h->w.get("estimator.cond_block.0.bias");
+        vp.w2 = h->w.get("estimator.cond_block.2.weight"); vp.b2 = h->w.get("estimator.cond_block.2.bias");
         vp.out = cond_out + (size_t)i * B * dc; vp.B = B; vp.dc = dc; vp.use_ref = cf.use_ref_t ? 1 : 0;
         n += launch_vc_cond(vp, s);
     }
-    if (h->capture) {
-        for (size_t i = nsnap; i < h->vc_snaps.size(); ++i) cudaFree(h->vc_snaps[i].buf);
-        h->vc_snaps.resize(nsnap);
-    }
-    if (snap_err != cudaSuccess) return fail(SBK_ERR_CUDA, "sbk_vc_conditioning: debug capture failed: %s", cudaGetErrorString(snap_err));
+    if (const cudaError_t e = h->vc_snaps.finish()) return fail(SBK_ERR_CUDA, "sbk_vc_conditioning: debug capture failed: %s", cudaGetErrorString(e));
     CU(cudaGetLastError());
     h->last_launches = n;
     return SBK_OK;
 }
 
-extern "C" int sbk_vc_cond_debug_num(const sbk_handle* h) { return h ? (int)h->vc_snaps.size() : 0; }
+extern "C" int sbk_vc_cond_debug_num(const sbk_handle* h) { return h ? (int)h->vc_snaps.list.size() : 0; }
 extern "C" const char* sbk_vc_cond_debug_name(const sbk_handle* h, int i) {
-    if (!h || i < 0 || i >= (int)h->vc_snaps.size()) return nullptr;
-    return h->vc_snaps[i].name.c_str();
+    if (!h || i < 0 || i >= (int)h->vc_snaps.list.size()) return nullptr;
+    return h->vc_snaps.list[i].name.c_str();
 }
 extern "C" int sbk_vc_cond_debug_op_layout(const sbk_handle* h, const char* name) {
-    if (!h || !name) return -1;
-    for (auto& sn : h->vc_snaps) if (sn.name == name) return sn.fmt;
-    return -1;
+    const Snapshots::Snap* sn = h && name ? h->vc_snaps.find(name) : nullptr;
+    return sn ? sn->fmt : -1;
 }
 extern "C" int sbk_vc_cond_debug_read(sbk_handle* h, const char* name, void* dst, int64_t* numel) {
     if (!h || !name) return fail(SBK_ERR_ARG, "sbk_vc_cond_debug_read: null argument");
-    for (auto& sn : h->vc_snaps) {
-        if (sn.name != name) continue;
-        if (numel) *numel = (int64_t)sn.numel;
-        if (dst && sn.numel > 0) {
-            CU(cudaSetDevice(h->cfg.device));
-            CU(cudaDeviceSynchronize());
-            CU(cudaMemcpy(dst, sn.buf, sn.numel * (sn.fmt == 3 ? sizeof(double) : sizeof(float)), cudaMemcpyDefault));
-        }
-        return SBK_OK;
-    }
-    return fail(SBK_ERR_ARG, "sbk_vc_cond_debug_read: no intermediate named '%s'", name);
+    return h->vc_snaps.read(name, dst, numel, h->cfg.device, "sbk_vc_cond_debug_read");
 }
 
 extern "C" int sbk_prior_expand(const float* mu_x, const float* w_ceil, const float* x_mask, const int64_t* y_lengths,
@@ -1577,7 +1448,7 @@ extern "C" int sbk_last_host_launches(const sbk_handle* h) { return h ? h->last_
 
 extern "C" int sbk_debug_capture(sbk_handle* h, int on) {
     if (!h) return fail(SBK_ERR_ARG, "sbk_debug_capture: null handle");
-    h->capture = on != 0;
+    h->capture = h->vc_snaps.on = on != 0;
     return SBK_OK;
 }
 extern "C" int sbk_debug_layout(const sbk_handle* h) { return (h && h->cfg.precision != SBK_PREC_FP32) ? 1 : 0; }
@@ -1601,14 +1472,7 @@ extern "C" int sbk_debug_read(sbk_handle* h, const char* name, float* dst, int64
         if (dst && op.dbg_ptr && op.dbg_numel > 0) {
             CU(cudaDeviceSynchronize());
             const void* src = op.dbg_copy ? (const void*)op.dbg_copy : (const void*)op.dbg_ptr;
-            if (op.dbg_fmt == 2) {
-                // bf16 operand tensor: widened to fp32 on the host (dst must be host memory), element order unchanged
-                std::vector<uint16_t> tmp(op.dbg_numel);
-                CU(cudaMemcpy(tmp.data(), src, op.dbg_numel * 2, cudaMemcpyDeviceToHost));
-                for (int64_t i = 0; i < op.dbg_numel; ++i) { const uint32_t u = (uint32_t)tmp[i] << 16; memcpy(&dst[i], &u, 4); }
-            } else {
-                CU(cudaMemcpy(dst, src, op.dbg_numel * sizeof(float), cudaMemcpyDefault));
-            }
+            return read_widened(dst, src, op.dbg_numel, op.dbg_fmt);
         }
         return SBK_OK;
     }

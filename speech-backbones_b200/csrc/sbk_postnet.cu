@@ -14,8 +14,7 @@
 //      equals final_conv.bias).  A separate CUDA-core pass: dim MACs per pixel, < 1 % of the PostNet's time; the 1x1 res
 //      conv's epilogue would need a new template variant for it.
 // GroupNorm statistics cover the whole n_feats x T grid, padded columns included, as the reference's GroupNorm does.
-#include "../../include/sbk.h"
-#include "sbk_internal.h"
+#include "sbk_host.h"
 
 #include <math.h>
 #include <stdio.h>
@@ -26,15 +25,6 @@
 #include <vector>
 
 using namespace sbk;
-
-int sbk_set_error(int code, const char* fmt, ...);     // sbk_api.cu: fills the thread-local error text
-
-#define PCU(x)                                                                                              \
-    do {                                                                                                    \
-        cudaError_t e_ = (x);                                                                               \
-        if (e_ != cudaSuccess)                                                                              \
-            return sbk_set_error(SBK_ERR_CUDA, "%s failed: %s (%s:%d)", #x, cudaGetErrorString(e_), __FILE__, __LINE__); \
-    } while (0)
 
 namespace {
 
@@ -82,44 +72,49 @@ __global__ void k_pn_final(const float* y, const float* w, const float* bias, fl
     }
 }
 
-int pn_grid(long long n) {
-    const long long g = (n + 255) / 256, cap = 16LL * device_sm_count();
-    return (int)(g < 1 ? 1 : (g > cap ? cap : g));
+// The workspace of one (B, n_feats, T): a0 (+ a0_lo), raw (raw1, then raw2), act (act1, then the res conv's output y)
+// (+ act_lo), and the two blocks' [B][8][2] fp64 GroupNorm statistics.  Over a null-base arena only the size is computed.
+struct PnBufs { float *a0, *raw, *act, *a0_lo, *act_lo; double* st; };
+size_t pn_carve(int B, int H, int C, int T, bool x3, Arena& ar, PnBufs* o) {
+    const size_t big = (size_t)B * H * C * T * sizeof(float);
+    PnBufs b;
+    b.a0 = (float*)ar.take(big);
+    b.raw = (float*)ar.take(big);
+    b.act = (float*)ar.take(big);
+    b.a0_lo = x3 ? (float*)ar.take(big) : nullptr;
+    b.act_lo = x3 ? (float*)ar.take(big) : nullptr;
+    b.st = (double*)ar.take(2 * (size_t)B * kGroups * 2 * sizeof(double));
+    if (o) *o = b;
+    return ar.bytes();
 }
-
-// the precision mapping of the PostNet handle: the fp32-class modes run the fp32x3 path, tf32 and bf16 the tf32 path
-// (bf16 operands are not implemented for the 7x7 geometry)
-bool pn_x3(int precision) { return precision == SBK_PREC_FP32X3 || precision == SBK_PREC_FP32; }
-
-struct PWSpec { std::string name; std::vector<int64_t> shape; };
 
 }  // namespace
 
 struct sbk_postnet {
+    // precision: the fp32-class modes run the fp32x3 path (prec_runs_x3), tf32 and bf16 the tf32 path (bf16 operands are not
+    // implemented for the 7x7 geometry)
     sbk_postnet_config cfg;
-    std::vector<PWSpec> spec;
-    std::map<std::string, float*> raw;       // device copies, reference layout
-    std::map<std::string, void*> packed;     // tensor-core stage images
+    WeightSet w;                             // raw: reference layout; packed: tensor-core stage images
     float* zero = nullptr;                   // zero page: A-tile borders, and k_gn_act's (absent) time bias
-    void* mem = nullptr; size_t cap = 0;     // grow-only workspace
+    Workspace ws;
     bool is_packed = false;
     int64_t last_launches = 0;
 };
 
 extern "C" int sbk_postnet_create(const sbk_postnet_config* cfg, sbk_postnet** out) {
-    if (!cfg || !out) return sbk_set_error(SBK_ERR_ARG, "sbk_postnet_create: null argument");
+    if (!cfg || !out) return fail(SBK_ERR_ARG, "sbk_postnet_create: null argument");
     if (cfg->groups != kGroups)
-        return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_postnet_create: groups = %d; the GroupNorm kernels are built for %d groups", cfg->groups, kGroups);
+        return fail(SBK_ERR_UNSUPPORTED, "sbk_postnet_create: groups = %d; the GroupNorm kernels are built for %d groups", cfg->groups, kGroups);
     // the conv epilogue reduces GroupNorm partials per 32-channel block: a group must be 8 or 16 channels wide (dim 64, 128)
     // or a whole number of blocks (dim a multiple of 256); channels come in 64-wide N tiles
     const int d = cfg->dim;
     if (d <= 0 || d % 64 != 0 || (d > 128 && d % 256 != 0))
-        return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_postnet_create: dim = %d; supported: 64, 128 and multiples of 256", d);
+        return fail(SBK_ERR_UNSUPPORTED, "sbk_postnet_create: dim = %d; supported: 64, 128 and multiples of 256", d);
     if (cfg->precision < SBK_PREC_FP32 || cfg->precision > SBK_PREC_FP32X3)
-        return sbk_set_error(SBK_ERR_ARG, "sbk_postnet_create: unknown precision %d", cfg->precision);
+        return fail(SBK_ERR_ARG, "sbk_postnet_create: unknown precision %d", cfg->precision);
     sbk_postnet* p = new sbk_postnet();
     p->cfg = *cfg;
-    auto add = [&](const std::string& n, std::vector<int64_t> s) { p->spec.push_back({n, s}); };
+    auto add = [&](const std::string& n, std::vector<int64_t> s) { p->w.add(n, std::move(s)); };
     add("init_conv.weight", {d, 1, 1, 1}); add("init_conv.bias", {d});
     for (const char* blk : {"block1", "block2"}) {
         const std::string q = std::string("res_block.") + blk + ".block.";
@@ -134,120 +129,88 @@ extern "C" int sbk_postnet_create(const sbk_postnet_config* cfg, sbk_postnet** o
 
 extern "C" void sbk_postnet_destroy(sbk_postnet* p) {
     if (!p) return;
-    for (auto& kv : p->raw) cudaFree(kv.second);
-    for (auto& kv : p->packed) cudaFree(kv.second);
     if (p->zero) cudaFree(p->zero);
-    if (p->mem) cudaFree(p->mem);
     delete p;
 }
 
-extern "C" int sbk_postnet_num_weights(const sbk_postnet* p) { return p ? (int)p->spec.size() : 0; }
-extern "C" const char* sbk_postnet_weight_name(const sbk_postnet* p, int i) {
-    if (!p || i < 0 || i >= (int)p->spec.size()) return nullptr;
-    return p->spec[i].name.c_str();
-}
+extern "C" int sbk_postnet_num_weights(const sbk_postnet* p) { return p ? p->w.count() : 0; }
+extern "C" const char* sbk_postnet_weight_name(const sbk_postnet* p, int i) { return p ? p->w.name(i) : nullptr; }
 
 extern "C" int sbk_postnet_set_weight(sbk_postnet* p, const char* name, const void* data, const int64_t* shape, int ndim) {
-    if (!p || !name || !data || !shape) return sbk_set_error(SBK_ERR_ARG, "sbk_postnet_set_weight: null argument");
-    const PWSpec* ws = nullptr;
-    for (auto& s : p->spec) if (s.name == name) { ws = &s; break; }
-    if (!ws) return sbk_set_error(SBK_ERR_ARG, "sbk_postnet_set_weight: unexpected key '%s' (strict)", name);
-    if ((int)ws->shape.size() != ndim) return sbk_set_error(SBK_ERR_ARG, "sbk_postnet_set_weight: '%s' rank %d, expected %d", name, ndim, (int)ws->shape.size());
-    size_t numel = 1;
-    for (int i = 0; i < ndim; ++i) {
-        if (ws->shape[i] != shape[i]) return sbk_set_error(SBK_ERR_ARG, "sbk_postnet_set_weight: '%s' dim %d is %lld, expected %lld", name, i, (long long)shape[i], (long long)ws->shape[i]);
-        numel *= (size_t)shape[i];
-    }
-    PCU(cudaSetDevice(p->cfg.device));
-    float*& dst = p->raw[name];
-    if (!dst) PCU(cudaMalloc(&dst, numel * sizeof(float)));
-    PCU(cudaMemcpy(dst, data, numel * sizeof(float), cudaMemcpyDefault));
+    if (!p || !name || !data || !shape) return fail(SBK_ERR_ARG, "sbk_postnet_set_weight: null argument");
+    TRY(p->w.set(name, data, shape, ndim, p->cfg.device, "sbk_postnet_set_weight"));
     p->is_packed = false;
     return SBK_OK;
 }
 
-static int pn_pack(sbk_postnet* p, const std::string& name, int geom, int taps) {
+static int pn_pack(sbk_postnet* p, const std::string& name, int geom) {
     const int d = p->cfg.dim;
-    std::vector<float> w((size_t)d * d * taps);
-    PCU(cudaMemcpy(w.data(), p->raw[name], w.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    const bool x3 = pn_x3(p->cfg.precision);
+    std::vector<float> w;
+    TRY(p->w.fetch(name, w));
+    const bool x3 = prec_runs_x3(p->cfg.precision);
     std::vector<uint8_t> img(conv_tc_pack_image(w.data(), d, d, geom, false, x3, 0, nullptr));
     conv_tc_pack_image(w.data(), d, d, geom, false, x3, 0, img.data());
-    void*& dst = p->packed[name];
-    if (!dst) PCU(cudaMalloc(&dst, img.size()));
-    PCU(cudaMemcpy(dst, img.data(), img.size(), cudaMemcpyHostToDevice));
-    return SBK_OK;
+    return upload(p->w.packed, name, img.size(), img.data());
 }
 
 extern "C" int sbk_postnet_pack(sbk_postnet* p) {
-    if (!p) return sbk_set_error(SBK_ERR_ARG, "sbk_postnet_pack: null handle");
-    for (auto& s : p->spec) if (!p->raw.count(s.name)) return sbk_set_error(SBK_ERR_STATE, "sbk_postnet_pack: missing key '%s' (strict)", s.name.c_str());
-    PCU(cudaSetDevice(p->cfg.device));
-    int rc;
-    if ((rc = pn_pack(p, "res_block.block1.block.0.weight", G_C7, 49)) != SBK_OK) return rc;
-    if ((rc = pn_pack(p, "res_block.block2.block.0.weight", G_C7, 49)) != SBK_OK) return rc;
-    if ((rc = pn_pack(p, "res_block.res.weight", G_PW, 1)) != SBK_OK) return rc;
-    if (!p->zero) { PCU(cudaMalloc(&p->zero, 8192)); PCU(cudaMemset(p->zero, 0, 8192)); }
+    if (!p) return fail(SBK_ERR_ARG, "sbk_postnet_pack: null handle");
+    TRY(p->w.require_all("sbk_postnet_pack"));
+    CU(cudaSetDevice(p->cfg.device));
+    TRY(pn_pack(p, "res_block.block1.block.0.weight", G_C7));
+    TRY(pn_pack(p, "res_block.block2.block.0.weight", G_C7));
+    TRY(pn_pack(p, "res_block.res.weight", G_PW));
+    if (!p->zero) { CU(cudaMalloc(&p->zero, 8192)); CU(cudaMemset(p->zero, 0, 8192)); }
     p->is_packed = true;
     return SBK_OK;
 }
 
-// a0 (+ a0_lo), raw (raw1, then raw2), act (act1, then the res conv's output y) (+ act_lo), 2 x [B][8][2] fp64 statistics
 extern "C" size_t sbk_postnet_workspace_bytes(const sbk_postnet* p, int B, int n_feats, int T) {
     if (!p || B <= 0 || n_feats <= 0 || T <= 0) return 0;
-    const size_t big = (size_t)B * n_feats * p->cfg.dim * T * sizeof(float) + 256;
-    return big * (pn_x3(p->cfg.precision) ? 5 : 3) + 2 * (size_t)B * kGroups * 2 * sizeof(double) + 256;
+    Arena probe;
+    return pn_carve(B, n_feats, p->cfg.dim, T, prec_runs_x3(p->cfg.precision), probe, nullptr);
 }
 
 extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* mask, float* out, int B, int n_feats, int T, void* stream) {
-    if (!p || !x || !mask || !out) return sbk_set_error(SBK_ERR_ARG, "sbk_postnet_forward: null argument");
-    if (!p->is_packed) return sbk_set_error(SBK_ERR_STATE, "sbk_postnet_forward: weights not packed (sbk_postnet_set_weight for every key, then sbk_postnet_pack)");
-    if (B <= 0 || n_feats <= 0 || T <= 0) return sbk_set_error(SBK_ERR_ARG, "sbk_postnet_forward: B, n_feats and T must be positive (got %d, %d, %d)", B, n_feats, T);
-    PCU(cudaSetDevice(p->cfg.device));
+    if (!p || !x || !mask || !out) return fail(SBK_ERR_ARG, "sbk_postnet_forward: null argument");
+    if (!p->is_packed) return fail(SBK_ERR_STATE, "sbk_postnet_forward: weights not packed (sbk_postnet_set_weight for every key, then sbk_postnet_pack)");
+    if (B <= 0 || n_feats <= 0 || T <= 0) return fail(SBK_ERR_ARG, "sbk_postnet_forward: B, n_feats and T must be positive (got %d, %d, %d)", B, n_feats, T);
+    CU(cudaSetDevice(p->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
     const int C = p->cfg.dim, H = n_feats;
-    const bool x3 = pn_x3(p->cfg.precision);
+    const bool x3 = prec_runs_x3(p->cfg.precision);
     const size_t need = sbk_postnet_workspace_bytes(p, B, n_feats, T);
-    if (need > p->cap) {
-        if (p->mem) { PCU(cudaFree(p->mem)); p->mem = nullptr; p->cap = 0; }
-        const cudaError_t e = cudaMalloc(&p->mem, need);
-        if (e != cudaSuccess) { p->mem = nullptr; cudaGetLastError(); return sbk_set_error(SBK_ERR_CUDA, "out of memory: the PostNet workspace for (B=%d, n_feats=%d, T=%d) needs %zu bytes", B, n_feats, T, need); }
-        p->cap = need;
-    }
-    char* base = (char*)p->mem; size_t off = 0;
-    auto take = [&](size_t bytes) { off = (off + 255) & ~size_t(255); void* r = base + off; off += bytes; return r; };
-    const size_t big = (size_t)B * H * C * T * sizeof(float);
-    float* a0 = (float*)take(big);
-    float* raw = (float*)take(big);
-    float* act = (float*)take(big);
-    float* a0_lo = x3 ? (float*)take(big) : nullptr;
-    float* act_lo = x3 ? (float*)take(big) : nullptr;
-    double* st = (double*)take(2 * (size_t)B * kGroups * 2 * sizeof(double));
+    if (p->ws.reserve(need)) return fail(SBK_ERR_CUDA, "out of memory: the PostNet workspace for (B=%d, n_feats=%d, T=%d) needs %zu bytes", B, n_feats, T, need);
+    PnBufs wb;
+    Arena ar = p->ws.arena();
+    pn_carve(B, H, C, T, x3, ar, &wb);
+    float *a0 = wb.a0, *raw = wb.raw, *act = wb.act, *a0_lo = wb.a0_lo, *act_lo = wb.act_lo;
+    double* st = wb.st;
     double* st1 = st; double* st2 = st + (size_t)B * kGroups * 2;
-    auto R = [&](const char* k) -> const float* { return p->raw[k]; };
+    auto R = [&](const std::string& k) { return p->w.get(k); };
     const float inv_count = (float)(1.0 / ((double)(C / kGroups) * H * T));
     int64_t n = 0;
     auto refused = [&](const char* what) {
-        return sbk_set_error(SBK_ERR_CUDA, "sbk_postnet_forward: the %s launch was refused (device attribute / geometry)", what);
+        return fail(SBK_ERR_CUDA, "sbk_postnet_forward: the %s launch was refused (device attribute / geometry)", what);
     };
     int k;
 
-    PCU(cudaMemsetAsync(st, 0, 2 * (size_t)B * kGroups * 2 * sizeof(double), s)); ++n;
-    k_pn_init<<<pn_grid((long long)B * H * (C / 4) * T), 256, 0, s>>>(x, mask, R("init_conv.weight"), R("init_conv.bias"), a0, a0_lo,
+    CU(cudaMemsetAsync(st, 0, 2 * (size_t)B * kGroups * 2 * sizeof(double), s)); ++n;
+    k_pn_init<<<ew_grid((long long)B * H * (C / 4) * T), 256, 0, s>>>(x, mask, R("init_conv.weight"), R("init_conv.bias"), a0, a0_lo,
                                                                       B, H, C, T, x3 ? 0 : 1);
     ++n;
     auto conv7 = [&](const char* blk, const float* in, const float* in_lo, double* ost) {
         ConvTcParams cp; memset(&cp, 0, sizeof(cp));
         const std::string q = std::string("res_block.") + blk + ".block.0.";
         cp.geom = G_C7; cp.in0 = in; cp.c0 = C; cp.H = H; cp.W = T; cp.B = B; cp.Ho = H; cp.Wo = T;
-        cp.wpk = p->packed[q + "weight"]; cp.bias = p->raw[q + "bias"]; cp.out = raw; cp.Cout = C; cp.epi = EPI_PLAIN;
+        cp.wpk = R(q + "weight"); cp.bias = R(q + "bias"); cp.out = raw; cp.Cout = C; cp.epi = EPI_PLAIN;
         cp.ostats = ost; cp.mask = mask; cp.T = T; cp.zero_page = p->zero;
         if (x3) { cp.x3 = 1; cp.in0_lo = in_lo; }
         return launch_conv_tc(cp, s);
     };
     auto gnref = [&](double* stp, const char* blk) {
         const std::string q = std::string("res_block.") + blk + ".block.1.";
-        GnRef g; g.stats = stp; g.gamma = p->raw[q + "weight"]; g.beta = p->raw[q + "bias"]; g.inv_count = inv_count;
+        GnRef g; g.stats = stp; g.gamma = R(q + "weight"); g.beta = R(q + "bias"); g.inv_count = inv_count;
         return g;
     };
     if ((k = conv7("block1", a0, a0_lo, st1)) < 0) return refused("block1 conv");
@@ -265,16 +228,16 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
     {
         ConvTcParams cp; memset(&cp, 0, sizeof(cp));
         cp.geom = G_PW; cp.in0 = a0; cp.c0 = C; cp.H = H; cp.W = T; cp.B = B; cp.Ho = H; cp.Wo = T;
-        cp.wpk = p->packed["res_block.res.weight"]; cp.bias = R("res_block.res.bias"); cp.out = act; cp.Cout = C;
+        cp.wpk = R("res_block.res.weight"); cp.bias = R("res_block.res.bias"); cp.out = act; cp.Cout = C;
         cp.epi = EPI_RES; cp.rraw = raw; cp.rgn = gnref(st2, "block2"); cp.out_mask = 1;
         cp.mask = mask; cp.T = T; cp.zero_page = p->zero;
         if (x3) { cp.x3 = 1; cp.in0_lo = a0_lo; }
         if ((k = launch_conv_tc(cp, s)) < 0) return refused("residual conv");
         n += k;
     }
-    k_pn_final<<<pn_grid((long long)B * H * T), 256, 0, s>>>(act, R("final_conv.weight"), R("final_conv.bias"), out, B, H, C, T);
+    k_pn_final<<<ew_grid((long long)B * H * T), 256, 0, s>>>(act, R("final_conv.weight"), R("final_conv.bias"), out, B, H, C, T);
     ++n;
-    PCU(cudaGetLastError());
+    CU(cudaGetLastError());
     p->last_launches = n;
     return SBK_OK;
 }

@@ -17,8 +17,7 @@
 // k_te_attn: one warp per (utterance, head, query): scores over all keys with the windowed relative-position logits
 // q_i.E_k[j-i+w] added for |j-i| <= w (:151-157 restated directly instead of through the pad/reshape skewing), the
 // reference's masked_fill(-1e4), softmax, p.V plus the relative-value term sum_j p_ij E_v[j-i+w] (:164-169).
-#include "../../include/sbk.h"
-#include "sbk_internal.h"
+#include "sbk_host.h"
 
 #include <math.h>
 #include <stdio.h>
@@ -29,14 +28,7 @@
 #include <string>
 #include <vector>
 
-int sbk_set_error(int code, const char* fmt, ...);
-
-#define TCU(x)                                                                                              \
-    do {                                                                                                    \
-        cudaError_t e_ = (x);                                                                               \
-        if (e_ != cudaSuccess)                                                                              \
-            return sbk_set_error(SBK_ERR_CUDA, "%s failed: %s (%s:%d)", #x, cudaGetErrorString(e_), __FILE__, __LINE__); \
-    } while (0)
+using namespace sbk;
 
 namespace {
 
@@ -252,35 +244,32 @@ __global__ void k_te_concat_spk(const float* h, const float* spk, float* out, in
     }
 }
 
-struct TWSpec { std::string name; std::vector<int64_t> shape; };
-
 }  // namespace
 
 struct sbk_textenc {
     sbk_textenc_config cfg;
-    std::vector<TWSpec> spec;
-    std::map<std::string, float*> raw, packed;
-    void* mem = nullptr; size_t cap = 0;
+    WeightSet w;
+    Workspace ws;
     bool is_packed = false;
     int64_t last_launches = 0;
     int enc_ch() const { return cfg.n_channels + (cfg.n_spks > 1 ? cfg.spk_emb_dim : 0); }
 };
 
 extern "C" int sbk_textenc_create(const sbk_textenc_config* cfg, sbk_textenc** out) {
-    if (!cfg || !out) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_create: null argument");
+    if (!cfg || !out) return fail(SBK_ERR_ARG, "sbk_textenc_create: null argument");
     const int C = cfg->n_channels, Ce = C + (cfg->n_spks > 1 ? cfg->spk_emb_dim : 0);
-    if (C <= 0 || C % 4 != 0 || Ce % 4 != 0) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_create: channel counts must be multiples of 4");
-    if (cfg->n_heads <= 0 || Ce % cfg->n_heads != 0 || (Ce / cfg->n_heads) % 4 != 0) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_create: channels / heads must be a multiple of 4");
+    if (C <= 0 || C % 4 != 0 || Ce % 4 != 0) return fail(SBK_ERR_ARG, "sbk_textenc_create: channel counts must be multiples of 4");
+    if (cfg->n_heads <= 0 || Ce % cfg->n_heads != 0 || (Ce / cfg->n_heads) % 4 != 0) return fail(SBK_ERR_ARG, "sbk_textenc_create: channels / heads must be a multiple of 4");
     if (3 * Ce > 256 * TE_MAXCO || cfg->filter_channels > 256 * TE_MAXCO || cfg->filter_channels_dp > 256 * TE_MAXCO || cfg->n_feats > 256 * TE_MAXCO)
-        return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_textenc_create: at most %d output channels per conv", 256 * TE_MAXCO);
-    if (cfg->kernel_size < 1 || cfg->kernel_size % 2 == 0 || cfg->kernel_size > 9) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_create: kernel_size must be odd and <= 9");
-    if (cfg->window_size < 1 || cfg->window_size > 15) return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_textenc_create: window_size must be in 1..15 (relative-position attention)");
+        return fail(SBK_ERR_UNSUPPORTED, "sbk_textenc_create: at most %d output channels per conv", 256 * TE_MAXCO);
+    if (cfg->kernel_size < 1 || cfg->kernel_size % 2 == 0 || cfg->kernel_size > 9) return fail(SBK_ERR_ARG, "sbk_textenc_create: kernel_size must be odd and <= 9");
+    if (cfg->window_size < 1 || cfg->window_size > 15) return fail(SBK_ERR_UNSUPPORTED, "sbk_textenc_create: window_size must be in 1..15 (relative-position attention)");
     sbk_textenc* e = new sbk_textenc();
     e->cfg = *cfg;
-    auto add = [&](const std::string& n, std::vector<int64_t> s) { e->spec.push_back({n, s}); };
+    auto add = [&](const std::string& n, std::vector<int64_t> s) { e->w.add(n, std::move(s)); };
     const int F = cfg->filter_channels, Fd = cfg->filter_channels_dp, K = cfg->kernel_size, d = Ce / cfg->n_heads, nrel = 2 * cfg->window_size + 1;
     const bool mel = cfg->kind == 1;         // DiffVC MelEncoder (DiffVC/model/encoder.py:257-284): init_proj | prenet | encoder | term_proj
-    if (mel && cfg->n_spks > 1) { delete e; return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_create: the mel encoder has no speaker input"); }
+    if (mel && cfg->n_spks > 1) { delete e; return fail(SBK_ERR_ARG, "sbk_textenc_create: the mel encoder has no speaker input"); }
     if (mel) { add("init_proj.weight", {C, cfg->n_feats, 1}); add("init_proj.bias", {C}); }
     else add("emb.weight", {cfg->n_vocab, C});
     for (int i = 0; i < 3; ++i) {
@@ -313,33 +302,14 @@ extern "C" int sbk_textenc_create(const sbk_textenc_config* cfg, sbk_textenc** o
 }
 
 extern "C" void sbk_textenc_destroy(sbk_textenc* e) {
-    if (!e) return;
-    for (auto& kv : e->raw) cudaFree(kv.second);
-    for (auto& kv : e->packed) cudaFree(kv.second);
-    if (e->mem) cudaFree(e->mem);
     delete e;
 }
-extern "C" int sbk_textenc_num_weights(const sbk_textenc* e) { return e ? (int)e->spec.size() : 0; }
-extern "C" const char* sbk_textenc_weight_name(const sbk_textenc* e, int i) {
-    if (!e || i < 0 || i >= (int)e->spec.size()) return nullptr;
-    return e->spec[i].name.c_str();
-}
+extern "C" int sbk_textenc_num_weights(const sbk_textenc* e) { return e ? e->w.count() : 0; }
+extern "C" const char* sbk_textenc_weight_name(const sbk_textenc* e, int i) { return e ? e->w.name(i) : nullptr; }
 
 extern "C" int sbk_textenc_set_weight(sbk_textenc* e, const char* name, const void* data, const int64_t* shape, int ndim) {
-    if (!e || !name || !data || !shape) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_set_weight: null argument");
-    const TWSpec* ws = nullptr;
-    for (auto& s : e->spec) if (s.name == name) { ws = &s; break; }
-    if (!ws) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_set_weight: unexpected key '%s' (strict)", name);
-    if ((int)ws->shape.size() != ndim) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_set_weight: '%s' rank %d, expected %d", name, ndim, (int)ws->shape.size());
-    size_t numel = 1;
-    for (int i = 0; i < ndim; ++i) {
-        if (ws->shape[i] != shape[i]) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_set_weight: '%s' dim %d is %lld, expected %lld", name, i, (long long)shape[i], (long long)ws->shape[i]);
-        numel *= (size_t)shape[i];
-    }
-    TCU(cudaSetDevice(e->cfg.device));
-    float*& dst = e->raw[name];
-    if (!dst) TCU(cudaMalloc(&dst, numel * sizeof(float)));
-    TCU(cudaMemcpy(dst, data, numel * sizeof(float), cudaMemcpyDefault));
+    if (!e || !name || !data || !shape) return fail(SBK_ERR_ARG, "sbk_textenc_set_weight: null argument");
+    TRY(e->w.set(name, data, shape, ndim, e->cfg.device, "sbk_textenc_set_weight"));
     e->is_packed = false;
     return SBK_OK;
 }
@@ -349,13 +319,10 @@ static int te_pack(sbk_textenc* e, const std::vector<std::string>& srcs, const s
     std::vector<std::vector<float>> ws; std::vector<std::vector<int64_t>> shapes;
     int64_t co_total = 0;
     for (auto& n : srcs) {
-        const TWSpec* s = nullptr;
-        for (auto& q : e->spec) if (q.name == n) { s = &q; break; }
-        if (!s) return sbk_set_error(SBK_ERR_STATE, "te_pack: no spec for %s", n.c_str());
-        size_t numel = 1; for (auto d : s->shape) numel *= (size_t)d;
-        std::vector<float> w(numel);
-        TCU(cudaMemcpy(w.data(), e->raw[n], numel * 4, cudaMemcpyDeviceToHost));
-        ws.push_back(std::move(w)); shapes.push_back(s->shape); co_total += s->shape[0];
+        std::vector<float> w;
+        TRY(e->w.fetch(n, w));
+        const std::vector<int64_t>& shape = e->w.find(n)->shape;
+        ws.push_back(std::move(w)); shapes.push_back(shape); co_total += shape[0];
     }
     std::vector<float> outw;
     if (bias) {
@@ -371,36 +338,31 @@ static int te_pack(sbk_textenc* e, const std::vector<std::string>& srcs, const s
             off += co;
         }
     }
-    float*& d = e->packed[key];
-    if (!d) TCU(cudaMalloc(&d, outw.size() * 4));
-    TCU(cudaMemcpy(d, outw.data(), outw.size() * 4, cudaMemcpyHostToDevice));
-    return SBK_OK;
+    return upload(e->w.packed, key, outw.size() * 4, outw.data());
 }
 
-#define TTRY(x) do { int rc_ = (x); if (rc_ != SBK_OK) return rc_; } while (0)
-
 extern "C" int sbk_textenc_pack(sbk_textenc* e) {
-    if (!e) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_pack: null handle");
-    for (auto& s : e->spec) if (!e->raw.count(s.name)) return sbk_set_error(SBK_ERR_STATE, "sbk_textenc_pack: missing key '%s' (strict)", s.name.c_str());
-    TCU(cudaSetDevice(e->cfg.device));
-    for (int i = 0; i < 3; ++i) TTRY(te_pack(e, {"prenet.conv_layers." + std::to_string(i) + ".weight"}, "prenet.conv" + std::to_string(i), false));
-    TTRY(te_pack(e, {"prenet.proj.weight"}, "prenet.proj", false));
+    if (!e) return fail(SBK_ERR_ARG, "sbk_textenc_pack: null handle");
+    TRY(e->w.require_all("sbk_textenc_pack"));
+    CU(cudaSetDevice(e->cfg.device));
+    for (int i = 0; i < 3; ++i) TRY(te_pack(e, {"prenet.conv_layers." + std::to_string(i) + ".weight"}, "prenet.conv" + std::to_string(i), false));
+    TRY(te_pack(e, {"prenet.proj.weight"}, "prenet.proj", false));
     for (int i = 0; i < e->cfg.n_layers; ++i) {
         const std::string a = "encoder.attn_layers." + std::to_string(i), n = std::to_string(i);
-        TTRY(te_pack(e, {a + ".conv_q.weight", a + ".conv_k.weight", a + ".conv_v.weight"}, a + ".qkv.w", false));
-        TTRY(te_pack(e, {a + ".conv_q.bias", a + ".conv_k.bias", a + ".conv_v.bias"}, a + ".qkv.b", true));
-        TTRY(te_pack(e, {a + ".conv_o.weight"}, a + ".o.w", false));
-        TTRY(te_pack(e, {"encoder.ffn_layers." + n + ".conv_1.weight"}, "ffn" + n + ".1", false));
-        TTRY(te_pack(e, {"encoder.ffn_layers." + n + ".conv_2.weight"}, "ffn" + n + ".2", false));
+        TRY(te_pack(e, {a + ".conv_q.weight", a + ".conv_k.weight", a + ".conv_v.weight"}, a + ".qkv.w", false));
+        TRY(te_pack(e, {a + ".conv_q.bias", a + ".conv_k.bias", a + ".conv_v.bias"}, a + ".qkv.b", true));
+        TRY(te_pack(e, {a + ".conv_o.weight"}, a + ".o.w", false));
+        TRY(te_pack(e, {"encoder.ffn_layers." + n + ".conv_1.weight"}, "ffn" + n + ".1", false));
+        TRY(te_pack(e, {"encoder.ffn_layers." + n + ".conv_2.weight"}, "ffn" + n + ".2", false));
     }
     if (e->cfg.kind == 1) {
-        TTRY(te_pack(e, {"init_proj.weight"}, "init_proj", false));
-        TTRY(te_pack(e, {"term_proj.weight"}, "term_proj", false));
+        TRY(te_pack(e, {"init_proj.weight"}, "init_proj", false));
+        TRY(te_pack(e, {"term_proj.weight"}, "term_proj", false));
     } else {
-        TTRY(te_pack(e, {"proj_m.weight"}, "proj_m", false));
-        TTRY(te_pack(e, {"proj_w.conv_1.weight"}, "dp.1", false));
-        TTRY(te_pack(e, {"proj_w.conv_2.weight"}, "dp.2", false));
-        TTRY(te_pack(e, {"proj_w.proj.weight"}, "dp.p", false));
+        TRY(te_pack(e, {"proj_m.weight"}, "proj_m", false));
+        TRY(te_pack(e, {"proj_w.conv_1.weight"}, "dp.1", false));
+        TRY(te_pack(e, {"proj_w.conv_2.weight"}, "dp.2", false));
+        TRY(te_pack(e, {"proj_w.proj.weight"}, "dp.p", false));
     }
     e->is_packed = true;
     return SBK_OK;
@@ -409,33 +371,34 @@ extern "C" int sbk_textenc_pack(sbk_textenc* e) {
 // shared body of TextEncoder.forward (x, x_lengths given; mel == nullptr) and MelEncoder.forward (mel, mask_in given)
 static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths, const float* spk, const float* mel, const float* mask_in,
                       float* mu_x, float* logw, float* x_mask, int B, int Tx, void* stream) {
-    if (!e->is_packed) return sbk_set_error(SBK_ERR_STATE, "sbk_textenc_forward: weights not packed");
-    if (B <= 0 || Tx <= 0) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_forward: B and Tx must be positive");
+    if (!e->is_packed) return fail(SBK_ERR_STATE, "sbk_textenc_forward: weights not packed");
+    if (B <= 0 || Tx <= 0) return fail(SBK_ERR_ARG, "sbk_textenc_forward: B and Tx must be positive");
     const sbk_textenc_config& c = e->cfg;
-    if (c.n_spks > 1 && !spk) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_forward: spk is required when n_spks > 1");
-    TCU(cudaSetDevice(c.device));
+    if (c.n_spks > 1 && !spk) return fail(SBK_ERR_ARG, "sbk_textenc_forward: spk is required when n_spks > 1");
+    CU(cudaSetDevice(c.device));
     cudaStream_t s = (cudaStream_t)stream;
     const int C = c.n_channels, Ce = e->enc_ch(), F = c.filter_channels, Fd = c.filter_channels_dp, K = c.kernel_size;
     const size_t ntok = (size_t)B * Tx;
     const size_t wide = (size_t)std::max(std::max(3 * Ce, F), Fd);
-    const size_t need = (ntok * (3 * (size_t)Ce + 2 * wide) + 64) * sizeof(float) + 8 * 256;
-    if (need > e->cap) {
-        if (e->mem) { cudaFree(e->mem); e->mem = nullptr; e->cap = 0; }
-        if (cudaMalloc(&e->mem, need) != cudaSuccess) { e->mem = nullptr; cudaGetLastError(); return sbk_set_error(SBK_ERR_CUDA, "out of memory: text-encoder workspace %zu bytes", need); }
-        e->cap = need;
-    }
-    char* base = (char*)e->mem; size_t off = 0;
-    auto take = [&](size_t floats) { off = (off + 255) & ~size_t(255); float* r = (float*)(base + off); off += floats * sizeof(float); return r; };
-    float *h0 = take(ntok * Ce), *h1 = take(ntok * Ce), *h2 = take(ntok * Ce), *wa = take(ntok * wide), *wb = take(ntok * wide);
-    auto W = [&](const std::string& k) -> const float* { auto it = e->packed.find(k); if (it != e->packed.end()) return it->second; auto i2 = e->raw.find(k); return i2 != e->raw.end() ? i2->second : nullptr; };
+    // three token-major [B][Tx][Ce] activations and two [B][Tx][wide] scratch buffers (q|k|v, the hidden layers)
+    float *h0, *h1, *h2, *wa, *wb;
+    auto carve = [&](Arena& ar) {
+        auto take = [&](size_t floats) { return (float*)ar.take(floats * sizeof(float)); };
+        h0 = take(ntok * Ce); h1 = take(ntok * Ce); h2 = take(ntok * Ce); wa = take(ntok * wide); wb = take(ntok * wide);
+    };
+    Arena probe;
+    carve(probe);
+    if (e->ws.reserve(probe.bytes())) return fail(SBK_ERR_CUDA, "out of memory: text-encoder workspace %zu bytes", probe.bytes());
+    Arena ar = e->ws.arena();
+    carve(ar);
     int64_t n = 0;
     auto conv = [&](const float* in, int Cin, const float* spk_in, int E, const std::string& wkey, const std::string& bkey, int Kk, int Cout,
                     int in_mask, int relu1, int mask1, const float* res, int res_mask, const std::string& ln, int relu2, int mask2,
                     float* out, int planar, int in_planar = 0) {
         TeConvParams p; memset(&p, 0, sizeof(p));
-        p.in = in; p.Cin = Cin; p.in_planar = in_planar; p.spk = spk_in; p.E = E; p.w = W(wkey); p.bias = W(bkey); p.K = Kk; p.Cout = Cout; p.B = B; p.T = Tx;
+        p.in = in; p.Cin = Cin; p.in_planar = in_planar; p.spk = spk_in; p.E = E; p.w = e->w.get(wkey); p.bias = e->w.get(bkey); p.K = Kk; p.Cout = Cout; p.B = B; p.T = Tx;
         p.mask = x_mask; p.in_mask = in_mask; p.relu1 = relu1; p.mask1 = mask1; p.res = res; p.res_mask = res_mask;
-        if (!ln.empty()) { p.ln_g = W(ln + ".gamma"); p.ln_b = W(ln + ".beta"); }
+        if (!ln.empty()) { p.ln_g = e->w.get(ln + ".gamma"); p.ln_b = e->w.get(ln + ".beta"); }
         p.relu2 = relu2; p.mask2 = mask2; p.out = out; p.out_planar = planar;
         const size_t smem = sizeof(float) * std::max((size_t)(TE_TOK + Kk - 1) * (Cin + E), (size_t)TE_TOK * Cout);
         k_te_conv<<<dim3((Tx + TE_TOK - 1) / TE_TOK, B), 256, smem, s>>>(p);
@@ -443,8 +406,8 @@ static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths
     };
     static bool attr_done[64] = {};
     if (c.device >= 0 && c.device < 64 && !attr_done[c.device]) {
-        TCU(cudaFuncSetAttribute(k_te_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        TCU(cudaFuncSetAttribute(k_te_attn, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        CU(cudaFuncSetAttribute(k_te_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        CU(cudaFuncSetAttribute(k_te_attn, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         attr_done[c.device] = true;
     }
     if (mel) {
@@ -453,7 +416,7 @@ static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths
         conv(mel, c.n_feats, nullptr, 0, "init_proj", "init_proj.bias", 1, C, 1, 0, 0, nullptr, 0, "", 0, 0, h0, 0, 1);
     } else {
         k_te_mask<<<(B * Tx + 255) / 256, 256, 0, s>>>(reinterpret_cast<const long long*>(x_lengths), x_mask, B, Tx); ++n;
-        k_te_embed<<<(int)std::min<size_t>((ntok * (C / 4) + 255) / 256, 8 * (size_t)sbk::device_sm_count()), 256, 0, s>>>(reinterpret_cast<const long long*>(x), W("emb.weight"), h0, (int)ntok, C, c.n_vocab, sqrtf((float)C)); ++n;
+        k_te_embed<<<(int)std::min<size_t>((ntok * (C / 4) + 255) / 256, 8 * (size_t)sbk::device_sm_count()), 256, 0, s>>>(reinterpret_cast<const long long*>(x), e->w.get("emb.weight"), h0, (int)ntok, C, c.n_vocab, sqrtf((float)C)); ++n;
     }
     // ---- prenet (ConvReluNorm, :57-64): x = relu(LN(conv5(x * mask))) x3; x = (x_org + proj(x)) * mask
     const float* cur = h0; float* pp[2] = {h1, h2};
@@ -467,10 +430,9 @@ static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths
     // (multi-speaker: the speaker embedding is concatenated to every token after the prenet, :317-318)
     float* h = hx;
     if (c.n_spks > 1) {
-        float* hc = (hx == h1) ? h2 : h1;
         // h0 is free now but sized for Ce as well: concatenate into it
         k_te_concat_spk<<<(int)std::min<size_t>((ntok * Ce + 255) / 256, 8 * (size_t)sbk::device_sm_count()), 256, 0, s>>>(hx, spk, h0, B, Tx, C, c.spk_emb_dim); ++n;
-        h = h0; (void)hc;
+        h = h0;
     }
     float* other[2];
     { int k = 0; for (float* q : {h0, h1, h2}) if (q != h && k < 2) other[k++] = q; }
@@ -480,8 +442,8 @@ static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths
         const std::string a = "encoder.attn_layers." + std::to_string(i), nn = std::to_string(i);
         conv(h, Ce, nullptr, 0, a + ".qkv.w", a + ".qkv.b", 1, 3 * Ce, 1, 0, 0, nullptr, 0, "", 0, 0, wa, 0);          // x = x * mask; q|k|v
         const size_t asm_ = (size_t)8 * (d + ((Tx + 3) & ~3) + 32) * sizeof(float);
-        if (asm_ > 200 * 1024) return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_textenc_forward: Tx = %d tokens exceeds the attention kernel's shared-memory budget", Tx);
-        k_te_attn<<<dim3((Tx + 7) / 8, c.n_heads, B), 256, asm_, s>>>(wa, x_mask, W(a + ".emb_rel_k"), W(a + ".emb_rel_v"), wb, B, Tx, Ce, c.n_heads, c.window_size); ++n;
+        if (asm_ > 200 * 1024) return fail(SBK_ERR_UNSUPPORTED, "sbk_textenc_forward: Tx = %d tokens exceeds the attention kernel's shared-memory budget", Tx);
+        k_te_attn<<<dim3((Tx + 7) / 8, c.n_heads, B), 256, asm_, s>>>(wa, x_mask, e->w.get(a + ".emb_rel_k"), e->w.get(a + ".emb_rel_v"), wb, B, Tx, Ce, c.n_heads, c.window_size); ++n;
         conv(wb, Ce, nullptr, 0, a + ".o.w", a + ".conv_o.bias", 1, Ce, 0, 0, 0, h, 1, "encoder.norm_layers_1." + nn, 0, 0, other[0], 0);   // LN(x*mask + attn)
         conv(other[0], Ce, nullptr, 0, "ffn" + nn + ".1", "encoder.ffn_layers." + nn + ".conv_1.bias", K, F, 1, 1, 1, nullptr, 0, "", 0, 0, wa, 0);
         conv(wa, F, nullptr, 0, "ffn" + nn + ".2", "encoder.ffn_layers." + nn + ".conv_2.bias", K, Ce, 0, 0, 1, other[0], 0, "encoder.norm_layers_2." + nn, 0, 0, other[1], 0);
@@ -490,7 +452,7 @@ static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths
     if (mel) {
         // x = term_proj(x * x_mask): no output mask (DiffVC/model/encoder.py:283)
         conv(h, Ce, nullptr, 0, "term_proj", "term_proj.bias", 1, c.n_feats, 1, 0, 0, nullptr, 0, "", 0, 0, mu_x, 1);
-        TCU(cudaGetLastError());
+        CU(cudaGetLastError());
         e->last_launches = n;
         return SBK_OK;
     }
@@ -499,22 +461,22 @@ static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths
     conv(h, Ce, nullptr, 0, "dp.1", "proj_w.conv_1.bias", K, Fd, 1, 1, 0, nullptr, 0, "proj_w.norm_1", 0, 0, wa, 0);
     conv(wa, Fd, nullptr, 0, "dp.2", "proj_w.conv_2.bias", K, Fd, 1, 1, 0, nullptr, 0, "proj_w.norm_2", 0, 0, wb, 0);
     conv(wb, Fd, nullptr, 0, "dp.p", "proj_w.proj.bias", 1, 1, 1, 0, 0, nullptr, 0, "", 0, 1, logw, 1);
-    TCU(cudaGetLastError());
+    CU(cudaGetLastError());
     e->last_launches = n;
     return SBK_OK;
 }
 
 extern "C" int sbk_textenc_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths, const float* spk,
                                    float* mu_x, float* logw, float* x_mask, int B, int Tx, void* stream) {
-    if (!e || !x || !x_lengths || !mu_x || !logw || !x_mask) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_forward: null argument");
-    if (e->cfg.kind != 0) return sbk_set_error(SBK_ERR_ARG, "sbk_textenc_forward: this handle is a mel encoder, use sbk_melenc_forward");
+    if (!e || !x || !x_lengths || !mu_x || !logw || !x_mask) return fail(SBK_ERR_ARG, "sbk_textenc_forward: null argument");
+    if (e->cfg.kind != 0) return fail(SBK_ERR_ARG, "sbk_textenc_forward: this handle is a mel encoder, use sbk_melenc_forward");
     return te_forward(e, x, x_lengths, spk, nullptr, nullptr, mu_x, logw, x_mask, B, Tx, stream);
 }
 
 // MelEncoder.forward(x, x_mask) (DiffVC/model/encoder.py:279-284): x [B,n_feats,T], x_mask [B,1,T] -> out [B,n_feats,T]
 extern "C" int sbk_melenc_forward(sbk_textenc* e, const float* x, const float* x_mask, float* out, int B, int T, void* stream) {
-    if (!e || !x || !x_mask || !out) return sbk_set_error(SBK_ERR_ARG, "sbk_melenc_forward: null argument");
-    if (e->cfg.kind != 1) return sbk_set_error(SBK_ERR_ARG, "sbk_melenc_forward: this handle is a text encoder, use sbk_textenc_forward");
+    if (!e || !x || !x_mask || !out) return fail(SBK_ERR_ARG, "sbk_melenc_forward: null argument");
+    if (e->cfg.kind != 1) return fail(SBK_ERR_ARG, "sbk_melenc_forward: this handle is a text encoder, use sbk_textenc_forward");
     return te_forward(e, nullptr, nullptr, nullptr, x, x_mask, out, nullptr, nullptr, B, T, stream);
 }
 

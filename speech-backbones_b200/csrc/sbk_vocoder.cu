@@ -19,11 +19,9 @@
 //   bf16            bf16 weights, and the conv inputs (the LeakyReLU operands mel_in, SA, A0, A1, A2, Hb) stored as bf16
 //                   [B][C/8][L][8]; the residual stream x (X0, X1, X2, R[j]), the GEMM output Z and conv_post's input stay fp32.
 // conv_post, tanh, the folds and the MRF mean are fp32 in every mode.
-#include "../../include/sbk.h"
-#include "sbk_internal.h"
+#include "sbk_host.h"
 
 #include <math.h>
-#include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
 
@@ -39,15 +37,6 @@ int sbk::device_sm_count() {
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
     return n;
 }
-
-int sbk_set_error(int code, const char* fmt, ...);     // sbk_api.cu: fills the thread-local error text
-
-#define VCU(x)                                                                                              \
-    do {                                                                                                    \
-        cudaError_t e_ = (x);                                                                               \
-        if (e_ != cudaSuccess)                                                                              \
-            return sbk_set_error(SBK_ERR_CUDA, "%s failed: %s (%s:%d)", #x, cudaGetErrorString(e_), __FILE__, __LINE__); \
-    } while (0)
 
 namespace {
 
@@ -151,16 +140,7 @@ __global__ void __launch_bounds__(256) k_voc_post(const float* a, const float* w
     }
 }
 
-// grid-stride elementwise kernels: 256-thread blocks, at most 16 blocks per SM
-int ew_grid(long long n) {
-    const long long g = (n + 255) / 256, cap = 16LL * device_sm_count();
-    return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
-struct VWSpec { std::string name; std::vector<int64_t> shape; };
-
 // the tensor-core form of each mode: fp32 and fp32x3 run the fp32x3 split, bf16 its bf16 operands, tf32 tf32 operands
-bool prec_x3(int precision) { return precision == SBK_PREC_FP32X3 || precision == SBK_PREC_FP32; }
 bool prec_bf16(int precision) { return precision == SBK_PREC_BF16; }
 
 }  // namespace
@@ -168,49 +148,44 @@ bool prec_bf16(int precision) { return precision == SBK_PREC_BF16; }
 struct sbk_vocoder {
     sbk_vocoder_config cfg;
     int precision = SBK_PREC_TF32;
-    std::vector<VWSpec> spec;
-    std::map<std::string, float*> raw;       // device copies, reference layout (after remove_weight_norm)
-    std::map<std::string, void*> packed;     // tensor-core stage images
-    std::map<std::string, size_t> packed_bytes;
+    WeightSet w;                             // raw: reference layout (after remove_weight_norm); packed: tensor-core stage images
     float* zero = nullptr;
-    void* mem = nullptr; size_t cap = 0;
+    Workspace ws;
     bool is_packed = false;
     int64_t last_launches = 0;
-    // test hook (sbk_vocoder_debug_*): per-name snapshots of the last forward's intermediates, in launch order; fmt 1 = fp32
-    // [B][C/4][L][4] (wav: [B][1][L]), 2 = bf16 [B][C/8][L][8]
-    struct Snap { std::string name; void* buf; size_t cap, numel; int fmt; };
-    bool capture = false;
-    std::vector<Snap> snaps;
+    // test hook (sbk_vocoder_debug_*): the last forward's intermediates; fmt 1 = fp32 [B][C/4][L][4] (wav: [B][1][L]),
+    // 2 = bf16 [B][C/8][L][8]
+    Snapshots snaps;
     int n_res() const { return cfg.n_kernels; }
-    bool x3() const { return prec_x3(precision); }
+    bool x3() const { return prec_runs_x3(precision); }
     bool bf16() const { return prec_bf16(precision); }
 };
 
 static int voc_geom(int k) { return k == 3 ? G_C1K3 : (k == 7 ? G_C1K7 : (k == 11 ? G_C1K11 : -1)); }
 
 extern "C" int sbk_vocoder_create(const sbk_vocoder_config* cfg, sbk_vocoder** out) {
-    if (!cfg || !out) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_create: null argument");
-    if (cfg->n_ups < 1 || cfg->n_ups > 4 || cfg->n_kernels != 3) return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: needs 1..4 upsample stages and 3 resblock kernels (HiFi-GAN V1/V2 layout)");
-    if (cfg->num_mels <= 0 || cfg->num_mels % 8 != 0) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_create: num_mels must be a multiple of 8 (one K stage), got %d", cfg->num_mels);
+    if (!cfg || !out) return fail(SBK_ERR_ARG, "sbk_vocoder_create: null argument");
+    if (cfg->n_ups < 1 || cfg->n_ups > 4 || cfg->n_kernels != 3) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: needs 1..4 upsample stages and 3 resblock kernels (HiFi-GAN V1/V2 layout)");
+    if (cfg->num_mels <= 0 || cfg->num_mels % 8 != 0) return fail(SBK_ERR_ARG, "sbk_vocoder_create: num_mels must be a multiple of 8 (one K stage), got %d", cfg->num_mels);
     int ch = cfg->upsample_initial_channel;
-    if (ch % 64 != 0) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_create: upsample_initial_channel must be a multiple of 64");
+    if (ch % 64 != 0) return fail(SBK_ERR_ARG, "sbk_vocoder_create: upsample_initial_channel must be a multiple of 64");
     for (int i = 0; i < cfg->n_ups; ++i) {
         const int u = cfg->upsample_rates[i], k = cfg->upsample_kernel_sizes[i];
-        if (k != 2 * u || u % 2 != 0) return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: stage %d: ConvTranspose1d needs k = 2*stride and an even stride (got k=%d, u=%d)", i, k, u);
-        if (ch % 32 != 0) return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: stage %d input channels %d: need a multiple of 32", i, ch);
+        if (k != 2 * u || u % 2 != 0) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: stage %d: ConvTranspose1d needs k = 2*stride and an even stride (got k=%d, u=%d)", i, k, u);
+        if (ch % 32 != 0) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: stage %d input channels %d: need a multiple of 32", i, ch);
         ch /= 2;
-        if (ch % 32 != 0) return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: stage %d has %d channels; the tensor-core path needs multiples of 32 (HiFi-GAN V1)", i, ch);
+        if (ch % 32 != 0) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: stage %d has %d channels; the tensor-core path needs multiples of 32 (HiFi-GAN V1)", i, ch);
     }
     for (int j = 0; j < 3; ++j) {
-        if (voc_geom(cfg->resblock_kernel_sizes[j]) < 0) return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: resblock kernel %d (supported: 3, 7, 11)", cfg->resblock_kernel_sizes[j]);
+        if (voc_geom(cfg->resblock_kernel_sizes[j]) < 0) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: resblock kernel %d (supported: 3, 7, 11)", cfg->resblock_kernel_sizes[j]);
         for (int d = 0; d < 3; ++d) {
             const int dil = cfg->resblock_dilations[j][d];
-            if (dil < 1 || (cfg->resblock_kernel_sizes[j] - 1) * dil > 64) return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: halo (k-1)*d = %d exceeds 64 samples", (cfg->resblock_kernel_sizes[j] - 1) * dil);
+            if (dil < 1 || (cfg->resblock_kernel_sizes[j] - 1) * dil > 64) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: halo (k-1)*d = %d exceeds 64 samples", (cfg->resblock_kernel_sizes[j] - 1) * dil);
         }
     }
     sbk_vocoder* v = new sbk_vocoder();
     v->cfg = *cfg;
-    auto add = [&](const std::string& n, std::vector<int64_t> s) { v->spec.push_back({n, s}); };
+    auto add = [&](const std::string& n, std::vector<int64_t> s) { v->w.add(n, std::move(s)); };
     const int c0 = cfg->upsample_initial_channel;
     add("conv_pre.weight", {c0, cfg->num_mels, 7}); add("conv_pre.bias", {c0});
     for (int i = 0; i < cfg->n_ups; ++i) {
@@ -234,51 +209,32 @@ extern "C" int sbk_vocoder_create(const sbk_vocoder_config* cfg, sbk_vocoder** o
 
 extern "C" void sbk_vocoder_destroy(sbk_vocoder* v) {
     if (!v) return;
-    for (auto& kv : v->raw) cudaFree(kv.second);
-    for (auto& kv : v->packed) cudaFree(kv.second);
     if (v->zero) cudaFree(v->zero);
-    if (v->mem) cudaFree(v->mem);
-    for (auto& sn : v->snaps) cudaFree(sn.buf);
     delete v;
 }
 
 // Host logic only (no device work): the mode's tiling rules, then the packed state is dropped.
 extern "C" int sbk_vocoder_set_precision(sbk_vocoder* v, int32_t precision) {
-    if (!v) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_set_precision: null handle");
-    if (precision < SBK_PREC_FP32 || precision > SBK_PREC_FP32X3) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_set_precision: unknown precision %d", precision);
+    if (!v) return fail(SBK_ERR_ARG, "sbk_vocoder_set_precision: null handle");
+    if (precision < SBK_PREC_FP32 || precision > SBK_PREC_FP32X3) return fail(SBK_ERR_ARG, "sbk_vocoder_set_precision: unknown precision %d", precision);
     if (prec_bf16(precision)) {
         // bf16 K stages hold 16 input channels (Conv1d) and 64 (GEMM, sbk_conv_tc.cu conv_tc_stage_channels).  Every stage
         // has a multiple of 32 channels (sbk_vocoder_create), so its GEMM reads a multiple of 64: only conv_pre can fail.
         const int c1 = conv_tc_stage_channels(G_C1K3, 1);
         if (v->cfg.num_mels % c1 != 0)
-            return sbk_set_error(SBK_ERR_UNSUPPORTED, "sbk_vocoder_set_precision: bf16 needs num_mels to be a multiple of %d, got %d", c1, v->cfg.num_mels);
+            return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_set_precision: bf16 needs num_mels to be a multiple of %d, got %d", c1, v->cfg.num_mels);
     }
     v->precision = precision;
     v->is_packed = false;
     return SBK_OK;
 }
 
-extern "C" int sbk_vocoder_num_weights(const sbk_vocoder* v) { return v ? (int)v->spec.size() : 0; }
-extern "C" const char* sbk_vocoder_weight_name(const sbk_vocoder* v, int i) {
-    if (!v || i < 0 || i >= (int)v->spec.size()) return nullptr;
-    return v->spec[i].name.c_str();
-}
+extern "C" int sbk_vocoder_num_weights(const sbk_vocoder* v) { return v ? v->w.count() : 0; }
+extern "C" const char* sbk_vocoder_weight_name(const sbk_vocoder* v, int i) { return v ? v->w.name(i) : nullptr; }
 
 extern "C" int sbk_vocoder_set_weight(sbk_vocoder* v, const char* name, const void* data, const int64_t* shape, int ndim) {
-    if (!v || !name || !data || !shape) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_set_weight: null argument");
-    const VWSpec* ws = nullptr;
-    for (auto& s : v->spec) if (s.name == name) { ws = &s; break; }
-    if (!ws) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_set_weight: unexpected key '%s' (strict)", name);
-    if ((int)ws->shape.size() != ndim) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_set_weight: '%s' rank %d, expected %d", name, ndim, (int)ws->shape.size());
-    size_t numel = 1;
-    for (int i = 0; i < ndim; ++i) {
-        if (ws->shape[i] != shape[i]) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_set_weight: '%s' dim %d is %lld, expected %lld", name, i, (long long)shape[i], (long long)ws->shape[i]);
-        numel *= (size_t)shape[i];
-    }
-    VCU(cudaSetDevice(v->cfg.device));
-    float*& dst = v->raw[name];
-    if (!dst) VCU(cudaMalloc(&dst, numel * sizeof(float)));
-    VCU(cudaMemcpy(dst, data, numel * sizeof(float), cudaMemcpyDefault));
+    if (!v || !name || !data || !shape) return fail(SBK_ERR_ARG, "sbk_vocoder_set_weight: null argument");
+    TRY(v->w.set(name, data, shape, ndim, v->cfg.device, "sbk_vocoder_set_weight"));
     v->is_packed = false;
     return SBK_OK;
 }
@@ -288,27 +244,21 @@ extern "C" int sbk_vocoder_set_weight(sbk_vocoder* v, const char* name, const vo
 static int voc_pack(sbk_vocoder* v, const std::vector<float>& w, const std::string& key, int cout, int cin, int geom) {
     const bool bf = v->bf16(), x3 = v->x3();
     const int NT = x3 ? conv_tc_ntile_x3(geom, cout) : conv_tc_ntile(geom, cout), CPS = conv_tc_stage_channels(geom, bf ? 1 : 0);
-    if (cin % CPS != 0 || cout % NT != 0) return sbk_set_error(SBK_ERR_UNSUPPORTED, "vocoder pack '%s': %d -> %d channels do not tile (K stage %d, N tile %d)", key.c_str(), cin, cout, CPS, NT);
+    if (cin % CPS != 0 || cout % NT != 0) return fail(SBK_ERR_UNSUPPORTED, "vocoder pack '%s': %d -> %d channels do not tile (K stage %d, N tile %d)", key.c_str(), cin, cout, CPS, NT);
     std::vector<uint8_t> img(conv_tc_pack_image(w.data(), cout, cin, geom, bf, x3, 0, nullptr));
     conv_tc_pack_image(w.data(), cout, cin, geom, bf, x3, 0, img.data());
-    void*& d = v->packed[key];
-    size_t& have = v->packed_bytes[key];
-    if (d && have != img.size()) { VCU(cudaFree(d)); d = nullptr; }     // another mode's image
-    if (!d) { VCU(cudaMalloc(&d, img.size())); have = img.size(); }
-    VCU(cudaMemcpy(d, img.data(), img.size(), cudaMemcpyHostToDevice));
-    return SBK_OK;
+    return upload(v->w.packed, key, img.size(), img.data());
 }
 
 extern "C" int sbk_vocoder_pack(sbk_vocoder* v) {
-    if (!v) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_pack: null handle");
-    for (auto& s : v->spec) if (!v->raw.count(s.name)) return sbk_set_error(SBK_ERR_STATE, "sbk_vocoder_pack: missing key '%s' (strict)", s.name.c_str());
-    VCU(cudaSetDevice(v->cfg.device));
+    if (!v) return fail(SBK_ERR_ARG, "sbk_vocoder_pack: null handle");
+    TRY(v->w.require_all("sbk_vocoder_pack"));
+    CU(cudaSetDevice(v->cfg.device));
     v->is_packed = false;
-    for (auto& s : v->spec) {
+    for (auto& s : v->w.spec) {
         if (s.name.size() < 7 || s.name.compare(s.name.size() - 7, 7, ".weight") != 0 || s.name == "conv_post.weight") continue;
-        size_t numel = 1; for (auto d : s.shape) numel *= (size_t)d;
-        std::vector<float> w(numel);
-        VCU(cudaMemcpy(w.data(), v->raw[s.name], numel * 4, cudaMemcpyDeviceToHost));
+        std::vector<float> w;
+        TRY(v->w.fetch(s.name, w));
         const std::string key = s.name.substr(0, s.name.size() - 7) + ".wtc";
         int rc;
         if (s.name.compare(0, 4, "ups.") == 0) {
@@ -323,7 +273,7 @@ extern "C" int sbk_vocoder_pack(sbk_vocoder* v) {
         }
         if (rc != SBK_OK) return rc;
     }
-    if (!v->zero) { VCU(cudaMalloc(&v->zero, 8192)); VCU(cudaMemset(v->zero, 0, 8192)); }
+    if (!v->zero) { CU(cudaMalloc(&v->zero, 8192)); CU(cudaMemset(v->zero, 0, 8192)); }
     v->is_packed = true;
     return SBK_OK;
 }
@@ -332,7 +282,7 @@ namespace {
 
 // The workspace of one (B, T) in the handle's mode: 11 activation buffers of the largest stage, the transposed-conv GEMM
 // output and the re-laid-out mel.  SA, A0, A1, A2, Hb and the mel are conv inputs: bf16 in the bf16 mode, and with a
-// correction twin each in fp32x3.  With base = null only the size is computed.
+// correction twin each in fp32x3.  Over a null-base arena only the size is computed.
 struct VocBufs {
     void* melc; float* melc_lo; float* Z;
     void *SA, *A0, *A1, *A2, *Hb;
@@ -340,15 +290,14 @@ struct VocBufs {
     float *X0, *X1, *X2, *R[3];
 };
 
-size_t voc_carve(const sbk_vocoder* v, int B, int T, char* base, VocBufs* o) {
+size_t voc_carve(const sbk_vocoder* v, int B, int T, Arena& ar, VocBufs* o) {
     const sbk_vocoder_config& c = v->cfg;
     size_t big = 0, zmax = 0;
     { long long L = T; int ch = c.upsample_initial_channel; big = (size_t)B * ch * L;
       for (int i = 0; i < c.n_ups; ++i) { zmax = std::max<size_t>(zmax, (size_t)B * c.upsample_kernel_sizes[i] * (ch / 2) * L); L *= c.upsample_rates[i]; ch /= 2; big = std::max<size_t>(big, (size_t)B * ch * L); } }
     const size_t ob = v->bf16() ? 2 : 4;            // bytes per element of an operand tensor
     const bool x3 = v->x3();
-    size_t off = 0;
-    auto take = [&](size_t bytes) -> char* { off = (off + 255) & ~size_t(255); char* r = base ? base + off : nullptr; off += bytes; return r; };
+    auto take = [&](size_t bytes) { return (char*)ar.take(bytes); };
     VocBufs b{};
     b.melc = take((size_t)B * c.num_mels * T * ob);
     b.Z = (float*)take(zmax * 4);
@@ -363,38 +312,33 @@ size_t voc_carve(const sbk_vocoder* v, int B, int T, char* base, VocBufs* o) {
         b.A2_lo = (float*)take(big * 4); b.Hb_lo = (float*)take(big * 4);
     }
     if (o) *o = b;
-    return off + 256;
+    return ar.bytes();
 }
 
 }  // namespace
 
 extern "C" size_t sbk_vocoder_workspace_bytes(const sbk_vocoder* v, int B, int T) {
     if (!v || B <= 0 || T <= 0) return 0;
-    return voc_carve(v, B, T, nullptr, nullptr);
+    Arena probe;
+    return voc_carve(v, B, T, probe, nullptr);
 }
 
 extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav, int B, int T, void* stream) {
-    if (!v || !mel || !wav) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_forward: null argument");
-    if (!v->is_packed) return sbk_set_error(SBK_ERR_STATE, "sbk_vocoder_forward: weights not packed for the current precision (sbk_vocoder_set_weight for every key, then sbk_vocoder_pack)");
-    if (B <= 0 || T <= 0) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_forward: B and T must be positive (got %d, %d)", B, T);
-    VCU(cudaSetDevice(v->cfg.device));
+    if (!v || !mel || !wav) return fail(SBK_ERR_ARG, "sbk_vocoder_forward: null argument");
+    if (!v->is_packed) return fail(SBK_ERR_STATE, "sbk_vocoder_forward: weights not packed for the current precision (sbk_vocoder_set_weight for every key, then sbk_vocoder_pack)");
+    if (B <= 0 || T <= 0) return fail(SBK_ERR_ARG, "sbk_vocoder_forward: B and T must be positive (got %d, %d)", B, T);
+    CU(cudaSetDevice(v->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
     const sbk_vocoder_config& c = v->cfg;
     const size_t need = sbk_vocoder_workspace_bytes(v, B, T);
-    if (need > v->cap) {
-        if (v->mem) { cudaFree(v->mem); v->mem = nullptr; v->cap = 0; }
-        const cudaError_t e = cudaMalloc(&v->mem, need);
-        if (e != cudaSuccess) { v->mem = nullptr; cudaGetLastError(); return sbk_set_error(SBK_ERR_CUDA, "out of memory: the vocoder workspace for (B=%d, T=%d) needs %zu bytes", B, T, need); }
-        v->cap = need;
-    }
+    if (v->ws.reserve(need)) return fail(SBK_ERR_CUDA, "out of memory: the vocoder workspace for (B=%d, T=%d) needs %zu bytes", B, T, need);
     VocBufs wb;
-    voc_carve(v, B, T, (char*)v->mem, &wb);
+    Arena ar = v->ws.arena();
+    voc_carve(v, B, T, ar, &wb);
     const bool x3 = v->x3(), bf = v->bf16();
     const int ofmt = bf ? 2 : 1;                     // debug layout of the operand tensors
     void *melc = wb.melc, *SA = wb.SA, *A0 = wb.A0, *A1 = wb.A1, *A2 = wb.A2, *Hb = wb.Hb;
     float *Z = wb.Z, *X0 = wb.X0, *X1 = wb.X1, *X2 = wb.X2, **R = wb.R;
-    auto W = [&](const std::string& k) -> const void* { auto it = v->packed.find(k); if (it != v->packed.end()) return it->second; auto i2 = v->raw.find(k); return i2 != v->raw.end() ? i2->second : nullptr; };
-    auto Wf = [&](const std::string& k) { return (const float*)W(k); };
     int64_t n = 0;
     int rcl = 0;
     // act_out: out = lrelu(conv + bias), the next conv's operand (fp32x3: a_corr = its correction chunks); otherwise
@@ -403,7 +347,7 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
                     int act_out, const float* addin, void* a_out, float* a_corr) {
         ConvTcParams p; memset(&p, 0, sizeof(p));
         p.geom = geom; p.in0 = in; p.c0 = cin; p.H = 1; p.W = L; p.B = B; p.Ho = 1; p.Wo = L;
-        p.wpk = W(pre + ".wtc"); p.bias = geom == G_PW ? nullptr : Wf(pre + ".bias"); p.out = (float*)out; p.Cout = cout; p.epi = EPI_PLAIN;
+        p.wpk = v->w.get(pre + ".wtc"); p.bias = geom == G_PW ? nullptr : v->w.get(pre + ".bias"); p.out = (float*)out; p.Cout = cout; p.epi = EPI_PLAIN;
         p.zero_page = v->zero; p.dil = dil; p.pad = geom == G_PW ? 0 : (conv_tc_taps(geom) - 1) * dil / 2;
         p.slope = kSlope; p.act_out = act_out; p.addin = addin;
         if (act_out) { p.out_lo = a_corr; p.act_out2 = 0; }
@@ -412,23 +356,10 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
         const int k = launch_conv_tc(p, s);
         if (k < 0) rcl = -1; else n += k;
     };
-    // debug capture: the workspace buffers are overwritten within the call, so each written tensor is copied (stream-ordered)
-    // right after its launch into a per-name buffer.  The copies are not launches and do not count in last_launches.
-    size_t nsnap = 0;
-    cudaError_t snap_err = cudaSuccess;
-    // (the name is pre + suf, put together only when capturing)
+    // debug capture (the name is pre + suf, put together only when capturing)
+    v->snaps.begin();
     auto snap = [&](const std::string& pre, const char* suf, const void* src, size_t numel, int fmt) {
-        if (!v->capture || snap_err != cudaSuccess) return;
-        if (nsnap == v->snaps.size()) v->snaps.push_back({std::string(), nullptr, 0, 0, 1});
-        sbk_vocoder::Snap& sn = v->snaps[nsnap++];
-        const size_t bytes = numel * (fmt == 2 ? 2 : 4);
-        sn.name = pre + suf; sn.numel = numel; sn.fmt = fmt;
-        if (bytes > sn.cap) {
-            cudaFree(sn.buf); sn.buf = nullptr; sn.cap = 0;
-            if ((snap_err = cudaMalloc(&sn.buf, bytes)) != cudaSuccess) { sn.buf = nullptr; sn.numel = 0; return; }
-            sn.cap = bytes;
-        }
-        snap_err = cudaMemcpyAsync(sn.buf, src, bytes, cudaMemcpyDeviceToDevice, s);
+        if (v->snaps.on) v->snaps.record(pre + suf, src, numel, fmt, s);
     };
     const size_t bn = (size_t)B;
     k_voc_mel_in<<<ew_grid((long long)B * (c.num_mels / 4) * T), 256, 0, s>>>(mel, melc, wb.melc_lo, B, c.num_mels, T, bf ? 1 : 0); ++n;
@@ -445,7 +376,7 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
         conv(G_PW, up, SA, wb.SA_lo, ch, k * co, L, 1, Z, 0, nullptr, nullptr, nullptr);    // Z[i][t*co + c] (models.py:108)
         snap(up, ".z", Z, bn * k * co * L, 1);
         const int Lo = L * u;
-        k_voc_ct_fold<<<ew_grid((long long)B * (co / 4) * Lo), 256, 0, s>>>(Z, Wf(up + ".bias"), X0, A0, wb.A0_lo, B, co, L, u, kSlope, bf ? 1 : 0); ++n;
+        k_voc_ct_fold<<<ew_grid((long long)B * (co / 4) * Lo), 256, 0, s>>>(Z, v->w.get(up + ".bias"), X0, A0, wb.A0_lo, B, co, L, u, kSlope, bf ? 1 : 0); ++n;
         snap(up, ".x", X0, bn * co * Lo, 1); snap(up, ".a", A0, bn * co * Lo, ofmt);
         ch = co; L = Lo;
         const size_t na = bn * ch * L;
@@ -474,18 +405,15 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
         void* mo = last ? (void*)X0 : SA;
         k_voc_mrf<<<ew_grid(n4), 256, 0, s>>>(reinterpret_cast<const float4*>(R[0]), reinterpret_cast<const float4*>(R[1]), reinterpret_cast<const float4*>(R[2]),
                                                mo, last ? nullptr : wb.SA_lo, n4, L, 1.0f / 3.0f, last ? 0.01f : kSlope, (bf && !last) ? 1 : 0); ++n;
-        if (v->capture) snap("mrf." + std::to_string(i), "", mo, na, last ? 1 : ofmt);
+        if (v->snaps.on) snap("mrf." + std::to_string(i), "", mo, na, last ? 1 : ofmt);
         if (last) post_in = X0;
     }
-    k_voc_post<<<ew_grid((long long)B * L), 256, 7 * ch * sizeof(float), s>>>(post_in, Wf("conv_post.weight"), Wf("conv_post.bias"), wav, B, ch, L); ++n;
+    k_voc_post<<<ew_grid((long long)B * L), 256, 7 * ch * sizeof(float), s>>>(post_in, v->w.get("conv_post.weight"), v->w.get("conv_post.bias"), wav, B, ch, L); ++n;
     snap("wav", "", wav, bn * L, 1);
-    if (v->capture) {
-        for (size_t i = nsnap; i < v->snaps.size(); ++i) cudaFree(v->snaps[i].buf);
-        v->snaps.resize(nsnap);
-    }
-    if (rcl < 0) return sbk_set_error(SBK_ERR_CUDA, "sbk_vocoder_forward: a tensor-core launch was refused (device attribute / geometry)");
-    if (snap_err != cudaSuccess) return sbk_set_error(SBK_ERR_CUDA, "sbk_vocoder_forward: debug capture failed: %s", cudaGetErrorString(snap_err));
-    VCU(cudaGetLastError());
+    const cudaError_t snap_err = v->snaps.finish();
+    if (rcl < 0) return fail(SBK_ERR_CUDA, "sbk_vocoder_forward: a tensor-core launch was refused (device attribute / geometry)");
+    if (snap_err != cudaSuccess) return fail(SBK_ERR_CUDA, "sbk_vocoder_forward: debug capture failed: %s", cudaGetErrorString(snap_err));
+    CU(cudaGetLastError());
     v->last_launches = n;
     return SBK_OK;
 }
@@ -493,40 +421,20 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
 extern "C" int64_t sbk_vocoder_last_launch_count(const sbk_vocoder* v) { return v ? v->last_launches : 0; }
 
 extern "C" int sbk_vocoder_debug_capture(sbk_vocoder* v, int on) {
-    if (!v) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_debug_capture: null handle");
-    v->capture = on != 0;
+    if (!v) return fail(SBK_ERR_ARG, "sbk_vocoder_debug_capture: null handle");
+    v->snaps.on = on != 0;
     return SBK_OK;
 }
-extern "C" int sbk_vocoder_debug_num(const sbk_vocoder* v) { return v ? (int)v->snaps.size() : 0; }
+extern "C" int sbk_vocoder_debug_num(const sbk_vocoder* v) { return v ? (int)v->snaps.list.size() : 0; }
 extern "C" const char* sbk_vocoder_debug_name(const sbk_vocoder* v, int i) {
-    if (!v || i < 0 || i >= (int)v->snaps.size()) return nullptr;
-    return v->snaps[i].name.c_str();
+    if (!v || i < 0 || i >= (int)v->snaps.list.size()) return nullptr;
+    return v->snaps.list[i].name.c_str();
 }
 extern "C" int sbk_vocoder_debug_op_layout(const sbk_vocoder* v, const char* name) {
-    if (!v || !name) return -1;
-    for (auto& sn : v->snaps) if (sn.name == name) return sn.fmt;
-    return -1;
+    const Snapshots::Snap* sn = v && name ? v->snaps.find(name) : nullptr;
+    return sn ? sn->fmt : -1;
 }
 extern "C" int sbk_vocoder_debug_read(sbk_vocoder* v, const char* name, float* dst, int64_t* numel) {
-    if (!v || !name) return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_debug_read: null argument");
-    for (auto& sn : v->snaps) {
-        if (sn.name != name) continue;
-        if (numel) *numel = (int64_t)sn.numel;
-        if (dst && sn.numel > 0) {
-            VCU(cudaSetDevice(v->cfg.device));
-            VCU(cudaDeviceSynchronize());
-            if (sn.fmt == 2) {
-                // bf16 snapshot: widened to fp32 on the host (exact), element order unchanged; dst may be host or device memory
-                std::vector<uint16_t> h16(sn.numel);
-                VCU(cudaMemcpy(h16.data(), sn.buf, sn.numel * 2, cudaMemcpyDeviceToHost));
-                std::vector<float> h32(sn.numel);
-                for (size_t i = 0; i < sn.numel; ++i) { const uint32_t u = (uint32_t)h16[i] << 16; memcpy(&h32[i], &u, 4); }
-                VCU(cudaMemcpy(dst, h32.data(), sn.numel * sizeof(float), cudaMemcpyDefault));
-            } else {
-                VCU(cudaMemcpy(dst, sn.buf, sn.numel * sizeof(float), cudaMemcpyDefault));
-            }
-        }
-        return SBK_OK;
-    }
-    return sbk_set_error(SBK_ERR_ARG, "sbk_vocoder_debug_read: no intermediate named '%s'", name);
+    if (!v || !name) return fail(SBK_ERR_ARG, "sbk_vocoder_debug_read: null argument");
+    return v->snaps.read(name, dst, numel, v->cfg.device, "sbk_vocoder_debug_read");
 }

@@ -24,7 +24,7 @@ import torch
 import torch.nn as nn
 from torch.nn.utils import remove_weight_norm, weight_norm
 
-from .binding import PREC, _check, _ptr, load_library
+from .binding import PREC, _check, _check_precision, _NativeHandle, _ptr
 
 
 class SbkVocoderConfig(C.Structure):
@@ -52,34 +52,21 @@ class _ResBlock1(nn.Module):                                   # reference name:
             remove_weight_norm(l)
 
 
-def _check_precision(precision):
-    if precision not in PREC:
-        raise ValueError(f"precision must be one of {sorted(PREC)}, got {precision!r}")
-    return precision
-
-
-class VocoderEngine:
-    """One sbk_vocoder handle (device + packed weights + workspace) in one precision mode."""
+class VocoderEngine(_NativeHandle):
+    """One sbk_vocoder handle (device + packed weights + workspace) in one precision mode.  load_state_dict takes the
+    effective weights (after remove_weight_norm) under the reference names."""
+    PREFIX = "sbk_vocoder"
+    STATE_DICT = "the vocoder state_dict"
 
     def __init__(self, h, device, precision="tf32"):
         self.precision = _check_precision(precision)
-        self.lib = load_library()
+        super().__init__()
         P, I = C.c_void_p, C.c_int
-        self.lib.sbk_vocoder_create.argtypes = [C.POINTER(SbkVocoderConfig), C.POINTER(P)]
-        self.lib.sbk_vocoder_destroy.argtypes = [P]
-        self.lib.sbk_vocoder_destroy.restype = None
-        self.lib.sbk_vocoder_num_weights.argtypes = [P]
-        self.lib.sbk_vocoder_weight_name.argtypes = [P, I]
-        self.lib.sbk_vocoder_weight_name.restype = C.c_char_p
-        self.lib.sbk_vocoder_set_weight.argtypes = [P, C.c_char_p, P, C.POINTER(C.c_int64), I]
-        self.lib.sbk_vocoder_pack.argtypes = [P]
         self.lib.sbk_vocoder_set_precision.argtypes = [P, C.c_int32]
         self.lib.sbk_vocoder_debug_op_layout.argtypes = [P, C.c_char_p]
         self.lib.sbk_vocoder_workspace_bytes.argtypes = [P, I, I]
         self.lib.sbk_vocoder_workspace_bytes.restype = C.c_size_t
         self.lib.sbk_vocoder_forward.argtypes = [P, P, P, I, I, P]
-        self.lib.sbk_vocoder_last_launch_count.argtypes = [P]
-        self.lib.sbk_vocoder_last_launch_count.restype = C.c_int64
         self.lib.sbk_vocoder_debug_capture.argtypes = [P, I]
         self.lib.sbk_vocoder_debug_num.argtypes = [P]
         self.lib.sbk_vocoder_debug_name.argtypes = [P, I]
@@ -100,8 +87,7 @@ class VocoderEngine:
             cfg.resblock_kernel_sizes[j] = rk[j]
             for d in range(3):
                 cfg.resblock_dilations[j][d] = rd[j][d]
-        self.h = C.c_void_p()
-        _check(self.lib.sbk_vocoder_create(C.byref(cfg), C.byref(self.h)), "sbk_vocoder_create")
+        _check(self._create(cfg), "sbk_vocoder_create")
         rc = self.lib.sbk_vocoder_set_precision(self.h, PREC[precision])
         if rc != 0:
             self.close()
@@ -113,31 +99,6 @@ class VocoderEngine:
         for u in rates:
             self.hop *= u
         self._last_bt = None
-
-    def close(self):
-        if getattr(self, "h", None) and self.h.value:
-            self.lib.sbk_vocoder_destroy(self.h)
-            self.h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def weight_names(self):
-        return [self.lib.sbk_vocoder_weight_name(self.h, i).decode() for i in range(self.lib.sbk_vocoder_num_weights(self.h))]
-
-    def load_state_dict(self, sd):
-        """`sd`: effective weights (after remove_weight_norm), reference names."""
-        for name in self.weight_names():
-            if name not in sd:
-                raise RuntimeError(f"missing key '{name}' in the vocoder state_dict (strict)")
-            t = sd[name].detach().to(torch.float32).contiguous()
-            shape = (C.c_int64 * t.dim())(*t.shape)
-            _check(self.lib.sbk_vocoder_set_weight(self.h, name.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()),
-                   f"sbk_vocoder_set_weight({name})")
-        _check(self.lib.sbk_vocoder_pack(self.h), "sbk_vocoder_pack")
 
     def workspace_bytes(self, B, T):
         return int(self.lib.sbk_vocoder_workspace_bytes(self.h, B, T))
@@ -156,17 +117,9 @@ class VocoderEngine:
         B, _, T = mel.shape
         wav = torch.empty((B, 1, T * self.hop), dtype=torch.float32, device=mel.device)
         with torch.cuda.device(mel.device):
-            stream = C.c_void_p(torch.cuda.current_stream(mel.device).cuda_stream)
-            rc = self.lib.sbk_vocoder_forward(self.h, _ptr(mel), _ptr(wav), B, T, stream)
-            if rc != 0 and b"out of memory" in self.lib.sbk_last_error():
-                torch.cuda.empty_cache()
-                rc = self.lib.sbk_vocoder_forward(self.h, _ptr(mel), _ptr(wav), B, T, stream)
-            _check(rc, "sbk_vocoder_forward")
+            self._call(self.lib.sbk_vocoder_forward, "sbk_vocoder_forward", self.h, _ptr(mel), _ptr(wav), B, T, self._stream())
         self._last_bt = (B, T)
         return wav
-
-    def last_launch_count(self):
-        return int(self.lib.sbk_vocoder_last_launch_count(self.h))
 
     # ---- test hooks: the intermediates of the last forward run with capture on (sbk_vocoder_debug_*)
     def debug_capture(self, on=True):

@@ -15,7 +15,7 @@ import ctypes as C
 import torch
 import torch.nn as nn
 
-from .binding import PREC, _check, _ptr, load_library
+from .binding import PREC, _check, _check_precision, _NativeHandle, _ptr
 from .gradtts import BaseModule, Mish
 
 
@@ -40,60 +40,22 @@ class _ResnetBlock(BaseModule):                  # reference name: ResnetBlock (
         self.res = nn.Conv2d(dim, dim, 1)
 
 
-def _bind(lib):
-    P, I = C.c_void_p, C.c_int
-    lib.sbk_postnet_create.argtypes = [C.POINTER(SbkPostNetConfig), C.POINTER(P)]
-    lib.sbk_postnet_destroy.argtypes = [P]
-    lib.sbk_postnet_destroy.restype = None
-    lib.sbk_postnet_num_weights.argtypes = [P]
-    lib.sbk_postnet_weight_name.argtypes = [P, I]
-    lib.sbk_postnet_weight_name.restype = C.c_char_p
-    lib.sbk_postnet_set_weight.argtypes = [P, C.c_char_p, P, C.POINTER(C.c_int64), I]
-    lib.sbk_postnet_pack.argtypes = [P]
-    lib.sbk_postnet_workspace_bytes.argtypes = [P, I, I, I]
-    lib.sbk_postnet_workspace_bytes.restype = C.c_size_t
-    lib.sbk_postnet_forward.argtypes = [P, P, P, P, I, I, I, P]
-    lib.sbk_postnet_last_launch_count.argtypes = [P]
-    lib.sbk_postnet_last_launch_count.restype = C.c_int64
-    return lib
-
-
-class PostNetEngine:
+class PostNetEngine(_NativeHandle):
     """One sbk_postnet handle.  Creating it is host logic (no GPU work): the weight inventory can be queried anywhere."""
+    PREFIX = "sbk_postnet"
+    STATE_DICT = "the PostNet state_dict"
 
     def __init__(self, dim, groups=8, device=0, precision="fp32x3"):
-        self.lib = _bind(load_library())
-        cfg = SbkPostNetConfig(device, dim, groups, PREC[precision])
-        self.h = C.c_void_p()
-        rc = self.lib.sbk_postnet_create(C.byref(cfg), C.byref(self.h))
+        super().__init__()
+        P, I = C.c_void_p, C.c_int
+        self.lib.sbk_postnet_workspace_bytes.argtypes = [P, I, I, I]
+        self.lib.sbk_postnet_workspace_bytes.restype = C.c_size_t
+        self.lib.sbk_postnet_forward.argtypes = [P, P, P, P, I, I, I, P]
+        rc = self._create(SbkPostNetConfig(device, dim, groups, PREC[precision]))
         if rc == _SBK_ERR_UNSUPPORTED:
             raise ValueError(self.lib.sbk_last_error().decode())
         _check(rc, "sbk_postnet_create")
         self.device, self.dim = device, dim
-
-    def close(self):
-        if getattr(self, "h", None) and self.h.value:
-            self.lib.sbk_postnet_destroy(self.h)
-            self.h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def weight_names(self):
-        return [self.lib.sbk_postnet_weight_name(self.h, i).decode() for i in range(self.lib.sbk_postnet_num_weights(self.h))]
-
-    def load_state_dict(self, sd):
-        for name in self.weight_names():
-            if name not in sd:
-                raise RuntimeError(f"missing key '{name}' in the PostNet state_dict (strict)")
-            t = sd[name].detach().to(torch.float32).contiguous()
-            shape = (C.c_int64 * t.dim())(*t.shape)
-            _check(self.lib.sbk_postnet_set_weight(self.h, name.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()),
-                   f"sbk_postnet_set_weight({name})")
-        _check(self.lib.sbk_postnet_pack(self.h), "sbk_postnet_pack")
 
     def forward(self, x, mask):
         for n, v in (("x", x), ("mask", mask)):
@@ -107,24 +69,15 @@ class PostNetEngine:
         x, mask = x.contiguous(), mask.to(torch.float32).contiguous()
         out = torch.empty_like(x)
         with torch.cuda.device(x.device):
-            stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
-            args = (self.h, _ptr(x), _ptr(mask), _ptr(out), B, Fm, T, stream)
-            rc = self.lib.sbk_postnet_forward(*args)
-            if rc != 0 and b"out of memory" in self.lib.sbk_last_error():
-                torch.cuda.empty_cache()          # the workspace is raw cudaMalloc, outside torch's caching allocator
-                rc = self.lib.sbk_postnet_forward(*args)
-            _check(rc, "sbk_postnet_forward")
+            self._call(self.lib.sbk_postnet_forward, "sbk_postnet_forward", self.h, _ptr(x), _ptr(mask), _ptr(out), B, Fm, T,
+                       self._stream())
         return out
-
-    def last_launch_count(self):
-        return int(self.lib.sbk_postnet_last_launch_count(self.h))
 
 
 class PostNet(BaseModule):
     def __init__(self, dim, groups=8, *, precision="fp32x3"):
         super().__init__()
-        if precision not in PREC:
-            raise ValueError(f"precision must be one of {sorted(PREC)}, got {precision!r}")
+        _check_precision(precision)
         PostNetEngine(dim, groups, precision=precision).close()     # the library's config check (host logic): ValueError
         self.dim, self.groups, self.precision = dim, groups, precision
         self.init_conv = nn.Conv2d(1, dim, 1)

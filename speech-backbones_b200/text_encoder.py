@@ -13,7 +13,7 @@ import ctypes as C
 import torch
 import torch.nn as nn
 
-from .binding import _check, _ptr, load_library
+from .binding import _check, _NativeHandle, _ptr
 from .gradtts import BaseModule
 
 
@@ -72,54 +72,21 @@ class _DurationPredictor(BaseModule):            # reference name: DurationPredi
         self.proj = nn.Conv1d(filt, 1, 1)
 
 
-class TextEncEngine:
-    """One sbk_textenc handle."""
+class TextEncEngine(_NativeHandle):
+    """One sbk_textenc handle (the text encoder, kind 0, or the mel encoder, kind 1).  Its calls are not retried on out of
+    memory."""
+    PREFIX = "sbk_textenc"
+    STATE_DICT = "the text-encoder state_dict"
 
     def __init__(self, m, device, kind=0):
-        self.lib = load_library()
+        super().__init__()
         P, I = C.c_void_p, C.c_int
-        L = self.lib
-        L.sbk_textenc_create.argtypes = [C.POINTER(SbkTextEncConfig), C.POINTER(P)]
-        L.sbk_textenc_destroy.argtypes = [P]
-        L.sbk_textenc_destroy.restype = None
-        L.sbk_textenc_num_weights.argtypes = [P]
-        L.sbk_textenc_weight_name.argtypes = [P, I]
-        L.sbk_textenc_weight_name.restype = C.c_char_p
-        L.sbk_textenc_set_weight.argtypes = [P, C.c_char_p, P, C.POINTER(C.c_int64), I]
-        L.sbk_textenc_pack.argtypes = [P]
-        L.sbk_textenc_forward.argtypes = [P, P, P, P, P, P, P, I, I, P]
-        L.sbk_textenc_last_launch_count.argtypes = [P]
-        L.sbk_textenc_last_launch_count.restype = C.c_int64
-        L.sbk_melenc_forward.argtypes = [P, P, P, P, I, I, P]
+        self.lib.sbk_textenc_forward.argtypes = [P, P, P, P, P, P, P, I, I, P]
+        self.lib.sbk_melenc_forward.argtypes = [P, P, P, P, I, I, P]
         cfg = SbkTextEncConfig(device, m.n_vocab, m.n_feats, m.n_channels, m.filter_channels, m.filter_channels_dp, m.n_heads,
                                m.n_layers, m.kernel_size, m.window_size, m.n_spks, m.spk_emb_dim, kind)
-        self.h = C.c_void_p()
-        _check(L.sbk_textenc_create(C.byref(cfg), C.byref(self.h)), "sbk_textenc_create")
+        _check(self._create(cfg), "sbk_textenc_create")
         self.device, self.n_feats, self.n_spks, self.spk_emb_dim = device, m.n_feats, m.n_spks, m.spk_emb_dim
-
-    def close(self):
-        if getattr(self, "h", None) and self.h.value:
-            self.lib.sbk_textenc_destroy(self.h)
-            self.h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def weight_names(self):
-        return [self.lib.sbk_textenc_weight_name(self.h, i).decode() for i in range(self.lib.sbk_textenc_num_weights(self.h))]
-
-    def load_state_dict(self, sd):
-        for name in self.weight_names():
-            if name not in sd:
-                raise RuntimeError(f"missing key '{name}' in the text-encoder state_dict (strict)")
-            t = sd[name].detach().to(torch.float32).contiguous()
-            shape = (C.c_int64 * t.dim())(*t.shape)
-            _check(self.lib.sbk_textenc_set_weight(self.h, name.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()),
-                   f"sbk_textenc_set_weight({name})")
-        _check(self.lib.sbk_textenc_pack(self.h), "sbk_textenc_pack")
 
     def forward(self, x, x_lengths, spk=None):
         for n, v in (("x", x), ("x_lengths", x_lengths), ("spk", spk)):
@@ -139,9 +106,8 @@ class TextEncEngine:
         logw = torch.empty((B, 1, Tx), dtype=torch.float32, device=x.device)
         mask = torch.empty((B, 1, Tx), dtype=torch.float32, device=x.device)
         with torch.cuda.device(x.device):
-            stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
             _check(self.lib.sbk_textenc_forward(self.h, _ptr(x), _ptr(x_lengths), _ptr(spk), _ptr(mu), _ptr(logw), _ptr(mask),
-                                                B, Tx, stream), "sbk_textenc_forward")
+                                                B, Tx, self._stream()), "sbk_textenc_forward")
         return mu, logw, mask
 
     def forward_mel(self, x, x_mask):
@@ -154,12 +120,8 @@ class TextEncEngine:
         x, x_mask = x.contiguous(), x_mask.to(torch.float32).contiguous()
         out = torch.empty_like(x)
         with torch.cuda.device(x.device):
-            stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
-            _check(self.lib.sbk_melenc_forward(self.h, _ptr(x), _ptr(x_mask), _ptr(out), B, T, stream), "sbk_melenc_forward")
+            _check(self.lib.sbk_melenc_forward(self.h, _ptr(x), _ptr(x_mask), _ptr(out), B, T, self._stream()), "sbk_melenc_forward")
         return out
-
-    def last_launch_count(self):
-        return int(self.lib.sbk_textenc_last_launch_count(self.h))
 
 
 class MelEncoder(BaseModule):
