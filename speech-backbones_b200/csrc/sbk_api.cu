@@ -204,6 +204,10 @@ extern "C" int sbk_create(const sbk_config* cfg, sbk_handle** out) {
     if (cfg->model == SBK_MODEL_DIFFVC && cfg->use_ref_t && cfg->dim_cond % 128 != 0)
         return fail(SBK_ERR_ARG, "sbk_create: the native RefBlock needs dim_cond to be a multiple of 128 (its first conv writes 64-channel "
                                  "tiles and every conv reads 32-channel K stages), got %d", cfg->dim_cond);
+    // Past the planar network inputs (k_first_conv and the first block's res_conv), every U-Net channel count, concatenations
+    // included, is a multiple of dim, and no tensor-core conv reads a K stage of more than 64 channels
+    // (conv_tc_stage_channels).  A multiple of 64 therefore lets every other U-Net conv of the tensor-core modes run on the
+    // tensor cores: the CUDA-core convs serve the fp32 mode alone.
     if (cfg->dim <= 0 || cfg->dim % 64 != 0) return fail(SBK_ERR_ARG, "sbk_create: dim must be a positive multiple of 64 (got %d)", cfg->dim);
     if (cfg->n_feats <= 0 || cfg->n_feats % 4 != 0) return fail(SBK_ERR_ARG, "sbk_create: n_feats must be a multiple of 4 (two stride-2 levels), got %d", cfg->n_feats);
     if (cfg->n_spks < 1 || cfg->spk_emb_dim <= 0) return fail(SBK_ERR_ARG, "sbk_create: bad speaker configuration");
@@ -402,28 +406,43 @@ extern "C" int sbk_pack(sbk_handle* h) {
             d[ci * 256 + hd * 64 + 32 + x] = s[(256 + hd * 32 + x) * C + ci];
         }
     };
-    for (size_t k = 0; k < h->resnets.size(); ++k) {
-        const ResnetInfo& r = h->resnets[k];
-        if (k == 0) TRY(repack(h, r.prefix + ".block1.block.0.weight", r.prefix + ".block1.w", (size_t)r.cin * 9 * r.cout, first_pack));
-        else TRY(repack(h, r.prefix + ".block1.block.0.weight", r.prefix + ".block1.w", (size_t)r.cin * 9 * r.cout, conv_pack));
-        TRY(repack(h, r.prefix + ".block2.block.0.weight", r.prefix + ".block2.w", (size_t)r.cout * 9 * r.cout, conv_pack));
-        if (r.cin != r.cout) TRY(repack(h, r.prefix + ".res_conv.weight", r.prefix + ".res.w", (size_t)r.cin * r.cout, conv_pack));
-    }
+    // the first ResnetBlock's block1 conv (k_first_conv) and res_conv (the planar-input tail) run on CUDA cores in every mode
+    const ResnetInfo& r0 = h->resnets[0];
+    TRY(repack(h, r0.prefix + ".block1.block.0.weight", r0.prefix + ".block1.w", (size_t)r0.cin * 9 * r0.cout, first_pack));
+    TRY(repack(h, r0.prefix + ".res_conv.weight", r0.prefix + ".res.w", (size_t)r0.cin * r0.cout, conv_pack));
     const bool x3 = h->cfg.precision == SBK_PREC_FP32X3;
-    if (h->cfg.precision != SBK_PREC_FP32) {
+    if (h->cfg.precision == SBK_PREC_FP32) {
+        for (size_t k = 0; k < h->resnets.size(); ++k) {
+            const ResnetInfo& r = h->resnets[k];
+            if (k != 0) TRY(repack(h, r.prefix + ".block1.block.0.weight", r.prefix + ".block1.w", (size_t)r.cin * 9 * r.cout, conv_pack));
+            TRY(repack(h, r.prefix + ".block2.block.0.weight", r.prefix + ".block2.w", (size_t)r.cout * 9 * r.cout, conv_pack));
+            if (k != 0 && r.cin != r.cout) TRY(repack(h, r.prefix + ".res_conv.weight", r.prefix + ".res.w", (size_t)r.cin * r.cout, conv_pack));
+        }
+        for (auto& a : h->attns) TRY(repack(h, a.prefix + ".fn.fn.to_qkv.weight", a.prefix + ".kv.w", (size_t)a.c * 256, kv_pack));
+        for (int l = 0; l < 2; ++l) {
+            const std::string p = "estimator.downs." + std::to_string(l) + ".3.conv";
+            const int c = h->cfg.dim << l;
+            TRY(repack(h, p + ".weight", p + ".w", (size_t)c * c * 9, conv_pack));
+        }
+        for (int j = 0; j < 2; ++j) {
+            const std::string p = "estimator.ups." + std::to_string(j) + ".3.conv";
+            const int c = h->cfg.dim << (1 - j);
+            TRY(repack(h, p + ".weight", p + ".w", (size_t)c * c * 16, convt_pack));
+        }
+        TRY(repack(h, "estimator.final_block.block.0.weight", "estimator.final_block.w", (size_t)h->cfg.dim * h->cfg.dim * 9, conv_pack));
+    } else {
         const bool bf = h->cfg.precision == SBK_PREC_BF16;
-        const int cps3 = conv_tc_stage_channels(G_C3, bf ? 1 : 0), cps1 = conv_tc_stage_channels(G_PW, bf ? 1 : 0);
-        for (auto& r : h->resnets) {
-            if (r.cin % cps3 == 0) TRY(pack_tc(h, r.prefix + ".block1.block.0.weight", r.prefix + ".block1.wtc", r.cout, r.cin, G_C3, bf));
+        for (size_t k = 0; k < h->resnets.size(); ++k) {
+            const ResnetInfo& r = h->resnets[k];
+            if (k != 0) TRY(pack_tc(h, r.prefix + ".block1.block.0.weight", r.prefix + ".block1.wtc", r.cout, r.cin, G_C3, bf));
             TRY(pack_tc(h, r.prefix + ".block2.block.0.weight", r.prefix + ".block2.wtc", r.cout, r.cout, G_C3, bf));
-            if (r.cin != r.cout && r.cin % cps1 == 0) TRY(pack_tc(h, r.prefix + ".res_conv.weight", r.prefix + ".res.wtc", r.cout, r.cin, G_PW, bf));
+            if (k != 0 && r.cin != r.cout) TRY(pack_tc(h, r.prefix + ".res_conv.weight", r.prefix + ".res.wtc", r.cout, r.cin, G_PW, bf));
         }
         TRY(pack_tc(h, "estimator.final_block.block.0.weight", "estimator.final_block.wtc", h->cfg.dim, h->cfg.dim, G_C3, bf));
-        for (auto& a : h->attns)
-            if (a.c % cps1 == 0) {
-                if (x3) TRY(pack_tc_kvx(h, a.prefix + ".fn.fn.to_qkv.weight", a.prefix + ".kvx.wtc", a.c));
-                else TRY(pack_tc_kv(h, a.prefix + ".fn.fn.to_qkv.weight", a.prefix + ".kv.wtc", a.c, bf));
-            }
+        for (auto& a : h->attns) {
+            if (x3) TRY(pack_tc_kvx(h, a.prefix + ".fn.fn.to_qkv.weight", a.prefix + ".kvx.wtc", a.c));
+            else TRY(pack_tc_kv(h, a.prefix + ".fn.fn.to_qkv.weight", a.prefix + ".kv.wtc", a.c, bf));
+        }
         for (int l = 0; l < 2; ++l) {
             const std::string p = "estimator.downs." + std::to_string(l) + ".3.conv";
             TRY(pack_tc(h, p + ".weight", p + ".wtc", h->cfg.dim << l, h->cfg.dim << l, G_DOWN, bf));
@@ -446,18 +465,6 @@ extern "C" int sbk_pack(sbk_handle* h) {
         }
         TRY(repack(h, "estimator.ref_block.block11.0.weight", "estimator.ref_block.block11.w", (size_t)9 * 2 * base, first_pack));
     }
-    for (auto& a : h->attns) TRY(repack(h, a.prefix + ".fn.fn.to_qkv.weight", a.prefix + ".kv.w", (size_t)a.c * 256, kv_pack));
-    for (int l = 0; l < 2; ++l) {
-        const std::string p = "estimator.downs." + std::to_string(l) + ".3.conv";
-        const int c = h->cfg.dim << l;
-        TRY(repack(h, p + ".weight", p + ".w", (size_t)c * c * 9, conv_pack));
-    }
-    for (int j = 0; j < 2; ++j) {
-        const std::string p = "estimator.ups." + std::to_string(j) + ".3.conv";
-        const int c = h->cfg.dim << (1 - j);
-        TRY(repack(h, p + ".weight", p + ".w", (size_t)c * c * 16, convt_pack));
-    }
-    TRY(repack(h, "estimator.final_block.block.0.weight", "estimator.final_block.w", (size_t)h->cfg.dim * h->cfg.dim * 9, conv_pack));
     // sinusoid frequencies, SinusoidalPosEmb.forward (diffusion.py:121-122): fp32 exp of fp32(j) * fp32(-ln(1e4)/(half-1))
     {
         const int half = h->cfg.dim / 2;
@@ -588,12 +595,12 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
     const bool b16 = c.precision == SBK_PREC_BF16;          // operand tensors in bf16 [B][H][C/8][W][8]
     const double osz = b16 ? 2.0 : 4.0;                     // bytes per operand-tensor element
     const int fmt_raw = use_tc ? 1 : 0, fmt_opnd = b16 ? 2 : fmt_raw;
-    const int tc_cps3 = conv_tc_stage_channels(G_C3, b16 ? 1 : 0), tc_cps1 = conv_tc_stage_channels(G_PW, b16 ? 1 : 0);
+    const int form = b16 ? FORM_BF16 : (x3 ? FORM_X3 : (use_tc ? FORM_TF32 : FORM_NHWC));
     auto push = [&](Op& op, const float* dbg, int64_t numel) {
         op.dbg_ptr = dbg; op.dbg_numel = numel;
         // raw Block-conv outputs (and the attention contexts) are fp32; every other named output is an operand tensor
-        const bool raw_out = op.kind == OP_FIRST || op.kind == OP_CTX || (op.kind == OP_CONVTC && op.tc.geom == G_C3) ||
-                             (op.kind == OP_IGEMM && op.ig.epi == EPI_PLAIN && op.ig.ostats);
+        // (the CUDA-core ops run in the fp32 mode only, where both formats are NHWC fp32)
+        const bool raw_out = op.kind == OP_FIRST || op.kind == OP_CTX || (op.kind == OP_CONVTC && op.tc.geom == G_C3);
         op.dbg_fmt = raw_out ? fmt_raw : fmt_opnd;
         if (op.kind == OP_IGEMM) {
             const IgemmParams& p = op.ig;
@@ -671,7 +678,6 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         const ResnetInfo& r = h->resnets[k];
         float* A = bf.A[lvl]; float* Bb = bf.Bf[lvl];
         double* st1 = stats_slot(); double* st2 = stats_slot();
-        const bool tc1 = use_tc && k != 0 && (c0 + c1) % tc_cps3 == 0 && c0 % tc_cps3 == 0;
         // ---- block1 conv -> raw h1 (A)
         if (k == 0) {
             Op op; op.kind = OP_FIRST; op.name = r.prefix + ".block1.raw";
@@ -682,7 +688,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             if (vc) { p.w_extra = pl.vc_wextra; p.step = pl.step_cur; }
             pl.first_op = (int)pl.ops.size();
             push(op, A, npix(lvl) * r.cout);
-        } else if (tc1) {
+        } else if (use_tc) {
             Op op = tc_conv(r.prefix + ".block1.raw", G_C3, r.prefix + ".block1.wtc", r.prefix + ".block1.block.0.bias", lvl,
                             in0, c0, in1, c1, r.cout, A, st1);
             push(op, A, npix(lvl) * r.cout);
@@ -699,7 +705,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
                 GnActParams& p = op.ga; memset(&p, 0, sizeof(p));
                 p.raw = A; p.gn = g1; p.tb = pl.tb + h->tb_off[k]; p.tb_stride = pl.tb_stride; p.step = pl.step_cur;
                 p.mask = pl.mask; p.T = T; p.lvl = lvl; p.out = Bb; p.B = B; p.H = Hs[lvl]; p.W = Ws[lvl]; p.C = r.cout;
-                p.round_tf32 = (b16 || x3) ? 0 : 1; p.chw4 = 1; p.out_bf16 = b16 ? 1 : 0; p.out_lo = LO(Bb);
+                p.form = form; p.out_lo = LO(Bb);
                 op.bytes = (4.0 + osz) * npix(lvl) * r.cout;
                 push(op, nullptr, 0);
             }
@@ -718,7 +724,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             ResFinalParams& p = op.rf; memset(&p, 0, sizeof(p));
             p.h2raw = h2; p.gn = g2;
             p.mask = pl.mask; p.T = T; p.lvl = lvl; p.out = out; p.B = B; p.H = Hs[lvl]; p.W = Ws[lvl]; p.C = r.cout;
-            p.out_mask = store_masked ? 1 : 0; p.chw4 = use_tc ? 1 : 0; p.bf16 = b16 ? 1 : 0; p.out_lo = LO(out);
+            p.out_mask = store_masked ? 1 : 0; p.form = form; p.out_lo = LO(out);
             if (k == 0) {
                 p.x = nullptr; p.mu = pl.mu; p.xt = pl.xt; p.spk_s = pl.spk_s; p.cin = cin0;
                 p.wres = h->w.get(r.prefix + ".res.w"); p.bres = h->w.get(r.prefix + ".res_conv.bias");
@@ -729,7 +735,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             }
             op.bytes = (4.0 + (k == 0 ? 0.0 : osz) + osz) * npix(lvl) * r.cout;
             push(op, out, npix(lvl) * r.cout);
-        } else if (use_tc && (c0 + c1) % tc_cps1 == 0 && c0 % tc_cps1 == 0) {
+        } else if (use_tc) {
             Op op = tc_conv(r.prefix + ".out", G_PW, r.prefix + ".res.wtc", r.prefix + ".res_conv.bias", lvl,
                             in0, c0, in1, c1, r.cout, out, nullptr);
             op.tc.epi = EPI_RES; op.tc.rraw = h2; op.tc.rgn = g2; op.tc.out_mask = store_masked ? 1 : 0;
@@ -742,7 +748,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             p.in0 = in0; p.c0 = c0; p.in1 = in1; p.c1 = c1;
             p.w = h->w.get(r.prefix + ".res.w"); p.bias = h->w.get(r.prefix + ".res_conv.bias");
             p.out = out; p.Cout = r.cout; p.pro = PRO_MASK; p.epi = EPI_RES;
-            p.rraw = h2; p.rgn = g2; p.out_mask = store_masked ? 1 : 0;
+            p.rraw = h2; p.rgn = g2;
             push(op, out, npix(lvl) * r.cout);
         }
     };
@@ -750,8 +756,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
     auto attention = [&](int k, int lvl, const float* x, float* out) {
         const AttnInfo& a = h->attns[k];
         int mt = igemm_mtiles(G_PW, Hs[lvl], Ws[lvl], Hs[lvl], Ws[lvl]);
-        const bool tc_apply = use_tc && a.c % tc_cps1 == 0;
-        if (tc_apply && x3) {
+        if (x3) {
             // fp32-class attention, fused (k_attn_kv_x3): k|v projection (tf32 + fp16 correction), softmax, context
             // partials - k and v never reach HBM.  One partial per item of attn_kv_tile_pixels() pixels: an utterance is cut
             // at the same pixels whatever batch it sits in.
@@ -761,7 +766,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             op.bytes = 8.0 * npix(lvl) * a.c;
             op.flops += 2.0 * npix(lvl) * 4096.0;
             push(op, nullptr, 0);
-        } else if (tc_apply) {
+        } else if (use_tc) {
             // k/v projection + softmax partials on tensor cores (k_attn_kv): items of attn_kv_tile_pixels() pixels x 4 heads
             Op op = tc_conv(a.prefix + ".kvpart", G_PW, a.prefix + ".kv.wtc", "", lvl, x, a.c, nullptr, 0, 256, nullptr, nullptr);
             op.tc.epi = EPI_KV; op.tc.kv_part = bf.kv_part;
@@ -788,10 +793,13 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             p.ctx = bf.ctx; p.wq = h->w.get(a.prefix + ".fn.fn.to_qkv.weight"); p.wout = h->w.get(a.prefix + ".fn.fn.to_out.weight");
             p.bout = h->w.get(a.prefix + ".fn.fn.to_out.bias"); p.g = h->w.get(a.prefix + ".fn.g");
             p.w_eff = bf.w_eff; p.b_eff = bf.b_eff; p.B = B; p.C = a.c;
-            if (tc_apply) { p.tc_nt = x3 ? conv_tc_ntile_x3(G_PW, a.c) : conv_tc_ntile(G_PW, a.c); p.tc_cps = tc_cps1; p.tc_bf16 = b16 ? 1 : 0; p.tc_x3 = x3 ? 1 : 0; }
+            if (use_tc) {
+                p.tc_nt = x3 ? conv_tc_ntile_x3(G_PW, a.c) : conv_tc_ntile(G_PW, a.c); p.tc_cps = conv_tc_stage_channels(G_PW, b16 ? 1 : 0);
+                p.tc_bf16 = b16 ? 1 : 0; p.tc_x3 = x3 ? 1 : 0;
+            }
             push(op, nullptr, 0);
         }
-        if (tc_apply) {
+        if (use_tc) {
             // the per-sample (I + g P_b) matrix is written by k_attn_mix directly in the tensor-core weight-stage layout
             Op op = tc_conv(a.prefix + ".out", G_PW, "", "", lvl, x, a.c, nullptr, 0, a.c, out, nullptr);
             op.tc.wpk = bf.w_eff; op.tc.w_bstride_bytes = (long long)a.c * a.c * (b16 ? 2 : (x3 ? 8 : 4)); op.tc.bias = bf.b_eff;
@@ -803,12 +811,12 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             op.ig = base_ig(G_PW, lvl, lvl);
             IgemmParams& p = op.ig;
             p.in0 = x; p.c0 = a.c; p.w = bf.w_eff; p.w_bstride = (long long)a.c * a.c; p.bias = bf.b_eff;
-            p.out = out; p.Cout = a.c; p.pro = PRO_NONE; p.epi = EPI_PLAIN; p.out_mask = use_tc ? 1 : 0;
+            p.out = out; p.Cout = a.c; p.pro = PRO_NONE; p.epi = EPI_PLAIN;
             push(op, out, npix(lvl) * a.c);
         }
     };
     auto resample = [&](int geom, const std::string& pre, int lvl_in, int lvl_out, const float* x, int C, float* out) {
-        if (use_tc && C % tc_cps3 == 0 && C % 64 == 0) {
+        if (use_tc) {
             Op op = tc_conv(pre + ".out", geom, pre + ".conv.wtc", pre + ".conv.bias", lvl_in, x, C, nullptr, 0, C, out, nullptr);
             op.tc.Ho = Hs[lvl_out]; op.tc.Wo = Ws[lvl_out]; op.tc.lvl = lvl_out; op.tc.out_mask = 1;
             op.flops = 2.0 * npix(lvl_out) * C * C * (geom == G_UP ? 4.0 : 9.0);
@@ -820,7 +828,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         op.ig = base_ig(geom, lvl_in, lvl_out);
         IgemmParams& p = op.ig;
         p.in0 = x; p.c0 = C; p.w = h->w.get(pre + ".conv.w"); p.bias = h->w.get(pre + ".conv.bias");
-        p.out = out; p.Cout = C; p.pro = PRO_MASK; p.epi = EPI_PLAIN; p.out_mask = use_tc ? 1 : 0;
+        p.out = out; p.Cout = C; p.pro = PRO_MASK; p.epi = EPI_PLAIN;
         push(op, out, npix(lvl_out) * C);
     };
 

@@ -35,7 +35,7 @@ struct IgemmParams {
     int Hin, Win, Hout, Wout;
     int B;
     const float* w; long long w_bstride;          // packed [ntaps][Cin][Cout] (+ optional per-sample stride)
-    const float* bias; long long bias_bstride;    // [Cout] or nullptr
+    const float* bias;                            // [Cout] or nullptr
     float* out; int Cout;
     // prologue
     int pro;
@@ -47,7 +47,6 @@ struct IgemmParams {
     double* ostats;                               // EPI_PLAIN: accumulate GN statistics of `out` (nullable)
     const float* rraw; GnRef rgn; int out_lvl;    // EPI_RES: out = acc + bias + Mish(GN(rraw))*mask
     float* kv_part;                               // EPI_KV: [B][mtiles][4][kKvPartFloats]
-    int out_mask;                                 // multiply the stored output by mask[b][wo << out_lvl]
 };
 
 // Tensor-core (wgmma) convolution (sbk_conv_tc.cu).  Inputs are operand-form tensors: already masked / activated, so the
@@ -92,15 +91,23 @@ struct ConvTcParams {
     float* out_corr;
 };
 
+// Layout and number form of the U-Net's activation tensors, one per precision mode (GnActParams / ResFinalParams::form).
+// Raw conv outputs (the GroupNorm inputs) are fp32 in every form: NHWC for FORM_NHWC, else [B][H][C/4][W][4].
+enum Form {
+    FORM_NHWC = 0,              // fp32 CUDA-core mode: NHWC fp32 [B][H][W][C], exact Mish
+    FORM_TF32 = 1,              // fp32 [B][H][C/4][W][4]; the Block activation is rounded to tf32 (cvt.rna), fast Mish
+    FORM_X3 = 2,                // fp32 [B][H][C/4][W][4] plus the correction twin through out_lo (corr_chunk), exact Mish
+    FORM_BF16 = 3,              // bf16 [B][H][C/8][W][8], fast Mish
+};
+
 // Block activation between the two convs of a ResnetBlock, written once in operand form (diffusion.py:57,76):
-//   act = mask ? tf32(Mish(GN(raw)) + tproj) : 0
+//   act = mask ? Mish(GN(raw)) + tproj : 0        (tensor-core forms only: the fp32 mode fuses it into the next conv)
 struct GnActParams {
     const float* raw; GnRef gn; const float* tb; int tb_stride; int tb_per_sample; const int* step;
     const float* mask; int T; int lvl;
-    float* out; int B, H, W, C; int round_tf32;
-    int chw4;
-    int out_bf16;               // write the activation as bf16 [B][H][C/8][W][8] (raw stays fp32 [B][H][C/4][W][4])
-    float* out_lo;              // fp32x3 mode: out keeps the unrounded fp32 value, out_lo = out - trunc_tf32(out); exact Mish
+    float* out; int B, H, W, C;
+    int form;                   // FORM_TF32 | FORM_X3 | FORM_BF16
+    float* out_lo;              // FORM_X3: the correction twin of out
 };
 
 struct FirstConvParams {        // Block.conv of downs.0.0.block1 on the planar stack([mu, xt(, s)]) * mask
@@ -125,10 +132,9 @@ struct ResFinalParams {         // out = Mish(GN(h2raw))*mask + res(x*mask)
     const float* mask; int T; int lvl;
     float* out;
     int B, H, W, C;
-    int out_mask;               // store out*mask (operand form for the next conv)
-    int chw4;                   // activations are [B][H][C/4][W][4] (tensor-core modes) instead of NHWC
-    int bf16;                   // x and out are bf16 [B][H][C/8][W][8]; h2raw stays fp32 [B][H][C/4][W][4]
-    float* out_lo;              // fp32x3 mode: also write out - trunc_tf32(out); exact Mish
+    int out_mask;               // planar first block in a tensor-core form: store out*mask (operand form for the next conv)
+    int form;                   // layout and number form of x and out (enum Form)
+    float* out_lo;              // FORM_X3: the correction twin of out
 };
 
 struct AttnCtxParams {          // merge per-tile softmax partials -> normalised context [B][4][32][32]

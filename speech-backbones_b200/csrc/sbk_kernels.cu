@@ -12,6 +12,7 @@
 #include "sbk_internal.h"
 
 #include <math.h>
+#include <type_traits>
 
 namespace sbk {
 
@@ -235,11 +236,10 @@ __global__ void __launch_bounds__(IG_THREADS, 3) k_igemm(const IgemmParams p) {
     // ---- epilogue
     float bia[8];
     {
-        const float* bp = p.bias ? p.bias + (long long)b * p.bias_bstride : nullptr;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            bia[j] = bp ? bp[n0 + tx * 4 + j] : 0.f;
-            bia[4 + j] = bp ? bp[n0 + 32 + tx * 4 + j] : 0.f;
+            bia[j] = p.bias ? p.bias[n0 + tx * 4 + j] : 0.f;
+            bia[4 + j] = p.bias ? p.bias[n0 + 32 + tx * 4 + j] : 0.f;
         }
     }
 
@@ -336,11 +336,6 @@ __global__ void __launch_bounds__(IG_THREADS, 3) k_igemm(const IgemmParams p) {
                 st_s[0] += v[j]; st_q[0] = fmaf(v[j], v[j], st_q[0]);
                 st_s[1] += v[4 + j]; st_q[1] = fmaf(v[4 + j], v[4 + j], st_q[1]);
             }
-        }
-        if (p.out_mask) {
-            const float mo = __ldg(p.mask + (long long)b * p.T + ((long long)wo << p.out_lvl));
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] *= mo;
         }
         *reinterpret_cast<float4*>(op + tx * 4) = make_float4(v[0], v[1], v[2], v[3]);
         *reinterpret_cast<float4*>(op + 32 + tx * 4) = make_float4(v[4], v[5], v[6], v[7]);
@@ -503,9 +498,9 @@ int launch_first_conv(const FirstConvParams& p, cudaStream_t s) {
 // ResnetBlock tail for identity / planar-input residuals (ResnetBlock.forward, diffusion.py:77-78):
 //   out = Mish(GN(h2raw))*mask + x*mask                      (dim == dim_out)
 //   out = Mish(GN(h2raw))*mask + W_res (in*mask) + b_res     (first block, planar cin = 2|3)
+// This kernel is the fp32 CUDA-core mode's (NHWC activations, exact Mish); k_resfinal below serves the tensor-core forms.
 // ----------------------------------------------------------------------------------------------
-template <bool X3>
-__global__ void __launch_bounds__(256) k_resfinal(const ResFinalParams p) {
+__global__ void __launch_bounds__(256) k_resfinal_nhwc(const ResFinalParams p) {
     extern __shared__ __align__(16) float sm[];
     float* mean = sm; float* scale = mean + p.C; float* beta = scale + p.C;
     float* wres = beta + p.C;            // [cin][C] + [C] bias when planar
@@ -520,46 +515,6 @@ __global__ void __launch_bounds__(256) k_resfinal(const ResFinalParams p) {
     __syncthreads();
     const int c4n = p.C >> 2;
     const long long n4 = (long long)p.H * p.W * c4n;
-    if (p.x && p.chw4) {
-        // planar layout, identity residual: one channel chunk per CTA, walking mel bins (see k_gn_act)
-        constexpr int U = 4;
-        const int ch = blockIdx.x % c4n, hg = blockIdx.x / c4n, nhg = gridDim.x / c4n;
-        const int tw = p.W >= 256 ? 256 : p.W, nsub = 256 / tw, sub = tid / tw, wl = tid - sub * tw;
-        if (sub >= nsub) return;
-        const float4 pm = reinterpret_cast<const float4*>(mean)[ch], ps = reinterpret_cast<const float4*>(scale)[ch];
-        const float4 pb = reinterpret_cast<const float4*>(beta)[ch];
-        const long long base = ((long long)b * n4 + (long long)ch * p.W) * 4;
-        const float* hb = p.h2raw + base; const float* xb = p.x + base; float* outb = p.out + base;
-        const int hstride = c4n * p.W * 4;
-        for (int w = wl; w < p.W; w += tw) {
-            const float mk = __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl));
-            for (int h0 = (hg * nsub + sub) * U; h0 < p.H; h0 += nhg * nsub * U) {
-                float4 r[U], xv[U];
-#pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    const bool live = mk != 0.f && h0 + u < p.H;
-                    const long long off = (long long)(h0 + u) * hstride + w * 4;
-                    r[u] = live ? ldg4(hb + off) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    xv[u] = live ? ldg4(xb + off) : make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-#pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    if (h0 + u >= p.H) continue;
-                    float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (mk != 0.f) {
-                        o.x = mish_sel<X3>((r[u].x - pm.x) * ps.x + pb.x) + xv[u].x;
-                        o.y = mish_sel<X3>((r[u].y - pm.y) * ps.y + pb.y) + xv[u].y;
-                        o.z = mish_sel<X3>((r[u].z - pm.z) * ps.z + pb.z) + xv[u].z;
-                        o.w = mish_sel<X3>((r[u].w - pm.w) * ps.w + pb.w) + xv[u].w;
-                    }
-                    *reinterpret_cast<float4*>(outb + (long long)(h0 + u) * hstride + w * 4) = o;
-                    if (X3) *reinterpret_cast<float4*>(p.out_lo + base + (long long)(h0 + u) * hstride + w * 4) =
-                                corr_chunk(o.x, o.y, o.z, o.w);
-                }
-            }
-        }
-        return;
-    }
     if (p.x) {
         // identity residual: pure streaming (2 reads + 1 write per element); 4 independent units per thread
         constexpr int U = 4;
@@ -571,15 +526,9 @@ __global__ void __launch_bounds__(256) k_resfinal(const ResFinalParams p) {
                 in[u] = i < n4;
                 int c = 0, w = 0;
                 if (in[u]) {
-                    if (p.chw4) {
-                        const long long hc = i / p.W;
-                        w = (int)(i - hc * p.W);
-                        c = (int)(hc % c4n) * 4;
-                    } else {
-                        const long long pix = i / c4n;
-                        c = (int)(i - pix * c4n) * 4;
-                        w = (int)(pix % p.W);
-                    }
+                    const long long pix = i / c4n;
+                    c = (int)(i - pix * c4n) * 4;
+                    w = (int)(pix % p.W);
                 }
                 cc[u] = c;
                 mk[u] = in[u] ? __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl)) : 0.f;
@@ -597,53 +546,166 @@ __global__ void __launch_bounds__(256) k_resfinal(const ResFinalParams p) {
                     const float rv[4] = {r[u].x, r[u].y, r[u].z, r[u].w};
                     const float xx[4] = {xv[u].x, xv[u].y, xv[u].z, xv[u].w};
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        const float xn = (rv[q] - mean[c + q]) * scale[c + q] + beta[c + q];
-                        o[q] = (p.chw4 ? mish_fast_f(xn) : mish_f(xn)) + xx[q];
-                    }
+                    for (int q = 0; q < 4; ++q) o[q] = mish_f((rv[q] - mean[c + q]) * scale[c + q] + beta[c + q]) + xx[q];
                 }
                 *reinterpret_cast<float4*>(p.out + ((long long)b * n4 + i0 + u * 256) * 4) = make_float4(o[0], o[1], o[2], o[3]);
             }
         }
         return;
     }
-    if (p.chw4) {
-        // planar layout, res_conv over the 2-3 network inputs (first ResnetBlock): one channel chunk per CTA (see k_gn_act)
-        constexpr int U = 4;
-        const int ch = blockIdx.x % c4n, hg = blockIdx.x / c4n, nhg = gridDim.x / c4n;
-        const int tw = p.W >= 256 ? 256 : p.W, nsub = 256 / tw, sub = tid / tw, wl = tid - sub * tw;
-        if (sub >= nsub) return;
-        const int nreal = p.r_extra ? p.cin - 1 : p.cin;
-        const float* re = p.r_extra ? p.r_extra + ((long long)(p.extra_per_sample_row ? 0 : *p.step) * p.B + b) * p.C : nullptr;
-        const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        const float4 pm = reinterpret_cast<const float4*>(mean)[ch], ps = reinterpret_cast<const float4*>(scale)[ch];
-        const float4 pb = reinterpret_cast<const float4*>(beta)[ch];
-        const float4 wb = reinterpret_cast<const float4*>(wres + p.cin * p.C)[ch];
-        const float4 w0 = reinterpret_cast<const float4*>(wres)[ch];
-        const float4 w1 = nreal > 1 ? reinterpret_cast<const float4*>(wres + p.C)[ch] : z4;
-        const float4 w2 = nreal > 2 ? reinterpret_cast<const float4*>(wres + 2 * p.C)[ch] : z4;
-        const float4 rx = re ? ldg4(re + ch * 4) : z4;
-        const bool has_spk = p.cin > 2 && !p.r_extra;
-        const long long base = ((long long)b * n4 + (long long)ch * p.W) * 4;
-        const float* hb = p.h2raw + base; float* outb = p.out + base;
-        const int hstride = c4n * p.W * 4;
-        for (int w = wl; w < p.W; w += tw) {
-            const float mk = __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl));
-            for (int h0 = (hg * nsub + sub) * U; h0 < p.H; h0 += nhg * nsub * U) {
-                float4 r[U]; float i0[U], i1[U], i2[U];
+    const int nreal = p.r_extra ? p.cin - 1 : p.cin;
+    const float* re = p.r_extra ? p.r_extra + ((long long)(p.extra_per_sample_row ? 0 : *p.step) * p.B + b) * p.C : nullptr;
+    for (long long i = (long long)blockIdx.x * 256 + tid; i < n4; i += (long long)gridDim.x * 256) {
+        // float4 unit i of this sample -> (pixel, channel quad)
+        const long long pix = i / c4n;
+        const int c = (int)(i - pix * c4n) * 4, w = (int)(pix % p.W), h = (int)(pix / p.W);
+        const float mk = __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl));
+        const long long off = ((long long)b * n4 + i) * 4;
+        float o[4] = {0.f, 0.f, 0.f, 0.f};
+        if (mk != 0.f) {
+            const float4 r = ldg4(p.h2raw + off);
+            const float rv[4] = {r.x, r.y, r.z, r.w};
 #pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    const bool live = mk != 0.f && h0 + u < p.H;
+            for (int q = 0; q < 4; ++q) o[q] = mish_f((rv[q] - mean[c + q]) * scale[c + q] + beta[c + q]);
+        }
+        const long long idx = ((long long)b * p.H + h) * p.T + w;
+        float in[3];
+        in[0] = __ldg(p.mu + idx) * mk;
+        in[1] = __ldg(p.xt + idx) * mk;
+        in[2] = (p.cin > 2 && !p.r_extra) ? __ldg(p.spk_s + b * p.H + h) * mk : 0.f;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            float a = wres[p.cin * p.C + c + q];
+#pragma unroll
+            for (int ci = 0; ci < 3; ++ci)
+                if (ci < nreal) a = fmaf(in[ci], wres[ci * p.C + c + q], a);
+            if (re) a = fmaf(mk, __ldg(re + c + q), a);
+            o[q] += a;
+        }
+        *reinterpret_cast<float4*>(p.out + off) = make_float4(o[0], o[1], o[2], o[3]);
+    }
+}
+
+// ----------------------------------------------------------------------------------------------
+// Element-wise kernels of the tensor-core forms (enum Form), over planar tensors: the Block activation
+//   k_gn_act:    act = mask ? Mish(GN(raw)) + tproj : 0
+// (Block.forward output * mask, then ResnetBlock's time projection, then the next Block's input mask: diffusion.py:56-58,76;
+//  one read + one write per element, so the conv's A path is a pure copy), and the ResnetBlock tail
+//   k_resfinal:  out = mask ? Mish(GN(h2raw)) + x : 0                                   (identity residual)
+//                out = (W_res (in*mask) + b_res + (mask ? Mish(GN(h2raw)) : 0)) (*mask)  (first block: planar inputs)
+// A CTA owns ONE output channel chunk, whose GN / time / residual parameters live in registers for the whole kernel, and
+// walks mel bins 4 at a time; a thread owns frame(s) w, so the mask is read once and every index is 32-bit and
+// division-free (a generic flat loop was issue-bound on 64-bit divisions).  In the fp32 forms a chunk is 4 channels and a
+// lane owns a frame.  In bf16 a chunk is 8 channels and a LANE PAIR owns a frame: lane half h handles the fp32 raw chunk
+// 2*ch+h (the same register footprint as the fp32 forms) and writes its 8-byte half of the 16-byte bf16 chunk, so loads are
+// two interleaved 256-byte runs per warp and stores one contiguous 256-byte run.
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t pack_bf16x2_f(float lo, float hi) {
+    uint32_t d;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
+    return d;
+}
+__device__ __forceinline__ float bf16_lo_f(uint32_t u) { return __uint_as_float(u << 16); }
+__device__ __forceinline__ float bf16_hi_f(uint32_t u) { return __uint_as_float(u & 0xFFFF0000u); }
+__device__ __forceinline__ float4 opnd_f32(float4 v) { return v; }
+__device__ __forceinline__ float4 opnd_f32(uint2 v) { return make_float4(bf16_lo_f(v.x), bf16_hi_f(v.x), bf16_lo_f(v.y), bf16_hi_f(v.y)); }
+__device__ __forceinline__ float rna_tf32(float x) {
+    uint32_t t;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t) : "f"(x));
+    return __uint_as_float(t);
+}
+
+enum Tail { TAIL_ACT, TAIL_ID, TAIL_PLANAR };
+__host__ __device__ constexpr int lanes_per_frame(int form) { return form == FORM_BF16 ? 2 : 1; }
+
+// grid.x = (channel chunks) x (mel-bin groups); a 256-thread CTA covers min(W, F) frames x F / min(W, F) bin sub-groups
+// (F = 256 / lanes per frame), each walking 4 bins per pass, ~2 passes per thread
+static int planar_ew_grid(int form, int H, int W, int C) {
+    const int lanes = lanes_per_frame(form), F = 256 / lanes;
+    const int nsub = W >= F ? 1 : F / W;
+    int nhg = (H + 8 * nsub - 1) / (8 * nsub);
+    if (nhg < 1) nhg = 1;
+    return C / (4 * lanes) * nhg;
+}
+
+template <int FORM, int TAIL, class P>
+__device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
+    constexpr bool B16 = FORM == FORM_BF16, X3 = FORM == FORM_X3;
+    constexpr int LPF = lanes_per_frame(FORM), F = 256 / LPF;
+    constexpr int U = 4;                         // independent 16-byte loads in flight per thread
+    using Unit = typename std::conditional<B16, uint2, float4>::type;   // a thread's 4 channels of an operand tensor
+    extern __shared__ __align__(16) float sm[];
+    float* mean = sm; float* scale = mean + p.C; float* beta = scale + p.C;
+    float* ext = beta + p.C;                     // TAIL_ACT: time projection [C]; TAIL_PLANAR: res_conv [cin][C] + bias [C]
+    const int b = blockIdx.y, tid = threadIdx.x;
+    gn_fill(p.gn, b, p.C, 0, p.C, mean, scale, beta);
+    if constexpr (TAIL == TAIL_ACT) {
+        const int row = p.tb_per_sample ? b : *p.step;
+        const float* tb = p.tb + (long long)row * p.tb_stride;
+        for (int c = tid; c < p.C; c += 256) ext[c] = tb[c];
+    } else if constexpr (TAIL == TAIL_PLANAR) {
+        // rows [0, nreal) = shared res_conv weights of the planar channels, row cin = bias (rows in between unused)
+        const int nreal = p.r_extra ? p.cin - 1 : p.cin;
+        for (int i = tid; i < (p.cin + 1) * p.C; i += 256)
+            ext[i] = i < nreal * p.C ? p.wres[i] : (i >= p.cin * p.C ? p.bres[i - p.cin * p.C] : 0.f);
+    }
+    __syncthreads();
+    const int c4n = p.C >> 2, ncc = p.C >> (1 + LPF);                  // fp32 chunks, output chunks
+    const int ch = blockIdx.x % ncc, hg = blockIdx.x / ncc, nhg = gridDim.x / ncc;
+    const int half = tid & (LPF - 1), q = tid >> (LPF - 1);
+    const int tw = p.W >= F ? F : p.W, nsub = F / tw, sub = q / tw, wl = q - sub * tw;
+    if (sub >= nsub) return;
+    const int c4 = LPF * ch + half;                                      // this thread's fp32 chunk
+    const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 pm = reinterpret_cast<const float4*>(mean)[c4], ps = reinterpret_cast<const float4*>(scale)[c4];
+    const float4 pb = reinterpret_cast<const float4*>(beta)[c4];
+    const float* rawb = raw + ((long long)b * p.H * c4n + c4) * p.W * 4;
+    const int hs4 = c4n * p.W * 4;                                       // floats between mel bins (raw)
+    // out and the identity residual x, in Units: mel bins are c4n * W Units apart in every form, frames LPF Units
+    const long long obase = B16 ? ((long long)b * p.H * ncc + ch) * p.W * 2 + half : ((long long)b * p.H * c4n + c4) * p.W;
+    const int ohs = c4n * p.W;
+    float4 pt = z4, rx = z4;
+    bool has_spk = false;
+    if constexpr (TAIL == TAIL_ACT) pt = reinterpret_cast<const float4*>(ext)[c4];
+    if constexpr (TAIL == TAIL_PLANAR) {
+        // first ResnetBlock: res_conv over the 2-3 planar network inputs (+ DiffVC's folded conditioning channel)
+        if (p.r_extra) rx = ldg4(p.r_extra + ((long long)(p.extra_per_sample_row ? 0 : *p.step) * p.B + b) * p.C + c4 * 4);
+        has_spk = p.cin > 2 && !p.r_extra;      // = a third real weight row
+    }
+    // this chunk's res_conv bias and weight rows: bf16, whose launch bounds leave room, holds them in registers; the fp32
+    // forms re-read them from shared memory per element (broadcast loads), which keeps them under the registers of the
+    // fp32 kernels this walk replaced
+    float4 wb = z4, w0 = z4, w1 = z4, w2 = z4;
+    auto res_w = [&](const auto& q) {             // q = p (generic, so that only TAIL_PLANAR instantiates it)
+        wb = reinterpret_cast<const float4*>(ext + q.cin * q.C)[c4];
+        w0 = reinterpret_cast<const float4*>(ext)[c4];
+        w1 = reinterpret_cast<const float4*>(ext + q.C)[c4];
+        w2 = has_spk ? reinterpret_cast<const float4*>(ext + 2 * q.C)[c4] : z4;
+    };
+    if constexpr (TAIL == TAIL_PLANAR && B16) res_w(p);
+    for (int w = wl; w < p.W; w += tw) {
+        const float mk = __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl));
+        for (int h0 = (hg * nsub + sub) * U; h0 < p.H; h0 += nhg * nsub * U) {
+            float4 r[U]; Unit xv[U]; float i0[U], i1[U], i2[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const bool live = mk != 0.f && h0 + u < p.H;
+                r[u] = live ? ldg4(rawb + (long long)(h0 + u) * hs4 + w * 4) : z4;
+                if constexpr (TAIL == TAIL_ID)
+                    xv[u] = live ? __ldg(reinterpret_cast<const Unit*>(p.x) + obase + (long long)(h0 + u) * ohs + w * LPF) : Unit{};
+                if constexpr (TAIL == TAIL_PLANAR) {
                     const long long idx = ((long long)b * p.H + h0 + u) * p.T + w;
-                    r[u] = live ? ldg4(hb + (long long)(h0 + u) * hstride + w * 4) : z4;
                     i0[u] = live ? __ldg(p.mu + idx) * mk : 0.f;
                     i1[u] = live ? __ldg(p.xt + idx) * mk : 0.f;
                     i2[u] = (live && has_spk) ? __ldg(p.spk_s + b * p.H + h0 + u) * mk : 0.f;
                 }
+            }
 #pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    if (h0 + u >= p.H) continue;
-                    float4 o;
+            for (int u = 0; u < U; ++u) {
+                if (h0 + u >= p.H) continue;
+                float4 o = z4;
+                if constexpr (TAIL == TAIL_PLANAR) {
+                    if constexpr (!B16) res_w(p);
                     o.x = fmaf(mk, rx.x, fmaf(i2[u], w2.x, fmaf(i1[u], w1.x, fmaf(i0[u], w0.x, wb.x))));
                     o.y = fmaf(mk, rx.y, fmaf(i2[u], w2.y, fmaf(i1[u], w1.y, fmaf(i0[u], w0.y, wb.y))));
                     o.z = fmaf(mk, rx.z, fmaf(i2[u], w2.z, fmaf(i1[u], w1.z, fmaf(i0[u], w0.z, wb.z))));
@@ -655,391 +717,70 @@ __global__ void __launch_bounds__(256) k_resfinal(const ResFinalParams p) {
                         o.w += mish_sel<X3>((r[u].w - pm.w) * ps.w + pb.w);
                     }
                     if (p.out_mask) { o.x *= mk; o.y *= mk; o.z *= mk; o.w *= mk; }
-                    *reinterpret_cast<float4*>(outb + (long long)(h0 + u) * hstride + w * 4) = o;
-                    if (X3) *reinterpret_cast<float4*>(p.out_lo + base + (long long)(h0 + u) * hstride + w * 4) =
-                                corr_chunk(o.x, o.y, o.z, o.w);
+                } else if (mk != 0.f) {
+                    float4 a;
+                    if constexpr (TAIL == TAIL_ACT) a = pt; else a = opnd_f32(xv[u]);
+                    o.x = mish_sel<X3>((r[u].x - pm.x) * ps.x + pb.x) + a.x;
+                    o.y = mish_sel<X3>((r[u].y - pm.y) * ps.y + pb.y) + a.y;
+                    o.z = mish_sel<X3>((r[u].z - pm.z) * ps.z + pb.z) + a.z;
+                    o.w = mish_sel<X3>((r[u].w - pm.w) * ps.w + pb.w) + a.w;
+                    if constexpr (FORM == FORM_TF32 && TAIL == TAIL_ACT) o = make_float4(rna_tf32(o.x), rna_tf32(o.y), rna_tf32(o.z), rna_tf32(o.w));
                 }
-            }
-        }
-        return;
-    }
-    for (long long i = (long long)blockIdx.x * 256 + tid; i < n4; i += (long long)gridDim.x * 256) {
-        // float4 unit i of this sample -> (pixel, channel quad); in both layouts the unit index IS the memory order
-        long long pix; int c, w;
-        if (p.chw4) {
-            const long long hc = i / p.W;                    // (h, chunk)
-            w = (int)(i - hc * p.W);
-            const int h = (int)(hc / c4n);
-            c = (int)(hc - (long long)h * c4n) * 4;
-            pix = (long long)h * p.W + w;
-        } else {
-            pix = i / c4n;
-            c = (int)(i - pix * c4n) * 4;
-            w = (int)(pix % p.W);
-        }
-        const float mk = __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl));
-        const long long off = ((long long)b * n4 + i) * 4;
-        float o[4] = {0.f, 0.f, 0.f, 0.f};
-        if (mk != 0.f) {
-            const float4 r = ldg4(p.h2raw + off);
-            const float rv[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-            for (int q = 0; q < 4; ++q) o[q] = mish_f((rv[q] - mean[c + q]) * scale[c + q] + beta[c + q]);
-        }
-        if (p.x) {
-            if (mk != 0.f) {
-                const float4 xv = ldg4(p.x + off);
-                o[0] += xv.x; o[1] += xv.y; o[2] += xv.z; o[3] += xv.w;
-            }
-        } else {
-            const int h = (int)(pix / p.W);
-            const long long idx = ((long long)b * p.H + h) * p.T + w;
-            float in[3];
-            in[0] = __ldg(p.mu + idx) * mk;
-            in[1] = __ldg(p.xt + idx) * mk;
-            in[2] = (p.cin > 2 && !p.r_extra) ? __ldg(p.spk_s + b * p.H + h) * mk : 0.f;
-            const int nreal = p.r_extra ? p.cin - 1 : p.cin;
-            const float* re = nullptr;
-            if (p.r_extra) re = p.r_extra + ((long long)(p.extra_per_sample_row ? 0 : *p.step) * p.B + b) * p.C;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                float a = wres[p.cin * p.C + c + q];
-                for (int ci = 0; ci < nreal; ++ci) a = fmaf(in[ci], wres[ci * p.C + c + q], a);
-                if (re) a = fmaf(mk, __ldg(re + c + q), a);
-                o[q] += a;
-            }
-        }
-        if (p.out_mask) { o[0] *= mk; o[1] *= mk; o[2] *= mk; o[3] *= mk; }
-        *reinterpret_cast<float4*>(p.out + off) = make_float4(o[0], o[1], o[2], o[3]);
-    }
-}
-
-// Block activation in operand form for the tensor-core convs:  act = mask ? Mish(GN(raw)) + tproj : 0
-// (Block.forward output * mask, then ResnetBlock's time projection, then the next Block's input mask:
-//  diffusion.py:56-58,76).  One read + one write per element; the conv's A path is then a pure copy.
-template <bool X3>
-__global__ void __launch_bounds__(256) k_gn_act(const GnActParams p) {
-    extern __shared__ __align__(16) float sm[];
-    float* mean = sm; float* scale = mean + p.C; float* beta = scale + p.C; float* tbv = beta + p.C;
-    const int b = blockIdx.y, tid = threadIdx.x;
-    gn_fill(p.gn, b, p.C, 0, p.C, mean, scale, beta);
-    {
-        const int row = p.tb_per_sample ? b : *p.step;
-        const float* tb = p.tb + (long long)row * p.tb_stride;
-        for (int c = tid; c < p.C; c += 256) tbv[c] = tb[c];
-    }
-    __syncthreads();
-    const int c4n = p.C >> 2;
-    const long long n4 = (long long)p.H * p.W * c4n;
-    constexpr int U = 4;                         // independent 16-byte loads in flight per thread
-    if (p.chw4) {
-        // planar layout: a CTA owns ONE channel chunk (4 channels: their GN / time parameters live in registers for the
-        // whole kernel) and walks mel bins, 4 at a time; a thread owns frame(s) w, so the mask is read once and every
-        // index is 32-bit and division-free (the generic loop below was issue-bound on 64-bit divisions).
-        const int ch = blockIdx.x % c4n, hg = blockIdx.x / c4n, nhg = gridDim.x / c4n;
-        const int tw = p.W >= 256 ? 256 : p.W, nsub = 256 / tw, sub = tid / tw, wl = tid - sub * tw;
-        if (sub >= nsub) return;
-        const float4 pm = reinterpret_cast<const float4*>(mean)[ch], ps = reinterpret_cast<const float4*>(scale)[ch];
-        const float4 pb = reinterpret_cast<const float4*>(beta)[ch], pt = reinterpret_cast<const float4*>(tbv)[ch];
-        const float* rawb = p.raw + ((long long)b * n4 + (long long)ch * p.W) * 4;
-        float* outb = p.out + ((long long)b * n4 + (long long)ch * p.W) * 4;
-        float* lob = X3 ? p.out_lo + ((long long)b * n4 + (long long)ch * p.W) * 4 : nullptr;
-        const int hstride = c4n * p.W * 4;                               // floats between consecutive mel bins of one chunk
-        for (int w = wl; w < p.W; w += tw) {
-            const float mk = __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl));
-            for (int h0 = (hg * nsub + sub) * U; h0 < p.H; h0 += nhg * nsub * U) {
-                float4 r[U];
-#pragma unroll
-                for (int u = 0; u < U; ++u)
-                    r[u] = (mk != 0.f && h0 + u < p.H) ? ldg4(rawb + (long long)(h0 + u) * hstride + w * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    if (h0 + u >= p.H) continue;
-                    float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (mk != 0.f) {
-                        o.x = mish_sel<X3>((r[u].x - pm.x) * ps.x + pb.x) + pt.x;
-                        o.y = mish_sel<X3>((r[u].y - pm.y) * ps.y + pb.y) + pt.y;
-                        o.z = mish_sel<X3>((r[u].z - pm.z) * ps.z + pb.z) + pt.z;
-                        o.w = mish_sel<X3>((r[u].w - pm.w) * ps.w + pb.w) + pt.w;
-                        if (!X3 && p.round_tf32) {
-                            uint32_t t0, t1, t2, t3;
-                            asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t0) : "f"(o.x)); asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t1) : "f"(o.y));
-                            asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t2) : "f"(o.z)); asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t3) : "f"(o.w));
-                            o = make_float4(__uint_as_float(t0), __uint_as_float(t1), __uint_as_float(t2), __uint_as_float(t3));
-                        }
-                    }
-                    *reinterpret_cast<float4*>(outb + (long long)(h0 + u) * hstride + w * 4) = o;
-                    if (X3) *reinterpret_cast<float4*>(lob + (long long)(h0 + u) * hstride + w * 4) =
-                                corr_chunk(o.x, o.y, o.z, o.w);
-                }
-            }
-        }
-        return;
-    }
-    for (long long i0 = (long long)blockIdx.x * (256 * U) + tid; i0 < n4; i0 += (long long)gridDim.x * (256 * U)) {
-        float4 r[U]; float mk[U]; int cc[U]; bool in[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const long long i = i0 + u * 256;
-            in[u] = i < n4;
-            int c = 0, w = 0;
-            if (in[u]) {
-                if (p.chw4) {
-                    const long long hc = i / p.W;
-                    w = (int)(i - hc * p.W);
-                    c = (int)(hc % c4n) * 4;
+                const long long oi = obase + (long long)(h0 + u) * ohs + w * LPF;
+                if constexpr (B16) {
+                    reinterpret_cast<uint2*>(p.out)[oi] = make_uint2(pack_bf16x2_f(o.x, o.y), pack_bf16x2_f(o.z, o.w));
                 } else {
-                    const long long pix = i / c4n;
-                    c = (int)(i - pix * c4n) * 4;
-                    w = (int)(pix % p.W);
+                    reinterpret_cast<float4*>(p.out)[oi] = o;
+                    if constexpr (X3) reinterpret_cast<float4*>(p.out_lo)[oi] = corr_chunk(o.x, o.y, o.z, o.w);
                 }
-            }
-            cc[u] = c;
-            mk[u] = in[u] ? __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl)) : 0.f;
-            r[u] = (in[u] && mk[u] != 0.f) ? ldg4(p.raw + ((long long)b * n4 + i) * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-            if (!in[u]) continue;
-            const int c = cc[u];
-            float o[4] = {0.f, 0.f, 0.f, 0.f};
-            if (mk[u] != 0.f) {
-                const float rv[4] = {r[u].x, r[u].y, r[u].z, r[u].w};
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const float xn = (rv[q] - mean[c + q]) * scale[c + q] + beta[c + q];
-                    float y = (p.chw4 ? mish_fast_f(xn) : mish_f(xn)) + tbv[c + q];
-                    if (p.round_tf32) { uint32_t t; asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t) : "f"(y)); y = __uint_as_float(t); }
-                    o[q] = y;
-                }
-            }
-            *reinterpret_cast<float4*>(p.out + ((long long)b * n4 + i0 + u * 256) * 4) = make_float4(o[0], o[1], o[2], o[3]);
-        }
-    }
-}
-
-// ----------------------------------------------------------------------------------------------
-// bf16 operand tensors (precision = bf16): [B][H][C/8][W][8], one 16-byte chunk = 8 channels of one pixel.
-// Raw conv outputs (the GroupNorm inputs) stay fp32 [B][H][C/4][W][4], so an 8-channel output chunk is fed by
-// two fp32 chunks.  Same walk as the planar fp32 kernels: a CTA owns one output chunk (its GN / time / residual
-// parameters live in registers), a thread owns frame(s) w and walks mel bins four at a time.
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t pack_bf16x2_f(float lo, float hi) {
-    uint32_t d;
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
-    return d;
-}
-__device__ __forceinline__ float bf16_lo_f(uint32_t u) { return __uint_as_float(u << 16); }
-__device__ __forceinline__ float bf16_hi_f(uint32_t u) { return __uint_as_float(u & 0xFFFF0000u); }
-
-// Thread mapping of the two kernels below: a LANE PAIR owns one frame - lane half h handles the fp32 chunk 2*ch+h
-// (4 channels: the same register footprint as the fp32 kernels, so the same 4 CTAs/SM) and writes its 8-byte half of
-// the 16-byte bf16 chunk: loads are two interleaved 256-byte runs per warp, stores one contiguous 256-byte run.
-__global__ void __launch_bounds__(256) k_gn_act_bf16(const GnActParams p) {
-    extern __shared__ __align__(16) float sm[];
-    float* mean = sm; float* scale = mean + p.C; float* beta = scale + p.C; float* tbv = beta + p.C;
-    const int b = blockIdx.y, tid = threadIdx.x;
-    gn_fill(p.gn, b, p.C, 0, p.C, mean, scale, beta);
-    {
-        const int row = p.tb_per_sample ? b : *p.step;
-        const float* tb = p.tb + (long long)row * p.tb_stride;
-        for (int c = tid; c < p.C; c += 256) tbv[c] = tb[c];
-    }
-    __syncthreads();
-    constexpr int U = 4;
-    const int c4n = p.C >> 2, c8n = p.C >> 3;
-    const int ch = blockIdx.x % c8n, hg = blockIdx.x / c8n, nhg = gridDim.x / c8n;
-    const int half = tid & 1, q = tid >> 1;
-    const int tw = p.W >= 128 ? 128 : p.W, nsub = 128 / tw, sub = q / tw, wl = q - sub * tw;
-    if (sub >= nsub) return;
-    const int c4 = 2 * ch + half;                                                    // this thread's fp32 chunk
-    const float4 pm = reinterpret_cast<const float4*>(mean)[c4], ps = reinterpret_cast<const float4*>(scale)[c4];
-    const float4 pb = reinterpret_cast<const float4*>(beta)[c4], pt = reinterpret_cast<const float4*>(tbv)[c4];
-    const float* rawb = p.raw + ((long long)b * p.H * c4n + c4) * p.W * 4;
-    uint2* outb = reinterpret_cast<uint2*>(p.out) + (((long long)b * p.H * c8n + ch) * p.W) * 2 + half;
-    const int hs4 = c4n * p.W * 4;                                                   // floats between mel bins (raw)
-    const int hs8 = c8n * p.W * 2;                                                   // 8-byte units between mel bins (out)
-    for (int w = wl; w < p.W; w += tw) {
-        const float mk = __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl));
-        for (int h0 = (hg * nsub + sub) * U; h0 < p.H; h0 += nhg * nsub * U) {
-            float4 r[U];
-#pragma unroll
-            for (int u = 0; u < U; ++u)
-                r[u] = (mk != 0.f && h0 + u < p.H) ? ldg4(rawb + (long long)(h0 + u) * hs4 + w * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                if (h0 + u >= p.H) continue;
-                uint2 o = make_uint2(0u, 0u);
-                if (mk != 0.f) {
-                    const float y0 = mish_fast_f((r[u].x - pm.x) * ps.x + pb.x) + pt.x;
-                    const float y1 = mish_fast_f((r[u].y - pm.y) * ps.y + pb.y) + pt.y;
-                    const float y2 = mish_fast_f((r[u].z - pm.z) * ps.z + pb.z) + pt.z;
-                    const float y3 = mish_fast_f((r[u].w - pm.w) * ps.w + pb.w) + pt.w;
-                    o = make_uint2(pack_bf16x2_f(y0, y1), pack_bf16x2_f(y2, y3));
-                }
-                outb[(long long)(h0 + u) * hs8 + w * 2] = o;
             }
         }
     }
 }
 
-// ResnetBlock tail with bf16 operand tensors: out = Mish(GN(h2raw))*mask + x*mask (identity residual, x bf16) or
-// + W_res(in*mask) + b_res over the planar network inputs (first block).  Same contract as k_resfinal.
-// (PLANAR is a template parameter so that the streaming identity variant does not pay the planar variant's registers.)
-template <bool PLANAR>
-__global__ void __launch_bounds__(256, PLANAR ? 2 : 4) k_resfinal_bf16(const ResFinalParams p) {
-    extern __shared__ __align__(16) float sm[];
-    float* mean = sm; float* scale = mean + p.C; float* beta = scale + p.C;
-    float* wres = beta + p.C;            // [cin][C] + [C] bias when planar
-    const int b = blockIdx.y, tid = threadIdx.x;
-    gn_fill(p.gn, b, p.C, 0, p.C, mean, scale, beta);
-    if constexpr (PLANAR) {
-        const int nreal = p.r_extra ? p.cin - 1 : p.cin;
-        for (int i = tid; i < (p.cin + 1) * p.C; i += 256)
-            wres[i] = i < nreal * p.C ? p.wres[i] : (i >= p.cin * p.C ? p.bres[i - p.cin * p.C] : 0.f);
-    }
-    __syncthreads();
-    constexpr int U = 4;
-    const int c4n = p.C >> 2, c8n = p.C >> 3;
-    const int ch = blockIdx.x % c8n, hg = blockIdx.x / c8n, nhg = gridDim.x / c8n;
-    const int half = tid & 1, q = tid >> 1;
-    const int tw = p.W >= 128 ? 128 : p.W, nsub = 128 / tw, sub = q / tw, wl = q - sub * tw;
-    if (sub >= nsub) return;
-    const int c4 = 2 * ch + half;
-    const float4 pm = reinterpret_cast<const float4*>(mean)[c4], ps = reinterpret_cast<const float4*>(scale)[c4];
-    const float4 pb = reinterpret_cast<const float4*>(beta)[c4];
-    const float* hb = p.h2raw + ((long long)b * p.H * c4n + c4) * p.W * 4;
-    uint2* outb = reinterpret_cast<uint2*>(p.out) + (((long long)b * p.H * c8n + ch) * p.W) * 2 + half;
-    const int hs4 = c4n * p.W * 4, hs8 = c8n * p.W * 2;
-    const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    if constexpr (!PLANAR) {
-        const uint2* xb = reinterpret_cast<const uint2*>(p.x) + (((long long)b * p.H * c8n + ch) * p.W) * 2 + half;
-        for (int w = wl; w < p.W; w += tw) {
-            const float mk = __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl));
-            for (int h0 = (hg * nsub + sub) * U; h0 < p.H; h0 += nhg * nsub * U) {
-                float4 r[U]; uint2 xv[U];
-#pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    const bool live = mk != 0.f && h0 + u < p.H;
-                    r[u] = live ? ldg4(hb + (long long)(h0 + u) * hs4 + w * 4) : z4;
-                    xv[u] = live ? __ldg(xb + (long long)(h0 + u) * hs8 + w * 2) : make_uint2(0u, 0u);
-                }
-#pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    if (h0 + u >= p.H) continue;
-                    uint2 o = make_uint2(0u, 0u);
-                    if (mk != 0.f) {
-                        const float y0 = mish_fast_f((r[u].x - pm.x) * ps.x + pb.x) + bf16_lo_f(xv[u].x);
-                        const float y1 = mish_fast_f((r[u].y - pm.y) * ps.y + pb.y) + bf16_hi_f(xv[u].x);
-                        const float y2 = mish_fast_f((r[u].z - pm.z) * ps.z + pb.z) + bf16_lo_f(xv[u].y);
-                        const float y3 = mish_fast_f((r[u].w - pm.w) * ps.w + pb.w) + bf16_hi_f(xv[u].y);
-                        o = make_uint2(pack_bf16x2_f(y0, y1), pack_bf16x2_f(y2, y3));
-                    }
-                    outb[(long long)(h0 + u) * hs8 + w * 2] = o;
-                }
-            }
-        }
-    } else {
-    // first ResnetBlock: res_conv over the 2-3 planar network inputs (+ DiffVC's folded conditioning channel)
-    const int nreal = p.r_extra ? p.cin - 1 : p.cin;
-    const float* re = p.r_extra ? p.r_extra + ((long long)(p.extra_per_sample_row ? 0 : *p.step) * p.B + b) * p.C : nullptr;
-    const float4 wb = reinterpret_cast<const float4*>(wres + p.cin * p.C)[c4];
-    const float4 w0 = reinterpret_cast<const float4*>(wres)[c4];
-    const float4 w1 = nreal > 1 ? reinterpret_cast<const float4*>(wres + p.C)[c4] : z4;
-    const float4 w2 = nreal > 2 ? reinterpret_cast<const float4*>(wres + 2 * p.C)[c4] : z4;
-    const float4 rx = re ? ldg4(re + c4 * 4) : z4;
-    const bool has_spk = p.cin > 2 && !p.r_extra;
-    for (int w = wl; w < p.W; w += tw) {
-        const float mk = __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl));
-        for (int h0 = (hg * nsub + sub) * U; h0 < p.H; h0 += nhg * nsub * U) {
-            float4 r[U]; float i0[U], i1[U], i2[U];
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const bool live = mk != 0.f && h0 + u < p.H;
-                const long long idx = ((long long)b * p.H + h0 + u) * p.T + w;
-                r[u] = live ? ldg4(hb + (long long)(h0 + u) * hs4 + w * 4) : z4;
-                i0[u] = live ? __ldg(p.mu + idx) * mk : 0.f;
-                i1[u] = live ? __ldg(p.xt + idx) * mk : 0.f;
-                i2[u] = (live && has_spk) ? __ldg(p.spk_s + b * p.H + h0 + u) * mk : 0.f;
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                if (h0 + u >= p.H) continue;
-                float4 o;
-                o.x = fmaf(mk, rx.x, fmaf(i2[u], w2.x, fmaf(i1[u], w1.x, fmaf(i0[u], w0.x, wb.x))));
-                o.y = fmaf(mk, rx.y, fmaf(i2[u], w2.y, fmaf(i1[u], w1.y, fmaf(i0[u], w0.y, wb.y))));
-                o.z = fmaf(mk, rx.z, fmaf(i2[u], w2.z, fmaf(i1[u], w1.z, fmaf(i0[u], w0.z, wb.z))));
-                o.w = fmaf(mk, rx.w, fmaf(i2[u], w2.w, fmaf(i1[u], w1.w, fmaf(i0[u], w0.w, wb.w))));
-                if (mk != 0.f) {
-                    o.x += mish_fast_f((r[u].x - pm.x) * ps.x + pb.x);
-                    o.y += mish_fast_f((r[u].y - pm.y) * ps.y + pb.y);
-                    o.z += mish_fast_f((r[u].z - pm.z) * ps.z + pb.z);
-                    o.w += mish_fast_f((r[u].w - pm.w) * ps.w + pb.w);
-                }
-                if (p.out_mask) { o.x *= mk; o.y *= mk; o.z *= mk; o.w *= mk; }
-                outb[(long long)(h0 + u) * hs8 + w * 2] = make_uint2(pack_bf16x2_f(o.x, o.y), pack_bf16x2_f(o.z, o.w));
-            }
-        }
-    }
-    }
-}
+template <int FORM>
+__global__ void __launch_bounds__(256) k_gn_act(const GnActParams p) { planar_ew<FORM, TAIL_ACT>(p, p.raw); }
 
-// planar elementwise kernels: grid.x = (channel chunks) x (mel-bin groups); a 256-thread CTA covers min(W,256) frames x
-// 256/min(W,256) bin sub-groups, each walking 4 bins per pass, ~2 passes per thread.
-static int planar_ew_grid(int H, int W, int C) {
-    const int nsub = W >= 256 ? 1 : 256 / W;
-    int nhg = (H + 8 * nsub - 1) / (8 * nsub);
-    if (nhg < 1) nhg = 1;
-    return (C / 4) * nhg;
-}
-
-// bf16 kernels: 8-channel chunks, a lane pair per frame (128 frames per CTA pass), ~2 four-bin passes per thread
-static int planar_ew_grid_bf16(int H, int W, int C) {
-    const int nsub = W >= 128 ? 1 : 128 / W;
-    int nhg = (H + 8 * nsub - 1) / (8 * nsub);
-    if (nhg < 1) nhg = 1;
-    return (C / 8) * nhg;
+// the bf16 identity tail keeps to 64 registers for 4 CTAs per SM; its planar-input tail needs more and runs 2 (0: no minimum)
+template <int FORM, bool PLANAR>
+__global__ void __launch_bounds__(256, FORM == FORM_BF16 ? (PLANAR ? 2 : 4) : 0) k_resfinal(const ResFinalParams p) {
+    planar_ew<FORM, PLANAR ? TAIL_PLANAR : TAIL_ID>(p, p.h2raw);
 }
 
 int launch_gn_act(const GnActParams& p, cudaStream_t s) {
-    if (p.out_bf16) {
-        k_gn_act_bf16<<<dim3(planar_ew_grid_bf16(p.H, p.W, p.C), p.B), 256, 4 * p.C * sizeof(float), s>>>(p);
-        return 1;
+    const dim3 grid(planar_ew_grid(p.form, p.H, p.W, p.C), p.B);
+    const size_t sm = 4 * p.C * sizeof(float);
+    switch (p.form) {
+        case FORM_TF32: k_gn_act<FORM_TF32><<<grid, 256, sm, s>>>(p); return 1;
+        case FORM_X3:   k_gn_act<FORM_X3><<<grid, 256, sm, s>>>(p); return 1;
+        case FORM_BF16: k_gn_act<FORM_BF16><<<grid, 256, sm, s>>>(p); return 1;
     }
-    const long long n4 = (long long)p.H * p.W * (p.C / 4);
-    int gx = (int)((n4 + 256 * 4 * 8 - 1) / (256 * 4 * 8));   // ~8 passes of the 4-way unrolled loop per CTA (amortises the GN table set-up)
-    if (gx < 1) gx = 1;
-    if (gx > 4096) gx = 4096;
-    if (p.chw4) gx = planar_ew_grid(p.H, p.W, p.C);           // must stay a multiple of C/4 (chunk = blockIdx.x % (C/4))
-    if (p.out_lo) {
-        if (!p.chw4) return -1;
-        k_gn_act<true><<<dim3(gx, p.B), 256, 4 * p.C * sizeof(float), s>>>(p);
-    } else {
-        k_gn_act<false><<<dim3(gx, p.B), 256, 4 * p.C * sizeof(float), s>>>(p);
-    }
-    return 1;
+    return -1;
+}
+
+template <int FORM>
+static void launch_resfinal_planar(const ResFinalParams& p, size_t sm, cudaStream_t s) {
+    const dim3 grid(planar_ew_grid(FORM, p.H, p.W, p.C), p.B);
+    if (p.x) k_resfinal<FORM, false><<<grid, 256, sm, s>>>(p);
+    else k_resfinal<FORM, true><<<grid, 256, sm, s>>>(p);
 }
 
 int launch_resfinal(const ResFinalParams& p, cudaStream_t s) {
-    if (p.bf16) {
-        const size_t smb = (3 * p.C + (p.x ? 0 : (p.cin + 1) * p.C)) * sizeof(float);
-        if (p.x) k_resfinal_bf16<false><<<dim3(planar_ew_grid_bf16(p.H, p.W, p.C), p.B), 256, smb, s>>>(p);
-        else k_resfinal_bf16<true><<<dim3(planar_ew_grid_bf16(p.H, p.W, p.C), p.B), 256, smb, s>>>(p);
-        return 1;
-    }
-    const long long n4 = (long long)p.H * p.W * (p.C / 4);
-    int gx = p.x ? (int)((n4 + 256 * 4 * 8 - 1) / (256 * 4 * 8)) : (int)((n4 + 256 * 4 - 1) / (256 * 4));
-    if (gx < 1) gx = 1;
-    if (gx > 4096) gx = 4096;
-    if (p.chw4) gx = planar_ew_grid(p.H, p.W, p.C);           // must stay a multiple of C/4 (chunk = blockIdx.x % (C/4))
     const size_t sm = (3 * p.C + (p.x ? 0 : (p.cin + 1) * p.C)) * sizeof(float);
-    if (p.out_lo) {
-        if (!p.chw4) return -1;
-        k_resfinal<true><<<dim3(gx, p.B), 256, sm, s>>>(p);
-    } else {
-        k_resfinal<false><<<dim3(gx, p.B), 256, sm, s>>>(p);
+    switch (p.form) {
+        case FORM_NHWC: {
+            const long long n4 = (long long)p.H * p.W * (p.C / 4);
+            int gx = p.x ? (int)((n4 + 256 * 4 * 8 - 1) / (256 * 4 * 8)) : (int)((n4 + 256 * 4 - 1) / (256 * 4));
+            if (gx < 1) gx = 1;
+            if (gx > 4096) gx = 4096;
+            k_resfinal_nhwc<<<dim3(gx, p.B), 256, sm, s>>>(p);
+            return 1;
+        }
+        case FORM_TF32: launch_resfinal_planar<FORM_TF32>(p, sm, s); return 1;
+        case FORM_X3:   launch_resfinal_planar<FORM_X3>(p, sm, s); return 1;
+        case FORM_BF16: launch_resfinal_planar<FORM_BF16>(p, sm, s); return 1;
     }
-    return 1;
+    return -1;
 }
 
 // ----------------------------------------------------------------------------------------------

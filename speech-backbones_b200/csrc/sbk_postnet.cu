@@ -219,7 +219,7 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
         GnActParams g; memset(&g, 0, sizeof(g));
         g.raw = raw; g.gn = gnref(st1, "block1"); g.tb = p->zero; g.tb_stride = 0; g.tb_per_sample = 1;
         g.mask = mask; g.T = T; g.lvl = 0; g.out = act; g.B = B; g.H = H; g.W = T; g.C = C;
-        g.round_tf32 = x3 ? 0 : 1; g.chw4 = 1; g.out_lo = act_lo;
+        g.form = x3 ? FORM_X3 : FORM_TF32; g.out_lo = act_lo;
         if ((k = launch_gn_act(g, s)) < 0) return refused("block1 GroupNorm/Mish");
         n += k;
     }

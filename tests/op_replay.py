@@ -445,7 +445,7 @@ class Replay:
         wname = f"{q}.res_conv.weight"
         if wname in p:
             res, Ares, floor, Alin = _lin(F.conv2d, xin * mk, p[wname], p[f"{q}.res_conv.bias"])
-            # the planar first block's 1x1 and the fallback IGEMM run on CUDA cores; the rest on the tensor cores
+            # the planar first block's 1x1 runs on CUDA cores; in the tensor-core modes every other 1x1 on the tensor cores
             on_tc = tc and ins is not None
             k = kappa(mode, cin, tc=on_tc, nl=True, store_bf16=b16, extra=EPS_RECOMPUTED if recomputed else 0.0)
         else:
