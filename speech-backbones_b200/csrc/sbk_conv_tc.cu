@@ -24,8 +24,10 @@
 // Pipeline.  STAGES-deep ring with full_a / full_b / empty mbarriers; a loader warp (the first warp of the producer
 // warpgroup) fills it with bulk copies (the
 // Downsample gathers are cp.async issued by the consumers themselves) while the consumer warpgroups issue one stage's
-// MMAs back to back, wait for them and free the stage.  The epilogue stages the accumulators through shared
-// memory ([pixel][column]), so one thread owns one pixel and a contiguous run of output channels.
+// MMAs back to back as one wgmma group.  fp32x3 keeps that group in flight while it issues the next stage's and frees a
+// stage once the group after it has been issued; tf32 / bf16 (and Downsample) wait for each group and then free its
+// stage.  The epilogue stages the accumulators through shared memory ([pixel][column]), so one thread owns one pixel and
+// a contiguous run of output channels.
 // All waits are bounded spins that trap instead of hanging the GPU.
 #include "sbk_tc.cuh"
 
@@ -244,90 +246,146 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 __syncwarp();
                 if (lane == 0) mbar_arrive(empty(g % STAGES));
             };
-            // MMAs of K sub-stage ks; keeps one stage of MMAs in flight, folds a finished accumulation run (CHUNKED)
-            // (kind: the MMA kind of sub-stage ks as a compile-time constant, so no branch separates the wgmmas of a run)
-            auto compute = [&](int ks, auto kind) {
-                const uint32_t g = it + ks;
+            auto wait_full = [&](uint32_t g) {
                 const int s = g % STAGES;
                 const uint32_t ph = (g / STAGES) & 1;
                 if (!BULK) mbar_wait(full_a(s), ph);
                 mbar_wait(full_b(s), ph);                  // weights (+ the A runs when they are bulk copies)
-                const int run_lo = CHUNKED ? ks - ks % FLUSH : 0;
-                const bool last = ks == ksteps_t - 1 || (CHUNKED && ks - run_lo == FLUSH - 1);
+            };
+            // MMAs of ring stage g as one wgmma group; first: g starts an accumulation run (the first MMA overwrites)
+            // (kind: the MMA kind of the sub-stage as a compile-time constant, so no branch separates the wgmmas of a run)
+            auto issue = [&](uint32_t g, bool first, auto kind) {
+                constexpr int KD = decltype(kind)::value;
+                const int s = g % STAGES;
                 // this warpgroup's 64 pixels (2-row tile: its halo row; block a of the row adds 64 a)
                 const uint32_t a_lo = desc_lo(a0 + s * A_STAGE_BYTES, PLANE) + (uint32_t)(ROW2 ? wg * PXP : 64 * wg);
                 const uint32_t b_lo = desc_lo(b0 + s * B_STAGE_BYTES, NT * 16);
                 const uint32_t dil = C1 ? (uint32_t)p.dil : 0u;
-                auto issue = [&](auto kind) {
-                    constexpr int KD = decltype(kind)::value;
+                wg_fence();
 #pragma unroll
-                    for (int kk = 0; kk < KCH / 2; ++kk) {
-                        const uint32_t a_k = a_lo + (uint32_t)(kk * 2 * (PLANE / 16)), b_k = b_lo + (uint32_t)(kk * 2 * NT);
-                        if (GEOM == G_UP) {
-                            // ho = 2*hi - 1 + kh: parity ph uses (kh=1,dh=0),(kh=3,dh=-1) if ph=0 and (kh=0,dh=+1),(kh=2,dh=0) if ph=1
+                for (int kk = 0; kk < KCH / 2; ++kk) {
+                    const uint32_t a_k = a_lo + (uint32_t)(kk * 2 * (PLANE / 16)), b_k = b_lo + (uint32_t)(kk * 2 * NT);
+                    if (GEOM == G_UP) {
+                        // ho = 2*hi - 1 + kh: parity ph uses (kh=1,dh=0),(kh=3,dh=-1) if ph=0 and (kh=0,dh=+1),(kh=2,dh=0) if ph=1
 #pragma unroll
-                            for (int phase = 0; phase < 4; ++phase) {
-                                const int pph = phase >> 1, pw = phase & 1;
+                        for (int phase = 0; phase < 4; ++phase) {
+                            const int pph = phase >> 1, pw = phase & 1;
 #pragma unroll
-                                for (int t2 = 0; t2 < 4; ++t2) {
-                                    const int a = t2 >> 1, bb = t2 & 1;
-                                    const int kh = pph ? (a ? 2 : 0) : (a ? 3 : 1), kw = pw ? (bb ? 2 : 0) : (bb ? 3 : 1);
-                                    const int dh = pph ? (a ? 0 : 1) : (a ? -1 : 0), dw = pw ? (bb ? 0 : 1) : (bb ? -1 : 0);
-                                    wgmma<NT, KD>(acc[GEOM == G_UP ? phase : 0], desc_pack(a_k + (uint32_t)((1 + dh) * PXP + 1 + dw), D_HI),
-                                                  desc_pack(b_k + (uint32_t)((kh * 4 + kw) * KCH * NT), D_HI),
-                                                  ((ks - run_lo) | kk | t2) != 0 ? 1u : 0u);
-                                }
-                            }
-                        } else {
-#pragma unroll
-                            for (int tap = 0; tap < TAPS; ++tap) {
-                                const int r = TAPS == 9 ? tap / 3 : 0, sx = TAPS == 9 ? tap % 3 : (GEOM == G_C7 ? tap : 0);
-                                // DOWN: input row r; column tap s reads the odd plane at x (s=0) / x+1 (s=2), the even plane at x (s=1)
-                                const uint32_t aoff = GEOM == G_DOWN ? (uint32_t)(r * PXP + (sx == 1 ? TPX + 1 : (sx == 2 ? 1 : 0)))
-                                                    : C1 ? (uint32_t)tap * dil
-                                                         : (uint32_t)(r * PXP + sx);
-#pragma unroll
-                                for (int a = 0; a < NACC; ++a)
-                                    wgmma<NT, KD>(acc[a], desc_pack(a_k + aoff + (uint32_t)(64 * a), D_HI),
-                                                  desc_pack(b_k + (uint32_t)(tap * KCH * NT), D_HI), ((ks - run_lo) | kk | tap) != 0 ? 1u : 0u);
+                            for (int t2 = 0; t2 < 4; ++t2) {
+                                const int a = t2 >> 1, bb = t2 & 1;
+                                const int kh = pph ? (a ? 2 : 0) : (a ? 3 : 1), kw = pw ? (bb ? 2 : 0) : (bb ? 3 : 1);
+                                const int dh = pph ? (a ? 0 : 1) : (a ? -1 : 0), dw = pw ? (bb ? 0 : 1) : (bb ? -1 : 0);
+                                wgmma<NT, KD>(acc[GEOM == G_UP ? phase : 0], desc_pack(a_k + (uint32_t)((1 + dh) * PXP + 1 + dw), D_HI),
+                                              desc_pack(b_k + (uint32_t)((kh * 4 + kw) * KCH * NT), D_HI),
+                                              (!first || (kk | t2) != 0) ? 1u : 0u);
                             }
                         }
+                    } else {
+#pragma unroll
+                        for (int tap = 0; tap < TAPS; ++tap) {
+                            const int r = TAPS == 9 ? tap / 3 : 0, sx = TAPS == 9 ? tap % 3 : (GEOM == G_C7 ? tap : 0);
+                            // DOWN: input row r; column tap s reads the odd plane at x (s=0) / x+1 (s=2), the even plane at x (s=1)
+                            const uint32_t aoff = GEOM == G_DOWN ? (uint32_t)(r * PXP + (sx == 1 ? TPX + 1 : (sx == 2 ? 1 : 0)))
+                                                : C1 ? (uint32_t)tap * dil
+                                                     : (uint32_t)(r * PXP + sx);
+#pragma unroll
+                            for (int a = 0; a < NACC; ++a)
+                                wgmma<NT, KD>(acc[a], desc_pack(a_k + aoff + (uint32_t)(64 * a), D_HI),
+                                              desc_pack(b_k + (uint32_t)(tap * KCH * NT), D_HI), (!first || (kk | tap) != 0) ? 1u : 0u);
+                        }
                     }
-                };
-                wg_fence();
-                issue(kind);
+                }
                 wg_commit();
-                // The stage's MMAs run back to back; the wait sits on the uniform path after them (the loader keeps the
-                // next stages in flight meanwhile), and a finished accumulation run is folded branch-free.
-                wg_wait<0>();
+            };
+            auto fence_acc = [&]() {
 #pragma unroll
                 for (int a = 0; a < NACC; ++a) wg_fence_regs(acc[a]);
-                release(g);
-                if constexpr (CHUNKED) {
-                    const bool first = run_lo == 0;
-#pragma unroll
-                    for (int a = 0; a < NACC; ++a)
-#pragma unroll
-                        for (int i = 0; i < FR; ++i) sum[a][i] = last ? (first ? acc[a][i] : sum[a][i] + acc[a][i]) : sum[a][i];
-                }
             };
             constexpr auto kind_c = std::integral_constant<int, K_F16>{};     // fp32x3 correction sub-stage (even ks)
             constexpr auto kind_m = std::integral_constant<int, KMAIN>{};
             if constexpr (BULK && X3) {
-                for (int ks = 0; ks < ksteps_t; ks += 2) { compute(ks, kind_c); compute(ks + 1, kind_m); }
-            } else if constexpr (BULK) {
-                for (int ks = 0; ks < ksteps_t; ++ks) compute(ks, kind_m);
+                // One wgmma group in flight: sub-stage ks is issued while ks - 1 still runs, and stage ks - 1 is released
+                // once wait<1> has retired it, so the tensor pipe does not drain between sub-stages.  The accumulators are
+                // only read at the end of a run (every FLUSH sub-stages; Upsample: once per tile), after wait<0>; every
+                // stage is released exactly once per consumer warp, one sub-stage late, the last one after wait<0>.
+                // (tf32 / bf16 keep one wait per stage below: with nothing to fold their drains are short, and the stage
+                // a consumer holds while its MMAs are in flight costs the loader more lead than the drains cost.)
+                auto step = [&](int ks, bool first, auto kind) {
+                    const uint32_t g = it + ks;
+                    wait_full(g);
+                    issue(g, first, kind);
+                    wg_wait<1>();                            // every group but g's has completed
+                    __syncwarp();
+                    if (lane == 0 && !first) mbar_arrive(empty((g - 1) % STAGES));
+                };
+                if constexpr (CHUNKED) {
+                    // (the first MMA of a run ignores acc; defining it here ends its live range at the last fold of the
+                    // previous tile, so the epilogue, which stages sum, can use its registers)
+#pragma unroll
+                    for (int a = 0; a < NACC; ++a)
+#pragma unroll
+                        for (int i = 0; i < FR; ++i) acc[a][i] = 0.f;
+                }
+                bool first_run = true;
+                for (int ks = 0; ks < ksteps_t;) {
+                    const int run_hi = ksteps_t - ks < FLUSH ? ksteps_t : ks + FLUSH;
+                    bool first = true;
+                    do {                                     // K stage: correction, then main sub-stage
+                        step(ks, first, kind_c);
+                        step(ks + 1, false, kind_m);
+                        ks += 2;
+                        first = false;
+                    } while (ks < run_hi);
+                    wg_wait<0>();
+                    fence_acc();
+                    release(it + ks - 1);
+                    if constexpr (CHUNKED) {                 // fold the run into the running sums (round-to-nearest fp32)
+                        if (first_run) {
+#pragma unroll
+                            for (int a = 0; a < NACC; ++a)
+#pragma unroll
+                                for (int i = 0; i < FR; ++i) sum[a][i] = acc[a][i];
+                        } else {
+#pragma unroll
+                            for (int a = 0; a < NACC; ++a)
+#pragma unroll
+                                for (int i = 0; i < FR; ++i) sum[a][i] += acc[a][i];
+                        }
+                    }
+                    first_run = false;
+                }
             } else {
-                for (int ks = 0; ks < ksteps_t + LAG; ++ks) {
-                    if (ks < ksteps_t) produce(ks);
-                    cp_async_commit();                       // (empty groups past the last stage keep the accounting uniform)
-                    if (ks >= LAG) {
-                        cp_async_wait<LAG>();                // this thread's copies of stage ks-LAG have landed
-                        fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor core
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(full_a((it + ks - LAG) % STAGES));
-                        if (X3 && ((ks - LAG) & 1) == 0) compute(ks - LAG, kind_c);
-                        else compute(ks - LAG, kind_m);
+                // Each sub-stage's MMAs are waited for before its stage is released, and a finished run is folded
+                // branch-free.  Downsample: the consumers themselves gather the A tile by cp.async, LAG stages ahead.
+                auto compute = [&](int ks, auto kind) {
+                    wait_full(it + ks);
+                    const int run_lo = CHUNKED ? ks - ks % FLUSH : 0;
+                    issue(it + ks, ks == run_lo, kind);
+                    wg_wait<0>();
+                    fence_acc();
+                    release(it + ks);
+                    if constexpr (CHUNKED) {
+                        const bool first = run_lo == 0, last = ks == ksteps_t - 1 || ks - run_lo == FLUSH - 1;
+#pragma unroll
+                        for (int a = 0; a < NACC; ++a)
+#pragma unroll
+                            for (int i = 0; i < FR; ++i) sum[a][i] = last ? (first ? acc[a][i] : sum[a][i] + acc[a][i]) : sum[a][i];
+                    }
+                };
+                if constexpr (BULK) {
+                    for (int ks = 0; ks < ksteps_t; ++ks) compute(ks, kind_m);
+                } else {
+                    for (int ks = 0; ks < ksteps_t + LAG; ++ks) {
+                        if (ks < ksteps_t) produce(ks);
+                        cp_async_commit();                       // (empty groups past the last stage keep the accounting uniform)
+                        if (ks >= LAG) {
+                            cp_async_wait<LAG>();                // this thread's copies of stage ks-LAG have landed
+                            fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor core
+                            __syncwarp();
+                            if (lane == 0) mbar_arrive(full_a((it + ks - LAG) % STAGES));
+                            if (X3 && ((ks - LAG) & 1) == 0) compute(ks - LAG, kind_c);
+                            else compute(ks - LAG, kind_m);
+                        }
                     }
                 }
             }
