@@ -100,7 +100,7 @@ def operand_rounding(mode, p):
         return round_bf16(y) if mode == "bf16" else y
 
     def einsum(eq, a, b):
-        if eq == "bhdn,bhen->bhde" and x3:                                     # k_attn_kv_x3: P_hi V_hi + [P_lo V + P V_lo], fp16 chunks
+        if eq == "bhdn,bhen->bhde" and x3:                                     # k_attn_kv_wg (fp32x3): P_hi V_hi + [P_lo V + P V_lo], fp16 chunks
             ah, bh = trunc_tf32(a), trunc_tf32(b)                              # scaled by exact powers of two (sbk_attn_x3.cu)
             d = T0.float64
             return (T0.einsum(eq, ah.to(d), bh.to(d))

@@ -3,7 +3,6 @@
 // Mirrors Diffusion / GradLogPEstimator2d (Grad-TTS/model/diffusion.py:128-279); see include/sbk.h.
 #include "sbk_host.h"
 
-#include <cuda_fp16.h>
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -258,122 +257,38 @@ static int repack(sbk_handle* h, const std::string& src, const std::string& key,
 }
 
 
-// Pack a 3x3 conv weight [co][ci][3][3] into the tensor-core kernel's per-stage shared-memory image
-// [ntile][kstage][tap][16-byte chunk][co % NT][elements]: tf32-rounded fp32 (4 per chunk) or bf16 (8 per chunk).
-static uint32_t f32_to_tf32_rna(float x) {
-    uint32_t u; memcpy(&u, &x, 4);
-    if ((u & 0x7F800000u) != 0x7F800000u) u += 0x1000u;     // round to nearest, ties away (cvt.rna.tf32.f32)
-    return u & 0xFFFFE000u;
+// logical weights [cout][cin][taps] -> the conv kernel's weight image for N tile nt, uploaded under `key`
+static int pack_tc_host(sbk_handle* h, const std::vector<float>& hs, const std::string& key, int cout, int cin, int geom, int form, int nt) {
+    std::vector<uint8_t> hd(conv_tc_pack_image(hs.data(), cout, cin, geom, form, nt, nullptr));
+    conv_tc_pack_image(hs.data(), cout, cin, geom, form, nt, hd.data());
+    return upload(h->w.packed, key, hd.size(), hd.data());
 }
-static uint16_t f32_to_f16_rn(float x) {              // saturating, like the device side's cvt.rn.satfinite.f16x2.f32
-    if (x > 65504.f) x = 65504.f;
-    if (x < -65504.f) x = -65504.f;
-    const __half h = __float2half_rn(x);
-    uint16_t u; memcpy(&u, &h, 2);
-    return u;
-}
-static uint16_t f32_to_bf16_rn(float x) {
-    uint32_t u; memcpy(&u, &x, 4);
-    if ((u & 0x7FFFFFFFu) > 0x7F800000u) return (uint16_t)((u >> 16) | 0x40);
-    u += 0x7FFFu + ((u >> 16) & 1u);
-    return (uint16_t)(u >> 16);
-}
-static int pack_tc_host(sbk_handle* h, const std::vector<float>& hs, const std::string& key, int cout, int cin, int geom, bool bf16, int nt_override = 0);
-static int pack_tc(sbk_handle* h, const std::string& src, const std::string& key, int cout, int cin, int geom, bool bf16) {
+static int pack_tc(sbk_handle* h, const std::string& src, const std::string& key, int cout, int cin, int geom, int form) {
     std::vector<float> hs;
     TRY(h->w.fetch(src, hs));
-    TRY(pack_tc_host(h, hs, key, cout, cin, geom, bf16));
+    const int nt = conv_tc_ntile(geom, cout, form);
+    TRY(pack_tc_host(h, hs, key, cout, cin, geom, form, nt));
     // 3x3 convs with >= 128 output channels also get a 64-wide N-tile image: the two-row tiles run 64 channels wide, and
     // small batches have too few 128-wide tiles to fill the GPU's SMs, so the planner switches those launches to twice as
     // many half-width tiles
-    if (geom == G_C3 && conv_tc_ntile(geom, cout) == 128) TRY(pack_tc_host(h, hs, key + "64", cout, cin, geom, bf16, 64));
+    if (geom == G_C3 && nt == 128) TRY(pack_tc_host(h, hs, key + "64", cout, cin, geom, form, 64));
     return SBK_OK;
 }
-// k and v rows of to_qkv ('(qkv heads c)': k = rows 128.., v = rows 256..) in k_attn_kv's per-stage shared-memory image
-// [32-channel stage][k|v][16-byte chunk][row = head*32 + c][4], tf32-rounded
-// (bf16: [64-channel stage][k|v][16-byte chunk][row][8] as bf16)
-static int pack_tc_kv(sbk_handle* h, const std::string& src, const std::string& key, int C, bool bf16) {
+// the k and v rows of to_qkv for k_attn_kv_wg (sbk_attn_x3.cu)
+static int pack_tc_kv(sbk_handle* h, const std::string& src, const std::string& key, int C, int form) {
     std::vector<float> q;
     TRY(h->w.fetch(src, q));
-    const int EPC = bf16 ? 8 : 4, CPS = 8 * EPC;
-    std::vector<uint8_t> m((size_t)256 * C * (bf16 ? 2 : 4));
-    for (int ks = 0; ks < C / CPS; ++ks) for (int kv = 0; kv < 2; ++kv) for (int k = 0; k < 8; ++k)
-        for (int row = 0; row < 128; ++row) for (int e = 0; e < EPC; ++e) {
-            const size_t idx = ((((size_t)ks * 2 + kv) * 8 + k) * 128 + row) * EPC + e;
-            const float w = q[(size_t)(128 + kv * 128 + row) * C + ks * CPS + k * EPC + e];
-            if (bf16) reinterpret_cast<uint16_t*>(m.data())[idx] = f32_to_bf16_rn(w);
-            else reinterpret_cast<uint32_t*>(m.data())[idx] = f32_to_tf32_rna(w);
-        }
-    return upload(h->w.packed, key, m.size(), m.data());
-}
-// fp32x3 mode: the same k and v rows for k_attn_kv_x3 (sbk_attn_x3.cu): per 32-channel stage a (w_hi, correction) pair of
-// images [k|v][16-byte chunk][row][16 B] - tf32 (RNA) w_hi, and the fp16 chunks {w[c0..c3], (w - w_hi)[c0..c3] * 2^12}
-static int pack_tc_kvx(sbk_handle* h, const std::string& src, const std::string& key, int C) {
-    std::vector<float> q;
-    TRY(h->w.fetch(src, q));
-    std::vector<uint8_t> m((size_t)2 * 256 * C * 4);
-    for (int ks = 0; ks < C / 32; ++ks) for (int kv = 0; kv < 2; ++kv) for (int k = 0; k < 8; ++k)
-        for (int row = 0; row < 128; ++row) for (int e = 0; e < 4; ++e) {
-            const size_t chunk_hi = (((((size_t)ks * 2 + 0) * 2 + kv) * 8 + k) * 128 + row) * 4;      // in 4-byte units
-            const size_t chunk_c = (((((size_t)ks * 2 + 1) * 2 + kv) * 8 + k) * 128 + row) * 4;
-            const float w = q[(size_t)(128 + kv * 128 + row) * C + ks * 32 + k * 4 + e];
-            const uint32_t uh = f32_to_tf32_rna(w);
-            float fh; memcpy(&fh, &uh, 4);
-            reinterpret_cast<uint32_t*>(m.data())[chunk_hi + e] = uh;
-            uint16_t* cc = reinterpret_cast<uint16_t*>(m.data()) + 2 * chunk_c;
-            cc[e] = f32_to_f16_rn(w);
-            cc[4 + e] = f32_to_f16_rn((w - fh) * 4096.f);
-        }
+    std::vector<uint8_t> m(attn_kv_pack_image(q.data(), C, form, nullptr));
+    attn_kv_pack_image(q.data(), C, form, m.data());
     return upload(h->w.packed, key, m.size(), m.data());
 }
 // ConvTranspose2d weight [ci][co][4][4] -> logical [co][ci][kh*4+kw]
-static int pack_tc_up(sbk_handle* h, const std::string& src, const std::string& key, int C, bool bf16) {
+static int pack_tc_up(sbk_handle* h, const std::string& src, const std::string& key, int C, int form) {
     std::vector<float> w, m((size_t)C * C * 16);
     TRY(h->w.fetch(src, w));
     for (int ci = 0; ci < C; ++ci) for (int co = 0; co < C; ++co) for (int t = 0; t < 16; ++t)
         m[((size_t)co * C + ci) * 16 + t] = w[((size_t)ci * C + co) * 16 + t];
-    return pack_tc_host(h, m, key, C, C, G_UP, bf16);
-}
-// The 7x7 geometry streams one kernel row per stage: weight stage ks = (K step ks / 7, kernel row ks % 7) holds the 7 taps
-// of that row, so with `rows` stages per K step a stage carries taps / rows taps, stage tap s being tap (ks % rows) * (taps
-// / rows) + s of the kernel.  rows = 1 for every other geometry.
-size_t sbk::conv_tc_pack_image(const float* hs, int cout, int cin, int geom, bool bf16, bool x3, int nt_override, uint8_t* dst) {
-    const int taps = conv_tc_taps(geom), rows = conv_tc_stage_rows(geom), tps = taps / rows;
-    const int NT = nt_override ? nt_override : (x3 ? conv_tc_ntile_x3(geom, cout) : conv_tc_ntile(geom, cout)), CPS = conv_tc_stage_channels(geom, bf16 ? 1 : 0), EPC = bf16 ? 8 : 4, KCHK = CPS / EPC;
-    const int ksteps = cin / CPS * rows;
-    const size_t esz = bf16 ? 2 : 4;
-    const size_t bytes = (size_t)cout * cin * taps * esz * (x3 ? 2 : 1);
-    if (!dst) return bytes;
-    uint8_t* hd = dst;
-    for (int nt = 0; nt < cout / NT; ++nt) for (int ks = 0; ks < ksteps; ++ks) for (int tap = 0; tap < tps; ++tap)
-        for (int k = 0; k < KCHK; ++k) for (int col = 0; col < NT; ++col) for (int e = 0; e < EPC; ++e) {
-            const int co = nt * NT + col, ci = (ks / rows) * CPS + k * EPC + e;
-            const float w = hs[((size_t)co * cin + ci) * taps + (ks % rows) * tps + tap];
-            if (x3) {
-                // [ntile][kstage][hi|correction][tap][chunk][co % NT][16 B]: the main image holds w_hi = tf32(w) (RNA), the
-                // correction image the fp16 chunk {w[c0..c3], (w - w_hi)[c0..c3] * 2^12} that pairs with the activations'
-                // {x_lo, x * 2^-12} chunk in one f16 MMA (sbk_internal.h: corr_chunk)
-                const size_t ih = ((((((size_t)nt * ksteps + ks) * 2) * tps + tap) * KCHK + k) * NT + col) * EPC + e;
-                const uint32_t uh = f32_to_tf32_rna(w);
-                float fh; memcpy(&fh, &uh, 4);
-                reinterpret_cast<uint32_t*>(hd)[ih] = uh;
-                uint16_t* cc = reinterpret_cast<uint16_t*>(hd) + 2 * ((ih - e) + (size_t)tps * KCHK * NT * EPC);   // this (chunk, co)'s 8 halfs
-                cc[e] = f32_to_f16_rn(w);
-                cc[4 + e] = f32_to_f16_rn((w - fh) * 4096.f);
-                continue;
-            }
-            const size_t idx = (((((size_t)nt * ksteps + ks) * tps + tap) * KCHK + k) * NT + col) * EPC + e;
-            if (bf16) reinterpret_cast<uint16_t*>(hd)[idx] = f32_to_bf16_rn(w);
-            else reinterpret_cast<uint32_t*>(hd)[idx] = f32_to_tf32_rna(w);
-        }
-    return bytes;
-}
-// fp32x3 handles (and the CUDA-core fp32 handles' RefBlock branch) pack every tensor-core weight as (hi, lo) stage pairs
-static int pack_tc_host(sbk_handle* h, const std::vector<float>& hs, const std::string& key, int cout, int cin, int geom, bool bf16, int nt_override) {
-    const bool x3 = !bf16 && prec_runs_x3(h->cfg.precision);
-    std::vector<uint8_t> hd(conv_tc_pack_image(hs.data(), cout, cin, geom, bf16, x3, nt_override, nullptr));
-    conv_tc_pack_image(hs.data(), cout, cin, geom, bf16, x3, nt_override, hd.data());
-    return upload(h->w.packed, key, hd.size(), hd.data());
+    return pack_tc_host(h, m, key, C, C, G_UP, form, conv_tc_ntile(G_UP, C, form));
 }
 
 extern "C" int sbk_pack(sbk_handle* h) {
@@ -431,25 +346,22 @@ extern "C" int sbk_pack(sbk_handle* h) {
         }
         TRY(repack(h, "estimator.final_block.block.0.weight", "estimator.final_block.w", (size_t)h->cfg.dim * h->cfg.dim * 9, conv_pack));
     } else {
-        const bool bf = h->cfg.precision == SBK_PREC_BF16;
+        const int form = h->cfg.precision == SBK_PREC_BF16 ? FORM_BF16 : (x3 ? FORM_X3 : FORM_TF32);
         for (size_t k = 0; k < h->resnets.size(); ++k) {
             const ResnetInfo& r = h->resnets[k];
-            if (k != 0) TRY(pack_tc(h, r.prefix + ".block1.block.0.weight", r.prefix + ".block1.wtc", r.cout, r.cin, G_C3, bf));
-            TRY(pack_tc(h, r.prefix + ".block2.block.0.weight", r.prefix + ".block2.wtc", r.cout, r.cout, G_C3, bf));
-            if (k != 0 && r.cin != r.cout) TRY(pack_tc(h, r.prefix + ".res_conv.weight", r.prefix + ".res.wtc", r.cout, r.cin, G_PW, bf));
+            if (k != 0) TRY(pack_tc(h, r.prefix + ".block1.block.0.weight", r.prefix + ".block1.wtc", r.cout, r.cin, G_C3, form));
+            TRY(pack_tc(h, r.prefix + ".block2.block.0.weight", r.prefix + ".block2.wtc", r.cout, r.cout, G_C3, form));
+            if (k != 0 && r.cin != r.cout) TRY(pack_tc(h, r.prefix + ".res_conv.weight", r.prefix + ".res.wtc", r.cout, r.cin, G_PW, form));
         }
-        TRY(pack_tc(h, "estimator.final_block.block.0.weight", "estimator.final_block.wtc", h->cfg.dim, h->cfg.dim, G_C3, bf));
-        for (auto& a : h->attns) {
-            if (x3) TRY(pack_tc_kvx(h, a.prefix + ".fn.fn.to_qkv.weight", a.prefix + ".kvx.wtc", a.c));
-            else TRY(pack_tc_kv(h, a.prefix + ".fn.fn.to_qkv.weight", a.prefix + ".kv.wtc", a.c, bf));
-        }
+        TRY(pack_tc(h, "estimator.final_block.block.0.weight", "estimator.final_block.wtc", h->cfg.dim, h->cfg.dim, G_C3, form));
+        for (auto& a : h->attns) TRY(pack_tc_kv(h, a.prefix + ".fn.fn.to_qkv.weight", a.prefix + ".kv.wtc", a.c, form));
         for (int l = 0; l < 2; ++l) {
             const std::string p = "estimator.downs." + std::to_string(l) + ".3.conv";
-            TRY(pack_tc(h, p + ".weight", p + ".wtc", h->cfg.dim << l, h->cfg.dim << l, G_DOWN, bf));
+            TRY(pack_tc(h, p + ".weight", p + ".wtc", h->cfg.dim << l, h->cfg.dim << l, G_DOWN, form));
         }
         for (int j = 0; j < 2; ++j) {
             const std::string p = "estimator.ups." + std::to_string(j) + ".3.conv";
-            TRY(pack_tc_up(h, p + ".weight", p + ".wtc", h->cfg.dim << (1 - j), bf));
+            TRY(pack_tc_up(h, p + ".weight", p + ".wtc", h->cfg.dim << (1 - j), form));
         }
     }
     if (h->cfg.model == SBK_MODEL_DIFFVC && h->cfg.use_ref_t) {
@@ -461,7 +373,7 @@ extern "C" int sbk_pack(sbk_handle* h) {
             // the hoisted RefBlock branch (sbk_vc_conditioning) runs once per call outside the loop, on the tensor cores in
             // every precision: tf32 operands with fp32 activations for the tf32 / bf16 handles, (w_hi, correction) image pairs for
             // the fp32-class handles (fp32x3 and the CUDA-core fp32 mode, whose U-Net kernels have no InstanceNorm/GLU path)
-            TRY(pack_tc(h, q + ".0.weight", q + ".wtc", co[k], ci[k], G_C3, false));
+            TRY(pack_tc(h, q + ".0.weight", q + ".wtc", co[k], ci[k], G_C3, prec_runs_x3(h->cfg.precision) ? FORM_X3 : FORM_TF32));
         }
         TRY(repack(h, "estimator.ref_block.block11.0.weight", "estimator.ref_block.block11.w", (size_t)9 * 2 * base, first_pack));
     }
@@ -633,10 +545,8 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         p.Ho = p.H; p.Wo = p.W;
         p.wpk = h->w.get(wkey); p.bias = bkey.empty() ? nullptr : h->w.get(bkey); p.out = out; p.Cout = cout;
         p.epi = EPI_PLAIN; p.ostats = st; p.mask = pl.mask; p.T = T; p.lvl = lvl; p.zero_page = h->d_zero;
-        p.bf16 = b16 ? 1 : 0;
-        if (x3) {
-            p.x3 = 1; p.in0_lo = LO(in0); p.in1_lo = LO(in1); p.out_lo = geom != G_C3 ? LO(out) : nullptr;
-        }
+        p.form = form; p.nt = conv_tc_ntile(geom, cout, form);
+        if (x3) { p.in0_lo = LO(in0); p.in1_lo = LO(in1); p.out_corr = geom != G_C3 ? LO(out) : nullptr; }
         if (geom == G_C3) {
             // Two-row tiles (2 rows x 128 pixels x 64 channels) bring a third less operand traffic from L2 per MAC than
             // one-row tiles, but there are half as many per 64 channels.  A persistent grid runs ceil(tiles / SMs) waves,
@@ -646,7 +556,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             const long long tiles2 = (long long)B * wt * ((Hs[lvl] + 1) / 2) * (cout / 64);
             bool two = tiles2 >= 4LL * num_sms;
             if (conv_rows_env == 1 || conv_rows_env == 2) two = conv_rows_env == 2;
-            const bool wide = conv_tc_ntile(geom, cout) == 128;
+            const bool wide = p.nt == 128;
             if (two && (!wide || h->w.packed.count(wkey + "64"))) {
                 p.rows = 2;
                 if (wide) { p.nt = 64; p.wpk = h->w.get(wkey + "64"); }
@@ -756,21 +666,13 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
     auto attention = [&](int k, int lvl, const float* x, float* out) {
         const AttnInfo& a = h->attns[k];
         int mt = igemm_mtiles(G_PW, Hs[lvl], Ws[lvl], Hs[lvl], Ws[lvl]);
-        if (x3) {
-            // fp32-class attention, fused (k_attn_kv_x3): k|v projection (tf32 + fp16 correction), softmax, context
-            // partials - k and v never reach HBM.  One partial per item of attn_kv_tile_pixels() pixels: an utterance is cut
-            // at the same pixels whatever batch it sits in.
-            Op op = tc_conv(a.prefix + ".kvpart", G_PW, a.prefix + ".kvx.wtc", "", lvl, x, a.c, nullptr, 0, 256, nullptr, nullptr);
-            mt = (Hs[lvl] * Ws[lvl] + attn_kv_tile_pixels() - 1) / attn_kv_tile_pixels();
-            op.tc.epi = EPI_KV; op.tc.kv_part = bf.kv_part;
-            op.bytes = 8.0 * npix(lvl) * a.c;
-            op.flops += 2.0 * npix(lvl) * 4096.0;
-            push(op, nullptr, 0);
-        } else if (use_tc) {
-            // k/v projection + softmax partials on tensor cores (k_attn_kv): items of attn_kv_tile_pixels() pixels x 4 heads
+        if (use_tc) {
+            // k|v projection, softmax and context partials fused on the tensor cores (k_attn_kv_wg): k and v never reach
+            // HBM.  One partial per item of attn_kv_tile_pixels() pixels x 4 heads: an utterance is cut at the same pixels
+            // whatever batch it sits in.
             Op op = tc_conv(a.prefix + ".kvpart", G_PW, a.prefix + ".kv.wtc", "", lvl, x, a.c, nullptr, 0, 256, nullptr, nullptr);
             op.tc.epi = EPI_KV; op.tc.kv_part = bf.kv_part;
-            op.bytes = osz * npix(lvl) * a.c;
+            op.bytes = (x3 ? 8.0 : osz) * npix(lvl) * a.c;
             op.flops += 2.0 * npix(lvl) * 4096.0;
             mt = (Hs[lvl] * Ws[lvl] + attn_kv_tile_pixels() - 1) / attn_kv_tile_pixels();
             push(op, nullptr, 0);
@@ -793,16 +695,14 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             p.ctx = bf.ctx; p.wq = h->w.get(a.prefix + ".fn.fn.to_qkv.weight"); p.wout = h->w.get(a.prefix + ".fn.fn.to_out.weight");
             p.bout = h->w.get(a.prefix + ".fn.fn.to_out.bias"); p.g = h->w.get(a.prefix + ".fn.g");
             p.w_eff = bf.w_eff; p.b_eff = bf.b_eff; p.B = B; p.C = a.c;
-            if (use_tc) {
-                p.tc_nt = x3 ? conv_tc_ntile_x3(G_PW, a.c) : conv_tc_ntile(G_PW, a.c); p.tc_cps = conv_tc_stage_channels(G_PW, b16 ? 1 : 0);
-                p.tc_bf16 = b16 ? 1 : 0; p.tc_x3 = x3 ? 1 : 0;
-            }
+            if (use_tc) { p.nt = conv_tc_ntile(G_PW, a.c, form); p.form = form; }
             push(op, nullptr, 0);
         }
         if (use_tc) {
             // the per-sample (I + g P_b) matrix is written by k_attn_mix directly in the tensor-core weight-stage layout
             Op op = tc_conv(a.prefix + ".out", G_PW, "", "", lvl, x, a.c, nullptr, 0, a.c, out, nullptr);
-            op.tc.wpk = bf.w_eff; op.tc.w_bstride_bytes = (long long)a.c * a.c * (b16 ? 2 : (x3 ? 8 : 4)); op.tc.bias = bf.b_eff;
+            op.tc.wpk = bf.w_eff; op.tc.bias = bf.b_eff;
+            op.tc.w_bstride_bytes = (long long)conv_tc_wimg_bytes(conv_tc_wimg(G_PW, form, op.tc.nt, a.c), a.c);
             op.tc.out_mask = 1; op.tc.addin = x;
             op.bytes += osz * npix(lvl) * a.c;
             push(op, out, npix(lvl) * a.c);
@@ -1355,7 +1255,8 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
         p.geom = G_C3; p.in0 = act; p.c0 = cin; p.H = H; p.W = Tr; p.B = B; p.Ho = H; p.Wo = Tr;
         p.wpk = h->w.get(q + ".wtc"); p.bias = h->w.get(q + ".0.bias"); p.out = raw; p.Cout = cout; p.epi = EPI_PLAIN;
         p.mask = ref_mask; p.T = Tr; p.zero_page = h->d_zero;
-        if (x3) { p.x3 = 1; p.in0_lo = act_lo; }
+        p.form = x3 ? FORM_X3 : FORM_TF32; p.nt = conv_tc_ntile(G_C3, cout, p.form);     // as sbk_pack packed it
+        if (x3) p.in0_lo = act_lo;
         return launch_conv_tc(p, s);
     };
     // debug capture: every step writes the same workspace buffers, so the last step's tensors are recorded

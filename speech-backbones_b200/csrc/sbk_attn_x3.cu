@@ -41,7 +41,8 @@ static_assert(SMEM <= 227 * 1024, "shared memory budget");
 }
 
 // MODE: 0 = tf32, 1 = bf16, 2 = fp32x3.  p.in0 (/ p.in0_lo): x (and its correction chunks); p.c0 = C; p.wpk: the k|v rows
-// of to_qkv as per-stage images [k|v][chunk][row][16 B] (fp32x3: [32-channel stage][hi | correction][k|v]...);
+// of to_qkv as per-stage images [k|v][chunk][row][16 B] (fp32x3: [32-channel stage][hi | correction][k|v]...,
+// sbk_conv_tc.cu attn_kv_pack_image);
 // p.kv_part: [B][items per sample][4][kKvPartFloats]
 template <int MODE>
 __global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcParams p) {
@@ -243,7 +244,8 @@ static int launch_kv(const ConvTcParams& p, cudaStream_t s) {
 }
 
 int attn_kv_tile_pixels() { return kx3::PX; }
-int launch_attn_kv(const ConvTcParams& p, cudaStream_t s) { return p.bf16 ? launch_kv<1>(p, s) : launch_kv<0>(p, s); }
-int launch_attn_kv_x3(const ConvTcParams& p, cudaStream_t s) { return launch_kv<2>(p, s); }
+int launch_attn_kv(const ConvTcParams& p, cudaStream_t s) {
+    return p.form == FORM_X3 ? launch_kv<2>(p, s) : p.form == FORM_BF16 ? launch_kv<1>(p, s) : launch_kv<0>(p, s);
+}
 
 }  // namespace sbk

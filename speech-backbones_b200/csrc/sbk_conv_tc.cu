@@ -31,6 +31,8 @@
 // All waits are bounded spins that trap instead of hanging the GPU.
 #include "sbk_tc.cuh"
 
+#include <cuda_fp16.h>
+#include <string.h>
 #include <type_traits>
 
 namespace sbk {
@@ -77,8 +79,9 @@ template <> struct Geo<G_C1K11> : GeoC1<11> {};
 // (28 KB at NT = 128); tap s is the descriptor start s pixels into the row, as in the 3x3 halo tile.  Every input row is
 // fetched by up to 7 stages of a tile (from L2 after the first), ~15 % of the weight bytes.
 template <> struct Geo<G_C7> { static constexpr int ROWS = 1, HR = 1, PXP = TPX + 6, TAPS = 7, KCH = 2, NACC = 1; };
-// stages per K step (kernel rows streamed one stage at a time)
-template <int GEOM> constexpr int kRows = GEOM == G_C7 ? 7 : 1;
+// (the weight image's stage shape, sbk_internal.h: conv_tc_wimg)
+static_assert(Geo<G_PW>::KCH == conv_tc_kch(G_PW) && Geo<G_C3>::KCH == conv_tc_kch(G_C3) && Geo<G_C7>::KCH == conv_tc_kch(G_C7) &&
+              Geo<G_C7>::TAPS * conv_tc_stage_rows(G_C7) == conv_tc_taps(G_C7), "weight-image stage shape");
 
 }  // namespace tc
 
@@ -102,7 +105,7 @@ template <int GEOM, int NT, int R = 1> struct Depth {
 // RES: ResnetBlock-tail epilogue (1x1 res_conv + Mish(GN(h2raw)) side input), compile-time so that the plain 1x1 /
 // 3x3 instantiations do not pay its registers.
 //
-// X3 (fp32x3 mode, p.x3): two sub-stages per K stage (the f16 correction MMAs over the packed fp16 chunks, then the tf32
+// X3 (fp32x3 mode, FORM_X3): two sub-stages per K stage (the f16 correction MMAs over the packed fp16 chunks, then the tf32
 // main MMAs - sbk_internal.h: corr_chunk) AND chunked accumulation.  The tensor core truncates its fp32 accumulator on
 // every MMA (a bias of ~2^-25 |acc| per instruction towards zero), so a single accumulation run over the hundreds of MMAs
 // of a 3x3 conv would lose several 1e-6 relative - more than the fp32 rounding of the reference's own sums.  An
@@ -111,7 +114,7 @@ template <int GEOM, int NT, int R = 1> struct Depth {
 //
 // VOC: the vocoder's output forms (ConvTcParams::voc) on a 1x1 GEMM; the Conv1d geometries always use them.  They only
 // differ from the sampler's in the bf16 mode (an output is bf16 only when it is an activated operand) and, for fp32x3,
-// in the correction chunks of the second output (out_corr).
+// in the correction chunks of the second output (act_corr).
 template <int GEOM, bool BF16, int NT, bool RES, bool X3, bool VOC = false, int R = 1>
 __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     static_assert(!(X3 && BF16), "fp32x3 runs on tf32 operands");
@@ -131,7 +134,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     constexpr bool C1 = geom_is_c1(GEOM);                  // Conv1d strip geometry
     // bf16 mode: the raw Block-conv outputs (GroupNorm inputs) stay fp32 [C/4]; every other output is an operand tensor
     // of a later tensor-core kernel and is written as bf16 [B][H][C/8][W][8].  The vocoder's forms (VF16) instead pick
-    // the dtype per output: bf16 for an activated output (act_out) and the act_out2 output, fp32 for the others.
+    // the dtype per output: bf16 for an activated output (act_out) and the second output act, fp32 for the others.
     constexpr bool VF16 = BF16 && (C1 || VOC);
     constexpr bool OUT16 = BF16 && GEOM != G_C3 && !VF16;
     constexpr int PLANE = HR * PXP * 16;                   // bytes between K chunks of the A tile
@@ -160,7 +163,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
     const int Cin = p.c0 + p.c1;
     const int HW = p.H * p.W;
-    const int ksteps = Cin / CPS * kRows<GEOM>;            // ring stages per tile (7x7: one per K step and kernel row)
+    const int ksteps = Cin / CPS * conv_tc_stage_rows(GEOM);            // ring stages per tile (7x7: one per K step and kernel row)
     // fp32x3 mode: each K stage runs twice - the f16 correction sub-stage (x_lo*w + x*w_lo from the packed fp16 chunks,
     // sbk_internal.h: corr_chunk) first, then the tf32 main sub-stage (x_hi*w_hi): small terms first
     const int ksteps_t = X3 ? 2 * ksteps : ksteps;
@@ -537,7 +540,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                             op[(long long)j * Wo] = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
                                                                pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
                     } else if constexpr (VF16) {
-                        // bf16 [C/8] chunks of the activated operand (out, or lrelu(out) through out_lo); fp32 x / Z otherwise
+                        // bf16 [C/8] chunks of the activated operand (out, or lrelu(out) through act); fp32 x / Z otherwise
                         auto st16 = [&](void* base, float sl) {
                             uint4* op = reinterpret_cast<uint4*>(base) + ochunk + (long long)(cb / 8) * Wo;
                             float a[32];
@@ -554,29 +557,32 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                             float* op = p.out + obase + (cb / 4) * cstride;
 #pragma unroll
                             for (int i = 0; i < 32; i += 4) *reinterpret_cast<float4*>(op + (i / 4) * cstride) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-                            if (C1 && p.out_lo) st16(p.out_lo, p.slope);
+                            if (C1 && p.act) st16(p.act, p.slope);
                         }
                     } else {
                         float* op = p.out + obase + (cb / 4) * cstride;
 #pragma unroll
                         for (int i = 0; i < 32; i += 4) *reinterpret_cast<float4*>(op + (i / 4) * cstride) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-                        if (GEOM != G_C3 && GEOM != G_C7 && p.out_lo) {
-                            float* lp = p.out_lo + obase + (cb / 4) * cstride;
+                        if (GEOM != G_C3 && GEOM != G_C7) {
+                            if (C1 && p.act) {
+                                float* ap = reinterpret_cast<float*>(p.act) + obase + (cb / 4) * cstride;
+                                const float sl = p.slope;
 #pragma unroll
-                            for (int i = 0; i < 32; i += 4) {
-                                if (C1 && p.act_out2) {
-                                    const float sl = p.slope;
+                                for (int i = 0; i < 32; i += 4) {
                                     const float4 a = make_float4(v[i] > 0.f ? v[i] : v[i] * sl, v[i + 1] > 0.f ? v[i + 1] : v[i + 1] * sl,
                                                                  v[i + 2] > 0.f ? v[i + 2] : v[i + 2] * sl, v[i + 3] > 0.f ? v[i + 3] : v[i + 3] * sl);
-                                    *reinterpret_cast<float4*>(lp + (i / 4) * cstride) = a;
-                                    if constexpr (X3 && C1) {
+                                    *reinterpret_cast<float4*>(ap + (i / 4) * cstride) = a;
+                                    if constexpr (X3) {
                                         // fp32x3 vocoder: x, lrelu(x) and the correction chunks of lrelu(x)
-                                        if (p.out_corr)
-                                            *reinterpret_cast<float4*>(p.out_corr + obase + (cb / 4) * cstride + (i / 4) * cstride) = corr_chunk(a.x, a.y, a.z, a.w);
+                                        if (p.act_corr)
+                                            *reinterpret_cast<float4*>(p.act_corr + obase + (cb / 4) * cstride + (i / 4) * cstride) = corr_chunk(a.x, a.y, a.z, a.w);
                                     }
-                                } else {
-                                    *reinterpret_cast<float4*>(lp + (i / 4) * cstride) = corr_chunk(v[i], v[i + 1], v[i + 2], v[i + 3]);
                                 }
+                            } else if (p.out_corr) {
+                                float* cp = p.out_corr + obase + (cb / 4) * cstride;
+#pragma unroll
+                                for (int i = 0; i < 32; i += 4)
+                                    *reinterpret_cast<float4*>(cp + (i / 4) * cstride) = corr_chunk(v[i], v[i + 1], v[i + 2], v[i + 3]);
                             }
                         }
                     }
@@ -651,7 +657,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
             for (int ks = 0; ks < ksteps_t; ++ks, ++it) {
                 const int s = it % STAGES;
                 const int st = X3 ? ks / 2 : ks, var = X3 ? (ks & 1) : 1;          // 0: correction (fp16 chunks), 1: main (x, w_hi)
-                const int kb = st / kRows<GEOM>, krow = st - kb * kRows<GEOM>;     // K step, kernel row (7x7) of weight stage st
+                const int kb = st / conv_tc_stage_rows(GEOM), krow = st - kb * conv_tc_stage_rows(GEOM);     // K step, kernel row (7x7) of weight stage st
                 if (lane == 0) {
                     mbar_wait(empty(s), ((it / STAGES) & 1) ^ 1);
                     uint32_t a_tx = BULK ? A_STAGE_BYTES : 0;
@@ -738,18 +744,23 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_gemm_voc_bf16(const ConvTcParam
     conv_tc_body<G_PW, true, NT, false, false, true>(p);
 }
 
-template <int GEOM, bool BF16, int NT, bool RES = false, bool X3 = false, bool VOC = false, int R = 1>
+// the kernel of one launch configuration; VOC: the vocoder's bf16 GEMM
+template <int GEOM, int FORM, int NT, bool RES, int R, bool VOC>
+constexpr auto tc_kernel() {
+    if constexpr (VOC) return k_gemm_voc_bf16<NT>;
+    else if constexpr (FORM == FORM_X3) return k_conv_tc_x3<GEOM, NT, RES, R>;
+    else return k_conv_tc<GEOM, FORM == FORM_BF16, NT, RES, R>;
+}
+
+template <int GEOM, int FORM, int NT, bool RES = false, int R = 1, bool VOC = false>
 static int launch_tc(const ConvTcParams& p, cudaStream_t s) {
     using D = Depth<GEOM, NT, R>;
-    static_assert(!VOC || (GEOM == G_PW && BF16 && !RES && !X3), "VOC selects the bf16 GEMM with fp32 output");
+    static_assert(!VOC || (GEOM == G_PW && FORM == FORM_BF16 && !RES), "VOC selects the bf16 GEMM with fp32 output");
+    constexpr auto kernel = tc_kernel<GEOM, FORM, NT, RES, R, VOC>();
     // the dynamic-shared-memory opt-in is a per-device function attribute and the persistent grid is sized from the
     // current device's SM count: both are cached per device ordinal (a process may drive several GPUs through several handles)
     static DevCache cache;
-    const void* fn;
-    if constexpr (VOC) fn = reinterpret_cast<const void*>(k_gemm_voc_bf16<NT>);
-    else if constexpr (X3) fn = reinterpret_cast<const void*>(k_conv_tc_x3<GEOM, NT, RES, R>);
-    else fn = reinterpret_cast<const void*>(k_conv_tc<GEOM, BF16, NT, RES, R>);
-    const int num_sms = cache.get(fn);
+    const int num_sms = cache.get(reinterpret_cast<const void*>(kernel));
     if (num_sms <= 0) return -1;
     int mt;
     if (geom_is_c1(GEOM)) mt = (p.W + TPX - 1) / TPX;
@@ -758,109 +769,161 @@ static int launch_tc(const ConvTcParams& p, cudaStream_t s) {
     else mt = (p.H * p.W + TPX - 1) / TPX;
     const long long total = (long long)mt * (p.Cout / NT) * p.B;
     const int grid = (int)(total < num_sms ? total : num_sms);       // persistent: one wave of resident CTAs
-    if constexpr (VOC) k_gemm_voc_bf16<NT><<<grid, NTHREADS, D::SMEM, s>>>(p);
-    else if constexpr (X3) k_conv_tc_x3<GEOM, NT, RES, R><<<grid, NTHREADS, D::SMEM, s>>>(p);
-    else k_conv_tc<GEOM, BF16, NT, RES, R><<<grid, NTHREADS, D::SMEM, s>>>(p);
+    kernel<<<grid, NTHREADS, D::SMEM, s>>>(p);
     return 1;
 }
 
-// N tile per geometry: Upsample keeps 4 phase accumulators per thread, so its tiles are 64 channels wide
-int conv_tc_ntile(int geom, int Cout) {
+// N tile per geometry and form: Upsample keeps 4 phase accumulators per thread, so its tiles are 64 channels wide.  In
+// fp32x3 the running sums live in registers next to the accumulators: the 128-wide variants of the 7x7 conv and of the
+// Conv1d would spill them.
+int conv_tc_ntile(int geom, int Cout, int form) {
     if (geom == G_UP || geom == G_DOWN) return 64;
-    if (geom_is_c1(geom)) return Cout % 128 == 0 ? 128 : (Cout % 64 == 0 ? 64 : 32);
+    if (geom_is_c1(geom)) return Cout % 128 == 0 && form != FORM_X3 ? 128 : (Cout % 64 == 0 ? 64 : 32);
+    if (geom == G_C7 && form == FORM_X3) return 64;
     return Cout % 128 == 0 ? 128 : 64;
 }
-// (the running sums live in registers next to the accumulators; the 128-wide variants of the 7x7 conv and of the Conv1d
-// would spill them)
-int conv_tc_ntile_x3(int geom, int Cout) {
-    if (geom == G_C7) return 64;
-    if (geom_is_c1(geom)) return Cout % 64 == 0 ? 64 : 32;
-    return conv_tc_ntile(geom, Cout);
-}
-int conv_tc_taps(int geom) {
-    switch (geom) {
-        case G_PW: return 1;
-        case G_UP: return 16;
-        case G_C1K3: return 3;
-        case G_C1K7: return 7;
-        case G_C1K11: return 11;
-        case G_C7: return 49;
-        default: return 9;
-    }
-}
-int conv_tc_stage_rows(int geom) { return geom == G_C7 ? kRows<G_C7> : 1; }
-int conv_tc_stage_channels(int geom, int bf16) {
-    const int epc = bf16 ? 8 : 4;
-    return (geom == G_PW ? Geo<G_PW>::KCH : geom == G_C7 ? Geo<G_C7>::KCH : Geo<G_C3>::KCH) * epc;
-}
 
-template <bool BF16>
-static int dispatch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
-    const int nt = (p.nt == 64 && p.geom == G_C3) ? 64 : conv_tc_ntile(p.geom, p.Cout);
-    switch (p.geom) {
-        case G_C3:
-            if (p.rows == 2) return nt == 64 ? launch_tc<G_C3, BF16, 64, false, false, false, 2>(p, s) : -1;
-            return nt == 128 ? launch_tc<G_C3, BF16, 128>(p, s) : launch_tc<G_C3, BF16, 64>(p, s);
-        case G_PW:
-            if (p.epi == EPI_KV) return launch_attn_kv(p, s);
-            if (p.epi == EPI_RES) return nt == 128 ? launch_tc<G_PW, BF16, 128, true>(p, s) : launch_tc<G_PW, BF16, 64, true>(p, s);
-            return nt == 128 ? launch_tc<G_PW, BF16, 128>(p, s) : launch_tc<G_PW, BF16, 64>(p, s);
-        case G_DOWN: return launch_tc<G_DOWN, BF16, 64>(p, s);
-        case G_UP:   return launch_tc<G_UP, BF16, 64>(p, s);
-        case G_C7:                                                    // tf32 only
-            if constexpr (BF16) return -1;
-            else return nt == 128 ? launch_tc<G_C7, false, 128>(p, s) : launch_tc<G_C7, false, 64>(p, s);
-        default:     return -1;
-    }
-}
-
-// Conv1d (vocoder): tf32 operands, bf16 operands, or fp32x3 (the N tile of conv_tc_ntile_x3, as the weights are packed)
-template <int GEOM, bool BF16, bool X3>
-static int launch_conv1d(const ConvTcParams& p, cudaStream_t s, int nt) {
-    switch (nt) {
-        case 128:
-            if constexpr (X3) return -1;                               // conv_tc_ntile_x3: at most 64 wide
-            else return launch_tc<GEOM, BF16, 128, false, X3>(p, s);
-        case 64:  return launch_tc<GEOM, BF16, 64, false, X3>(p, s);
-        default:  return p.Cout % 32 == 0 ? launch_tc<GEOM, BF16, 32, false, X3>(p, s) : -1;
-    }
-}
-template <int GEOM>
-static int dispatch_conv1d(const ConvTcParams& p, cudaStream_t s) {
-    if (p.dil < 1 || p.pad < 0 || 2 * p.pad > 64) return -1;      // the strip carries at most 64 halo samples
-    if (p.x3) return launch_conv1d<GEOM, false, true>(p, s, conv_tc_ntile_x3(p.geom, p.Cout));
-    if (p.bf16) return launch_conv1d<GEOM, true, false>(p, s, conv_tc_ntile(p.geom, p.Cout));
-    return launch_conv1d<GEOM, false, false>(p, s, conv_tc_ntile(p.geom, p.Cout));
-}
-
-// fp32x3 mode (p.x3): correction + main sub-stages, chunked accumulation
-static int dispatch_conv_tc_x3(const ConvTcParams& p, cudaStream_t s) {
-    const int nt = (p.nt == 64 && p.geom == G_C3) ? 64 : conv_tc_ntile(p.geom, p.Cout);
-    switch (p.geom) {
-        case G_C3:
-            if (p.rows == 2) return nt == 64 ? launch_tc<G_C3, false, 64, false, true, false, 2>(p, s) : -1;
-            return nt == 128 ? launch_tc<G_C3, false, 128, false, true>(p, s) : launch_tc<G_C3, false, 64, false, true>(p, s);
-        case G_PW:
-            if (p.epi == EPI_KV) return launch_attn_kv_x3(p, s);      // fused projection + softmax + context (sbk_attn_x3.cu)
-            if (p.epi == EPI_RES) return nt == 128 ? launch_tc<G_PW, false, 128, true, true>(p, s) : launch_tc<G_PW, false, 64, true, true>(p, s);
-            return nt == 128 ? launch_tc<G_PW, false, 128, false, true>(p, s) : launch_tc<G_PW, false, 64, false, true>(p, s);
-        case G_DOWN: return launch_tc<G_DOWN, false, 64, false, true>(p, s);
-        case G_C7:   return launch_tc<G_C7, false, 64, false, true>(p, s);          // conv_tc_ntile_x3
-        default:     return launch_tc<G_UP, false, 64, false, true>(p, s);
-    }
+// one launch configuration: geometry, operand form, N tile, output rows per tile, ResnetBlock tail, vocoder GEMM
+static constexpr int tc_key(int geom, int form, int nt, int rows = 1, bool res = false, bool voc = false) {
+    return ((((geom * 4 + form) * 256 + nt) * 2 + rows - 1) * 2 + (res ? 1 : 0)) * 2 + (voc ? 1 : 0);
 }
 
 int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
-    if (p.x3 && p.bf16) return -1;
-    if (geom_is_c1(p.geom))
-        return p.geom == G_C1K3 ? dispatch_conv1d<G_C1K3>(p, s) : p.geom == G_C1K7 ? dispatch_conv1d<G_C1K7>(p, s) : dispatch_conv1d<G_C1K11>(p, s);
-    if (p.voc && p.bf16) {                                            // the vocoder's GEMM: fp32 Z from bf16 operands
-        if (p.geom != G_PW || p.epi != EPI_PLAIN) return -1;
-        return conv_tc_ntile(G_PW, p.Cout) == 128 ? launch_tc<G_PW, true, 128, false, false, true>(p, s)
-                                                  : launch_tc<G_PW, true, 64, false, false, true>(p, s);
+    if (p.form < FORM_TF32 || p.form > FORM_BF16 || p.nt <= 0 || p.nt > 128 || p.Cout % p.nt != 0) return -1;
+    if (p.geom == G_PW && p.epi == EPI_KV) return launch_attn_kv(p, s);   // fused projection + softmax + context (sbk_attn_x3.cu)
+    if (geom_is_c1(p.geom) && (p.dil < 1 || p.pad < 0 || 2 * p.pad > 64)) return -1;   // the strip carries at most 64 halo samples
+    const int rows = p.geom == G_C3 && p.rows == 2 ? 2 : 1;
+    const bool res = p.geom == G_PW && p.epi == EPI_RES;
+    const bool voc = p.voc && p.geom == G_PW && p.form == FORM_BF16;     // the vocoder's GEMM: fp32 Z from bf16 operands
+    constexpr int T = FORM_TF32, X = FORM_X3, B = FORM_BF16;
+    switch (tc_key(p.geom, p.form, p.nt, rows, res, voc)) {
+        // 3x3: one-row tiles, and two-row tiles 64 channels wide
+        case tc_key(G_C3, T, 128):                  return launch_tc<G_C3, T, 128>(p, s);
+        case tc_key(G_C3, T, 64):                   return launch_tc<G_C3, T, 64>(p, s);
+        case tc_key(G_C3, T, 64, 2):                return launch_tc<G_C3, T, 64, false, 2>(p, s);
+        case tc_key(G_C3, B, 128):                  return launch_tc<G_C3, B, 128>(p, s);
+        case tc_key(G_C3, B, 64):                   return launch_tc<G_C3, B, 64>(p, s);
+        case tc_key(G_C3, B, 64, 2):                return launch_tc<G_C3, B, 64, false, 2>(p, s);
+        case tc_key(G_C3, X, 128):                  return launch_tc<G_C3, X, 128>(p, s);
+        case tc_key(G_C3, X, 64):                   return launch_tc<G_C3, X, 64>(p, s);
+        case tc_key(G_C3, X, 64, 2):                return launch_tc<G_C3, X, 64, false, 2>(p, s);
+        // 1x1: plain, the ResnetBlock tail, and the vocoder's bf16 GEMM
+        case tc_key(G_PW, T, 128):                  return launch_tc<G_PW, T, 128>(p, s);
+        case tc_key(G_PW, T, 64):                   return launch_tc<G_PW, T, 64>(p, s);
+        case tc_key(G_PW, T, 128, 1, true):         return launch_tc<G_PW, T, 128, true>(p, s);
+        case tc_key(G_PW, T, 64, 1, true):          return launch_tc<G_PW, T, 64, true>(p, s);
+        case tc_key(G_PW, B, 128):                  return launch_tc<G_PW, B, 128>(p, s);
+        case tc_key(G_PW, B, 64):                   return launch_tc<G_PW, B, 64>(p, s);
+        case tc_key(G_PW, B, 128, 1, true):         return launch_tc<G_PW, B, 128, true>(p, s);
+        case tc_key(G_PW, B, 64, 1, true):          return launch_tc<G_PW, B, 64, true>(p, s);
+        case tc_key(G_PW, B, 128, 1, false, true):  return launch_tc<G_PW, B, 128, false, 1, true>(p, s);
+        case tc_key(G_PW, B, 64, 1, false, true):   return launch_tc<G_PW, B, 64, false, 1, true>(p, s);
+        case tc_key(G_PW, X, 128):                  return launch_tc<G_PW, X, 128>(p, s);
+        case tc_key(G_PW, X, 64):                   return launch_tc<G_PW, X, 64>(p, s);
+        case tc_key(G_PW, X, 128, 1, true):         return launch_tc<G_PW, X, 128, true>(p, s);
+        case tc_key(G_PW, X, 64, 1, true):          return launch_tc<G_PW, X, 64, true>(p, s);
+        // Downsample, Upsample
+        case tc_key(G_DOWN, T, 64):                 return launch_tc<G_DOWN, T, 64>(p, s);
+        case tc_key(G_DOWN, B, 64):                 return launch_tc<G_DOWN, B, 64>(p, s);
+        case tc_key(G_DOWN, X, 64):                 return launch_tc<G_DOWN, X, 64>(p, s);
+        case tc_key(G_UP, T, 64):                   return launch_tc<G_UP, T, 64>(p, s);
+        case tc_key(G_UP, B, 64):                   return launch_tc<G_UP, B, 64>(p, s);
+        case tc_key(G_UP, X, 64):                   return launch_tc<G_UP, X, 64>(p, s);
+        // 7x7 (PostNet): tf32 and fp32x3
+        case tc_key(G_C7, T, 128):                  return launch_tc<G_C7, T, 128>(p, s);
+        case tc_key(G_C7, T, 64):                   return launch_tc<G_C7, T, 64>(p, s);
+        case tc_key(G_C7, X, 64):                   return launch_tc<G_C7, X, 64>(p, s);
+        // Conv1d (vocoder)
+        case tc_key(G_C1K3, T, 128):                return launch_tc<G_C1K3, T, 128>(p, s);
+        case tc_key(G_C1K3, T, 64):                 return launch_tc<G_C1K3, T, 64>(p, s);
+        case tc_key(G_C1K3, T, 32):                 return launch_tc<G_C1K3, T, 32>(p, s);
+        case tc_key(G_C1K3, B, 128):                return launch_tc<G_C1K3, B, 128>(p, s);
+        case tc_key(G_C1K3, B, 64):                 return launch_tc<G_C1K3, B, 64>(p, s);
+        case tc_key(G_C1K3, B, 32):                 return launch_tc<G_C1K3, B, 32>(p, s);
+        case tc_key(G_C1K3, X, 64):                 return launch_tc<G_C1K3, X, 64>(p, s);
+        case tc_key(G_C1K3, X, 32):                 return launch_tc<G_C1K3, X, 32>(p, s);
+        case tc_key(G_C1K7, T, 128):                return launch_tc<G_C1K7, T, 128>(p, s);
+        case tc_key(G_C1K7, T, 64):                 return launch_tc<G_C1K7, T, 64>(p, s);
+        case tc_key(G_C1K7, T, 32):                 return launch_tc<G_C1K7, T, 32>(p, s);
+        case tc_key(G_C1K7, B, 128):                return launch_tc<G_C1K7, B, 128>(p, s);
+        case tc_key(G_C1K7, B, 64):                 return launch_tc<G_C1K7, B, 64>(p, s);
+        case tc_key(G_C1K7, B, 32):                 return launch_tc<G_C1K7, B, 32>(p, s);
+        case tc_key(G_C1K7, X, 64):                 return launch_tc<G_C1K7, X, 64>(p, s);
+        case tc_key(G_C1K7, X, 32):                 return launch_tc<G_C1K7, X, 32>(p, s);
+        case tc_key(G_C1K11, T, 128):               return launch_tc<G_C1K11, T, 128>(p, s);
+        case tc_key(G_C1K11, T, 64):                return launch_tc<G_C1K11, T, 64>(p, s);
+        case tc_key(G_C1K11, T, 32):                return launch_tc<G_C1K11, T, 32>(p, s);
+        case tc_key(G_C1K11, B, 128):               return launch_tc<G_C1K11, B, 128>(p, s);
+        case tc_key(G_C1K11, B, 64):                return launch_tc<G_C1K11, B, 64>(p, s);
+        case tc_key(G_C1K11, B, 32):                return launch_tc<G_C1K11, B, 32>(p, s);
+        case tc_key(G_C1K11, X, 64):                return launch_tc<G_C1K11, X, 64>(p, s);
+        case tc_key(G_C1K11, X, 32):                return launch_tc<G_C1K11, X, 32>(p, s);
+        default:                                    return -1;
     }
-    if (p.x3) return dispatch_conv_tc_x3(p, s);
-    return p.bf16 ? dispatch_conv_tc<true>(p, s) : dispatch_conv_tc<false>(p, s);
+}
+
+// ---- host: weight images (sbk_internal.h: ConvTcWImg) ----
+static uint32_t f32_to_tf32_rna(float x) {
+    uint32_t u; memcpy(&u, &x, 4);
+    if ((u & 0x7F800000u) != 0x7F800000u) u += 0x1000u;     // round to nearest, ties away (cvt.rna.tf32.f32)
+    return u & 0xFFFFE000u;
+}
+static uint16_t f32_to_f16_rn(float x) {              // saturating, like the device side's cvt.rn.satfinite.f16x2.f32
+    if (x > 65504.f) x = 65504.f;
+    if (x < -65504.f) x = -65504.f;
+    const __half h = __float2half_rn(x);
+    uint16_t u; memcpy(&u, &h, 2);
+    return u;
+}
+static uint16_t f32_to_bf16_rn(float x) {
+    uint32_t u; memcpy(&u, &x, 4);
+    if ((u & 0x7FFFFFFFu) > 0x7F800000u) return (uint16_t)((u >> 16) | 0x40);
+    u += 0x7FFFu + ((u >> 16) & 1u);
+    return (uint16_t)(u >> 16);
+}
+// weight w -> its element of image g: tf32 (RNA), bf16 (RNE), or FORM_X3's w_hi = tf32(w) in the main stage and
+// {w, (w - w_hi) * 2^12} in the correction stage
+static void wimg_put(uint8_t* img, const ConvTcWImg& g, int co, int ks, int tap, int ch, int e, float w) {
+    const size_t i = conv_tc_wimg_index(g, co, ks, tap, ch, e);
+    if (g.form == FORM_BF16) {
+        reinterpret_cast<uint16_t*>(img)[i] = f32_to_bf16_rn(w);
+        return;
+    }
+    const uint32_t uh = f32_to_tf32_rna(w);
+    reinterpret_cast<uint32_t*>(img)[i] = uh;
+    if (g.form == FORM_X3) {
+        float fh; memcpy(&fh, &uh, 4);
+        uint16_t* cc = reinterpret_cast<uint16_t*>(img) + 2 * conv_tc_wimg_index(g, co, ks, tap, ch, 0, 1);
+        cc[e] = f32_to_f16_rn(w);
+        cc[4 + e] = f32_to_f16_rn((w - fh) * 4096.f);
+    }
+}
+
+// The 7x7 geometry streams one kernel row per stage: weight stage ks = (K step ks / 7, kernel row ks % 7) holds the 7 taps
+// of that row.  Every other geometry has one stage per K step, holding all taps.
+size_t conv_tc_pack_image(const float* w, int cout, int cin, int geom, int form, int nt, uint8_t* dst) {
+    const ConvTcWImg g = conv_tc_wimg(geom, form, nt, cin);
+    const int taps = conv_tc_taps(geom), rows = conv_tc_stage_rows(geom), epc = form_epc(form), cps = g.kch * epc;
+    if (dst)
+        for (int co = 0; co < cout / nt * nt; ++co) for (int ks = 0; ks < g.ksteps; ++ks) for (int tap = 0; tap < g.taps; ++tap)
+            for (int ch = 0; ch < g.kch; ++ch) for (int e = 0; e < epc; ++e) {
+                const int ci = ks / rows * cps + ch * epc + e;
+                wimg_put(dst, g, co, ks, tap, ch, e, w[((size_t)co * cin + ci) * taps + ks % rows * g.taps + tap]);
+            }
+    return conv_tc_wimg_bytes(g, cout);
+}
+
+// k and v rows of to_qkv ('(qkv heads c)': k = rows 128.., v = rows 256..) as k_attn_kv_wg's per-stage image
+// [k|v][chunk][row][16 B]: the 1x1 conv's image of one 128-wide N tile with two taps per stage, k and v
+size_t attn_kv_pack_image(const float* q, int C, int form, uint8_t* dst) {
+    ConvTcWImg g = conv_tc_wimg(G_PW, form, 128, C);
+    g.taps = 2;
+    const int epc = form_epc(form), cps = g.kch * epc;
+    if (dst)
+        for (int row = 0; row < 128; ++row) for (int ks = 0; ks < g.ksteps; ++ks) for (int kv = 0; kv < 2; ++kv)
+            for (int ch = 0; ch < g.kch; ++ch) for (int e = 0; e < epc; ++e)
+                wimg_put(dst, g, row, ks, kv, ch, e, q[(size_t)(128 + kv * 128 + row) * C + ks * cps + ch * epc + e]);
+    return conv_tc_wimg_bytes(g, 128);
 }
 
 }  // namespace sbk

@@ -49,17 +49,30 @@ struct IgemmParams {
     float* kv_part;                               // EPI_KV: [B][mtiles][4][kKvPartFloats]
 };
 
+// Layout and number form of the U-Net's activation tensors, one per precision mode (GnActParams / ResFinalParams::form),
+// and, in its tensor-core values, the operand form of a wgmma conv (ConvTcParams::form).
+// Raw conv outputs (the GroupNorm inputs) are fp32 in every form: NHWC for FORM_NHWC, else [B][H][C/4][W][4].
+enum Form {
+    FORM_NHWC = 0,              // fp32 CUDA-core mode: NHWC fp32 [B][H][W][C], exact Mish
+    FORM_TF32 = 1,              // fp32 [B][H][C/4][W][4]; the Block activation is rounded to tf32 (cvt.rna), fast Mish
+    FORM_X3 = 2,                // fp32 [B][H][C/4][W][4] plus the correction twin through out_lo (corr_chunk), exact Mish
+    FORM_BF16 = 3,              // bf16 [B][H][C/8][W][8], fast Mish
+};
+
 // Tensor-core (wgmma) convolution (sbk_conv_tc.cu).  Inputs are operand-form tensors: already masked / activated, so the
 // kernel's A path is a pure copy.  geom = G_C3 (3x3, pad 1) or G_PW (1x1 over the flattened image).
 struct ConvTcParams {
     int geom;
+    int form;                                       // operand form: FORM_TF32 | FORM_X3 | FORM_BF16
     const void* in0; const void* in1; int c0, c1;   // channel concat of two operand tensors: fp32 [B][H][C/4][W][4], or bf16
-                                                    // [B][H][C/8][W][8] when bf16=1 (16-byte channel chunks either way)
+                                                    // [B][H][C/8][W][8] in FORM_BF16 (16-byte channel chunks either way)
     int H, W, B;                                    // input grid
     int Ho, Wo;                                     // output grid (G_DOWN: ~H/2 x W/2, G_UP: 2H x 2W; else = H, W)
-    const void* wpk; long long w_bstride_bytes;     // [ntile][kstage][tap][chunk][cout NT][16 B] (+ per-sample stride)
-    const float* bias; long long bias_bstride;
-    float* out; int Cout;                           // bf16=1: G_C3 still writes fp32 raw [C/4] (GroupNorm input); the other
+    const void* wpk; long long w_bstride_bytes;     // weight image conv_tc_pack_image(.., nt, ..) (+ per-sample stride)
+    const float* bias; long long bias_bstride;      // per-sample bias stride, 0 in every engine.  Kept: dropping the term
+                                                    // reschedules every conv kernel, and bench.py's fp32x3 rate fell 0.4 %
+                                                    // without it (H100 80GB HBM3, 700 W)
+    float* out; int Cout;                           // FORM_BF16: G_C3 still writes fp32 raw [C/4] (GroupNorm input); the other
                                                     // geometries write bf16 operand tensors [C/8] through this pointer
     int epi;                                        // EPI_PLAIN | EPI_RES | EPI_KV
     double* ostats;                                 // EPI_PLAIN: GroupNorm statistics of the raw output (nullable)
@@ -68,37 +81,57 @@ struct ConvTcParams {
     float* kv_part;                                 // EPI_KV: [B][ceil(HW/attn_kv_tile_pixels())][4][kKvPartFloats]
     const float* addin;                             // EPI_PLAIN: out += addin (same shape/layout/dtype as out): residual added in fp32
     const float* zero_page;                         // >= 4 KB of zeros in global memory (out-of-image parts of A tiles)
-    int bf16;
-    int nt;                                         // N tile override (64) for launches with too few 128-wide tiles to fill the
-                                                    // GPU (small batches); 0 = conv_tc_ntile(geom, Cout).  The weights must be packed for it.
+    int nt;                                         // N tile: the width the weights were packed with (conv_tc_ntile, or 64 for
+                                                    // the U-Net's second 3x3 image, used when 128-wide tiles cannot fill the GPU)
     int rows;                                       // G_C3: output rows per tile, 1 (0 = 1) or 2; 2 runs 64-wide N tiles (nt = 64)
     // Conv1d geometries: dilation and left padding ((K-1)*dil/2) in samples; output activation LeakyReLU(slope) on `out`
-    // (act_out) and/or on the second output written through out_lo (act_out2: out_lo = lrelu(out) instead of the x_lo split)
-    int dil, pad; float slope; int act_out, act_out2;
-    // fp32-class mode (SBK_PREC_FP32X3): every operand x is carried as the pair (x, correction chunks - see corr_chunk
-    // below); the tensor core reads the top 19 bits of x (= x_hi) by itself.  Weights are packed as (w_hi, correction)
-    // stage pairs and each K stage is issued twice into the same fp32 register accumulator: the f16 correction MMAs
-    // (x_lo*w + x*w_lo) first, then the tf32 main MMAs (x_hi*w_hi).
-    int x3;
+    // (act_out) and/or the second output `act`
+    int dil, pad; float slope; int act_out;
+    // fp32-class mode (FORM_X3): every operand x is carried as the pair (x, correction chunks - see corr_chunk below); the
+    // tensor core reads the top 19 bits of x (= x_hi) by itself.  Weights are packed as (w_hi, correction) stage pairs and
+    // each K stage is issued twice into the same fp32 register accumulator: the f16 correction MMAs (x_lo*w + x*w_lo) first,
+    // then the tf32 main MMAs (x_hi*w_hi).
     const void* in0_lo; const void* in1_lo;         // the correction tensors, same chunk layout as in0 / in1
-    float* out_lo;                                  // operand-form outputs (non-3x3 geometries): also write the correction chunks
+    float* out_corr;                                // operand-form outputs (non-3x3 / 7x7 geometries, act_out): their correction chunks
     // The vocoder's output forms (Conv1d geometries, and the transposed convs' 1x1 GEMM when voc = 1).  The output dtype is
     // per output, not per mode: an activated output (act_out) is the next conv's operand and takes the mode's operand form
     // (bf16 mode: bf16 [B][C/8][L][8]); every other output (the residual stream x, the GEMM output Z) stays fp32, with a
-    // fp32 addin; the act_out2 output lrelu(out) is an operand again (bf16 in bf16 mode).  fp32x3: out_corr receives the
-    // correction chunks of the act_out2 output (those of an act_out output go through out_lo, see above).
+    // fp32 addin.
     int voc;
-    float* out_corr;
+    void* act;                                      // Conv1d: second output lrelu(out) in operand form (fp32, bf16 in bf16 mode)
+    float* act_corr;                                // FORM_X3: the correction chunks of act
 };
 
-// Layout and number form of the U-Net's activation tensors, one per precision mode (GnActParams / ResFinalParams::form).
-// Raw conv outputs (the GroupNorm inputs) are fp32 in every form: NHWC for FORM_NHWC, else [B][H][C/4][W][4].
-enum Form {
-    FORM_NHWC = 0,              // fp32 CUDA-core mode: NHWC fp32 [B][H][W][C], exact Mish
-    FORM_TF32 = 1,              // fp32 [B][H][C/4][W][4]; the Block activation is rounded to tf32 (cvt.rna), fast Mish
-    FORM_X3 = 2,                // fp32 [B][H][C/4][W][4] plus the correction twin through out_lo (corr_chunk), exact Mish
-    FORM_BF16 = 3,              // bf16 [B][H][C/8][W][8], fast Mish
-};
+// ---- the wgmma conv's weight image: per N tile and K stage exactly the stage's shared-memory image --------------------
+//   [ntile][kstage][main | correction][tap][16-byte chunk][co % nt][e]
+// A K stage holds `taps` taps (7x7: the 7 of one kernel row) x `kch` 16-byte chunks of input channels, e = 4 tf32 elements
+// per chunk (8 bf16).  FORM_X3 streams a (main, correction) stage pair per K stage: the main stage holds w_hi = tf32(w)
+// (RNA), the correction stage per chunk the 8 fp16 {w[c0..c3], (w - w_hi)[c0..c3] * 2^12} that pair with the
+// activations' corr_chunk in one f16 MMA.  The other forms have no correction stage.
+struct ConvTcWImg { int form, nt, ksteps, taps, kch; };        // ksteps: K stages per N tile
+
+__host__ __device__ constexpr int form_epc(int form) { return form == FORM_BF16 ? 8 : 4; }      // elements per 16-byte chunk
+__host__ __device__ constexpr int conv_tc_taps(int geom) {
+    return geom == G_PW ? 1 : geom == G_UP ? 16 : geom == G_C1K3 ? 3 : geom == G_C1K7 ? 7 : geom == G_C1K11 ? 11 : geom == G_C7 ? 49 : 9;
+}
+__host__ __device__ constexpr int conv_tc_stage_rows(int geom) { return geom == G_C7 ? 7 : 1; }  // weight stages per K step
+__host__ __device__ constexpr int conv_tc_kch(int geom) { return geom == G_PW ? 8 : 2; }         // 16-byte chunks per stage
+__host__ __device__ constexpr int conv_tc_stage_channels(int geom, int form) { return conv_tc_kch(geom) * form_epc(form); }
+__host__ __device__ inline ConvTcWImg conv_tc_wimg(int geom, int form, int nt, int cin) {
+    const int rows = conv_tc_stage_rows(geom);
+    return {form, nt, cin / conv_tc_stage_channels(geom, form) * rows, conv_tc_taps(geom) / rows, conv_tc_kch(geom)};
+}
+// elements of one (main or correction) stage
+__host__ __device__ inline size_t conv_tc_wimg_stage(const ConvTcWImg& g) { return (size_t)g.taps * g.kch * g.nt * form_epc(g.form); }
+// index of element e of chunk ch of output channel co at tap `tap` of K stage ks, in elements of the main stage (4 bytes,
+// bf16: 2); corr = 1: the same chunk's place in the correction stage, in 4-byte units
+__host__ __device__ inline size_t conv_tc_wimg_index(const ConvTcWImg& g, int co, int ks, int tap, int ch, int e, int corr = 0) {
+    return (((size_t)(co / g.nt) * g.ksteps + ks) * (g.form == FORM_X3 ? 2 : 1) + corr) * conv_tc_wimg_stage(g) +
+           (((size_t)tap * g.kch + ch) * g.nt + co % g.nt) * form_epc(g.form) + e;
+}
+__host__ __device__ inline size_t conv_tc_wimg_bytes(const ConvTcWImg& g, int cout) {
+    return (size_t)(cout / g.nt) * g.ksteps * (g.form == FORM_X3 ? 2 : 1) * conv_tc_wimg_stage(g) * (g.form == FORM_BF16 ? 2 : 4);
+}
 
 // Block activation between the two convs of a ResnetBlock, written once in operand form (diffusion.py:57,76):
 //   act = mask ? Mish(GN(raw)) + tproj : 0        (tensor-core forms only: the fp32 mode fuses it into the next conv)
@@ -150,10 +183,9 @@ struct AttnMixParams {          // A_b = I + g * Wout * blockdiag(ctx^T) * Wq ; 
     float* w_eff;               // [B][C(ci)][C(co)]
     float* b_eff;               // [C]
     int B, C;
-    int tc_nt, tc_cps;          // != 0: write g*P only (the identity/residual is added in fp32 by the conv epilogue),
-                                // in the tensor-core 1x1 weight-stage layout, tf32-rounded
-    int tc_bf16;                // ... as bf16, 8 input channels per 16-byte chunk (tc_cps = 64)
-    int tc_x3;                  // fp32x3 mode: (hi, lo) stage pairs [ntile][kstage][hi|lo][chunk][cout % NT][4]
+    int nt;                     // != 0: write g*P only (the identity/residual is added in fp32 by the conv epilogue), as the
+                                // 1x1 conv's weight image of N tile nt in operand form `form` (conv_tc_wimg), per sample
+    int form;
 };
 
 struct FinalParams {            // final_block GN+Mish, final_conv 1x1 -> 1, mask, Euler(-Maruyama) update
@@ -250,14 +282,14 @@ struct StepBeginParams { double* stats; int n_doubles; int* step_cur; int* step_
 int launch_igemm(const IgemmParams& p, cudaStream_t s);
 int launch_first_conv(const FirstConvParams& p, cudaStream_t s);
 int launch_conv_tc(const ConvTcParams& p, cudaStream_t s);
-int conv_tc_ntile(int geom, int Cout);
-int conv_tc_ntile_x3(int geom, int Cout);
-int conv_tc_taps(int geom);
-int conv_tc_stage_rows(int geom);       // weight stages per K step: 7 for G_C7 (one per kernel row), else 1
-int conv_tc_stage_channels(int geom, int bf16);
-// host: logical weights [cout][cin][taps] -> the conv kernel's per-stage shared-memory image (sbk_api.cu); nt = 0 picks
-// conv_tc_ntile.  Returns the image size in bytes; dst may be null to query it.
-size_t conv_tc_pack_image(const float* w, int cout, int cin, int geom, bool bf16, bool x3, int nt, uint8_t* dst);
+// N tile of a conv: the width its weights are packed with and its launch runs (ConvTcParams::nt)
+int conv_tc_ntile(int geom, int Cout, int form);
+// host: logical weights [cout][cin][taps] -> the conv kernel's weight image for N tile nt (conv_tc_wimg).  Returns the
+// image size in bytes; dst may be null to query it.
+size_t conv_tc_pack_image(const float* w, int cout, int cin, int geom, int form, int nt, uint8_t* dst);
+// host: the k and v rows of to_qkv [384][C] -> k_attn_kv_wg's weight image (sbk_conv_tc.cu).  Returns its size in bytes;
+// dst may be null to query it.
+size_t attn_kv_pack_image(const float* qkv, int C, int form, uint8_t* dst);
 int launch_gn_act(const GnActParams& p, cudaStream_t s);
 int launch_resfinal(const ResFinalParams& p, cudaStream_t s);
 int launch_attn_ctx(const AttnCtxParams& p, cudaStream_t s);
@@ -265,7 +297,6 @@ int launch_attn_ctx(const AttnCtxParams& p, cudaStream_t s);
 // p.kv_part = [B][items per sample][4][kKvPartFloats]; tf32 / bf16 operands, or fp32-class (fp32x3 mode)
 int attn_kv_tile_pixels();
 int launch_attn_kv(const ConvTcParams& p, cudaStream_t s);
-int launch_attn_kv_x3(const ConvTcParams& p, cudaStream_t s);
 int launch_attn_mix(const AttnMixParams& p, cudaStream_t s);
 int launch_final(const FinalParams& p, cudaStream_t s);
 int launch_time_table(const TimeTableParams& p, cudaStream_t s);

@@ -893,35 +893,31 @@ __global__ void __launch_bounds__(256) k_attn_mix(const AttnMixParams p) {
             acc[0] = fmaf(m0.x, wq, acc[0]); acc[1] = fmaf(m0.y, wq, acc[1]); acc[2] = fmaf(m0.z, wq, acc[2]); acc[3] = fmaf(m0.w, wq, acc[3]);
             acc[4] = fmaf(m1.x, wq, acc[4]); acc[5] = fmaf(m1.y, wq, acc[5]); acc[6] = fmaf(m1.z, wq, acc[6]); acc[7] = fmaf(m1.w, wq, acc[7]);
         }
-        if (p.tc_nt) {
-            // tensor-core 1x1 weight image: [ntile][kstage][chunk][cout % NT][4 cin], tf32 (RNA); g*P only (see AttnMixParams)
-            // (bf16 mode: 8 cin per 16-byte chunk, stored as bf16)
-            const int epc = p.tc_bf16 ? 8 : 4;
-            const int NT = p.tc_nt, kch = p.tc_cps / epc, ksteps = C / p.tc_cps;
-            const int ks = cp / p.tc_cps, kc = (cp % p.tc_cps) / epc, e = cp % epc;
+        if (p.nt) {
+            // g*P only (see AttnMixParams), this sample's image of the 1x1 conv's weights (sbk_internal.h: conv_tc_wimg)
+            const ConvTcWImg wi = conv_tc_wimg(G_PW, p.form, p.nt, C);
+            const int epc = form_epc(p.form), cps = wi.kch * epc;
+            const int ks = cp / cps, kc = (cp % cps) / epc, e = cp % epc;
+            uint8_t* wb = reinterpret_cast<uint8_t*>(p.w_eff) + (long long)b * conv_tc_wimg_bytes(wi, C);
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 const int co = cb + cl0 + i;
                 float v = g * acc[i];
-                if (p.tc_x3) {
-                    // fp32x3: (w_hi, correction) stage pair - tf32 (RNA) main image and the fp16 chunk {w[c0..c3], w_lo[c0..c3] * 2^12}
-                    // of the f16 correction MMA (sbk_internal.h: corr_chunk)
-                    const long long ih = (((((long long)(co / NT) * ksteps + ks) * 2) * kch + kc) * NT + (co % NT)) * 4 + e;
+                const long long idx = conv_tc_wimg_index(wi, co, ks, 0, kc, e);
+                if (p.form == FORM_X3) {
+                    // tf32 (RNA) main image and the correction chunk {w[c0..c3], w_lo[c0..c3] * 2^12} of the f16 MMA
+                    // (sbk_internal.h: corr_chunk)
                     uint32_t uh;
                     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(uh) : "f"(v));
-                    float* wb = p.w_eff + (long long)b * 2 * C * C;
-                    wb[ih] = __uint_as_float(uh);
-                    unsigned short* cb16 = reinterpret_cast<unsigned short*>(wb + (ih - e) + (long long)kch * NT * 4);   // the chunk of (kc, co)
+                    reinterpret_cast<float*>(wb)[idx] = __uint_as_float(uh);
+                    unsigned short* cb16 = reinterpret_cast<unsigned short*>(wb) + 2 * conv_tc_wimg_index(wi, co, ks, 0, kc, 0, 1);
                     cb16[e] = (unsigned short)(f16x2_sat(v, 0.f) & 0xFFFFu);
                     cb16[4 + e] = (unsigned short)(f16x2_sat((v - __uint_as_float(uh)) * kCorrUp, 0.f) & 0xFFFFu);
-                    continue;
-                }
-                const long long idx = ((((long long)(co / NT) * ksteps + ks) * kch + kc) * NT + (co % NT)) * epc + e;
-                if (p.tc_bf16) {
-                    reinterpret_cast<unsigned short*>(p.w_eff)[(long long)b * C * C + idx] = (unsigned short)(pack_bf16x2_f(v, 0.f) & 0xFFFFu);
+                } else if (p.form == FORM_BF16) {
+                    reinterpret_cast<unsigned short*>(wb)[idx] = (unsigned short)(pack_bf16x2_f(v, 0.f) & 0xFFFFu);
                 } else {
                     uint32_t u; asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v));
-                    p.w_eff[(long long)b * C * C + idx] = __uint_as_float(u);
+                    reinterpret_cast<float*>(wb)[idx] = __uint_as_float(u);
                 }
             }
         } else {

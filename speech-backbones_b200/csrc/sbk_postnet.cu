@@ -147,9 +147,9 @@ static int pn_pack(sbk_postnet* p, const std::string& name, int geom) {
     const int d = p->cfg.dim;
     std::vector<float> w;
     TRY(p->w.fetch(name, w));
-    const bool x3 = prec_runs_x3(p->cfg.precision);
-    std::vector<uint8_t> img(conv_tc_pack_image(w.data(), d, d, geom, false, x3, 0, nullptr));
-    conv_tc_pack_image(w.data(), d, d, geom, false, x3, 0, img.data());
+    const int form = prec_runs_x3(p->cfg.precision) ? FORM_X3 : FORM_TF32, nt = conv_tc_ntile(geom, d, form);
+    std::vector<uint8_t> img(conv_tc_pack_image(w.data(), d, d, geom, form, nt, nullptr));
+    conv_tc_pack_image(w.data(), d, d, geom, form, nt, img.data());
     return upload(p->w.packed, name, img.size(), img.data());
 }
 
@@ -179,6 +179,7 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
     cudaStream_t s = (cudaStream_t)stream;
     const int C = p->cfg.dim, H = n_feats;
     const bool x3 = prec_runs_x3(p->cfg.precision);
+    const int form = x3 ? FORM_X3 : FORM_TF32;
     const size_t need = sbk_postnet_workspace_bytes(p, B, n_feats, T);
     if (p->ws.reserve(need)) return fail(SBK_ERR_CUDA, "out of memory: the PostNet workspace for (B=%d, n_feats=%d, T=%d) needs %zu bytes", B, n_feats, T, need);
     PnBufs wb;
@@ -205,7 +206,7 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
         cp.geom = G_C7; cp.in0 = in; cp.c0 = C; cp.H = H; cp.W = T; cp.B = B; cp.Ho = H; cp.Wo = T;
         cp.wpk = R(q + "weight"); cp.bias = R(q + "bias"); cp.out = raw; cp.Cout = C; cp.epi = EPI_PLAIN;
         cp.ostats = ost; cp.mask = mask; cp.T = T; cp.zero_page = p->zero;
-        if (x3) { cp.x3 = 1; cp.in0_lo = in_lo; }
+        cp.form = form; cp.nt = conv_tc_ntile(G_C7, C, form); cp.in0_lo = in_lo;     // as pn_pack packed it
         return launch_conv_tc(cp, s);
     };
     auto gnref = [&](double* stp, const char* blk) {
@@ -219,7 +220,7 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
         GnActParams g; memset(&g, 0, sizeof(g));
         g.raw = raw; g.gn = gnref(st1, "block1"); g.tb = p->zero; g.tb_stride = 0; g.tb_per_sample = 1;
         g.mask = mask; g.T = T; g.lvl = 0; g.out = act; g.B = B; g.H = H; g.W = T; g.C = C;
-        g.form = x3 ? FORM_X3 : FORM_TF32; g.out_lo = act_lo;
+        g.form = form; g.out_lo = act_lo;
         if ((k = launch_gn_act(g, s)) < 0) return refused("block1 GroupNorm/Mish");
         n += k;
     }
@@ -231,7 +232,7 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
         cp.wpk = R("res_block.res.weight"); cp.bias = R("res_block.res.bias"); cp.out = act; cp.Cout = C;
         cp.epi = EPI_RES; cp.rraw = raw; cp.rgn = gnref(st2, "block2"); cp.out_mask = 1;
         cp.mask = mask; cp.T = T; cp.zero_page = p->zero;
-        if (x3) { cp.x3 = 1; cp.in0_lo = a0_lo; }
+        cp.form = form; cp.nt = conv_tc_ntile(G_PW, C, form); cp.in0_lo = a0_lo;
         if ((k = launch_conv_tc(cp, s)) < 0) return refused("residual conv");
         n += k;
     }

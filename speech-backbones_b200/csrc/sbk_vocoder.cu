@@ -159,6 +159,7 @@ struct sbk_vocoder {
     int n_res() const { return cfg.n_kernels; }
     bool x3() const { return prec_runs_x3(precision); }
     bool bf16() const { return prec_bf16(precision); }
+    int form() const { return x3() ? FORM_X3 : (bf16() ? FORM_BF16 : FORM_TF32); }
 };
 
 static int voc_geom(int k) { return k == 3 ? G_C1K3 : (k == 7 ? G_C1K7 : (k == 11 ? G_C1K11 : -1)); }
@@ -220,7 +221,7 @@ extern "C" int sbk_vocoder_set_precision(sbk_vocoder* v, int32_t precision) {
     if (prec_bf16(precision)) {
         // bf16 K stages hold 16 input channels (Conv1d) and 64 (GEMM, sbk_conv_tc.cu conv_tc_stage_channels).  Every stage
         // has a multiple of 32 channels (sbk_vocoder_create), so its GEMM reads a multiple of 64: only conv_pre can fail.
-        const int c1 = conv_tc_stage_channels(G_C1K3, 1);
+        const int c1 = conv_tc_stage_channels(G_C1K3, FORM_BF16);
         if (v->cfg.num_mels % c1 != 0)
             return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_set_precision: bf16 needs num_mels to be a multiple of %d, got %d", c1, v->cfg.num_mels);
     }
@@ -242,11 +243,10 @@ extern "C" int sbk_vocoder_set_weight(sbk_vocoder* v, const char* name, const vo
 // logical [co][ci][taps] -> the conv kernel's per-stage shared-memory image in the handle's mode (conv_tc_pack_image: tf32
 // RNA, bf16 RNE, or fp32x3 (w_hi, correction) stage pairs)
 static int voc_pack(sbk_vocoder* v, const std::vector<float>& w, const std::string& key, int cout, int cin, int geom) {
-    const bool bf = v->bf16(), x3 = v->x3();
-    const int NT = x3 ? conv_tc_ntile_x3(geom, cout) : conv_tc_ntile(geom, cout), CPS = conv_tc_stage_channels(geom, bf ? 1 : 0);
+    const int form = v->form(), NT = conv_tc_ntile(geom, cout, form), CPS = conv_tc_stage_channels(geom, form);
     if (cin % CPS != 0 || cout % NT != 0) return fail(SBK_ERR_UNSUPPORTED, "vocoder pack '%s': %d -> %d channels do not tile (K stage %d, N tile %d)", key.c_str(), cin, cout, CPS, NT);
-    std::vector<uint8_t> img(conv_tc_pack_image(w.data(), cout, cin, geom, bf, x3, 0, nullptr));
-    conv_tc_pack_image(w.data(), cout, cin, geom, bf, x3, 0, img.data());
+    std::vector<uint8_t> img(conv_tc_pack_image(w.data(), cout, cin, geom, form, NT, nullptr));
+    conv_tc_pack_image(w.data(), cout, cin, geom, form, NT, img.data());
     return upload(v->w.packed, key, img.size(), img.data());
 }
 
@@ -335,7 +335,7 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
     VocBufs wb;
     Arena ar = v->ws.arena();
     voc_carve(v, B, T, ar, &wb);
-    const bool x3 = v->x3(), bf = v->bf16();
+    const bool bf = v->bf16();
     const int ofmt = bf ? 2 : 1;                     // debug layout of the operand tensors
     void *melc = wb.melc, *SA = wb.SA, *A0 = wb.A0, *A1 = wb.A1, *A2 = wb.A2, *Hb = wb.Hb;
     float *Z = wb.Z, *X0 = wb.X0, *X1 = wb.X1, *X2 = wb.X2, **R = wb.R;
@@ -350,9 +350,10 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
         p.wpk = v->w.get(pre + ".wtc"); p.bias = geom == G_PW ? nullptr : v->w.get(pre + ".bias"); p.out = (float*)out; p.Cout = cout; p.epi = EPI_PLAIN;
         p.zero_page = v->zero; p.dil = dil; p.pad = geom == G_PW ? 0 : (conv_tc_taps(geom) - 1) * dil / 2;
         p.slope = kSlope; p.act_out = act_out; p.addin = addin;
-        if (act_out) { p.out_lo = a_corr; p.act_out2 = 0; }
-        else { p.out_lo = (float*)a_out; p.act_out2 = a_out ? 1 : 0; p.out_corr = a_corr; }
-        p.x3 = x3 ? 1 : 0; p.in0_lo = in_lo; p.bf16 = bf ? 1 : 0; p.voc = 1;
+        if (act_out) p.out_corr = a_corr;
+        else { p.act = a_out; p.act_corr = a_corr; }
+        p.form = v->form(); p.nt = conv_tc_ntile(geom, cout, p.form);      // as voc_pack packed it
+        p.in0_lo = in_lo; p.voc = 1;
         const int k = launch_conv_tc(p, s);
         if (k < 0) rcl = -1; else n += k;
     };

@@ -579,7 +579,7 @@ VOC_SLOPE = 0.1                         # LRELU_SLOPE (models.py:10); 0.01 (torc
 
 
 def conv1d_ntile(C):
-    """N-tile width of k_conv_tc for a Conv1d with C output channels (sbk_conv_tc.cu conv_tc_ntile)"""
+    """N-tile width of k_conv_tc for a Conv1d with C output channels (sbk_conv_tc.cu conv_tc_ntile, tf32 / bf16)"""
     return 128 if C % 128 == 0 else (64 if C % 64 == 0 else 32)
 
 
@@ -791,7 +791,7 @@ def rb_branch_mode(precision):
 
 
 def rb_ntile(cout):
-    """N tile of the RefBlock's wgmma convs (sbk_conv_tc.cu conv_tc_ntile(G_C3, Cout), no planner override)"""
+    """N tile of the RefBlock's wgmma convs (sbk_conv_tc.cu conv_tc_ntile(G_C3, Cout, form), no planner override)"""
     return 128 if cout % 128 == 0 else 64
 
 

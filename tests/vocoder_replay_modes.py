@@ -5,7 +5,7 @@ mode changes:
 
   fp32x3  kappa("fp32x3", K) with the Conv1d kernel's accumulation runs: 6 sub-stages of TAPS MMAs each (18, 42, 66
           MMAs; the GEMM's runs, 6 x 4 MMAs, are shorter than op_replay.X3_RUN).  Its Conv1d N tiles are at most 64 wide
-          (conv_tc_ntile_x3), which the uniformity check groups by.
+          (conv_tc_ntile in FORM_X3), which the uniformity check groups by.
   bf16    the weights are replayed as the packer stores them (bf16, round to nearest even); the conv inputs are bf16 as
           captured (read back through sbk_vocoder_debug_op_layout).  An activated output (conv_pre, convs1) is stored as
           bf16: + EPS_STORE_BF16.  The bitwise ops (mel layout, LeakyReLU second outputs, the MRF mean before the last
