@@ -7,19 +7,22 @@ Each rep runs one worker process per tree, alternating, so both builds see the s
 imports the package of ITS tree only and, for B = 32 and B = 1 and each of fp32x3 / tf32 / bf16, plans the engine, runs
 two warm-up reverse steps and records one `sbk_profile_ops` profile (one CUDA-event pair per launch).  The report is the
 median over the reps of the per-launch ms, summed per launch kind: 3x3 Block convs (`.raw`), ResnetBlock 1x1 tails,
-attention output (the per-sample 1x1 mix), Downsample, Upsample; and the sum over every launch of the step."""
+attention output (the per-sample 1x1 mix), Downsample, Upsample, the GroupNorm / Mish activation passes (`.act`), the
+attention k|v kernel (`.kvpart`); and the sum over every launch of the step."""
 import json
 import os
 import statistics
 import subprocess
 import sys
 
-KINDS = ("conv3x3", "tail1x1", "attn_out", "down", "up", "other")
+KINDS = ("conv3x3", "tail1x1", "attn_out", "down", "up", "act", "kvpart", "other")
 
 
 def kind(name):
     if name.endswith(".raw"):
         return "conv3x3"
+    if name.endswith(".act") or name.endswith(".kvpart"):
+        return name.rsplit(".", 1)[1]
     if name.endswith(".3.out"):
         return "down" if ".downs." in name else "up"
     if name.endswith(".out") and (".2." in name or "mid_attn" in name):

@@ -402,7 +402,6 @@ namespace {
 struct Bufs {
     float *A[3], *Bf[3], *X[3], *Y[3], *S[3], *D[3], *U1;
     float *kv_part, *ctx, *w_eff, *b_eff;
-    std::map<const void*, float*> lo;          // fp32x3: operand tensor -> its x_lo twin
 };
 }
 
@@ -416,11 +415,8 @@ static size_t layout(const sbk_handle* h, int B, int T, int tb_rows, Arena& ar, 
     const size_t osz = c.precision == SBK_PREC_BF16 ? 2 : 4;
     const bool x3 = c.precision == SBK_PREC_FP32X3;
     Bufs b{};
-    auto fo = [&](size_t n) {
-        float* r = (float*)ar.take(n * osz);
-        if (x3) { float* l = (float*)ar.take(n * osz); if (r) b.lo[r] = l; }
-        return r;
-    };
+    // (fp32x3 keeps no correction twin of these: the conv kernels derive the correction operand in shared memory)
+    auto fo = [&](size_t n) { return (float*)ar.take(n * osz); };
     for (int l = 0; l < 3; ++l) {
         const size_t n = (size_t)B * P[l] * C[l];
         b.A[l] = f(n); b.Bf[l] = fo(n); b.X[l] = fo(n); b.Y[l] = fo(n);
@@ -500,7 +496,6 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
     };
     const bool use_tc = c.precision != SBK_PREC_FP32;
     const bool x3 = c.precision == SBK_PREC_FP32X3;
-    auto LO = [&](const void* q) -> float* { auto it = bf.lo.find(q); return it == bf.lo.end() ? nullptr : it->second; };
     const int num_sms = device_sm_count();
     const char* rows_env = getenv("SBK_CONV3_ROWS");
     const int conv_rows_env = rows_env ? atoi(rows_env) : 0;
@@ -546,7 +541,6 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         p.wpk = h->w.get(wkey); p.bias = bkey.empty() ? nullptr : h->w.get(bkey); p.out = out; p.Cout = cout;
         p.epi = EPI_PLAIN; p.ostats = st; p.mask = pl.mask; p.T = T; p.lvl = lvl; p.zero_page = h->d_zero;
         p.form = form; p.nt = conv_tc_ntile(geom, cout, form);
-        if (x3) { p.in0_lo = LO(in0); p.in1_lo = LO(in1); p.out_corr = geom != G_C3 ? LO(out) : nullptr; }
         if (geom == G_C3) {
             // Two-row tiles (2 rows x 128 pixels x 64 channels) bring a third less operand traffic from L2 per MAC than
             // one-row tiles, but there are half as many per 64 channels.  A persistent grid runs ceil(tiles / SMs) waves,
@@ -615,7 +609,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
                 GnActParams& p = op.ga; memset(&p, 0, sizeof(p));
                 p.raw = A; p.gn = g1; p.tb = pl.tb + h->tb_off[k]; p.tb_stride = pl.tb_stride; p.step = pl.step_cur;
                 p.mask = pl.mask; p.T = T; p.lvl = lvl; p.out = Bb; p.B = B; p.H = Hs[lvl]; p.W = Ws[lvl]; p.C = r.cout;
-                p.form = form; p.out_lo = LO(Bb);
+                p.form = form;
                 op.bytes = (4.0 + osz) * npix(lvl) * r.cout;
                 push(op, nullptr, 0);
             }
@@ -634,7 +628,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             ResFinalParams& p = op.rf; memset(&p, 0, sizeof(p));
             p.h2raw = h2; p.gn = g2;
             p.mask = pl.mask; p.T = T; p.lvl = lvl; p.out = out; p.B = B; p.H = Hs[lvl]; p.W = Ws[lvl]; p.C = r.cout;
-            p.out_mask = store_masked ? 1 : 0; p.form = form; p.out_lo = LO(out);
+            p.out_mask = store_masked ? 1 : 0; p.form = form;
             if (k == 0) {
                 p.x = nullptr; p.mu = pl.mu; p.xt = pl.xt; p.spk_s = pl.spk_s; p.cin = cin0;
                 p.wres = h->w.get(r.prefix + ".res.w"); p.bres = h->w.get(r.prefix + ".res_conv.bias");
@@ -672,7 +666,7 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
             // whatever batch it sits in.
             Op op = tc_conv(a.prefix + ".kvpart", G_PW, a.prefix + ".kv.wtc", "", lvl, x, a.c, nullptr, 0, 256, nullptr, nullptr);
             op.tc.epi = EPI_KV; op.tc.kv_part = bf.kv_part;
-            op.bytes = (x3 ? 8.0 : osz) * npix(lvl) * a.c;
+            op.bytes = osz * npix(lvl) * a.c;
             op.flops += 2.0 * npix(lvl) * 4096.0;
             mt = (Hs[lvl] * Ws[lvl] + attn_kv_tile_pixels() - 1) / attn_kv_tile_pixels();
             push(op, nullptr, 0);

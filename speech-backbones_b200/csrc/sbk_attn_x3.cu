@@ -38,9 +38,12 @@ constexpr int THREADS = 256 + 32;              // 2 consumer warpgroups + loader
 constexpr int NBARS = 2 * STAGES;
 constexpr size_t SMEM = (size_t)STAGES * STAGE + 4 * OPI + 4 * 128 * 4 + NBARS * 8 + 16;
 static_assert(SMEM <= 227 * 1024, "shared memory budget");
+static_assert(XS <= OPI && STAGES == 2, "fp32x3: the converted x fits a context image; a K stage is the whole ring");
 }
 
-// MODE: 0 = tf32, 1 = bf16, 2 = fp32x3.  p.in0 (/ p.in0_lo): x (and its correction chunks); p.c0 = C; p.wpk: the k|v rows
+// MODE: 0 = tf32, 1 = bf16, 2 = fp32x3.  p.in0: x (fp32x3: its correction chunks are derived here, p.in0_lo is not read:
+// the loader brings x with the main sub-stage only and the consumers convert it into the idle Pc / Vc images, alternating
+// between them per K stage so that one warpgroup may still read the last stage's chunks); p.c0 = C; p.wpk: the k|v rows
 // of to_qkv as per-stage images [k|v][chunk][row][16 B] (fp32x3: [32-channel stage][hi | correction][k|v]...,
 // sbk_conv_tc.cu attn_kv_pack_image);
 // p.kv_part: [B][items per sample][4][kKvPartFloats]
@@ -86,6 +89,41 @@ __global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcPara
             const int b = t / items, mt = t - b * items;
             // ---- projection: warpgroup 0 -> K^T, warpgroup 1 -> V^T  (64 pixels x 128 rows)
             float acc[64];
+            if constexpr (X3) {
+                // K stage kb = ring stages it (correction weights) and it + 1 (x, main weights): correction MMAs, then main
+                for (int kb = 0; kb < ksteps; ++kb, it += 2) {
+                    const int sc = it % STAGES, sm = (it + 1) % STAGES;
+                    mbar_wait(full(sc), (it / STAGES) & 1);
+                    mbar_wait(full(sm), ((it + 1) / STAGES) & 1);
+                    const uint32_t xc = s0 + sc * STAGE, xm = s0 + sm * STAGE;
+                    uint8_t* cx = (kb & 1) ? vc : pc;
+                    {
+                        const float4* src = reinterpret_cast<const float4*>(sS + sm * STAGE);
+#pragma unroll
+                        for (int i = tid; i < XS / 16; i += 256) {
+                            const float4 v = src[i];
+                            reinterpret_cast<float4*>(cx)[i] = corr_chunk(v.x, v.y, v.z, v.w);
+                        }
+                    }
+                    fence_proxy_async();                           // converted chunks -> visible to the tensor core
+                    asm volatile("bar.sync 1, 256;" ::: "memory");
+                    const uint32_t c_lo = desc_lo(smem_u32(cx), PX * 16), x_lo = desc_lo(xm, PX * 16);
+                    const uint32_t wc_lo = desc_lo(xc + XS + wg * (KCH * 128 * 16), 128 * 16), wm_lo = desc_lo(xm + XS + wg * (KCH * 128 * 16), 128 * 16);
+                    wg_fence();
+#pragma unroll
+                    for (int kk = 0; kk < KCH / 2; ++kk)
+                        wgmma<128, K_F16>(acc, desc_pack(c_lo + (uint32_t)(kk * 2 * PX), D_HI), desc_pack(wc_lo + (uint32_t)(kk * 2 * 128), D_HI),
+                                          (kb | kk) != 0 ? 1u : 0u);
+#pragma unroll
+                    for (int kk = 0; kk < KCH / 2; ++kk)
+                        wgmma<128, K_TF32>(acc, desc_pack(x_lo + (uint32_t)(kk * 2 * PX), D_HI), desc_pack(wm_lo + (uint32_t)(kk * 2 * 128), D_HI), 1u);
+                    wg_commit();
+                    wg_wait<0>();
+                    wg_fence_regs(acc);
+                    __syncwarp();
+                    if (lane == 0) { mbar_arrive(empty(sc)); mbar_arrive(empty(sm)); }
+                }
+            } else
             for (int ks = 0; ks < ksteps_t; ++ks, ++it) {
                 const int s = it % STAGES;
                 mbar_wait(full(s), (it / STAGES) & 1);
@@ -98,8 +136,7 @@ __global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcPara
                                                           desc_pack(w_lo + (uint32_t)(kk * 2 * 128), D_HI), (ks | kk) != 0 ? 1u : 0u);
                 };
                 wg_fence();
-                if (X3 && (ks & 1) == 0) issue(std::integral_constant<int, K_F16>{});   // correction sub-stage (fp16 chunks)
-                else issue(std::integral_constant<int, KMAIN>{});
+                issue(std::integral_constant<int, KMAIN>{});
                 wg_commit();
                 wg_wait<0>();
                 wg_fence_regs(acc);
@@ -210,12 +247,12 @@ __global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcPara
                 const uint32_t xs = smem_u32(sS) + s * STAGE;
                 if (lane == 0) {
                     mbar_wait(empty(s), ((it / STAGES) & 1) ^ 1);
-                    mbar_arrive_expect_tx(full(s), STAGE);
+                    mbar_arrive_expect_tx(full(s), corr ? WS : STAGE);
                     bulk_g2s(xs + XS, reinterpret_cast<const uint8_t*>(p.wpk) + (size_t)(X3 ? 2 * kb + (corr ? 1 : 0) : ks) * WS, WS, full(s));
                 }
                 __syncwarp();
-                if (lane < KCH) {
-                    const uint8_t* src = reinterpret_cast<const uint8_t*>(corr ? p.in0_lo : p.in0);
+                if (lane < KCH && !corr) {
+                    const uint8_t* src = reinterpret_cast<const uint8_t*>(p.in0);
                     const int k = lane, cl = kb * KCH + k;
                     int m = m0, hh = hh0, ww = ww0, qx = 0;
                     while (m < m_hi) {                             // split the flattened run at image-row boundaries

@@ -41,7 +41,9 @@ namespace tc {
 
 constexpr int TPX = 128;              // pixels per row = 2 consumer warpgroups x wgmma M (64)
 constexpr int NCONS = 256;            // consumer threads (2 warpgroups): MMAs + epilogue (Downsample: + A gathers)
-constexpr int NTHREADS = NCONS + 128; // + producer warpgroup (its first warp is the loader, the other three exit)
+constexpr int NTHREADS = NCONS + 128; // + producer warpgroup: its first warp is the loader; the other three exit, or derive
+                                      // the fp32x3 correction operand in shared memory (NCONV converter threads)
+constexpr int NCONV = 96;
 // Register split (setmaxnreg): the CTA starts with 65536 / 384 registers per thread; the producer warpgroup gives most of
 // its share back so that the consumers can hold a 128-register accumulator tile (+ fp32x3 running sums) without spilling.
 constexpr int PROD_REGS = 40, CONS_REGS = 232;
@@ -101,6 +103,12 @@ template <int GEOM, int NT, int R = 1> struct Depth {
     static_assert(STAGES >= 2, "need at least 2 stages");
     static_assert(SMEM <= 227 * 1024, "shared memory budget");
 };
+// fp32x3 launches without a correction twin derive a correction sub-stage's A tile from the main sub-stage that FOLLOWS it
+// in the ring, so stage g is full only once stage g + 1 has landed.  A consumer that waits for stage g has released every
+// stage up to g - 2 (one MMA group in flight), and the loader fills stage g + 1 once stage g + 1 - STAGES is released:
+// g + 1 - STAGES <= g - 2, i.e. three stages.  (Downsample's consumers gather stage g + 1 themselves before they convert
+// it, LAG = STAGES - 2 >= 1 stages ahead of the MMAs: three stages again.)
+template <int GEOM, int NT, int R> constexpr bool x3_depth_ok = Depth<GEOM, NT, R>::STAGES >= 3;
 
 // RES: ResnetBlock-tail epilogue (1x1 res_conv + Mish(GN(h2raw)) side input), compile-time so that the plain 1x1 /
 // 3x3 instantiations do not pay its registers.
@@ -167,6 +175,12 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     // fp32x3 mode: each K stage runs twice - the f16 correction sub-stage (x_lo*w + x*w_lo from the packed fp16 chunks,
     // sbk_internal.h: corr_chunk) first, then the tf32 main sub-stage (x_hi*w_hi): small terms first
     const int ksteps_t = X3 ? 2 * ksteps : ksteps;
+    // fp32x3 without a correction twin (in0_lo / in1_lo null): the correction sub-stage's A tile is corr_chunk of the main
+    // sub-stage's tile, computed in shared memory - by the converter warps of the producer warpgroup for the bulk-copy
+    // geometries, by the gathering consumers themselves for Downsample.  The tile is converted whole, so the zero padding
+    // (border columns, out-of-image rows, the ragged end of a 1x1 tile) becomes zero chunks and needs no pattern logic.
+    const bool insm = X3 && p.in0_lo == nullptr;
+    static_assert(!X3 || x3_depth_ok<GEOM, NT, R>, "in-SM correction operand: stage g needs stage g + 1, three stages");
     // ---- tile space: (sample, pixel tile, N tile), N tile fastest so neighbours in time share the A tile in L2
     const int wt_w = (GEOM == G_DOWN ? p.Wo : p.W), wt_h = (GEOM == G_DOWN ? p.Ho : p.H);
     const int wtiles = (wt_w + SPAN - 1) / SPAN;
@@ -187,7 +201,9 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
 
     // ---- one-time setup
     if (tid == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full_a(s), NCONS / 32); mbar_init(full_b(s), 1); mbar_init(empty(s), NCONS / 32); }
+        // full_a: one arrival per warp that writes A tiles from registers (Downsample's consumers, else the converter warps)
+        constexpr int A_WARPS = X3 && BULK ? NCONV / 32 : NCONS / 32;
+        for (int s = 0; s < STAGES; ++s) { mbar_init(full_a(s), A_WARPS); mbar_init(full_b(s), 1); mbar_init(empty(s), NCONS / 32); }
         fence_barrier_init();
     }
     if (tid < 128 * ROWS) s_st[tid] = 0.f;
@@ -237,6 +253,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 const uint8_t* src = reinterpret_cast<const uint8_t*>(second ? (lo ? p.in1_lo : p.in1) : (lo ? p.in0_lo : p.in0));
                 const int chs = (second ? p.c1 : p.c0) / EPC;
                 const int c0k = second ? ck - p.c0 / EPC : ck;
+                if (X3 && insm && lo) return;              // converted from the main sub-stage's gathers (convert_own)
 #pragma unroll
                 for (int j = 0; j < PER; ++j) {
                     if (sl_dst[j] == 0xFFFFFFFFu) continue;
@@ -249,10 +266,14 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 __syncwarp();
                 if (lane == 0) mbar_arrive(empty(g % STAGES));
             };
-            auto wait_full = [&](uint32_t g) {
+            // conv: a correction sub-stage whose A tile the converter warps write.  Its full_a only completes a phase when the
+            // buffer holds a correction sub-stage: every turn of the ring when STAGES is even (even buffers always do), every
+            // second turn when it is odd.
+            auto wait_full = [&](uint32_t g, bool conv = false) {
                 const int s = g % STAGES;
                 const uint32_t ph = (g / STAGES) & 1;
                 if (!BULK) mbar_wait(full_a(s), ph);
+                else if (conv) mbar_wait(full_a(s), (g / (STAGES % 2 ? 2 * STAGES : STAGES)) & 1);
                 mbar_wait(full_b(s), ph);                  // weights (+ the A runs when they are bulk copies)
             };
             // MMAs of ring stage g as one wgmma group; first: g starts an accumulation run (the first MMA overwrites)
@@ -315,7 +336,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 // a consumer holds while its MMAs are in flight costs the loader more lead than the drains cost.)
                 auto step = [&](int ks, bool first, auto kind) {
                     const uint32_t g = it + ks;
-                    wait_full(g);
+                    wait_full(g, insm && decltype(kind)::value == K_F16);
                     issue(g, first, kind);
                     wg_wait<1>();                            // every group but g's has completed
                     __syncwarp();
@@ -382,11 +403,27 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         if (ks < ksteps_t) produce(ks);
                         cp_async_commit();                       // (empty groups past the last stage keep the accounting uniform)
                         if (ks >= LAG) {
+                            const bool corr = X3 && ((ks - LAG) & 1) == 0;
+                            if (X3 && insm && corr) {
+                                // In-SM correction operand: this thread's gathers of the main sub-stage ks-LAG+1 (issued at
+                                // iteration ks-LAG+1 <= ks) have landed; their corr_chunk goes to the same slots of the
+                                // correction stage, whose previous occupant produce(ks-LAG) saw released.  Zero-filled
+                                // slots (padding) convert to zero chunks.
+                                static_assert(!X3 || LAG >= 1, "the main gather runs ahead of its correction sub-stage");
+                                cp_async_wait<(LAG > 0 ? LAG - 1 : 0)>();
+                                const uint32_t sc = (it + ks - LAG) % STAGES, sm = (it + ks - LAG + 1) % STAGES;
+#pragma unroll
+                                for (int j = 0; j < PER; ++j) {
+                                    if (sl_dst[j] == 0xFFFFFFFFu) continue;
+                                    const float4 v = *reinterpret_cast<const float4*>(sA + sm * A_STAGE_BYTES + sl_dst[j]);
+                                    *reinterpret_cast<float4*>(sA + sc * A_STAGE_BYTES + sl_dst[j]) = corr_chunk(v.x, v.y, v.z, v.w);
+                                }
+                            }
                             cp_async_wait<LAG>();                // this thread's copies of stage ks-LAG have landed
                             fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor core
                             __syncwarp();
                             if (lane == 0) mbar_arrive(full_a((it + ks - LAG) % STAGES));
-                            if (X3 && ((ks - LAG) & 1) == 0) compute(ks - LAG, kind_c);
+                            if (corr) compute(ks - LAG, kind_c);
                             else compute(ks - LAG, kind_m);
                         }
                     }
@@ -634,7 +671,44 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
         }
     } else {
         setmaxnreg_dec<PROD_REGS>();
-        if (warp != NCONS / 32) return;
+        if (warp != NCONS / 32) {
+            if constexpr (X3 && BULK) {
+                // =================================================================================================
+                // converter warps (fp32x3 without a correction twin): correction stage g = corr_chunk of main stage g + 1
+                // =================================================================================================
+                // Stage g + 1's full_b says its A tile has landed AND that the loader, which fills the ring in order, has
+                // seen stage g's previous occupant released, so stage g's A area is free to write.  Stage g + 1 cannot be
+                // overwritten while it is read here: the consumers release it after its MMAs, which they issue after stage
+                // g's, which wait for this warp's arrival on full_a(g).
+                if (insm) {
+                    const int ct = tid - (NCONS + 32);
+                    uint32_t it = 0;
+                    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+                        for (int ks = 0; ks < ksteps_t; ks += 2, it += 2) {
+                            const uint32_t sc = it % STAGES, sm = (it + 1) % STAGES;
+                            mbar_wait(full_b(sm), ((it + 1) / STAGES) & 1);
+                            const float4* src = reinterpret_cast<const float4*>(sA + sm * A_STAGE_BYTES);
+                            float4* dst = reinterpret_cast<float4*>(sA + sc * A_STAGE_BYTES);
+                            // (four loads in flight per thread: the conversion's latency is lead the loader loses)
+                            constexpr int NCHK = A_STAGE_BYTES / 16, UN = 4;
+                            for (int i0 = ct; i0 < NCHK; i0 += UN * NCONV) {
+                                float4 v[UN];
+#pragma unroll
+                                for (int u = 0; u < UN; ++u)
+                                    if (i0 + u * NCONV < NCHK) v[u] = src[i0 + u * NCONV];
+#pragma unroll
+                                for (int u = 0; u < UN; ++u)
+                                    if (i0 + u * NCONV < NCHK) dst[i0 + u * NCONV] = corr_chunk(v[u].x, v[u].y, v[u].z, v[u].w);
+                            }
+                            fence_proxy_async();             // generic-proxy smem writes -> visible to the tensor core
+                            __syncwarp();
+                            if (lane == 0) mbar_arrive(full_a(sc));
+                        }
+                    }
+                }
+            }
+            return;
+        }
         // =========================================================================================================
         // loader warp: weights + A runs by cp.async.bulk.  Every byte of the A tile is written every stage:
         // out-of-image rows / columns (the conv's zero padding, the ragged last 1x1 tile) come from a zero page.
@@ -658,9 +732,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 const int s = it % STAGES;
                 const int st = X3 ? ks / 2 : ks, var = X3 ? (ks & 1) : 1;          // 0: correction (fp16 chunks), 1: main (x, w_hi)
                 const int kb = st / conv_tc_stage_rows(GEOM), krow = st - kb * conv_tc_stage_rows(GEOM);     // K step, kernel row (7x7) of weight stage st
+                const bool conv = X3 && BULK && insm && var == 0;     // A tile written by the converter warps: weights only
                 if (lane == 0) {
                     mbar_wait(empty(s), ((it / STAGES) & 1) ^ 1);
-                    uint32_t a_tx = BULK ? A_STAGE_BYTES : 0;
+                    uint32_t a_tx = BULK && !conv ? A_STAGE_BYTES : 0;
                     if (BULK && GEOM != G_PW) {
                         // Image-border columns (the conv's zero padding) are never written by the row copies, so they only
                         // need zeroing when this stage buffer last served a tile with a different border pattern.  With
@@ -670,7 +745,9 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         const int wlo = w0 - pad < 0 ? 0 : w0 - pad, whi = w0 + SPAN + pad > p.W ? p.W : w0 + SPAN + pad;
                         const int qlo = wlo - (w0 - pad), qhi = qlo + (whi - wlo);
                         const uint32_t pat = (uint32_t)qlo | ((uint32_t)qhi << 16);
-                        if (stage_pat[s] != pat) {
+                        if (conv) {
+                            stage_pat[s] = pat;              // the converters write the whole tile, its zero borders included
+                        } else if (stage_pat[s] != pat) {
                             stage_pat[s] = pat;
                             if (qlo > 0 || qhi < PXP) {
                                 uint8_t* st = sA + s * A_STAGE_BYTES;
@@ -685,14 +762,14 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         }
                         int vrows = 0;
                         for (int r = 0; r < HR; ++r) { const int hi = C1 ? 0 : h0 - PADK + krow + r; vrows += (hi >= 0 && hi < p.H) ? 1 : 0; }
-                        a_tx -= (uint32_t)(KCH * vrows * (PXP - (qhi - qlo))) * 16u;
+                        if (!conv) a_tx -= (uint32_t)(KCH * vrows * (PXP - (qhi - qlo))) * 16u;
                     }
                     mbar_arrive_expect_tx(full_b(s), B_STAGE_BYTES + a_tx);
                     bulk_g2s(smem_u32(sB + s * B_STAGE_BYTES), wsrc + (size_t)(X3 ? 2 * st + (var == 0) : ks) * B_STAGE_BYTES,
                              B_STAGE_BYTES, full_b(s));
                 }
                 __syncwarp();
-                if (BULK && lane < KCH * HR) {
+                if (BULK && !conv && lane < KCH * HR) {
                     const uint32_t a_s = smem_u32(sA) + s * A_STAGE_BYTES;
                     const int k = lane / HR, r = lane - k * HR;
                     const int ck = kb * KCH + k;                     // 16-byte channel chunk index over the concat
@@ -792,6 +869,7 @@ int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
     if (p.form < FORM_TF32 || p.form > FORM_BF16 || p.nt <= 0 || p.nt > 128 || p.Cout % p.nt != 0) return -1;
     if (p.geom == G_PW && p.epi == EPI_KV) return launch_attn_kv(p, s);   // fused projection + softmax + context (sbk_attn_x3.cu)
     if (geom_is_c1(p.geom) && (p.dil < 1 || p.pad < 0 || 2 * p.pad > 64)) return -1;   // the strip carries at most 64 halo samples
+    if (p.form == FORM_X3 && p.c1 > 0 && (p.in0_lo == nullptr) != (p.in1_lo == nullptr)) return -1;   // twins for both inputs or for neither
     const int rows = p.geom == G_C3 && p.rows == 2 ? 2 : 1;
     const bool res = p.geom == G_PW && p.epi == EPI_RES;
     const bool voc = p.voc && p.geom == G_PW && p.form == FORM_BF16;     // the vocoder's GEMM: fp32 Z from bf16 operands

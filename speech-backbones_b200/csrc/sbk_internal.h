@@ -55,7 +55,7 @@ struct IgemmParams {
 enum Form {
     FORM_NHWC = 0,              // fp32 CUDA-core mode: NHWC fp32 [B][H][W][C], exact Mish
     FORM_TF32 = 1,              // fp32 [B][H][C/4][W][4]; the Block activation is rounded to tf32 (cvt.rna), fast Mish
-    FORM_X3 = 2,                // fp32 [B][H][C/4][W][4] plus the correction twin through out_lo (corr_chunk), exact Mish
+    FORM_X3 = 2,                // fp32 [B][H][C/4][W][4], exact Mish; a correction twin (corr_chunk) only where out_lo is given
     FORM_BF16 = 3,              // bf16 [B][H][C/8][W][8], fast Mish
 };
 
@@ -91,7 +91,8 @@ struct ConvTcParams {
     // tensor core reads the top 19 bits of x (= x_hi) by itself.  Weights are packed as (w_hi, correction) stage pairs and
     // each K stage is issued twice into the same fp32 register accumulator: the f16 correction MMAs (x_lo*w + x*w_lo) first,
     // then the tf32 main MMAs (x_hi*w_hi).
-    const void* in0_lo; const void* in1_lo;         // the correction tensors, same chunk layout as in0 / in1
+    const void* in0_lo; const void* in1_lo;         // the correction tensors, same chunk layout as in0 / in1; both null: the
+                                                    // kernel derives the correction chunks from in0 / in1 in shared memory
     float* out_corr;                                // operand-form outputs (non-3x3 / 7x7 geometries, act_out): their correction chunks
     // The vocoder's output forms (Conv1d geometries, and the transposed convs' 1x1 GEMM when voc = 1).  The output dtype is
     // per output, not per mode: an activated output (act_out) is the next conv's operand and takes the mode's operand form
@@ -140,7 +141,7 @@ struct GnActParams {
     const float* mask; int T; int lvl;
     float* out; int B, H, W, C;
     int form;                   // FORM_TF32 | FORM_X3 | FORM_BF16
-    float* out_lo;              // FORM_X3: the correction twin of out
+    float* out_lo;              // FORM_X3: the correction twin of out, or null for none
 };
 
 struct FirstConvParams {        // Block.conv of downs.0.0.block1 on the planar stack([mu, xt(, s)]) * mask
@@ -167,7 +168,7 @@ struct ResFinalParams {         // out = Mish(GN(h2raw))*mask + res(x*mask)
     int B, H, W, C;
     int out_mask;               // planar first block in a tensor-core form: store out*mask (operand form for the next conv)
     int form;                   // layout and number form of x and out (enum Form)
-    float* out_lo;              // FORM_X3: the correction twin of out
+    float* out_lo;              // FORM_X3: the correction twin of out, or null for none
 };
 
 struct AttnCtxParams {          // merge per-tile softmax partials -> normalised context [B][4][32][32]

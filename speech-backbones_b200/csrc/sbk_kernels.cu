@@ -731,7 +731,9 @@ __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
                     reinterpret_cast<uint2*>(p.out)[oi] = make_uint2(pack_bf16x2_f(o.x, o.y), pack_bf16x2_f(o.z, o.w));
                 } else {
                     reinterpret_cast<float4*>(p.out)[oi] = o;
-                    if constexpr (X3) reinterpret_cast<float4*>(p.out_lo)[oi] = corr_chunk(o.x, o.y, o.z, o.w);
+                    if constexpr (X3) {
+                        if (p.out_lo) reinterpret_cast<float4*>(p.out_lo)[oi] = corr_chunk(o.x, o.y, o.z, o.w);
+                    }
                 }
             }
         }
