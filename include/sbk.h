@@ -190,7 +190,8 @@ int sbk_debug_num(const sbk_handle* h);
 const char* sbk_debug_name(const sbk_handle* h, int i);
 
 /* ---- the step after the path (SURVEY.md 8f rank 3): the HiFi-GAN generator, mel -> waveform ----------------------------
- * Grad-TTS/hifi-gan/models.py:77-128 (Generator) with ResBlock1 (:13-49), built from Grad-TTS/checkpts/hifigan-config.json and
+ * Grad-TTS/hifi-gan/models.py:77-128 (Generator) with ResBlock1 (:13-49) or ResBlock2 (:53-74, sbk_vocoder_create_ex), built
+ * from Grad-TTS/checkpts/hifigan-config.json (or the public HiFi-GAN V3 config) and
  * called as `vocoder.forward(y_dec)` at Grad-TTS/inference.py:81 after `remove_weight_norm()` (:63).  The fields below are that
  * JSON's; weights are the generator's state_dict AFTER remove_weight_norm ("conv_pre.weight" [C0,num_mels,7],
  * "ups.i.weight" [Cin,Cout,k], "resblocks.n.convs{1,2}.j.weight" [C,C,k], "conv_post.weight" [1,C,7] and the biases).
@@ -213,7 +214,30 @@ typedef struct sbk_vocoder_config {
     int32_t resblock_kernel_sizes[3];     /* [3, 7, 11]                                                */
     int32_t resblock_dilations[3][3];     /* [[1,3,5],[1,3,5],[1,3,5]]                                 */
 } sbk_vocoder_config;
-int sbk_vocoder_create(const sbk_vocoder_config* cfg, sbk_vocoder** out);        /* Generator.__init__, models.py:78-101 */
+/* Generator.__init__, models.py:78-101, for a ResBlock1 generator (HiFi-GAN V1).  SBK_ERR_UNSUPPORTED unless there are 1..4
+ * upsample stages with k = 2 * rate and an even rate, every stage has a multiple of 32 channels, there are 3 resblock
+ * kernels, and every halo (k-1)*d is at most 64 samples.  Equivalent to sbk_vocoder_create_ex with resblock = 1 under that
+ * tighter halo limit. */
+int sbk_vocoder_create(const sbk_vocoder_config* cfg, sbk_vocoder** out);
+/* The fields of sbk_vocoder_config plus the config's "resblock": 1 (ResBlock1, models.py:13-49: convs1 / convs2 at all three
+ * dilations) or 2 (ResBlock2, :53-74: two convs, at the first two dilations of each kernel; HiFi-GAN V3).  ResBlock2
+ * weights are "resblocks.n.convs.j.weight" [C,C,k] (j < 2) and their biases. */
+typedef struct sbk_vocoder_config_ex {
+    int32_t device;
+    int32_t num_mels;
+    int32_t upsample_initial_channel;
+    int32_t n_ups;
+    int32_t upsample_rates[4];
+    int32_t upsample_kernel_sizes[4];
+    int32_t n_kernels;
+    int32_t resblock_kernel_sizes[3];     /* each 3, 5, 7 or 11                                        */
+    int32_t resblock_dilations[3][3];     /* ResBlock2 reads [j][0] and [j][1]                         */
+    int32_t resblock;                     /* 1 or 2                                                    */
+} sbk_vocoder_config_ex;
+/* The limits of sbk_vocoder_create, except that a halo (k-1)*d may reach 128 samples (a launch whose halo exceeds 64 runs on
+ * the wide Conv1d strip); d >= 1.  SBK_ERR_UNSUPPORTED names the rule a refused config breaks (HiFi-GAN V2's 16- and
+ * 8-channel stages break the 32-channel rule). */
+int sbk_vocoder_create_ex(const sbk_vocoder_config_ex* cfg, sbk_vocoder** out);
 void sbk_vocoder_destroy(sbk_vocoder* v);
 int sbk_vocoder_num_weights(const sbk_vocoder* v);
 const char* sbk_vocoder_weight_name(const sbk_vocoder* v, int i);
@@ -232,7 +256,8 @@ int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav, int B, int
 int64_t sbk_vocoder_last_launch_count(const sbk_vocoder* v);
 /* test hook: when on, sbk_vocoder_forward copies every tensor it writes right after the launch that wrote it (the workspace
  * buffers are reused within a call) into a per-name device buffer; the copies do not count as launches.  Names in launch
- * order: mel_in, conv_pre, ups.i.{z,x,a}, resblocks.n.convs1.d, resblocks.n.convs2.d.x (and .a for d < 2), mrf.i, wav.
+ * order: mel_in, conv_pre, ups.i.{z,x,a}, resblocks.n.convs1.d, resblocks.n.convs2.d.x (and .a for d < 2), mrf.i, wav;
+ * a ResBlock2 generator captures resblocks.n.convs.0.x, resblocks.n.convs.0.a, resblocks.n.convs.1.x for each block.
  * Activations keep the kernel layout (sbk_vocoder_debug_op_layout); wav is [B][1][L].  The fp32x3 correction chunks are not
  * captured: they are a function of the fp32 tensor they accompany. */
 int sbk_vocoder_debug_capture(sbk_vocoder* v, int on);

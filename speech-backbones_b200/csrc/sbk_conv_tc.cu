@@ -67,13 +67,22 @@ template <> struct Geo<G_DOWN> { static constexpr int ROWS = 1, HR = 3, PXP = 2 
 // all four phases are computed from one halo tile into 4 accumulators; the stage carries all 16 (kh,kw) taps.
 template <> struct Geo<G_UP> { static constexpr int ROWS = 1, HR = 3, PXP = TPX + 2, TAPS = 16, KCH = 2, NACC = 4; };
 
-// Conv1d, K taps, runtime dilation d (HiFi-GAN: K in {3,7,11}, d in {1,3,5}; halo (K-1)*d <= 50 samples): ONE strip of
-// TPX + 64 samples per channel chunk; tap t is the descriptor start t*d samples into it - each input sample is fetched
-// once for all taps.
-template <int K> struct GeoC1 { static constexpr int ROWS = 1, HR = 1, PXP = TPX + 64, TAPS = K, KCH = 2, NACC = 1; };
+// Conv1d, K taps, runtime dilation d (HiFi-GAN V1: K in {3,7,11}, d in {1,3,5}; halo (K-1)*d <= 50 samples): ONE strip of
+// TPX + HALO samples per channel chunk; tap t is the descriptor start t*d samples into it - each input sample is fetched
+// once for all taps.  HALO = 64, or 128 for the wide geometries G_C1K*W (V3's K = 7 at d = 12: 72 samples); the strip
+// width only changes the A tile, so both widths read the same weight image.
+template <int K, int HALO = 64> struct GeoC1 { static constexpr int ROWS = 1, HR = 1, PXP = TPX + HALO, TAPS = K, KCH = 2, NACC = 1; };
 template <> struct Geo<G_C1K3> : GeoC1<3> {};
+template <> struct Geo<G_C1K5> : GeoC1<5> {};
 template <> struct Geo<G_C1K7> : GeoC1<7> {};
 template <> struct Geo<G_C1K11> : GeoC1<11> {};
+template <> struct Geo<G_C1K3W> : GeoC1<3, 128> {};
+template <> struct Geo<G_C1K5W> : GeoC1<5, 128> {};
+template <> struct Geo<G_C1K7W> : GeoC1<7, 128> {};
+template <> struct Geo<G_C1K11W> : GeoC1<11, 128> {};
+static_assert(Geo<G_C1K3>::PXP == TPX + conv_tc_c1_halo(G_C1K3) && Geo<G_C1K3W>::PXP == TPX + conv_tc_c1_halo(G_C1K3W), "strip widths");
+// (a wide strip row is the longest run copied from ConvTcParams::zero_page)
+static_assert(Geo<G_C1K3W>::PXP * 16 <= 4096, "zero page");
 
 // 7x7, pad 3 (PostNet): a 3x3-style stage (halo tile + all taps of one 8-channel K step) would carry 49 x 2 x NT x 16 B
 // of weights - 200 KB at NT = 128 - and leave no room for a second stage.  A K step is therefore split by kernel row:
@@ -865,11 +874,38 @@ static constexpr int tc_key(int geom, int form, int nt, int rows = 1, bool res =
     return ((((geom * 4 + form) * 256 + nt) * 2 + rows - 1) * 2 + (res ? 1 : 0)) * 2 + (voc ? 1 : 0);
 }
 
+// Conv1d (vocoder): tf32 and bf16 at N tiles 128 / 64 / 32, fp32x3 at 64 / 32 (conv_tc_ntile)
+template <int GEOM> static int launch_c1(const ConvTcParams& p, cudaStream_t s) {
+    constexpr int T = FORM_TF32, X = FORM_X3, B = FORM_BF16;
+    switch (tc_key(GEOM, p.form, p.nt)) {
+        case tc_key(GEOM, T, 128): return launch_tc<GEOM, T, 128>(p, s);
+        case tc_key(GEOM, T, 64):  return launch_tc<GEOM, T, 64>(p, s);
+        case tc_key(GEOM, T, 32):  return launch_tc<GEOM, T, 32>(p, s);
+        case tc_key(GEOM, B, 128): return launch_tc<GEOM, B, 128>(p, s);
+        case tc_key(GEOM, B, 64):  return launch_tc<GEOM, B, 64>(p, s);
+        case tc_key(GEOM, B, 32):  return launch_tc<GEOM, B, 32>(p, s);
+        case tc_key(GEOM, X, 64):  return launch_tc<GEOM, X, 64>(p, s);
+        case tc_key(GEOM, X, 32):  return launch_tc<GEOM, X, 32>(p, s);
+        default:                   return -1;
+    }
+}
+
 int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
     if (p.form < FORM_TF32 || p.form > FORM_BF16 || p.nt <= 0 || p.nt > 128 || p.Cout % p.nt != 0) return -1;
     if (p.geom == G_PW && p.epi == EPI_KV) return launch_attn_kv(p, s);   // fused projection + softmax + context (sbk_attn_x3.cu)
-    if (geom_is_c1(p.geom) && (p.dil < 1 || p.pad < 0 || 2 * p.pad > 64)) return -1;   // the strip carries at most 64 halo samples
+    if (geom_is_c1(p.geom) && (p.dil < 1 || p.pad < 0 || 2 * p.pad > conv_tc_c1_halo(p.geom))) return -1;   // the strip's halo
     if (p.form == FORM_X3 && p.c1 > 0 && (p.in0_lo == nullptr) != (p.in1_lo == nullptr)) return -1;   // twins for both inputs or for neither
+    switch (p.geom) {                                // Conv1d (vocoder): K = 3, 5, 7, 11, each with the 64- and the 128-sample-halo strip
+        case G_C1K3:   return launch_c1<G_C1K3>(p, s);
+        case G_C1K5:   return launch_c1<G_C1K5>(p, s);
+        case G_C1K7:   return launch_c1<G_C1K7>(p, s);
+        case G_C1K11:  return launch_c1<G_C1K11>(p, s);
+        case G_C1K3W:  return launch_c1<G_C1K3W>(p, s);
+        case G_C1K5W:  return launch_c1<G_C1K5W>(p, s);
+        case G_C1K7W:  return launch_c1<G_C1K7W>(p, s);
+        case G_C1K11W: return launch_c1<G_C1K11W>(p, s);
+        default:       break;
+    }
     const int rows = p.geom == G_C3 && p.rows == 2 ? 2 : 1;
     const bool res = p.geom == G_PW && p.epi == EPI_RES;
     const bool voc = p.voc && p.geom == G_PW && p.form == FORM_BF16;     // the vocoder's GEMM: fp32 Z from bf16 operands
@@ -911,31 +947,6 @@ int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
         case tc_key(G_C7, T, 128):                  return launch_tc<G_C7, T, 128>(p, s);
         case tc_key(G_C7, T, 64):                   return launch_tc<G_C7, T, 64>(p, s);
         case tc_key(G_C7, X, 64):                   return launch_tc<G_C7, X, 64>(p, s);
-        // Conv1d (vocoder)
-        case tc_key(G_C1K3, T, 128):                return launch_tc<G_C1K3, T, 128>(p, s);
-        case tc_key(G_C1K3, T, 64):                 return launch_tc<G_C1K3, T, 64>(p, s);
-        case tc_key(G_C1K3, T, 32):                 return launch_tc<G_C1K3, T, 32>(p, s);
-        case tc_key(G_C1K3, B, 128):                return launch_tc<G_C1K3, B, 128>(p, s);
-        case tc_key(G_C1K3, B, 64):                 return launch_tc<G_C1K3, B, 64>(p, s);
-        case tc_key(G_C1K3, B, 32):                 return launch_tc<G_C1K3, B, 32>(p, s);
-        case tc_key(G_C1K3, X, 64):                 return launch_tc<G_C1K3, X, 64>(p, s);
-        case tc_key(G_C1K3, X, 32):                 return launch_tc<G_C1K3, X, 32>(p, s);
-        case tc_key(G_C1K7, T, 128):                return launch_tc<G_C1K7, T, 128>(p, s);
-        case tc_key(G_C1K7, T, 64):                 return launch_tc<G_C1K7, T, 64>(p, s);
-        case tc_key(G_C1K7, T, 32):                 return launch_tc<G_C1K7, T, 32>(p, s);
-        case tc_key(G_C1K7, B, 128):                return launch_tc<G_C1K7, B, 128>(p, s);
-        case tc_key(G_C1K7, B, 64):                 return launch_tc<G_C1K7, B, 64>(p, s);
-        case tc_key(G_C1K7, B, 32):                 return launch_tc<G_C1K7, B, 32>(p, s);
-        case tc_key(G_C1K7, X, 64):                 return launch_tc<G_C1K7, X, 64>(p, s);
-        case tc_key(G_C1K7, X, 32):                 return launch_tc<G_C1K7, X, 32>(p, s);
-        case tc_key(G_C1K11, T, 128):               return launch_tc<G_C1K11, T, 128>(p, s);
-        case tc_key(G_C1K11, T, 64):                return launch_tc<G_C1K11, T, 64>(p, s);
-        case tc_key(G_C1K11, T, 32):                return launch_tc<G_C1K11, T, 32>(p, s);
-        case tc_key(G_C1K11, B, 128):               return launch_tc<G_C1K11, B, 128>(p, s);
-        case tc_key(G_C1K11, B, 64):                return launch_tc<G_C1K11, B, 64>(p, s);
-        case tc_key(G_C1K11, B, 32):                return launch_tc<G_C1K11, B, 32>(p, s);
-        case tc_key(G_C1K11, X, 64):                return launch_tc<G_C1K11, X, 64>(p, s);
-        case tc_key(G_C1K11, X, 32):                return launch_tc<G_C1K11, X, 32>(p, s);
         default:                                    return -1;
     }
 }

@@ -11,10 +11,15 @@ constexpr int kDimHead = 32;
 constexpr int kAttnHidden = 128;  // heads * dim_head
 constexpr int kKvPartFloats = 32 + 32 + 32 * 32;   // per (tile, head): max[32], sum[32], S[32][32]
 
-// G_C1K*: Conv1d with K taps and a runtime dilation over [B][1][C/4][L][4] tensors (the HiFi-GAN vocoder, sbk_vocoder.cu)
+// G_C1K*: Conv1d with K taps and a runtime dilation over [B][1][C/4][L][4] tensors (the HiFi-GAN vocoder, sbk_vocoder.cu);
+// the strip of a G_C1K*W geometry carries a halo (K-1)*dil of up to 128 samples instead of 64 (conv_tc_c1_halo)
 // G_C7: 7x7 conv, pad 3, stride 1 (DiffVC's PostNet Block, sbk_postnet.cu): tf32 operands or fp32x3, EPI_PLAIN output
-enum Geom { G_PW = 0, G_C3 = 1, G_DOWN = 2, G_UP = 3, G_C1K3 = 4, G_C1K7 = 5, G_C1K11 = 6, G_C7 = 7 };
-__host__ __device__ constexpr bool geom_is_c1(int g) { return g >= G_C1K3 && g <= G_C1K11; }
+enum Geom { G_PW = 0, G_C3 = 1, G_DOWN = 2, G_UP = 3, G_C1K3 = 4, G_C1K7 = 5, G_C1K11 = 6, G_C7 = 7, G_C1K5 = 8,
+            G_C1K3W = 9, G_C1K5W = 10, G_C1K7W = 11, G_C1K11W = 12 };
+__host__ __device__ constexpr bool geom_c1_wide(int g) { return g >= G_C1K3W && g <= G_C1K11W; }
+__host__ __device__ constexpr bool geom_is_c1(int g) { return (g >= G_C1K3 && g <= G_C1K11) || g == G_C1K5 || geom_c1_wide(g); }
+// the largest halo (K-1)*dil, in samples, that a Conv1d geometry's strip carries
+__host__ __device__ constexpr int conv_tc_c1_halo(int g) { return geom_c1_wide(g) ? 128 : 64; }
 enum Pro { PRO_NONE = 0, PRO_MASK = 1, PRO_GN = 2 };
 enum Epi { EPI_PLAIN = 0, EPI_RES = 1, EPI_KV = 2 };
 
@@ -80,7 +85,8 @@ struct ConvTcParams {
     const float* rraw; GnRef rgn;                   // EPI_RES: out = acc + bias + Mish(GN(rraw))*mask
     float* kv_part;                                 // EPI_KV: [B][ceil(HW/attn_kv_tile_pixels())][4][kKvPartFloats]
     const float* addin;                             // EPI_PLAIN: out += addin (same shape/layout/dtype as out): residual added in fp32
-    const float* zero_page;                         // >= 4 KB of zeros in global memory (out-of-image parts of A tiles)
+    const float* zero_page;                         // >= 4 KB of zeros in global memory (out-of-image parts of A tiles; the
+                                                    // longest run is a wide Conv1d strip row, 256 samples x 16 B)
     int nt;                                         // N tile: the width the weights were packed with (conv_tc_ntile, or 64 for
                                                     // the U-Net's second 3x3 image, used when 128-wide tiles cannot fill the GPU)
     int rows;                                       // G_C3: output rows per tile, 1 (0 = 1) or 2; 2 runs 64-wide N tiles (nt = 64)
@@ -113,7 +119,8 @@ struct ConvTcWImg { int form, nt, ksteps, taps, kch; };        // ksteps: K stag
 
 __host__ __device__ constexpr int form_epc(int form) { return form == FORM_BF16 ? 8 : 4; }      // elements per 16-byte chunk
 __host__ __device__ constexpr int conv_tc_taps(int geom) {
-    return geom == G_PW ? 1 : geom == G_UP ? 16 : geom == G_C1K3 ? 3 : geom == G_C1K7 ? 7 : geom == G_C1K11 ? 11 : geom == G_C7 ? 49 : 9;
+    return geom == G_PW ? 1 : geom == G_UP ? 16 : geom == G_C1K3 || geom == G_C1K3W ? 3 : geom == G_C1K5 || geom == G_C1K5W ? 5
+         : geom == G_C1K7 || geom == G_C1K7W ? 7 : geom == G_C1K11 || geom == G_C1K11W ? 11 : geom == G_C7 ? 49 : 9;
 }
 __host__ __device__ constexpr int conv_tc_stage_rows(int geom) { return geom == G_C7 ? 7 : 1; }  // weight stages per K step
 __host__ __device__ constexpr int conv_tc_kch(int geom) { return geom == G_PW ? 8 : 2; }         // 16-byte chunks per stage

@@ -1,11 +1,12 @@
 // HiFi-GAN generator (mel -> waveform), the step immediately after the sampler: Grad-TTS/hifi-gan/models.py:77-128 (Generator),
-// :13-49 (ResBlock1), called at Grad-TTS/inference.py:81.  SURVEY.md 8(f) rank 3.
+// :13-49 (ResBlock1) or :53-74 (ResBlock2, HiFi-GAN V3), called at Grad-TTS/inference.py:81.  SURVEY.md 8(f) rank 3.
 //
 // Mapping onto the sampler's wgmma kernels (sbk_conv_tc.cu), all activations fp32 [B][C/4][L][4] (the 2-D layout with H = 1):
-//   * Conv1d(K in {3,7,11}, dilation d)   -> k_conv_tc<G_C1K*>: one strip of 128 + 64 samples per channel chunk in shared memory,
-//                                            tap t of the wgmma A operand = descriptor start + t*d samples; bias, LeakyReLU and
-//                                            the ResBlock residual (x + conv2(...), models.py:47) live in its epilogue, which
-//                                            also writes lrelu(x) - the next conv's operand - so no activation pass exists;
+//   * Conv1d(K in {3,5,7,11}, dilation d) -> k_conv_tc<G_C1K*>: one strip of 128 + 64 samples per channel chunk in shared memory
+//                                            (128 + 128, G_C1K*W, for a launch whose halo (K-1)*d exceeds 64), tap t of the
+//                                            wgmma A operand = descriptor start + t*d samples; bias, LeakyReLU and the ResBlock
+//                                            residual (x + conv2(...), models.py:47; x + conv_d(...), :68) live in its epilogue,
+//                                            which also writes lrelu(x) - the next conv's operand - so no activation pass exists;
 //   * ConvTranspose1d(k = 2u, stride u)   -> ONE 1x1 GEMM (k_conv_tc<G_PW>) to k*Cout channels, Z[i][t][co] = sum_ci x[i][ci] w[ci][co][t],
 //                                            then k_ct_fold adds the two taps that reach each output sample (o = u*i - p + t), the
 //                                            bias and the LeakyReLU.  (A transposed conv with k = 2u is exactly a 2-tap overlap-add.)
@@ -146,7 +147,7 @@ bool prec_bf16(int precision) { return precision == SBK_PREC_BF16; }
 }  // namespace
 
 struct sbk_vocoder {
-    sbk_vocoder_config cfg;
+    sbk_vocoder_config_ex cfg;
     int precision = SBK_PREC_TF32;
     WeightSet w;                             // raw: reference layout (after remove_weight_norm); packed: tensor-core stage images
     float* zero = nullptr;
@@ -162,11 +163,26 @@ struct sbk_vocoder {
     int form() const { return x3() ? FORM_X3 : (bf16() ? FORM_BF16 : FORM_TF32); }
 };
 
-static int voc_geom(int k) { return k == 3 ? G_C1K3 : (k == 7 ? G_C1K7 : (k == 11 ? G_C1K11 : -1)); }
+// the Conv1d geometry of a kernel size: the 64-sample-halo strip, or the 128-sample one when the launch's halo (K-1)*dil
+// needs it (both read the weight image packed for the narrow geometry); -1 for an unsupported size
+static int voc_geom(int k, int halo = 0) {
+    const bool wide = halo > conv_tc_c1_halo(G_C1K3);
+    switch (k) {
+        case 3:  return wide ? G_C1K3W : G_C1K3;
+        case 5:  return wide ? G_C1K5W : G_C1K5;
+        case 7:  return wide ? G_C1K7W : G_C1K7;
+        case 11: return wide ? G_C1K11W : G_C1K11;
+        default: return -1;
+    }
+}
 
-extern "C" int sbk_vocoder_create(const sbk_vocoder_config* cfg, sbk_vocoder** out) {
+// dilations a ResBlock applies: ResBlock1 all three, ResBlock2 the first two (models.py:13-74)
+static int voc_ndil(const sbk_vocoder_config_ex& c) { return c.resblock == 2 ? 2 : 3; }
+
+extern "C" int sbk_vocoder_create_ex(const sbk_vocoder_config_ex* cfg, sbk_vocoder** out) {
     if (!cfg || !out) return fail(SBK_ERR_ARG, "sbk_vocoder_create: null argument");
-    if (cfg->n_ups < 1 || cfg->n_ups > 4 || cfg->n_kernels != 3) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: needs 1..4 upsample stages and 3 resblock kernels (HiFi-GAN V1/V2 layout)");
+    if (cfg->resblock != 1 && cfg->resblock != 2) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: resblock %d (HiFi-GAN defines ResBlock1 and ResBlock2)", cfg->resblock);
+    if (cfg->n_ups < 1 || cfg->n_ups > 4 || cfg->n_kernels != 3) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: needs 1..4 upsample stages and 3 resblock kernels (got %d, %d)", cfg->n_ups, cfg->n_kernels);
     if (cfg->num_mels <= 0 || cfg->num_mels % 8 != 0) return fail(SBK_ERR_ARG, "sbk_vocoder_create: num_mels must be a multiple of 8 (one K stage), got %d", cfg->num_mels);
     int ch = cfg->upsample_initial_channel;
     if (ch % 64 != 0) return fail(SBK_ERR_ARG, "sbk_vocoder_create: upsample_initial_channel must be a multiple of 64");
@@ -175,13 +191,16 @@ extern "C" int sbk_vocoder_create(const sbk_vocoder_config* cfg, sbk_vocoder** o
         if (k != 2 * u || u % 2 != 0) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: stage %d: ConvTranspose1d needs k = 2*stride and an even stride (got k=%d, u=%d)", i, k, u);
         if (ch % 32 != 0) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: stage %d input channels %d: need a multiple of 32", i, ch);
         ch /= 2;
-        if (ch % 32 != 0) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: stage %d has %d channels; the tensor-core path needs multiples of 32 (HiFi-GAN V1)", i, ch);
+        if (ch % 32 != 0) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: stage %d has %d channels; the Conv1d tiles need a multiple of 32 (HiFi-GAN V2's 16- and 8-channel stages are not supported)", i, ch);
     }
+    const int halo_max = conv_tc_c1_halo(G_C1K3W);
     for (int j = 0; j < 3; ++j) {
-        if (voc_geom(cfg->resblock_kernel_sizes[j]) < 0) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: resblock kernel %d (supported: 3, 7, 11)", cfg->resblock_kernel_sizes[j]);
-        for (int d = 0; d < 3; ++d) {
+        const int k = cfg->resblock_kernel_sizes[j];
+        if (voc_geom(k) < 0) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: resblock kernel %d (supported: 3, 5, 7, 11)", k);
+        for (int d = 0; d < voc_ndil(*cfg); ++d) {
             const int dil = cfg->resblock_dilations[j][d];
-            if (dil < 1 || (cfg->resblock_kernel_sizes[j] - 1) * dil > 64) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: halo (k-1)*d = %d exceeds 64 samples", (cfg->resblock_kernel_sizes[j] - 1) * dil);
+            if (dil < 1) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: resblock kernel %d: dilation %d", j, dil);
+            if ((k - 1) * dil > halo_max) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: halo (k-1)*d = %d exceeds %d samples", (k - 1) * dil, halo_max);
         }
     }
     sbk_vocoder* v = new sbk_vocoder();
@@ -194,11 +213,13 @@ extern "C" int sbk_vocoder_create(const sbk_vocoder_config* cfg, sbk_vocoder** o
         add("ups." + std::to_string(i) + ".bias", {c0 >> (i + 1)});
     }
     int n = 0;
+    // ResBlock1: convs1.d, convs2.d (d < 3); ResBlock2: convs.d (d < 2)
+    const std::vector<const char*> groups = cfg->resblock == 2 ? std::vector<const char*>{"convs"} : std::vector<const char*>{"convs1", "convs2"};
     for (int i = 0; i < cfg->n_ups; ++i) {
         const int c = c0 >> (i + 1);
         for (int j = 0; j < 3; ++j, ++n)
-            for (const char* grp : {"convs1", "convs2"})
-                for (int d = 0; d < 3; ++d) {
+            for (const char* grp : groups)
+                for (int d = 0; d < voc_ndil(*cfg); ++d) {
                     const std::string q = "resblocks." + std::to_string(n) + "." + grp + "." + std::to_string(d);
                     add(q + ".weight", {c, c, cfg->resblock_kernel_sizes[j]}); add(q + ".bias", {c});
                 }
@@ -206,6 +227,25 @@ extern "C" int sbk_vocoder_create(const sbk_vocoder_config* cfg, sbk_vocoder** o
     add("conv_post.weight", {1, c0 >> cfg->n_ups, 7}); add("conv_post.bias", {1});
     *out = v;
     return SBK_OK;
+}
+
+// The V1 entry point: a ResBlock1 generator with its documented 64-sample halo limit.
+extern "C" int sbk_vocoder_create(const sbk_vocoder_config* cfg, sbk_vocoder** out) {
+    if (!cfg || !out) return fail(SBK_ERR_ARG, "sbk_vocoder_create: null argument");
+    sbk_vocoder_config_ex ex;
+    memset(&ex, 0, sizeof(ex));
+    ex.device = cfg->device; ex.num_mels = cfg->num_mels; ex.upsample_initial_channel = cfg->upsample_initial_channel;
+    ex.n_ups = cfg->n_ups; ex.n_kernels = cfg->n_kernels; ex.resblock = 1;
+    memcpy(ex.upsample_rates, cfg->upsample_rates, sizeof(ex.upsample_rates));
+    memcpy(ex.upsample_kernel_sizes, cfg->upsample_kernel_sizes, sizeof(ex.upsample_kernel_sizes));
+    memcpy(ex.resblock_kernel_sizes, cfg->resblock_kernel_sizes, sizeof(ex.resblock_kernel_sizes));
+    memcpy(ex.resblock_dilations, cfg->resblock_dilations, sizeof(ex.resblock_dilations));
+    for (int j = 0; j < 3; ++j)
+        for (int d = 0; d < 3; ++d) {
+            const int halo = (cfg->resblock_kernel_sizes[j] - 1) * cfg->resblock_dilations[j][d];
+            if (halo > conv_tc_c1_halo(G_C1K3)) return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_create: halo (k-1)*d = %d exceeds 64 samples (sbk_vocoder_create_ex takes up to 128)", halo);
+        }
+    return sbk_vocoder_create_ex(&ex, out);
 }
 
 extern "C" void sbk_vocoder_destroy(sbk_vocoder* v) {
@@ -291,7 +331,7 @@ struct VocBufs {
 };
 
 size_t voc_carve(const sbk_vocoder* v, int B, int T, Arena& ar, VocBufs* o) {
-    const sbk_vocoder_config& c = v->cfg;
+    const sbk_vocoder_config_ex& c = v->cfg;
     size_t big = 0, zmax = 0;
     { long long L = T; int ch = c.upsample_initial_channel; big = (size_t)B * ch * L;
       for (int i = 0; i < c.n_ups; ++i) { zmax = std::max<size_t>(zmax, (size_t)B * c.upsample_kernel_sizes[i] * (ch / 2) * L); L *= c.upsample_rates[i]; ch /= 2; big = std::max<size_t>(big, (size_t)B * ch * L); } }
@@ -329,7 +369,7 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
     if (B <= 0 || T <= 0) return fail(SBK_ERR_ARG, "sbk_vocoder_forward: B and T must be positive (got %d, %d)", B, T);
     CU(cudaSetDevice(v->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
-    const sbk_vocoder_config& c = v->cfg;
+    const sbk_vocoder_config_ex& c = v->cfg;
     const size_t need = sbk_vocoder_workspace_bytes(v, B, T);
     if (v->ws.reserve(need)) return fail(SBK_ERR_CUDA, "out of memory: the vocoder workspace for (B=%d, T=%d) needs %zu bytes", B, T, need);
     VocBufs wb;
@@ -382,18 +422,30 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
         ch = co; L = Lo;
         const size_t na = bn * ch * L;
         for (int j = 0; j < 3; ++j, ++rb) {
-            const int geom = voc_geom(c.resblock_kernel_sizes[j]);
+            const int k = c.resblock_kernel_sizes[j];
             const std::string rp = "resblocks." + std::to_string(rb);
-            // per dilation d: xt = conv2(lrelu(conv1_d(lrelu(x)))); x = xt + x   (models.py:42-47)
-            conv(geom, rp + ".convs1.0", A0, wb.A0_lo, ch, ch, L, c.resblock_dilations[j][0], Hb, 1, nullptr, nullptr, wb.Hb_lo);
+            if (c.resblock == 2) {
+                // per dilation d: x = conv_d(lrelu(x)) + x   (models.py:64-69); the second conv's x is the block output
+                const int d0 = c.resblock_dilations[j][0], d1 = c.resblock_dilations[j][1];
+                conv(voc_geom(k, (k - 1) * d0), rp + ".convs.0", A0, wb.A0_lo, ch, ch, L, d0, X1, 0, X0, A1, wb.A1_lo);
+                snap(rp, ".convs.0.x", X1, na, 1); snap(rp, ".convs.0.a", A1, na, ofmt);
+                conv(voc_geom(k, (k - 1) * d1), rp + ".convs.1", A1, wb.A1_lo, ch, ch, L, d1, R[j], 0, X1, nullptr, nullptr);
+                snap(rp, ".convs.1.x", R[j], na, 1);
+                continue;
+            }
+            const int geom = voc_geom(k);
+            // per dilation d: xt = conv2(lrelu(conv1_d(lrelu(x)))); x = xt + x   (models.py:42-47); the dilated convs1 pick
+            // their strip from the halo
+            auto g1 = [&](int d) { return voc_geom(k, (k - 1) * c.resblock_dilations[j][d]); };
+            conv(g1(0), rp + ".convs1.0", A0, wb.A0_lo, ch, ch, L, c.resblock_dilations[j][0], Hb, 1, nullptr, nullptr, wb.Hb_lo);
             snap(rp, ".convs1.0", Hb, na, ofmt);
             conv(geom, rp + ".convs2.0", Hb, wb.Hb_lo, ch, ch, L, 1, X1, 0, X0, A1, wb.A1_lo);
             snap(rp, ".convs2.0.x", X1, na, 1); snap(rp, ".convs2.0.a", A1, na, ofmt);
-            conv(geom, rp + ".convs1.1", A1, wb.A1_lo, ch, ch, L, c.resblock_dilations[j][1], Hb, 1, nullptr, nullptr, wb.Hb_lo);
+            conv(g1(1), rp + ".convs1.1", A1, wb.A1_lo, ch, ch, L, c.resblock_dilations[j][1], Hb, 1, nullptr, nullptr, wb.Hb_lo);
             snap(rp, ".convs1.1", Hb, na, ofmt);
             conv(geom, rp + ".convs2.1", Hb, wb.Hb_lo, ch, ch, L, 1, X2, 0, X1, A2, wb.A2_lo);
             snap(rp, ".convs2.1.x", X2, na, 1); snap(rp, ".convs2.1.a", A2, na, ofmt);
-            conv(geom, rp + ".convs1.2", A2, wb.A2_lo, ch, ch, L, c.resblock_dilations[j][2], Hb, 1, nullptr, nullptr, wb.Hb_lo);
+            conv(g1(2), rp + ".convs1.2", A2, wb.A2_lo, ch, ch, L, c.resblock_dilations[j][2], Hb, 1, nullptr, nullptr, wb.Hb_lo);
             snap(rp, ".convs1.2", Hb, na, ofmt);
             conv(geom, rp + ".convs2.2", Hb, wb.Hb_lo, ch, ch, L, 1, R[j], 0, X2, nullptr, nullptr);
             snap(rp, ".convs2.2.x", R[j], na, 1);

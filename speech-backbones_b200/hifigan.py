@@ -7,10 +7,14 @@
     vocoder.remove_weight_norm()                                             # :63
     audio = vocoder.forward(y_dec)                                           # :81   mel [B,80,T] -> wav [B,1,256*T]
 
-Same constructor argument, same parameter names (`conv_pre.weight_g/_v`, `ups.i.*`, `resblocks.n.convs{1,2}.j.*`, `conv_post.*`,
-and the plain `.weight` names after `remove_weight_norm()`), so the reference checkpoint loads with `strict=True`.  The modules
-below are parameter containers only: `forward` runs in libsbk.so (`sbk_vocoder_forward`: dilated Conv1d and the transposed
-convs on wgmma, see csrc/sbk_vocoder.cu).  There is no CPU or eager-PyTorch path: calling `forward` with CPU tensors raises.
+Same constructor argument, same parameter names (`conv_pre.weight_g/_v`, `ups.i.*`, `resblocks.n.convs{1,2}.j.*` for a
+ResBlock1 config, `resblocks.n.convs.j.*` for a ResBlock2 one, `conv_post.*`, and the plain `.weight` names after
+`remove_weight_norm()`), so the reference checkpoint loads with `strict=True`.  `h.resblock` picks the block as models.py:84
+does: V1 (resblock "1") and V3 (resblock "2", spec.HIFIGAN_V3) both run; V2's 16- and 8-channel stages are refused (the
+Conv1d tiles need multiples of 32 channels).  Dilated convs with a halo (k-1)*d of up to 128 samples run.  The modules
+below are parameter containers only: `forward` runs in libsbk.so (`sbk_vocoder_create_ex` / `sbk_vocoder_forward`: dilated
+Conv1d and the transposed convs on wgmma, see csrc/sbk_vocoder.cu).  There is no CPU or eager-PyTorch path: calling
+`forward` with CPU tensors raises.
 
 `Generator(h, precision=...)` picks the operand arithmetic of those convs (the binding's PREC names): "tf32" (the default),
 "fp32x3" ("fp32" maps to it: fp32-class results on the tensor cores) or "bf16".  In the bf16 mode `forward` also takes a
@@ -41,6 +45,20 @@ def _padding(k, d=1):
     return (k * d - d) // 2                                   # xutils.get_padding
 
 
+def _resblock(h):
+    """the engine's block type, 1 or 2.  models.py:84 (and Generator below) take ResBlock2 for any resblock other than '1';
+    the engine runs only the values HiFi-GAN's configs use and names any other"""
+    rb = str(_get(h, "resblock", "1"))
+    if rb not in ("1", "2"):
+        raise RuntimeError(f"resblock {rb!r}: HiFi-GAN configs use '1' (ResBlock1, V1/V2) or '2' (ResBlock2, V3)")
+    return int(rb)
+
+
+class SbkVocoderConfigEx(C.Structure):
+    """sbk_vocoder_config_ex: sbk_vocoder_config's fields plus the config's resblock (1 or 2)"""
+    _fields_ = SbkVocoderConfig._fields_ + [("resblock", C.c_int32)]
+
+
 class _ResBlock1(nn.Module):                                   # reference name: ResBlock1 (models.py:13-49)
     def __init__(self, ch, k, dilations):
         super().__init__()
@@ -49,6 +67,17 @@ class _ResBlock1(nn.Module):                                   # reference name:
 
     def remove_weight_norm(self):
         for l in list(self.convs1) + list(self.convs2):
+            remove_weight_norm(l)
+
+
+class _ResBlock2(nn.Module):                                   # reference name: ResBlock2 (models.py:53-74)
+    def __init__(self, ch, k, dilations):
+        super().__init__()
+        self.convs = nn.ModuleList([weight_norm(nn.Conv1d(ch, ch, k, 1, dilation=d, padding=_padding(k, d)))
+                                    for d in (dilations[0], dilations[1])])
+
+    def remove_weight_norm(self):
+        for l in self.convs:
             remove_weight_norm(l)
 
 
@@ -74,20 +103,25 @@ class VocoderEngine(_NativeHandle):
         self.lib.sbk_vocoder_debug_read.argtypes = [P, C.c_char_p, P, C.POINTER(C.c_int64)]
         rates, ks = list(_get(h, "upsample_rates")), list(_get(h, "upsample_kernel_sizes"))
         rk, rd = list(_get(h, "resblock_kernel_sizes")), [list(d) for d in _get(h, "resblock_dilation_sizes")]
-        if str(_get(h, "resblock", "1")) != "1":
-            raise RuntimeError("only ResBlock1 generators (HiFi-GAN V1/V2 configs, resblock='1') are supported")
-        if len(rates) > 4 or len(rk) != 3 or any(len(d) != 3 for d in rd):
-            raise RuntimeError("unsupported HiFi-GAN configuration (need <= 4 upsample stages, 3 resblock kernels x 3 dilations)")
-        cfg = SbkVocoderConfig()
-        cfg.device, cfg.num_mels = device, int(_get(h, "num_mels", 80))
+        rb = _resblock(h)
+        nd = 3 if rb == 1 else 2                                 # dilations the block applies (models.py:13-74)
+        if len(rates) > 4:
+            raise RuntimeError(f"unsupported HiFi-GAN configuration: {len(rates)} upsample stages (at most 4)")
+        if len(rk) != 3 or len(rd) != 3 or any(len(d) < nd or (rb == 1 and len(d) != 3) for d in rd):
+            raise RuntimeError(f"unsupported HiFi-GAN configuration: ResBlock{rb} needs 3 resblock kernels with "
+                               f"{'3' if rb == 1 else 'at least 2'} dilations each (got {rk}, {rd})")
+        cfg = SbkVocoderConfigEx()
+        cfg.device, cfg.num_mels, cfg.resblock = device, int(_get(h, "num_mels", 80)), rb
         cfg.upsample_initial_channel, cfg.n_ups, cfg.n_kernels = int(_get(h, "upsample_initial_channel")), len(rates), len(rk)
         for i, (u, k) in enumerate(zip(rates, ks)):
             cfg.upsample_rates[i], cfg.upsample_kernel_sizes[i] = u, k
         for j in range(3):
             cfg.resblock_kernel_sizes[j] = rk[j]
-            for d in range(3):
+            for d in range(nd):
                 cfg.resblock_dilations[j][d] = rd[j][d]
-        _check(self._create(cfg), "sbk_vocoder_create")
+        create = self.lib.sbk_vocoder_create_ex
+        create.argtypes = [C.POINTER(SbkVocoderConfigEx), C.POINTER(C.c_void_p)]
+        _check(create(C.byref(cfg), C.byref(self.h)), "sbk_vocoder_create_ex")
         rc = self.lib.sbk_vocoder_set_precision(self.h, PREC[precision])
         if rc != 0:
             self.close()
@@ -176,12 +210,13 @@ class Generator(nn.Module):
         self.conv_pre = weight_norm(nn.Conv1d(int(_get(h, "num_mels", 80)), c0, 7, 1, padding=3))
         self.ups = nn.ModuleList([weight_norm(nn.ConvTranspose1d(c0 // 2 ** i, c0 // 2 ** (i + 1), k, u, padding=(k - u) // 2))
                                   for i, (u, k) in enumerate(zip(rates, ks))])
+        resblock = _ResBlock1 if str(_get(h, "resblock", "1")) == "1" else _ResBlock2     # models.py:84
         self.resblocks = nn.ModuleList()
         ch = c0
         for i in range(len(rates)):
             ch = c0 // 2 ** (i + 1)
             for k, d in zip(rk, rd):
-                self.resblocks.append(_ResBlock1(ch, k, d))
+                self.resblocks.append(resblock(ch, k, d))
         self.conv_post = weight_norm(nn.Conv1d(ch, 1, 7, 1, padding=3))
         self._engine = None
         self._engine_sig = None

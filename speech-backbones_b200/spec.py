@@ -214,20 +214,27 @@ HIFIGAN_V1 = dict(upsample_rates=[8, 8, 2, 2], upsample_kernel_sizes=[16, 16, 4,
                   resblock_kernel_sizes=[3, 7, 11], resblock_dilation_sizes=[[1, 3, 5], [1, 3, 5], [1, 3, 5]], num_mels=80)
 
 
+# the public HiFi-GAN config_v3.json: ResBlock2 (two convs per block), 1,462,273 parameters after remove_weight_norm
+HIFIGAN_V3 = dict(resblock="2", upsample_rates=[8, 8, 4], upsample_kernel_sizes=[16, 16, 8], upsample_initial_channel=256,
+                  resblock_kernel_sizes=[3, 5, 7], resblock_dilation_sizes=[[1, 2], [2, 6], [3, 12]], num_mels=80)
+
+
 def hifigan_param_spec(h=None):
-    """[(name, shape)] of the HiFi-GAN V1 generator's state_dict after remove_weight_norm
-    (Grad-TTS/hifi-gan/models.py:77-101, Grad-TTS/checkpts/hifigan-config.json; inference.py:60-63)."""
+    """[(name, shape)] of the HiFi-GAN generator's state_dict after remove_weight_norm (`h`, default V1;
+    Grad-TTS/hifi-gan/models.py:77-101, Grad-TTS/checkpts/hifigan-config.json; inference.py:60-63).  resblock "1":
+    resblocks.n.convs{1,2}.j per dilation j; "2" (ResBlock2, models.py:53-74): resblocks.n.convs.j for the first two."""
     h = h or HIFIGAN_V1
     c0 = h["upsample_initial_channel"]
     spec = [("conv_pre.weight", (c0, h["num_mels"], 7)), ("conv_pre.bias", (c0,))]
     for i, k in enumerate(h["upsample_kernel_sizes"]):
         spec += [(f"ups.{i}.weight", (c0 // 2 ** i, c0 // 2 ** (i + 1), k)), (f"ups.{i}.bias", (c0 // 2 ** (i + 1),))]
+    rb2 = str(h.get("resblock", "1")) != "1"
     n, ch = 0, c0
     for i in range(len(h["upsample_rates"])):
         ch = c0 // 2 ** (i + 1)
         for k, d in zip(h["resblock_kernel_sizes"], h["resblock_dilation_sizes"]):
-            for grp in ("convs1", "convs2"):
-                for j in range(len(d)):
+            for grp in (("convs",) if rb2 else ("convs1", "convs2")):
+                for j in range(2 if rb2 else len(d)):
                     spec += [(f"resblocks.{n}.{grp}.{j}.weight", (ch, ch, k)), (f"resblocks.{n}.{grp}.{j}.bias", (ch,))]
             n += 1
     return spec + [("conv_post.weight", (1, ch, 7)), ("conv_post.bias", (1,))]
@@ -236,7 +243,8 @@ def hifigan_param_spec(h=None):
 def synthetic_hifigan_state_dict(seed: int = 1234, h=None):
     """Seeded weights for a HiFi-GAN generator (`h`, default V1) after remove_weight_norm: the reference ships no vocoder
     checkpoint.  He-style scales (std = 1/sqrt(fan_in)) keep the activations O(1) through the 15-conv-deep residual stacks,
-    so the tanh output is neither saturated nor vanishing."""
+    so the tanh output is neither saturated nor vanishing.  Each tensor's seed depends only on its name, so a config's
+    weights do not move when another config is added."""
     import math
     sd = {}
     for name, shape in hifigan_param_spec(h):
