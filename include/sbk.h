@@ -258,8 +258,8 @@ int64_t sbk_vocoder_last_launch_count(const sbk_vocoder* v);
  * buffers are reused within a call) into a per-name device buffer; the copies do not count as launches.  Names in launch
  * order: mel_in, conv_pre, ups.i.{z,x,a}, resblocks.n.convs1.d, resblocks.n.convs2.d.x (and .a for d < 2), mrf.i, wav;
  * a ResBlock2 generator captures resblocks.n.convs.0.x, resblocks.n.convs.0.a, resblocks.n.convs.1.x for each block.
- * Activations keep the kernel layout (sbk_vocoder_debug_op_layout); wav is [B][1][L].  The fp32x3 correction chunks are not
- * captured: they are a function of the fp32 tensor they accompany. */
+ * Activations keep the kernel layout (sbk_vocoder_debug_op_layout); wav is [B][1][L].  fp32x3 captures the same fp32
+ * tensors as tf32: its correction chunks are derived inside the conv kernels and never stored. */
 int sbk_vocoder_debug_capture(sbk_vocoder* v, int on);
 int sbk_vocoder_debug_num(const sbk_vocoder* v);                                  /* names captured by the last forward */
 const char* sbk_vocoder_debug_name(const sbk_vocoder* v, int i);

@@ -39,9 +39,9 @@ HBM_PEAK = 3.35e12                     # H100 SXM5 HBM3, bytes/s
 def hbm_bytes_per_frame(h, mode):
     """Activation bytes per mel frame one call reads and writes in HBM if every launch reads each input element once
     (strip halos and GEMM A re-reads hit L2) and writes each output once; weights are not counted.  A conv input (operand)
-    takes 4 bytes per element in tf32, 2 in bf16, 8 in fp32x3 (fp32 + its correction chunk); the residual stream, the GEMM
-    output and the MRF inputs are fp32."""
-    ob = {"tf32": 4, "bf16": 2, "fp32x3": 8}[mode]
+    takes 4 bytes per element in tf32 and fp32x3 (its correction chunks are derived in shared memory), 2 in bf16; the
+    residual stream, the GEMM output and the MRF inputs are fp32."""
+    ob = {"tf32": 4, "bf16": 2, "fp32x3": 4}[mode]
     rb2 = str(h.get("resblock", "1")) != "1"
     c, nm = h["upsample_initial_channel"], h["num_mels"]
     total = 4 * nm + ob * nm                                  # mel_in

@@ -1197,7 +1197,7 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
     if (!h->is_packed) return fail(SBK_ERR_STATE, "sbk_vc_conditioning: weights not packed");
     if (h->cfg.use_ref_t && h->cfg.dim_cond % 128 != 0) return fail(SBK_ERR_ARG, "sbk_vc_conditioning: dim_cond must be a multiple of 128");
     // fp32-class handles (fp32x3 and the CUDA-core fp32 mode) run the RefBlock convs with the tf32 + fp16-correction split and exact IN / GLU
-    const bool x3 = prec_runs_x3(h->cfg.precision);
+    const int form = prec_runs_x3(h->cfg.precision) ? FORM_X3 : FORM_TF32;
     if (B <= 0 || Tr <= 0 || n_timesteps < 1) return fail(SBK_ERR_ARG, "sbk_vc_conditioning: bad sizes");
     CU(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
@@ -1205,12 +1205,11 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
     const int H = cf.n_feats, dc = cf.dim_cond, base = dc / 4, N = n_timesteps, dim = cf.dim;
     const size_t px = (size_t)B * H * Tr;
     // ---- workspace
-    float *xt_ref, *raw, *act, *act_lo, *tb, *trows; double *st, *ys;
+    float *xt_ref, *raw, *act, *tb, *trows; double *st, *ys;
     auto carve = [&](Arena& ar) {
         xt_ref = (float*)ar.take(px * sizeof(float));
         raw = (float*)ar.take(px * 8 * base * sizeof(float));
         act = (float*)ar.take(px * 4 * base * sizeof(float));
-        act_lo = x3 ? (float*)ar.take(px * 4 * base * sizeof(float)) : nullptr;
         st = (double*)ar.take((size_t)B * 8 * base * 2 * sizeof(double));
         ys = (double*)ar.take((size_t)B * dc * 2 * sizeof(double));
         tb = (float*)ar.take((size_t)N * 3 * base * sizeof(float));
@@ -1249,8 +1248,7 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
         p.geom = G_C3; p.in0 = act; p.c0 = cin; p.H = H; p.W = Tr; p.B = B; p.Ho = H; p.Wo = Tr;
         p.wpk = h->w.get(q + ".wtc"); p.bias = h->w.get(q + ".0.bias"); p.out = raw; p.Cout = cout; p.epi = EPI_PLAIN;
         p.mask = ref_mask; p.T = Tr; p.zero_page = h->d_zero;
-        p.form = x3 ? FORM_X3 : FORM_TF32; p.nt = conv_tc_ntile(G_C3, cout, p.form);     // as sbk_pack packed it
-        if (x3) p.in0_lo = act_lo;
+        p.form = form; p.nt = conv_tc_ntile(G_C3, cout, p.form);     // as sbk_pack packed it
         return launch_conv_tc(p, s);
     };
     // debug capture: every step writes the same workspace buffers, so the last step's tensors are recorded
@@ -1266,7 +1264,7 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
         snap(name, ".stats", st, (size_t)B * C * 2, 3);
         InGluParams g; memset(&g, 0, sizeof(g));
         g.raw = raw; g.stats = st; g.gamma = h->w.get(q + ".1.weight"); g.beta = h->w.get(q + ".1.bias"); g.tb = tbias;
-        g.mask = ref_mask; g.T = Tr; g.out = act; g.out_lo = act_lo; g.B = B; g.H = H; g.W = Tr; g.C = C;
+        g.mask = ref_mask; g.T = Tr; g.out = act; g.B = B; g.H = H; g.W = Tr; g.C = C; g.form = form;
         k += launch_in_glu(g, s);
         snap(name, ".act", act, px * C / 2, 1);
         return k;

@@ -41,8 +41,7 @@ static_assert(SMEM <= 227 * 1024, "shared memory budget");
 static_assert(XS <= OPI && STAGES == 2, "fp32x3: the converted x fits a context image; a K stage is the whole ring");
 }
 
-// MODE: 0 = tf32, 1 = bf16, 2 = fp32x3.  p.in0: x (fp32x3: its correction chunks are derived here, p.in0_lo is not read:
-// the loader brings x with the main sub-stage only and the consumers convert it into the idle Pc / Vc images, alternating
+// MODE: 0 = tf32, 1 = bf16, 2 = fp32x3.  p.in0: x (fp32x3: its correction chunks are derived here: the loader brings x with the main sub-stage only and the consumers convert it into the idle Pc / Vc images, alternating
 // between them per K stage so that one warpgroup may still read the last stage's chunks); p.c0 = C; p.wpk: the k|v rows
 // of to_qkv as per-stage images [k|v][chunk][row][16 B] (fp32x3: [32-channel stage][hi | correction][k|v]...,
 // sbk_conv_tc.cu attn_kv_pack_image);

@@ -112,8 +112,8 @@ template <int GEOM, int NT, int R = 1> struct Depth {
     static_assert(STAGES >= 2, "need at least 2 stages");
     static_assert(SMEM <= 227 * 1024, "shared memory budget");
 };
-// fp32x3 launches without a correction twin derive a correction sub-stage's A tile from the main sub-stage that FOLLOWS it
-// in the ring, so stage g is full only once stage g + 1 has landed.  A consumer that waits for stage g has released every
+// fp32x3 derives a correction sub-stage's A tile from the main sub-stage that FOLLOWS it in the ring, so stage g is full
+// only once stage g + 1 has landed.  A consumer that waits for stage g has released every
 // stage up to g - 2 (one MMA group in flight), and the loader fills stage g + 1 once stage g + 1 - STAGES is released:
 // g + 1 - STAGES <= g - 2, i.e. three stages.  (Downsample's consumers gather stage g + 1 themselves before they convert
 // it, LAG = STAGES - 2 >= 1 stages ahead of the MMAs: three stages again.)
@@ -130,8 +130,7 @@ template <int GEOM, int NT, int R> constexpr bool x3_depth_ok = Depth<GEOM, NT, 
 // second register array.  (Upsample runs unchunked: its runs are short, 4 taps per phase.)
 //
 // VOC: the vocoder's output forms (ConvTcParams::voc) on a 1x1 GEMM; the Conv1d geometries always use them.  They only
-// differ from the sampler's in the bf16 mode (an output is bf16 only when it is an activated operand) and, for fp32x3,
-// in the correction chunks of the second output (act_corr).
+// differ from the sampler's in the bf16 mode (an output is bf16 only when it is an activated operand).
 template <int GEOM, bool BF16, int NT, bool RES, bool X3, bool VOC = false, int R = 1>
 __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     static_assert(!(X3 && BF16), "fp32x3 runs on tf32 operands");
@@ -184,11 +183,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     // fp32x3 mode: each K stage runs twice - the f16 correction sub-stage (x_lo*w + x*w_lo from the packed fp16 chunks,
     // sbk_internal.h: corr_chunk) first, then the tf32 main sub-stage (x_hi*w_hi): small terms first
     const int ksteps_t = X3 ? 2 * ksteps : ksteps;
-    // fp32x3 without a correction twin (in0_lo / in1_lo null): the correction sub-stage's A tile is corr_chunk of the main
-    // sub-stage's tile, computed in shared memory - by the converter warps of the producer warpgroup for the bulk-copy
-    // geometries, by the gathering consumers themselves for Downsample.  The tile is converted whole, so the zero padding
-    // (border columns, out-of-image rows, the ragged end of a 1x1 tile) becomes zero chunks and needs no pattern logic.
-    const bool insm = X3 && p.in0_lo == nullptr;
+    // fp32x3: the correction sub-stage's A tile is corr_chunk of the main sub-stage's tile, computed in shared memory - by
+    // the converter warps of the producer warpgroup for the bulk-copy geometries, by the gathering consumers themselves for
+    // Downsample.  The tile is converted whole, so the zero padding (border columns, out-of-image rows, the ragged end of a
+    // 1x1 tile) becomes zero chunks and needs no pattern logic.
     static_assert(!X3 || x3_depth_ok<GEOM, NT, R>, "in-SM correction operand: stage g needs stage g + 1, three stages");
     // ---- tile space: (sample, pixel tile, N tile), N tile fastest so neighbours in time share the A tile in L2
     const int wt_w = (GEOM == G_DOWN ? p.Wo : p.W), wt_h = (GEOM == G_DOWN ? p.Ho : p.H);
@@ -255,14 +253,12 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 const uint32_t g = it + ks;
                 const int s = g % STAGES;
                 mbar_wait(empty(s), ((g / STAGES) & 1) ^ 1);
-                const int kb = X3 ? ks / 2 : ks;
-                const bool lo = X3 && (ks & 1) == 0;
-                const int ck = kb * KCH;
+                if (X3 && (ks & 1) == 0) return;           // correction sub-stage: converted from the main sub-stage's gathers
+                const int ck = (X3 ? ks / 2 : ks) * KCH;
                 const bool second = ck * EPC >= p.c0;
-                const uint8_t* src = reinterpret_cast<const uint8_t*>(second ? (lo ? p.in1_lo : p.in1) : (lo ? p.in0_lo : p.in0));
+                const uint8_t* src = reinterpret_cast<const uint8_t*>(second ? p.in1 : p.in0);
                 const int chs = (second ? p.c1 : p.c0) / EPC;
                 const int c0k = second ? ck - p.c0 / EPC : ck;
-                if (X3 && insm && lo) return;              // converted from the main sub-stage's gathers (convert_own)
 #pragma unroll
                 for (int j = 0; j < PER; ++j) {
                     if (sl_dst[j] == 0xFFFFFFFFu) continue;
@@ -345,7 +341,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 // a consumer holds while its MMAs are in flight costs the loader more lead than the drains cost.)
                 auto step = [&](int ks, bool first, auto kind) {
                     const uint32_t g = it + ks;
-                    wait_full(g, insm && decltype(kind)::value == K_F16);
+                    wait_full(g, decltype(kind)::value == K_F16);
                     issue(g, first, kind);
                     wg_wait<1>();                            // every group but g's has completed
                     __syncwarp();
@@ -413,8 +409,8 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         cp_async_commit();                       // (empty groups past the last stage keep the accounting uniform)
                         if (ks >= LAG) {
                             const bool corr = X3 && ((ks - LAG) & 1) == 0;
-                            if (X3 && insm && corr) {
-                                // In-SM correction operand: this thread's gathers of the main sub-stage ks-LAG+1 (issued at
+                            if (X3 && corr) {
+                                // Correction operand: this thread's gathers of the main sub-stage ks-LAG+1 (issued at
                                 // iteration ks-LAG+1 <= ks) have landed; their corr_chunk goes to the same slots of the
                                 // correction stage, whose previous occupant produce(ks-LAG) saw released.  Zero-filled
                                 // slots (padding) convert to zero chunks.
@@ -606,30 +602,18 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                             if (C1 && p.act) st16(p.act, p.slope);
                         }
                     } else {
+                        // (__stwb: one 16-byte store per chunk; the compiler splits a plain float4 store here into four)
                         float* op = p.out + obase + (cb / 4) * cstride;
 #pragma unroll
-                        for (int i = 0; i < 32; i += 4) *reinterpret_cast<float4*>(op + (i / 4) * cstride) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-                        if (GEOM != G_C3 && GEOM != G_C7) {
-                            if (C1 && p.act) {
-                                float* ap = reinterpret_cast<float*>(p.act) + obase + (cb / 4) * cstride;
-                                const float sl = p.slope;
+                        for (int i = 0; i < 32; i += 4) __stwb(reinterpret_cast<float4*>(op + (i / 4) * cstride), make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]));
+                        if (C1 && p.act) {
+                            float* ap = reinterpret_cast<float*>(p.act) + obase + (cb / 4) * cstride;
+                            const float sl = p.slope;
 #pragma unroll
-                                for (int i = 0; i < 32; i += 4) {
-                                    const float4 a = make_float4(v[i] > 0.f ? v[i] : v[i] * sl, v[i + 1] > 0.f ? v[i + 1] : v[i + 1] * sl,
-                                                                 v[i + 2] > 0.f ? v[i + 2] : v[i + 2] * sl, v[i + 3] > 0.f ? v[i + 3] : v[i + 3] * sl);
-                                    *reinterpret_cast<float4*>(ap + (i / 4) * cstride) = a;
-                                    if constexpr (X3) {
-                                        // fp32x3 vocoder: x, lrelu(x) and the correction chunks of lrelu(x)
-                                        if (p.act_corr)
-                                            *reinterpret_cast<float4*>(p.act_corr + obase + (cb / 4) * cstride + (i / 4) * cstride) = corr_chunk(a.x, a.y, a.z, a.w);
-                                    }
-                                }
-                            } else if (p.out_corr) {
-                                float* cp = p.out_corr + obase + (cb / 4) * cstride;
-#pragma unroll
-                                for (int i = 0; i < 32; i += 4)
-                                    *reinterpret_cast<float4*>(cp + (i / 4) * cstride) = corr_chunk(v[i], v[i + 1], v[i + 2], v[i + 3]);
-                            }
+                            for (int i = 0; i < 32; i += 4)
+                                *reinterpret_cast<float4*>(ap + (i / 4) * cstride) =
+                                    make_float4(v[i] > 0.f ? v[i] : v[i] * sl, v[i + 1] > 0.f ? v[i + 1] : v[i + 1] * sl,
+                                                v[i + 2] > 0.f ? v[i + 2] : v[i + 2] * sl, v[i + 3] > 0.f ? v[i + 3] : v[i + 3] * sl);
                         }
                     }
                 }
@@ -683,36 +667,34 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
         if (warp != NCONS / 32) {
             if constexpr (X3 && BULK) {
                 // =================================================================================================
-                // converter warps (fp32x3 without a correction twin): correction stage g = corr_chunk of main stage g + 1
+                // converter warps (fp32x3): correction stage g = corr_chunk of main stage g + 1
                 // =================================================================================================
                 // Stage g + 1's full_b says its A tile has landed AND that the loader, which fills the ring in order, has
                 // seen stage g's previous occupant released, so stage g's A area is free to write.  Stage g + 1 cannot be
                 // overwritten while it is read here: the consumers release it after its MMAs, which they issue after stage
                 // g's, which wait for this warp's arrival on full_a(g).
-                if (insm) {
-                    const int ct = tid - (NCONS + 32);
-                    uint32_t it = 0;
-                    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-                        for (int ks = 0; ks < ksteps_t; ks += 2, it += 2) {
-                            const uint32_t sc = it % STAGES, sm = (it + 1) % STAGES;
-                            mbar_wait(full_b(sm), ((it + 1) / STAGES) & 1);
-                            const float4* src = reinterpret_cast<const float4*>(sA + sm * A_STAGE_BYTES);
-                            float4* dst = reinterpret_cast<float4*>(sA + sc * A_STAGE_BYTES);
-                            // (four loads in flight per thread: the conversion's latency is lead the loader loses)
-                            constexpr int NCHK = A_STAGE_BYTES / 16, UN = 4;
-                            for (int i0 = ct; i0 < NCHK; i0 += UN * NCONV) {
-                                float4 v[UN];
+                const int ct = tid - (NCONS + 32);
+                uint32_t it = 0;
+                for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+                    for (int ks = 0; ks < ksteps_t; ks += 2, it += 2) {
+                        const uint32_t sc = it % STAGES, sm = (it + 1) % STAGES;
+                        mbar_wait(full_b(sm), ((it + 1) / STAGES) & 1);
+                        const float4* src = reinterpret_cast<const float4*>(sA + sm * A_STAGE_BYTES);
+                        float4* dst = reinterpret_cast<float4*>(sA + sc * A_STAGE_BYTES);
+                        // (four loads in flight per thread: the conversion's latency is lead the loader loses)
+                        constexpr int NCHK = A_STAGE_BYTES / 16, UN = 4;
+                        for (int i0 = ct; i0 < NCHK; i0 += UN * NCONV) {
+                            float4 v[UN];
 #pragma unroll
-                                for (int u = 0; u < UN; ++u)
-                                    if (i0 + u * NCONV < NCHK) v[u] = src[i0 + u * NCONV];
+                            for (int u = 0; u < UN; ++u)
+                                if (i0 + u * NCONV < NCHK) v[u] = src[i0 + u * NCONV];
 #pragma unroll
-                                for (int u = 0; u < UN; ++u)
-                                    if (i0 + u * NCONV < NCHK) dst[i0 + u * NCONV] = corr_chunk(v[u].x, v[u].y, v[u].z, v[u].w);
-                            }
-                            fence_proxy_async();             // generic-proxy smem writes -> visible to the tensor core
-                            __syncwarp();
-                            if (lane == 0) mbar_arrive(full_a(sc));
+                            for (int u = 0; u < UN; ++u)
+                                if (i0 + u * NCONV < NCHK) dst[i0 + u * NCONV] = corr_chunk(v[u].x, v[u].y, v[u].z, v[u].w);
                         }
+                        fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor core
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(full_a(sc));
                     }
                 }
             }
@@ -741,7 +723,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 const int s = it % STAGES;
                 const int st = X3 ? ks / 2 : ks, var = X3 ? (ks & 1) : 1;          // 0: correction (fp16 chunks), 1: main (x, w_hi)
                 const int kb = st / conv_tc_stage_rows(GEOM), krow = st - kb * conv_tc_stage_rows(GEOM);     // K step, kernel row (7x7) of weight stage st
-                const bool conv = X3 && BULK && insm && var == 0;     // A tile written by the converter warps: weights only
+                const bool conv = X3 && BULK && var == 0;     // A tile written by the converter warps: weights only
                 if (lane == 0) {
                     mbar_wait(empty(s), ((it / STAGES) & 1) ^ 1);
                     uint32_t a_tx = BULK && !conv ? A_STAGE_BYTES : 0;
@@ -783,7 +765,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                     const int k = lane / HR, r = lane - k * HR;
                     const int ck = kb * KCH + k;                     // 16-byte channel chunk index over the concat
                     const bool second = ck * EPC >= p.c0;
-                    const uint8_t* src = reinterpret_cast<const uint8_t*>(var == 0 ? (second ? p.in1_lo : p.in0_lo) : (second ? p.in1 : p.in0));
+                    const uint8_t* src = reinterpret_cast<const uint8_t*>(second ? p.in1 : p.in0);
                     const int chs = (second ? p.c1 : p.c0) / EPC;
                     const int cl = second ? ck - p.c0 / EPC : ck;
                     if (GEOM == G_PW) {
@@ -894,7 +876,6 @@ int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
     if (p.form < FORM_TF32 || p.form > FORM_BF16 || p.nt <= 0 || p.nt > 128 || p.Cout % p.nt != 0) return -1;
     if (p.geom == G_PW && p.epi == EPI_KV) return launch_attn_kv(p, s);   // fused projection + softmax + context (sbk_attn_x3.cu)
     if (geom_is_c1(p.geom) && (p.dil < 1 || p.pad < 0 || 2 * p.pad > conv_tc_c1_halo(p.geom))) return -1;   // the strip's halo
-    if (p.form == FORM_X3 && p.c1 > 0 && (p.in0_lo == nullptr) != (p.in1_lo == nullptr)) return -1;   // twins for both inputs or for neither
     switch (p.geom) {                                // Conv1d (vocoder): K = 3, 5, 7, 11, each with the 64- and the 128-sample-halo strip
         case G_C1K3:   return launch_c1<G_C1K3>(p, s);
         case G_C1K5:   return launch_c1<G_C1K5>(p, s);

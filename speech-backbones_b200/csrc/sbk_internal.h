@@ -60,7 +60,7 @@ struct IgemmParams {
 enum Form {
     FORM_NHWC = 0,              // fp32 CUDA-core mode: NHWC fp32 [B][H][W][C], exact Mish
     FORM_TF32 = 1,              // fp32 [B][H][C/4][W][4]; the Block activation is rounded to tf32 (cvt.rna), fast Mish
-    FORM_X3 = 2,                // fp32 [B][H][C/4][W][4], exact Mish; a correction twin (corr_chunk) only where out_lo is given
+    FORM_X3 = 2,                // fp32 [B][H][C/4][W][4], exact Mish; the convs derive the correction operand (corr_chunk)
     FORM_BF16 = 3,              // bf16 [B][H][C/8][W][8], fast Mish
 };
 
@@ -93,20 +93,16 @@ struct ConvTcParams {
     // Conv1d geometries: dilation and left padding ((K-1)*dil/2) in samples; output activation LeakyReLU(slope) on `out`
     // (act_out) and/or the second output `act`
     int dil, pad; float slope; int act_out;
-    // fp32-class mode (FORM_X3): every operand x is carried as the pair (x, correction chunks - see corr_chunk below); the
-    // tensor core reads the top 19 bits of x (= x_hi) by itself.  Weights are packed as (w_hi, correction) stage pairs and
-    // each K stage is issued twice into the same fp32 register accumulator: the f16 correction MMAs (x_lo*w + x*w_lo) first,
-    // then the tf32 main MMAs (x_hi*w_hi).
-    const void* in0_lo; const void* in1_lo;         // the correction tensors, same chunk layout as in0 / in1; both null: the
-                                                    // kernel derives the correction chunks from in0 / in1 in shared memory
-    float* out_corr;                                // operand-form outputs (non-3x3 / 7x7 geometries, act_out): their correction chunks
+    // fp32-class mode (FORM_X3): operands are plain fp32; the tensor core reads the top 19 bits of x (= x_hi) by itself and
+    // the kernel derives each A tile's correction chunks (corr_chunk below) in shared memory.  Weights are packed as (w_hi,
+    // correction) stage pairs and each K stage is issued twice into the same fp32 register accumulator: the f16 correction
+    // MMAs (x_lo*w + x*w_lo) first, then the tf32 main MMAs (x_hi*w_hi).
     // The vocoder's output forms (Conv1d geometries, and the transposed convs' 1x1 GEMM when voc = 1).  The output dtype is
     // per output, not per mode: an activated output (act_out) is the next conv's operand and takes the mode's operand form
     // (bf16 mode: bf16 [B][C/8][L][8]); every other output (the residual stream x, the GEMM output Z) stays fp32, with a
     // fp32 addin.
     int voc;
     void* act;                                      // Conv1d: second output lrelu(out) in operand form (fp32, bf16 in bf16 mode)
-    float* act_corr;                                // FORM_X3: the correction chunks of act
 };
 
 // ---- the wgmma conv's weight image: per N tile and K stage exactly the stage's shared-memory image --------------------
@@ -148,7 +144,6 @@ struct GnActParams {
     const float* mask; int T; int lvl;
     float* out; int B, H, W, C;
     int form;                   // FORM_TF32 | FORM_X3 | FORM_BF16
-    float* out_lo;              // FORM_X3: the correction twin of out, or null for none
 };
 
 struct FirstConvParams {        // Block.conv of downs.0.0.block1 on the planar stack([mu, xt(, s)]) * mask
@@ -175,7 +170,6 @@ struct ResFinalParams {         // out = Mish(GN(h2raw))*mask + res(x*mask)
     int B, H, W, C;
     int out_mask;               // planar first block in a tensor-core form: store out*mask (operand form for the next conv)
     int form;                   // layout and number form of x and out (enum Form)
-    float* out_lo;              // FORM_X3: the correction twin of out, or null for none
 };
 
 struct AttnCtxParams {          // merge per-tile softmax partials -> normalised context [B][4][32][32]
@@ -252,7 +246,7 @@ struct InGluParams {             // y = mask ? tf32( IN(raw[c]) * sigmoid(IN(raw
     const float* tb;             // [C/2] time bias (mlp1 / mlp2 row of this step) or nullptr
     const float* mask; int T;    // ref_mask [B][T]
     float* out; int B, H, W, C;  // C = raw channels
-    float* out_lo;               // fp32x3 mode: out unrounded, out_lo = out - trunc_tf32(out)
+    int form;                    // FORM_TF32: fast sigmoid, out rounded to tf32; FORM_X3: exact sigmoid, out unrounded
 };
 struct VcCondParams {            // cond_block( [sinusoid(t) | final_conv(mean-pooled RefBlock) | c] )  (diffusion.py:62-71)
     const double* ysum;          // [B][dc][2] channel sums of the masked RefBlock output (before final_conv)
@@ -319,12 +313,12 @@ __device__ __forceinline__ float tf32_lo(float x) { return x - __uint_as_float(_
 // ---- fp32x3 mode: the correction operand ------------------------------------------------------------------------------
 // x*w = x_hi*w_hi + (x_lo*w + x*w_lo) + O(2^-23): the first product runs as a tf32 MMA on the fp32 tensor itself (the
 // tensor core reads the top 19 bits = x_hi), the bracket is ONE f16 MMA over a packed correction operand.  For every
-// 16-byte chunk of 4 channels the producers write, next to the fp32 chunk, a second 16-byte chunk of eight fp16 values
+// 16-byte chunk of 4 channels of an A tile the conv kernel derives, in shared memory, a 16-byte chunk of eight fp16 values
 //     { x_lo[c0..c3] , x[c0..c3] * 2^-12 }            with x_lo = x - trunc_tf32(x)  (|x_lo| <= 2^-10 |x|)
 // and the weight packers write the matching K order { w[c0..c3] , w_lo[c0..c3] * 2^12 } (w_lo = w - tf32(w)), so one
 // K = 16 fp16 MMA over two chunks adds x_lo*w + x*w_lo for 8 channels.  fp16 carries the same 11 significant bits as tf32;
 // the exact 2^-12 / 2^12 scaling keeps x in fp16's range up to |x| = 2.7e8 and keeps w_lo (~2^-12 |w|) out of its subnormals.
-// The stored chunk has the same address and size as the old fp32 x_lo chunk.  Two MMAs per algorithmic MAC instead of the
+// Two MMAs per algorithmic MAC instead of the
 // three of a 3xTF32 split, at the same modelled accuracy (CPU operand-rounding model: 1.1e-6 vs 1.2e-6 per estimator call).
 constexpr float kCorrDown = 1.f / 4096.f;     // 2^-12 (activation side)
 constexpr float kCorrUp = 4096.f;             // 2^12  (weight side)

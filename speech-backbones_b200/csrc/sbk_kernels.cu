@@ -731,9 +731,6 @@ __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
                     reinterpret_cast<uint2*>(p.out)[oi] = make_uint2(pack_bf16x2_f(o.x, o.y), pack_bf16x2_f(o.z, o.w));
                 } else {
                     reinterpret_cast<float4*>(p.out)[oi] = o;
-                    if constexpr (X3) {
-                        if (p.out_lo) reinterpret_cast<float4*>(p.out_lo)[oi] = corr_chunk(o.x, o.y, o.z, o.w);
-                    }
                 }
             }
         }
@@ -1221,7 +1218,7 @@ __global__ void __launch_bounds__(256) k_in_glu(const InGluParams p) {
                 const int c = ch * 4 + q;
                 const float xa = (av[q] - mean[c]) * scale[c] + beta[c];
                 const float xg = (gv[q] - mean[Ch + c]) * scale[Ch + c] + beta[Ch + c];
-                if (p.out_lo) {
+                if (p.form == FORM_X3) {
                     o[q] = xa * (1.f / (1.f + expf(-xg))) + tbv[c];          // fp32x3 mode: exact sigmoid, no operand rounding
                 } else {
                     float y = xa * __fdividef(1.f, 1.f + __expf(-xg)) + tbv[c];
@@ -1231,8 +1228,6 @@ __global__ void __launch_bounds__(256) k_in_glu(const InGluParams p) {
             }
         }
         *reinterpret_cast<float4*>(p.out + ((long long)b * n4 + i) * 4) = make_float4(o[0], o[1], o[2], o[3]);
-        if (p.out_lo) *reinterpret_cast<float4*>(p.out_lo + ((long long)b * n4 + i) * 4) =
-                          corr_chunk(o[0], o[1], o[2], o[3]);
     }
 }
 int launch_in_glu(const InGluParams& p, cudaStream_t s) {

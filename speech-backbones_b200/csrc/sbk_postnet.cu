@@ -4,7 +4,7 @@
 //
 // Launch plan (all asynchronous on the caller's stream):
 //   1. zero the two blocks' GroupNorm statistics
-//   2. k_pn_init: a0 = init_conv(x*mask)*mask in operand form [B][n_feats][dim/4][T][4] (+ the fp32x3 correction twin) - the
+//   2. k_pn_init: a0 = init_conv(x*mask)*mask in operand form [B][n_feats][dim/4][T][4] - the
 //      input of block1 AND of the residual conv (ResnetBlock.forward multiplies both by the mask, postnet.py:22,36)
 //   3. k_conv_tc<G_C7>: block1 conv -> raw1 + GroupNorm partials (fixed-order, fp64)
 //   4. k_gn_act: act = mask ? Mish(GN(raw1)) : 0 (no time bias: tb is the zero page, postnet.py:22-23)
@@ -29,9 +29,9 @@ using namespace sbk;
 namespace {
 
 // a0 = (w*(x*m) + b)*m per channel, written as [B][H][C/4][T][4] operand chunks; tf32 mode rounds to nearest (as k_gn_act),
-// fp32x3 mode keeps fp32 and writes the correction chunks (sbk_internal.h: corr_chunk)
-__global__ void k_pn_init(const float* x, const float* mask, const float* w, const float* bias, float* out, float* out_lo,
-                          int B, int H, int C, int T, int round_tf32) {
+// fp32x3 mode keeps fp32
+__global__ void k_pn_init(const float* x, const float* mask, const float* w, const float* bias, float* out, int B, int H, int C, int T,
+                          int round_tf32) {
     const int c4n = C / 4;
     const long long n = (long long)B * H * c4n * T;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -49,7 +49,6 @@ __global__ void k_pn_init(const float* x, const float* mask, const float* w, con
             for (int q = 0; q < 4; ++q) { uint32_t u; asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(o[q])); o[q] = __uint_as_float(u); }
         }
         reinterpret_cast<float4*>(out)[i] = make_float4(o[0], o[1], o[2], o[3]);
-        if (out_lo) reinterpret_cast<float4*>(out_lo)[i] = corr_chunk(o[0], o[1], o[2], o[3]);
     }
 }
 
@@ -72,17 +71,15 @@ __global__ void k_pn_final(const float* y, const float* w, const float* bias, fl
     }
 }
 
-// The workspace of one (B, n_feats, T): a0 (+ a0_lo), raw (raw1, then raw2), act (act1, then the res conv's output y)
-// (+ act_lo), and the two blocks' [B][8][2] fp64 GroupNorm statistics.  Over a null-base arena only the size is computed.
-struct PnBufs { float *a0, *raw, *act, *a0_lo, *act_lo; double* st; };
-size_t pn_carve(int B, int H, int C, int T, bool x3, Arena& ar, PnBufs* o) {
+// The workspace of one (B, n_feats, T), the same in every mode: a0, raw (raw1, then raw2), act (act1, then the res conv's
+// output y), and the two blocks' [B][8][2] fp64 GroupNorm statistics.  Over a null-base arena only the size is computed.
+struct PnBufs { float *a0, *raw, *act; double* st; };
+size_t pn_carve(int B, int H, int C, int T, Arena& ar, PnBufs* o) {
     const size_t big = (size_t)B * H * C * T * sizeof(float);
     PnBufs b;
     b.a0 = (float*)ar.take(big);
     b.raw = (float*)ar.take(big);
     b.act = (float*)ar.take(big);
-    b.a0_lo = x3 ? (float*)ar.take(big) : nullptr;
-    b.act_lo = x3 ? (float*)ar.take(big) : nullptr;
     b.st = (double*)ar.take(2 * (size_t)B * kGroups * 2 * sizeof(double));
     if (o) *o = b;
     return ar.bytes();
@@ -168,7 +165,7 @@ extern "C" int sbk_postnet_pack(sbk_postnet* p) {
 extern "C" size_t sbk_postnet_workspace_bytes(const sbk_postnet* p, int B, int n_feats, int T) {
     if (!p || B <= 0 || n_feats <= 0 || T <= 0) return 0;
     Arena probe;
-    return pn_carve(B, n_feats, p->cfg.dim, T, prec_runs_x3(p->cfg.precision), probe, nullptr);
+    return pn_carve(B, n_feats, p->cfg.dim, T, probe, nullptr);
 }
 
 extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* mask, float* out, int B, int n_feats, int T, void* stream) {
@@ -184,8 +181,8 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
     if (p->ws.reserve(need)) return fail(SBK_ERR_CUDA, "out of memory: the PostNet workspace for (B=%d, n_feats=%d, T=%d) needs %zu bytes", B, n_feats, T, need);
     PnBufs wb;
     Arena ar = p->ws.arena();
-    pn_carve(B, H, C, T, x3, ar, &wb);
-    float *a0 = wb.a0, *raw = wb.raw, *act = wb.act, *a0_lo = wb.a0_lo, *act_lo = wb.act_lo;
+    pn_carve(B, H, C, T, ar, &wb);
+    float *a0 = wb.a0, *raw = wb.raw, *act = wb.act;
     double* st = wb.st;
     double* st1 = st; double* st2 = st + (size_t)B * kGroups * 2;
     auto R = [&](const std::string& k) { return p->w.get(k); };
@@ -197,16 +194,16 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
     int k;
 
     CU(cudaMemsetAsync(st, 0, 2 * (size_t)B * kGroups * 2 * sizeof(double), s)); ++n;
-    k_pn_init<<<ew_grid((long long)B * H * (C / 4) * T), 256, 0, s>>>(x, mask, R("init_conv.weight"), R("init_conv.bias"), a0, a0_lo,
-                                                                      B, H, C, T, x3 ? 0 : 1);
+    k_pn_init<<<ew_grid((long long)B * H * (C / 4) * T), 256, 0, s>>>(x, mask, R("init_conv.weight"), R("init_conv.bias"), a0, B, H, C, T,
+                                                                      x3 ? 0 : 1);
     ++n;
-    auto conv7 = [&](const char* blk, const float* in, const float* in_lo, double* ost) {
+    auto conv7 = [&](const char* blk, const float* in, double* ost) {
         ConvTcParams cp; memset(&cp, 0, sizeof(cp));
         const std::string q = std::string("res_block.") + blk + ".block.0.";
         cp.geom = G_C7; cp.in0 = in; cp.c0 = C; cp.H = H; cp.W = T; cp.B = B; cp.Ho = H; cp.Wo = T;
         cp.wpk = R(q + "weight"); cp.bias = R(q + "bias"); cp.out = raw; cp.Cout = C; cp.epi = EPI_PLAIN;
         cp.ostats = ost; cp.mask = mask; cp.T = T; cp.zero_page = p->zero;
-        cp.form = form; cp.nt = conv_tc_ntile(G_C7, C, form); cp.in0_lo = in_lo;     // as pn_pack packed it
+        cp.form = form; cp.nt = conv_tc_ntile(G_C7, C, form);     // as pn_pack packed it
         return launch_conv_tc(cp, s);
     };
     auto gnref = [&](double* stp, const char* blk) {
@@ -214,17 +211,17 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
         GnRef g; g.stats = stp; g.gamma = R(q + "weight"); g.beta = R(q + "bias"); g.inv_count = inv_count;
         return g;
     };
-    if ((k = conv7("block1", a0, a0_lo, st1)) < 0) return refused("block1 conv");
+    if ((k = conv7("block1", a0, st1)) < 0) return refused("block1 conv");
     n += k;
     {
         GnActParams g; memset(&g, 0, sizeof(g));
         g.raw = raw; g.gn = gnref(st1, "block1"); g.tb = p->zero; g.tb_stride = 0; g.tb_per_sample = 1;
         g.mask = mask; g.T = T; g.lvl = 0; g.out = act; g.B = B; g.H = H; g.W = T; g.C = C;
-        g.form = form; g.out_lo = act_lo;
+        g.form = form;
         if ((k = launch_gn_act(g, s)) < 0) return refused("block1 GroupNorm/Mish");
         n += k;
     }
-    if ((k = conv7("block2", act, act_lo, st2)) < 0) return refused("block2 conv");
+    if ((k = conv7("block2", act, st2)) < 0) return refused("block2 conv");
     n += k;
     {
         ConvTcParams cp; memset(&cp, 0, sizeof(cp));
@@ -232,7 +229,7 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
         cp.wpk = R("res_block.res.weight"); cp.bias = R("res_block.res.bias"); cp.out = act; cp.Cout = C;
         cp.epi = EPI_RES; cp.rraw = raw; cp.rgn = gnref(st2, "block2"); cp.out_mask = 1;
         cp.mask = mask; cp.T = T; cp.zero_page = p->zero;
-        cp.form = form; cp.nt = conv_tc_ntile(G_PW, C, form); cp.in0_lo = a0_lo;
+        cp.form = form; cp.nt = conv_tc_ntile(G_PW, C, form);
         if ((k = launch_conv_tc(cp, s)) < 0) return refused("residual conv");
         n += k;
     }

@@ -15,8 +15,9 @@
 // Precision (sbk_vocoder_set_precision), the same launches in every mode:
 //   tf32 (default)  tf32 operands (weights rounded to nearest at pack time, activations truncated by the tensor core), fp32
 //                   accumulation and fp32 everywhere else - the arithmetic PyTorch's own GPU convs use by default;
-//   fp32x3 (and fp32)  x*w = x_hi*w_hi + one f16 correction MMA (sbk_internal.h: corr_chunk), chunked accumulation: every
-//                   conv input (mel_in, SA, A0, A1, A2, Hb) carries a correction twin, written by its producer in the same pass;
+//   fp32x3 (and fp32)  x*w = x_hi*w_hi + one f16 correction MMA (sbk_internal.h: corr_chunk), chunked accumulation: the
+//                   conv inputs are the tf32 mode's fp32 tensors, and the conv kernel derives the correction operand in
+//                   shared memory;
 //   bf16            bf16 weights, and the conv inputs (the LeakyReLU operands mel_in, SA, A0, A1, A2, Hb) stored as bf16
 //                   [B][C/8][L][8]; the residual stream x (X0, X1, X2, R[j]), the GEMM output Z and conv_post's input stay fp32.
 // conv_post, tanh, the folds and the MRF mean are fp32 in every mode.
@@ -45,9 +46,9 @@ constexpr float kSlope = 0.1f;        // LRELU_SLOPE, models.py:10
 
 // An activation operand (a conv input) in the mode's form.  The 4 channels v of element i = bc*L + l of a [B][C/4][L][4]
 // tensor (bc = b*C/4 + channel chunk) go to
-//   bf16 = 0: out[i] fp32 and, when out_lo is set (fp32x3), out_lo[i] = their correction chunk (sbk_internal.h: corr_chunk);
+//   bf16 = 0: out[i] fp32 (tf32 and fp32x3);
 //   bf16 = 1: half of the 16-byte chunk (b, c/8, l) of a bf16 [B][C/8][L][8] tensor (C/4 even), round to nearest even.
-__device__ __forceinline__ void store_operand(float4 v, long long bc, long long l, long long L, void* out, float* out_lo, int bf16) {
+__device__ __forceinline__ void store_operand(float4 v, long long bc, long long l, long long L, void* out, int bf16) {
     if (bf16) {
         uint32_t lo, hi;
         asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(v.y), "f"(v.x));
@@ -55,7 +56,6 @@ __device__ __forceinline__ void store_operand(float4 v, long long bc, long long 
         reinterpret_cast<uint2*>(out)[((bc >> 1) * L + l) * 2 + (bc & 1)] = make_uint2(lo, hi);
     } else {
         reinterpret_cast<float4*>(out)[bc * L + l] = v;
-        if (out_lo) reinterpret_cast<float4*>(out_lo)[bc * L + l] = corr_chunk(v.x, v.y, v.z, v.w);
     }
 }
 
@@ -63,23 +63,22 @@ __device__ __forceinline__ float4 lrelu4(float4 v, float slope) {
     return make_float4(v.x > 0.f ? v.x : v.x * slope, v.y > 0.f ? v.y : v.y * slope, v.z > 0.f ? v.z : v.z * slope, v.w > 0.f ? v.w : v.w * slope);
 }
 
-// mel [B][F][T] (the reference's planar layout) -> the operand [B][F/4][T][4] (+ correction chunks), or bf16 [B][F/8][T][8]
-__global__ void k_voc_mel_in(const float* mel, void* out, float* out_lo, int B, int F, int T, int bf16) {
+// mel [B][F][T] (the reference's planar layout) -> the operand [B][F/4][T][4], or bf16 [B][F/8][T][8]
+__global__ void k_voc_mel_in(const float* mel, void* out, int B, int F, int T, int bf16) {
     const long long n = (long long)B * (F / 4) * T;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         const int t = (int)(i % T);
         const long long bc = i / T;
         const int ch = (int)(bc % (F / 4)); const long long b = bc / (F / 4);
         const float* src = mel + ((b * F + ch * 4) * T) + t;
-        store_operand(make_float4(src[0], src[T], src[2 * (long long)T], src[3 * (long long)T]), bc, t, T, out, out_lo, bf16);
+        store_operand(make_float4(src[0], src[T], src[2 * (long long)T], src[3 * (long long)T]), bc, t, T, out, bf16);
     }
 }
 
 // ConvTranspose1d(k = 2u, stride u, padding u/2) overlap-add (models.py:108): output sample o = u*q + r receives tap
 // t1 = (o + p) mod u of input i1 = (o + p) / u and tap t1 + u of input i1 - 1 (p = u/2).
 //   z: [B][(2u*C)/4][Lin][4], channel index t*C + co;  x (raw): [B][C/4][Lin*u][4];  a = lrelu(x) in operand form (store_operand)
-__global__ void k_voc_ct_fold(const float* z, const float* bias, float* x, void* a, float* a_lo, int B, int C, int Lin, int u, float slope,
-                              int bf16) {
+__global__ void k_voc_ct_fold(const float* z, const float* bias, float* x, void* a, int B, int C, int Lin, int u, float slope, int bf16) {
     const int Lout = Lin * u, c4n = C / 4, p = u / 2;
     const long long n = (long long)B * c4n * Lout;
     const long long zc = (long long)Lin * 4;                       // floats between consecutive channel chunks of z
@@ -99,19 +98,19 @@ __global__ void k_voc_ct_fold(const float* z, const float* bias, float* x, void*
             v.x += w.x; v.y += w.y; v.z += w.z; v.w += w.w;
         }
         reinterpret_cast<float4*>(x)[i] = v;
-        store_operand(lrelu4(v, slope), bc, o, Lout, a, a_lo, bf16);
+        store_operand(lrelu4(v, slope), bc, o, Lout, a, bf16);
     }
 }
 
 // Multi-receptive-field fusion (models.py:109-114): x = ((r0 + r1) + r2) / 3, written as the next consumer's operand lrelu(x)
-// (store_operand over [B][C/4][L][4] chunks, i = bc*L + l; conv_post's input is plain fp32: bf16 = 0, a_lo = null)
-__global__ void k_voc_mrf(const float4* r0, const float4* r1, const float4* r2, void* a, float* a_lo, long long n4, int L, float inv,
-                          float slope, int bf16) {
+// (store_operand over [B][C/4][L][4] chunks, i = bc*L + l; conv_post's input is plain fp32: bf16 = 0)
+__global__ void k_voc_mrf(const float4* r0, const float4* r1, const float4* r2, void* a, long long n4, int L, float inv, float slope,
+                          int bf16) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
         const float4 p = __ldg(r0 + i), q = __ldg(r1 + i), r = __ldg(r2 + i);
         float4 v = make_float4(((p.x + q.x) + r.x) * inv, ((p.y + q.y) + r.y) * inv, ((p.z + q.z) + r.z) * inv, ((p.w + q.w) + r.w) * inv);
         const long long bc = bf16 ? i / L : 0;
-        store_operand(lrelu4(v, slope), bc, bf16 ? i - bc * L : i, L, a, a_lo, bf16);
+        store_operand(lrelu4(v, slope), bc, bf16 ? i - bc * L : i, L, a, bf16);
     }
 }
 
@@ -321,12 +320,11 @@ extern "C" int sbk_vocoder_pack(sbk_vocoder* v) {
 namespace {
 
 // The workspace of one (B, T) in the handle's mode: 11 activation buffers of the largest stage, the transposed-conv GEMM
-// output and the re-laid-out mel.  SA, A0, A1, A2, Hb and the mel are conv inputs: bf16 in the bf16 mode, and with a
-// correction twin each in fp32x3.  Over a null-base arena only the size is computed.
+// output and the re-laid-out mel.  SA, A0, A1, A2, Hb and the mel are conv inputs: bf16 in the bf16 mode, fp32 in the
+// others.  Over a null-base arena only the size is computed.
 struct VocBufs {
-    void* melc; float* melc_lo; float* Z;
+    void* melc; float* Z;
     void *SA, *A0, *A1, *A2, *Hb;
-    float *SA_lo, *A0_lo, *A1_lo, *A2_lo, *Hb_lo;
     float *X0, *X1, *X2, *R[3];
 };
 
@@ -336,7 +334,6 @@ size_t voc_carve(const sbk_vocoder* v, int B, int T, Arena& ar, VocBufs* o) {
     { long long L = T; int ch = c.upsample_initial_channel; big = (size_t)B * ch * L;
       for (int i = 0; i < c.n_ups; ++i) { zmax = std::max<size_t>(zmax, (size_t)B * c.upsample_kernel_sizes[i] * (ch / 2) * L); L *= c.upsample_rates[i]; ch /= 2; big = std::max<size_t>(big, (size_t)B * ch * L); } }
     const size_t ob = v->bf16() ? 2 : 4;            // bytes per element of an operand tensor
-    const bool x3 = v->x3();
     auto take = [&](size_t bytes) { return (char*)ar.take(bytes); };
     VocBufs b{};
     b.melc = take((size_t)B * c.num_mels * T * ob);
@@ -346,11 +343,6 @@ size_t voc_carve(const sbk_vocoder* v, int B, int T, Arena& ar, VocBufs* o) {
     b.SA = take(big * ob); b.X0 = (float*)take(big * 4); b.A0 = take(big * ob); b.X1 = (float*)take(big * 4); b.A1 = take(big * ob);
     b.X2 = (float*)take(big * 4); b.A2 = take(big * ob); b.Hb = take(big * ob);
     for (int j = 0; j < 3; ++j) b.R[j] = (float*)take(big * 4);
-    if (x3) {
-        b.melc_lo = (float*)take((size_t)B * c.num_mels * T * 4);
-        b.SA_lo = (float*)take(big * 4); b.A0_lo = (float*)take(big * 4); b.A1_lo = (float*)take(big * 4);
-        b.A2_lo = (float*)take(big * 4); b.Hb_lo = (float*)take(big * 4);
-    }
     if (o) *o = b;
     return ar.bytes();
 }
@@ -381,19 +373,17 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
     float *Z = wb.Z, *X0 = wb.X0, *X1 = wb.X1, *X2 = wb.X2, **R = wb.R;
     int64_t n = 0;
     int rcl = 0;
-    // act_out: out = lrelu(conv + bias), the next conv's operand (fp32x3: a_corr = its correction chunks); otherwise
-    // out = conv + bias (+ addin) in fp32 and a_out = lrelu(out) in operand form (+ a_corr)
-    auto conv = [&](int geom, const std::string& pre, const void* in, const void* in_lo, int cin, int cout, int L, int dil, void* out,
-                    int act_out, const float* addin, void* a_out, float* a_corr) {
+    // act_out: out = lrelu(conv + bias), the next conv's operand; otherwise out = conv + bias (+ addin) in fp32 and
+    // a_out = lrelu(out) in operand form
+    auto conv = [&](int geom, const std::string& pre, const void* in, int cin, int cout, int L, int dil, void* out, int act_out,
+                    const float* addin, void* a_out) {
         ConvTcParams p; memset(&p, 0, sizeof(p));
         p.geom = geom; p.in0 = in; p.c0 = cin; p.H = 1; p.W = L; p.B = B; p.Ho = 1; p.Wo = L;
         p.wpk = v->w.get(pre + ".wtc"); p.bias = geom == G_PW ? nullptr : v->w.get(pre + ".bias"); p.out = (float*)out; p.Cout = cout; p.epi = EPI_PLAIN;
         p.zero_page = v->zero; p.dil = dil; p.pad = geom == G_PW ? 0 : (conv_tc_taps(geom) - 1) * dil / 2;
-        p.slope = kSlope; p.act_out = act_out; p.addin = addin;
-        if (act_out) p.out_corr = a_corr;
-        else { p.act = a_out; p.act_corr = a_corr; }
+        p.slope = kSlope; p.act_out = act_out; p.addin = addin; p.act = a_out;
         p.form = v->form(); p.nt = conv_tc_ntile(geom, cout, p.form);      // as voc_pack packed it
-        p.in0_lo = in_lo; p.voc = 1;
+        p.voc = 1;
         const int k = launch_conv_tc(p, s);
         if (k < 0) rcl = -1; else n += k;
     };
@@ -403,21 +393,21 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
         if (v->snaps.on) v->snaps.record(pre + suf, src, numel, fmt, s);
     };
     const size_t bn = (size_t)B;
-    k_voc_mel_in<<<ew_grid((long long)B * (c.num_mels / 4) * T), 256, 0, s>>>(mel, melc, wb.melc_lo, B, c.num_mels, T, bf ? 1 : 0); ++n;
+    k_voc_mel_in<<<ew_grid((long long)B * (c.num_mels / 4) * T), 256, 0, s>>>(mel, melc, B, c.num_mels, T, bf ? 1 : 0); ++n;
     snap("mel_in", "", melc, bn * c.num_mels * T, ofmt);
     int ch = c.upsample_initial_channel; int L = T;
     // conv_pre + the first stage's leaky_relu (models.py:105,107)
-    conv(G_C1K7, "conv_pre", melc, wb.melc_lo, c.num_mels, ch, L, 1, SA, 1, nullptr, nullptr, wb.SA_lo);
+    conv(G_C1K7, "conv_pre", melc, c.num_mels, ch, L, 1, SA, 1, nullptr, nullptr);
     snap("conv_pre", "", SA, bn * ch * L, ofmt);
     int rb = 0;
     const float* post_in = nullptr;
     for (int i = 0; i < c.n_ups; ++i) {
         const int u = c.upsample_rates[i], k = c.upsample_kernel_sizes[i], co = ch / 2;
         const std::string up = "ups." + std::to_string(i);
-        conv(G_PW, up, SA, wb.SA_lo, ch, k * co, L, 1, Z, 0, nullptr, nullptr, nullptr);    // Z[i][t*co + c] (models.py:108)
+        conv(G_PW, up, SA, ch, k * co, L, 1, Z, 0, nullptr, nullptr);    // Z[i][t*co + c] (models.py:108)
         snap(up, ".z", Z, bn * k * co * L, 1);
         const int Lo = L * u;
-        k_voc_ct_fold<<<ew_grid((long long)B * (co / 4) * Lo), 256, 0, s>>>(Z, v->w.get(up + ".bias"), X0, A0, wb.A0_lo, B, co, L, u, kSlope, bf ? 1 : 0); ++n;
+        k_voc_ct_fold<<<ew_grid((long long)B * (co / 4) * Lo), 256, 0, s>>>(Z, v->w.get(up + ".bias"), X0, A0, B, co, L, u, kSlope, bf ? 1 : 0); ++n;
         snap(up, ".x", X0, bn * co * Lo, 1); snap(up, ".a", A0, bn * co * Lo, ofmt);
         ch = co; L = Lo;
         const size_t na = bn * ch * L;
@@ -427,9 +417,9 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
             if (c.resblock == 2) {
                 // per dilation d: x = conv_d(lrelu(x)) + x   (models.py:64-69); the second conv's x is the block output
                 const int d0 = c.resblock_dilations[j][0], d1 = c.resblock_dilations[j][1];
-                conv(voc_geom(k, (k - 1) * d0), rp + ".convs.0", A0, wb.A0_lo, ch, ch, L, d0, X1, 0, X0, A1, wb.A1_lo);
+                conv(voc_geom(k, (k - 1) * d0), rp + ".convs.0", A0, ch, ch, L, d0, X1, 0, X0, A1);
                 snap(rp, ".convs.0.x", X1, na, 1); snap(rp, ".convs.0.a", A1, na, ofmt);
-                conv(voc_geom(k, (k - 1) * d1), rp + ".convs.1", A1, wb.A1_lo, ch, ch, L, d1, R[j], 0, X1, nullptr, nullptr);
+                conv(voc_geom(k, (k - 1) * d1), rp + ".convs.1", A1, ch, ch, L, d1, R[j], 0, X1, nullptr);
                 snap(rp, ".convs.1.x", R[j], na, 1);
                 continue;
             }
@@ -437,17 +427,17 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
             // per dilation d: xt = conv2(lrelu(conv1_d(lrelu(x)))); x = xt + x   (models.py:42-47); the dilated convs1 pick
             // their strip from the halo
             auto g1 = [&](int d) { return voc_geom(k, (k - 1) * c.resblock_dilations[j][d]); };
-            conv(g1(0), rp + ".convs1.0", A0, wb.A0_lo, ch, ch, L, c.resblock_dilations[j][0], Hb, 1, nullptr, nullptr, wb.Hb_lo);
+            conv(g1(0), rp + ".convs1.0", A0, ch, ch, L, c.resblock_dilations[j][0], Hb, 1, nullptr, nullptr);
             snap(rp, ".convs1.0", Hb, na, ofmt);
-            conv(geom, rp + ".convs2.0", Hb, wb.Hb_lo, ch, ch, L, 1, X1, 0, X0, A1, wb.A1_lo);
+            conv(geom, rp + ".convs2.0", Hb, ch, ch, L, 1, X1, 0, X0, A1);
             snap(rp, ".convs2.0.x", X1, na, 1); snap(rp, ".convs2.0.a", A1, na, ofmt);
-            conv(g1(1), rp + ".convs1.1", A1, wb.A1_lo, ch, ch, L, c.resblock_dilations[j][1], Hb, 1, nullptr, nullptr, wb.Hb_lo);
+            conv(g1(1), rp + ".convs1.1", A1, ch, ch, L, c.resblock_dilations[j][1], Hb, 1, nullptr, nullptr);
             snap(rp, ".convs1.1", Hb, na, ofmt);
-            conv(geom, rp + ".convs2.1", Hb, wb.Hb_lo, ch, ch, L, 1, X2, 0, X1, A2, wb.A2_lo);
+            conv(geom, rp + ".convs2.1", Hb, ch, ch, L, 1, X2, 0, X1, A2);
             snap(rp, ".convs2.1.x", X2, na, 1); snap(rp, ".convs2.1.a", A2, na, ofmt);
-            conv(g1(2), rp + ".convs1.2", A2, wb.A2_lo, ch, ch, L, c.resblock_dilations[j][2], Hb, 1, nullptr, nullptr, wb.Hb_lo);
+            conv(g1(2), rp + ".convs1.2", A2, ch, ch, L, c.resblock_dilations[j][2], Hb, 1, nullptr, nullptr);
             snap(rp, ".convs1.2", Hb, na, ofmt);
-            conv(geom, rp + ".convs2.2", Hb, wb.Hb_lo, ch, ch, L, 1, R[j], 0, X2, nullptr, nullptr);
+            conv(geom, rp + ".convs2.2", Hb, ch, ch, L, 1, R[j], 0, X2, nullptr);
             snap(rp, ".convs2.2.x", R[j], na, 1);
         }
         // x = xs / num_kernels, then the next consumer's leaky_relu: LRELU_SLOPE before the next ups, torch's default 0.01
@@ -457,7 +447,7 @@ extern "C" int sbk_vocoder_forward(sbk_vocoder* v, const float* mel, float* wav,
         const bool last = i + 1 == c.n_ups;
         void* mo = last ? (void*)X0 : SA;
         k_voc_mrf<<<ew_grid(n4), 256, 0, s>>>(reinterpret_cast<const float4*>(R[0]), reinterpret_cast<const float4*>(R[1]), reinterpret_cast<const float4*>(R[2]),
-                                               mo, last ? nullptr : wb.SA_lo, n4, L, 1.0f / 3.0f, last ? 0.01f : kSlope, (bf && !last) ? 1 : 0); ++n;
+                                               mo, n4, L, 1.0f / 3.0f, last ? 0.01f : kSlope, (bf && !last) ? 1 : 0); ++n;
         if (v->snaps.on) snap("mrf." + std::to_string(i), "", mo, na, last ? 1 : ofmt);
         if (last) post_in = X0;
     }

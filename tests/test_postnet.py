@@ -96,6 +96,19 @@ def test_supported_postnet_dims_are_accepted(sbk_lib, dim):
     assert PostNet(dim).dim == dim
 
 
+def test_postnet_workspace_same_for_fp32x3_and_tf32(sbk_lib):
+    """fp32x3 stores the tf32 mode's tensors: its convs derive the correction operand in shared memory (host-only)."""
+    from speech_backbones_b200.postnet import PostNetEngine
+    ws = {}
+    for precision in ("fp32x3", "tf32", "fp32"):
+        e = PostNetEngine(128, precision=precision)
+        try:
+            ws[precision] = [int(e.lib.sbk_postnet_workspace_bytes(e.h, B, 80, T)) for B, T in ((1, 1), (2, 17), (64, 256))]
+        finally:
+            e.close()
+    assert ws["fp32x3"] == ws["tf32"] == ws["fp32"] and min(ws["tf32"]) > 0, ws
+
+
 def test_cpu_tensors_raise(sbk_lib):
     from speech_backbones_b200.diffvc import FwdDiffusion
     from speech_backbones_b200.postnet import PostNet

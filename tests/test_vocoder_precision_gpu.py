@@ -74,6 +74,27 @@ def test_vocoder_mode_vs_oracle_long_ragged_batch_independent_repeatable(vocoder
     assert torch.equal(y2, y)
 
 
+def test_refused_bf16_switch_keeps_fp32x3():
+    """num_mels = 72 does not tile in bf16 (test_vocoder_precision.py): after the refused switch the handle still runs
+    fp32x3 - its waveform equals a fresh fp32x3 handle's bit for bit and differs from a tf32 handle's."""
+    h72 = dict(HIFIGAN_V1, num_mels=72)
+    sd = synthetic_hifigan_state_dict(72, h72)
+    mel = torch.randn(1, 72, 16, generator=torch.Generator().manual_seed(72)).cuda()
+
+    def run(precision, refuse_bf16=False):
+        eng = VocoderEngine(h72, 0, precision)
+        try:
+            if refuse_bf16:
+                assert eng.lib.sbk_vocoder_set_precision(eng.h, PREC["bf16"]) == 4       # SBK_ERR_UNSUPPORTED
+            eng.load_state_dict(sd)
+            return eng.forward(mel).cpu()
+        finally:
+            eng.close()
+    y = run("fp32x3", refuse_bf16=True)
+    assert torch.equal(y, run("fp32x3"))
+    assert not torch.equal(y, run("tf32"))
+
+
 @pytest.mark.parametrize("mode", MODES)
 def test_vocoder_mode_edge_config_vs_oracle(mode):
     """The strip-limit config (64-sample halos, stride-4 folds) at a ragged and at a one-frame input."""

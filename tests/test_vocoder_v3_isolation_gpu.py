@@ -1,6 +1,7 @@
 """Op isolation for HiFi-GAN V3 (ResBlock2) on the GPU: every captured op of one sbk_vocoder_forward call against its float64
-(or bitwise) replay from the GPU's own captured inputs, as tests/test_vocoder_isolation_gpu.py does for V1, at shapes where
-the Conv1d strips of V3 break:
+(or bitwise) replay from the GPU's own captured inputs, as tests/test_vocoder_isolation_gpu.py does for V1, in tf32 and in
+fp32x3 (whose convs derive the correction operand in shared memory, here on the wide strips too), at shapes where the
+Conv1d strips of V3 break:
 
   * B=1, T=1: stage 0 is 8 samples long, against the 36-sample pad of K = 7 at d = 12 (a wide-strip launch);
   * B=2, T=17: ragged last tiles at every stage;
@@ -13,19 +14,20 @@ Run with -s to see, per op, the worst |err| / (kappa A) (must be <= 1) and the w
 import pytest
 import torch
 
-from op_replay import EPS_ADD, VOC_SLOPE, VocoderReplay, _bitwise, check, conv1d_ntile, kappa, lrelu_f32
+from op_replay import EPS_ADD, VOC_SLOPE, _bitwise, check, conv1d_ntile, kappa, lrelu_f32
 from speech_backbones_b200.spec import HIFIGAN_V3, synthetic_hifigan_state_dict
 from test_hifigan_v3 import HIFIGAN_V3_HALO128
 from test_vocoder_isolation_gpu import _report_and_assert, _sm_count
+from vocoder_replay_modes import VocoderModeReplay, x3_run
 
 pytestmark = pytest.mark.gpu
 CONFIGS = {"v3": HIFIGAN_V3, "halo128": HIFIGAN_V3_HALO128}
 T_MANY = 301
 
 
-class ResBlock2Replay(VocoderReplay):
-    """VocoderReplay for a ResBlock2 generator: resblocks.n.convs.d.x = conv_d(lrelu(x)) + x, its lrelu (.a, d = 0) and the
-    MRF mean over the blocks' convs.1.x; every other op is the V1 replay's."""
+class ResBlock2Replay(VocoderModeReplay):
+    """VocoderModeReplay (tf32, fp32x3) for a ResBlock2 generator: resblocks.n.convs.d.x = conv_d(lrelu(x)) + x, its lrelu
+    (.a, d = 0) and the MRF mean over the blocks' convs.1.x; every other op is the V1 replay's."""
 
     def __init__(self, *a, **k):
         super().__init__(*a, **k)
@@ -46,8 +48,10 @@ class ResBlock2Replay(VocoderReplay):
         addin = self.got(f"ups.{st}.x" if d == 0 else f"{pre}.convs.0.x")
         dil = self.h["resblock_dilation_sizes"][j][d]
         ref, A, Alin, floor = self._conv(x, w, b, dil, addin)
-        k = kappa("tf32", w.shape[1] * w.shape[2], extra=2 * EPS_ADD)       # bias add + residual add
-        return check(self.got(name), ref, A, k, floor, Alin, pad=(w.shape[2] - 1) * dil // 2, ntile=conv1d_ntile(w.shape[0]))
+        k = kappa(self.mode, w.shape[1] * w.shape[2], extra=2 * EPS_ADD, run=x3_run(w.shape[2]))     # bias add + residual add
+        nt = conv1d_ntile(w.shape[0])
+        return check(self.got(name), ref, A, k, floor, Alin, pad=(w.shape[2] - 1) * dil // 2,
+                     ntile=min(nt, 64) if self.mode == "fp32x3" else nt)
 
     def run(self):
         nu = len(self.h["upsample_rates"])
@@ -91,34 +95,37 @@ def vocoders(sbk_lib):
     from speech_backbones_b200.hifigan import VocoderEngine
     cache = {}
 
-    def get(cfg):
-        if cfg not in cache:
+    def get(cfg, mode="tf32"):
+        if (cfg, mode) not in cache:
             sd = synthetic_hifigan_state_dict(1234, CONFIGS[cfg])
-            e = VocoderEngine(CONFIGS[cfg], 0)
+            e = VocoderEngine(CONFIGS[cfg], 0, mode)
             e.load_state_dict(sd)
-            cache[cfg] = (e, sd)
-        return cache[cfg]
+            cache[cfg, mode] = (e, sd)
+        return cache[cfg, mode]
     yield get
     for e, _ in cache.values():
         e.close()
 
 
-CASES = [("v3", 1, 1), ("v3", 2, 17), ("v3", None, T_MANY), ("halo128", 2, 17), ("halo128", 1, 1)]
+SHAPES = [("v3", 1, 1), ("v3", 2, 17), ("v3", None, T_MANY), ("halo128", 2, 17), ("halo128", 1, 1)]
+CASES = [(c, b, t, m) for m in ("tf32", "fp32x3") for c, b, t in SHAPES]
 
 
-@pytest.mark.parametrize("cfg,B,T", CASES, ids=[f"{c}-B{b or 'many'}-T{t}" for c, b, t in CASES])
-def test_v3_vocoder_ops_in_isolation(vocoders, cfg, B, T):
+# (the many-tile batch is counted in tf32's N tiles: fp32x3's are at most 64 wide, so it has at least as many tiles)
+@pytest.mark.parametrize("cfg,B,T,mode", CASES,
+                         ids=[f"{c}-B{b or 'many'}-T{t}" + ("" if m == "tf32" else f"-{m}") for c, b, t, m in CASES])
+def test_v3_vocoder_ops_in_isolation(vocoders, cfg, B, T, mode):
     if B is None:
         B = _many_tiles_batch()
         sms = _sm_count()
         assert _stage0_tiles(B, T) > sms >= _stage0_tiles(B - 1, T), (B, sms)
         print(f"device has {sms} SMs: B = {B} gives {_stage0_tiles(B, T)} stage-0 tiles")
-    eng, sd = vocoders(cfg)
+    eng, sd = vocoders(cfg, mode)
     mel = torch.randn(B, 80, T, generator=torch.Generator().manual_seed(1000 * B + T))
-    rows = ResBlock2Replay(eng, sd, CONFIGS[cfg], mel).run()
+    rows = ResBlock2Replay(eng, sd, CONFIGS[cfg], mel, mode).run()
     names = [r[0] for r in rows]
     assert sum(n.endswith(".x") and ".convs." in n for n in names) == 6 * len(CONFIGS[cfg]["upsample_rates"])
-    _report_and_assert(f"{cfg} B={B} T={T}", rows)
+    _report_and_assert(f"{cfg} {mode} B={B} T={T}", rows)
 
 
 def _expected_names(h):
