@@ -4,13 +4,18 @@
 // operands from shared memory, fp32 accumulation in registers.
 //
 //   D[pixel][cout] (fp32, registers) += A[pixel][tap, cin] (smem) * W[cout][tap, cin] (smem)
+//   3x3: D[cout][pixel] += W[cout][tap, cin] * A[pixel][tap, cin]^T (the same products, operand roles swapped)
 //
 // Mapping.  One CTA owns one row of TPX = 128 pixels x NT output channels of one sample; each of its two consumer
 // warpgroups owns 64 of the pixels (one m64nNT wgmma per tap and K step).  For the 3x3 conv a row is 128 consecutive
-// frames of one mel bin; for 1x1 convs the image is flattened and a row is any 128 consecutive pixels.  A 3x3 tile may
-// also be two rows x 128 pixels x 64 channels (Geo<G_C3, 2>): each consumer warpgroup owns one row, and every weight stage
-// feeds twice the pixels.  The consumers hold up to 128 accumulator registers (fp32x3: accumulators + running sums)
-// because the producer warpgroup hands its registers over (setmaxnreg).
+// frames of one mel bin; for 1x1 convs the image is flattened and a row is any 128 consecutive pixels.  The 3x3 conv puts
+// the output channels on wgmma's M side instead, so that its MMAs can be 128 pixels wide: a 128-channel tile gives each
+// warpgroup 64 channels x the row's 128 pixels (m64n128), a 64-channel tile gives both warpgroups the 64 channels x
+// their 64 pixels (m64n64), and a two-row tile (2 rows x 128 pixels x 64 channels, Geo<G_C3, 2>) gives warpgroup w the
+// 64 channels x row w (m64n128): every weight stage feeds twice the pixels.  An m64n128 reads 96 B of shared memory per
+// tensor-core clock where an m64n64 reads 128 B, the whole port, which leaves the bulk copies no room (DESIGN 4.1).  The
+// consumers hold up to 128 accumulator registers (fp32x3: accumulators + running sums) because the producer warpgroup
+// hands its registers over (setmaxnreg).
 //
 // A operand.  Conv inputs are stored in HBM already in operand form (masked; Block activations GroupNorm-ed, Mish-ed
 // and time-biased by k_gn_act, see sbk_kernels.cu), so producing the A tile is a pure copy straight into the wgmma
@@ -52,12 +57,13 @@ static_assert(128 * PROD_REGS + NCONS * CONS_REGS <= 65536, "register file");
 // geometry of the A tile in shared memory, [16-byte K chunk][row][pixel][16 B]; ROWS output rows of TPX pixels per tile,
 // NACC accumulators per consumer thread
 template <int GEOM, int R = 1> struct Geo;
-// 3x3: halo tile of R + 2 input rows.  R = 1: consumer warpgroup w owns pixels 64w..64w+63 of the row.  R = 2: warpgroup w
-// owns output row h0 + w, i.e. two m64 pixel blocks (two accumulators) that share every weight descriptor - each weight
-// byte brought to shared memory feeds twice the pixels.
+// 3x3: halo tile of R + 2 input rows, MMAs issued transposed (channels on wgmma's M side, see conv_tc_body: TR).  R = 1,
+// NT = 128: consumer warpgroup w owns channels 64w..64w+63 over the row's 128 pixels; R = 1, NT = 64: both warpgroups own
+// the 64 channels, warpgroup w over pixels 64w..64w+63.  R = 2 (NT = 64): warpgroup w owns output row h0 + w, all 128
+// pixels of it - each weight byte brought to shared memory feeds twice the pixels.  One accumulator in every case.
 template <int R> struct Geo<G_C3, R> {
     static_assert(R == 1 || R == 2, "3x3 tiles are 1 or 2 rows");
-    static constexpr int ROWS = R, HR = R + 2, PXP = TPX + 2, TAPS = 9, KCH = 2, NACC = R;
+    static constexpr int ROWS = R, HR = R + 2, PXP = TPX + 2, TAPS = 9, KCH = 2, NACC = 1;
 };
 template <> struct Geo<G_PW> { static constexpr int ROWS = 1, HR = 1, PXP = TPX, TAPS = 1, KCH = 8, NACC = 1; };           // 1x1: plain tile
 // 3x3 stride 2 (Downsample): 3 input rows; input columns de-interleaved into an odd plane (129 px: 2*w0-1+2i) and
@@ -141,7 +147,15 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     using G = Geo<GEOM, R>;
     using D = Depth<GEOM, NT, R>;
     constexpr int NACC = G::NACC, ROWS = G::ROWS;
-    constexpr bool ROW2 = ROWS == 2;                       // 3x3, 2-row tile: accumulator a = pixel block a of the row
+    constexpr bool ROW2 = ROWS == 2;                       // 3x3, 2-row tile: warpgroup w = output row h0 + w
+    // 3x3: the MMAs run transposed, D[cout][pixel] = W[cout][tap, cin] * A[pixel][tap, cin]^T: the weight stage is wgmma's
+    // A operand (64 channels, M) and the halo tile its B operand (NW pixels, N).  Both images are K-major with SBO = 128,
+    // so only the operand roles change; an element still sees the same products in the same K order.  With N = 128 an
+    // MMA reads 96 B of shared memory per tensor-core clock instead of the 128 B of an m64n64 (2-row tile).
+    constexpr bool TR = GEOM == G_C3;
+    static_assert(!TR || NT == 128 || (NT == 64 && ROWS * NT <= 128), "3x3 tiles: 128 channels x 1 row or 64 x 1-2 rows");
+    constexpr int NW = TR ? ROWS * NT : NT;                // wgmma N: this warpgroup's pixels (3x3) or the tile's channels
+    constexpr int NPASS = TR ? ROWS : NACC;                // epilogue passes through the [TPX][LDS] staging tile
     constexpr bool CHUNKED = X3 && GEOM != G_UP;
     // sub-stages per accumulation run: 6 = three K stages of correction + main sub-stage, 54 MMAs per accumulator for a
     // 3x3 conv (7x7: three (K step, kernel row) stages, 42 MMAs)
@@ -162,7 +176,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     constexpr int B_STAGE_BYTES = TAPS * KCH * NT * 16;
     constexpr bool BULK = GEOM != G_DOWN;                  // A tile = contiguous runs -> cp.async.bulk (no LSU work)
     constexpr int SPAN = TPX;                              // output pixels per tile along W
-    constexpr int FR = NT / 2;                             // accumulator registers per thread and accumulator
+    constexpr int FR = NW / 2;                             // accumulator registers per thread and accumulator
     constexpr int KMAIN = BF16 ? K_BF16 : K_TF32;
 
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -244,7 +258,8 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
         // consumer warpgroups: (G_DOWN: cp.async A producers,) MMAs, epilogue of every tile
         // =========================================================================================================
         setmaxnreg_inc<CONS_REGS>();
-        const int wg = warp >> 2, wt = tid & 127;                  // warpgroup = pixel half of the tile (2-row tile: its row)
+        // warpgroup = pixel half of the tile (2-row tile: its row; 128-channel 3x3 tile: channel half)
+        const int wg = warp >> 2, wt = tid & 127;
         uint32_t it = 0;                                           // ring counter (stages consumed by this CTA)
         // ---- A producers (Downsample only): 16-byte cp.async gathers that de-interleave even/odd columns
         constexpr int SLOTS = HR * PXP * KCH;
@@ -316,15 +331,17 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
             auto issue = [&](uint32_t g, bool first, auto kind) {
                 constexpr int KD = decltype(kind)::value;
                 const int s = g % STAGES;
-                // this warpgroup's 64 pixels (2-row tile: its halo row; block a of the row adds 64 a)
-                const uint32_t a_lo = desc_lo(a0 + s * A_STAGE_BYTES, PLANE) + (uint32_t)(ROW2 ? wg * PXP : 64 * wg);
-                const uint32_t b_lo = desc_lo(b0 + s * B_STAGE_BYTES, NT * 16);
-                const uint32_t dil = C1 ? (uint32_t)p.dil : 0u;
+                // this warpgroup's pixels of the A tile (2-row tile: its halo row; 128-channel 3x3 tile: all 128, else 64 w..)
+                // and its channels of the weight stage (128-channel 3x3 tile: 64 w..64 w + 63, else all NT)
+                const uint32_t a_lo = desc_lo(a0 + s * A_STAGE_BYTES, PLANE) +
+                                      (uint32_t)(ROW2 ? wg * PXP : (TR && NT == 128 ? 0 : 64 * wg));
+                const uint32_t b_lo = desc_lo(b0 + s * B_STAGE_BYTES, NT * 16) + (uint32_t)(TR && NT == 128 ? 64 * wg : 0);
+                [[maybe_unused]] const uint32_t dil = C1 ? (uint32_t)p.dil : 0u;
                 wg_fence();
 #pragma unroll
                 for (int kk = 0; kk < KCH / 2; ++kk) {
                     const uint32_t a_k = a_lo + (uint32_t)(kk * 2 * (PLANE / 16)), b_k = b_lo + (uint32_t)(kk * 2 * NT);
-                    if (GEOM == G_UP) {
+                    if constexpr (GEOM == G_UP) {
                         // ho = 2*hi - 1 + kh: parity ph uses (kh=1,dh=0),(kh=3,dh=-1) if ph=0 and (kh=0,dh=+1),(kh=2,dh=0) if ph=1
 #pragma unroll
                         for (int phase = 0; phase < 4; ++phase) {
@@ -347,10 +364,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                             const uint32_t aoff = GEOM == G_DOWN ? (uint32_t)(r * PXP + (sx == 1 ? TPX + 1 : (sx == 2 ? 1 : 0)))
                                                 : C1 ? (uint32_t)tap * dil
                                                      : (uint32_t)(r * PXP + sx);
-#pragma unroll
-                            for (int a = 0; a < NACC; ++a)
-                                wgmma<NT, KD>(acc[a], desc_pack(a_k + aoff + (uint32_t)(64 * a), D_HI),
-                                              desc_pack(b_k + (uint32_t)(tap * KCH * NT), D_HI), (!first || (kk | tap) != 0) ? 1u : 0u);
+                            const uint64_t x_d = desc_pack(a_k + aoff, D_HI), w_d = desc_pack(b_k + (uint32_t)(tap * KCH * NT), D_HI);
+                            const uint32_t keep = (!first || (kk | tap) != 0) ? 1u : 0u;
+                            if constexpr (TR) wgmma<NW, KD>(acc[0], w_d, x_d, keep);       // D[cout][pixel]
+                            else wgmma<NT, KD>(acc[0], x_d, w_d, keep);                    // D[pixel][cout]
                         }
                     }
                 }
@@ -507,7 +524,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
             const int cpg = p.Cout / kGroups;
             const float* bp = p.bias ? p.bias + (long long)b * p.bias_bstride + n0 : nullptr;
 #pragma unroll
-            for (int phase = 0; phase < NACC; ++phase) {
+            for (int phase = 0; phase < NPASS; ++phase) {
             if constexpr (ROW2) {
                 // pass `phase` stages pixel block `phase` of both rows: staging pixel px is row px / 64, column 64 phase + px % 64
                 ho = h0 + (px >> 6); wo = w0 + 64 * phase + (px & 63);
@@ -520,12 +537,26 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
             asm volatile("bar.sync 2, 256;" ::: "memory");            // previous readers of the staging tile are done
             {
                 auto stage_out = [&](const float (&res)[FR]) {
+                    if constexpr (TR) {
+                        // fragment rows = channels, columns = pixels; pass `phase` of a 2-row tile takes fragment columns
+                        // 64 phase..64 phase + 63 (registers FR/2 phase..), this warpgroup's row's share of pixel block
+                        // `phase`.  A warp's scalar stores hit pixels p + 2 (lane % 4) and channels c + lane / 4: banks
+                        // 8 (lane % 4) + lane / 4 (mod 32, LDS = 4 mod 32), all distinct.
+                        constexpr int NI = FR / NPASS;
+                        const int pb = (NT == 128 ? 0 : 64 * wg) - 64 * phase, cb = NT == 128 ? 64 * wg : 0;
 #pragma unroll
-                    for (int i = 0; i < FR; i += 2)
-                        *reinterpret_cast<float2*>(&sD[(64 * wg + frag_row(wt, i)) * LDS + frag_col(wt, i)]) = make_float2(res[i], res[i + 1]);
+                        for (int j = 0; j < NI; ++j) {
+                            const int i = phase * NI + j;
+                            sD[(pb + frag_col(wt, i)) * LDS + cb + frag_row(wt, i)] = res[i];
+                        }
+                    } else {
+#pragma unroll
+                        for (int i = 0; i < FR; i += 2)
+                            *reinterpret_cast<float2*>(&sD[(64 * wg + frag_row(wt, i)) * LDS + frag_col(wt, i)]) = make_float2(res[i], res[i + 1]);
+                    }
                 };
-                if constexpr (CHUNKED) stage_out(sum[phase]);
-                else stage_out(acc[phase]);
+                if constexpr (CHUNKED) stage_out(sum[TR ? 0 : phase]);
+                else stage_out(acc[TR ? 0 : phase]);
             }
             asm volatile("bar.sync 2, 256;" ::: "memory");
             const int ho_p = GEOM == G_UP ? ho + (phase >> 1) : ho;

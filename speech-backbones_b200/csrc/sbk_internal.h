@@ -89,7 +89,8 @@ struct ConvTcParams {
                                                     // longest run is a wide Conv1d strip row, 256 samples x 16 B)
     int nt;                                         // N tile: the width the weights were packed with (conv_tc_ntile, or 64 for
                                                     // the U-Net's second 3x3 image, used when 128-wide tiles cannot fill the GPU)
-    int rows;                                       // G_C3: output rows per tile, 1 (0 = 1) or 2; 2 runs 64-wide N tiles (nt = 64)
+    int rows;                                       // G_C3: output rows per tile, 1 (0 = 1) or 2; 2 runs 64-wide N tiles (nt = 64),
+                                                    // each consumer warpgroup one row: 64 channels x 128 pixels per MMA
     // Conv1d geometries: dilation and left padding ((K-1)*dil/2) in samples; output activation LeakyReLU(slope) on `out`
     // (act_out) and/or the second output `act`
     int dil, pad; float slope; int act_out;
