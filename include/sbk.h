@@ -85,6 +85,17 @@ size_t sbk_workspace_bytes_n(const sbk_handle* h, int B, int T, int n_timesteps)
  * x, mu, out: [B,n_feats,T]; mask: [B,1,T] in {0,1}; t: [B]; spk: NULL or [B,spk_emb_dim]. Device pointers. */
 int sbk_estimator(sbk_handle* h, const float* x, const float* mask, const float* mu, const float* t,
                   const float* spk, float* out, int B, int T, void* stream);
+/* Ragged batches.  lengths: NULL (the dense call above: sbk_estimator, sbk_reverse_diffusion and sbk_reverse_steps are these
+ * entry points with lengths = NULL) or device int64 [B], each utterance's valid frames, such as Grad-TTS's y_lengths.
+ * Utterance b is computed on its own grid of T_b = fix_len_compatibility(lengths[b]) frames (a multiple of 4, <= T):
+ * out[b, :, :T_b] is the call on x[b:b+1, :, :T_b], mask[b:b+1, :, :T_b], mu[b:b+1, :, :T_b] (and noise[:, b, :, :T_b],
+ * spk[b:b+1]) - its GroupNorm statistics, attention softmax and conv borders see its own T_b frames only - and
+ * out[b, :, T_b:] is 0.  Nothing at or past T_b is read.  The kernels clamp each length to [1, T]; validating them is the
+ * caller's job.  The plan keeps its own device copy of lengths, refreshed on the stream by every call, so the captured
+ * graphs never hold the caller's pointer; a ragged loop is still one host launch.  tf32 and bf16 rows are bit for bit their
+ * own B = 1 calls; fp32x3 and fp32 rows agree with them to fp32 rounding. */
+int sbk_estimator_lengths(sbk_handle* h, const float* x, const float* mask, const float* mu, const float* t,
+                          const float* spk, const int64_t* lengths, float* out, int B, int T, void* stream);
 
 /* Diffusion.reverse_diffusion(z, mask, mu, n_timesteps, stoc, spk) (diffusion.py:254-275).
  * noise: NULL when stoc==0, else [N,B,n_feats,T] pre-drawn N(0,1) (the reference draws it with
@@ -92,6 +103,10 @@ int sbk_estimator(sbk_handle* h, const float* x, const float* mask, const float*
  * out may alias z.  Device pointers. */
 int sbk_reverse_diffusion(sbk_handle* h, const float* z, const float* mask, const float* mu, const float* spk,
                           const float* noise, float* out, int B, int T, int n_timesteps, int stoc, void* stream);
+/* the same over a ragged batch (lengths: see sbk_estimator_lengths) */
+int sbk_reverse_diffusion_lengths(sbk_handle* h, const float* z, const float* mask, const float* mu, const float* spk,
+                                  const float* noise, const int64_t* lengths, float* out, int B, int T, int n_timesteps,
+                                  int stoc, void* stream);
 
 /* ---- DiffVC (SBK_MODEL_DIFFVC) ------------------------------------------------------------------------------
  * GradLogPEstimator.forward (DiffVC/model/diffusion.py:61-106) with the xt-independent conditioning vector
@@ -136,6 +151,10 @@ int sbk_vc_cond_debug_read(sbk_handle* h, const char* name, void* dst, int64_t* 
 int sbk_reverse_steps(sbk_handle* h, float* xt, const float* mask, const float* mu, const float* spk,
                       const float* noise, int B, int T, int n_timesteps, int step_begin, int step_end,
                       int stoc, void* stream);
+/* the same over a ragged batch (lengths: see sbk_estimator_lengths); xt at or past T_b is neither read nor kept (0 after) */
+int sbk_reverse_steps_lengths(sbk_handle* h, float* xt, const float* mask, const float* mu, const float* spk,
+                              const float* noise, const int64_t* lengths, int B, int T, int n_timesteps, int step_begin,
+                              int step_end, int stoc, void* stream);
 
 /* Diffusion.forward with HOST buffers (the call `GradTTS.forward` makes at tts.py:96 when the caller's
  * tensors live on the CPU): copies z/mask/mu(/spk/noise) to the device, runs the loop, copies the result

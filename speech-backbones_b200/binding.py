@@ -20,6 +20,7 @@ EXPORTS = [
     "sbk_debug_name", "sbk_last_error", "sbk_version", "sbk_profile_ops", "sbk_debug_capture", "sbk_debug_layout", "sbk_debug_op_layout", "sbk_vc_estimator", "sbk_vc_reverse_diffusion", "sbk_vc_conditioning",
     "sbk_prior_expand", "sbk_last_host_launches", "sbk_workspace_bytes_n",
     "sbk_vc_cond_debug_num", "sbk_vc_cond_debug_name", "sbk_vc_cond_debug_op_layout", "sbk_vc_cond_debug_read",
+    "sbk_estimator_lengths", "sbk_reverse_diffusion_lengths", "sbk_reverse_steps_lengths",
 ]
 
 
@@ -52,6 +53,9 @@ def load_library() -> C.CDLL:
     lib.sbk_vc_reverse_diffusion.argtypes = [P, F, F, F, F, F, F, I, I, I, I, P]
     lib.sbk_vc_conditioning.argtypes = [P, F, F, F, F, F, I, I, I, P]
     lib.sbk_reverse_steps.argtypes = [P, F, F, F, F, F, I, I, I, I, I, I, P]
+    lib.sbk_estimator_lengths.argtypes = [P, F, F, F, F, F, P, F, I, I, P]
+    lib.sbk_reverse_diffusion_lengths.argtypes = [P, F, F, F, F, F, P, F, I, I, I, I, P]
+    lib.sbk_reverse_steps_lengths.argtypes = [P, F, F, F, F, F, P, I, I, I, I, I, I, P]
     lib.sbk_reverse_diffusion_host.argtypes = [P, F, F, F, F, F, F, I, I, I, I]
     lib.sbk_prior_expand.argtypes = [F, F, F, F, F, C.c_float, I, I, I, I, F, F, F, F, P]
     lib.sbk_last_host_launches.argtypes = [P]
@@ -87,6 +91,23 @@ def _check_precision(precision):
     if precision not in PREC:
         raise ValueError(f"precision must be one of {sorted(PREC)}, got {precision!r}")
     return precision
+
+
+def check_lengths(lengths, B, T, device, what="mel"):
+    """lengths of a ragged batch: int64 [B] on the device of the input `what`, each in 1..T (one device-to-host read of its
+    min and max).  Raises ValueError with the reason; returns the lengths contiguous."""
+    if not isinstance(lengths, torch.Tensor):
+        raise ValueError(f"lengths: expected an int64 tensor of shape [{B}], got {type(lengths).__name__}")
+    if lengths.dtype != torch.int64:
+        raise ValueError(f"lengths: expected int64, got {lengths.dtype}")
+    if tuple(lengths.shape) != (B,):
+        raise ValueError(f"lengths shape {tuple(lengths.shape)}: expected [{B}] (one length per utterance)")
+    if lengths.device != device:
+        raise ValueError(f"lengths lives on {lengths.device}; it must be on the {what}'s device {device}")
+    lo, hi = torch.stack(lengths.aminmax()).tolist()
+    if lo < 1 or hi > T:
+        raise ValueError(f"lengths must lie in 1..{T} (the {what}'s frames), got min {lo}, max {hi}")
+    return lengths.contiguous()
 
 
 def _f32c(t: torch.Tensor, name: str) -> torch.Tensor:
@@ -240,13 +261,18 @@ class Engine(_NativeHandle):
             raise RuntimeError(f"spk shape {tuple(spk.shape)} != {(B, self.spk_emb_dim)}")
         return B, T
 
-    def estimator(self, x, mask, mu, t, spk=None):
+    # Ragged batches: `lengths` (int64 [B] on the input's device, each in 1..T, e.g. Grad-TTS's y_lengths) computes utterance
+    # b on its own T_b = fix_len_compatibility(lengths[b]) frames, as the call on its [:T_b] slices would (sbk.h:
+    # sbk_estimator_lengths); its frames from T_b on come out 0.  None: the padded batch, as before.
+    def estimator(self, x, mask, mu, t, spk=None, lengths=None):
         B, T = self._check_inputs(x, mask, mu, spk, t)
+        if lengths is not None:
+            lengths = check_lengths(lengths, B, T, x.device, "x")
         x, mask, mu, t = _f32c(x, "x"), _f32c(mask, "mask"), _f32c(mu, "mu"), _f32c(t, "t")
         spk = _f32c(spk, "spk") if (spk is not None and self.n_spks > 1) else None
         out = torch.empty_like(x)
-        self._call(self.lib.sbk_estimator, "sbk_estimator", self.h, _ptr(x), _ptr(mask), _ptr(mu), _ptr(t), _ptr(spk), _ptr(out),
-                   B, T, self._stream())
+        self._call(self.lib.sbk_estimator_lengths, "sbk_estimator", self.h, _ptr(x), _ptr(mask), _ptr(mu), _ptr(t), _ptr(spk),
+                   _ptr(lengths), _ptr(out), B, T, self._stream())
         return out
 
     # ---- oversize batches: utterances are independent, so a batch whose workspace would not fit is run in slices
@@ -263,13 +289,16 @@ class Engine(_NativeHandle):
         chunk = max(1, int(limit // per))
         return [(lo, min(B, lo + chunk)) for lo in range(0, B, chunk)]
 
-    def reverse_diffusion(self, z, mask, mu, n_timesteps, stoc=False, spk=None, noise=None):
+    def reverse_diffusion(self, z, mask, mu, n_timesteps, stoc=False, spk=None, noise=None, lengths=None):
         B, T = self._check_inputs(z, mask, mu, spk)
+        if lengths is not None:
+            lengths = check_lengths(lengths, B, T, z.device, "z")
         sl = self.batch_slices(B, T, n_timesteps)
         if len(sl) > 1:
             outs = [self.reverse_diffusion(z[a:b], mask[a:b], mu[a:b], n_timesteps, stoc,
                                            None if spk is None else spk[a:b],
-                                           None if noise is None else noise[:, a:b].contiguous()) for a, b in sl]
+                                           None if noise is None else noise[:, a:b].contiguous(),
+                                           None if lengths is None else lengths[a:b]) for a, b in sl]
             return torch.cat(outs, 0)
         z, mask, mu = _f32c(z, "z"), _f32c(mask, "mask"), _f32c(mu, "mu")
         spk = _f32c(spk, "spk") if (spk is not None and self.n_spks > 1) else None
@@ -280,19 +309,22 @@ class Engine(_NativeHandle):
             if tuple(noise.shape) != (n_timesteps, B, self.n_feats, T):
                 raise RuntimeError(f"noise shape {tuple(noise.shape)} != {(n_timesteps, B, self.n_feats, T)}")
         out = torch.empty_like(z)
-        self._call(self.lib.sbk_reverse_diffusion, "sbk_reverse_diffusion", self.h, _ptr(z), _ptr(mask), _ptr(mu), _ptr(spk),
-                   _ptr(noise) if stoc else None, _ptr(out), B, T, int(n_timesteps), 1 if stoc else 0, self._stream())
+        self._call(self.lib.sbk_reverse_diffusion_lengths, "sbk_reverse_diffusion", self.h, _ptr(z), _ptr(mask), _ptr(mu),
+                   _ptr(spk), _ptr(noise) if stoc else None, _ptr(lengths), _ptr(out), B, T, int(n_timesteps), 1 if stoc else 0,
+                   self._stream())
         return out
 
-    def reverse_steps(self, xt, mask, mu, n_timesteps, step_begin, step_end, stoc=False, spk=None, noise=None):
+    def reverse_steps(self, xt, mask, mu, n_timesteps, step_begin, step_end, stoc=False, spk=None, noise=None, lengths=None):
         B, T = self._check_inputs(xt, mask, mu, spk)
+        if lengths is not None:
+            lengths = check_lengths(lengths, B, T, xt.device, "xt")
         assert xt.is_contiguous() and xt.dtype == torch.float32
         mask, mu = _f32c(mask, "mask"), _f32c(mu, "mu")
         spk = _f32c(spk, "spk") if (spk is not None and self.n_spks > 1) else None
         noise = _f32c(noise, "noise") if stoc else None
-        _check(self.lib.sbk_reverse_steps(self.h, _ptr(xt), _ptr(mask), _ptr(mu), _ptr(spk), _ptr(noise), B, T,
-                                          int(n_timesteps), int(step_begin), int(step_end), 1 if stoc else 0,
-                                          self._stream()), "sbk_reverse_steps")
+        _check(self.lib.sbk_reverse_steps_lengths(self.h, _ptr(xt), _ptr(mask), _ptr(mu), _ptr(spk), _ptr(noise), _ptr(lengths),
+                                                  B, T, int(n_timesteps), int(step_begin), int(step_end), 1 if stoc else 0,
+                                                  self._stream()), "sbk_reverse_steps")
         return xt
 
     # ---- DiffVC (model="diffvc")

@@ -60,11 +60,15 @@ struct Plan {
     float *vc_cond = nullptr, *vc_wextra = nullptr, *vc_rextra = nullptr;   // DiffVC conditioning tables [rows][B][...]
     int first_op = -1, first_res_op = -1;
     int tb_stride = 0;
-    cudaGraphExec_t gexec[4] = {nullptr, nullptr, nullptr, nullptr};   // one reverse step, per FinalParams.mode
+    // a ragged call's lengths (sbk_*_lengths): the plan's own device copy [B], refreshed on the stream by every such call, so
+    // the ragged graphs read it and never a caller's pointer
+    int64_t* lengths = nullptr;
+    // graphs per FinalParams.mode and per batch kind: index mode + 4 * ragged
+    cudaGraphExec_t gexec[8] = {};                          // one reverse step
     // the WHOLE loop as one graph: a conditional WHILE node whose body is one reverse step + k_loop_cond, so a sampler
     // call is ONE host launch for any N (N = 1000 needs no 75k-node graph).  loop_state: 0 untried, 1 built, -1 unavailable
-    cudaGraphExec_t gloop[4] = {nullptr, nullptr, nullptr, nullptr};
-    int loop_state[4] = {0, 0, 0, 0};
+    cudaGraphExec_t gloop[8] = {};
+    int loop_state[8] = {};
     int* step_end = nullptr;
     int launches_per_step = 0;
 };
@@ -222,8 +226,8 @@ extern "C" int sbk_create(const sbk_config* cfg, sbk_handle** out) {
 // inside it without a cudaFree/cudaMalloc pair)
 static void free_plan(sbk_handle* h) {
     Plan& p = h->plan;
-    for (int i = 0; i < 4; ++i) if (p.gexec[i]) { cudaGraphExecDestroy(p.gexec[i]); p.gexec[i] = nullptr; }
-    for (int i = 0; i < 4; ++i) if (p.gloop[i]) { cudaGraphExecDestroy(p.gloop[i]); p.gloop[i] = nullptr; }
+    for (int i = 0; i < 8; ++i) if (p.gexec[i]) { cudaGraphExecDestroy(p.gexec[i]); p.gexec[i] = nullptr; }
+    for (int i = 0; i < 8; ++i) if (p.gloop[i]) { cudaGraphExecDestroy(p.gloop[i]); p.gloop[i] = nullptr; }
     for (auto& op : p.ops) if (op.dbg_copy) cudaFree(op.dbg_copy);
     p = Plan();
 }
@@ -444,6 +448,7 @@ static size_t layout(const sbk_handle* h, int B, int T, int tb_rows, Arena& ar, 
     p.step_next = (int*)ar.take(sizeof(int));
     p.step_end = (int*)ar.take(sizeof(int));
     p.noise_pp = (const float**)ar.take(sizeof(float*));
+    p.lengths = (int64_t*)ar.take((size_t)B * sizeof(int64_t));
     if (c.model == SBK_MODEL_DIFFVC) {
         p.vc_cond = f((size_t)tb_rows * B * c.dim_cond);
         p.vc_wextra = f((size_t)tb_rows * B * 9 * dim);
@@ -485,6 +490,8 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
     auto gnref = [&](const double* st, const std::string& blk, int C, int lvl) {
         GnRef g; g.stats = st; g.gamma = h->w.get(blk + ".block.1.weight"); g.beta = h->w.get(blk + ".block.1.bias");
         g.inv_count = 1.0f / ((float)(C / kGroups) * (float)Hs[lvl] * (float)Ws[lvl]);
+        // a ragged call's per-sample divisor (gn_inv_count): the same product with W_b in place of W
+        g.lengths = nullptr; g.cnt_ch = (float)(C / kGroups) * (float)Hs[lvl]; g.T = T; g.lvl = lvl;
         return g;
     };
     auto base_ig = [&](int geom, int lvl_in, int lvl_out) {
@@ -680,7 +687,9 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
         }
         {
             Op op; op.kind = OP_CTX; op.name = a.prefix + ".ctx";
+            op.cx = AttnCtxParams();
             op.cx.kv_part = bf.kv_part; op.cx.mtiles = mt; op.cx.ctx = bf.ctx; op.cx.B = B;
+            op.cx.T = T; op.cx.lvl = lvl; op.cx.H = Hs[lvl]; op.cx.tile_px = use_tc ? attn_kv_tile_pixels() : 128;   // (k_igemm: 128-pixel tiles)
             push(op, bf.ctx, (int64_t)B * kHeads * 1024);
         }
         {
@@ -846,6 +855,23 @@ static int speaker(sbk_handle* h, const float* spk, int B, cudaStream_t s) {
     return launch_spk(p, s);
 }
 
+// ragged: every launch reads the plan's lengths (a ragged call), or none (a dense call runs exactly its own kernels)
+static void set_ragged(Plan& pl, bool ragged) {
+    const int64_t* L = ragged ? pl.lengths : nullptr;
+    for (auto& op : pl.ops) {
+        switch (op.kind) {
+            case OP_FIRST: op.fc.lengths = L; break;
+            case OP_IGEMM: op.ig.lengths = L; op.ig.pgn.lengths = L; op.ig.rgn.lengths = L; break;
+            case OP_CONVTC: op.tc.lengths = L; op.tc.rgn.lengths = L; break;
+            case OP_GNACT: op.ga.gn.lengths = L; break;
+            case OP_RESFINAL: op.rf.gn.lengths = L; break;
+            case OP_CTX: op.cx.lengths = L; break;
+            case OP_FINAL: op.fn.lengths = L; op.fn.gn.lengths = L; break;
+            case OP_MIX: break;
+        }
+    }
+}
+
 static void set_mode(Plan& pl, int mode, bool per_sample_t, float* out) {
     for (auto& op : pl.ops)
         if (op.kind == OP_IGEMM && op.ig.pro == PRO_GN) op.ig.tb_per_sample = per_sample_t ? 1 : 0;
@@ -857,8 +883,21 @@ static void set_mode(Plan& pl, int mode, bool per_sample_t, float* out) {
     f.mode = mode; f.xt_out = out; f.noise_pp = pl.noise_pp;
 }
 
+// a ragged call: copy the caller's lengths into the plan (on the stream, before any launch reads them)
+static int load_lengths(sbk_handle* h, const int64_t* lengths, int B, cudaStream_t s) {
+    Plan& pl = h->plan;
+    set_ragged(pl, lengths != nullptr);
+    if (lengths) CU(cudaMemcpyAsync(pl.lengths, lengths, (size_t)B * sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
+    return SBK_OK;
+}
+
 extern "C" int sbk_estimator(sbk_handle* h, const float* x, const float* mask, const float* mu, const float* t,
                              const float* spk, float* out, int B, int T, void* stream) {
+    return sbk_estimator_lengths(h, x, mask, mu, t, spk, nullptr, out, B, T, stream);
+}
+
+extern "C" int sbk_estimator_lengths(sbk_handle* h, const float* x, const float* mask, const float* mu, const float* t,
+                                     const float* spk, const int64_t* lengths, float* out, int B, int T, void* stream) {
     if (!h || !x || !mask || !mu || !t || !out) return fail(SBK_ERR_ARG, "sbk_estimator: null argument");
     if (h->cfg.model != SBK_MODEL_GRADTTS) return fail(SBK_ERR_ARG, "sbk_estimator: this handle is a DiffVC model, use sbk_vc_*");
     if (h->cfg.n_spks > 1 && !spk) return fail(SBK_ERR_ARG, "sbk_estimator: spk is required when n_spks > 1");
@@ -870,6 +909,7 @@ extern "C" int sbk_estimator(sbk_handle* h, const float* x, const float* mask, c
     CU(cudaMemcpyAsync(pl.mu, mu, nb, cudaMemcpyDeviceToDevice, s));
     CU(cudaMemcpyAsync(pl.mask, mask, (size_t)B * T * sizeof(float), cudaMemcpyDeviceToDevice, s));
     CU(cudaMemcpyAsync(pl.t_rows, t, (size_t)B * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    TRY(load_lengths(h, lengths, B, s));
     int64_t n = 0;
     n += speaker(h, spk, B, s);
     n += time_table(h, B, s);
@@ -893,7 +933,7 @@ static void step_coefs(const sbk_config& c, int n_timesteps, int i, float* t_out
 
 // Build (once per plan and sampler mode) the single-launch loop graph.  Returns false - and the caller falls back to one
 // graph launch per step - if this driver / toolkit refuses conditional nodes; the reason is kept in sbk_last_error().
-static bool build_loop_graph(sbk_handle* h, int mode) {
+static bool build_loop_graph(sbk_handle* h, int mode) {     // (mode: the graph index, FinalParams.mode + 4 * ragged)
     Plan& pl = h->plan;
     if (pl.loop_state[mode] != 0) return pl.loop_state[mode] > 0;
     pl.loop_state[mode] = -1;
@@ -936,8 +976,10 @@ static bool build_loop_graph(sbk_handle* h, int mode) {
 
 static int run_steps(sbk_handle* h, const float* noise, int B, int T, int N, int s0, int s1, int stoc, cudaStream_t s, int64_t* launches) {
     Plan& pl = h->plan;
-    const int mode = h->cfg.model == SBK_MODEL_DIFFVC ? 3 : (stoc ? 2 : 1);
-    set_mode(pl, mode, false, pl.xt);
+    const int fmode = h->cfg.model == SBK_MODEL_DIFFVC ? 3 : (stoc ? 2 : 1);
+    set_mode(pl, fmode, false, pl.xt);
+    // graph index: a ragged loop (set_ragged) captures other launch parameters than a dense one
+    const int mode = fmode + (pl.ops[pl.first_op].fc.lengths ? 4 : 0);
     // the kernel indexes noise by absolute step: bias the base so slab s0 is the first one supplied
     const float* nbase = noise ? noise - (long long)s0 * B * h->cfg.n_feats * T : nullptr;
     k_set_int<<<1, 1, 0, s>>>(pl.step_next, s0);
@@ -990,6 +1032,12 @@ static int prepare_loop(sbk_handle* h, const float* mask, const float* mu, const
 extern "C" int sbk_reverse_steps(sbk_handle* h, float* xt, const float* mask, const float* mu, const float* spk,
                                  const float* noise, int B, int T, int n_timesteps, int step_begin, int step_end,
                                  int stoc, void* stream) {
+    return sbk_reverse_steps_lengths(h, xt, mask, mu, spk, noise, nullptr, B, T, n_timesteps, step_begin, step_end, stoc, stream);
+}
+
+extern "C" int sbk_reverse_steps_lengths(sbk_handle* h, float* xt, const float* mask, const float* mu, const float* spk,
+                                         const float* noise, const int64_t* lengths, int B, int T, int n_timesteps,
+                                         int step_begin, int step_end, int stoc, void* stream) {
     if (!h || !xt || !mask || !mu) return fail(SBK_ERR_ARG, "sbk_reverse_steps: null argument");
     if (n_timesteps < 1 || step_begin < 0 || step_end > n_timesteps || step_begin > step_end)
         return fail(SBK_ERR_ARG, "sbk_reverse_steps: bad step range [%d,%d) of %d", step_begin, step_end, n_timesteps);
@@ -1002,6 +1050,7 @@ extern "C" int sbk_reverse_steps(sbk_handle* h, float* xt, const float* mask, co
     int64_t n = 0;
     const size_t nb = (size_t)B * h->cfg.n_feats * T * sizeof(float);
     CU(cudaMemcpyAsync(pl.xt, xt, nb, cudaMemcpyDeviceToDevice, s));
+    TRY(load_lengths(h, lengths, B, s));
     TRY(prepare_loop(h, mask, mu, spk, B, T, n_timesteps, s, &n));
     TRY(run_steps(h, noise, B, T, n_timesteps, step_begin, step_end, stoc, s, &n));
     CU(cudaMemcpyAsync(xt, pl.xt, nb, cudaMemcpyDeviceToDevice, s));
@@ -1011,6 +1060,12 @@ extern "C" int sbk_reverse_steps(sbk_handle* h, float* xt, const float* mask, co
 
 extern "C" int sbk_reverse_diffusion(sbk_handle* h, const float* z, const float* mask, const float* mu, const float* spk,
                                      const float* noise, float* out, int B, int T, int n_timesteps, int stoc, void* stream) {
+    return sbk_reverse_diffusion_lengths(h, z, mask, mu, spk, noise, nullptr, out, B, T, n_timesteps, stoc, stream);
+}
+
+extern "C" int sbk_reverse_diffusion_lengths(sbk_handle* h, const float* z, const float* mask, const float* mu, const float* spk,
+                                             const float* noise, const int64_t* lengths, float* out, int B, int T,
+                                             int n_timesteps, int stoc, void* stream) {
     if (!h || !z || !mask || !mu || !out) return fail(SBK_ERR_ARG, "sbk_reverse_diffusion: null argument");
     if (n_timesteps < 1) return fail(SBK_ERR_ARG, "sbk_reverse_diffusion: n_timesteps must be >= 1");
     if (stoc && !noise) return fail(SBK_ERR_ARG, "sbk_reverse_diffusion: stoc=1 needs a noise buffer");
@@ -1021,8 +1076,9 @@ extern "C" int sbk_reverse_diffusion(sbk_handle* h, const float* z, const float*
     Plan& pl = h->plan;
     int64_t n = 0;
     const size_t nb = (size_t)B * h->cfg.n_feats * T * sizeof(float);
+    TRY(load_lengths(h, lengths, B, s));
     TRY(prepare_loop(h, mask, mu, spk, B, T, n_timesteps, s, &n));
-    n += launch_scale_mask(z, pl.mask, pl.xt, 0, B, h->cfg.n_feats, T, s);     // xt = z * mask (:256)
+    n += launch_scale_mask(z, pl.mask, pl.xt, 0, B, h->cfg.n_feats, T, s, lengths ? pl.lengths : nullptr);     // xt = z * mask (:256)
     TRY(run_steps(h, noise, B, T, n_timesteps, 0, n_timesteps, stoc, s, &n));
     CU(cudaMemcpyAsync(out, pl.xt, nb, cudaMemcpyDeviceToDevice, s));
     h->last_launches = n;
@@ -1052,6 +1108,7 @@ extern "C" int sbk_reverse_diffusion_host(sbk_handle* h, const float* z, const f
         CU(cudaMemcpyAsync(d_noise, noise, nb * n_timesteps, cudaMemcpyHostToDevice, s));
     }
     int64_t n = 0;
+    set_ragged(pl, false);
     TRY(prepare_loop(h, pl.mask, pl.mu, spk ? pl.spk_in : nullptr, B, T, n_timesteps, s, &n));
     n += launch_scale_mask(d_z, pl.mask, pl.xt, 0, B, h->cfg.n_feats, T, s);
     TRY(run_steps(h, d_noise, B, T, n_timesteps, 0, n_timesteps, stoc, s, &n));
@@ -1154,6 +1211,7 @@ extern "C" int sbk_vc_estimator(sbk_handle* h, const float* x, const float* mask
     int64_t n = 0;
     n += vc_fold(h, cond, 1, B, s);               // one row: the per-sample conditioning vectors
     n += time_table(h, B, s);
+    set_ragged(pl, false);
     set_mode(pl, 0, true, out);
     k_set_int<<<1, 1, 0, s>>>(pl.step_next, 0); ++n;
     { const int k = run_ops(h, s); if (k < 0) return SBK_ERR_CUDA; n += k; }
@@ -1183,6 +1241,7 @@ extern "C" int sbk_vc_reverse_diffusion(sbk_handle* h, const float* z, const flo
     CU(cudaMemcpyAsync(pl.coef, cf.data(), N * sizeof(float4), cudaMemcpyHostToDevice, s));
     n += vc_fold(h, cond, N, B, s);
     n += time_table(h, N, s);
+    set_ragged(pl, false);
     n += launch_scale_mask(z, pl.mask, pl.xt, 0, B, h->cfg.n_feats, T, s);
     TRY(run_steps(h, noise, B, T, N, 0, N, mode != 0, s, &n));
     CU(cudaMemcpyAsync(out, pl.xt, nb, cudaMemcpyDeviceToDevice, s));

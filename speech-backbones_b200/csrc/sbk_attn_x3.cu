@@ -46,7 +46,11 @@ static_assert(XS <= OPI && STAGES == 2, "fp32x3: the converted x fits a context 
 // of to_qkv as per-stage images [k|v][chunk][row][16 B] (fp32x3: [32-channel stage][hi | correction][k|v]...,
 // sbk_conv_tc.cu attn_kv_pack_image);
 // p.kv_part: [B][items per sample][4][kKvPartFloats]
-template <int MODE>
+// RAG: a ragged Grad-TTS batch (p.lengths, unet_edge at level p.lvl).  Sample b's items cut its own [H][W_b] image, flattened
+// with row width W_b as its own call flattens it, so every item holds the pixels (and the softmax partial) of that call; items
+// past its H * W_b pixels are skipped by the loader and the consumers alike.  The padded pixels are excluded, not zeroed:
+// x = 0 still gives k = 0, which would add exp(-max) to every softmax denominator.
+template <int MODE, bool RAG = false>
 __global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcParams p) {
     using namespace kx3;
     constexpr bool X3 = MODE == 2;
@@ -66,8 +70,9 @@ __global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcPara
     const int HW = p.H * p.W;
     const int ksteps = p.c0 / (KCH * EPC);
     const int ksteps_t = X3 ? 2 * ksteps : ksteps;                 // fp32x3: correction + main sub-stage per 32 channels
-    const int items = (HW + PX - 1) / PX;                          // items per sample
+    const int items = (HW + PX - 1) / PX;                          // items per sample (the partials' stride)
     const int total = p.B * items;
+    auto width = [&](int b) { return RAG ? unet_edge(p.lengths, b, p.T, p.lvl) : p.W; };   // the sample's image width
     const uint32_t bar0 = smem_u32(bars);
     auto full = [&](int s) { return bar0 + 8u * s; };
     auto empty = [&](int s) { return bar0 + 8u * (STAGES + s); };
@@ -86,6 +91,8 @@ __global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcPara
         uint32_t it = 0;
         for (int t = blockIdx.x; t < total; t += gridDim.x) {
             const int b = t / items, mt = t - b * items;
+            const int HWb = p.H * width(b);
+            if (RAG && mt * PX >= HWb) continue;
             // ---- projection: warpgroup 0 -> K^T, warpgroup 1 -> V^T  (64 pixels x 128 rows)
             float acc[64];
             if constexpr (X3) {
@@ -153,7 +160,7 @@ __global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcPara
             }
             asm volatile("bar.sync 1, 256;" ::: "memory");
             // ---- softmax over the item's pixels: max, P = exp(k - max) in place, row sums
-            const int nvalid = min(PX, HW - mt * PX) - half * (PX / 2);   // valid pixels of this thread's half (may be <= 0)
+            const int nvalid = min(PX, HWb - mt * PX) - half * (PX / 2);   // valid pixels of this thread's half (may be <= 0)
             float kr[PX / 2];
 #pragma unroll
             for (int c = 0; c < PX / 8; ++c) {
@@ -237,8 +244,10 @@ __global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcPara
         const int chs = p.c0 / EPC;
         for (int t = blockIdx.x; t < total; t += gridDim.x) {
             const int b = t / items, mt = t - b * items;
-            const int m0 = mt * PX, m_hi = m0 + PX < HW ? m0 + PX : HW;
-            const int hh0 = m0 / p.W, ww0 = m0 - hh0 * p.W;
+            const int Wb = width(b), HWb = p.H * Wb;
+            if (RAG && mt * PX >= HWb) continue;
+            const int m0 = mt * PX, m_hi = m0 + PX < HWb ? m0 + PX : HWb;
+            const int hh0 = m0 / Wb, ww0 = m0 - hh0 * Wb;
             for (int ks = 0; ks < ksteps_t; ++ks, ++it) {
                 const int s = it % STAGES;
                 const int kb = X3 ? ks >> 1 : ks;
@@ -255,7 +264,7 @@ __global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcPara
                     const int k = lane, cl = kb * KCH + k;
                     int m = m0, hh = hh0, ww = ww0, qx = 0;
                     while (m < m_hi) {                             // split the flattened run at image-row boundaries
-                        const int n = (p.W - ww) < (m_hi - m) ? (p.W - ww) : (m_hi - m);
+                        const int n = (Wb - ww) < (m_hi - m) ? (Wb - ww) : (m_hi - m);
                         bulk_g2s(xs + (k * PX + qx) * 16, src + (((long long)(b * p.H + hh) * chs + cl) * p.W + ww) * 16,
                                  (uint32_t)n * 16u, full(s));
                         m += n; qx += n; ++hh; ww = 0;
@@ -267,17 +276,19 @@ __global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcPara
     }
 }
 
-template <int MODE>
+template <int MODE, bool RAG>
 static int launch_kv(const ConvTcParams& p, cudaStream_t s) {
     static DevCache cache;
-    const int num_sms = cache.get(reinterpret_cast<const void*>(k_attn_kv_wg<MODE>));
+    const int num_sms = cache.get(reinterpret_cast<const void*>(k_attn_kv_wg<MODE, RAG>));
     if (num_sms <= 0) return -1;
     if (p.c0 % (kx3::KCH * (MODE == 1 ? 8 : 4)) != 0) return -1;
     const long long total = (long long)p.B * ((p.H * p.W + kx3::PX - 1) / kx3::PX);
     const int grid = (int)(total < num_sms ? total : num_sms);
-    k_attn_kv_wg<MODE><<<grid, kx3::THREADS, kx3::SMEM, s>>>(p);
+    k_attn_kv_wg<MODE, RAG><<<grid, kx3::THREADS, kx3::SMEM, s>>>(p);
     return 1;
 }
+template <int MODE>
+static int launch_kv(const ConvTcParams& p, cudaStream_t s) { return p.lengths ? launch_kv<MODE, true>(p, s) : launch_kv<MODE, false>(p, s); }
 
 int attn_kv_tile_pixels() { return kx3::PX; }
 int launch_attn_kv(const ConvTcParams& p, cudaStream_t s) {

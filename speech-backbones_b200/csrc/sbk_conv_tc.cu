@@ -138,12 +138,13 @@ template <int GEOM, int NT, int R> constexpr bool x3_depth_ok = Depth<GEOM, NT, 
 // VOC: the vocoder's output forms (ConvTcParams::voc) on a 1x1 GEMM; the Conv1d geometries always use them.  They only
 // differ from the sampler's in the bf16 mode (an output is bf16 only when it is an activated operand).
 //
-// RAG: a ragged Conv1d batch (ConvTcParams::lengths non-null): each sample's strips end at its own length and its tiles past
-// it are not visited.  A dense batch runs the RAG = false kernels.
+// RAG: a ragged batch (ConvTcParams::lengths non-null): each sample's strips (Conv1d) or images (the U-Net geometries) end at
+// its own edge, inputs at or past it read as zero and its tiles wholly past it are not visited.  A dense batch runs the
+// RAG = false kernels.
 template <int GEOM, bool BF16, int NT, bool RES, bool X3, bool VOC = false, int R = 1, bool RAG = false>
 __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     static_assert(!(X3 && BF16), "fp32x3 runs on tf32 operands");
-    static_assert(!RAG || geom_is_c1(GEOM), "ragged batches are Conv1d launches");
+    static_assert(!RAG || GEOM != G_C7, "ragged batches are Conv1d and U-Net launches");
     using G = Geo<GEOM, R>;
     using D = Depth<GEOM, NT, R>;
     constexpr int NACC = G::NACC, ROWS = G::ROWS;
@@ -166,6 +167,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     constexpr int EPC = BF16 ? 8 : 4;                      // elements per 16-byte channel chunk
     constexpr int CPS = KCH * EPC;                         // input channels per stage
     constexpr bool C1 = geom_is_c1(GEOM);                  // Conv1d strip geometry
+    constexpr bool RAG2 = RAG && !C1;                      // a ragged Grad-TTS batch (unet_edge)
     // bf16 mode: the raw Block-conv outputs (GroupNorm inputs) stay fp32 [C/4]; every other output is an operand tensor
     // of a later tensor-core kernel and is written as bf16 [B][H][C/8][W][8].  The vocoder's forms (VF16) instead pick
     // the dtype per output: bf16 for an activated output (act_out) and the second output act, fp32 for the others.
@@ -225,6 +227,24 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     // round-robin order of a dense batch: the work divides evenly and neighbours in time share A tiles in L2.  walk returns
     // false past the last tile.
     auto edge = [&](int b) { return ragged_edge(p.lengths, b, p.W, p.len_mul); };
+    // RAG2: sample b's output image ends at column eout(b) of level p.lvl and its input image at ein(b) (Downsample reads
+    // the level above, Upsample the level below).  The tiles keep the dense numbering; every role skips the same tiles
+    // (skip), so the ring stays in step.  A tile is skipped when every output pixel it owns lies at or past the edge:
+    // 3x3 / Downsample / Upsample tiles start at a row's column w0, and a 1x1 tile (128 flattened pixels) only when it
+    // lies inside one image row.  The ResnetBlock-tail 1x1 (RES) visits every tile: at its 168-register cap the test
+    // would spill.  Its padded outputs, like every 1x1 output past the edge, are computed but never read into a valid one.
+    auto ein = [&](int b) { return unet_edge(p.lengths, b, p.T, GEOM == G_DOWN ? p.lvl - 1 : (GEOM == G_UP ? p.lvl + 1 : p.lvl)); };
+    auto eout = [&](int b) { return unet_edge(p.lengths, b, p.T, p.lvl); };
+    auto skip = [&](int b, int h0, int w0) {
+        if constexpr (GEOM == G_PW && RES) {
+            return false;
+        } else if constexpr (GEOM == G_PW) {
+            const int ww = h0 * TPX % p.W;
+            return ww >= eout(b) && ww + TPX <= p.W;
+        } else {
+            return w0 >= (GEOM == G_UP ? ein(b) : eout(b));
+        }
+    };
     auto tiles = [&](int e) { return (e + SPAN - 1) / SPAN * ntn; };
     struct Cursor { int b, first, e; };             // a sample, the number of its first tile, its edge
     auto start = [&]() { return Cursor{0, 0, edge(0)}; };
@@ -273,13 +293,15 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
         if constexpr (RAG) cur = start();
         for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
             int b, h0, w0, n0;
-            if constexpr (RAG) {
+            if constexpr (RAG && C1) {
                 if (!walk(t, cur, b, w0, n0)) break;
                 h0 = 0;
             } else {
                 decode(t, b, h0, w0, n0);
+                if constexpr (RAG2) { if (skip(b, h0, w0)) continue; }
             }
             if constexpr (!BULK) {
+                const int win = RAG2 ? ein(b) : p.W;
 #pragma unroll
                 for (int j = 0; j < PER; ++j) {
                     const int e = tid + j * NCONS;
@@ -288,7 +310,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                     const int r = item / PXP, q = item - r * PXP;
                     const int par = q / (TPX + 1), i = q - par * (TPX + 1);      // plane 0: odd columns, plane 1: even
                     const int hi = 2 * h0 - 1 + r, wi = par == 0 ? 2 * w0 - 1 + 2 * i : 2 * w0 + 2 * i;
-                    const bool ok = in && hi >= 0 && hi < p.H && wi >= 0 && wi < p.W && !(par == 1 && i == TPX);
+                    const bool ok = in && hi >= 0 && hi < p.H && wi >= 0 && wi < win && !(par == 1 && i == TPX);
                     sl_ok[j] = ok; sl_chunk[j] = k;
                     sl_off[j] = (ok ? (long long)(b * p.H + hi) : 0) * 1048576 + (ok ? wi : 0);   // pack (row, w)
                     sl_dst[j] = in ? (uint32_t)(k * PLANE + (r * PXP + q) * 16) : 0xFFFFFFFFu;
@@ -490,8 +512,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 for (int i = tid; i < NT; i += NCONS) {
                     const int c = n0 + i, g = c / cpg;
                     const double sm_ = p.rgn.stats[(b * kGroups + g) * 2], ss = p.rgn.stats[(b * kGroups + g) * 2 + 1];
-                    const double m = sm_ * (double)p.rgn.inv_count;
-                    double var = ss * (double)p.rgn.inv_count - m * m;
+                    float inv = p.rgn.inv_count;
+                    if constexpr (RAG2) inv = gn_inv_count(p.rgn, b);
+                    const double m = sm_ * (double)inv;
+                    double var = ss * (double)inv - m * m;
                     var = var < 0.0 ? 0.0 : var;
                     s_rg[i] = (float)m;
                     s_rg[NT + i] = (float)(1.0 / sqrt(var + 1e-5)) * p.rgn.gamma[c];
@@ -504,15 +528,18 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
             const int cb_lo = NT >= 64 ? chalf * (NT / 2) : 0, cb_hi = NT >= 64 ? cb_lo + NT / 2 : (chalf == 0 ? NT : 0);
             const int Ho = (GEOM == G_DOWN || GEOM == G_UP) ? p.Ho : p.H, Wo = (GEOM == G_DOWN || GEOM == G_UP) ? p.Wo : p.W;
             const int CHo = p.Cout / 4;                            // 16-byte channel chunks of the output tensor
+            // (a ragged batch: the columns at or past the sample's edge are neither stored nor counted in the statistics)
+            // (1x1 outputs are computed and stored for every pixel: no reader takes a padded one into a valid output)
+            const int Wv = RAG2 && GEOM != G_PW ? eout(b) : Wo;
             int ho, wo; bool valid;
             if (GEOM == G_C3 || GEOM == G_C7 || GEOM == G_DOWN) {
                 ho = h0; wo = w0 + px;
-                valid = ho < Ho && wo < Wo;
+                valid = ho < Ho && wo < Wv;
             } else if (C1) {
                 ho = 0; wo = w0 + px;
                 valid = wo < Wo;
             } else if (GEOM == G_UP) {
-                valid = h0 < p.H && (w0 + px) < p.W;                 // per-phase coordinates are formed below
+                valid = h0 < p.H && (w0 + px) < (RAG2 ? ein(b) : p.W);   // per-phase coordinates are formed below
                 ho = 2 * h0; wo = 2 * (w0 + px);
             } else {
                 const long long m = (long long)h0 * TPX + px;
@@ -528,7 +555,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
             if constexpr (ROW2) {
                 // pass `phase` stages pixel block `phase` of both rows: staging pixel px is row px / 64, column 64 phase + px % 64
                 ho = h0 + (px >> 6); wo = w0 + 64 * phase + (px & 63);
-                valid = ho < Ho && wo < Wo;
+                valid = ho < Ho && wo < Wv;
                 if (!valid) { ho = 0; wo = 0; }
             }
             // GroupNorm slot row of this warp's 32 pixels (2-row tile: the row's slot set, the warp of the 1-row tile)
@@ -739,9 +766,13 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                 Cursor cur{};
                 if constexpr (RAG) cur = start();
                 for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-                    if constexpr (RAG) {
+                    if constexpr (RAG && C1) {
                         int b, w0, n0;
                         if (!walk(t, cur, b, w0, n0)) break;
+                    } else if constexpr (RAG2) {
+                        int b, h0, w0, n0;
+                        decode(t, b, h0, w0, n0);
+                        if (skip(b, h0, w0)) continue;
                     }
                     for (int ks = 0; ks < ksteps_t; ks += 2, it += 2) {
                         const uint32_t sc = it % STAGES, sm = (it + 1) % STAGES;
@@ -782,12 +813,14 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
         if constexpr (RAG) cur = start();
         for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
             int b, h0, w0, n0;
-            if constexpr (RAG) {
+            if constexpr (RAG && C1) {
                 if (!walk(t, cur, b, w0, n0)) break;
                 h0 = 0;
             } else {
                 decode(t, b, h0, w0, n0);
+                if constexpr (RAG2) { if (skip(b, h0, w0)) continue; }
             }
+            const int wedge = RAG ? (C1 ? cur.e : ein(b)) : p.W;     // input columns at or past it read as zero
             // weight image: [ntile][kstage][tap][chunk][NT][16 B]; fp32x3: [ntile][kstage][hi|correction][tap][chunk][NT][16 B]
             const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.wpk) + (size_t)b * p.w_bstride_bytes +
                                   (size_t)(n0 / NT) * ksteps * (X3 ? 2 : 1) * B_STAGE_BYTES;
@@ -807,8 +840,13 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         // the round-robin tile order a CTA normally keeps one pattern, so this (and its proxy fence,
                         // which would otherwise serialise against the bulk copies in flight) runs a handful of times.
                         const int pad = C1 ? p.pad : PADK;          // Conv1d: (K-1)*dil/2 samples of halo on each side
-                        const int wlo = w0 - pad < 0 ? 0 : w0 - pad, whi = w0 + SPAN + pad > (RAG ? cur.e : p.W) ? (RAG ? cur.e : p.W) : w0 + SPAN + pad;
-                        const int qlo = wlo - (w0 - pad), qhi = qlo + (whi - wlo);
+                        const int wlo = w0 - pad < 0 ? 0 : w0 - pad, whi = w0 + SPAN + pad > wedge ? wedge : w0 + SPAN + pad;
+                        // RAG2: only the first column at the sample's edge has to read zero - the columns past it feed
+                        // only outputs past the edge, which are neither stored nor counted - and the row's copy brings it
+                        // from the zero page (below).  So the pattern, and the one-lane zeroing, covers the left border
+                        // alone, which every sample shares: a right border that moves from tile to tile would re-zero a
+                        // stage buffer for nearly every tile.
+                        const int qlo = wlo - (w0 - pad), qdata = qlo + (whi - wlo), qhi = RAG2 ? PXP : qdata;
                         const uint32_t pat = (uint32_t)qlo | ((uint32_t)qhi << 16);
                         if (conv) {
                             stage_pat[s] = pat;              // the converters write the whole tile, its zero borders included
@@ -827,7 +865,8 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         }
                         int vrows = 0;
                         for (int r = 0; r < HR; ++r) { const int hi = C1 ? 0 : h0 - PADK + krow + r; vrows += (hi >= 0 && hi < p.H) ? 1 : 0; }
-                        if (!conv) a_tx -= (uint32_t)(KCH * vrows * (PXP - (qhi - qlo))) * 16u;
+                        const int qtx = RAG2 ? (qdata < PXP ? qdata + 1 : PXP) : qhi;     // columns a valid row's copies write
+                        if (!conv) a_tx -= (uint32_t)(KCH * vrows * (PXP - (qtx - qlo))) * 16u;
                     }
                     mbar_arrive_expect_tx(full_b(s), B_STAGE_BYTES + a_tx);
                     bulk_g2s(smem_u32(sB + s * B_STAGE_BYTES), wsrc + (size_t)(X3 ? 2 * st + (var == 0) : ks) * B_STAGE_BYTES,
@@ -858,13 +897,18 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         if (q < PXP) bulk_g2s(a_s + k * PLANE + (r * PXP + q) * 16, zero, (uint32_t)(PXP - q) * 16u, full_b(s));
                     } else {
                         const int pad = C1 ? p.pad : PADK;
-                        const int wlo = w0 - pad < 0 ? 0 : w0 - pad, whi = w0 + SPAN + pad > (RAG ? cur.e : p.W) ? (RAG ? cur.e : p.W) : w0 + SPAN + pad;
+                        const int wlo = w0 - pad < 0 ? 0 : w0 - pad, whi = w0 + SPAN + pad > wedge ? wedge : w0 + SPAN + pad;
                         const int qlo = wlo - (w0 - pad);
                         const int hi = C1 ? 0 : h0 - PADK + krow + r;
                         const uint32_t row_s = a_s + k * PLANE + (r * PXP) * 16;
-                        if (hi < 0 || hi >= p.H) bulk_g2s(row_s, zero, PXP * 16u, full_b(s));
-                        else bulk_g2s(row_s + qlo * 16, src + (((long long)(b * p.H + hi) * chs + cl) * p.W + wlo) * 16,
-                                      (uint32_t)(whi - wlo) * 16u, full_b(s));
+                        if (hi < 0 || hi >= p.H) {
+                            bulk_g2s(row_s, zero, PXP * 16u, full_b(s));
+                        } else {
+                            bulk_g2s(row_s + qlo * 16, src + (((long long)(b * p.H + hi) * chs + cl) * p.W + wlo) * 16,
+                                     (uint32_t)(whi - wlo) * 16u, full_b(s));
+                            const int qe = qlo + (whi - wlo);       // RAG2: the row's first column at or past the edge
+                            if (RAG2 && qe < PXP) bulk_g2s(row_s + qe * 16, zero, 16u, full_b(s));
+                        }
                     }
                 }
             }
@@ -879,6 +923,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc(const ConvTcParams p) {
 template <int GEOM, int NT, bool RES = false, int R = 1>
 __global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc_x3(const ConvTcParams p) {
     conv_tc_body<GEOM, false, NT, RES, true, false, R>(p);
+}
+// a ragged U-Net batch (ConvTcParams::lengths): tf32 / bf16, and fp32x3
+template <int GEOM, bool BF16, int NT, bool RES = false, int R = 1>
+__global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc_ragged(const ConvTcParams p) {
+    conv_tc_body<GEOM, BF16, NT, RES, false, false, R, true>(p);
+}
+template <int GEOM, int NT, bool RES = false, int R = 1>
+__global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc_ragged_x3(const ConvTcParams p) {
+    conv_tc_body<GEOM, false, NT, RES, true, false, R, true>(p);
 }
 // a ragged Conv1d batch (ConvTcParams::lengths): tf32 / bf16, and fp32x3
 template <int GEOM, bool BF16, int NT>
@@ -895,10 +948,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_gemm_voc_bf16(const ConvTcParam
     conv_tc_body<G_PW, true, NT, false, false, true>(p);
 }
 
-// the kernel of one launch configuration; VOC: the vocoder's bf16 GEMM; RAG: a ragged Conv1d batch
+// the kernel of one launch configuration; VOC: the vocoder's bf16 GEMM; RAG: a ragged Conv1d or U-Net batch
 template <int GEOM, int FORM, int NT, bool RES, int R, bool VOC, bool RAG>
 constexpr auto tc_kernel() {
     if constexpr (VOC) return k_gemm_voc_bf16<NT>;
+    else if constexpr (RAG && !geom_is_c1(GEOM) && FORM == FORM_X3) return k_conv_tc_ragged_x3<GEOM, NT, RES, R>;
+    else if constexpr (RAG && !geom_is_c1(GEOM)) return k_conv_tc_ragged<GEOM, FORM == FORM_BF16, NT, RES, R>;
     else if constexpr (RAG && FORM == FORM_X3) return k_conv1d_ragged_x3<GEOM, NT>;
     else if constexpr (RAG) return k_conv1d_ragged<GEOM, FORM == FORM_BF16, NT>;
     else if constexpr (FORM == FORM_X3) return k_conv_tc_x3<GEOM, NT, RES, R>;
@@ -959,6 +1014,12 @@ template <int GEOM, bool RAG> static int launch_c1_batch(const ConvTcParams& p, 
 template <int GEOM> static int launch_c1(const ConvTcParams& p, cudaStream_t s) {
     return p.lengths ? launch_c1_batch<GEOM, true>(p, s) : launch_c1_batch<GEOM, false>(p, s);
 }
+// a U-Net launch: the dense kernel, or its ragged twin when the sampler passes lengths (the vocoder's 1x1 GEMM carries
+// its Conv1d lengths but computes every row: voc)
+template <int GEOM, int FORM, int NT, bool RES = false, int R = 1>
+static int launch_unet(const ConvTcParams& p, cudaStream_t s) {
+    return p.lengths && !p.voc ? launch_tc<GEOM, FORM, NT, RES, R, false, true>(p, s) : launch_tc<GEOM, FORM, NT, RES, R>(p, s);
+}
 
 int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
     if (p.form < FORM_TF32 || p.form > FORM_BF16 || p.nt <= 0 || p.nt > 128 || p.Cout % p.nt != 0) return -1;
@@ -981,37 +1042,37 @@ int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
     constexpr int T = FORM_TF32, X = FORM_X3, B = FORM_BF16;
     switch (tc_key(p.geom, p.form, p.nt, rows, res, voc)) {
         // 3x3: one-row tiles, and two-row tiles 64 channels wide
-        case tc_key(G_C3, T, 128):                  return launch_tc<G_C3, T, 128>(p, s);
-        case tc_key(G_C3, T, 64):                   return launch_tc<G_C3, T, 64>(p, s);
-        case tc_key(G_C3, T, 64, 2):                return launch_tc<G_C3, T, 64, false, 2>(p, s);
-        case tc_key(G_C3, B, 128):                  return launch_tc<G_C3, B, 128>(p, s);
-        case tc_key(G_C3, B, 64):                   return launch_tc<G_C3, B, 64>(p, s);
-        case tc_key(G_C3, B, 64, 2):                return launch_tc<G_C3, B, 64, false, 2>(p, s);
-        case tc_key(G_C3, X, 128):                  return launch_tc<G_C3, X, 128>(p, s);
-        case tc_key(G_C3, X, 64):                   return launch_tc<G_C3, X, 64>(p, s);
-        case tc_key(G_C3, X, 64, 2):                return launch_tc<G_C3, X, 64, false, 2>(p, s);
+        case tc_key(G_C3, T, 128):                  return launch_unet<G_C3, T, 128>(p, s);
+        case tc_key(G_C3, T, 64):                   return launch_unet<G_C3, T, 64>(p, s);
+        case tc_key(G_C3, T, 64, 2):                return launch_unet<G_C3, T, 64, false, 2>(p, s);
+        case tc_key(G_C3, B, 128):                  return launch_unet<G_C3, B, 128>(p, s);
+        case tc_key(G_C3, B, 64):                   return launch_unet<G_C3, B, 64>(p, s);
+        case tc_key(G_C3, B, 64, 2):                return launch_unet<G_C3, B, 64, false, 2>(p, s);
+        case tc_key(G_C3, X, 128):                  return launch_unet<G_C3, X, 128>(p, s);
+        case tc_key(G_C3, X, 64):                   return launch_unet<G_C3, X, 64>(p, s);
+        case tc_key(G_C3, X, 64, 2):                return launch_unet<G_C3, X, 64, false, 2>(p, s);
         // 1x1: plain, the ResnetBlock tail, and the vocoder's bf16 GEMM
-        case tc_key(G_PW, T, 128):                  return launch_tc<G_PW, T, 128>(p, s);
-        case tc_key(G_PW, T, 64):                   return launch_tc<G_PW, T, 64>(p, s);
-        case tc_key(G_PW, T, 128, 1, true):         return launch_tc<G_PW, T, 128, true>(p, s);
-        case tc_key(G_PW, T, 64, 1, true):          return launch_tc<G_PW, T, 64, true>(p, s);
-        case tc_key(G_PW, B, 128):                  return launch_tc<G_PW, B, 128>(p, s);
-        case tc_key(G_PW, B, 64):                   return launch_tc<G_PW, B, 64>(p, s);
-        case tc_key(G_PW, B, 128, 1, true):         return launch_tc<G_PW, B, 128, true>(p, s);
-        case tc_key(G_PW, B, 64, 1, true):          return launch_tc<G_PW, B, 64, true>(p, s);
+        case tc_key(G_PW, T, 128):                  return launch_unet<G_PW, T, 128>(p, s);
+        case tc_key(G_PW, T, 64):                   return launch_unet<G_PW, T, 64>(p, s);
+        case tc_key(G_PW, T, 128, 1, true):         return launch_unet<G_PW, T, 128, true>(p, s);
+        case tc_key(G_PW, T, 64, 1, true):          return launch_unet<G_PW, T, 64, true>(p, s);
+        case tc_key(G_PW, B, 128):                  return launch_unet<G_PW, B, 128>(p, s);
+        case tc_key(G_PW, B, 64):                   return launch_unet<G_PW, B, 64>(p, s);
+        case tc_key(G_PW, B, 128, 1, true):         return launch_unet<G_PW, B, 128, true>(p, s);
+        case tc_key(G_PW, B, 64, 1, true):          return launch_unet<G_PW, B, 64, true>(p, s);
         case tc_key(G_PW, B, 128, 1, false, true):  return launch_tc<G_PW, B, 128, false, 1, true>(p, s);
         case tc_key(G_PW, B, 64, 1, false, true):   return launch_tc<G_PW, B, 64, false, 1, true>(p, s);
-        case tc_key(G_PW, X, 128):                  return launch_tc<G_PW, X, 128>(p, s);
-        case tc_key(G_PW, X, 64):                   return launch_tc<G_PW, X, 64>(p, s);
-        case tc_key(G_PW, X, 128, 1, true):         return launch_tc<G_PW, X, 128, true>(p, s);
-        case tc_key(G_PW, X, 64, 1, true):          return launch_tc<G_PW, X, 64, true>(p, s);
+        case tc_key(G_PW, X, 128):                  return launch_unet<G_PW, X, 128>(p, s);
+        case tc_key(G_PW, X, 64):                   return launch_unet<G_PW, X, 64>(p, s);
+        case tc_key(G_PW, X, 128, 1, true):         return launch_unet<G_PW, X, 128, true>(p, s);
+        case tc_key(G_PW, X, 64, 1, true):          return launch_unet<G_PW, X, 64, true>(p, s);
         // Downsample, Upsample
-        case tc_key(G_DOWN, T, 64):                 return launch_tc<G_DOWN, T, 64>(p, s);
-        case tc_key(G_DOWN, B, 64):                 return launch_tc<G_DOWN, B, 64>(p, s);
-        case tc_key(G_DOWN, X, 64):                 return launch_tc<G_DOWN, X, 64>(p, s);
-        case tc_key(G_UP, T, 64):                   return launch_tc<G_UP, T, 64>(p, s);
-        case tc_key(G_UP, B, 64):                   return launch_tc<G_UP, B, 64>(p, s);
-        case tc_key(G_UP, X, 64):                   return launch_tc<G_UP, X, 64>(p, s);
+        case tc_key(G_DOWN, T, 64):                 return launch_unet<G_DOWN, T, 64>(p, s);
+        case tc_key(G_DOWN, B, 64):                 return launch_unet<G_DOWN, B, 64>(p, s);
+        case tc_key(G_DOWN, X, 64):                 return launch_unet<G_DOWN, X, 64>(p, s);
+        case tc_key(G_UP, T, 64):                   return launch_unet<G_UP, T, 64>(p, s);
+        case tc_key(G_UP, B, 64):                   return launch_unet<G_UP, B, 64>(p, s);
+        case tc_key(G_UP, X, 64):                   return launch_unet<G_UP, X, 64>(p, s);
         // 7x7 (PostNet): tf32 and fp32x3
         case tc_key(G_C7, T, 128):                  return launch_tc<G_C7, T, 128>(p, s);
         case tc_key(G_C7, T, 64):                   return launch_tc<G_C7, T, 64>(p, s);

@@ -23,13 +23,34 @@ __host__ __device__ constexpr int conv_tc_c1_halo(int g) { return geom_c1_wide(g
 enum Pro { PRO_NONE = 0, PRO_MASK = 1, PRO_GN = 2 };
 enum Epi { EPI_PLAIN = 0, EPI_RES = 1, EPI_KV = 2 };
 
+// A ragged Grad-TTS batch (sbk_*_lengths): utterance b runs on its own grid of T_b = fix_len_compatibility(lengths[b])
+// frames (a multiple of 4; the length clamped to [1, T] first), so its image at U-Net level l is W_b,l = T_b >> l wide.
+// lengths == nullptr: every utterance has all T frames.
+__host__ __device__ __forceinline__ int unet_frames(const int64_t* lengths, long long b, int T) {
+    if (!lengths) return T;
+    const long long t = lengths[b];
+    return ((t < 1 ? 1 : (t > T ? T : (int)t)) + 3) & ~3;
+}
+__host__ __device__ __forceinline__ int unet_edge(const int64_t* lengths, long long b, int T, int lvl) {
+    return unet_frames(lengths, b, T) >> lvl;
+}
+
 // GroupNorm statistics of one conv output: per (sample, group) {sum, sum of squares} in fp64.
 struct GnRef {
     const double* stats;   // [B][8][2]
     const float* gamma;    // [C]
     const float* beta;     // [C]
     float inv_count;       // 1 / ((C/8) * H * W)
+    // ragged batch (nullable): sample b counts H * W_b,lvl pixels, 1 / (cnt_ch * W_b) with cnt_ch = (C/8) * H rounded as
+    // the planner rounds it, so the divisor is bit for bit the one of the sample's own call
+    const int64_t* lengths = nullptr; float cnt_ch = 0.f; int T = 0, lvl = 0;
 };
+#ifdef __CUDACC__
+__device__ __forceinline__ float gn_inv_count(const GnRef& g, int b) {
+    if (!g.lengths) return g.inv_count;
+    return __frcp_rn(__fmul_rn(g.cnt_ch, (float)unet_edge(g.lengths, b, g.T, g.lvl)));
+}
+#endif
 
 // Implicit-GEMM convolution over NHWC fp32 activations.
 //   out[b][m][co] = epilogue( sum_{tap, ci} prologue(in[b][pix(m,tap)][ci]) * w[tap][ci][co] )
@@ -52,6 +73,9 @@ struct IgemmParams {
     double* ostats;                               // EPI_PLAIN: accumulate GN statistics of `out` (nullable)
     const float* rraw; GnRef rgn; int out_lvl;    // EPI_RES: out = acc + bias + Mish(GN(rraw))*mask
     float* kv_part;                               // EPI_KV: [B][mtiles][4][kKvPartFloats]
+    // ragged batch (nullable, unet_edge): the m index of a sample runs over its own [Hout][W_b] image, so tiles, GroupNorm
+    // partials and attention items cut its pixels as its own call does; inputs at or past W_b read as zero
+    const int64_t* lengths = nullptr;
 };
 
 // Layout and number form of the U-Net's activation tensors, one per precision mode (GnActParams / ResFinalParams::form),
@@ -107,6 +131,9 @@ struct ConvTcParams {
     // Conv1d geometries: a ragged batch.  lengths (device int64 [B], nullable: every utterance W samples) holds each
     // utterance's mel frames and len_mul the samples per frame at this stage; utterance b ends at ragged_edge(..).  Its
     // strips read zeros past that edge, as past W, and its tiles that start at or past it are skipped.
+    // U-Net geometries: a ragged Grad-TTS batch, utterance b's output image ends at unet_edge(lengths, b, T, lvl) and its
+    // input image at the input level's edge.  Inputs at or past the edge read as zero, tiles wholly past it are skipped,
+    // and GroupNorm partials count only the columns below it.
     const int64_t* lengths; int len_mul;
 };
 
@@ -153,7 +180,7 @@ __host__ __device__ inline size_t conv_tc_wimg_bytes(const ConvTcWImg& g, int co
 
 // Block activation between the two convs of a ResnetBlock, written once in operand form (diffusion.py:57,76):
 //   act = mask ? Mish(GN(raw)) + tproj : 0        (tensor-core forms only: the fp32 mode fuses it into the next conv)
-struct GnActParams {
+struct GnActParams {          // (a ragged batch: gn.lengths; frames at or past the edge are not visited)
     const float* raw; GnRef gn; const float* tb; int tb_stride; int tb_per_sample; const int* step;
     const float* mask; int T; int lvl;
     float* out; int B, H, W, C;
@@ -171,9 +198,10 @@ struct FirstConvParams {        // Block.conv of downs.0.0.block1 on the planar 
     // DiffVC: the 128 conditioning channels are spatially constant, so they act as ONE extra input channel whose
     // value is the mask and whose weights are per (row, sample): w_extra[(row*B + b)][9][C] (row = *step or 0)
     const float* w_extra; const int* step; int extra_per_sample_row;
+    const int64_t* lengths = nullptr;   // ragged batch: frames at or past T_b read as zero and count in no statistic
 };
 
-struct ResFinalParams {         // out = Mish(GN(h2raw))*mask + res(x*mask)
+struct ResFinalParams {         // (a ragged batch: gn.lengths; frames at or past the edge are not visited)         // out = Mish(GN(h2raw))*mask + res(x*mask)
     const float* h2raw; GnRef gn;
     const float* x;             // identity residual source (NHWC, same C) or nullptr for the planar first block
     const float* mu; const float* xt; const float* spk_s;   // planar inputs for downs.0.0.res_conv
@@ -188,6 +216,9 @@ struct ResFinalParams {         // out = Mish(GN(h2raw))*mask + res(x*mask)
 
 struct AttnCtxParams {          // merge per-tile softmax partials -> normalised context [B][4][32][32]
     const float* kv_part; int mtiles; float* ctx; int B;
+    // ragged batch (nullable): sample b merges only the ceil(H * W_b,lvl / tile_px) partials of its own pixels (mtiles
+    // stays the per-sample stride)
+    const int64_t* lengths = nullptr; int T = 0, lvl = 0, H = 0, tile_px = 0;
 };
 
 struct AttnMixParams {          // A_b = I + g * Wout * blockdiag(ctx^T) * Wq ; packed as [ci][co]; bias' = g*bout
@@ -217,6 +248,7 @@ struct FinalParams {            // final_block GN+Mish, final_conv 1x1 -> 1, mas
     int B, H, T, C;
     int chw4;
     int exact;                  // fp32x3 mode: exact Mish (expf + IEEE division) instead of the fast intrinsics
+    const int64_t* lengths = nullptr;   // ragged batch: frames at or past T_b are written as 0
 };
 
 struct TimeTableParams {        // SinusoidalPosEmb + mlp + the 12 per-ResnetBlock projections
@@ -319,7 +351,9 @@ int launch_time_table(const TimeTableParams& p, cudaStream_t s);
 int launch_spk(const SpkParams& p, cudaStream_t s);
 int launch_step_begin(const StepBeginParams& p, cudaStream_t s);
 int device_sm_count();      // SMs of the current device (grid caps of the grid-stride kernels)
-int launch_scale_mask(const float* z, const float* mask, float* out, long long n_per_b_row, int B, int H, int T, cudaStream_t s);
+// lengths (nullable): a ragged batch, frames at or past T_b are written as 0
+int launch_scale_mask(const float* z, const float* mask, float* out, long long n_per_b_row, int B, int H, int T, cudaStream_t s,
+                      const int64_t* lengths = nullptr);
 
 // the part of an fp32 value the tensor core's tf32 operand path drops (low 13 mantissa bits): exact in fp32
 __device__ __forceinline__ float tf32_lo(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }

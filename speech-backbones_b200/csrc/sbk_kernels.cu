@@ -43,8 +43,9 @@ template <bool EXACT> __device__ __forceinline__ float mish_sel(float x) { retur
 __device__ __forceinline__ void gn_mean_rstd(const GnRef& g, int b, int grp, float& mean, float& rstd) {
     const double s = g.stats[(b * kGroups + grp) * 2 + 0];
     const double ss = g.stats[(b * kGroups + grp) * 2 + 1];
-    const double m = s * (double)g.inv_count;
-    double var = ss * (double)g.inv_count - m * m;
+    const float inv = gn_inv_count(g, b);
+    const double m = s * (double)inv;
+    double var = ss * (double)inv - m * m;
     var = var < 0.0 ? 0.0 : var;
     mean = (float)m;
     rstd = (float)(1.0 / sqrt(var + 1e-5));   // GroupNorm eps, torch default (diffusion.py:53)
@@ -87,18 +88,23 @@ __global__ void __launch_bounds__(IG_THREADS, 3) k_igemm(const IgemmParams p) {
     const int Cin = p.c0 + p.c1;
     const int Cout = p.Cout;
 
+    // a ragged batch: sample b's images are Win_b / Wout_b wide (unet_edge), and its m index runs over them alone - the
+    // flattening its own call uses - while addresses keep the batch's row pitch; its tiles past them exit here
+    const int Win_b = p.lengths ? unet_edge(p.lengths, b, p.T, p.in_lvl) : p.Win;
+    const int Wout_b = p.lengths ? unet_edge(p.lengths, b, p.T, p.out_lvl) : p.Wout;
     int mt = blockIdx.x, phase = 0, HWm;
     if (GEOM == G_UP) {
         const int per = (p.Hin * p.Win + IG_TM - 1) / IG_TM;
         phase = mt / per;
         mt -= phase * per;
-        HWm = p.Hin * p.Win;
+        HWm = p.Hin * Win_b;
     } else {
-        HWm = p.Hout * p.Wout;
+        HWm = p.Hout * Wout_b;
     }
     const int m0 = mt * IG_TM;
+    if (m0 >= HWm) return;
     const int ph = phase >> 1, pw = phase & 1;
-    const int Wm = (GEOM == G_UP) ? p.Win : p.Wout;   // width of the m index space
+    const int Wm = (GEOM == G_UP) ? Win_b : Wout_b;   // width of the m index space
 
     // ---- prologue tables
     float* pg_mean = ext;
@@ -163,7 +169,7 @@ __global__ void __launch_bounds__(IG_THREADS, 3) k_igemm(const IgemmParams p) {
             int hi, wi;
             if (GEOM == G_DOWN) { hi = 2 * g_h[i] + dh; wi = 2 * g_w[i] + dw; }
             else { hi = g_h[i] + dh; wi = g_w[i] + dw; }
-            const bool ok = g_ok[i] && hi >= 0 && hi < p.Hin && wi >= 0 && wi < p.Win;
+            const bool ok = g_ok[i] && hi >= 0 && hi < p.Hin && wi >= 0 && wi < Win_b;
             if (ok) {
                 ra[i] = ldg4(src + ((long long)(b * p.Hin + hi) * p.Win + wi) * cs + co);
                 rm[i] = (p.pro != PRO_NONE) ? __ldg(p.mask + (long long)b * p.T + ((long long)wi << p.in_lvl)) : 1.f;
@@ -311,8 +317,9 @@ __global__ void __launch_bounds__(IG_THREADS, 3) k_igemm(const IgemmParams p) {
             wo = 2 * mw + pw;
             opix = (2 * mh + ph) * p.Wout + wo;
         } else {
-            opix = m;
-            wo = m % p.Wout;
+            const int mh = m / Wm;
+            wo = m - mh * Wm;
+            opix = mh * p.Wout + wo;
         }
         float v[8];
 #pragma unroll
@@ -398,6 +405,11 @@ __global__ void __launch_bounds__(256) k_first_conv(const FirstConvParams p) {
     const int tid = threadIdx.x, b = blockIdx.z, n0 = blockIdx.y * 64;
     const int wtiles = (p.T + 255) / 256;
     const int h = blockIdx.x / wtiles, w0 = (blockIdx.x - h * wtiles) * 256;
+    // a ragged batch: the sample's grid ends at T_b; its frames past it read as zero (its own call's padding), count in no
+    // statistic and are not stored, and a CTA wholly past it exits.  CTAs start at frame 0 of a row, so every warp partial
+    // covers the frames it covers in the sample's own call.
+    const int Tb = unet_frames(p.lengths, b, p.T);
+    if (w0 >= Tb) return;
     const int K = p.cin * 9;
     const int kreal = p.w_extra ? (p.cin - 1) * 9 : K;       // rows of s_w that come from the shared weight
     for (int i = tid; i < kreal * 64; i += 256) s_w[i] = p.w[(i >> 6) * p.C + n0 + (i & 63)];
@@ -412,7 +424,7 @@ __global__ void __launch_bounds__(256) k_first_conv(const FirstConvParams p) {
         const int ci = i / 774, rem = i - ci * 774, r = rem / 258, q = rem - r * 258;
         const int hi = h + r - 1, wi = w0 + q - 1;
         float v = 0.f;
-        if (hi >= 0 && hi < p.H && wi >= 0 && wi < p.T) {
+        if (hi >= 0 && hi < p.H && wi >= 0 && wi < Tb) {
             const float mk = __ldg(p.mask + (long long)b * p.T + wi);
             const long long idx = ((long long)b * p.H + hi) * p.T + wi;
             const float x = ci == 0 ? __ldg(p.mu + idx) : (ci == 1 ? __ldg(p.xt + idx) : (p.w_extra ? 1.f : __ldg(p.spk_s + b * p.H + hi)));
@@ -454,7 +466,7 @@ __global__ void __launch_bounds__(256) k_first_conv(const FirstConvParams p) {
         float s = 0.f, q = 0.f;
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            if (w0 + pg + 64 * i < p.T) {
+            if (w0 + pg + 64 * i < Tb) {
 #pragma unroll
                 for (int j = 0; j < 8; ++j) { const float v = acc[i][hf * 8 + j]; s += v; q = fmaf(v, v, q); }
             }
@@ -470,7 +482,7 @@ __global__ void __launch_bounds__(256) k_first_conv(const FirstConvParams p) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         const int w = w0 + pg + 64 * i;
-        if (w >= p.T) continue;
+        if (w >= Tb) continue;
         if (p.chw4) {
             float* o = p.out + ((((long long)b * p.H + h) * (p.C / 4) + (n0 + cg * 16) / 4) * p.T + w) * 4;
 #pragma unroll
@@ -628,7 +640,9 @@ static int planar_ew_grid(int form, int H, int W, int C) {
     return C / (4 * lanes) * nhg;
 }
 
-template <int FORM, int TAIL, class P>
+// RAG: a ragged batch (p.gn.lengths): the frames at or past the sample's edge are not visited - no reader of this output
+// looks at them.  (A template flag: the edge in a register would cost the dense loop a spill.)
+template <int FORM, int TAIL, bool RAG, class P>
 __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
     constexpr bool B16 = FORM == FORM_BF16, X3 = FORM == FORM_X3;
     constexpr int LPF = lanes_per_frame(FORM), F = 256 / LPF;
@@ -683,7 +697,8 @@ __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
         w2 = has_spk ? reinterpret_cast<const float4*>(ext + 2 * q.C)[c4] : z4;
     };
     if constexpr (TAIL == TAIL_PLANAR && B16) res_w(p);
-    for (int w = wl; w < p.W; w += tw) {
+    // (RAG: the edge is re-read per frame rather than held in a register the exact-Mish fp32x3 walk has no room for)
+    for (int w = wl; w < (RAG ? unet_edge(p.gn.lengths, b, p.T, p.lvl) : p.W); w += tw) {
         const float mk = __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl));
         for (int h0 = (hg * nsub + sub) * U; h0 < p.H; h0 += nhg * nsub * U) {
             float4 r[U]; Unit xv[U]; float i0[U], i1[U], i2[U];
@@ -737,22 +752,28 @@ __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
     }
 }
 
-template <int FORM>
-__global__ void __launch_bounds__(256) k_gn_act(const GnActParams p) { planar_ew<FORM, TAIL_ACT>(p, p.raw); }
+template <int FORM, bool RAG>
+__global__ void __launch_bounds__(256) k_gn_act(const GnActParams p) { planar_ew<FORM, TAIL_ACT, RAG>(p, p.raw); }
 
 // the bf16 identity tail keeps to 64 registers for 4 CTAs per SM; its planar-input tail needs more and runs 2 (0: no minimum)
-template <int FORM, bool PLANAR>
+template <int FORM, bool PLANAR, bool RAG>
 __global__ void __launch_bounds__(256, FORM == FORM_BF16 ? (PLANAR ? 2 : 4) : 0) k_resfinal(const ResFinalParams p) {
-    planar_ew<FORM, PLANAR ? TAIL_PLANAR : TAIL_ID>(p, p.h2raw);
+    planar_ew<FORM, PLANAR ? TAIL_PLANAR : TAIL_ID, RAG>(p, p.h2raw);
+}
+
+template <int FORM>
+static void launch_gn_act_form(const GnActParams& p, cudaStream_t s) {
+    const dim3 grid(planar_ew_grid(p.form, p.H, p.W, p.C), p.B);
+    const size_t sm = 4 * p.C * sizeof(float);
+    if (p.gn.lengths) k_gn_act<FORM, true><<<grid, 256, sm, s>>>(p);
+    else k_gn_act<FORM, false><<<grid, 256, sm, s>>>(p);
 }
 
 int launch_gn_act(const GnActParams& p, cudaStream_t s) {
-    const dim3 grid(planar_ew_grid(p.form, p.H, p.W, p.C), p.B);
-    const size_t sm = 4 * p.C * sizeof(float);
     switch (p.form) {
-        case FORM_TF32: k_gn_act<FORM_TF32><<<grid, 256, sm, s>>>(p); return 1;
-        case FORM_X3:   k_gn_act<FORM_X3><<<grid, 256, sm, s>>>(p); return 1;
-        case FORM_BF16: k_gn_act<FORM_BF16><<<grid, 256, sm, s>>>(p); return 1;
+        case FORM_TF32: launch_gn_act_form<FORM_TF32>(p, s); return 1;
+        case FORM_X3:   launch_gn_act_form<FORM_X3>(p, s); return 1;
+        case FORM_BF16: launch_gn_act_form<FORM_BF16>(p, s); return 1;
     }
     return -1;
 }
@@ -760,8 +781,13 @@ int launch_gn_act(const GnActParams& p, cudaStream_t s) {
 template <int FORM>
 static void launch_resfinal_planar(const ResFinalParams& p, size_t sm, cudaStream_t s) {
     const dim3 grid(planar_ew_grid(FORM, p.H, p.W, p.C), p.B);
-    if (p.x) k_resfinal<FORM, false><<<grid, 256, sm, s>>>(p);
-    else k_resfinal<FORM, true><<<grid, 256, sm, s>>>(p);
+    if (p.gn.lengths) {
+        if (p.x) k_resfinal<FORM, false, true><<<grid, 256, sm, s>>>(p);
+        else k_resfinal<FORM, true, true><<<grid, 256, sm, s>>>(p);
+    } else {
+        if (p.x) k_resfinal<FORM, false, false><<<grid, 256, sm, s>>>(p);
+        else k_resfinal<FORM, true, false><<<grid, 256, sm, s>>>(p);
+    }
 }
 
 int launch_resfinal(const ResFinalParams& p, cudaStream_t s) {
@@ -794,10 +820,12 @@ __global__ void __launch_bounds__(1024) k_attn_ctx(const AttnCtxParams p) {
     const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
     const float* base = p.kv_part + ((long long)b * p.mtiles * kHeads + h) * kKvPartFloats;
     const long long tstride = (long long)kHeads * kKvPartFloats;
+    // partials of this sample: all mtiles, or in a ragged batch the ones of its own H * W_b pixels (in its own order)
+    const int nt = p.lengths ? (p.H * unet_edge(p.lengths, b, p.T, p.lvl) + p.tile_px - 1) / p.tile_px : p.mtiles;
     {
         const int w = tid >> 5, lane = tid & 31;
         float mx = -INFINITY;
-        for (int i = w; i < p.mtiles; i += 32) mx = fmaxf(mx, base[i * tstride + lane]);
+        for (int i = w; i < nt; i += 32) mx = fmaxf(mx, base[i * tstride + lane]);
         s_red[w * 33 + lane] = mx;
     }
     __syncthreads();
@@ -812,7 +840,7 @@ __global__ void __launch_bounds__(1024) k_attn_ctx(const AttnCtxParams p) {
     const float M = s_M[d];
     float z = 0.f, a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
 #pragma unroll 2
-    for (int i = sub; i < p.mtiles; i += 4) {
+    for (int i = sub; i < nt; i += 4) {
         const float* pt = base + i * tstride;
         const float f = expf(pt[d] - M);
         z = fmaf(f, pt[32 + d], z);
@@ -979,11 +1007,14 @@ __global__ void __launch_bounds__(256) k_final(const FinalParams p) {
             p.xt_out[idx] = (xt - dxt) * mk;
         }
     };
+    // a ragged batch: frames at or past T_b are written as 0 and nothing there is read
+    const int Tb = unet_frames(p.lengths, b, p.T);
     if (p.chw4) {
         // [B][H][C/4][T][4]: one thread per frame; per channel chunk a warp reads 32 frames x 16 B = 512 contiguous bytes
         const int c4n = p.C / 4;
         for (int m = blockIdx.x * 256 + tid; m < HW; m += gridDim.x * 256) {
             const int h = m / p.T, w = m - h * p.T;
+            if (w >= Tb) { p.xt_out[(long long)b * HW + m] = 0.f; continue; }
             const float mk = __ldg(p.mask + (long long)b * p.T + w);
             float dot = 0.f;
             if (mk != 0.f) {
@@ -1008,7 +1039,8 @@ __global__ void __launch_bounds__(256) k_final(const FinalParams p) {
             const int m = base + it * 16 + pl;
             const bool inb = m < HW;        // shuffles below run for the full warp regardless
             const int w = inb ? m % p.T : 0;
-            const float mk = inb ? __ldg(p.mask + (long long)b * p.T + w) : 0.f;
+            const bool live = inb && w < Tb;
+            const float mk = live ? __ldg(p.mask + (long long)b * p.T + w) : 0.f;
             float dot = 0.f;
             if (mk != 0.f) {
                 const float* rp = p.raw + ((long long)b * HW + m) * p.C;
@@ -1022,7 +1054,8 @@ __global__ void __launch_bounds__(256) k_final(const FinalParams p) {
             }
 #pragma unroll
             for (int o = 8; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o, 16);
-            if (lane16 == 0 && inb) update((long long)b * HW + m, mk, dot);
+            if (lane16 == 0 && live) update((long long)b * HW + m, mk, dot);
+            else if (lane16 == 0 && inb) p.xt_out[(long long)b * HW + m] = 0.f;
         }
     }
 }
@@ -1355,17 +1388,19 @@ int launch_step_begin(const StepBeginParams& p, cudaStream_t s) {
 }
 
 // xt0 = z * mask (diffusion.py:256)
-__global__ void k_scale_mask(const float* z, const float* mask, float* out, int H, int T, long long n) {
+// (a ragged batch: 0 at or past T_b)
+__global__ void k_scale_mask(const float* z, const float* mask, float* out, int H, int T, long long n, const int64_t* lengths) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int w = (int)(i % T);
     const long long b = i / ((long long)H * T);
-    out[i] = z[i] * mask[b * T + w];
+    out[i] = w < unet_frames(lengths, b, T) ? z[i] * mask[b * T + w] : 0.f;
 }
 
-int launch_scale_mask(const float* z, const float* mask, float* out, long long, int B, int H, int T, cudaStream_t s) {
+int launch_scale_mask(const float* z, const float* mask, float* out, long long, int B, int H, int T, cudaStream_t s,
+                      const int64_t* lengths) {
     const long long n = (long long)B * H * T;
-    k_scale_mask<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(z, mask, out, H, T, n);
+    k_scale_mask<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(z, mask, out, H, T, n, lengths);
     return 1;
 }
 

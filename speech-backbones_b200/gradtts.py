@@ -19,7 +19,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .binding import Engine, prior_expand
+from .binding import Engine, check_lengths, prior_expand
 
 
 class BaseModule(nn.Module):
@@ -230,7 +230,10 @@ class Diffusion(BaseModule):
 
     # ---- sampling (diffusion.py:254-279) -----------------------------------------------------
     @torch.no_grad()
-    def reverse_diffusion(self, z, mask, mu, n_timesteps, stoc=False, spk=None):
+    def reverse_diffusion(self, z, mask, mu, n_timesteps, stoc=False, spk=None, *, lengths=None):
+        """lengths: optional int64 [B] valid frames per utterance (e.g. y_lengths): utterance b is then sampled on its own
+        fix_len_compatibility(lengths[b]) frames, as a call on its slices alone would be, and its frames past them are 0
+        (Engine.estimator).  None keeps the padded-batch semantics of the reference's batched call."""
         eng = self.engine()
         # The sampler state (xt, mu, noise, Euler update) is fp32 in every precision mode; reduced-precision callers
         # (config 3: bf16 tensors in / out) are widened here and the result is cast back to the caller's dtype.
@@ -239,16 +242,18 @@ class Diffusion(BaseModule):
             z, mask, mu = z.float(), mask.float(), mu.float()
             spk = None if spk is None else spk.float()
         with torch.cuda.device(z.device):
+            if lengths is not None:     # checked before any launch or noise draw
+                lengths = check_lengths(lengths, z.shape[0], z.shape[2], z.device, "z")
             if not stoc:
-                out = eng.reverse_diffusion(z, mask, mu, n_timesteps, False, spk, None)
+                out = eng.reverse_diffusion(z, mask, mu, n_timesteps, False, spk, None, lengths)
             else:
-                out = self._stochastic(eng, z, mask, mu, n_timesteps, spk)
+                out = self._stochastic(eng, z, mask, mu, n_timesteps, spk, lengths)
         return out if io_dtype == torch.float32 else out.to(io_dtype)
 
     # bytes of pre-drawn Euler-Maruyama noise resident at once (config 3: N=1000 x B=128 would be 21 GB if materialised)
     noise_window_bytes = 256 << 20
 
-    def _stochastic(self, eng, z, mask, mu, n_timesteps, spk):
+    def _stochastic(self, eng, z, mask, mu, n_timesteps, spk, lengths=None):
         """stoc=True: the reference draws torch.randn(z.shape) once per step, in step order (:267).  The same draws, in the
         same order, are made here a window of steps at a time and streamed through `sbk_reverse_steps`, so the noise
         resident at any moment is bounded by `noise_window_bytes` instead of growing with N."""
@@ -256,16 +261,16 @@ class Diffusion(BaseModule):
         window = max(1, min(n_timesteps, self.noise_window_bytes // per_step))
         draw = lambda n: torch.stack([torch.randn(z.shape, dtype=z.dtype, device=z.device) for _ in range(n)])
         if window >= n_timesteps or len(eng.batch_slices(z.shape[0], z.shape[2])) > 1:
-            return eng.reverse_diffusion(z, mask, mu, n_timesteps, True, spk, draw(n_timesteps))
+            return eng.reverse_diffusion(z, mask, mu, n_timesteps, True, spk, draw(n_timesteps), lengths)
         xt = (z * mask).contiguous()                                                # :256
         for s0 in range(0, n_timesteps, window):
             s1 = min(n_timesteps, s0 + window)
-            eng.reverse_steps(xt, mask, mu, n_timesteps, s0, s1, True, spk, draw(s1 - s0))
+            eng.reverse_steps(xt, mask, mu, n_timesteps, s0, s1, True, spk, draw(s1 - s0), lengths)
         return xt
 
     @torch.no_grad()
-    def forward(self, z, mask, mu, n_timesteps, stoc=False, spk=None):
-        return self.reverse_diffusion(z, mask, mu, n_timesteps, stoc, spk)
+    def forward(self, z, mask, mu, n_timesteps, stoc=False, spk=None, *, lengths=None):
+        return self.reverse_diffusion(z, mask, mu, n_timesteps, stoc, spk, lengths=lengths)
 
     @torch.no_grad()
     def forward_host(self, z, mask, mu, n_timesteps, stoc=False, spk=None):
@@ -313,7 +318,7 @@ def reference_order_noise(B, n_feats, Ty, dtype, device):
 
 @torch.no_grad()
 def synthesize_from_encoder(decoder, mu_x, logw, x_mask, n_timesteps, temperature=1.0, stoc=False, spk=None,
-                            length_scale=1.0, want_attn=True, noise_tf=None):
+                            length_scale=1.0, want_attn=True, noise_tf=None, *, ragged=False):
     """Drop-in for Grad-TTS/model/tts.py:77-99 - everything `GradTTS.forward` does after `self.encoder(...)`:
 
         mu_x, logw, x_mask = self.encoder(x, x_lengths, spk)
@@ -324,7 +329,11 @@ def synthesize_from_encoder(decoder, mu_x, logw, x_mask, n_timesteps, temperatur
     Everything sized [B,Tx,Ty] or [B,F,Ty] - generate_path, the 0/1 matmul, the terminal sample - is one libsbk kernel
     (`sbk_prior_expand`) that writes mu_y / z / y_mask in the layout the sampler reads.  The noise is drawn by torch with
     the reference's own call on a tensor with the reference's strides (`reference_order_noise`), so with the same
-    generator state z equals the reference's z bit for bit.  Returns (encoder_outputs, decoder_outputs, attn) like the reference."""
+    generator state z equals the reference's z bit for bit.  Returns (encoder_outputs, decoder_outputs, attn) like the reference.
+
+    ragged=True samples each utterance on its own fix_len_compatibility(y_lengths[b]) frames (the decoder gets
+    lengths=y_lengths), as the reference's B = 1 call on that utterance would, instead of the padded batch; its frames past
+    them come out 0.  Follow it with the vocoder's `lengths=y_lengths` for per-utterance waveforms."""
     if not mu_x.is_cuda:
         raise RuntimeError("synthesize_from_encoder runs only on a CUDA device (sm_90a); there is no CPU fallback")
     B, Fm, Tx = mu_x.shape
@@ -337,7 +346,10 @@ def synthesize_from_encoder(decoder, mu_x, logw, x_mask, n_timesteps, temperatur
         noise_tf = reference_order_noise(B, Fm, y_max_length_, mu_x.dtype, mu_x.device)  # :94, the reference's draws
     mu_y, z, y_mask, attn = prior_expand(mu_x, w_ceil.reshape(B, Tx), x_mask.reshape(B, Tx).to(torch.float32), y_lengths,
                                          y_max_length_, noise_tf, temperature, want_attn)
-    decoder_outputs = decoder(z, y_mask, mu_y, n_timesteps, stoc, spk)             # :96
+    if ragged:
+        decoder_outputs = decoder(z, y_mask, mu_y, n_timesteps, stoc, spk, lengths=y_lengths)
+    else:
+        decoder_outputs = decoder(z, y_mask, mu_y, n_timesteps, stoc, spk)         # :96
     # (the reference slices attn's dim 2 - the token axis - with the frame count, tts.py:99; kept as is)
     return (mu_y[:, :, :y_max_length], decoder_outputs[:, :, :y_max_length],
             None if attn is None else attn[:, :, :y_max_length])

@@ -35,7 +35,7 @@ import torch
 import torch.nn as nn
 from torch.nn.utils import remove_weight_norm, weight_norm
 
-from .binding import PREC, _check, _check_precision, _NativeHandle, _ptr
+from .binding import PREC, _check, _check_precision, _NativeHandle, _ptr, check_lengths
 
 
 class SbkVocoderConfig(C.Structure):
@@ -147,18 +147,7 @@ class VocoderEngine(_NativeHandle):
 
     def _check_lengths(self, lengths, B, T, device):
         """lengths: int64 [B] on the mel's device, each in 1..T (one device-to-host read of its min and max)"""
-        if not isinstance(lengths, torch.Tensor):
-            raise ValueError(f"lengths: expected an int64 tensor of shape [{B}], got {type(lengths).__name__}")
-        if lengths.dtype != torch.int64:
-            raise ValueError(f"lengths: expected int64, got {lengths.dtype}")
-        if tuple(lengths.shape) != (B,):
-            raise ValueError(f"lengths shape {tuple(lengths.shape)}: expected [{B}] (one length per utterance)")
-        if lengths.device != device:
-            raise ValueError(f"lengths lives on {lengths.device}; it must be on the mel's device {device}")
-        lo, hi = torch.stack(lengths.aminmax()).tolist()
-        if lo < 1 or hi > T:
-            raise ValueError(f"lengths must lie in 1..{T} (the mel's frames), got min {lo}, max {hi}")
-        return lengths.contiguous()
+        return check_lengths(lengths, B, T, device, "mel")
 
     def forward(self, mel, lengths=None):
         """mel [B, num_mels, T] -> wav [B, 1, T*hop]; lengths: optional int64 [B] valid frames per utterance (module
