@@ -29,6 +29,7 @@ import torch.nn.functional as F
 from helpers import nhwc_to_nchw
 from oracle import gradtts_oracle as O
 from oracle.precision_model import round_bf16, round_tf32_rna
+from speech_backbones_b200.gradtts import fix_len_compatibility
 
 # ---- check 1: kappa, from the rounding points of oracle/precision_model.py ----------------------------------------------
 # Operand rounding, relative to |x||w| of one product:
@@ -323,48 +324,140 @@ def _gn_mish(p, blk, raw):
     return O.mish(y), 1.1 * ((raw - mean).abs() * scale.abs() + beta.abs())
 
 
+def ctx_replay(x, wqkv, mode, tc=True):
+    """LinearAttention's context softmax_n(k) v^T over all H*W pixels of x [B,C,H,W] (rezero_linear_attention up to its
+    einsum) -> (ref, A, kappa): ref [B, heads, 32, 32]."""
+    b, c, hh, ww = x.shape
+    K_items = math.ceil(hh * ww / 64)
+    kp = kappa(mode, c, tc=tc)                         # the k | v projection
+    qkv = F.conv2d(x, wqkv).reshape(b, 3, O.HEADS, -1, hh * ww)
+    qkvA = F.conv2d(x.abs(), wqkv.abs()).reshape(b, 3, O.HEADS, -1, hh * ww)
+    k, v, kA, vA = qkv[:, 1], qkv[:, 2], qkvA[:, 1], qkvA[:, 2]
+    pr = k.softmax(dim=-1)
+    ref = torch.einsum("bhdn,bhen->bhde", pr, v)
+    # linearised softmax: dp_n = p_n (dk_n - sum_m p_m dk_m), |dk| <= kappa kA, |dv| <= kappa vA
+    A = (torch.einsum("bhdn,bhen->bhde", pr, vA) + torch.einsum("bhdn,bhen->bhde", pr * kA, v.abs())
+         + (pr * kA).sum(-1)[..., None] * torch.einsum("bhdn,bhen->bhde", pr, v.abs()))
+    # + P and V rounded for the context product (tf32 datapath: 2 x 2^-10; fp32x3: the split, 2^-19; fp32: exact
+    # operands, 64-pixel FFMA chains) + the merge of one partial per 64-pixel item
+    pv = {"tf32": 2 ** -9, "bf16": 2 ** -9, "fp32x3": 2 ** -19, "fp32": 128 * 2 ** -24}[mode]
+    return ref, A, kp + pv + K_items * 2 ** -22 + EPS_NL
+
+
+def crop_utterance(t, b, W):
+    """utterance b of a tensor at a ragged call's dense shape [B, ..., W_dense]: its row, its first W columns"""
+    return t[b:b + 1, ..., :W]
+
+
 class Replay:
     """Run one estimator call with debug capture and judge every captured op against its float64 replay.
 
-    model: "gradtts" (x, mask, mu, t, spk) or "diffvc" (x, mask, mean, t, cond).  `sd` is the state_dict the engine holds."""
+    model: "gradtts" (x, mask, mu, t, spk) or "diffvc" (x, mask, mean, t, cond).  `sd` is the state_dict the engine holds.
 
-    def __init__(self, eng, sd, mode, model, x, mask, mu, t, spk=None, cond=None, dim=64, pe_scale=1000.0, dev="cuda"):
+    `lengths` (Grad-TTS only) makes it a ragged call (`Engine.estimator(..., lengths=)`), in which utterance b is the B = 1
+    call on its own T_b = fix_len_compatibility(lengths[b]) frames.  Each utterance is then judged on its own: the inputs
+    are sliced to row b and [:T_b], every capture is decoded at the call's dense shape and cropped to [b:b+1, ..., :W_b,l]
+    (W_b,l = T_b >> l at level l), and the output to [b, :, :T_b].  The replay judges nothing past an utterance's edge;
+    what the call left there is the caller's to check (e.g. that the output is 0)."""
+
+    def __init__(self, eng, sd, mode, model, x, mask, mu, t, spk=None, cond=None, dim=64, pe_scale=1000.0, dev="cuda",
+                 lengths=None):
         self.eng, self.mode, self.model, self.dev = eng, mode, model, dev
         self.tc = mode != "fp32"
+        self.dim, self.pe_scale = dim, pe_scale
         d = torch.float64
         self.p = {k: v.to(dev, d) for k, v in sd.items()}
+        assert lengths is None or model == "gradtts", "only the Grad-TTS estimator takes lengths"
         eng.debug_capture(True)
         try:
             if model == "diffvc":
                 y = eng.vc_estimator(x.cuda(), mask.cuda(), mu.cuda(), cond.cuda(), t.cuda())
             else:
-                y = eng.estimator(x.cuda(), mask.cuda(), mu.cuda(), t.cuda(), None if spk is None else spk.cuda())
+                L = None if lengths is None else torch.as_tensor(lengths, dtype=torch.int64).cuda()
+                y = eng.estimator(x.cuda(), mask.cuda(), mu.cuda(), t.cuda(), None if spk is None else spk.cuda(),
+                                  lengths=L)
             torch.cuda.synchronize()
         finally:
             eng.debug_capture(False)
-        self.y = y.to(dev, d)
-        self.x, self.mask, self.mu, self.t = (v.to(dev, d) for v in (x, mask, mu, t))
-        self.spk = None if spk is None else spk.to(dev, d)
-        self.cond = None if cond is None else cond.to(dev, d)
+        self.full = {"y": y.to(dev, d), "x": x.to(dev, d), "mask": mask.to(dev, d), "mu": mu.to(dev, d),
+                     "t": t.to(dev, d), "spk": None if spk is None else spk.to(dev, d),
+                     "cond": None if cond is None else cond.to(dev, d)}
         B, H0, T = x.shape
+        self.dense = (B, (H0, H0 // 2, H0 // 4), (T, T // 2, T // 4))
+        # the units judged one by one: the whole call (None), or each utterance (b, T_b) of a ragged one
+        self.utts = [None] if lengths is None else [(b, fix_len_compatibility(int(n))) for b, n in enumerate(lengths)]
+        self.names = eng.debug_names()
+        self.dense_cap = {}                 # captures decoded at the call's shape (fp32, as captured)
+        self.nonfinite = []                 # judged captures (cropped) holding a NaN or Inf
+        self.select(None if lengths is None else self.utts[0])
+
+    def select(self, utt):
+        """Judge `utt` = (b, T_b), utterance b of a ragged call on its own frames, or (None) the whole call."""
+        f, self.utt = self.full, utt
+        if utt is None:
+            row, frames = (lambda v: v), (lambda v: v)
+        else:
+            b, Tb = utt
+            row, frames = (lambda v: v[b:b + 1]), (lambda v: v[b:b + 1, ..., :Tb])
+        self.y, self.x, self.mask, self.mu = (frames(f[k]) for k in ("y", "x", "mask", "mu"))
+        self.t = row(f["t"])
+        self.spk = None if f["spk"] is None else row(f["spk"])
+        self.cond = None if f["cond"] is None else row(f["cond"])
+        B, H0, T = self.x.shape
         self.B, self.Hs, self.Ws = B, (H0, H0 // 2, H0 // 4), (T, T // 2, T // 4)
         m = self.mask[:, None]
         self.masks = [m, m[..., ::2], m[..., ::4]]
         # the time embedding: GradLogPEstimator2d.forward's first lines (oracle estimator / diffvc conditioning)
         p = self.p
-        temb = O.sinusoid(self.t, dim, pe_scale)
+        temb = O.sinusoid(self.t, self.dim, self.pe_scale)
         temb = F.linear(temb, p["estimator.mlp.0.weight"], p["estimator.mlp.0.bias"])
         self.temb = F.linear(O.mish(temb), p["estimator.mlp.2.weight"], p["estimator.mlp.2.bias"])
-        self.names = eng.debug_names()
         self.cap = {}
+        self.tag = "" if utt is None else f" b={utt[0]} W=({self.Ws[0]},{self.Ws[1]},{self.Ws[2]})"
+
+    def crop(self, t, lvl):
+        """a tensor at the call's shape [B, C, H, W_l] -> the selected unit's part of it"""
+        return t if self.utt is None else crop_utterance(t, self.utt[0], self.Ws[lvl])
 
     def got(self, name, C, lvl):
         if name not in self.cap:
-            flat = self.eng.debug_read(name)
-            assert flat is not None, f"{name}: the plan names it but captured nothing"
-            self.cap[name] = nhwc_to_nchw(flat, self.B, self.Hs[lvl], self.Ws[lvl], C,
-                                          self.eng.debug_layout(name)).to(self.dev, torch.float64)
+            if name not in self.dense_cap:
+                flat = self.eng.debug_read(name)
+                assert flat is not None, f"{name}: the plan names it but captured nothing"
+                B, Hs, Ws = self.dense
+                self.dense_cap[name] = nhwc_to_nchw(flat, B, Hs[lvl], Ws[lvl], C,
+                                                    self.eng.debug_layout(name)).to(self.dev)
+            self.cap[name] = self.crop(self.dense_cap[name], lvl).to(torch.float64)
         return self.cap[name]
+
+    def got_ctx(self, q):
+        """the captured LinearAttention context [B, heads, 32, 32] of attention `q`, the selected unit's rows"""
+        name = f"{q}.ctx"
+        if name not in self.dense_cap:
+            self.dense_cap[name] = self.eng.debug_read(name).view(self.dense[0], O.HEADS, 32, 32).to(self.dev)
+        t = self.dense_cap[name]
+        return (t if self.utt is None else t[self.utt[0]:self.utt[0] + 1]).to(torch.float64)
+
+    def judged_names(self):
+        """the captured ops run() replays (all but SKIP's, and the output, which the call returns)"""
+        return [n for n in self.names if skip_reason(n) is None and n != "estimator.out"]
+
+    def hold(self):
+        """read every judged capture now: the engine keeps only its last call's, which a later call replaces"""
+        utt = self.utt
+        for n in self.judged_names():
+            self.capture(n)
+        self.select(utt)
+        return self
+
+    def capture(self, name):
+        """the selected unit's capture of a replayed op `name` ([B, C, H, W_l]; a context [B, heads, 32, 32])"""
+        if name.endswith(".ctx"):
+            return self.got_ctx(name[:-len(".ctx")])
+        if name == "estimator.final_block.raw":
+            return self.got(name, self.p["estimator.final_block.block.0.weight"].shape[0], 0)
+        key = name.replace(".block1.raw", ".out").replace(".block2.raw", ".out")
+        return self.got(name, self._chan(key), self._level_of(key))
 
     def _chan(self, name):
         """channels of a captured resnet / attention / resample output"""
@@ -465,25 +558,12 @@ class Replay:
         x = self.captured(src)
         b, c, hh, ww = x.shape
         wqkv = p[f"{q}.fn.fn.to_qkv.weight"]
-        K_items = math.ceil(hh * ww / 64)
-        kp = kappa(mode, c, tc=self.tc)                    # the k | v projection
         if part == "ctx":
-            qkv = F.conv2d(x, wqkv).reshape(b, 3, O.HEADS, -1, hh * ww)
-            qkvA = F.conv2d(x.abs(), wqkv.abs()).reshape(b, 3, O.HEADS, -1, hh * ww)
-            k, v, kA, vA = qkv[:, 1], qkv[:, 2], qkvA[:, 1], qkvA[:, 2]
-            pr = k.softmax(dim=-1)
-            ref = torch.einsum("bhdn,bhen->bhde", pr, v)
-            # linearised softmax: dp_n = p_n (dk_n - sum_m p_m dk_m), |dk| <= kappa kA, |dv| <= kappa vA
-            A = (torch.einsum("bhdn,bhen->bhde", pr, vA) + torch.einsum("bhdn,bhen->bhde", pr * kA, v.abs())
-                 + (pr * kA).sum(-1)[..., None] * torch.einsum("bhdn,bhen->bhde", pr, v.abs()))
-            # + P and V rounded for the context product (tf32 datapath: 2 x 2^-10; fp32x3: the split, 2^-19; fp32: exact
-            # operands, 64-pixel FFMA chains) + the merge of one partial per 64-pixel item
-            pv = {"tf32": 2 ** -9, "bf16": 2 ** -9, "fp32x3": 2 ** -19, "fp32": 128 * 2 ** -24}[mode]
-            k_ctx = kp + pv + K_items * 2 ** -22 + EPS_NL
-            got = self.eng.debug_read(f"{q}.ctx").view(ref.shape).to(self.dev, torch.float64)
+            ref, A, k_ctx = ctx_replay(x, wqkv, mode, self.tc)
+            got = self.got_ctx(q)
             return got, ref, A, k_ctx, 0.0, False          # [B, heads, 32, 32]: no columns or rows to group
         # part == "out": g * to_out(ctx^T q) + x from the captured ctx
-        ctx = self.eng.debug_read(f"{q}.ctx").view(b, O.HEADS, 32, 32).to(self.dev, torch.float64)
+        ctx = self.got_ctx(q)
         wq = wqkv[:O.HEADS * 32]
         g, wo, bo = p[f"{q}.fn.g"], p[f"{q}.fn.fn.to_out.weight"], p[f"{q}.fn.fn.to_out.bias"]
         qq = F.conv2d(x, wq).reshape(b, O.HEADS, -1, hh * ww)
@@ -533,34 +613,40 @@ class Replay:
         return self.y[:, None], ref * m, A * m, kappa(mode, C, tc=False, nl=True), floor, Alin * m
 
     def run(self):
-        """-> rows (name, elem, unif, where); raises on an op that is neither replayed nor in SKIP."""
+        """-> rows (name, elem, unif, where), per judged unit (the call, or each utterance: its name carries b and the
+        utterance's level widths); raises on an op that is neither replayed nor in SKIP."""
         rows = []
-        for name in self.names:
-            why = skip_reason(name)
-            if why is not None:
-                continue
-            assert name.startswith("estimator."), f"unknown op '{name}': add a replay for it or a reason to SKIP"
-            short = name[len("estimator."):]
-            pre, _, part = short.partition(".block")
-            if short in ("final_block.raw", "out"):
-                r = self.final_ops(name)
-            elif part in ("1.raw", "2.raw") and pre in RESNETS:
-                r = self.resnet_op(pre, "block" + part)
-            else:
-                pre, part = short.rsplit(".", 1)
-                if pre in RESNETS and part == "out":
-                    r = self.resnet_op(pre, "out")
-                elif pre in ATTNS and part in ("ctx", "out"):
-                    r = self.attn_op(pre, part)
-                elif pre in RESAMPLES and part == "out":
-                    r = self.resample_op(pre)
+        for utt in self.utts:
+            self.select(utt)
+            n0 = len(rows)
+            for name in self.names:
+                why = skip_reason(name)
+                if why is not None:
+                    continue
+                assert name.startswith("estimator."), f"unknown op '{name}': add a replay for it or a reason to SKIP"
+                short = name[len("estimator."):]
+                pre, _, part = short.partition(".block")
+                if short in ("final_block.raw", "out"):
+                    r = self.final_ops(name)
+                elif part in ("1.raw", "2.raw") and pre in RESNETS:
+                    r = self.resnet_op(pre, "block" + part)
                 else:
-                    raise AssertionError(f"unknown op '{name}': add a replay for it or a reason to SKIP")
-            got, ref, A, k, floor, Alin = r
-            assert got.shape == ref.shape, f"{name}: captured {tuple(got.shape)} vs replay {tuple(ref.shape)}"
-            elem, unif, where = check(got, ref, A, k, floor, Alin, groups=Alin is not False)
-            rows.append((name, elem, unif, where))
-        assert any(r[0] == "estimator.out" for r in rows), "the plan no longer names estimator.out"
+                    pre, part = short.rsplit(".", 1)
+                    if pre in RESNETS and part == "out":
+                        r = self.resnet_op(pre, "out")
+                    elif pre in ATTNS and part in ("ctx", "out"):
+                        r = self.attn_op(pre, part)
+                    elif pre in RESAMPLES and part == "out":
+                        r = self.resample_op(pre)
+                    else:
+                        raise AssertionError(f"unknown op '{name}': add a replay for it or a reason to SKIP")
+                got, ref, A, k, floor, Alin = r
+                assert got.shape == ref.shape, f"{name}: captured {tuple(got.shape)} vs replay {tuple(ref.shape)}"
+                if not bool(torch.isfinite(got).all()):
+                    self.nonfinite.append(name + self.tag)
+                elem, unif, where = check(got, ref, A, k, floor, Alin, groups=Alin is not False)
+                rows.append((name + self.tag, elem, unif, where))
+            assert any(r[0] == "estimator.out" + self.tag for r in rows[n0:]), "the plan no longer names estimator.out"
         return rows
 
 

@@ -11,6 +11,7 @@ import torch
 from helpers import rel_l2
 from op_replay import MIN_GROUP, R_UNIFORM, Replay, ntile_widths, uniformity
 from speech_backbones_b200 import UNetConfig, synthetic_inputs, synthetic_state_dict
+from speech_backbones_b200.gradtts import fix_len_compatibility
 
 pytestmark = pytest.mark.gpu
 MODES = ["fp32", "fp32x3", "tf32", "bf16"]
@@ -23,6 +24,17 @@ GRADTTS_CASES = [
     (2, 260, [260, 131], 4),            # multi-speaker first Block (3 planar input channels)
 ]
 DIFFVC_CASES = [(1, 260), (2, 132)]     # DiffVC U-Net, dim 256, ragged masks
+# Ragged calls (Engine.estimator(..., lengths=)): (B, T, lengths, n_spks), utterance b on T_b = fix_len_compatibility(
+# lengths[b]) frames, i.e. level widths T_b, T_b/2, T_b/4.
+RAGGED_CASES = [
+    # T_b = 4, 516, 128, 132, 256, 260, 508, 388, 4.  The dense grid ends in a partial tile at every level (516 / 258 / 129),
+    # and at level 2 (W = 129) the 1x1 tiles straddle image rows at every phase.  Edges fall on a tile seam (128, 256 / 128),
+    # 4 columns past one (132, 260 / 130), one short of one at every level (508 / 254 / 127) and at level-2 widths 1, 33,
+    # 65, 97; a 4-frame utterance is first and last in the batch; frames [lengths, T_b) are masked inside an utterance.
+    (9, 516, [1, 516, 128, 129, 253, 257, 505, 385, 2], 1),
+    # the multi-speaker planar first Block (3 input planes); an utterance narrower than one tile at every level (64/32/16)
+    (3, 512, [64, 512, 301], 4),
+]
 
 
 def _mask(B, T, lengths):
@@ -54,12 +66,23 @@ def engines(sbk_lib):
         e.close()
 
 
-def _report_and_assert(tag, rows):
-    for name, elem, unif, where in rows:
-        print(f"{tag} {name:44s} |err|/(kA) {elem:.3e}  max/median {unif:6.2f} {where}")
+def _print_worst(tag, rows):
     we = max(rows, key=lambda r: r[1])
     wu = max(rows, key=lambda r: r[2])
     print(f"WORST {tag}: |err|/(kA) {we[1]:.3e} ({we[0]})  max/median {wu[2]:.2f} ({wu[0]} {wu[3]})")
+
+
+def _report_and_assert(tag, rows):
+    for name, elem, unif, where in rows:
+        print(f"{tag} {name:44s} |err|/(kA) {elem:.3e}  max/median {unif:6.2f} {where}")
+    # a ragged call's rows carry their utterance (" b=.. W=(..)", Replay.tag): one WORST line per utterance, then the call's
+    utts = {}
+    for r in rows:
+        if " b=" in r[0]:
+            utts.setdefault(r[0][r[0].index(" b="):], []).append(r)
+    for utt, urows in utts.items():
+        _print_worst(tag + utt, urows)
+    _print_worst(tag, rows)
     bad = [r for r in rows if not (r[1] <= 1.0 and r[2] <= R_UNIFORM)]
     assert not bad, "ops out of bounds: " + ", ".join(f"{n} ({e:.3g}, {u:.3g} {w})" for n, e, u, w in bad)
 
@@ -74,6 +97,53 @@ def test_gradtts_ops_in_isolation(engines, precision, B, T, lengths, n_spks):
     rows = Replay(eng, sd, precision, "gradtts", z * mask, mask, mu, t, spk=spk, dim=cfg.dim,
                   pe_scale=cfg.pe_scale).run()
     _report_and_assert(f"gradtts {precision} B={B} T={T} spk={n_spks}", rows)
+
+
+def _poison_plan(eng, B, T, t, spk):
+    """A dense call at (B, T) on z = mu = NaN (t finite, mask all ones), capture on: every buffer a captured op writes in
+    this plan's workspace - which later calls at (B, T) reuse, never cleared - then holds NaN.  Returns the names whose
+    capture is not all NaN (there should be none)."""
+    nan = torch.full((B, 80, T), float("nan"), device="cuda")
+    eng.debug_capture(True)
+    try:
+        eng.estimator(nan, torch.ones(B, 1, T, device="cuda"), nan, t.cuda(), None if spk is None else spk.cuda())
+        torch.cuda.synchronize()
+        left = []
+        for name in eng.debug_names():
+            v = eng.debug_read(name)
+            if v is not None and not bool(torch.isnan(v).all()):
+                left.append(f"{name} ({int((~torch.isnan(v)).sum())} of {v.numel()} not NaN)")
+        return left
+    finally:
+        eng.debug_capture(False)
+
+
+@pytest.mark.parametrize("precision", MODES)
+@pytest.mark.parametrize("B,T,lengths,n_spks", RAGGED_CASES, ids=[f"B{c[0]}-T{c[1]}-spk{c[3]}" for c in RAGGED_CASES])
+def test_gradtts_ragged_ops_in_isolation(engines, precision, B, T, lengths, n_spks):
+    """Every op of a ragged call, per utterance, on that utterance's own frames against its float64 replay, after a dense
+    NaN call at the same (B, T) has filled the workspace with NaN.  A ragged kernel must not read anything at or past an
+    utterance's edge (T_b >> level): inputs there are NaN too, so a load instead of a zero fill, or a mask applied by
+    multiplication (NaN * 0 = NaN) instead of by selection, puts a NaN into the utterance's own columns."""
+    eng, cfg, sd = engines("gradtts", precision, n_spks)
+    z, _, mu, spk, _ = synthetic_inputs(B, T, n_spks=n_spks)
+    t = torch.linspace(0.9, 0.2, B)
+    left = _poison_plan(eng, B, T, t, spk)
+    assert not left, "captures not poisoned by the NaN call: " + ", ".join(left)
+    L = torch.tensor(lengths)
+    TB = torch.tensor([fix_len_compatibility(n) for n in lengths])
+    frames = torch.arange(T)[None, :]
+    past = (frames >= TB[:, None])[:, None]                                   # [B, 1, T]
+    mask = torch.where(past, float("nan"), (frames < L[:, None]).float()[:, None])
+    x = torch.where(past, float("nan"), z * mask)
+    mu = torch.where(past, float("nan"), mu)
+    rp = Replay(eng, sd, precision, "gradtts", x, mask, mu, t, spk=spk, dim=cfg.dim, pe_scale=cfg.pe_scale,
+                lengths=lengths)
+    rows = rp.run()
+    assert not rp.nonfinite, "NaN / Inf inside an utterance: " + ", ".join(rp.nonfinite)
+    for b, Tb in enumerate(TB.tolist()):
+        assert torch.count_nonzero(rp.full["y"][b, :, Tb:]) == 0, f"utterance {b}: output not 0 past T_b = {Tb}"
+    _report_and_assert(f"gradtts ragged {precision} B={B} T={T} spk={n_spks}", rows)
 
 
 @pytest.mark.parametrize("precision", MODES)
@@ -103,6 +173,17 @@ def test_conv3x3_runs_both_ntile_widths():
         for B, T, _, _ in GRADTTS_CASES:
             widths |= ntile_widths(sd, B, 80, T, sms)
         assert widths == {64, 128}, f"{precision}: N-tile widths {widths} on {sms} SMs"
+
+
+def test_ragged_cases_run_both_ntile_widths():
+    """The same for the ragged cases: the planner sizes a ragged call's tiles from its dense (B, T), so across them the
+    64-channel level-0 convs run 64-wide N tiles and the others 128-wide ones."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    sd = synthetic_state_dict(UNetConfig(), 1234)
+    widths = set()
+    for B, T, _, _ in RAGGED_CASES:
+        widths |= ntile_widths(sd, B, 80, T, sms)
+    assert widths == {64, 128}, f"N-tile widths {widths} on {sms} SMs"
 
 
 # ---- PostNet: the dims its handle accepts, both precisions, against the float64 oracle ----------------------------------

@@ -9,7 +9,9 @@ import torch
 import torch.nn.functional as F
 
 from helpers import rel_l2
-from op_replay import FIRST_CONV_TILE, FLOOR_PER_W, R_UNIFORM, TC_TILE, check, ct_fold, kappa, passes, rb_act, rb_conv
+from op_replay import (FIRST_CONV_TILE, FLOOR_PER_W, R_UNIFORM, TC_TILE, _gn_mish, check, crop_utterance, ct_fold, ctx_replay,
+                       kappa, passes, rb_act, rb_conv)
+from oracle import gradtts_oracle as O
 from oracle.precision_model import fp32x3_product, round_bf16, round_tf32_rna, trunc_tf32
 
 B, CIN, COUT, H, W = 1, 64, 128, 6, 260
@@ -369,3 +371,193 @@ def test_refblock_stale_halo_at_first_conv_seam_fails(rb_stage):
     elem, unif, where = rb_conv(s["xt"], s["mask"], s["w1"], s["b1"], raw, "tf32", first=True)
     print(f"refblock stale first-conv halo: |err|/(kappa A) max {elem:.3g}, uniformity {unif:.3g} at {where}")
     assert elem > 10 and unif > R_UNIFORM and not passes(elem, unif)
+
+
+# ---- ragged batches: two utterances of different widths on one dense image, each judged on its own columns ----------------
+# A ragged call computes utterance b on its own W_b columns of the dense image (W_b = T_b >> level) and the checker crops
+# every capture to [b:b+1, ..., :W_b] (op_replay.Replay with lengths).  Utterance 0 fills the dense width (260: tiles
+# 128 | 128 | 4), utterance 1 ends 4 columns past a tile seam (132); past W_b the dense image holds stale values.
+RW = (W, 132)
+
+
+@pytest.fixture(scope="module")
+def ragged():
+    g = torch.Generator().manual_seed(19)
+    x = torch.randn(2, CIN, H, W, generator=g)
+    w = (torch.rand(COUT, CIN, 3, 3, generator=g) * 2 - 1) / (CIN * 9) ** 0.5
+    b = (torch.rand(COUT, generator=g) * 2 - 1) / (CIN * 9) ** 0.5
+    return x, w, b
+
+
+def _per_utterance(y, judge):
+    """judge(b, y cropped to utterance b) -> (elem, unif, where) for each utterance"""
+    return [judge(u, crop_utterance(y, u, RW[u])) for u in range(2)]
+
+
+def _judge_conv_utt(x, w, b, mode):
+    def judge(u, got):
+        xu = crop_utterance(x, u, RW[u]).double()
+        ref, A = F.conv2d(xu, w.double(), b.double(), padding=1), F.conv2d(xu.abs(), w.abs().double(), b.abs().double(), padding=1)
+        return _judge(got, ref, A, mode, w)
+    return judge
+
+
+def ragged_conv(x, w, b, mode, stale_edge=False):
+    """the ragged 3x3 conv: each utterance's output from its own columns, zero padding at its edge; NaN past it.
+    stale_edge: utterance 1's last column reads its right halo (dense column W_1) from the image instead of as zero."""
+    y = torch.full((2, COUT, H, W), float("nan"), dtype=torch.float64)
+    for u in range(2):
+        y[u:u + 1, ..., :RW[u]] = emulate(crop_utterance(x, u, RW[u]), w, b, mode)
+    if stale_edge:
+        e = RW[1] - 1
+        y[1:2, ..., e] = emulate(crop_utterance(x, 1, RW[1] + 1), w, b, mode)[..., e]
+    return y
+
+
+@pytest.mark.parametrize("mode", MODES)
+def test_ragged_conv_clean_passes(ragged, mode):
+    x, w, b = ragged
+    for u, (elem, unif, where) in enumerate(_per_utterance(ragged_conv(x, w, b, mode), _judge_conv_utt(x, w, b, mode))):
+        print(f"{mode} ragged conv clean b={u} W={RW[u]}: |err|/(kappa A) max {elem:.3f}, uniformity {unif:.2f} at {where}")
+        assert passes(elem, unif), (u, elem, unif, where)
+
+
+@pytest.mark.parametrize("mode", MODES)
+def test_ragged_stale_edge_column_fails(ragged, mode):
+    """(a) utterance 1's edge column reads the next column of the dense image instead of zero.  The column is the
+    utterance's image border, which check 2 leaves out (op_replay.R_UNIFORM): check 1 alone catches it, by 121x (tf32),
+    23x (bf16) and 1.2e4x (fp32x3), while the uniformity ratio stays ~1.1."""
+    x, w, b = ragged
+    rows = _per_utterance(ragged_conv(x, w, b, mode, stale_edge=True), _judge_conv_utt(x, w, b, mode))
+    elem, unif, where = rows[1]
+    print(f"{mode} ragged stale edge column b=1 W={RW[1]}: |err|/(kappa A) max {elem:.3g}, uniformity {unif:.3g} at {where}")
+    assert passes(*rows[0][:2]) and elem > 10 and not passes(elem, unif)
+
+
+# (b) GroupNorm + Mish of one Block (the captured raw conv output -> Mish(GN(raw)) * mask), as k_gn_act computes it: the
+# group statistics over the utterance's own H x W_b pixels, mean and rstd * gamma rounded to fp32, the rest in fp32, the
+# output stored as the mode stores it.  The defect divides the utterance's sums by the dense count C/G * H * W.
+def ragged_gn_mish(raw, gamma, beta, mode, dense_count=False):
+    y = torch.full_like(raw, float("nan"))
+    for u in range(2):
+        r = crop_utterance(raw, u, RW[u]).contiguous()
+        B_, C_, H_, W_ = r.shape
+        g = r.view(1, O.GROUPS, -1)
+        n = (C_ // O.GROUPS) * H_ * (W if dense_count else W_)
+        mean = g.sum(-1) / n
+        var = ((g * g).sum(-1) / n - mean * mean).clamp_min(0.0)
+        cpg = C_ // O.GROUPS
+        mean_f = mean.float().repeat_interleave(cpg, 1)[:, :, None, None]
+        scale = ((1.0 / torch.sqrt(var + 1e-5)).float().repeat_interleave(cpg, 1) * gamma.float()[None])[:, :, None, None]
+        h = F.mish((r.float() - mean_f) * scale + beta.float()[None, :, None, None])
+        y[u:u + 1, ..., :RW[u]] = (round_bf16(h) if mode == "bf16" else h).double()
+    return y
+
+
+@pytest.fixture(scope="module")
+def ragged_gn(ragged):
+    x, w, b = ragged
+    g = torch.Generator().manual_seed(23)
+    raw = torch.cat([emulate(crop_utterance(x, u, W), w, b, "tf32") for u in range(2)], 0)
+    gamma, beta = 1 + 0.1 * torch.randn(COUT, generator=g), 0.1 * torch.randn(COUT, generator=g)
+    return raw, gamma, beta
+
+
+def _judge_gn_utt(raw, gamma, beta, mode):
+    p = {"blk.block.1.weight": gamma.double(), "blk.block.1.bias": beta.double()}
+
+    def judge(u, got):
+        ref, A = _gn_mish(p, "blk", crop_utterance(raw, u, RW[u]).contiguous())
+        return check(got, ref, A, kappa(mode, 1, tc=False, nl=True, store_bf16=mode == "bf16"))
+    return judge
+
+
+@pytest.mark.parametrize("mode", MODES)
+def test_ragged_group_norm_clean_passes(ragged_gn, mode):
+    raw, gamma, beta = ragged_gn
+    rows = _per_utterance(ragged_gn_mish(raw, gamma, beta, mode), _judge_gn_utt(raw, gamma, beta, mode))
+    for u, (elem, unif, where) in enumerate(rows):
+        print(f"{mode} ragged GN clean b={u} W={RW[u]}: |err|/(kappa A) max {elem:.3f}, uniformity {unif:.2f} at {where}")
+        assert passes(elem, unif), (u, elem, unif, where)
+
+
+@pytest.mark.parametrize("mode", MODES)
+def test_ragged_group_norm_dense_count_fails(ragged_gn, mode):
+    """(b) the GroupNorm count of utterance 1 from the dense W instead of W_b: its mean and variance shrink by ~W_b / W,
+    which check 1 sees at every element: it fails by 9.9e4x (tf32, fp32x3) and 195x (bf16)."""
+    raw, gamma, beta = ragged_gn
+    rows = _per_utterance(ragged_gn_mish(raw, gamma, beta, mode, dense_count=True), _judge_gn_utt(raw, gamma, beta, mode))
+    elem, unif, where = rows[1]
+    print(f"{mode} ragged GN dense count b=1 W={RW[1]}: |err|/(kappa A) max {elem:.3g}, uniformity {unif:.3g} at {where}")
+    assert passes(*rows[0][:2]) and elem > 10 and not passes(elem, unif)
+
+
+# (c) LinearAttention's context over an utterance's own H x W_b pixels (k_attn_ctx): k | v projected with the mode's operand
+# rounding and stored fp32, softmax over the pixels in fp32, P and V rounded for the context product (tf32 datapath in the
+# tf32 and bf16 modes), the result stored fp32.  The defect lets the padded pixels of the dense image into the softmax as
+# k = 0, v = 0: the numerators keep their value, the denominators grow by n_pad * exp(-max k).  It is visible only where
+# exp(-max k) is not negligible against the sum over the valid pixels, i.e. while k stays O(1): here x ~ N(0.5, 1), so k
+# is O(1) and v has a mean that the context keeps (for zero-mean v the context is a cancelling sum and the defect smaller).
+ATT_C, ATT_H = 64, 4
+
+
+@pytest.fixture(scope="module")
+def ragged_attn():
+    g = torch.Generator().manual_seed(29)
+    x = torch.randn(2, ATT_C, ATT_H, W, generator=g) + 0.5
+    wqkv = torch.randn(3 * O.HEADS * 32, ATT_C, 1, 1, generator=g) / ATT_C ** 0.5
+    return x, wqkv
+
+
+def ragged_ctx(x, wqkv, mode, pad_in_softmax=False):
+    out = []
+    for u in range(2):
+        xu = crop_utterance(x, u, W if pad_in_softmax else RW[u]).clone()
+        if mode == "fp32x3":
+            kv = fp32x3_product(F.conv2d, xu, wqkv, 1, 0)
+        else:
+            xq, wq = (trunc_tf32(xu), round_tf32_rna(wqkv)) if mode == "tf32" else (round_bf16(xu), round_bf16(wqkv))
+            kv = F.conv2d(xq.double(), wq.double())
+        kv = kv.float().reshape(1, 3, O.HEADS, 32, -1)
+        k, v = kv[:, 1], kv[:, 2]
+        if pad_in_softmax:                  # the pixels at columns >= W_b of every row enter as k = 0, v = 0
+            k, v = k.clone(), v.clone()
+            k.view(1, O.HEADS, 32, ATT_H, W)[..., RW[u]:] = 0
+            v.view(1, O.HEADS, 32, ATT_H, W)[..., RW[u]:] = 0
+        pr = k.softmax(-1)
+        if mode != "fp32x3":
+            pr, v = round_tf32_rna(pr), round_tf32_rna(v)
+        out.append(torch.einsum("bhdn,bhen->bhde", pr.double(), v.double()).float().double())
+    return out
+
+
+def _judge_ctx(x, wqkv, mode, got):
+    rows = []
+    for u in range(2):
+        ref, A, k = ctx_replay(crop_utterance(x, u, RW[u]).double(), wqkv.double(), mode)
+        rows.append(check(got[u], ref, A, k, groups=False))
+    return rows
+
+
+@pytest.mark.parametrize("mode", MODES)
+def test_ragged_attention_context_clean_passes(ragged_attn, mode):
+    x, wqkv = ragged_attn
+    for u, (elem, unif, where) in enumerate(_judge_ctx(x, wqkv, mode, ragged_ctx(x, wqkv, mode))):
+        print(f"{mode} ragged ctx clean b={u} W={RW[u]}: |err|/(kappa A) max {elem:.3f}")
+        assert passes(elem, unif), (u, elem)
+
+
+@pytest.mark.parametrize("mode", MODES)
+def test_ragged_attention_padded_pixels_in_softmax_fail(ragged_attn, mode):
+    """(c) utterance 1's context with its padded pixels (columns 132..259 of each of the 4 rows: 512 pixels, against
+    528 valid ones) in the softmax as k = 0, v = 0.  It fails check 1 by 12.8x (tf32), 4.47x (bf16) and 2.5e3x
+    (fp32x3).  The margin shrinks as the keys grow against 0: shifting every k by +c scales the padded pixels' share of
+    the denominators by exp(-c), and at c ~ 2.5 bf16's bound (~ 2^-7) no longer separates the defect from rounding
+    (float64 estimate: 2.75x at c = 1, 1.35x at c = 2, 0.56x at c = 3).  There the bitwise per-op comparison of a ragged
+    call with its B = 1 calls in tf32 and bf16 (test_ragged_decoder_gpu.py) still sees it; fp32x3's bound is ~500x
+    tighter than bf16's."""
+    x, wqkv = ragged_attn
+    rows = _judge_ctx(x, wqkv, mode, ragged_ctx(x, wqkv, mode, pad_in_softmax=True))
+    elem, unif, where = rows[1]
+    print(f"{mode} ragged ctx padded pixels in softmax b=1 W={RW[1]}: |err|/(kappa A) max {elem:.3g}")
+    assert passes(*rows[0][:2]) and elem > 2 and not passes(elem, unif)

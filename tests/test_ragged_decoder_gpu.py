@@ -14,6 +14,7 @@ import pytest
 import torch
 
 from helpers import rel_l2
+from op_replay import Replay
 from speech_backbones_b200 import UNetConfig, synthetic_inputs, synthetic_noise, synthetic_state_dict
 from speech_backbones_b200.gradtts import fix_len_compatibility
 
@@ -231,3 +232,74 @@ def test_rows_match_the_reference_golden(engines, ref_golden, precision):
             print(precision, c["kind"], c.get("N"), c.get("stoc"), c["n_spks"], "utterance", b, "rel-L2", err)
             assert err <= tol, (precision, c, b, err)
             assert torch.count_nonzero(y[b, :, Tb:]) == 0
+
+
+# ---- a batch at the tile edges, with NaN wherever the call must not read ----------------------------------------------------
+# B = 9, T = 516 (test_op_isolation_gpu.py's first ragged case): T_b = 4, 516, 128, 132, 256, 260, 508, 388, 4 - the dense
+# grid ends in a partial tile at every level, edges on, past and short of tile seams, 4-frame utterances first and last.
+NB, NT = 9, 516
+NLENGTHS = [1, 516, 128, 129, 253, 257, 505, 385, 2]
+NTB = [fix_len_compatibility(n) for n in NLENGTHS]
+
+
+def _nan_past_edges(v, lengths=NLENGTHS):
+    """v [..., B, C, T] with NaN at every frame >= T_b of row b"""
+    TB = torch.tensor([fix_len_compatibility(n) for n in lengths], device=v.device)
+    past = torch.arange(v.shape[-1], device=v.device)[None, :] >= TB[:, None]
+    return torch.where(past[:, None], float("nan"), v)
+
+
+def _nan_inputs():
+    """(z, mask, mu, L): mask 1 below lengths[b], 0 on [lengths[b], T_b); z, mask and mu NaN from T_b on"""
+    z, _, mu, _, _ = synthetic_inputs(NB, NT)
+    L = torch.tensor(NLENGTHS, dtype=torch.int64)
+    mask = (torch.arange(NT)[None, :] < L[:, None]).to(torch.float32)[:, None, :]
+    return (_nan_past_edges(z).cuda(), _nan_past_edges(mask).cuda(), _nan_past_edges(mu).cuda(), L.cuda())
+
+
+@pytest.mark.parametrize("precision", ("tf32", "bf16"))
+def test_every_captured_op_equals_the_single_call(engines, precision):
+    """The ops of a ragged call, each cropped to utterance b's widths (T_b >> level), equal the captures of the engine's own
+    B = 1 call on [:T_b] bit for bit: a divergence is placed at the first op where it appears, not in the final mel."""
+    eng = engines(precision)
+    sd = synthetic_state_dict(UNetConfig())
+    z, mask, mu, L = _nan_inputs()
+    t = torch.linspace(0.9, 0.1, NB)
+    x = z * mask
+    rp = Replay(eng, sd, precision, "gradtts", x, mask, mu, t, lengths=NLENGTHS).hold()
+    judged = rp.judged_names()
+    for b, Tb in enumerate(NTB):
+        one = Replay(eng, sd, precision, "gradtts", _sl(x, b, Tb), _sl(mask, b, Tb), _sl(mu, b, Tb), t[b:b + 1])
+        assert one.names == rp.names, b
+        rp.select((b, Tb))
+        for n in judged:
+            got, want = rp.capture(n), one.capture(n)
+            assert got.shape == want.shape, (n, b, tuple(got.shape), tuple(want.shape))
+            assert torch.equal(got, want), f"{n}{rp.tag}: differs from the B = 1 call, max |diff| " \
+                                           f"{(got - want).abs().nan_to_num(float('inf')).max().item():.3g}"
+        assert torch.equal(rp.y, one.y), b
+
+
+@pytest.mark.parametrize("stoc", [False, True], ids=["det", "stoc"])
+@pytest.mark.parametrize("precision", MODES)
+def test_poisoned_loop_rows_equal_single_calls(engines, precision, stoc):
+    """reverse_diffusion (N = 3) on a batch whose inputs - and, stochastic, noise - are NaN past every T_b, right after a
+    dense NaN loop of the same kind at the same (B, T, N) has left NaN in the plan's buffers and in the graph's.  Every row
+    is finite and equals its single call, and is 0 past T_b."""
+    eng = engines(precision)
+    z, mask, mu, L = _nan_inputs()
+    noise = _nan_past_edges(synthetic_noise(3, NB, NT)).cuda() if stoc else None
+    # the single calls first: each builds a plan of its own shape, which would replace the poisoned one
+    single = [eng.reverse_diffusion(_sl(z, b, Tb), _sl(mask, b, Tb), _sl(mu, b, Tb), 3, stoc, None,
+                                    noise[:, b:b + 1, :, :Tb].contiguous() if stoc else None).cpu()
+              for b, Tb in enumerate(NTB)]
+    nan = torch.full_like(z, float("nan"))
+    dense = eng.reverse_diffusion(nan, torch.ones_like(mask), nan, 3, stoc, None, torch.full_like(noise, float("nan"))
+                                  if stoc else None)
+    assert bool(torch.isnan(dense).all())
+    out = eng.reverse_diffusion(z, mask, mu, 3, stoc, None, noise, lengths=L).cpu()
+    for b, Tb in enumerate(NTB):
+        row = out[b:b + 1, :, :Tb]
+        assert bool(torch.isfinite(row).all()), (precision, b, Tb)
+        assert _same(precision, row, single[b]), (precision, b, Tb, rel_l2(row, single[b]))
+        assert torch.count_nonzero(out[b, :, Tb:]) == 0, (precision, b)

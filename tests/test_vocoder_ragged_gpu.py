@@ -127,6 +127,24 @@ def test_debug_captures_valid_region_equals_single_calls(gens, mel, lengths, cfg
 
 @pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("cfg", sorted(CONFIGS))
+def test_poisoned_workspace_rows_equal_single_calls(gens, mel, lengths, cfg, mode):
+    """The ragged call right after a dense NaN-mel call at the same (B, T) - which leaves NaN in every workspace buffer the
+    next call at that shape reuses - on mel frames that are NaN past each lengths[b]: each waveform still equals its
+    single call bit for bit, and the rest of its row is 0.  A kernel that read a frame past an utterance's edge, or masked
+    one by multiplying it by 0, would carry the NaN into the utterance's samples."""
+    g, hop = gens(cfg, mode), _hop(CONFIGS[cfg])
+    # the single calls first: each plans its own shape, which would replace the poisoned workspace
+    single = [g(mel[b:b + 1, :, :n].cuda()) for b, n in enumerate(LENGTHS)]
+    assert bool(torch.isnan(g(torch.full_like(mel, float("nan")).cuda())).all())
+    past = torch.arange(T)[None, :] >= lengths[:, None]
+    wav = g(torch.where(past[:, None], float("nan"), mel).cuda(), lengths=lengths.cuda())
+    for b, n in enumerate(LENGTHS):
+        assert torch.equal(wav[b:b + 1, :, :n * hop], single[b]), (cfg, mode, b, n)
+        assert torch.count_nonzero(wav[b, :, n * hop:]) == 0, (cfg, mode, b, n)
+
+
+@pytest.mark.parametrize("mode", MODES)
+@pytest.mark.parametrize("cfg", sorted(CONFIGS))
 def test_ragged_rows_vs_oracle(gens, oracle, mel, lengths, cfg, mode):
     hop = _hop(CONFIGS[cfg])
     wav = gens(cfg, mode)(mel.cuda(), lengths=lengths.cuda()).cpu()
