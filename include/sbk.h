@@ -114,6 +114,13 @@ int sbk_reverse_diffusion_lengths(sbk_handle* h, const float* z, const float* ma
  * x, mean, out: [B,n_feats,T]; mask [B,1,T]; t [B].  Device pointers. */
 int sbk_vc_estimator(sbk_handle* h, const float* x, const float* mask, const float* mean, const float* cond,
                      const float* t, float* out, int B, int T, void* stream);
+/* A ragged DiffVC batch: lengths (device int64 [B], NULL = sbk_vc_estimator) holds each utterance's valid frames L_b (DiffVC's
+ * x_lengths); the kernels clamp them to [1, T].  As for Grad-TTS (sbk_estimator_lengths), utterance b runs on its own
+ * T_b = fix_len_compatibility(L_b) frames: out[b, :, :T_b] is what sbk_vc_estimator computes on the [:T_b] slices of row b
+ * with the same cond row (bit for bit in tf32 and bf16, within fp32 rounding in fp32x3 and fp32), out[b, :, T_b:] is 0, and
+ * x, mean and mask at or past T_b are not read. */
+int sbk_vc_estimator_lengths(sbk_handle* h, const float* x, const float* mask, const float* mean, const float* cond,
+                             const float* t, const int64_t* lengths, float* out, int B, int T, void* stream);
 
 /* Diffusion.reverse_diffusion (DiffVC/model/diffusion.py:164-196), mode 0 = 'pf', 1 = 'em', 2 = 'ml';
  * t_i = 1 - i/N.  cond: [N][B][dim_cond], the conditioning vector of every step (it depends on t, ref and c only,
@@ -121,6 +128,11 @@ int sbk_vc_estimator(sbk_handle* h, const float* x, const float* mask, const flo
  * 'em'/'ml' (the reference draws randn_like(z) per step, :194), NULL for 'pf'.  out may alias z. */
 int sbk_vc_reverse_diffusion(sbk_handle* h, const float* z, const float* mask, const float* mean, const float* cond,
                              const float* noise, float* out, int B, int T, int n_timesteps, int mode, void* stream);
+/* the same over a ragged batch (lengths: see sbk_vc_estimator_lengths).  Row b equals the call on its [:T_b] slices given the
+ * same draws noise[:, b, :, :T_b]; z, mean, mask and noise at or past T_b are not read, and out there is 0. */
+int sbk_vc_reverse_diffusion_lengths(sbk_handle* h, const float* z, const float* mask, const float* mean, const float* cond,
+                                     const float* noise, const int64_t* lengths, float* out, int B, int T, int n_timesteps,
+                                     int mode, void* stream);
 
 /* The hoisted conditioning branch natively: for every step i (t_i = 1 - i/N)
  * xt_ref = compute_diffused_mean(ref, ref_mask, mean_ref, t_i) (:151-155) -> RefBlock (modules.py:156-166: a CUDA-core
@@ -131,6 +143,14 @@ int sbk_vc_reverse_diffusion(sbk_handle* h, const float* z, const float* mask, c
  * SBK_ERR_UNSUPPORTED if a RefBlock conv has no tensor-core kernel. */
 int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float* ref_mask, const float* mean_ref, const float* c,
                         float* cond_out, int B, int Tr, int n_timesteps, void* stream);
+/* A ragged reference batch: ref_lengths (device int64 [B], NULL = sbk_vc_conditioning) holds each reference's valid frames
+ * R_b (DiffVC's x_ref_lengths); the kernels clamp them to [1, Tr].  Sample b's cond rows are bit for bit what
+ * sbk_vc_conditioning computes for ref[b, :, :R_b], mean_ref[b, :, :R_b] with an all-ones mask (B = 1, the reference's own
+ * call): the diffused reference, the block11 conv, the five 3x3 convs, the InstanceNorm statistics and divisor (H * R_b),
+ * the GLU outputs and the mean pooling all stop at R_b, with no rounding of the length.  ref and mean_ref at or past R_b
+ * are not read; ref_mask must be 1 below R_b.  Same workspace and launches as sbk_vc_conditioning. */
+int sbk_vc_conditioning_lengths(sbk_handle* h, const float* ref, const float* ref_mask, const float* mean_ref, const float* c,
+                                const int64_t* ref_lengths, float* cond_out, int B, int Tr, int n_timesteps, void* stream);
 /* test hook: with sbk_debug_capture on, sbk_vc_conditioning copies every tensor the RefBlock branch writes right after the
  * launch that wrote it into a per-name device buffer (the copies do not count as launches).  Each step overwrites the
  * previous step's copies, so they hold the LAST step (t = 1/N).  Names in launch order: ref_block.xt_ref [B][H][Tr];
@@ -353,6 +373,14 @@ size_t sbk_postnet_workspace_bytes(const sbk_postnet* p, int B, int n_feats, int
  * [B,n_feats,T].  The output is not masked, as in the reference: a padded column equals final_conv.bias.  Device pointers,
  * asynchronous on `stream`; a refused kernel launch fails the call. */
 int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* mask, float* out, int B, int n_feats, int T, void* stream);
+/* A ragged batch: lengths (device int64 [B], NULL = every utterance T frames, as sbk_postnet_forward) holds each utterance's
+ * valid frames L_b, as DiffVC's x_lengths or x_ref_lengths.  out[b, :, :L_b] is bit for bit what sbk_postnet_forward computes
+ * for x[b, :, :L_b] with an all-ones mask (B = 1, the reference's own call: its GroupNorm statistics and 7x7 borders see
+ * exactly L_b frames, no rounding of the length), and out[b, :, L_b:] is 0 - not final_conv.bias, since the utterance's own
+ * call has no such columns.  x at or past L_b is not read; mask must be 1 below L_b.  The kernels clamp each length to
+ * [1, T] (no host read of the lengths; callers validate them).  Same workspace and launches as sbk_postnet_forward. */
+int sbk_postnet_forward_lengths(sbk_postnet* p, const float* x, const float* mask, const int64_t* lengths, float* out, int B,
+                                int n_feats, int T, void* stream);
 /* kernel launches (and memsets) the last sbk_postnet_forward enqueued */
 int64_t sbk_postnet_last_launch_count(const sbk_postnet* p);
 

@@ -21,6 +21,7 @@ EXPORTS = [
     "sbk_prior_expand", "sbk_last_host_launches", "sbk_workspace_bytes_n",
     "sbk_vc_cond_debug_num", "sbk_vc_cond_debug_name", "sbk_vc_cond_debug_op_layout", "sbk_vc_cond_debug_read",
     "sbk_estimator_lengths", "sbk_reverse_diffusion_lengths", "sbk_reverse_steps_lengths",
+    "sbk_vc_estimator_lengths", "sbk_vc_reverse_diffusion_lengths", "sbk_vc_conditioning_lengths",
 ]
 
 
@@ -56,6 +57,9 @@ def load_library() -> C.CDLL:
     lib.sbk_estimator_lengths.argtypes = [P, F, F, F, F, F, P, F, I, I, P]
     lib.sbk_reverse_diffusion_lengths.argtypes = [P, F, F, F, F, F, P, F, I, I, I, I, P]
     lib.sbk_reverse_steps_lengths.argtypes = [P, F, F, F, F, F, P, I, I, I, I, I, I, P]
+    lib.sbk_vc_conditioning_lengths.argtypes = [P, F, F, F, F, P, F, I, I, I, P]
+    lib.sbk_vc_estimator_lengths.argtypes = [P, F, F, F, F, F, P, F, I, I, P]
+    lib.sbk_vc_reverse_diffusion_lengths.argtypes = [P, F, F, F, F, F, P, F, I, I, I, I, P]
     lib.sbk_reverse_diffusion_host.argtypes = [P, F, F, F, F, F, F, I, I, I, I]
     lib.sbk_prior_expand.argtypes = [F, F, F, F, F, C.c_float, I, I, I, I, F, F, F, F, P]
     lib.sbk_last_host_launches.argtypes = [P]
@@ -330,18 +334,24 @@ class Engine(_NativeHandle):
     # ---- DiffVC (model="diffvc")
     VC_MODES = {"pf": 0, "em": 1, "ml": 2}
 
-    def vc_estimator(self, x, mask, mean, cond, t):
+    # lengths (int64 [B] on the input's device, each in 1..T, DiffVC's x_lengths): the U-Net's ragged rule of `estimator`, row
+    # b computed on its own T_b = fix_len_compatibility(lengths[b]) frames and 0 after them (sbk.h: sbk_vc_estimator_lengths)
+    def vc_estimator(self, x, mask, mean, cond, t, lengths=None):
         B, T = self._check_inputs(x, mask, mean, None, t)
+        if lengths is not None:
+            lengths = check_lengths(lengths, B, T, x.device, "x")
         x, mask, mean, cond, t = (_f32c(v, n) for v, n in ((x, "x"), (mask, "mask"), (mean, "mean"), (cond, "cond"), (t, "t")))
         if tuple(cond.shape) != (B, self.dim_cond):
             raise RuntimeError(f"cond shape {tuple(cond.shape)} != {(B, self.dim_cond)}")
         out = torch.empty_like(x)
-        _check(self.lib.sbk_vc_estimator(self.h, _ptr(x), _ptr(mask), _ptr(mean), _ptr(cond), _ptr(t), _ptr(out), B, T,
-                                         self._stream()), "sbk_vc_estimator")
+        _check(self.lib.sbk_vc_estimator_lengths(self.h, _ptr(x), _ptr(mask), _ptr(mean), _ptr(cond), _ptr(t), _ptr(lengths),
+                                                 _ptr(out), B, T, self._stream()), "sbk_vc_estimator")
         return out
 
-    def vc_conditioning(self, ref, ref_mask, mean_ref, c, n_timesteps):
-        """Native hoisted conditioning branch (tensor-core modes): cond [N, B, dim_cond] for t_i = 1 - i/N."""
+    def vc_conditioning(self, ref, ref_mask, mean_ref, c, n_timesteps, ref_lengths=None):
+        """Native hoisted conditioning branch (tensor-core modes): cond [N, B, dim_cond] for t_i = 1 - i/N.  ref_lengths
+        (int64 [B] on ref's device, each in 1..Tr, DiffVC's x_ref_lengths): sample b's rows are the call on its own R_b
+        reference frames (sbk.h: sbk_vc_conditioning_lengths)."""
         for n, t in (("ref", ref), ("ref_mask", ref_mask), ("mean_ref", mean_ref), ("c", c)):
             if not t.is_cuda:
                 raise RuntimeError(f"{n} must be a CUDA tensor: the sampler has no CPU path")
@@ -349,9 +359,12 @@ class Engine(_NativeHandle):
         ref, ref_mask, mean_ref, c = _f32c(ref, "ref"), _f32c(ref_mask, "ref_mask"), _f32c(mean_ref, "mean_ref"), _f32c(c, "c")
         if Fm != self.n_feats or mean_ref.shape != ref.shape or ref_mask.shape != (B, 1, Tr) or tuple(c.shape) != (B, 256):
             raise RuntimeError("shape mismatch in vc_conditioning inputs")
+        if ref_lengths is not None:
+            ref_lengths = check_lengths(ref_lengths, B, Tr, ref.device, "ref")
         out = torch.empty((n_timesteps, B, self.dim_cond), dtype=torch.float32, device=ref.device)
-        _check(self.lib.sbk_vc_conditioning(self.h, _ptr(ref), _ptr(ref_mask), _ptr(mean_ref), _ptr(c), _ptr(out), B, Tr,
-                                            int(n_timesteps), self._stream()), "sbk_vc_conditioning")
+        _check(self.lib.sbk_vc_conditioning_lengths(self.h, _ptr(ref), _ptr(ref_mask), _ptr(mean_ref), _ptr(c),
+                                                    _ptr(ref_lengths), _ptr(out), B, Tr, int(n_timesteps), self._stream()),
+               "sbk_vc_conditioning")
         self._vc_shape = (B, Tr)
         return out
 
@@ -381,12 +394,15 @@ class Engine(_NativeHandle):
             out = out.view(B, H, Tr)
         return out.double().contiguous()
 
-    def vc_reverse_diffusion(self, z, mask, mean, cond, n_timesteps, mode, noise=None):
+    def vc_reverse_diffusion(self, z, mask, mean, cond, n_timesteps, mode, noise=None, lengths=None):
         B, T = self._check_inputs(z, mask, mean, None)
+        if lengths is not None:
+            lengths = check_lengths(lengths, B, T, z.device, "z")
         sl = self.batch_slices(B, T, n_timesteps)
         if len(sl) > 1:
             outs = [self.vc_reverse_diffusion(z[a:b], mask[a:b], mean[a:b], cond[:, a:b].contiguous(), n_timesteps, mode,
-                                              None if noise is None else noise[:, a:b].contiguous()) for a, b in sl]
+                                              None if noise is None else noise[:, a:b].contiguous(),
+                                              None if lengths is None else lengths[a:b]) for a, b in sl]
             return torch.cat(outs, 0)
         z, mask, mean, cond = _f32c(z, "z"), _f32c(mask, "mask"), _f32c(mean, "mean"), _f32c(cond, "cond")
         if tuple(cond.shape) != (n_timesteps, B, self.dim_cond):
@@ -396,8 +412,8 @@ class Engine(_NativeHandle):
                 raise RuntimeError("modes 'em'/'ml' need pre-drawn noise [N,B,n_feats,T]")
             noise = _f32c(noise, "noise")
         out = torch.empty_like(z)
-        self._call(self.lib.sbk_vc_reverse_diffusion, "sbk_vc_reverse_diffusion", self.h, _ptr(z), _ptr(mask), _ptr(mean),
-                   _ptr(cond), _ptr(noise) if mode != "pf" else None, _ptr(out), B, T, int(n_timesteps),
+        self._call(self.lib.sbk_vc_reverse_diffusion_lengths, "sbk_vc_reverse_diffusion", self.h, _ptr(z), _ptr(mask), _ptr(mean),
+                   _ptr(cond), _ptr(noise) if mode != "pf" else None, _ptr(lengths), _ptr(out), B, T, int(n_timesteps),
                    self.VC_MODES[mode], self._stream())
         return out
 

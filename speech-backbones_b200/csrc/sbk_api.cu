@@ -1198,6 +1198,12 @@ static int vc_fold(sbk_handle* h, const float* cond, int rows, int B, cudaStream
 
 extern "C" int sbk_vc_estimator(sbk_handle* h, const float* x, const float* mask, const float* mean, const float* cond,
                                 const float* t, float* out, int B, int T, void* stream) {
+    return sbk_vc_estimator_lengths(h, x, mask, mean, cond, t, nullptr, out, B, T, stream);
+}
+
+// a ragged DiffVC batch: the U-Net's Grad-TTS rule (unet_edge), utterance b on its own T_b = fix_len_compatibility(lengths[b])
+extern "C" int sbk_vc_estimator_lengths(sbk_handle* h, const float* x, const float* mask, const float* mean, const float* cond,
+                                        const float* t, const int64_t* lengths, float* out, int B, int T, void* stream) {
     if (!h || !x || !mask || !mean || !cond || !t || !out) return fail(SBK_ERR_ARG, "sbk_vc_estimator: null argument");
     if (h->cfg.model != SBK_MODEL_DIFFVC) return fail(SBK_ERR_ARG, "sbk_vc_estimator: this handle is not a DiffVC model");
     TRY(ensure_plan(h, B, T, B));
@@ -1208,10 +1214,10 @@ extern "C" int sbk_vc_estimator(sbk_handle* h, const float* x, const float* mask
     CU(cudaMemcpyAsync(pl.mu, mean, nb, cudaMemcpyDeviceToDevice, s));
     CU(cudaMemcpyAsync(pl.mask, mask, (size_t)B * T * sizeof(float), cudaMemcpyDeviceToDevice, s));
     CU(cudaMemcpyAsync(pl.t_rows, t, (size_t)B * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    TRY(load_lengths(h, lengths, B, s));
     int64_t n = 0;
     n += vc_fold(h, cond, 1, B, s);               // one row: the per-sample conditioning vectors
     n += time_table(h, B, s);
-    set_ragged(pl, false);
     set_mode(pl, 0, true, out);
     k_set_int<<<1, 1, 0, s>>>(pl.step_next, 0); ++n;
     { const int k = run_ops(h, s); if (k < 0) return SBK_ERR_CUDA; n += k; }
@@ -1222,6 +1228,13 @@ extern "C" int sbk_vc_estimator(sbk_handle* h, const float* x, const float* mask
 
 extern "C" int sbk_vc_reverse_diffusion(sbk_handle* h, const float* z, const float* mask, const float* mean, const float* cond,
                                         const float* noise, float* out, int B, int T, int n_timesteps, int mode, void* stream) {
+    return sbk_vc_reverse_diffusion_lengths(h, z, mask, mean, cond, noise, nullptr, out, B, T, n_timesteps, mode, stream);
+}
+
+// (a ragged loop runs its own graph: FinalParams.mode 3 + 4, index 7)
+extern "C" int sbk_vc_reverse_diffusion_lengths(sbk_handle* h, const float* z, const float* mask, const float* mean,
+                                                const float* cond, const float* noise, const int64_t* lengths, float* out, int B,
+                                                int T, int n_timesteps, int mode, void* stream) {
     if (!h || !z || !mask || !mean || !cond || !out) return fail(SBK_ERR_ARG, "sbk_vc_reverse_diffusion: null argument");
     if (h->cfg.model != SBK_MODEL_DIFFVC) return fail(SBK_ERR_ARG, "sbk_vc_reverse_diffusion: this handle is not a DiffVC model");
     if (mode < 0 || mode > 2) return fail(SBK_ERR_ARG, "sbk_vc_reverse_diffusion: mode must be 0 (pf), 1 (em) or 2 (ml)");
@@ -1239,10 +1252,10 @@ extern "C" int sbk_vc_reverse_diffusion(sbk_handle* h, const float* z, const flo
     for (int i = 0; i < N; ++i) vc_step_coefs(h->cfg, N, i, mode, &tr[i], &cf[i]);
     CU(cudaMemcpyAsync(pl.t_rows, tr.data(), N * sizeof(float), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(pl.coef, cf.data(), N * sizeof(float4), cudaMemcpyHostToDevice, s));
+    TRY(load_lengths(h, lengths, B, s));
     n += vc_fold(h, cond, N, B, s);
     n += time_table(h, N, s);
-    set_ragged(pl, false);
-    n += launch_scale_mask(z, pl.mask, pl.xt, 0, B, h->cfg.n_feats, T, s);
+    n += launch_scale_mask(z, pl.mask, pl.xt, 0, B, h->cfg.n_feats, T, s, lengths ? pl.lengths : nullptr);
     TRY(run_steps(h, noise, B, T, N, 0, N, mode != 0, s, &n));
     CU(cudaMemcpyAsync(out, pl.xt, nb, cudaMemcpyDeviceToDevice, s));
     h->last_launches = n;
@@ -1251,6 +1264,15 @@ extern "C" int sbk_vc_reverse_diffusion(sbk_handle* h, const float* z, const flo
 
 extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float* ref_mask, const float* mean_ref, const float* c,
                                    float* cond_out, int B, int Tr, int n_timesteps, void* stream) {
+    return sbk_vc_conditioning_lengths(h, ref, ref_mask, mean_ref, c, nullptr, cond_out, B, Tr, n_timesteps, stream);
+}
+
+// ref_lengths (device int64 [B], nullable): a ragged reference batch.  Every launch of the branch cuts at the reference's
+// own R_b = grid_edge(ref_lengths, b, Tr, 0, 1) frames - no rounding, as the reference's call on ref[b, :, :R_b] - so each
+// sample's cond rows are that call's.  The kernels read the caller's buffer directly (the branch is not captured in a graph).
+extern "C" int sbk_vc_conditioning_lengths(sbk_handle* h, const float* ref, const float* ref_mask, const float* mean_ref,
+                                           const float* c, const int64_t* ref_lengths, float* cond_out, int B, int Tr,
+                                           int n_timesteps, void* stream) {
     if (!h || !ref || !ref_mask || !mean_ref || !c || !cond_out) return fail(SBK_ERR_ARG, "sbk_vc_conditioning: null argument");
     if (h->cfg.model != SBK_MODEL_DIFFVC) return fail(SBK_ERR_ARG, "sbk_vc_conditioning: this handle is not a DiffVC model");
     if (!h->is_packed) return fail(SBK_ERR_STATE, "sbk_vc_conditioning: weights not packed");
@@ -1308,6 +1330,7 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
         p.wpk = h->w.get(q + ".wtc"); p.bias = h->w.get(q + ".0.bias"); p.out = raw; p.Cout = cout; p.epi = EPI_PLAIN;
         p.mask = ref_mask; p.T = Tr; p.zero_page = h->d_zero;
         p.form = form; p.nt = conv_tc_ntile(G_C3, cout, p.form);     // as sbk_pack packed it
+        p.lengths = ref_lengths; p.exact = 1;
         return launch_conv_tc(p, s);
     };
     // debug capture: every step writes the same workspace buffers, so the last step's tensors are recorded
@@ -1318,12 +1341,12 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
     };
     auto norm_glu = [&](const char* name, int C, const float* tbias) {
         const std::string q = std::string("estimator.ref_block.") + name;
-        ChanStatsParams cs{raw, st, B, H, Tr, C};
+        ChanStatsParams cs{raw, st, B, H, Tr, C, ref_lengths};
         int k = launch_chan_stats(cs, s);
         snap(name, ".stats", st, (size_t)B * C * 2, 3);
         InGluParams g; memset(&g, 0, sizeof(g));
         g.raw = raw; g.stats = st; g.gamma = h->w.get(q + ".1.weight"); g.beta = h->w.get(q + ".1.bias"); g.tb = tbias;
-        g.mask = ref_mask; g.T = Tr; g.out = act; g.B = B; g.H = H; g.W = Tr; g.C = C; g.form = form;
+        g.mask = ref_mask; g.T = Tr; g.out = act; g.B = B; g.H = H; g.W = Tr; g.C = C; g.form = form; g.lengths = ref_lengths;
         k += launch_in_glu(g, s);
         snap(name, ".act", act, px * C / 2, 1);
         return k;
@@ -1336,14 +1359,14 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
         last_step = i + 1 == N;
         if (cf.use_ref_t) {
             const float* tb_row = tb + (size_t)i * 3 * base;
-            DiffMeanParams dm{ref, mean_ref, ref_mask, xt_ref, (float)gamma0(1.0 - i * (1.0 / N)), B, H, Tr};
+            DiffMeanParams dm{ref, mean_ref, ref_mask, xt_ref, (float)gamma0(1.0 - i * (1.0 / N)), B, H, Tr, ref_lengths};
             n += launch_diff_mean(dm, s);
             snap("xt_ref", "", xt_ref, px, 0);
             snap("tb", "", tb_row, (size_t)3 * base, 0);
             FirstConvParams fc; memset(&fc, 0, sizeof(fc));
             fc.mu = xt_ref; fc.xt = xt_ref; fc.mask = ref_mask; fc.w = h->w.get("estimator.ref_block.block11.w");
             fc.bias = h->w.get("estimator.ref_block.block11.0.bias"); fc.out = raw; fc.ostats = nullptr;
-            fc.B = B; fc.H = H; fc.T = Tr; fc.cin = 1; fc.C = 2 * base; fc.chw4 = 1;
+            fc.B = B; fc.H = H; fc.T = Tr; fc.cin = 1; fc.C = 2 * base; fc.chw4 = 1; fc.lengths = ref_lengths; fc.exact = 1;
             n += launch_first_conv(fc, s);
             snap("block11", ".raw", raw, px * 2 * base, 1);
             n += norm_glu("block11", 2 * base, nullptr);
@@ -1354,7 +1377,7 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
                 snap(sg.name, ".raw", raw, px * sg.cout, 1);
                 n += norm_glu(sg.name, sg.cout, sg.tb_off < 0 ? nullptr : tb_row + sg.tb_off);
             }
-            ChanStatsParams ysm{act, ys, B, H, Tr, 4 * base};
+            ChanStatsParams ysm{act, ys, B, H, Tr, 4 * base, ref_lengths};
             n += launch_chan_stats(ysm, s);
             snap("ysum", "", ys, (size_t)B * dc * 2, 3);
         }
@@ -1364,7 +1387,7 @@ extern "C" int sbk_vc_conditioning(sbk_handle* h, const float* ref, const float*
         vp.c = c; vp.freqs = h->d_freqs; vp.t = tr[i]; vp.dim = dim;
         vp.w0 = h->w.get("estimator.cond_block.0.weight"); vp.b0 = h->w.get("estimator.cond_block.0.bias");
         vp.w2 = h->w.get("estimator.cond_block.2.weight"); vp.b2 = h->w.get("estimator.cond_block.2.bias");
-        vp.out = cond_out + (size_t)i * B * dc; vp.B = B; vp.dc = dc; vp.use_ref = cf.use_ref_t ? 1 : 0;
+        vp.out = cond_out + (size_t)i * B * dc; vp.B = B; vp.dc = dc; vp.use_ref = cf.use_ref_t ? 1 : 0; vp.lengths = ref_lengths;
         n += launch_vc_cond(vp, s);
     }
     if (const cudaError_t e = h->vc_snaps.finish()) return fail(SBK_ERR_CUDA, "sbk_vc_conditioning: debug capture failed: %s", cudaGetErrorString(e));

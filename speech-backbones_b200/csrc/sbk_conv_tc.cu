@@ -144,7 +144,6 @@ template <int GEOM, int NT, int R> constexpr bool x3_depth_ok = Depth<GEOM, NT, 
 template <int GEOM, bool BF16, int NT, bool RES, bool X3, bool VOC = false, int R = 1, bool RAG = false>
 __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     static_assert(!(X3 && BF16), "fp32x3 runs on tf32 operands");
-    static_assert(!RAG || GEOM != G_C7, "ragged batches are Conv1d and U-Net launches");
     using G = Geo<GEOM, R>;
     using D = Depth<GEOM, NT, R>;
     constexpr int NACC = G::NACC, ROWS = G::ROWS;
@@ -233,8 +232,9 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     // 3x3 / Downsample / Upsample tiles start at a row's column w0, and a 1x1 tile (128 flattened pixels) only when it
     // lies inside one image row.  The ResnetBlock-tail 1x1 (RES) visits every tile: at its 168-register cap the test
     // would spill.  Its padded outputs, like every 1x1 output past the edge, are computed but never read into a valid one.
-    auto ein = [&](int b) { return unet_edge(p.lengths, b, p.T, GEOM == G_DOWN ? p.lvl - 1 : (GEOM == G_UP ? p.lvl + 1 : p.lvl)); };
-    auto eout = [&](int b) { return unet_edge(p.lengths, b, p.T, p.lvl); };
+    // (the edge rule is p.exact: unet_edge for a U-Net, the length itself for the PostNet's 7x7 and the RefBlock's 3x3 convs)
+    auto ein = [&](int b) { return grid_edge(p.lengths, b, p.T, GEOM == G_DOWN ? p.lvl - 1 : (GEOM == G_UP ? p.lvl + 1 : p.lvl), p.exact); };
+    auto eout = [&](int b) { return grid_edge(p.lengths, b, p.T, p.lvl, p.exact); };
     auto skip = [&](int b, int h0, int w0) {
         if constexpr (GEOM == G_PW && RES) {
             return false;
@@ -513,7 +513,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                     const int c = n0 + i, g = c / cpg;
                     const double sm_ = p.rgn.stats[(b * kGroups + g) * 2], ss = p.rgn.stats[(b * kGroups + g) * 2 + 1];
                     float inv = p.rgn.inv_count;
-                    if constexpr (RAG2) inv = gn_inv_count(p.rgn, b);
+                    if constexpr (RAG2) inv = gn_inv_count_rag(p.rgn, b);
                     const double m = sm_ * (double)inv;
                     double var = ss * (double)inv - m * m;
                     var = var < 0.0 ? 0.0 : var;
@@ -841,9 +841,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         // which would otherwise serialise against the bulk copies in flight) runs a handful of times.
                         const int pad = C1 ? p.pad : PADK;          // Conv1d: (K-1)*dil/2 samples of halo on each side
                         const int wlo = w0 - pad < 0 ? 0 : w0 - pad, whi = w0 + SPAN + pad > wedge ? wedge : w0 + SPAN + pad;
-                        // RAG2: only the first column at the sample's edge has to read zero - the columns past it feed
-                        // only outputs past the edge, which are neither stored nor counted - and the row's copy brings it
-                        // from the zero page (below).  So the pattern, and the one-lane zeroing, covers the left border
+                        // RAG2: only the PADK columns from the sample's edge on have to read zero (one for a 3x3 halo,
+                        // three for a 7x7: output column edge - 1 reads up to input column edge + 2) - the columns past
+                        // them feed only outputs past the edge, which are neither stored nor counted - and the row's copy
+                        // brings them from the zero page (below).  So the pattern, and the one-lane zeroing, covers the left border
                         // alone, which every sample shares: a right border that moves from tile to tile would re-zero a
                         // stage buffer for nearly every tile.
                         const int qlo = wlo - (w0 - pad), qdata = qlo + (whi - wlo), qhi = RAG2 ? PXP : qdata;
@@ -865,7 +866,8 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         }
                         int vrows = 0;
                         for (int r = 0; r < HR; ++r) { const int hi = C1 ? 0 : h0 - PADK + krow + r; vrows += (hi >= 0 && hi < p.H) ? 1 : 0; }
-                        const int qtx = RAG2 ? (qdata < PXP ? qdata + 1 : PXP) : qhi;     // columns a valid row's copies write
+                        // columns a valid row's copies write (the PADK zero columns clipped at the tile's end)
+                        const int qtx = !RAG2 ? qhi : PADK == 1 ? (qdata < PXP ? qdata + 1 : PXP) : (qdata + PADK < PXP ? qdata + PADK : PXP);
                         if (!conv) a_tx -= (uint32_t)(KCH * vrows * (PXP - (qtx - qlo))) * 16u;
                     }
                     mbar_arrive_expect_tx(full_b(s), B_STAGE_BYTES + a_tx);
@@ -907,7 +909,8 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                             bulk_g2s(row_s + qlo * 16, src + (((long long)(b * p.H + hi) * chs + cl) * p.W + wlo) * 16,
                                      (uint32_t)(whi - wlo) * 16u, full_b(s));
                             const int qe = qlo + (whi - wlo);       // RAG2: the row's first column at or past the edge
-                            if (RAG2 && qe < PXP) bulk_g2s(row_s + qe * 16, zero, 16u, full_b(s));
+                            if (RAG2 && qe < PXP)
+                                bulk_g2s(row_s + qe * 16, zero, (uint32_t)(PADK == 1 ? 1 : (qe + PADK < PXP ? PADK : PXP - qe)) * 16u, full_b(s));
                         }
                     }
                 }
@@ -1073,10 +1076,10 @@ int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
         case tc_key(G_UP, T, 64):                   return launch_unet<G_UP, T, 64>(p, s);
         case tc_key(G_UP, B, 64):                   return launch_unet<G_UP, B, 64>(p, s);
         case tc_key(G_UP, X, 64):                   return launch_unet<G_UP, X, 64>(p, s);
-        // 7x7 (PostNet): tf32 and fp32x3
-        case tc_key(G_C7, T, 128):                  return launch_tc<G_C7, T, 128>(p, s);
-        case tc_key(G_C7, T, 64):                   return launch_tc<G_C7, T, 64>(p, s);
-        case tc_key(G_C7, X, 64):                   return launch_tc<G_C7, X, 64>(p, s);
+        // 7x7 (PostNet): tf32 and fp32x3, a dense or a ragged batch
+        case tc_key(G_C7, T, 128):                  return launch_unet<G_C7, T, 128>(p, s);
+        case tc_key(G_C7, T, 64):                   return launch_unet<G_C7, T, 64>(p, s);
+        case tc_key(G_C7, X, 64):                   return launch_unet<G_C7, X, 64>(p, s);
         default:                                    return -1;
     }
 }

@@ -34,6 +34,16 @@ __host__ __device__ __forceinline__ int unet_frames(const int64_t* lengths, long
 __host__ __device__ __forceinline__ int unet_edge(const int64_t* lengths, long long b, int T, int lvl) {
     return unet_frames(lengths, b, T) >> lvl;
 }
+// The edge rule of a ragged launch (ConvTcParams::exact, GnRef::exact), read by every part of a launch that cuts at the
+// edge: a conv's loader, tile skip and GroupNorm partials, the element-wise walks and the GroupNorm divisor.
+//   exact = 0: unet_edge, the length rounded up to a multiple of 4 (a U-Net runs on fix_len_compatibility frames);
+//   exact = 1: the length itself, clamped to [1, T] (DiffVC's PostNet and RefBlock run on exactly the utterance's frames).
+__host__ __device__ __forceinline__ int grid_edge(const int64_t* lengths, long long b, int T, int lvl, int exact) {
+    if (!exact) return unet_edge(lengths, b, T, lvl);
+    if (!lengths) return T >> lvl;
+    const long long t = lengths[b];
+    return (t < 1 ? 1 : (t > T ? T : (int)t)) >> lvl;
+}
 
 // GroupNorm statistics of one conv output: per (sample, group) {sum, sum of squares} in fp64.
 struct GnRef {
@@ -42,13 +52,20 @@ struct GnRef {
     const float* beta;     // [C]
     float inv_count;       // 1 / ((C/8) * H * W)
     // ragged batch (nullable): sample b counts H * W_b,lvl pixels, 1 / (cnt_ch * W_b) with cnt_ch = (C/8) * H rounded as
-    // the planner rounds it, so the divisor is bit for bit the one of the sample's own call
+    // the planner rounds it, so the divisor is bit for bit the one of the sample's own call.  exact (grid_edge): W_b is the
+    // length itself and the divisor is the PostNet's host expression (float)(1.0 / ((double)cnt_ch * W_b)), in double
     const int64_t* lengths = nullptr; float cnt_ch = 0.f; int T = 0, lvl = 0;
+    int exact = 0;         // (fills the struct's tail padding: the layout of every params struct that embeds one is unchanged)
 };
 #ifdef __CUDACC__
 __device__ __forceinline__ float gn_inv_count(const GnRef& g, int b) {
     if (!g.lengths) return g.inv_count;
     return __frcp_rn(__fmul_rn(g.cnt_ch, (float)unet_edge(g.lengths, b, g.T, g.lvl)));
+}
+// the divisor in a ragged-only kernel, either edge rule (the dense kernels keep gn_inv_count)
+__device__ __forceinline__ float gn_inv_count_rag(const GnRef& g, int b) {
+    if (!g.exact) return gn_inv_count(g, b);
+    return (float)(1.0 / ((double)g.cnt_ch * (double)grid_edge(g.lengths, b, g.T, g.lvl, 1)));
 }
 #endif
 
@@ -135,6 +152,9 @@ struct ConvTcParams {
     // input image at the input level's edge.  Inputs at or past the edge read as zero, tiles wholly past it are skipped,
     // and GroupNorm partials count only the columns below it.
     const int64_t* lengths; int len_mul;
+    // U-Net geometries, a ragged batch: the edge rule (grid_edge) - 0: unet_edge, 1: the length itself (level 0; the
+    // PostNet's 7x7 convs and the RefBlock's 3x3 convs).  The loader, the tile skip and the GroupNorm partials all cut there.
+    int exact;
 };
 
 // The valid samples of utterance b at a stage of W = T * mul samples: its length in frames clamped to [0, T], times mul.
@@ -180,7 +200,7 @@ __host__ __device__ inline size_t conv_tc_wimg_bytes(const ConvTcWImg& g, int co
 
 // Block activation between the two convs of a ResnetBlock, written once in operand form (diffusion.py:57,76):
 //   act = mask ? Mish(GN(raw)) + tproj : 0        (tensor-core forms only: the fp32 mode fuses it into the next conv)
-struct GnActParams {          // (a ragged batch: gn.lengths; frames at or past the edge are not visited)
+struct GnActParams {          // (a ragged batch: gn.lengths, edge rule gn.exact; frames at or past the edge are not visited)
     const float* raw; GnRef gn; const float* tb; int tb_stride; int tb_per_sample; const int* step;
     const float* mask; int T; int lvl;
     float* out; int B, H, W, C;
@@ -199,6 +219,7 @@ struct FirstConvParams {        // Block.conv of downs.0.0.block1 on the planar 
     // value is the mask and whose weights are per (row, sample): w_extra[(row*B + b)][9][C] (row = *step or 0)
     const float* w_extra; const int* step; int extra_per_sample_row;
     const int64_t* lengths = nullptr;   // ragged batch: frames at or past T_b read as zero and count in no statistic
+    int exact = 0;                      // edge rule (grid_edge): 1 = the length itself (the RefBlock's block11, at R_b)
 };
 
 struct ResFinalParams {         // (a ragged batch: gn.lengths; frames at or past the edge are not visited)         // out = Mish(GN(h2raw))*mask + res(x*mask)
@@ -281,11 +302,15 @@ struct CondFoldParams {
 int launch_cond_fold(const CondFoldParams& p, cudaStream_t s);
 
 // ---- DiffVC RefBlock / conditioning branch (DiffVC/model/modules.py:128-166, diffusion.py:62-71), tensor-core modes ----
+// (a ragged reference batch, sbk_vc_conditioning_lengths: `lengths` non-null, each sample's grid ends at its own R_b =
+// grid_edge(lengths, b, W, 0, 1); nothing at or past it is read, and the outputs there are 0)
 struct DiffMeanParams {          // xt_ref = (ref*g + mean_ref*(1-g)) * ref_mask  (compute_diffused_mean, diffusion.py:151-155)
     const float* ref; const float* mean_ref; const float* mask; float* out; float g; int B, H, T;
+    const int64_t* lengths = nullptr;
 };
 struct ChanStatsParams {         // per (sample, channel) {sum, sum of squares} over H*W of a [B][H][C/4][W][4] tensor (InstanceNorm2d)
     const float* x; double* stats; int B, H, W, C;
+    const int64_t* lengths = nullptr;
 };
 struct InGluParams {             // y = mask ? tf32( IN(raw[c]) * sigmoid(IN(raw[c + C/2])) + tb[c] ) : 0   -> C/2 channels
     const float* raw; const double* stats; const float* gamma; const float* beta;   // InstanceNorm2d affine, eps 1e-5
@@ -293,6 +318,7 @@ struct InGluParams {             // y = mask ? tf32( IN(raw[c]) * sigmoid(IN(raw
     const float* mask; int T;    // ref_mask [B][T]
     float* out; int B, H, W, C;  // C = raw channels
     int form;                    // FORM_TF32: fast sigmoid, out rounded to tf32; FORM_X3: exact sigmoid, out unrounded
+    const int64_t* lengths = nullptr;
 };
 struct VcCondParams {            // cond_block( [sinusoid(t) | final_conv(mean-pooled RefBlock) | c] )  (diffusion.py:62-71)
     const double* ysum;          // [B][dc][2] channel sums of the masked RefBlock output (before final_conv)
@@ -303,6 +329,7 @@ struct VcCondParams {            // cond_block( [sinusoid(t) | final_conv(mean-p
     const float* w0; const float* b0; const float* w2; const float* b2;   // cond_block
     float* out;                  // [B][dc] (row of this step)
     int B, dc, use_ref;
+    const int64_t* lengths = nullptr;
 };
 int launch_diff_mean(const DiffMeanParams& p, cudaStream_t s);
 int launch_chan_stats(const ChanStatsParams& p, cudaStream_t s);

@@ -40,10 +40,12 @@ __device__ __forceinline__ float mish_fast_f(float x) {
 __device__ __forceinline__ float mish_rt(float x, int exact) { return exact ? mish_f(x) : mish_fast_f(x); }
 template <bool EXACT> __device__ __forceinline__ float mish_sel(float x) { return EXACT ? mish_f(x) : mish_fast_f(x); }
 
+// RAG: a ragged-only kernel, which also honours the exact edge rule (GnRef::exact); the dense kernels keep gn_inv_count
+template <bool RAG = false>
 __device__ __forceinline__ void gn_mean_rstd(const GnRef& g, int b, int grp, float& mean, float& rstd) {
     const double s = g.stats[(b * kGroups + grp) * 2 + 0];
     const double ss = g.stats[(b * kGroups + grp) * 2 + 1];
-    const float inv = gn_inv_count(g, b);
+    const float inv = RAG ? gn_inv_count_rag(g, b) : gn_inv_count(g, b);
     const double m = s * (double)inv;
     double var = ss * (double)inv - m * m;
     var = var < 0.0 ? 0.0 : var;
@@ -52,13 +54,14 @@ __device__ __forceinline__ void gn_mean_rstd(const GnRef& g, int b, int grp, flo
 }
 
 // fill mean[c], scale[c] = rstd*gamma[c], beta[c] for channels [c_begin, c_begin+n) of a C-channel GN
+template <bool RAG = false>
 __device__ __forceinline__ void gn_fill(const GnRef& g, int b, int C, int c_begin, int n,
                                         float* mean, float* scale, float* beta) {
     const int cpg = C / kGroups;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
         const int c = c_begin + i;
         float m, r;
-        gn_mean_rstd(g, b, c / cpg, m, r);
+        gn_mean_rstd<RAG>(g, b, c / cpg, m, r);
         mean[i] = m;
         scale[i] = r * g.gamma[c];
         beta[i] = g.beta[c];
@@ -393,7 +396,9 @@ int launch_igemm(const IgemmParams& p, cudaStream_t s) {
 // first Block conv: planar stack([mu, xt(, s)])*mask -> Conv3x3(cin -> C) + bias, NHWC raw + GN stats
 // (GradLogPEstimator2d.forward, diffusion.py:181-186 feeding downs[0][0].block1, :56-58)
 // ----------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_first_conv(const FirstConvParams p) {
+// EXACT (p.exact, a ragged RefBlock): the grid ends at the reference's own length R_b (grid_edge), not at unet_frames
+template <bool EXACT>
+__device__ __forceinline__ void first_conv_body(const FirstConvParams& p) {
     // CTA = 256 consecutive frames of one mel row x 64 output channels.  The 3-row x 258-frame masked input halo and
     // the 27x64 weights are staged in shared memory.  A thread owns 16 output channels of 4 frames 64 apart: a weight
     // quad is read once for 4 frames (8 FMAs per shared-memory load; the one-frame version was LSU-bound), and for a
@@ -408,7 +413,7 @@ __global__ void __launch_bounds__(256) k_first_conv(const FirstConvParams p) {
     // a ragged batch: the sample's grid ends at T_b; its frames past it read as zero (its own call's padding), count in no
     // statistic and are not stored, and a CTA wholly past it exits.  CTAs start at frame 0 of a row, so every warp partial
     // covers the frames it covers in the sample's own call.
-    const int Tb = unet_frames(p.lengths, b, p.T);
+    const int Tb = EXACT ? grid_edge(p.lengths, b, p.T, 0, 1) : unet_frames(p.lengths, b, p.T);
     if (w0 >= Tb) return;
     const int K = p.cin * 9;
     const int kreal = p.w_extra ? (p.cin - 1) * 9 : K;       // rows of s_w that come from the shared weight
@@ -499,10 +504,13 @@ __global__ void __launch_bounds__(256) k_first_conv(const FirstConvParams p) {
     const int ng = (64 + cpg - 1) / cpg;
     if (p.ostats && tid < ng * 2) atomicAdd(&p.ostats[((long long)b * kGroups + gb + (tid >> 1)) * 2 + (tid & 1)], s_st[tid]);
 }
+__global__ void __launch_bounds__(256) k_first_conv(const FirstConvParams p) { first_conv_body<false>(p); }
+__global__ void __launch_bounds__(256) k_first_conv_exact(const FirstConvParams p) { first_conv_body<true>(p); }
 
 int launch_first_conv(const FirstConvParams& p, cudaStream_t s) {
     dim3 grid(((p.T + 255) / 256) * p.H, p.C / 64, p.B);
-    k_first_conv<<<grid, 256, 0, s>>>(p);
+    if (p.lengths && p.exact) k_first_conv_exact<<<grid, 256, 0, s>>>(p);
+    else k_first_conv<<<grid, 256, 0, s>>>(p);
     return 1;
 }
 
@@ -640,8 +648,8 @@ static int planar_ew_grid(int form, int H, int W, int C) {
     return C / (4 * lanes) * nhg;
 }
 
-// RAG: a ragged batch (p.gn.lengths): the frames at or past the sample's edge are not visited - no reader of this output
-// looks at them.  (A template flag: the edge in a register would cost the dense loop a spill.)
+// RAG: a ragged batch (p.gn.lengths, edge rule p.gn.exact): the frames at or past the sample's edge are not visited - no
+// reader of this output looks at them.  (A template flag: the edge in a register would cost the dense loop a spill.)
 template <int FORM, int TAIL, bool RAG, class P>
 __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
     constexpr bool B16 = FORM == FORM_BF16, X3 = FORM == FORM_X3;
@@ -652,7 +660,7 @@ __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
     float* mean = sm; float* scale = mean + p.C; float* beta = scale + p.C;
     float* ext = beta + p.C;                     // TAIL_ACT: time projection [C]; TAIL_PLANAR: res_conv [cin][C] + bias [C]
     const int b = blockIdx.y, tid = threadIdx.x;
-    gn_fill(p.gn, b, p.C, 0, p.C, mean, scale, beta);
+    gn_fill<RAG>(p.gn, b, p.C, 0, p.C, mean, scale, beta);
     if constexpr (TAIL == TAIL_ACT) {
         const int row = p.tb_per_sample ? b : *p.step;
         const float* tb = p.tb + (long long)row * p.tb_stride;
@@ -698,7 +706,7 @@ __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
     };
     if constexpr (TAIL == TAIL_PLANAR && B16) res_w(p);
     // (RAG: the edge is re-read per frame rather than held in a register the exact-Mish fp32x3 walk has no room for)
-    for (int w = wl; w < (RAG ? unet_edge(p.gn.lengths, b, p.T, p.lvl) : p.W); w += tw) {
+    for (int w = wl; w < (RAG ? grid_edge(p.gn.lengths, b, p.T, p.lvl, p.gn.exact) : p.W); w += tw) {
         const float mk = __ldg(p.mask + (long long)b * p.T + ((long long)w << p.lvl));
         for (int h0 = (hg * nsub + sub) * U; h0 < p.H; h0 += nhg * nsub * U) {
             float4 r[U]; Unit xv[U]; float i0[U], i1[U], i2[U];
@@ -1163,29 +1171,39 @@ int launch_cond_fold(const CondFoldParams& p, cudaStream_t s) {
 // ----------------------------------------------------------------------------------------------
 // DiffVC RefBlock glue (tensor-core modes; the six 3x3 convs themselves run on k_conv_tc<G_C3>)
 // ----------------------------------------------------------------------------------------------
-__global__ void k_diff_mean(const DiffMeanParams p) {
+// RAG (p.lengths, a ragged reference batch): frames at or past R_b (grid_edge, exact rule) are written as 0 and nothing is
+// read there - the four kernels below then cover exactly the reference's own call on its R_b frames
+template <bool RAG>
+__device__ __forceinline__ void diff_mean_body(const DiffMeanParams& p) {
     const long long n = (long long)p.B * p.H * p.T;
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int w = (int)(i % p.T);
     const long long b = i / ((long long)p.H * p.T);
+    if (RAG && w >= grid_edge(p.lengths, b, p.T, 0, 1)) { p.out[i] = 0.f; return; }
     p.out[i] = (p.ref[i] * p.g + p.mean_ref[i] * (1.0f - p.g)) * p.mask[b * p.T + w];
 }
+__global__ void k_diff_mean(const DiffMeanParams p) { diff_mean_body<false>(p); }
+__global__ void k_diff_mean_ragged(const DiffMeanParams p) { diff_mean_body<true>(p); }
 int launch_diff_mean(const DiffMeanParams& p, cudaStream_t s) {
     const long long n = (long long)p.B * p.H * p.T;
-    k_diff_mean<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p);
+    if (p.lengths) k_diff_mean_ragged<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p);
+    else k_diff_mean<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p);
     return 1;
 }
 
-// InstanceNorm2d statistics: one CTA per (16-byte channel chunk, sample); the chunk's rows are contiguous float4 runs
-__global__ void __launch_bounds__(256) k_chan_stats(const ChanStatsParams p) {
+// InstanceNorm2d statistics: one CTA per (16-byte channel chunk, sample); the chunk's rows are contiguous float4 runs.
+// RAG: the walk stops at R_b and keeps its w = tid + 256 k partition, so the sums are the reference's own call's bit for bit
+template <bool RAG>
+__device__ __forceinline__ void chan_stats_body(const ChanStatsParams& p) {
     __shared__ double s_s[8][8];
     const int ch = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, c4n = p.C / 4;
+    const int Wb = RAG ? grid_edge(p.lengths, b, p.W, 0, 1) : p.W;
     float sx[4] = {0.f, 0.f, 0.f, 0.f}, sq[4] = {0.f, 0.f, 0.f, 0.f};
     double ds[4] = {0, 0, 0, 0}, dq[4] = {0, 0, 0, 0};
     for (int h = 0; h < p.H; ++h) {
         const float* row = p.x + ((((long long)b * p.H + h) * c4n + ch) * p.W) * 4;
-        for (int w = tid; w < p.W; w += 256) {
+        for (int w = tid; w < Wb; w += 256) {
             const float4 v = ldg4(row + (long long)w * 4);
             sx[0] += v.x; sx[1] += v.y; sx[2] += v.z; sx[3] += v.w;
             sq[0] = fmaf(v.x, v.x, sq[0]); sq[1] = fmaf(v.y, v.y, sq[1]); sq[2] = fmaf(v.z, v.z, sq[2]); sq[3] = fmaf(v.w, v.w, sq[3]);
@@ -1212,17 +1230,23 @@ __global__ void __launch_bounds__(256) k_chan_stats(const ChanStatsParams p) {
         p.stats[((long long)b * p.C + ch * 4 + q) * 2 + which] = a;
     }
 }
+__global__ void __launch_bounds__(256) k_chan_stats(const ChanStatsParams p) { chan_stats_body<false>(p); }
+__global__ void __launch_bounds__(256) k_chan_stats_ragged(const ChanStatsParams p) { chan_stats_body<true>(p); }
 int launch_chan_stats(const ChanStatsParams& p, cudaStream_t s) {
-    k_chan_stats<<<dim3(p.C / 4, p.B), 256, 0, s>>>(p);
+    if (p.lengths) k_chan_stats_ragged<<<dim3(p.C / 4, p.B), 256, 0, s>>>(p);
+    else k_chan_stats<<<dim3(p.C / 4, p.B), 256, 0, s>>>(p);
     return 1;
 }
 
-// InstanceNorm2d(affine) + GLU(dim=1) (+ time bias) * mask, written in operand form (tf32-rounded)
-__global__ void __launch_bounds__(256) k_in_glu(const InGluParams p) {
+// InstanceNorm2d(affine) + GLU(dim=1) (+ time bias) * mask, written in operand form (tf32-rounded).
+// RAG: the divisor is the same expression at W = R_b, and frames at or past R_b are written as 0 without reading raw
+template <bool RAG>
+__device__ __forceinline__ void in_glu_body(const InGluParams& p) {
     extern __shared__ float sm[];
     float* mean = sm; float* scale = mean + p.C; float* beta = scale + p.C; float* tbv = beta + p.C;   // tbv: [C/2]
     const int b = blockIdx.y, tid = threadIdx.x, Ch = p.C / 2;
-    const double inv = 1.0 / ((double)p.H * p.W);
+    const int Wb = RAG ? grid_edge(p.lengths, b, p.W, 0, 1) : p.W;
+    const double inv = 1.0 / ((double)p.H * Wb);
     for (int c = tid; c < p.C; c += 256) {
         const double s = p.stats[((long long)b * p.C + c) * 2], ss = p.stats[((long long)b * p.C + c) * 2 + 1];
         const double m = s * inv;
@@ -1240,7 +1264,7 @@ __global__ void __launch_bounds__(256) k_in_glu(const InGluParams p) {
         const long long hc = i / p.W;
         const int w = (int)(i - hc * p.W);
         const int h = (int)(hc / o4n), ch = (int)(hc - (long long)h * o4n);
-        const float mk = __ldg(p.mask + (long long)b * p.T + w);
+        const float mk = RAG && w >= Wb ? 0.f : __ldg(p.mask + (long long)b * p.T + w);
         float o[4] = {0.f, 0.f, 0.f, 0.f};
         if (mk != 0.f) {
             const float* rowa = p.raw + ((((long long)b * p.H + h) * i4n + ch) * p.W + w) * 4;
@@ -1263,17 +1287,22 @@ __global__ void __launch_bounds__(256) k_in_glu(const InGluParams p) {
         *reinterpret_cast<float4*>(p.out + ((long long)b * n4 + i) * 4) = make_float4(o[0], o[1], o[2], o[3]);
     }
 }
+__global__ void __launch_bounds__(256) k_in_glu(const InGluParams p) { in_glu_body<false>(p); }
+__global__ void __launch_bounds__(256) k_in_glu_ragged(const InGluParams p) { in_glu_body<true>(p); }
 int launch_in_glu(const InGluParams& p, cudaStream_t s) {
     const long long n4 = (long long)p.H * p.W * (p.C / 8);
     int gx = (int)((n4 + 256 * 8 - 1) / (256 * 8));
     if (gx < 1) gx = 1;
     if (gx > 4096) gx = 4096;
-    k_in_glu<<<dim3(gx, p.B), 256, (3 * p.C + p.C / 2) * sizeof(float), s>>>(p);
+    if (p.lengths) k_in_glu_ragged<<<dim3(gx, p.B), 256, (3 * p.C + p.C / 2) * sizeof(float), s>>>(p);
+    else k_in_glu<<<dim3(gx, p.B), 256, (3 * p.C + p.C / 2) * sizeof(float), s>>>(p);
     return 1;
 }
 
-// conditioning vector of one step: [sinusoid(1000 t) | ref_block.final_conv(mean-pooled y) | c] -> cond_block
-__global__ void __launch_bounds__(256) k_vc_cond(const VcCondParams p) {
+// conditioning vector of one step: [sinusoid(1000 t) | ref_block.final_conv(mean-pooled y) | c] -> cond_block.
+// RAG: the mask sum of the mean pooling runs over the reference's own R_b frames
+template <bool RAG>
+__device__ __forceinline__ void vc_cond_body(const VcCondParams& p) {
     extern __shared__ float sm[];
     const int b = blockIdx.x, tid = threadIdx.x, dim = p.dim, dc = p.dc, half = dim / 2;
     const int n_in = dim + (p.use_ref ? dc : 0) + 256;
@@ -1288,7 +1317,8 @@ __global__ void __launch_bounds__(256) k_vc_cond(const VcCondParams p) {
     }
     if (p.use_ref) {
         float msum = 0.f;
-        for (int w = 0; w < p.Tr; ++w) msum += p.mask[(long long)b * p.Tr + w];
+        const int Wb = RAG ? grid_edge(p.lengths, b, p.Tr, 0, 1) : p.Tr;
+        for (int w = 0; w < Wb; ++w) msum += p.mask[(long long)b * p.Tr + w];
         const double den = (double)msum * p.H;
         for (int c = tid; c < dc; c += 256) ybar[c] = (float)(p.ysum[((long long)b * dc + c) * 2] / den);
     }
@@ -1314,9 +1344,12 @@ __global__ void __launch_bounds__(256) k_vc_cond(const VcCondParams p) {
         p.out[(long long)b * dc + o] = acc;
     }
 }
+__global__ void __launch_bounds__(256) k_vc_cond(const VcCondParams p) { vc_cond_body<false>(p); }
+__global__ void __launch_bounds__(256) k_vc_cond_ragged(const VcCondParams p) { vc_cond_body<true>(p); }
 int launch_vc_cond(const VcCondParams& p, cudaStream_t s) {
     const int n_in = p.dim + (p.use_ref ? p.dc : 0) + 256;
-    k_vc_cond<<<p.B, 256, (n_in + p.dc + 4 * p.dc) * sizeof(float), s>>>(p);
+    if (p.lengths) k_vc_cond_ragged<<<p.B, 256, (n_in + p.dc + 4 * p.dc) * sizeof(float), s>>>(p);
+    else k_vc_cond<<<p.B, 256, (n_in + p.dc + 4 * p.dc) * sizeof(float), s>>>(p);
     return 1;
 }
 

@@ -29,9 +29,10 @@ using namespace sbk;
 namespace {
 
 // a0 = (w*(x*m) + b)*m per channel, written as [B][H][C/4][T][4] operand chunks; tf32 mode rounds to nearest (as k_gn_act),
-// fp32x3 mode keeps fp32
-__global__ void k_pn_init(const float* x, const float* mask, const float* w, const float* bias, float* out, int B, int H, int C, int T,
-                          int round_tf32) {
+// fp32x3 mode keeps fp32.  RAG (a ragged batch): frames at or past the utterance's length are written as 0, x is not read there.
+template <bool RAG>
+__device__ __forceinline__ void pn_init(const float* x, const float* mask, const float* w, const float* bias, float* out, int B, int H,
+                                        int C, int T, int round_tf32, const int64_t* lengths) {
     const int c4n = C / 4;
     const long long n = (long long)B * H * c4n * T;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -40,6 +41,10 @@ __global__ void k_pn_init(const float* x, const float* mask, const float* w, con
         const int ch = (int)(r % c4n);
         const long long bh = r / c4n;                       // b*H + h
         const long long b = bh / H;
+        if (RAG && t >= grid_edge(lengths, b, T, 0, 1)) {
+            reinterpret_cast<float4*>(out)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            continue;
+        }
         const float m = __ldg(mask + b * T + t);
         const float xv = __ldg(x + bh * T + t) * m;
         const float4 wv = __ldg(reinterpret_cast<const float4*>(w) + ch), bv = __ldg(reinterpret_cast<const float4*>(bias) + ch);
@@ -51,15 +56,27 @@ __global__ void k_pn_init(const float* x, const float* mask, const float* w, con
         reinterpret_cast<float4*>(out)[i] = make_float4(o[0], o[1], o[2], o[3]);
     }
 }
+__global__ void k_pn_init(const float* x, const float* mask, const float* w, const float* bias, float* out, int B, int H, int C, int T,
+                          int round_tf32) {
+    pn_init<false>(x, mask, w, bias, out, B, H, C, T, round_tf32, nullptr);
+}
+__global__ void k_pn_init_ragged(const float* x, const float* mask, const float* w, const float* bias, float* out, int B, int H, int C,
+                                 int T, int round_tf32, const int64_t* lengths) {
+    pn_init<true>(x, mask, w, bias, out, B, H, C, T, round_tf32, lengths);
+}
 
-// final_conv (dim -> 1, postnet.py:52): out[b][h][t] = bias + sum_c w[c] * y[b][h][c][t], channels summed in order
-__global__ void k_pn_final(const float* y, const float* w, const float* bias, float* out, int B, int H, int C, int T) {
+// final_conv (dim -> 1, postnet.py:52): out[b][h][t] = bias + sum_c w[c] * y[b][h][c][t], channels summed in order.
+// RAG: frames at or past the utterance's length are written as 0 (its own call has no such frames), y is not read there.
+template <bool RAG>
+__device__ __forceinline__ void pn_final(const float* y, const float* w, const float* bias, float* out, int B, int H, int C, int T,
+                                         const int64_t* lengths) {
     const int c4n = C / 4;
     const long long n = (long long)B * H * T;
     const float bb = __ldg(bias);
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         const int t = (int)(i % T);
         const long long bh = i / T;
+        if (RAG && t >= grid_edge(lengths, bh / H, T, 0, 1)) { out[i] = 0.f; continue; }
         const float* yp = y + (bh * c4n * T + t) * 4;
         float acc = 0.f;
         for (int ch = 0; ch < c4n; ++ch) {
@@ -69,6 +86,13 @@ __global__ void k_pn_final(const float* y, const float* w, const float* bias, fl
         }
         out[i] = acc + bb;
     }
+}
+__global__ void k_pn_final(const float* y, const float* w, const float* bias, float* out, int B, int H, int C, int T) {
+    pn_final<false>(y, w, bias, out, B, H, C, T, nullptr);
+}
+__global__ void k_pn_final_ragged(const float* y, const float* w, const float* bias, float* out, int B, int H, int C, int T,
+                                  const int64_t* lengths) {
+    pn_final<true>(y, w, bias, out, B, H, C, T, lengths);
 }
 
 // The workspace of one (B, n_feats, T), the same in every mode: a0, raw (raw1, then raw2), act (act1, then the res conv's
@@ -169,6 +193,13 @@ extern "C" size_t sbk_postnet_workspace_bytes(const sbk_postnet* p, int B, int n
 }
 
 extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* mask, float* out, int B, int n_feats, int T, void* stream) {
+    return sbk_postnet_forward_lengths(p, x, mask, nullptr, out, B, n_feats, T, stream);
+}
+
+// lengths (device int64 [B], nullable): a ragged batch.  Utterance b runs on its own L_b = lengths[b] frames (clamped to
+// [1, T]) exactly as its own call on x[b, :, :L_b] does - no rounding of the length - and its output from L_b on is 0.
+extern "C" int sbk_postnet_forward_lengths(sbk_postnet* p, const float* x, const float* mask, const int64_t* lengths, float* out,
+                                           int B, int n_feats, int T, void* stream) {
     if (!p || !x || !mask || !out) return fail(SBK_ERR_ARG, "sbk_postnet_forward: null argument");
     if (!p->is_packed) return fail(SBK_ERR_STATE, "sbk_postnet_forward: weights not packed (sbk_postnet_set_weight for every key, then sbk_postnet_pack)");
     if (B <= 0 || n_feats <= 0 || T <= 0) return fail(SBK_ERR_ARG, "sbk_postnet_forward: B, n_feats and T must be positive (got %d, %d, %d)", B, n_feats, T);
@@ -187,6 +218,9 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
     double* st1 = st; double* st2 = st + (size_t)B * kGroups * 2;
     auto R = [&](const std::string& k) { return p->w.get(k); };
     const float inv_count = (float)(1.0 / ((double)(C / kGroups) * H * T));
+    // a ragged batch: every launch cuts at the utterance's own length (grid_edge, exact rule), and the GroupNorm divisor is
+    // the expression above at T = L_b, evaluated per sample in double on the device (gn_inv_count_rag)
+    const bool rag = lengths != nullptr;
     int64_t n = 0;
     auto refused = [&](const char* what) {
         return fail(SBK_ERR_CUDA, "sbk_postnet_forward: the %s launch was refused (device attribute / geometry)", what);
@@ -194,8 +228,12 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
     int k;
 
     CU(cudaMemsetAsync(st, 0, 2 * (size_t)B * kGroups * 2 * sizeof(double), s)); ++n;
-    k_pn_init<<<ew_grid((long long)B * H * (C / 4) * T), 256, 0, s>>>(x, mask, R("init_conv.weight"), R("init_conv.bias"), a0, B, H, C, T,
-                                                                      x3 ? 0 : 1);
+    if (rag)
+        k_pn_init_ragged<<<ew_grid((long long)B * H * (C / 4) * T), 256, 0, s>>>(x, mask, R("init_conv.weight"), R("init_conv.bias"), a0,
+                                                                                 B, H, C, T, x3 ? 0 : 1, lengths);
+    else
+        k_pn_init<<<ew_grid((long long)B * H * (C / 4) * T), 256, 0, s>>>(x, mask, R("init_conv.weight"), R("init_conv.bias"), a0, B, H, C, T,
+                                                                          x3 ? 0 : 1);
     ++n;
     auto conv7 = [&](const char* blk, const float* in, double* ost) {
         ConvTcParams cp; memset(&cp, 0, sizeof(cp));
@@ -204,11 +242,13 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
         cp.wpk = R(q + "weight"); cp.bias = R(q + "bias"); cp.out = raw; cp.Cout = C; cp.epi = EPI_PLAIN;
         cp.ostats = ost; cp.mask = mask; cp.T = T; cp.zero_page = p->zero;
         cp.form = form; cp.nt = conv_tc_ntile(G_C7, C, form);     // as pn_pack packed it
+        cp.lengths = lengths; cp.exact = 1;
         return launch_conv_tc(cp, s);
     };
     auto gnref = [&](double* stp, const char* blk) {
         const std::string q = std::string("res_block.") + blk + ".block.1.";
         GnRef g; g.stats = stp; g.gamma = R(q + "weight"); g.beta = R(q + "bias"); g.inv_count = inv_count;
+        g.lengths = lengths; g.cnt_ch = (float)(C / kGroups) * (float)H; g.T = T; g.lvl = 0; g.exact = 1;
         return g;
     };
     if ((k = conv7("block1", a0, st1)) < 0) return refused("block1 conv");
@@ -230,10 +270,15 @@ extern "C" int sbk_postnet_forward(sbk_postnet* p, const float* x, const float* 
         cp.epi = EPI_RES; cp.rraw = raw; cp.rgn = gnref(st2, "block2"); cp.out_mask = 1;
         cp.mask = mask; cp.T = T; cp.zero_page = p->zero;
         cp.form = form; cp.nt = conv_tc_ntile(G_PW, C, form);
+        cp.lengths = lengths; cp.exact = 1;
         if ((k = launch_conv_tc(cp, s)) < 0) return refused("residual conv");
         n += k;
     }
-    k_pn_final<<<ew_grid((long long)B * H * T), 256, 0, s>>>(act, R("final_conv.weight"), R("final_conv.bias"), out, B, H, C, T);
+    if (rag)
+        k_pn_final_ragged<<<ew_grid((long long)B * H * T), 256, 0, s>>>(act, R("final_conv.weight"), R("final_conv.bias"), out, B, H, C, T,
+                                                                        lengths);
+    else
+        k_pn_final<<<ew_grid((long long)B * H * T), 256, 0, s>>>(act, R("final_conv.weight"), R("final_conv.bias"), out, B, H, C, T);
     ++n;
     CU(cudaGetLastError());
     p->last_launches = n;

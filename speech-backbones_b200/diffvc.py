@@ -161,29 +161,36 @@ class Diffusion(BaseModule):
 
     # ---- sampling (diffusion.py:164-205) ------------------------------------------------------
     @torch.no_grad()
-    def conditioning_table(self, ref, ref_mask, mean_ref, c, n_timesteps):
+    def conditioning_table(self, ref, ref_mask, mean_ref, c, n_timesteps, *, ref_lengths=None):
         """cond[i] for every step i (t_i = 1 - i/N): the hoisted conditioning branch, native in every precision
         (libsbk `sbk_vc_conditioning`: RefBlock convs on wgmma - tf32 + fp16 correction for the fp32-class modes - plus the
-        InstanceNorm / GLU / cond_block kernels).  There is no PyTorch fallback."""
+        InstanceNorm / GLU / cond_block kernels).  There is no PyTorch fallback.  ref_lengths (int64 [B], keyword only): each
+        sample's rows are computed on exactly its own reference frames, as its B = 1 call."""
         with torch.cuda.device(ref.device):
-            return self.engine().vc_conditioning(ref, ref_mask, mean_ref, c, n_timesteps)
+            return self.engine().vc_conditioning(ref, ref_mask, mean_ref, c, n_timesteps, ref_lengths)
 
+    # lengths (int64 [B] on z's device, e.g. x_lengths; keyword only): a ragged batch for the score U-Net.  Row b is sampled
+    # on its own T_b = fix_len_compatibility(lengths[b]) frames, as the call on its [:T_b] slices would be given the same
+    # draws noise[:, b, :, :T_b], and is 0 from T_b on (Engine.vc_reverse_diffusion).  The noise is drawn on the batch
+    # shapes exactly as without lengths.  ref_lengths (int64 [B], e.g. x_ref_lengths): the conditioning table row by row on
+    # each reference's own frames (conditioning_table).
     @torch.no_grad()
-    def reverse_diffusion(self, z, mask, mean, ref, ref_mask, mean_ref, c, n_timesteps, mode):
+    def reverse_diffusion(self, z, mask, mean, ref, ref_mask, mean_ref, c, n_timesteps, mode, *, lengths=None, ref_lengths=None):
         eng = self.engine()
-        cond = self.conditioning_table(ref, ref_mask, mean_ref, c, n_timesteps)
+        cond = self.conditioning_table(ref, ref_mask, mean_ref, c, n_timesteps, ref_lengths=ref_lengths)
         noise = None
         if mode != "pf":   # the reference draws randn_like(z) once per step, in step order (:194)
             noise = torch.stack([torch.randn_like(z) for _ in range(n_timesteps)])
         with torch.cuda.device(z.device):
-            return eng.vc_reverse_diffusion(z, mask, mean, cond, n_timesteps, mode, noise)
+            return eng.vc_reverse_diffusion(z, mask, mean, cond, n_timesteps, mode, noise, lengths)
 
     @torch.no_grad()
-    def forward(self, z, mask, mean, ref, ref_mask, mean_ref, c, n_timesteps, mode):
+    def forward(self, z, mask, mean, ref, ref_mask, mean_ref, c, n_timesteps, mode, *, lengths=None, ref_lengths=None):
         if mode not in ["pf", "em", "ml"]:
             print("Inference mode must be one of [pf, em, ml]!")
             return z
-        return self.reverse_diffusion(z, mask, mean, ref, ref_mask, mean_ref, c, n_timesteps, mode)
+        return self.reverse_diffusion(z, mask, mean, ref, ref_mask, mean_ref, c, n_timesteps, mode, lengths=lengths,
+                                      ref_lengths=ref_lengths)
 
     # ---- training-time methods: plain PyTorch (diffusion.py:157-162, 207-222) ------------------
     def forward_diffusion(self, x0, mask, mean, t):
@@ -213,7 +220,8 @@ def fix_len_compatibility(length, num_downsamplings_in_unet=2):
 
 
 @torch.no_grad()
-def convert_from_encoder(decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode="ml"):
+def convert_from_encoder(decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode="ml", *,
+                         ragged=False, x_ref_lengths=None):
     """Drop-in for DiffVC/model/vc.py:107,110-127 - what `DiffVC.forward` does once `mean = self.encoder(x, x_mask)` and
     `mean_ref = self.encoder(x_ref, x_ref_mask)` exist:
 
@@ -223,7 +231,11 @@ def convert_from_encoder(decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_re
     `x_lengths[i]` on the host: 2B slice copies and B device-to-host synchronisations per call (vc.py:118-120).  Here the same
     tensors are one masked pad each (bit-identical: a copy of the valid prefix into zeros), the only synchronisation left is
     `int(x_lengths.max())`, which fixes the SHAPE of the returned tensor, and the noise draw is the reference's own call
-    (`randn_like` of a contiguous [B,n_feats,T'] tensor), so the generator stream is unchanged.  Returns (mean_x, y)."""
+    (`randn_like` of a contiguous [B,n_feats,T'] tensor), so the generator stream is unchanged.  Returns (mean_x, y).
+
+    ragged=True (keyword only): the decoder samples row b on its own fix_len_compatibility(x_lengths[b]) frames and runs the
+    conditioning branch on its own x_ref_lengths[b] reference frames (the sum of x_ref_mask's row when not given), so each
+    row is the reference's B = 1 call on that utterance given the same draws; y is 0 past x_lengths[b]'s U-Net grid."""
     b, n_feats, t_in = x.shape
     max_length = int(x_lengths.max())                                              # :111 (host sync: output shape)
     if t_in != max_length:                                                         # the reference's x_mask (:104) has max_length frames
@@ -242,7 +254,13 @@ def convert_from_encoder(decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_re
     mean_new, mean_x_new = repad(mean), repad(mean_x)
     z = mean_x_new
     z += torch.randn_like(mean_x_new, device=mean_x_new.device)                    # :122-123
-    y = decoder(z, x_mask_new, mean_new, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode)     # :125
+    if ragged:
+        if x_ref_lengths is None:
+            x_ref_lengths = x_ref_mask.sum((1, 2)).round().to(torch.int64)
+        y = decoder(z, x_mask_new, mean_new, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode, lengths=x_lengths,
+                    ref_lengths=x_ref_lengths)
+    else:
+        y = decoder(z, x_mask_new, mean_new, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode)     # :125
     return mean_x, y[:, :, :max_length]
 
 
@@ -268,11 +286,14 @@ class FwdDiffusion(BaseModule):
         self.encoder = MelEncoder(n_feats, channels, filters, heads, layers, kernel, dropout, window_size)
         self.postnet = PostNet(dim, precision=precision)
 
+    # lengths (int64 [B] or None; keyword only): a ragged batch.  The mel encoder's masked convs and masked softmax already
+    # keep each row's valid frames independent of its batch-mates; the PostNet then runs row b on exactly its lengths[b]
+    # frames (PostNet.forward), and the row is 0 after them where the padded batch has final_conv.bias.
     @torch.no_grad()
-    def forward(self, x, mask):                                                     # :37-41
+    def forward(self, x, mask, *, lengths=None):                                    # :37-41
         x, mask = self.relocate_input([x, mask])
         z = self.encoder(x, mask)
-        return self.postnet(z, mask)
+        return self.postnet(z, mask, lengths=lengths)
 
 
 class DiffVC(BaseModule):
@@ -296,14 +317,22 @@ class DiffVC(BaseModule):
         self.encoder.load_state_dict(enc_dict, strict=False)
 
     @torch.no_grad()
-    def forward(self, x, x_lengths, x_ref, x_ref_lengths, c, n_timesteps, mode="ml"):   # :82-127
+    # ragged=True (keyword only): each utterance of the padded batch is converted as the reference's own B = 1 call on it,
+    # given the same draws: x_lengths go to the encoder's PostNet and the U-Net, x_ref_lengths to the reference's PostNet
+    # and the RefBlock branch.  False: the reference's padded-batch semantics, byte for byte as before.
+    def forward(self, x, x_lengths, x_ref, x_ref_lengths, c, n_timesteps, mode="ml", *, ragged=False):   # :82-127
         x, x_lengths = self.relocate_input([x, x_lengths])
         x_ref, x_ref_lengths, c = self.relocate_input([x_ref, x_ref_lengths, c])
         x_mask = sequence_mask(x_lengths).unsqueeze(1).to(x.dtype)
         x_ref_mask = sequence_mask(x_ref_lengths).unsqueeze(1).to(x_ref.dtype)
-        mean = self.encoder(x, x_mask)
-        mean_ref = self.encoder(x_ref, x_ref_mask)
-        return convert_from_encoder(self.decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode)
+        if not ragged:
+            mean = self.encoder(x, x_mask)
+            mean_ref = self.encoder(x_ref, x_ref_mask)
+            return convert_from_encoder(self.decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode)
+        mean = self.encoder(x, x_mask, lengths=x_lengths)
+        mean_ref = self.encoder(x_ref, x_ref_mask, lengths=x_ref_lengths)
+        return convert_from_encoder(self.decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode,
+                                    ragged=True, x_ref_lengths=x_ref_lengths)
 
     def compute_loss(self, x, x_lengths, x_ref, c):                                 # :129-144
         x, x_lengths, x_ref, c = self.relocate_input([x, x_lengths, x_ref, c])

@@ -4,7 +4,7 @@ Same constructor `PostNet(dim, groups=8)`, the same submodule tree (`init_conv`,
 `res_block.res`, `final_conv`: 14 tensors, 1,623,297 parameters at dim = 128), so `FwdDiffusion` / `DiffVC` checkpoints load
 unchanged, and the same `forward(x, mask)` -> [B, n_feats, T].  The modules below are parameter containers; `forward` runs in
 libsbk.so (`sbk_postnet_forward`: the two 7x7 convs on wgmma, csrc/sbk_postnet.cu).  Inference only: there is no CPU path
-and no autograd through this module.
+and no autograd through this module.  `forward(x, mask, lengths=...)` runs a ragged batch, each row exactly its own call.
 
 `precision`: "fp32x3" (default; "fp32" maps to it) runs the fp32-class tf32 + fp16-correction split, "tf32" ("bf16" maps to
 it) plain tf32 operands.  The mapping lives in the library (sbk_postnet.cu)."""
@@ -15,7 +15,7 @@ import ctypes as C
 import torch
 import torch.nn as nn
 
-from .binding import PREC, _check, _check_precision, _NativeHandle, _ptr
+from .binding import PREC, _check, _check_precision, _NativeHandle, _ptr, check_lengths
 from .gradtts import BaseModule, Mish
 
 
@@ -51,13 +51,17 @@ class PostNetEngine(_NativeHandle):
         self.lib.sbk_postnet_workspace_bytes.argtypes = [P, I, I, I]
         self.lib.sbk_postnet_workspace_bytes.restype = C.c_size_t
         self.lib.sbk_postnet_forward.argtypes = [P, P, P, P, I, I, I, P]
+        self.lib.sbk_postnet_forward_lengths.argtypes = [P, P, P, P, P, I, I, I, P]
         rc = self._create(SbkPostNetConfig(device, dim, groups, PREC[precision]))
         if rc == _SBK_ERR_UNSUPPORTED:
             raise ValueError(self.lib.sbk_last_error().decode())
         _check(rc, "sbk_postnet_create")
         self.device, self.dim = device, dim
 
-    def forward(self, x, mask):
+    # Ragged batches: `lengths` (int64 [B] on x's device, each in 1..T, e.g. DiffVC's x_lengths) computes utterance b on its
+    # own L_b frames, as the call on x[b:b+1, :, :L_b] would (sbk.h: sbk_postnet_forward_lengths): GroupNorm statistics and
+    # 7x7 borders see exactly L_b frames.  Its output from L_b on is 0, where the padded batch writes final_conv.bias.
+    def forward(self, x, mask, lengths=None):
         for n, v in (("x", x), ("mask", mask)):
             if not v.is_cuda or v.device.index != self.device:
                 raise RuntimeError(f"{n} lives on {v.device}; the PostNet runs only on cuda:{self.device} (no CPU path)")
@@ -66,11 +70,13 @@ class PostNetEngine(_NativeHandle):
         B, Fm, T = x.shape
         if tuple(mask.shape) != (B, 1, T):
             raise RuntimeError(f"expected mask [B,1,T] = {(B, 1, T)}, got {tuple(mask.shape)}")
+        if lengths is not None:
+            lengths = check_lengths(lengths, B, T, x.device, "x")
         x, mask = x.contiguous(), mask.to(torch.float32).contiguous()
         out = torch.empty_like(x)
         with torch.cuda.device(x.device):
-            self._call(self.lib.sbk_postnet_forward, "sbk_postnet_forward", self.h, _ptr(x), _ptr(mask), _ptr(out), B, Fm, T,
-                       self._stream())
+            self._call(self.lib.sbk_postnet_forward_lengths, "sbk_postnet_forward", self.h, _ptr(x), _ptr(mask), _ptr(lengths),
+                       _ptr(out), B, Fm, T, self._stream())
         return out
 
 
@@ -104,5 +110,7 @@ class PostNet(BaseModule):
         return self._engine
 
     @torch.no_grad()
-    def forward(self, x, mask):
-        return self.engine().forward(x, mask)
+    def forward(self, x, mask, *, lengths=None):
+        """lengths (int64 [B] or None): a ragged batch, each row its own call on its first lengths[b] frames and 0 after
+        them (PostNetEngine.forward)."""
+        return self.engine().forward(x, mask, lengths)
