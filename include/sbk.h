@@ -108,6 +108,34 @@ int sbk_reverse_diffusion_lengths(sbk_handle* h, const float* z, const float* ma
                                   const float* noise, const int64_t* lengths, float* out, int B, int T, int n_timesteps,
                                   int stoc, void* stream);
 
+/* ---- rolling batches (Grad-TTS) -----------------------------------------------------------------------------
+ * A slot plan of `capacity` rows (slots) at T = max_frames keeps running while requests join and leave it: slot b holds
+ * one request - the arguments of one B = 1 Diffusion.forward call - at its own step i_b of its own n_timesteps N_b, and
+ * runs as a ragged row of its T_b frames (sbk_estimator_lengths).  Step i_b uses t = 1 - (i_b + 0.5)/N_b and the
+ * coefficients every other sampler call uses for it.  A finished request's mel is its own B = 1 sbk_reverse_diffusion
+ * (bit for bit in tf32 and bf16, within fp32 rounding in fp32x3 and fp32) and, in every mode bit for bit, row b of a
+ * sbk_reverse_diffusion_lengths call at (capacity, max_frames) with N_b steps, whatever the other slots hold and whenever
+ * the request was admitted.  An empty slot runs as a 4-frame row of zeros and is read by no other row.
+ * The schedule is deterministic: the caller knows when each slot finishes without reading device memory.
+ * The plan is the handle's one plan: another sampler call on the handle replaces it, and the rolling entry points then fail
+ * with SBK_ERR_STATE until the next sbk_rolling_reserve.  Grad-TTS handles only (SBK_ERR_ARG for DiffVC). */
+/* (Re)build the slot plan at (capacity >= 1, max_frames a multiple of 4) with every slot empty. */
+int sbk_rolling_reserve(sbk_handle* h, int capacity, int max_frames, void* stream);
+/* Admit a request into an empty slot (SBK_ERR_STATE if it is busy): z, mu [1,n_feats,T_b], mask [1,1,T_b] (copied on the
+ * stream: they may be reused after the call), T_b a multiple of 4 in [4, max_frames], n_timesteps >= 1, spk [1,spk_emb_dim]
+ * when n_spks > 1, and for stoc = 1 noise [n_timesteps,1,n_feats,T_b], the reference's per-step draws, which the slot reads
+ * until it finishes: the caller keeps it alive until then.  Only this slot's rows and schedule are written. */
+int sbk_rolling_admit(sbk_handle* h, int slot, const float* z, const float* mask, const float* mu, const float* spk,
+                      const float* noise, int T_b, int n_timesteps, int stoc, void* stream);
+/* Run `steps` >= 1 steps of every slot that has steps left (a finished or empty slot is left as it is).  One host launch
+ * of a CUDA graph (sbk_last_host_launches() == 1) where the driver supports conditional nodes. */
+int sbk_rolling_advance(sbk_handle* h, int steps, void* stream);
+/* Copy a finished slot's mel into out [1,n_feats,T_b] (device, stream-ordered, no host synchronisation); SBK_ERR_STATE if
+ * the slot holds no finished request. */
+int sbk_rolling_read(sbk_handle* h, int slot, float* out, void* stream);
+/* Empty a slot (finished or not) so that a new request can be admitted into it. */
+int sbk_rolling_release(sbk_handle* h, int slot, void* stream);
+
 /* ---- DiffVC (SBK_MODEL_DIFFVC) ------------------------------------------------------------------------------
  * GradLogPEstimator.forward (DiffVC/model/diffusion.py:61-106) with the xt-independent conditioning vector
  * (time sinusoid | RefBlock | speaker embedding -> cond_block, :62-71) supplied by the caller: cond [B][dim_cond].

@@ -22,6 +22,7 @@ EXPORTS = [
     "sbk_vc_cond_debug_num", "sbk_vc_cond_debug_name", "sbk_vc_cond_debug_op_layout", "sbk_vc_cond_debug_read",
     "sbk_estimator_lengths", "sbk_reverse_diffusion_lengths", "sbk_reverse_steps_lengths",
     "sbk_vc_estimator_lengths", "sbk_vc_reverse_diffusion_lengths", "sbk_vc_conditioning_lengths",
+    "sbk_rolling_reserve", "sbk_rolling_admit", "sbk_rolling_advance", "sbk_rolling_read", "sbk_rolling_release",
 ]
 
 
@@ -62,6 +63,11 @@ def load_library() -> C.CDLL:
     lib.sbk_vc_reverse_diffusion_lengths.argtypes = [P, F, F, F, F, F, P, F, I, I, I, I, P]
     lib.sbk_reverse_diffusion_host.argtypes = [P, F, F, F, F, F, F, I, I, I, I]
     lib.sbk_prior_expand.argtypes = [F, F, F, F, F, C.c_float, I, I, I, I, F, F, F, F, P]
+    lib.sbk_rolling_reserve.argtypes = [P, I, I, P]
+    lib.sbk_rolling_admit.argtypes = [P, I, F, F, F, F, F, I, I, I, P]
+    lib.sbk_rolling_advance.argtypes = [P, I, P]
+    lib.sbk_rolling_read.argtypes = [P, I, F, P]
+    lib.sbk_rolling_release.argtypes = [P, I, P]
     lib.sbk_last_host_launches.argtypes = [P]
     lib.sbk_debug_read.argtypes = [P, C.c_char_p, F, C.POINTER(C.c_int64)]
     lib.sbk_debug_num.argtypes = [P]
@@ -432,6 +438,34 @@ class Engine(_NativeHandle):
                                                    _ptr(out), B, T, int(n_timesteps), 1 if stoc else 0),
                "sbk_reverse_diffusion_host")
         return out
+
+    # ---- rolling batches (sbk.h: sbk_rolling_*): a slot plan whose rows each run one request at its own step.  These are
+    # the raw slot operations; RollingSampler (rolling.py) keeps the queue and the schedule and checks the arguments.
+    @property
+    def torch_device(self):
+        return torch.device("cuda", self.device)
+
+    def rolling_reserve(self, capacity, max_frames):
+        self._call(self.lib.sbk_rolling_reserve, "sbk_rolling_reserve", self.h, int(capacity), int(max_frames), self._stream())
+
+    def rolling_admit(self, slot, z, mask, mu, n_timesteps, stoc=False, spk=None, noise=None):
+        """z, mu [1,n_feats,T_b], mask [1,1,T_b], spk [1,spk_emb_dim] or None, noise [N,1,n_feats,T_b] or None: contiguous fp32
+        on this engine's device.  The slot reads `noise` until it finishes; the caller keeps it alive."""
+        _check(self.lib.sbk_rolling_admit(self.h, int(slot), _ptr(z), _ptr(mask), _ptr(mu), _ptr(spk), _ptr(noise),
+                                          int(z.shape[-1]), int(n_timesteps), 1 if stoc else 0, self._stream()),
+               "sbk_rolling_admit")
+
+    def rolling_advance(self, steps):
+        _check(self.lib.sbk_rolling_advance(self.h, int(steps), self._stream()), "sbk_rolling_advance")
+
+    def rolling_read(self, slot, frames):
+        """The finished mel of `slot`, [1, n_feats, frames] (frames = its T_b)"""
+        out = torch.empty((1, self.n_feats, int(frames)), dtype=torch.float32, device=self.torch_device)
+        _check(self.lib.sbk_rolling_read(self.h, int(slot), _ptr(out), self._stream()), "sbk_rolling_read")
+        return out
+
+    def rolling_release(self, slot):
+        _check(self.lib.sbk_rolling_release(self.h, int(slot), self._stream()), "sbk_rolling_release")
 
     def last_host_launches(self):
         """Host launches the Euler loop of the last sampler call took (1 = the whole loop ran as one CUDA graph)."""

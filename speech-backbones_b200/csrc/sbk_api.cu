@@ -71,6 +71,22 @@ struct Plan {
     int loop_state[8] = {};
     int* step_end = nullptr;
     int launches_per_step = 0;
+    // a slot plan (sbk_rolling_reserve): every row runs its own request at its own step.  Another sampler call on the
+    // handle replaces the plan (ensure_plan) and with it the slots' state.
+    bool rolling = false;
+    cudaGraphExec_t groll = nullptr;                        // WHILE { one rolling step }
+    int roll_state = 0;                                     // 0 untried, 1 built, -1 unavailable
+};
+
+// the host's record of the slots of a slot plan: what it admitted and how many steps it has advanced since, so it knows
+// when each slot finishes without reading device memory
+struct Rolling {
+    int capacity = 0, max_frames = 0;
+    SlotSched* sched = nullptr;             // device [capacity]
+    SlotStep* cur = nullptr;                // device [capacity], gathered by k_slot_begin every step
+    std::vector<SlotSched> host;            // host copies of sched (i advanced by sbk_rolling_advance as the device does)
+    std::vector<void*> tab;                 // per slot: device [cap] float4 coef, then [cap] float t
+    std::vector<int> tab_cap;
 };
 
 }  // namespace
@@ -94,6 +110,7 @@ struct sbk_handle {
     Snapshots vc_snaps;
     int tb_off[16];
     int tb_total = 0;
+    Rolling roll;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -228,6 +245,7 @@ static void free_plan(sbk_handle* h) {
     Plan& p = h->plan;
     for (int i = 0; i < 8; ++i) if (p.gexec[i]) { cudaGraphExecDestroy(p.gexec[i]); p.gexec[i] = nullptr; }
     for (int i = 0; i < 8; ++i) if (p.gloop[i]) { cudaGraphExecDestroy(p.gloop[i]); p.gloop[i] = nullptr; }
+    if (p.groll) cudaGraphExecDestroy(p.groll);
     for (auto& op : p.ops) if (op.dbg_copy) cudaFree(op.dbg_copy);
     p = Plan();
 }
@@ -235,6 +253,9 @@ static void free_plan(sbk_handle* h) {
 extern "C" void sbk_destroy(sbk_handle* h) {
     if (!h) return;
     free_plan(h);
+    cudaFree(h->roll.sched);
+    cudaFree(h->roll.cur);
+    for (void* t : h->roll.tab) cudaFree(t);
     cudaFree(h->d_freqs);
     cudaFree(h->d_zero);
     if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
@@ -807,7 +828,7 @@ static int run_ops(sbk_handle* h, cudaStream_t s) {
     StepBeginParams sb{pl.stats, pl.n_stat_doubles, pl.step_cur, pl.step_next};
     int n = launch_step_begin(sb, s);
     for (auto& op : pl.ops) {
-        const int k = launch_op(op, s);
+        const int k = pl.rolling && op.kind == OP_FINAL ? launch_final_slot(op.fn, h->roll.cur, h->roll.sched, s) : launch_op(op, s);
         if (k < 0) { fail(SBK_ERR_CUDA, "launch of '%s' was refused (device attribute / layout)", op.name.c_str()); return -1; }
         n += k;
         if (h->capture && op.dbg_ptr && op.dbg_numel > 0) {
@@ -824,7 +845,7 @@ static int ensure_plan(sbk_handle* h, int B, int T, int rows) {
     if (B <= 0 || T <= 0 || T % 4 != 0) return fail(SBK_ERR_ARG, "B must be > 0 and T a positive multiple of 4 (fix_len_compatibility), got B=%d T=%d", B, T);
     CU(cudaSetDevice(h->cfg.device));
     Plan& pl = h->plan;
-    if (pl.B == B && pl.T == T && pl.tb_rows >= rows) return SBK_OK;     // (a freed plan has B = 0)
+    if (!pl.rolling && pl.B == B && pl.T == T && pl.tb_rows >= rows) return SBK_OK;     // (a freed plan has B = 0)
     int cap = rows < 64 ? 64 : rows;
     if (pl.B == B && pl.T == T && cap < pl.tb_rows) cap = pl.tb_rows;
     return build_plan(h, B, T, cap);
@@ -931,13 +952,13 @@ static void step_coefs(const sbk_config& c, int n_timesteps, int i, float* t_out
     *cf = make_float4(beta, hf, sqrtf(beta * hf), 0.f);
 }
 
-// Build (once per plan and sampler mode) the single-launch loop graph.  Returns false - and the caller falls back to one
-// graph launch per step - if this driver / toolkit refuses conditional nodes; the reason is kept in sbk_last_error().
-static bool build_loop_graph(sbk_handle* h, int mode) {     // (mode: the graph index, FinalParams.mode + 4 * ragged)
+// Capture WHILE(step_next < step_end) { body } as one graph: `body(stream)` enqueues one step and returns its launches, or
+// -1 when a launcher refused.  Returns nullptr - the caller falls back to one launch per step - if this driver / toolkit
+// refuses conditional nodes; the reason is kept in sbk_last_error().
+template <class Body>
+static cudaGraphExec_t capture_loop_graph(sbk_handle* h, Body body) {
     Plan& pl = h->plan;
-    if (pl.loop_state[mode] != 0) return pl.loop_state[mode] > 0;
-    pl.loop_state[mode] = -1;
-    if (!h->cap_stream && cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking) != cudaSuccess) return false;
+    if (!h->cap_stream && cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking) != cudaSuccess) return nullptr;
     cudaGraph_t g = nullptr;
     cudaGraphExec_t exec = nullptr;
     bool ok = false;
@@ -953,9 +974,9 @@ static bool build_loop_graph(sbk_handle* h, int mode) {     // (mode: the graph 
         np.conditional.size = 1;
         cudaGraphNode_t node;
         if (cudaGraphAddNode(&node, g, nullptr, 0, &np) != cudaSuccess) break;
-        cudaGraph_t body = np.conditional.phGraph_out[0];
-        if (cudaStreamBeginCaptureToGraph(h->cap_stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal) != cudaSuccess) break;
-        const int k = run_ops(h, h->cap_stream);
+        cudaGraph_t bodyg = np.conditional.phGraph_out[0];
+        if (cudaStreamBeginCaptureToGraph(h->cap_stream, bodyg, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal) != cudaSuccess) break;
+        const int k = body(h->cap_stream);
         k_loop_cond<<<1, 1, 0, h->cap_stream>>>(handle, pl.step_next, pl.step_end);
         cudaGraph_t dummy = nullptr;
         if (cudaStreamEndCapture(h->cap_stream, &dummy) != cudaSuccess || k < 0) break;
@@ -966,12 +987,23 @@ static bool build_loop_graph(sbk_handle* h, int mode) {     // (mode: the graph 
         const cudaError_t e = cudaGetLastError();
         fail(SBK_ERR_CUDA, "single-launch loop graph unavailable (%s): falling back to one graph launch per step", cudaGetErrorString(e));
         if (exec) cudaGraphExecDestroy(exec);
-    } else {
-        pl.gloop[mode] = exec;
-        pl.loop_state[mode] = 1;
+        exec = nullptr;
     }
     if (g) cudaGraphDestroy(g);
-    return ok;
+    return exec;
+}
+
+// Build (once per plan and sampler mode) the single-launch loop graph.  Returns false - and the caller falls back to one
+// graph launch per step - if this driver / toolkit refuses conditional nodes.
+static bool build_loop_graph(sbk_handle* h, int mode) {     // (mode: the graph index, FinalParams.mode + 4 * ragged)
+    Plan& pl = h->plan;
+    if (pl.loop_state[mode] != 0) return pl.loop_state[mode] > 0;
+    pl.loop_state[mode] = -1;
+    const cudaGraphExec_t exec = capture_loop_graph(h, [&](cudaStream_t s) { return run_ops(h, s); });
+    if (!exec) return false;
+    pl.gloop[mode] = exec;
+    pl.loop_state[mode] = 1;
+    return true;
 }
 
 static int run_steps(sbk_handle* h, const float* noise, int B, int T, int N, int s0, int s1, int stoc, cudaStream_t s, int64_t* launches) {
@@ -1117,6 +1149,180 @@ extern "C" int sbk_reverse_diffusion_host(sbk_handle* h, const float* z, const f
     if (d_noise) CU(cudaFreeAsync(d_noise, s));
     CU(cudaStreamSynchronize(s));
     h->last_launches = n;
+    return SBK_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// rolling batches: a slot plan whose rows (slots) each run one request's Euler(-Maruyama) loop at its own step
+// ------------------------------------------------------------------------------------------------
+static int rolling_state(sbk_handle* h, const char* what) {
+    if (!h) return fail(SBK_ERR_ARG, "%s: null handle", what);
+    if (!h->plan.rolling)
+        return fail(SBK_ERR_STATE, "%s: no slot plan (call sbk_rolling_reserve; another sampler call on this handle replaces it)", what);
+    CU(cudaSetDevice(h->cfg.device));
+    return SBK_OK;
+}
+
+// the rows of slot b: xt = z * mask, mu and mask of the request over its T_b frames, 0 after them; z == nullptr clears the
+// row.  lengths[b] = T_b (a cleared slot runs as the shortest ragged row, 4 frames).
+static int slot_rows(sbk_handle* h, int b, const float* z, const float* mu, const float* mask, int Tb, cudaStream_t s) {
+    Plan& pl = h->plan;
+    const int H = h->cfg.n_feats, T = pl.T;
+    SlotWriteParams w{z, mu, mask, pl.xt + (size_t)b * H * T, pl.mu + (size_t)b * H * T, pl.mask + (size_t)b * T, H, T, Tb};
+    int n = launch_slot_write(w, s);
+    const int64_t len = Tb;
+    CU(cudaMemcpyAsync(pl.lengths + b, &len, sizeof(len), cudaMemcpyHostToDevice, s));
+    return n;
+}
+
+extern "C" int sbk_rolling_reserve(sbk_handle* h, int capacity, int max_frames, void* stream) {
+    if (!h) return fail(SBK_ERR_ARG, "sbk_rolling_reserve: null handle");
+    if (h->cfg.model != SBK_MODEL_GRADTTS) return fail(SBK_ERR_ARG, "sbk_rolling_reserve: this handle is a DiffVC model (rolling batches are Grad-TTS only)");
+    if (capacity < 1 || max_frames < 4 || max_frames % 4 != 0)
+        return fail(SBK_ERR_ARG, "sbk_rolling_reserve: capacity must be >= 1 and max_frames a positive multiple of 4, got %d, %d", capacity, max_frames);
+    if (!h->is_packed) return fail(SBK_ERR_STATE, "weights not packed: call sbk_set_weight for every key, then sbk_pack");
+    CU(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    TRY(build_plan(h, capacity, max_frames, capacity));
+    Plan& pl = h->plan;
+    Rolling& r = h->roll;
+    if (r.capacity != capacity) {
+        CU(cudaStreamSynchronize(s));           // (the previous plan's work may still read the old tables)
+        cudaFree(r.sched); cudaFree(r.cur);
+        r.sched = nullptr; r.cur = nullptr;
+        CU(cudaMalloc(&r.sched, capacity * sizeof(SlotSched)));
+        CU(cudaMalloc(&r.cur, capacity * sizeof(SlotStep)));
+        for (void* t : r.tab) cudaFree(t);
+        r.tab.assign(capacity, nullptr);
+        r.tab_cap.assign(capacity, 0);
+    }
+    r.capacity = capacity; r.max_frames = max_frames;
+    r.host.assign(capacity, SlotSched{});
+    CU(cudaMemsetAsync(r.sched, 0, capacity * sizeof(SlotSched), s));
+    CU(cudaMemsetAsync(pl.spk_s, 0, (size_t)capacity * h->cfg.n_feats * sizeof(float), s));
+    int64_t n = 0;
+    for (int b = 0; b < capacity; ++b) n += slot_rows(h, b, nullptr, nullptr, nullptr, 4, s);
+    set_ragged(pl, true);
+    set_mode(pl, 1, true, pl.xt);               // time rows per sample (row b = slot b); the update's mode is per slot
+    pl.rolling = true;
+    CU(cudaGetLastError());
+    h->last_launches = n;
+    return SBK_OK;
+}
+
+extern "C" int sbk_rolling_admit(sbk_handle* h, int slot, const float* z, const float* mask, const float* mu, const float* spk,
+                                 const float* noise, int T_b, int n_timesteps, int stoc, void* stream) {
+    TRY(rolling_state(h, "sbk_rolling_admit"));
+    Rolling& r = h->roll;
+    if (!z || !mask || !mu) return fail(SBK_ERR_ARG, "sbk_rolling_admit: null argument");
+    if (slot < 0 || slot >= r.capacity) return fail(SBK_ERR_ARG, "sbk_rolling_admit: slot %d out of range [0, %d)", slot, r.capacity);
+    if (r.host[slot].n != 0) return fail(SBK_ERR_STATE, "sbk_rolling_admit: slot %d is busy (release it first)", slot);
+    if (T_b < 4 || T_b > r.max_frames || T_b % 4 != 0)
+        return fail(SBK_ERR_ARG, "sbk_rolling_admit: T_b must be a multiple of 4 in [4, %d] (fix_len_compatibility), got %d", r.max_frames, T_b);
+    if (n_timesteps < 1) return fail(SBK_ERR_ARG, "sbk_rolling_admit: n_timesteps must be >= 1");
+    if (stoc && !noise) return fail(SBK_ERR_ARG, "sbk_rolling_admit: stoc=1 needs a noise buffer");
+    if (h->cfg.n_spks > 1 && !spk) return fail(SBK_ERR_ARG, "sbk_rolling_admit: spk is required when n_spks > 1");
+    cudaStream_t s = (cudaStream_t)stream;
+    Plan& pl = h->plan;
+    const int N = n_timesteps;
+    // the request's t and coefficient rows, computed as every other sampler call computes them (step_coefs)
+    std::vector<float4> tab((size_t)N + (N + 3) / 4);
+    float* tr = reinterpret_cast<float*>(tab.data() + N);
+    for (int i = 0; i < N; ++i) step_coefs(h->cfg, N, i, &tr[i], &tab[i]);
+    if (r.tab_cap[slot] < N) {
+        if (r.tab[slot]) CU(cudaFreeAsync(r.tab[slot], s));
+        r.tab[slot] = nullptr;
+        r.tab_cap[slot] = 0;
+        CU(cudaMallocAsync(&r.tab[slot], tab.size() * sizeof(float4), s));
+        r.tab_cap[slot] = N;
+    }
+    // pageable-source async copies are staged before returning, so the host vectors may die at scope exit
+    CU(cudaMemcpyAsync(r.tab[slot], tab.data(), tab.size() * sizeof(float4), cudaMemcpyHostToDevice, s));
+    SlotSched e;
+    e.n = N; e.i = 0; e.stoc = stoc ? 1 : 0; e.T = T_b; e.noise = stoc ? noise : nullptr;
+    e.coef_tab = static_cast<const float4*>(r.tab[slot]);
+    e.t_tab = reinterpret_cast<const float*>(e.coef_tab + N);
+    CU(cudaMemcpyAsync(r.sched + slot, &e, sizeof(e), cudaMemcpyHostToDevice, s));
+    int64_t n = slot_rows(h, slot, z, mu, mask, T_b, s);
+    if (h->cfg.n_spks > 1) {
+        SpkParams p; p.spk = spk; p.B = 1; p.E = h->cfg.spk_emb_dim; p.n_feats = h->cfg.n_feats;
+        p.out = pl.spk_s + (size_t)slot * h->cfg.n_feats;
+        p.w0 = h->w.get("estimator.spk_mlp.0.weight"); p.b0 = h->w.get("estimator.spk_mlp.0.bias");
+        p.w2 = h->w.get("estimator.spk_mlp.2.weight"); p.b2 = h->w.get("estimator.spk_mlp.2.bias");
+        n += launch_spk(p, s);
+    }
+    CU(cudaGetLastError());
+    r.host[slot] = e;
+    h->last_launches = n;
+    return SBK_OK;
+}
+
+// one rolling step: every slot's t, coefficients and noise slab, the time table of those rows, the U-Net and the update
+static int rolling_step(sbk_handle* h, cudaStream_t s) {
+    Plan& pl = h->plan;
+    SlotBeginParams p{h->roll.sched, h->roll.cur, pl.t_rows, pl.coef, pl.B, h->cfg.n_feats};
+    int n = launch_slot_begin(p, s);
+    n += time_table(h, pl.B, s);
+    const int k = run_ops(h, s);
+    return k < 0 ? -1 : n + k;
+}
+
+extern "C" int sbk_rolling_advance(sbk_handle* h, int steps, void* stream) {
+    TRY(rolling_state(h, "sbk_rolling_advance"));
+    if (steps < 1) return fail(SBK_ERR_ARG, "sbk_rolling_advance: steps must be >= 1, got %d", steps);
+    cudaStream_t s = (cudaStream_t)stream;
+    Plan& pl = h->plan;
+    int64_t n = 0;
+    h->last_host_launches = steps;
+    if (h->cfg.use_graph && pl.roll_state == 0) {
+        pl.roll_state = -1;
+        pl.groll = capture_loop_graph(h, [&](cudaStream_t cs) { return rolling_step(h, cs); });
+        if (pl.groll) pl.roll_state = 1;
+    }
+    if (pl.roll_state > 0) {
+        // one host launch: WHILE(step_next < step_end) { one rolling step }
+        k_set_int<<<1, 1, 0, s>>>(pl.step_next, 0);
+        k_set_int<<<1, 1, 0, s>>>(pl.step_end, steps);
+        CU(cudaGraphLaunch(pl.groll, s));
+        n += 3 + (int64_t)steps * (pl.launches_per_step + 3);
+        h->last_host_launches = 1;
+    } else {
+        for (int i = 0; i < steps; ++i) {
+            const int k = rolling_step(h, s);
+            if (k < 0) return SBK_ERR_CUDA;
+            n += k;
+        }
+    }
+    CU(cudaGetLastError());
+    for (SlotSched& e : h->roll.host) e.i = std::min(e.n, e.i + steps);
+    h->last_launches = n;
+    return SBK_OK;
+}
+
+extern "C" int sbk_rolling_read(sbk_handle* h, int slot, float* out, void* stream) {
+    TRY(rolling_state(h, "sbk_rolling_read"));
+    if (!out) return fail(SBK_ERR_ARG, "sbk_rolling_read: null argument");
+    const Rolling& r = h->roll;
+    if (slot < 0 || slot >= r.capacity) return fail(SBK_ERR_ARG, "sbk_rolling_read: slot %d out of range [0, %d)", slot, r.capacity);
+    const SlotSched& e = r.host[slot];
+    if (e.n == 0 || e.i < e.n)
+        return fail(SBK_ERR_STATE, "sbk_rolling_read: slot %d holds no finished request (%d of %d steps run)", slot, e.i, e.n);
+    const Plan& pl = h->plan;
+    const size_t row = (size_t)pl.T * sizeof(float), len = (size_t)e.T * sizeof(float);
+    CU(cudaMemcpy2DAsync(out, len, pl.xt + (size_t)slot * h->cfg.n_feats * pl.T, row, len, h->cfg.n_feats,
+                         cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    return SBK_OK;
+}
+
+extern "C" int sbk_rolling_release(sbk_handle* h, int slot, void* stream) {
+    TRY(rolling_state(h, "sbk_rolling_release"));
+    Rolling& r = h->roll;
+    if (slot < 0 || slot >= r.capacity) return fail(SBK_ERR_ARG, "sbk_rolling_release: slot %d out of range [0, %d)", slot, r.capacity);
+    cudaStream_t s = (cudaStream_t)stream;
+    CU(cudaMemsetAsync(r.sched + slot, 0, sizeof(SlotSched), s));
+    h->last_launches = slot_rows(h, slot, nullptr, nullptr, nullptr, 4, s);
+    CU(cudaGetLastError());
+    r.host[slot] = SlotSched{};
     return SBK_OK;
 }
 

@@ -353,6 +353,29 @@ int launch_prior_expand(const PriorExpandParams& p, cudaStream_t s);
 
 struct StepBeginParams { double* stats; int n_doubles; int* step_cur; int* step_next; };
 
+// ---- a rolling Grad-TTS batch (sbk_rolling_*): every row (slot) runs its own request at its own step --------------------
+// The schedule of slot b, in device memory.  Written whole by the host at admission and release; k_final_slot advances i.
+struct SlotSched {
+    int n;                      // the request's n_timesteps; 0: the slot is empty
+    int i;                      // the step it runs next (the request has finished when i == n)
+    int stoc;                   // 1: Euler-Maruyama with the request's own noise
+    int T;                      // its frames T_b (the row stride of its noise)
+    const float* noise;         // stoc: [n][n_feats][T_b], the request's draws; else nullptr
+    const float* t_tab;         // [n] t of each step, and
+    const float4* coef_tab;     // [n] its coefficients, both from the host's step_coefs
+};
+// What k_slot_begin gathers for the step about to run: mode 0 (idle or finished: the row is not updated), 1 (Euler) or
+// 2 (Euler-Maruyama, noise = this step's slab of the request's draws)
+struct SlotStep { const float* noise; int i; int mode; };
+struct SlotBeginParams { const SlotSched* sched; SlotStep* cur; float* t_rows; float4* coef; int B, H; };
+// admission / release of one slot: the plan's rows xt = z * mask, mu and mask over the plan's T frames, 0 from T_b on
+// (z, mu, mask [H][T_b] of the request; nullptr: the row is cleared)
+struct SlotWriteParams { const float* z; const float* mu; const float* mask; float* xt; float* mu_out; float* mask_out; int H, T, Tb; };
+int launch_slot_begin(const SlotBeginParams& p, cudaStream_t s);
+int launch_slot_write(const SlotWriteParams& p, cudaStream_t s);
+// k_final over a rolling batch: row b's mode and coefficients are its slot's (cur[b], p.coef[b]); advances sched[b].i
+int launch_final_slot(const FinalParams& p, const SlotStep* cur, SlotSched* sched, cudaStream_t s);
+
 // launchers (all asynchronous on `s`); return the number of kernels launched
 int launch_igemm(const IgemmParams& p, cudaStream_t s);
 int launch_first_conv(const FirstConvParams& p, cudaStream_t s);

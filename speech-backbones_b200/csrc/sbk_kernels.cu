@@ -982,10 +982,34 @@ int launch_attn_mix(const AttnMixParams& p, cudaStream_t s) {
 //   mode 1: xt' = (xt - (0.5*(mu - xt - est))*beta*h) * mask
 //   mode 2: xt' = (xt - ((0.5*(mu - xt) - est)*beta*h + eps*sqrt(beta*h))) * mask
 // ----------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_final(const FinalParams p) {
+// The Grad-TTS update of one element of a rolling batch's row b: mode 1 and 2 of k_final, with the slot's coefficients
+// cf and, stochastic, the request's own draws [n_feats][T_b] (the row is never past T_b here)
+__device__ __forceinline__ void slot_update(const FinalParams& p, const SlotStep& c, const float4 cf, int b, long long idx,
+                                            float mk, float est) {
+    const float xt = p.xt_in[idx], mu = __ldg(p.mu + idx);
+    float dxt;
+    if (c.mode == 1) {
+        dxt = ((0.5f * ((mu - xt) - est)) * cf.x) * cf.y;
+    } else {
+        const int m = (int)(idx - (long long)b * p.H * p.T), h = m / p.T;
+        const float eps = __ldg(c.noise + (long long)h * unet_frames(p.lengths, b, p.T) + (m - h * p.T));
+        dxt = ((0.5f * (mu - xt) - est) * cf.x) * cf.y + eps * cf.z;
+    }
+    p.xt_out[idx] = (xt - dxt) * mk;
+}
+
+// SLOT: a rolling batch (launch_final_slot) - row b takes its mode, coefficients and noise from its slot (slot_update), an
+// idle row is left as it is, and the row's step counter advances.  SLOT = false is the dense and ragged k_final: its code is
+// the part outside the `if constexpr (SLOT)` blocks, and its SASS is that of the kernel before the template.
+template <bool SLOT>
+__global__ void __launch_bounds__(256) k_final(const FinalParams p, const SlotStep* slot, SlotSched* sched) {
     extern __shared__ __align__(16) float sm[];
     float* mean = sm; float* scale = mean + p.C; float* beta = scale + p.C; float* wf = beta + p.C;
     const int b = blockIdx.y, tid = threadIdx.x;
+    if constexpr (SLOT) {
+        if (slot[b].mode == 0) return;                  // (the whole block: nothing below synchronises for it)
+        if (blockIdx.x == 0 && tid == 0) sched[b].i = slot[b].i + 1;
+    }
     gn_fill(p.gn, b, p.C, 0, p.C, mean, scale, beta);
     for (int i = tid; i < p.C; i += 256) wf[i] = p.wfin[i];
     __syncthreads();
@@ -994,9 +1018,13 @@ __global__ void __launch_bounds__(256) k_final(const FinalParams p) {
     const float bf = __ldg(p.bfin);
     float4 cf = make_float4(0.f, 0.f, 0.f, 0.f);
     int srow = 0;
-    if (p.mode != 0) { srow = *p.step; cf = p.coef[srow]; }
+    if (!SLOT && p.mode != 0) { srow = *p.step; cf = p.coef[srow]; }
     auto update = [&](long long idx, float mk, float dot) {
         const float est = mk != 0.f ? dot + bf : 0.f;
+        if constexpr (SLOT) {
+            slot_update(p, slot[b], p.coef[b], b, idx, mk, est);
+            return;
+        }
         if (p.mode == 0) {
             p.xt_out[idx] = est;
         } else {
@@ -1068,10 +1096,56 @@ __global__ void __launch_bounds__(256) k_final(const FinalParams p) {
     }
 }
 
+static int final_grid(const FinalParams& p) {
+    const int gx = p.chw4 ? (p.H * p.T + 255) / 256 : (p.H * p.T + 127) / 128;
+    return gx > 2048 ? 2048 : gx;
+}
+
 int launch_final(const FinalParams& p, cudaStream_t s) {
-    int gx = p.chw4 ? (p.H * p.T + 255) / 256 : (p.H * p.T + 127) / 128;
-    if (gx > 2048) gx = 2048;
-    k_final<<<dim3(gx, p.B), 256, 4 * p.C * sizeof(float), s>>>(p);
+    k_final<false><<<dim3(final_grid(p), p.B), 256, 4 * p.C * sizeof(float), s>>>(p, nullptr, nullptr);
+    return 1;
+}
+
+int launch_final_slot(const FinalParams& p, const SlotStep* cur, SlotSched* sched, cudaStream_t s) {
+    k_final<true><<<dim3(final_grid(p), p.B), 256, 4 * p.C * sizeof(float), s>>>(p, cur, sched);
+    return 1;
+}
+
+// the step's row of every slot: its t (the time table's input row b), its coefficients and its noise slab.  An idle or
+// finished slot gets t = 0.5 (any finite value: its row is computed and never read) and mode 0.
+__global__ void k_slot_begin(const SlotBeginParams p) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= p.B) return;
+    const SlotSched s = p.sched[b];
+    const bool live = s.i < s.n;
+    SlotStep c;
+    c.i = s.i;
+    c.mode = live ? (s.stoc ? 2 : 1) : 0;
+    c.noise = live && s.stoc ? s.noise + (long long)s.i * p.H * s.T : nullptr;
+    p.cur[b] = c;
+    p.t_rows[b] = live ? s.t_tab[s.i] : 0.5f;
+    p.coef[b] = live ? s.coef_tab[s.i] : make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+int launch_slot_begin(const SlotBeginParams& p, cudaStream_t s) {
+    k_slot_begin<<<(p.B + 127) / 128, 128, 0, s>>>(p);
+    return 1;
+}
+
+// xt0 = z * mask (diffusion.py:256) for one slot, as k_scale_mask computes it; mu and mask copied; 0 from T_b on
+__global__ void k_slot_write(const SlotWriteParams p) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= p.H * p.T) return;
+    const int h = i / p.T, w = i - h * p.T;
+    const bool in = p.z && w < p.Tb;
+    const float mk = in ? p.mask[w] : 0.f;
+    p.xt[i] = in ? p.z[h * p.Tb + w] * mk : 0.f;
+    p.mu_out[i] = in ? p.mu[h * p.Tb + w] : 0.f;
+    if (h == 0) p.mask_out[w] = mk;
+}
+
+int launch_slot_write(const SlotWriteParams& p, cudaStream_t s) {
+    k_slot_write<<<(p.H * p.T + 255) / 256, 256, 0, s>>>(p);
     return 1;
 }
 

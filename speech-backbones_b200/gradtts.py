@@ -272,6 +272,22 @@ class Diffusion(BaseModule):
     def forward(self, z, mask, mu, n_timesteps, stoc=False, spk=None, *, lengths=None):
         return self.reverse_diffusion(z, mask, mu, n_timesteps, stoc, spk, lengths=lengths)
 
+    def rolling(self, capacity, max_frames):
+        """A RollingSampler (rolling.py) of `capacity` slots at up to `max_frames` frames with this module's configuration,
+        precision and current weights: utterances join and leave a running batch at any step, each mel equal to its own
+        `forward` call.  The slot plan is a native plan of its own, so the sampler holds an engine of its own and this
+        module's `forward` calls stay usable alongside it; weights changed later are not seen by the sampler."""
+        from .rolling import RollingSampler
+        dev = next(self.parameters()).device
+        if dev.type != "cuda":
+            raise RuntimeError("Diffusion sampling runs only on a CUDA device (sm_90a); move the module with "
+                               ".cuda() first - there is no CPU fallback")
+        eng = Engine(self.n_feats, self.dim, self.n_spks, self.spk_emb_dim, self.beta_min, self.beta_max, self.pe_scale,
+                     device=dev.index, precision=self.precision, use_graph=self.use_graph)
+        with torch.cuda.device(dev):
+            eng.load_state_dict({"estimator." + k: v for k, v in self.estimator.state_dict().items()})
+            return RollingSampler(eng, capacity, max_frames)
+
     @torch.no_grad()
     def forward_host(self, z, mask, mu, n_timesteps, stoc=False, spk=None):
         """Same call for HOST tensors (pinned for async copies): H2D, loop, D2H inside libsbk."""
