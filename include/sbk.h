@@ -411,6 +411,19 @@ int sbk_postnet_forward_lengths(sbk_postnet* p, const float* x, const float* mas
                                 int n_feats, int T, void* stream);
 /* kernel launches (and memsets) the last sbk_postnet_forward enqueued */
 int64_t sbk_postnet_last_launch_count(const sbk_postnet* p);
+/* test hook: with capture on, sbk_postnet_forward copies every intermediate right after the launch that wrote it into a
+ * per-name device buffer (the copies do not count as launches; outputs and kernels are unchanged).  Names in launch order:
+ * a0 (init_conv(x*mask)*mask), block1.raw (7x7 conv output), block1.stats ([B][groups][2] float64 sums of x and x^2),
+ * block1.act (Mish(GN(raw)) * mask), block2.raw, block2.stats, res (the residual conv's output, final_conv's input).  The
+ * call's own output is not copied.  All are whole [B, n_feats, T] grids, past a ragged batch's edges included. */
+int sbk_postnet_debug_capture(sbk_postnet* p, int on);
+int sbk_postnet_debug_num(const sbk_postnet* p);
+const char* sbk_postnet_debug_name(const sbk_postnet* p, int i);
+/* 1 = fp32 [B][n_feats][dim/4][T][4], 3 = float64 array, -1 = no such name */
+int sbk_postnet_debug_op_layout(const sbk_postnet* p, const char* name);
+/* copy a snapshot to `dst` (host or device) in its own dtype (float64 for layout 3, else fp32); returns its element count
+ * through *numel; dst may be NULL to query it */
+int sbk_postnet_debug_read(sbk_postnet* p, const char* name, void* dst, int64_t* numel);
 
 const char* sbk_last_error(void);
 const char* sbk_version(void);

@@ -120,6 +120,8 @@ struct sbk_postnet {
     Workspace ws;
     bool is_packed = false;
     int64_t last_launches = 0;
+    // debug capture (fmt: 1 fp32 [B][H][C/4][T][4], 3 float64 [B][groups][2])
+    Snapshots snaps;
 };
 
 extern "C" int sbk_postnet_create(const sbk_postnet_config* cfg, sbk_postnet** out) {
@@ -226,6 +228,10 @@ extern "C" int sbk_postnet_forward_lengths(sbk_postnet* p, const float* x, const
         return fail(SBK_ERR_CUDA, "sbk_postnet_forward: the %s launch was refused (device attribute / geometry)", what);
     };
     int k;
+    // debug capture: raw and act are rewritten within the call, so each tensor is copied right after the launch that wrote it
+    const size_t px = (size_t)B * H * T * C;
+    p->snaps.begin();
+    auto snap = [&](const char* name, const void* src, size_t numel, int fmt) { p->snaps.record(name, src, numel, fmt, s); };
 
     CU(cudaMemsetAsync(st, 0, 2 * (size_t)B * kGroups * 2 * sizeof(double), s)); ++n;
     if (rag)
@@ -235,6 +241,7 @@ extern "C" int sbk_postnet_forward_lengths(sbk_postnet* p, const float* x, const
         k_pn_init<<<ew_grid((long long)B * H * (C / 4) * T), 256, 0, s>>>(x, mask, R("init_conv.weight"), R("init_conv.bias"), a0, B, H, C, T,
                                                                           x3 ? 0 : 1);
     ++n;
+    snap("a0", a0, px, 1);
     auto conv7 = [&](const char* blk, const float* in, double* ost) {
         ConvTcParams cp; memset(&cp, 0, sizeof(cp));
         const std::string q = std::string("res_block.") + blk + ".block.0.";
@@ -253,6 +260,8 @@ extern "C" int sbk_postnet_forward_lengths(sbk_postnet* p, const float* x, const
     };
     if ((k = conv7("block1", a0, st1)) < 0) return refused("block1 conv");
     n += k;
+    snap("block1.raw", raw, px, 1);
+    snap("block1.stats", st1, (size_t)B * kGroups * 2, 3);
     {
         GnActParams g; memset(&g, 0, sizeof(g));
         g.raw = raw; g.gn = gnref(st1, "block1"); g.tb = p->zero; g.tb_stride = 0; g.tb_per_sample = 1;
@@ -261,8 +270,11 @@ extern "C" int sbk_postnet_forward_lengths(sbk_postnet* p, const float* x, const
         if ((k = launch_gn_act(g, s)) < 0) return refused("block1 GroupNorm/Mish");
         n += k;
     }
+    snap("block1.act", act, px, 1);
     if ((k = conv7("block2", act, st2)) < 0) return refused("block2 conv");
     n += k;
+    snap("block2.raw", raw, px, 1);
+    snap("block2.stats", st2, (size_t)B * kGroups * 2, 3);
     {
         ConvTcParams cp; memset(&cp, 0, sizeof(cp));
         cp.geom = G_PW; cp.in0 = a0; cp.c0 = C; cp.H = H; cp.W = T; cp.B = B; cp.Ho = H; cp.Wo = T;
@@ -274,15 +286,36 @@ extern "C" int sbk_postnet_forward_lengths(sbk_postnet* p, const float* x, const
         if ((k = launch_conv_tc(cp, s)) < 0) return refused("residual conv");
         n += k;
     }
+    snap("res", act, px, 1);
     if (rag)
         k_pn_final_ragged<<<ew_grid((long long)B * H * T), 256, 0, s>>>(act, R("final_conv.weight"), R("final_conv.bias"), out, B, H, C, T,
                                                                         lengths);
     else
         k_pn_final<<<ew_grid((long long)B * H * T), 256, 0, s>>>(act, R("final_conv.weight"), R("final_conv.bias"), out, B, H, C, T);
     ++n;
+    if (const cudaError_t e = p->snaps.finish()) return fail(SBK_ERR_CUDA, "sbk_postnet_forward: debug capture failed: %s", cudaGetErrorString(e));
     CU(cudaGetLastError());
     p->last_launches = n;
     return SBK_OK;
 }
 
 extern "C" int64_t sbk_postnet_last_launch_count(const sbk_postnet* p) { return p ? p->last_launches : 0; }
+
+extern "C" int sbk_postnet_debug_capture(sbk_postnet* p, int on) {
+    if (!p) return fail(SBK_ERR_ARG, "sbk_postnet_debug_capture: null handle");
+    p->snaps.on = on != 0;
+    return SBK_OK;
+}
+extern "C" int sbk_postnet_debug_num(const sbk_postnet* p) { return p ? (int)p->snaps.list.size() : 0; }
+extern "C" const char* sbk_postnet_debug_name(const sbk_postnet* p, int i) {
+    if (!p || i < 0 || i >= (int)p->snaps.list.size()) return nullptr;
+    return p->snaps.list[i].name.c_str();
+}
+extern "C" int sbk_postnet_debug_op_layout(const sbk_postnet* p, const char* name) {
+    const Snapshots::Snap* sn = p && name ? p->snaps.find(name) : nullptr;
+    return sn ? sn->fmt : -1;
+}
+extern "C" int sbk_postnet_debug_read(sbk_postnet* p, const char* name, void* dst, int64_t* numel) {
+    if (!p || !name) return fail(SBK_ERR_ARG, "sbk_postnet_debug_read: null argument");
+    return p->snaps.read(name, dst, numel, p->cfg.device, "sbk_postnet_debug_read");
+}

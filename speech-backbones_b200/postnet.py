@@ -52,11 +52,18 @@ class PostNetEngine(_NativeHandle):
         self.lib.sbk_postnet_workspace_bytes.restype = C.c_size_t
         self.lib.sbk_postnet_forward.argtypes = [P, P, P, P, I, I, I, P]
         self.lib.sbk_postnet_forward_lengths.argtypes = [P, P, P, P, P, I, I, I, P]
+        self.lib.sbk_postnet_debug_capture.argtypes = [P, I]
+        self.lib.sbk_postnet_debug_num.argtypes = [P]
+        self.lib.sbk_postnet_debug_name.argtypes = [P, I]
+        self.lib.sbk_postnet_debug_name.restype = C.c_char_p
+        self.lib.sbk_postnet_debug_op_layout.argtypes = [P, C.c_char_p]
+        self.lib.sbk_postnet_debug_read.argtypes = [P, C.c_char_p, P, C.POINTER(C.c_int64)]
         rc = self._create(SbkPostNetConfig(device, dim, groups, PREC[precision]))
         if rc == _SBK_ERR_UNSUPPORTED:
             raise ValueError(self.lib.sbk_last_error().decode())
         _check(rc, "sbk_postnet_create")
         self.device, self.dim = device, dim
+        self._shape = None                               # (B, n_feats, T) of the last forward
 
     # Ragged batches: `lengths` (int64 [B] on x's device, each in 1..T, e.g. DiffVC's x_lengths) computes utterance b on its
     # own L_b frames, as the call on x[b:b+1, :, :L_b] would (sbk.h: sbk_postnet_forward_lengths): GroupNorm statistics and
@@ -77,7 +84,32 @@ class PostNetEngine(_NativeHandle):
         with torch.cuda.device(x.device):
             self._call(self.lib.sbk_postnet_forward_lengths, "sbk_postnet_forward", self.h, _ptr(x), _ptr(mask), _ptr(lengths),
                        _ptr(out), B, Fm, T, self._stream())
+        self._shape = (B, Fm, T)
         return out
+
+    # ---- test hooks: the intermediates of the last forward run with capture on (sbk_postnet_debug_*)
+    def debug_capture(self, on=True):
+        _check(self.lib.sbk_postnet_debug_capture(self.h, 1 if on else 0), "sbk_postnet_debug_capture")
+
+    def debug_names(self):
+        """Tensors the last forward captured, in launch order (sbk.h: sbk_postnet_debug_capture)."""
+        return [self.lib.sbk_postnet_debug_name(self.h, i).decode() for i in range(self.lib.sbk_postnet_debug_num(self.h))]
+
+    def debug_read(self, name):
+        """One captured tensor on the CPU: a0 / raw / act / res as NCHW fp32 [B, dim, n_feats, T], stats as float64
+        [B, groups, 2]."""
+        fmt = int(self.lib.sbk_postnet_debug_op_layout(self.h, name.encode()))
+        if fmt < 0:
+            raise RuntimeError(f"debug_read: no captured tensor named '{name}'")
+        n = C.c_int64(0)
+        _check(self.lib.sbk_postnet_debug_read(self.h, name.encode(), None, C.byref(n)), "sbk_postnet_debug_read")
+        out = torch.empty(n.value, dtype=torch.float64 if fmt == 3 else torch.float32)
+        _check(self.lib.sbk_postnet_debug_read(self.h, name.encode(), C.c_void_p(out.data_ptr()), C.byref(n)),
+               "sbk_postnet_debug_read")
+        B, H, T = self._shape
+        if fmt == 3:
+            return out.view(B, -1, 2)
+        return out.view(B, H, self.dim // 4, T, 4).permute(0, 2, 4, 1, 3).reshape(B, self.dim, H, T)
 
 
 class PostNet(BaseModule):

@@ -18,6 +18,9 @@ or one N tile stands out by orders of magnitude even where check 1's worst-case 
 `VocoderReplay` does the same for one HiFi-GAN vocoder call (oracle/hifigan_oracle.py semantics): its [B, C, L] signals
 are grouped by sample, 128-sample tile, within-tile phase and N-tile block (`uniformity1d`), and its elementwise kernels
 (mel layout, transposed-conv fold, LeakyReLU second outputs, MRF mean) must reproduce their fp32 arithmetic bit for bit.
+
+`RefBlockReplay` and `PostNetReplay` do the same for DiffVC's conditioning branch and PostNet.  With per-utterance lengths,
+`Replay`, `RefBlockReplay` and `PostNetReplay` judge each utterance of a ragged call on its own frames.
 """
 from __future__ import annotations
 
@@ -354,8 +357,8 @@ class Replay:
 
     model: "gradtts" (x, mask, mu, t, spk) or "diffvc" (x, mask, mean, t, cond).  `sd` is the state_dict the engine holds.
 
-    `lengths` (Grad-TTS only) makes it a ragged call (`Engine.estimator(..., lengths=)`), in which utterance b is the B = 1
-    call on its own T_b = fix_len_compatibility(lengths[b]) frames.  Each utterance is then judged on its own: the inputs
+    `lengths` makes it a ragged call (`Engine.estimator / vc_estimator(..., lengths=)`), in which utterance b is the B = 1
+    call on its own T_b = fix_len_compatibility(lengths[b]) frames, with its own t and spk (Grad-TTS) or cond (DiffVC) row.  Each utterance is then judged on its own: the inputs
     are sliced to row b and [:T_b], every capture is decoded at the call's dense shape and cropped to [b:b+1, ..., :W_b,l]
     (W_b,l = T_b >> l at level l), and the output to [b, :, :T_b].  The replay judges nothing past an utterance's edge;
     what the call left there is the caller's to check (e.g. that the output is 0)."""
@@ -367,13 +370,12 @@ class Replay:
         self.dim, self.pe_scale = dim, pe_scale
         d = torch.float64
         self.p = {k: v.to(dev, d) for k, v in sd.items()}
-        assert lengths is None or model == "gradtts", "only the Grad-TTS estimator takes lengths"
+        L = None if lengths is None else torch.as_tensor(lengths, dtype=torch.int64).cuda()
         eng.debug_capture(True)
         try:
             if model == "diffvc":
-                y = eng.vc_estimator(x.cuda(), mask.cuda(), mu.cuda(), cond.cuda(), t.cuda())
+                y = eng.vc_estimator(x.cuda(), mask.cuda(), mu.cuda(), cond.cuda(), t.cuda(), lengths=L)
             else:
-                L = None if lengths is None else torch.as_tensor(lengths, dtype=torch.int64).cuda()
                 y = eng.estimator(x.cuda(), mask.cuda(), mu.cuda(), t.cuda(), None if spk is None else spk.cuda(),
                                   lengths=L)
             torch.cuda.synchronize()
@@ -882,7 +884,9 @@ def rb_ntile(cout):
 
 
 def rb_chain(Tr):
-    """fp32 terms a k_chan_stats thread sums before it flushes to float64: 8 rows of ceil(Tr / 256) columns"""
+    """fp32 terms a k_chan_stats thread sums before it flushes to float64: 8 rows of ceil(Tr / 256) columns.  The ragged
+    twin keeps the dense call's partitions of the Tr columns and only drops those at or past R_b, so rb_chain(Tr) bounds its
+    chains too."""
     return 8 * math.ceil(Tr / 256)
 
 
@@ -1009,24 +1013,34 @@ def mish_layer(h, eh):
 
 class RefBlockReplay:
     """Run one sbk_vc_conditioning call with debug capture and judge every op of its last step against a float64 replay.
-    `sd` is the state_dict the engine holds; ref / mean_ref [B,H,Tr], ref_mask [B,1,Tr], c [B,256] (CPU fp32)."""
+    `sd` is the state_dict the engine holds; ref / mean_ref [B,H,Tr], ref_mask [B,1,Tr], c [B,256] (CPU fp32).
 
-    def __init__(self, eng, sd, precision, cfg, ref, ref_mask, mean_ref, c, n_timesteps, dev="cuda"):
+    `ref_lengths` makes it a ragged call (`vc_conditioning(..., ref_lengths=)`), in which reference b is the B = 1 call on
+    its own R_b frames with an all-ones mask.  Each reference is then judged on its own: the inputs and every capture are
+    cropped to [b:b+1, ..., :R_b], so the statistics, InstanceNorm and the masked mean normalise over H * R_b.  Nothing past
+    R_b is judged (the caller's mask there is not the reference's own)."""
+
+    def __init__(self, eng, sd, precision, cfg, ref, ref_mask, mean_ref, c, n_timesteps, dev="cuda", ref_lengths=None):
         self.eng, self.cfg, self.dev, self.N = eng, cfg, dev, n_timesteps
         self.mode = rb_branch_mode(precision)
+        RL = None if ref_lengths is None else torch.as_tensor(ref_lengths, dtype=torch.int64).cuda()
         eng.debug_capture(True)
         try:
-            self.table = eng.vc_conditioning(ref.cuda(), ref_mask.cuda(), mean_ref.cuda(), c.cuda(), n_timesteps)
+            self.table = eng.vc_conditioning(ref.cuda(), ref_mask.cuda(), mean_ref.cuda(), c.cuda(), n_timesteps,
+                                             ref_lengths=RL)
             torch.cuda.synchronize()
         finally:
             eng.debug_capture(False)
         self.names = eng.vc_cond_debug_names()
-        self.cap = {n: eng.vc_cond_debug_read(n).to(dev) for n in self.names}
         d = torch.float64
         self.p = {k: v.to(dev, d) for k, v in sd.items()}
-        self.ref, self.mean_ref, self.c = ref.to(dev, d), mean_ref.to(dev, d), c.to(dev, d)
-        self.mask = ref_mask[:, 0].to(dev, d)
-        self.B, self.H, self.Tr = ref.shape
+        self.full = {"cap": {n: eng.vc_cond_debug_read(n).to(dev) for n in self.names}, "ref": ref.to(dev, d),
+                     "mean_ref": mean_ref.to(dev, d), "c": c.to(dev, d), "mask": ref_mask[:, 0].to(dev, d),
+                     "table": self.table.to(dev, d)}
+        self.H, self.Tr = ref.shape[1], ref.shape[2]
+        # the units judged one by one: the whole call (None), or each reference (b, R_b) of a ragged one
+        self.units = [None] if ref_lengths is None else [(b, int(r)) for b, r in enumerate(ref_lengths)]
+        self.select(None)
         # the host's scalars of the last step: t as fp32(1 - i / N), gamma(0, t) in double from the fp32 config betas
         i = n_timesteps - 1
         td = 1.0 - i * (1.0 / n_timesteps)
@@ -1036,6 +1050,23 @@ class RefBlockReplay:
         bi *= td
         self.g = float(torch.tensor(math.exp(-0.5 * bi), dtype=torch.float32))
         self.base = cfg.dim_spk // 4
+
+    def select(self, unit):
+        """Judge `unit` = (b, R_b), reference b of a ragged call on its own frames, or (None) the whole call."""
+        f, self.unit = self.full, unit
+        if unit is None:
+            row, frames = (lambda v: v), (lambda v: v)
+            self.tag = ""
+        else:
+            b, R = unit
+            row, frames = (lambda v: v[b:b + 1]), (lambda v: v[b:b + 1, ..., :R])
+            self.tag = f" b={b} R={R}"
+        self.ref, self.mean_ref, self.mask = frames(f["ref"]), frames(f["mean_ref"]), frames(f["mask"])
+        self.c, self.table_last = row(f["c"]), row(f["table"][-1])
+        # stats / ysum [B, C, 2] are per sample; tb is one row for the batch; the rest are [B, (C,) H, Tr] grids
+        self.cap = {n: (row(v) if n.endswith((".stats", ".ysum")) else v if n == "ref_block.tb" else frames(v))
+                    for n, v in f["cap"].items()}
+        self.B = self.ref.shape[0]
 
     def _w(self, blk, part):
         return self.p[f"estimator.ref_block.{blk}.{part}"]
@@ -1084,16 +1115,26 @@ class RefBlockReplay:
                           p["estimator.cond_block.0.bias"])
         h, e = mish_layer(h, e)
         ref, bound = ffma_layer(h, e, p["estimator.cond_block.2.weight"], p["estimator.cond_block.2.bias"])
-        return check(self.table[-1].to(dev, torch.float64), ref, bound, 1.0, groups=False)
+        return check(self.table_last, ref, bound, 1.0, groups=False)
 
     def run(self):
-        """-> rows (name, elem, unif, where); raises on a captured name this replay does not know, and on a non-zero act
-        past the mask.  Also -> self.var_err: {block: worst relative error of the variance from the captured sums}."""
-        rows, self.var_err = [], {}
+        """-> rows (name, elem, unif, where), per judged unit (the call, or each reference: its name carries b and R_b);
+        raises on a captured name this replay does not know, and on a non-zero act past the mask.  Also -> self.var_err:
+        {block (+ unit): worst relative error of the variance from the captured sums}.  self.nonfinite lists the judged
+        (cropped) captures that hold a NaN or Inf."""
+        rows, self.var_err, self.nonfinite = [], {}, []
         known = {"ref_block.xt_ref", "ref_block.tb", "ref_block.ysum"}
         known |= {f"ref_block.{b}.{s}" for b in RB_BLOCKS for s in ("raw", "stats", "act")}
         for name in self.names:
             assert name in known, f"unknown RefBlock op '{name}': add a replay for it"
+        for unit in self.units:
+            self.select(unit)
+            self.nonfinite += [n + self.tag for n, v in self.cap.items() if not bool(torch.isfinite(v).all())]
+            rows += [(n + self.tag,) + tuple(r) for n, *r in self._run_unit()]
+        return rows
+
+    def _run_unit(self):
+        rows = []
         if self.cfg.use_ref_t:
             assert self.names[:2] == ["ref_block.xt_ref", "ref_block.tb"] and self.names[-1] == "ref_block.ysum", self.names
             rows.append(("xt_ref",) + self.xt_ref())
@@ -1105,7 +1146,7 @@ class RefBlockReplay:
                                                      self.mode, first=blk == "block11"))
                 st = self.cap[f"ref_block.{blk}.stats"]
                 rows.append((f"{blk}.stats",) + rb_stats(raw, st, self.Tr))
-                self.var_err[blk] = rb_var_error(raw, st)
+                self.var_err[blk + self.tag] = rb_var_error(raw, st)
                 tb = None
                 if blk in RB_TBIAS:
                     lo, hi = RB_TBIAS[blk]
@@ -1119,4 +1160,177 @@ class RefBlockReplay:
         else:
             assert not self.names, f"use_ref_t = False captured {self.names}"
         rows.append(("cond",) + self.cond())
+        return rows
+
+
+# ---- DiffVC's PostNet (csrc/sbk_postnet.cu), replayed op by op --------------------------------------------------------------
+# One sbk_postnet_forward call with capture on keeps a0, each block's conv output (raw) and GroupNorm sums (stats), block1's
+# Mish(GN) activation, and the residual conv's output (res); the call's own output is the last op.  Each is recomputed in
+# float64 from the GPU's own captured inputs with the semantics of oracle/postnet_oracle.py.  fp32x3 / fp32 handles run the
+# fp32x3 split, tf32 / bf16 handles tf32 operands (rb_branch_mode).
+PN_GROUPS = 8
+# fp32 roundings a GroupNorm partial sees before its float64 flush (sbk_conv_tc.cu, the epilogue's statistics): an 8-term
+# chain, the 8 -> group-width merge (<= 2), the 32-lane shuffle (5), and the tile's 32-column chunks and passes (<= 8)
+PN_STATS_CHAIN = 32
+# k_pn_init: one fma, the exact mask product, and on tf32 handles the rna rounding of the stored operand (<= 2^-11 of the
+# value; a value just above a power of two attains it, so tf32 a0 rows measure up to 0.999 of this bound on an H100)
+PN_A0_TF32 = 2 ** -11
+
+
+def pn_ntile(C, mode, geom):
+    """N tile of the PostNet's wgmma convs (sbk_conv_tc.cu conv_tc_ntile): the 7x7 runs 64 wide in fp32x3"""
+    if geom == "c7" and mode == "fp32x3":
+        return 64
+    return 128 if C % 128 == 0 else 64
+
+
+def pn_inv_count(C, H, L):
+    """the GroupNorm divisor the kernels use: fp32(1 / ((C/8) H L)), for a ragged sample from fp32((C/8) * H) (gn_inv_count_rag)
+    - the same value as the dense fp32(1.0 / ((double)(C/8) * H * T)) at L = T"""
+    cnt = float(torch.tensor(float(C // PN_GROUPS), dtype=torch.float32) * torch.tensor(float(H), dtype=torch.float32))
+    return float(torch.tensor(1.0 / (cnt * L), dtype=torch.float32))
+
+
+def pn_gn_mish(raw, stats, gamma, beta, inv):
+    """Block's GroupNorm(8) + Mish on raw [B,C,H,W] from the GPU's captured sums `stats` [B,8,2] and the kernels' fp32 divisor
+    `inv`, as gn_mean_rstd forms them: mean = s inv and var = ss inv - mean^2 in float64, mean and rstd * gamma rounded to
+    fp32 (the sums themselves are judged by pn_stats) -> (value, companion 1.1 (|raw - mean| |scale| + |beta|))"""
+    C = raw.shape[1]
+    mean = stats[..., 0] * inv
+    var = (stats[..., 1] * inv - mean * mean).clamp_min(0.0)
+    rstd = _f32(1.0 / torch.sqrt(var + 1e-5))
+    cpg = C // PN_GROUPS
+    mean = _f32(mean).repeat_interleave(cpg, 1)[:, :, None, None]
+    scale = _f32(rstd.repeat_interleave(cpg, 1) * _f32(gamma)[None])[:, :, None, None]
+    y = (raw - mean) * scale + beta[None, :, None, None]
+    return O.mish(y), 1.1 * ((raw - mean).abs() * scale.abs() + beta.abs()[None, :, None, None])
+
+
+def pn_stats(raw, got):
+    """[B, 8, 2] sums of x and x^2 over each group's channels and all H * W pixels of raw [B,C,H,W]"""
+    B = raw.shape[0]
+    g = raw.reshape(B, PN_GROUPS, -1)
+    ref = torch.stack([g.sum(-1), (g * g).sum(-1)], -1)
+    A = torch.stack([g.abs().sum(-1), (g * g).sum(-1)], -1)
+    return check(got, ref, A, PN_STATS_CHAIN * U32 + g.shape[-1] * 2 ** -53, groups=False)
+
+
+PN_NO_UNIFORMITY = {
+    "a0": "elementwise (k_pn_init, no tiles); held to its per-element bound",
+    "stats": "one pair of sums per (sample, group); no columns or rows",
+    "act.tf32": "the replay is rounded to tf32 as k_gn_act rounds, so the error is a sparse set of one-step differences",
+}
+
+
+class PostNetReplay:
+    """Run one PostNet forward with debug capture and judge every captured op, and the output, against a float64 replay.
+    `eng` is a PostNetEngine loaded with `sd`; x [B,H,T], mask [B,1,T] (CPU fp32).
+
+    `lengths` makes it a ragged call (`forward(..., lengths=)`), in which utterance b is the B = 1 call on its own L_b
+    frames with an all-ones mask (no rounding of the length).  Each utterance is then judged on its own: every capture and
+    the output are cropped to [b:b+1, ..., :L_b], and the GroupNorm count is (C/8) H L_b."""
+
+    def __init__(self, eng, sd, precision, x, mask, lengths=None, dev="cuda"):
+        self.eng, self.dev = eng, dev
+        self.mode = rb_branch_mode(precision)
+        L = None if lengths is None else torch.as_tensor(lengths, dtype=torch.int64).to(dev)
+        eng.debug_capture(True)
+        try:
+            y = eng.forward(x.to(dev), mask.to(dev), L)
+            if y.is_cuda:
+                torch.cuda.synchronize()
+        finally:
+            eng.debug_capture(False)
+        self.names = eng.debug_names()
+        d = torch.float64
+        self.p = {k: v.to(dev, d) for k, v in sd.items()}
+        self.full = {"cap": {n: eng.debug_read(n).to(dev, d) for n in self.names}, "y": y.to(dev, d), "x": x.to(dev, d),
+                     "mask": mask.to(dev, d)}
+        self.C = self.p["init_conv.weight"].shape[0]
+        self.units = [None] if lengths is None else [(b, int(n)) for b, n in enumerate(lengths)]
+        self.select(None)
+
+    def select(self, unit):
+        f, self.unit = self.full, unit
+        if unit is None:
+            frames, self.tag = (lambda v: v), ""
+            self.mask = f["mask"][:, :, None]                                  # [B, 1, 1, T]
+        else:
+            b, L = unit
+            frames, self.tag = (lambda v: v[b:b + 1, ..., :L]), f" b={b} L={L}"
+            self.mask = torch.ones(1, 1, 1, L, dtype=torch.float64, device=self.dev)
+        self.cap = {n: (v[unit[0]:unit[0] + 1] if unit is not None else v) if n.endswith(".stats") else frames(v)
+                    for n, v in f["cap"].items()}
+        self.x, self.y = frames(f["x"]), frames(f["y"])
+        self.B, self.H, self.T = self.x.shape
+
+    def a0(self):
+        m = self.mask
+        w, b = self.p["init_conv.weight"], self.p["init_conv.bias"]
+        x = self.x[:, None] * m
+        ref = (F.conv2d(x, w, b)) * m
+        A = (F.conv2d(x.abs(), w.abs(), b.abs())) * m
+        k = 2 * U32 + (PN_A0_TF32 if self.mode == "tf32" else 0.0)
+        return check(self.cap["a0"], ref, A, k, groups=False)
+
+    def conv7(self, blk, xin):
+        """blockN.raw: Conv2d 7x7 (padding 3) of the captured input times the mask, + bias: wgmma, K = 49 C (42-MMA fp32x3
+        runs).  Uniformity over columns, rows, the conv's N tiles and the phase within its 128-pixel tile."""
+        q = f"res_block.{blk}.block"
+        w, b = self.p[f"{q}.0.weight"], self.p[f"{q}.0.bias"]
+        ref, A, floor, Alin = _lin(F.conv2d, xin * self.mask, w, b, padding=3)
+        k = kappa(self.mode, 49 * w.shape[1], run=42)
+        return check(self.cap[f"block{blk[-1]}.raw"], ref, A, k, floor, Alin, ntile=pn_ntile(self.C, self.mode, "c7"),
+                     period=TC_TILE)
+
+    def act1(self):
+        """block1.act = Mish(GN(raw1)) * mask (k_gn_act; tf32 handles round it to tf32 rna)"""
+        q = "res_block.block1.block.1"
+        raw = self.cap["block1.raw"]
+        h, hA = pn_gn_mish(raw, self.cap["block1.stats"], self.p[f"{q}.weight"], self.p[f"{q}.bias"],
+                           pn_inv_count(self.C, self.H, self.T))
+        ref, A = h * self.mask, hA * self.mask
+        if self.mode == "tf32":
+            ref = round_tf32_rna(ref.float()).double()
+        k = IN_GLU_ROUNDINGS * U32 + EPS_NL + (2 ** -10 if self.mode == "tf32" else 0.0)
+        valid = self.mask.expand_as(ref)
+        return check(self.cap["block1.act"], ref, A, k, groups=self.mode != "tf32", min_group=RB_MIN_VALID, valid=valid)
+
+    def res(self):
+        """res = (res_conv(a0 * mask) + Mish(GN(raw2)) * mask) * mask: the EPI_RES 1x1 (K = C) and its fp32 GN + Mish term"""
+        q = "res_block.block2.block.1"
+        h, hA = pn_gn_mish(self.cap["block2.raw"], self.cap["block2.stats"], self.p[f"{q}.weight"], self.p[f"{q}.bias"],
+                           pn_inv_count(self.C, self.H, self.T))
+        m = self.mask
+        r, Ar, floor, Alin = _lin(F.conv2d, self.cap["a0"] * m, self.p["res_block.res.weight"], self.p["res_block.res.bias"])
+        ref, A, Alin = (r + h * m) * m, (Ar + hA * m) * m, (Alin + hA * m) * m
+        k = kappa(self.mode, self.C, nl=True)
+        return check(self.cap["res"], ref, A, k, floor, Alin, ntile=pn_ntile(self.C, self.mode, "pw"))
+
+    def out(self):
+        """the call's output: final_conv(res) + bias, an fp32 FFMA chain of C terms from 0, then the bias add"""
+        w, b = self.p["final_conv.weight"], self.p["final_conv.bias"]
+        ref, A, floor, Alin = _lin(F.conv2d, self.cap["res"], w, b)
+        return check(self.y[:, None], ref, A, kappa("fp32", self.C + 1), floor, Alin)
+
+    def run(self):
+        """-> rows (name, elem, unif, where) per judged unit (the call, or each utterance: its name carries b and L_b);
+        raises on a captured name this replay does not know.  self.nonfinite lists judged captures holding a NaN / Inf."""
+        want = ["a0", "block1.raw", "block1.stats", "block1.act", "block2.raw", "block2.stats", "res"]
+        assert self.names == want, f"PostNet captures {self.names}, the replay knows {want}"
+        rows, self.nonfinite = [], []
+        for unit in self.units:
+            self.select(unit)
+            self.nonfinite += [n + self.tag for n, v in self.cap.items() if not bool(torch.isfinite(v).all())]
+            if not bool(torch.isfinite(self.y).all()):
+                self.nonfinite.append("out" + self.tag)
+            r = [("a0",) + self.a0(),
+                 ("block1.raw",) + self.conv7("block1", self.cap["a0"]),
+                 ("block1.stats",) + pn_stats(self.cap["block1.raw"], self.cap["block1.stats"]),
+                 ("block1.act",) + self.act1(),
+                 ("block2.raw",) + self.conv7("block2", self.cap["block1.act"]),
+                 ("block2.stats",) + pn_stats(self.cap["block2.raw"], self.cap["block2.stats"]),
+                 ("res",) + self.res(),
+                 ("out",) + self.out()]
+            rows += [(n + self.tag,) + tuple(v) for n, *v in r]
         return rows

@@ -9,8 +9,8 @@ import torch
 import torch.nn.functional as F
 
 from helpers import rel_l2
-from op_replay import (FIRST_CONV_TILE, FLOOR_PER_W, R_UNIFORM, TC_TILE, _gn_mish, check, crop_utterance, ct_fold, ctx_replay,
-                       kappa, passes, rb_act, rb_conv)
+from op_replay import (FIRST_CONV_TILE, FLOOR_PER_W, R_UNIFORM, TC_TILE, PostNetReplay, _gn_mish, check, crop_utterance,
+                       ct_fold, ctx_replay, kappa, passes, pn_inv_count, rb_act, rb_conv, rb_stats)
 from oracle import gradtts_oracle as O
 from oracle.precision_model import fp32x3_product, round_bf16, round_tf32_rna, trunc_tf32
 
@@ -561,3 +561,173 @@ def test_ragged_attention_padded_pixels_in_softmax_fail(ragged_attn, mode):
     elem, unif, where = rows[1]
     print(f"{mode} ragged ctx padded pixels in softmax b=1 W={RW[1]}: |err|/(kappa A) max {elem:.3g}")
     assert passes(*rows[0][:2]) and elem > 2 and not passes(elem, unif)
+
+
+# ---- a ragged RefBlock row: reference 0 on its own R = RB_LEN frames of the Tr = RB_TR image (RefBlockReplay crops every
+# capture to [b:b+1, ..., :R_b], so its statistics and InstanceNorm normalise over H * R_b).  Past R the dense image holds the
+# conv of the whole row (a stale, finite value).
+def rb_ragged(s):
+    """(raw of the reference's own call [.., :R], the dense image's raw, the stats k_chan_stats_ragged writes)"""
+    R = RB_LEN
+    x = s["x"][..., :R]
+    raw = rb_emulate_conv(dict(s, x=x))
+    dense = rb_emulate_conv(dict(s, x=s["x"] + (s["mask"] == 0)[:, None, None, :].double()))
+    return raw, dense
+
+
+def rb_ragged_in_glu(raw, s, n_cols):
+    """k_in_glu_ragged on the reference's own columns, the InstanceNorm divisor H * n_cols"""
+    C = raw.shape[1]
+    n = raw.shape[2] * n_cols
+    m = raw.sum((2, 3)) / n
+    var = ((raw * raw).sum((2, 3)) / n - m * m).clamp_min(0)
+    mean = m.float()[:, :, None, None]
+    scale = ((1.0 / torch.sqrt(var + 1e-5)).float() * s["gamma"].float()[None])[:, :, None, None]
+    xn = (raw.float() - mean) * scale + s["beta"].float()[None, :, None, None]
+    y = xn[:, :C // 2] * torch.sigmoid(xn[:, C // 2:]) + s["tb"].float()[None, :, None, None]
+    return round_tf32_rna(y).double()
+
+
+def rb_judge_ragged(s, raw, stats, act):
+    ones = torch.ones(1, raw.shape[-1], dtype=torch.float64)
+    return {"stats": rb_stats(raw, stats, RB_TR), "act": rb_act(raw, s["gamma"], s["beta"], s["tb"], ones, act, "tf32")}
+
+
+def _sums(raw):
+    return torch.stack([raw.sum((2, 3)), (raw * raw).sum((2, 3))], -1)
+
+
+def test_refblock_ragged_clean_passes(rb_stage):
+    s = rb_stage
+    raw, _ = rb_ragged(s)
+    for k, (elem, unif, where) in rb_judge_ragged(s, raw, _sums(raw), rb_ragged_in_glu(raw, s, RB_LEN)).items():
+        print(f"refblock ragged clean {k}: |err|/(kappa A) max {elem:.3f}, uniformity {unif:.2f} at {where}")
+        assert passes(elem, unif), (k, elem, unif, where)
+
+
+def test_refblock_ragged_divisor_from_tr_fails(rb_stage):
+    """k_in_glu_ragged divides the reference's sums by H * Tr instead of H * R_b: the mean and variance shrink by R_b / Tr
+    (280 / 300), which check 1 sees at nearly every element: act fails by ~27x."""
+    s = rb_stage
+    raw, _ = rb_ragged(s)
+    rows = rb_judge_ragged(s, raw, _sums(raw), rb_ragged_in_glu(raw, s, RB_TR))
+    elem, unif, _ = rows["act"]
+    print(f"refblock ragged divisor H*Tr: act |err|/(kappa A) max {elem:.3g}")
+    assert passes(*rows["stats"][:2]) and elem > 10 and not passes(elem, unif)
+
+
+def test_refblock_ragged_stats_one_column_late_fails(rb_stage):
+    """k_chan_stats_ragged sums column R_b (the dense image's value there) too: one column of H in H * R_b terms, an error of
+    ~1 / R_b of the sums against a bound of rb_chain(Tr) * 2^-24 ~ 1e-6 of them; stats fail by ~3e4x."""
+    s = rb_stage
+    raw, dense = rb_ragged(s)
+    stats = _sums(raw) + _sums(dense[..., RB_LEN:RB_LEN + 1])
+    elem, unif, _ = rb_judge_ragged(s, raw, stats, rb_ragged_in_glu(raw, s, RB_LEN))["stats"]
+    print(f"refblock ragged stats one column late: |err|/(kappa A) max {elem:.3g}")
+    assert elem > 100 and not passes(elem, unif)
+
+
+# ---- a ragged PostNet: dim 32 on an 8 x 40 grid, utterances of 40 and 13 frames, driven through PostNetReplay ----------------
+# The emulation computes utterance b's own call on its L_b frames in fp32, with k_pn_init's and k_gn_act's tf32 (rna) stores
+# on tf32 handles and the kernels' GroupNorm divisor; every capture past L_b is NaN, as a poisoned workspace leaves it.
+PN_C, PN_H, PN_T, PN_LENS = 32, 8, 40, [40, 13]
+
+
+class PostNetEmulation:
+    """the engine surface PostNetReplay drives.  defect: "stale_third_zero_column" - utterance 1's block1 conv reads input
+    column L_b + 2 (the third of the 7x7's zero columns) from the dense image; "gn_count_from_T" - utterance 1's GroupNorm
+    divides by (C/8) H T instead of (C/8) H L_b."""
+
+    def __init__(self, sd, tf32, defect=None):
+        self.p, self.tf32, self.defect = {k: v.float() for k, v in sd.items()}, tf32, defect
+
+    def debug_capture(self, on):
+        pass
+
+    def debug_names(self):
+        return list(self.cap)
+
+    def debug_read(self, name):
+        return self.cap[name]
+
+    def forward(self, x, mask, lengths):
+        p, B, H, T = self.p, x.shape[0], x.shape[1], x.shape[2]
+        rnd = round_tf32_rna if self.tf32 else (lambda v: v)
+        big = {k: torch.full((B, PN_C, H, T), float("nan")) for k in ("a0", "block1.raw", "block1.act", "block2.raw", "res")}
+        stats = {k: torch.zeros(B, 8, 2, dtype=torch.float64) for k in ("block1.stats", "block2.stats")}
+        y = torch.zeros(B, H, T)
+        for b, L in enumerate(lengths.tolist()):
+            bad = b == 1
+            a0_row = rnd(F.conv2d(torch.nan_to_num(x[b:b + 1, None], 1.0), p["init_conv.weight"], p["init_conv.bias"]))
+            a0 = a0_row[..., :L]
+
+            def block(i, inp):
+                q = f"res_block.block{i}.block"
+                w, bias = p[f"{q}.0.weight"], p[f"{q}.0.bias"]
+                if i == 1 and bad and self.defect == "stale_third_zero_column":
+                    inp = torch.cat([inp, torch.zeros_like(a0_row[..., :3])], -1)
+                    inp[..., L + 2] = a0_row[..., L + 2]
+                    raw = F.conv2d(F.pad(inp, (3, 0, 3, 3)), w, bias)
+                else:
+                    raw = F.conv2d(inp, w, bias, padding=3)
+                g = raw.double().reshape(1, 8, -1)
+                st = torch.stack([g.sum(-1), (g * g).sum(-1)], -1)
+                inv = pn_inv_count(PN_C, H, T if bad and self.defect == "gn_count_from_T" else L)
+                mean = st[..., 0] * inv
+                var = (st[..., 1] * inv - mean * mean).clamp_min(0.0)
+                cpg = PN_C // 8
+                mean_f = mean.float().repeat_interleave(cpg, 1)[:, :, None, None]
+                sc = ((1.0 / torch.sqrt(var + 1e-5)).float().repeat_interleave(cpg, 1) * p[f"{q}.1.weight"][None])[:, :, None, None]
+                return raw, st, F.mish((raw - mean_f) * sc + p[f"{q}.1.bias"][None, :, None, None])
+            r1, s1, h1 = block(1, a0)
+            h1 = rnd(h1)
+            r2, s2, h2 = block(2, h1)
+            res = F.conv2d(a0, p["res_block.res.weight"], p["res_block.res.bias"]) + h2
+            for k, v in (("a0", a0), ("block1.raw", r1), ("block1.act", h1), ("block2.raw", r2), ("res", res)):
+                big[k][b:b + 1, ..., :L] = v
+            stats["block1.stats"][b], stats["block2.stats"][b] = s1[0], s2[0]
+            y[b, :, :L] = F.conv2d(res, p["final_conv.weight"], p["final_conv.bias"])[0, 0]
+        names = ("a0", "block1.raw", "block1.stats", "block1.act", "block2.raw", "block2.stats", "res")
+        self.cap = {k: big.get(k, stats.get(k)) for k in names}
+        return y
+
+
+def _pn_rows(precision, defect=None):
+    from speech_backbones_b200.spec import synthetic_postnet_state_dict
+    sd = synthetic_postnet_state_dict(PN_C, 29)
+    x = torch.randn(len(PN_LENS), PN_H, PN_T, generator=torch.Generator().manual_seed(31))
+    for b, L in enumerate(PN_LENS):
+        x[b, :, L:] = float("nan")
+    rp = PostNetReplay(PostNetEmulation(sd, precision == "tf32", defect), sd, precision, x,
+                       torch.ones(len(PN_LENS), 1, PN_T), lengths=PN_LENS, dev="cpu")
+    return {r[0]: r[1:] for r in rp.run()}, rp.nonfinite
+
+
+@pytest.mark.parametrize("precision", ["tf32", "fp32x3"])
+def test_postnet_ragged_clean_passes(precision):
+    rows, nonfinite = _pn_rows(precision)
+    assert not nonfinite
+    for k, (elem, unif, where) in rows.items():
+        print(f"postnet {precision} clean {k}: |err|/(kappa A) max {elem:.3f}, uniformity {unif:.2f} at {where}")
+        assert passes(elem, unif), (k, elem, unif, where)
+
+
+@pytest.mark.parametrize("precision", ["tf32", "fp32x3"])
+def test_postnet_stale_third_zero_column_fails(precision):
+    """utterance 1's 7x7 conv reads input column L_b + 2 from the image instead of as zero: only output column L_b - 1 (the
+    utterance's border, which check 2 leaves out) sees it, through one kernel column; check 1 fails it by ~40x (tf32) and
+    ~5e3x (fp32x3), and utterance 0 still passes."""
+    rows, _ = _pn_rows(precision, "stale_third_zero_column")
+    elem, unif, _ = rows["block1.raw b=1 L=13"]
+    print(f"postnet {precision} stale third zero column: |err|/(kappa A) max {elem:.3g}")
+    assert passes(*rows["block1.raw b=0 L=40"][:2]) and elem > 10 and not passes(elem, unif)
+
+
+@pytest.mark.parametrize("precision", ["tf32", "fp32x3"])
+def test_postnet_group_norm_count_from_t_fails(precision):
+    """utterance 1's GroupNorm divides by (C/8) H T instead of (C/8) H L_b: its mean and variance shrink by 13 / 40, which
+    check 1 sees at every element of block1.act (fails by ~2e4x in tf32, ~2e6x in fp32x3)."""
+    rows, _ = _pn_rows(precision, "gn_count_from_T")
+    elem, unif, _ = rows["block1.act b=1 L=13"]
+    print(f"postnet {precision} GroupNorm count from T: |err|/(kappa A) max {elem:.3g}")
+    assert passes(*rows["block1.act b=0 L=40"][:2]) and elem > 100 and not passes(elem, unif)

@@ -74,7 +74,8 @@ def test_postnet_handle_weight_inventory_is_the_modules(sbk_lib):
     from speech_backbones_b200.postnet import PostNet, PostNetEngine
     for sym in ("sbk_postnet_create", "sbk_postnet_destroy", "sbk_postnet_num_weights", "sbk_postnet_weight_name",
                 "sbk_postnet_set_weight", "sbk_postnet_pack", "sbk_postnet_workspace_bytes", "sbk_postnet_forward",
-                "sbk_postnet_last_launch_count"):
+                "sbk_postnet_last_launch_count", "sbk_postnet_debug_capture", "sbk_postnet_debug_num", "sbk_postnet_debug_name",
+                "sbk_postnet_debug_op_layout", "sbk_postnet_debug_read"):
         assert hasattr(sbk_lib, sym), sym
     for dim in (64, 128, 256):
         e = PostNetEngine(dim)
