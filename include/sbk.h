@@ -370,7 +370,22 @@ int sbk_textenc_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengt
 /* MelEncoder.forward(x, x_mask) (DiffVC/model/encoder.py:279-284, called at DiffVC/model/vc.py:39,45): x [B,n_feats,T],
  * x_mask [B,1,T] in {0,1} -> out [B,n_feats,T] (the "average voice" mel; not masked, as in the reference).  kind = 1 handles. */
 int sbk_melenc_forward(sbk_textenc* e, const float* x, const float* x_mask, float* out, int B, int T, void* stream);
+/* Both forwards check every argument, the attention kernel's sequence limit included (SBK_ERR_UNSUPPORTED once
+ * 8 * (d + Tx rounded up to 4 + 32) floats exceed 200 KB, i.e. Tx > 6272 at head dim 96), before anything is launched or
+ * written. */
 int64_t sbk_textenc_last_launch_count(const sbk_textenc* e);
+/* test hook: with capture on, both forwards copy every tensor right after the launch that wrote it into a per-name device
+ * buffer (the copies do not count as launches; outputs and kernels are unchanged).  Names in launch order: mask (text
+ * encoder only: x_mask [B][Tx]), embed (emb(x) * sqrt(C)) or init_proj (mel encoder), prenet.{0,1,2}, prenet.proj,
+ * spk_concat (n_spks > 1), then per layer i: enc.i.qkv (q | k | v), enc.i.attn (attention before conv_o), enc.i.ln1,
+ * enc.i.ffn1 (relu(conv_1) * mask), enc.i.ln2; then mu, dp.1, dp.2, logw (text encoder) or out (mel encoder). */
+int sbk_textenc_debug_capture(sbk_textenc* e, int on);
+int sbk_textenc_debug_num(const sbk_textenc* e);
+const char* sbk_textenc_debug_name(const sbk_textenc* e, int i);
+/* 0 = token-major fp32 [B][Tx][C], 1 = planar fp32 [B][C][Tx] (mu, logw, out), -1 = no such name */
+int sbk_textenc_debug_op_layout(const sbk_textenc* e, const char* name);
+/* copy a snapshot to `dst` (host or device) as fp32; returns its element count through *numel; dst may be NULL to query it */
+int sbk_textenc_debug_read(sbk_textenc* e, const char* name, void* dst, int64_t* numel);
 
 /* ---- DiffVC's PostNet: the second half of the "average voice" encoder --------------------------------------------------
  * FwdDiffusion (DiffVC/model/vc.py:19-48) is MelEncoder (above, kind = 1) followed by PostNet (DiffVC/model/postnet.py:40-53):

@@ -42,11 +42,13 @@ def param_spec(n_vocab=149, n_feats=80, ch=192, filt=768, filt_dp=256, n_layers=
     return s
 
 
-def synthetic_weights(seed, spk_extra=0):
-    """Seeded stand-in weights (the reference ships no Grad-TTS checkpoint): 1/sqrt(fan_in) scales, LayerNorm gains near 1."""
+def synthetic_weights(seed, spk_extra=0, **config):
+    """Seeded stand-in weights (the reference ships no Grad-TTS checkpoint): 1/sqrt(fan_in) scales, LayerNorm gains near 1.
+    `config`: param_spec's shape arguments (n_heads, kernel, window, filt, ...); each tensor depends only on the seed, its
+    name and its shape, so the defaults give Grad-TTS's tensors."""
     from speech_backbones_b200.spec import synthetic_tensor
     sd = {}
-    for name, shape in param_spec(spk_extra=spk_extra):
+    for name, shape in param_spec(spk_extra=spk_extra, **config):
         if name.endswith(".gamma"):
             sd[name] = 1.0 + 0.1 * synthetic_tensor(seed, "textenc/" + name, shape)
         elif name.endswith((".beta", ".bias")):
@@ -66,7 +68,7 @@ def layer_norm(x, gamma, beta, eps=1e-4):
 
 
 def rel_attention(p, pre, x, mask, n_heads, window):
-    """MultiHeadAttention.forward for self-attention (:133-171), eval mode."""
+    """MultiHeadAttention.forward for self-attention (:133-171), eval mode, in x's dtype and on x's device."""
     b, ch, t = x.shape
     d = ch // n_heads
     q = F.conv1d(x, p[f"{pre}.conv_q.weight"], p[f"{pre}.conv_q.bias"]).view(b, n_heads, d, t).transpose(2, 3)   # [b,h,t,d]
@@ -74,18 +76,19 @@ def rel_attention(p, pre, x, mask, n_heads, window):
     v = F.conv1d(x, p[f"{pre}.conv_v.weight"], p[f"{pre}.conv_v.bias"]).view(b, n_heads, d, t).transpose(2, 3)
     scores = torch.matmul(q, k.transpose(-2, -1)) / math.sqrt(d)
     ek, ev = p[f"{pre}.emb_rel_k"][0], p[f"{pre}.emb_rel_v"][0]                   # [2w+1, d], shared by the heads
-    idx = torch.arange(t)
+    idx = torch.arange(t, device=x.device)
+    zero = torch.zeros((), dtype=x.dtype, device=x.device)
     rel = idx[None, :] - idx[:, None]                                              # j - i
     band = rel.abs() <= window
     slot = (rel + window).clamp(0, 2 * window)
     qe = torch.matmul(q, ek.t())                                                   # [b,h,t,2w+1]: q_i . E_k[r]
-    scores = scores + torch.where(band, qe.gather(-1, slot.expand(b, n_heads, t, t)), torch.zeros(())) / math.sqrt(d)
+    scores = scores + torch.where(band, qe.gather(-1, slot.expand(b, n_heads, t, t)), zero) / math.sqrt(d)
     scores = scores.masked_fill(mask == 0, -1e4)
     pa = F.softmax(scores, dim=-1)
     out = torch.matmul(pa, v)
     # sum_j p[i,j] E_v[j-i+w] over the band = (band weights scattered by relative offset) @ E_v
-    wrel = torch.zeros(b, n_heads, t, 2 * window + 1)
-    wrel.scatter_add_(-1, slot.expand(b, n_heads, t, t), torch.where(band, pa, torch.zeros(())))
+    wrel = torch.zeros(b, n_heads, t, 2 * window + 1, dtype=x.dtype, device=x.device)
+    wrel.scatter_add_(-1, slot.expand(b, n_heads, t, t), torch.where(band, pa, zero))
     out = out + torch.matmul(wrel, ev)
     out = out.transpose(2, 3).contiguous().view(b, ch, t)
     return F.conv1d(out, p[f"{pre}.conv_o.weight"], p[f"{pre}.conv_o.bias"])
@@ -93,11 +96,12 @@ def rel_attention(p, pre, x, mask, n_heads, window):
 
 def text_encoder(p, x, x_lengths, n_heads=2, n_layers=6, kernel=3, window=4, spk=None):
     """TextEncoder.forward (:312-326): token ids [B,Tx] -> (mu_x [B,80,Tx], logw [B,1,Tx], x_mask [B,1,Tx]).  spk [B,E] for a
-    multi-speaker model: concatenated to every token after the prenet (:317-318)."""
+    multi-speaker model: concatenated to every token after the prenet (:317-318).  Runs in the weights' dtype (float32, or
+    float64 for a high-precision reference) on the tensors' device."""
     ch = p["emb.weight"].shape[1]
     h = (F.embedding(x, p["emb.weight"]) * math.sqrt(ch)).transpose(1, -1)
     t = h.shape[2]
-    x_mask = (torch.arange(t)[None, :] < x_lengths[:, None]).unsqueeze(1).to(h.dtype)
+    x_mask = (torch.arange(t, device=h.device)[None, :] < x_lengths[:, None]).unsqueeze(1).to(h.dtype)
     # prenet: ConvReluNorm (:57-64)
     org = h
     for i in range(3):
@@ -148,10 +152,11 @@ def mel_param_spec(n_feats=80, ch=192, filt=768, n_layers=6, kernel=3, window=4,
     return s
 
 
-def mel_synthetic_weights(seed):
+def mel_synthetic_weights(seed, **config):
+    """As synthetic_weights, for MelEncoder; `config`: mel_param_spec's shape arguments (defaults: DiffVC's)."""
     from speech_backbones_b200.spec import synthetic_tensor
     sd = {}
-    for name, shape in mel_param_spec():
+    for name, shape in mel_param_spec(**config):
         if name.endswith(".gamma"):
             sd[name] = 1.0 + 0.1 * synthetic_tensor(seed, "melenc/" + name, shape)
         elif name.endswith((".beta", ".bias")):

@@ -252,6 +252,8 @@ struct sbk_textenc {
     Workspace ws;
     bool is_packed = false;
     int64_t last_launches = 0;
+    // debug capture (fmt: 0 token-major fp32 [B][T][C], 1 planar fp32 [B][C][T])
+    Snapshots snaps;
     int enc_ch() const { return cfg.n_channels + (cfg.n_spks > 1 ? cfg.spk_emb_dim : 0); }
 };
 
@@ -375,6 +377,11 @@ static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths
     if (B <= 0 || Tx <= 0) return fail(SBK_ERR_ARG, "sbk_textenc_forward: B and Tx must be positive");
     const sbk_textenc_config& c = e->cfg;
     if (c.n_spks > 1 && !spk) return fail(SBK_ERR_ARG, "sbk_textenc_forward: spk is required when n_spks > 1");
+    // k_te_attn keeps one (d + Tx + 32)-float slice per warp in shared memory: a longer sequence is refused here, before
+    // anything is launched or written
+    const int d = e->enc_ch() / c.n_heads;
+    const size_t asm_ = (size_t)8 * (d + ((Tx + 3) & ~3) + 32) * sizeof(float);
+    if (asm_ > 200 * 1024) return fail(SBK_ERR_UNSUPPORTED, "sbk_textenc_forward: Tx = %d tokens exceeds the attention kernel's shared-memory budget", Tx);
     CU(cudaSetDevice(c.device));
     cudaStream_t s = (cudaStream_t)stream;
     const int C = c.n_channels, Ce = e->enc_ch(), F = c.filter_channels, Fd = c.filter_channels_dp, K = c.kernel_size;
@@ -392,6 +399,9 @@ static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths
     Arena ar = e->ws.arena();
     carve(ar);
     int64_t n = 0;
+    // debug capture: the activations are rewritten within the call, so each tensor is copied right after the launch that wrote it
+    e->snaps.begin();
+    auto snap = [&](const std::string& name, const float* src, size_t channels, int fmt) { e->snaps.record(name, src, ntok * channels, fmt, s); };
     auto conv = [&](const float* in, int Cin, const float* spk_in, int E, const std::string& wkey, const std::string& bkey, int Kk, int Cout,
                     int in_mask, int relu1, int mask1, const float* res, int res_mask, const std::string& ln, int relu2, int mask2,
                     float* out, int planar, int in_planar = 0) {
@@ -414,9 +424,12 @@ static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths
         // MelEncoder (DiffVC/model/encoder.py:279-284): x = init_proj(x * x_mask); the caller's mask is used as is
         x_mask = const_cast<float*>(mask_in);
         conv(mel, c.n_feats, nullptr, 0, "init_proj", "init_proj.bias", 1, C, 1, 0, 0, nullptr, 0, "", 0, 0, h0, 0, 1);
+        snap("init_proj", h0, C, 0);
     } else {
         k_te_mask<<<(B * Tx + 255) / 256, 256, 0, s>>>(reinterpret_cast<const long long*>(x_lengths), x_mask, B, Tx); ++n;
+        snap("mask", x_mask, 1, 0);
         k_te_embed<<<(int)std::min<size_t>((ntok * (C / 4) + 255) / 256, 8 * (size_t)sbk::device_sm_count()), 256, 0, s>>>(reinterpret_cast<const long long*>(x), e->w.get("emb.weight"), h0, (int)ntok, C, c.n_vocab, sqrtf((float)C)); ++n;
+        snap("embed", h0, C, 0);
     }
     // ---- prenet (ConvReluNorm, :57-64): x = relu(LN(conv5(x * mask))) x3; x = (x_org + proj(x)) * mask
     const float* cur = h0; float* pp[2] = {h1, h2};
@@ -424,46 +437,58 @@ static int te_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths
         conv(cur, C, nullptr, 0, "prenet.conv" + std::to_string(i), "prenet.conv_layers." + std::to_string(i) + ".bias", 5, C,
              1, 0, 0, nullptr, 0, "prenet.norm_layers." + std::to_string(i), 1, 0, pp[i & 1], 0);
         cur = pp[i & 1];
+        snap("prenet." + std::to_string(i), cur, C, 0);
     }
     float* hx = cur == h1 ? h2 : h1;
     conv(cur, C, nullptr, 0, "prenet.proj", "prenet.proj.bias", 1, C, 0, 0, 0, h0, 0, "", 0, 1, hx, 0);
+    snap("prenet.proj", hx, C, 0);
     // (multi-speaker: the speaker embedding is concatenated to every token after the prenet, :317-318)
     float* h = hx;
     if (c.n_spks > 1) {
         // h0 is free now but sized for Ce as well: concatenate into it
         k_te_concat_spk<<<(int)std::min<size_t>((ntok * Ce + 255) / 256, 8 * (size_t)sbk::device_sm_count()), 256, 0, s>>>(hx, spk, h0, B, Tx, C, c.spk_emb_dim); ++n;
         h = h0;
+        snap("spk_concat", h0, Ce, 0);
     }
     float* other[2];
     { int k = 0; for (float* q : {h0, h1, h2}) if (q != h && k < 2) other[k++] = q; }
     // ---- encoder (:267-278)
-    const int d = Ce / c.n_heads;
     for (int i = 0; i < c.n_layers; ++i) {
-        const std::string a = "encoder.attn_layers." + std::to_string(i), nn = std::to_string(i);
+        const std::string a = "encoder.attn_layers." + std::to_string(i), nn = std::to_string(i), q = "enc." + nn;
         conv(h, Ce, nullptr, 0, a + ".qkv.w", a + ".qkv.b", 1, 3 * Ce, 1, 0, 0, nullptr, 0, "", 0, 0, wa, 0);          // x = x * mask; q|k|v
-        const size_t asm_ = (size_t)8 * (d + ((Tx + 3) & ~3) + 32) * sizeof(float);
-        if (asm_ > 200 * 1024) return fail(SBK_ERR_UNSUPPORTED, "sbk_textenc_forward: Tx = %d tokens exceeds the attention kernel's shared-memory budget", Tx);
+        snap(q + ".qkv", wa, 3 * Ce, 0);
         k_te_attn<<<dim3((Tx + 7) / 8, c.n_heads, B), 256, asm_, s>>>(wa, x_mask, e->w.get(a + ".emb_rel_k"), e->w.get(a + ".emb_rel_v"), wb, B, Tx, Ce, c.n_heads, c.window_size); ++n;
+        snap(q + ".attn", wb, Ce, 0);
         conv(wb, Ce, nullptr, 0, a + ".o.w", a + ".conv_o.bias", 1, Ce, 0, 0, 0, h, 1, "encoder.norm_layers_1." + nn, 0, 0, other[0], 0);   // LN(x*mask + attn)
+        snap(q + ".ln1", other[0], Ce, 0);
         conv(other[0], Ce, nullptr, 0, "ffn" + nn + ".1", "encoder.ffn_layers." + nn + ".conv_1.bias", K, F, 1, 1, 1, nullptr, 0, "", 0, 0, wa, 0);
+        snap(q + ".ffn1", wa, F, 0);
         conv(wa, F, nullptr, 0, "ffn" + nn + ".2", "encoder.ffn_layers." + nn + ".conv_2.bias", K, Ce, 0, 0, 1, other[0], 0, "encoder.norm_layers_2." + nn, 0, 0, other[1], 0);
+        snap(q + ".ln2", other[1], Ce, 0);
         float* t = h; h = other[1]; other[1] = t;
     }
-    if (mel) {
-        // x = term_proj(x * x_mask): no output mask (DiffVC/model/encoder.py:283)
-        conv(h, Ce, nullptr, 0, "term_proj", "term_proj.bias", 1, c.n_feats, 1, 0, 0, nullptr, 0, "", 0, 0, mu_x, 1);
+    auto done = [&]() -> int {
+        if (const cudaError_t err = e->snaps.finish()) return fail(SBK_ERR_CUDA, "sbk_textenc_forward: debug capture failed: %s", cudaGetErrorString(err));
         CU(cudaGetLastError());
         e->last_launches = n;
         return SBK_OK;
+    };
+    if (mel) {
+        // x = term_proj(x * x_mask): no output mask (DiffVC/model/encoder.py:283)
+        conv(h, Ce, nullptr, 0, "term_proj", "term_proj.bias", 1, c.n_feats, 1, 0, 0, nullptr, 0, "", 0, 0, mu_x, 1);
+        snap("out", mu_x, c.n_feats, 1);
+        return done();
     }
     // ---- x = x * mask; mu = proj_m(x) * mask; logw = DurationPredictor(x, mask)  (:278, :321-324, :83-93)
     conv(h, Ce, nullptr, 0, "proj_m", "proj_m.bias", 1, c.n_feats, 1, 0, 0, nullptr, 0, "", 0, 1, mu_x, 1);
+    snap("mu", mu_x, c.n_feats, 1);
     conv(h, Ce, nullptr, 0, "dp.1", "proj_w.conv_1.bias", K, Fd, 1, 1, 0, nullptr, 0, "proj_w.norm_1", 0, 0, wa, 0);
+    snap("dp.1", wa, Fd, 0);
     conv(wa, Fd, nullptr, 0, "dp.2", "proj_w.conv_2.bias", K, Fd, 1, 1, 0, nullptr, 0, "proj_w.norm_2", 0, 0, wb, 0);
+    snap("dp.2", wb, Fd, 0);
     conv(wb, Fd, nullptr, 0, "dp.p", "proj_w.proj.bias", 1, 1, 1, 0, 0, nullptr, 0, "", 0, 1, logw, 1);
-    CU(cudaGetLastError());
-    e->last_launches = n;
-    return SBK_OK;
+    snap("logw", logw, 1, 1);
+    return done();
 }
 
 extern "C" int sbk_textenc_forward(sbk_textenc* e, const int64_t* x, const int64_t* x_lengths, const float* spk,
@@ -481,3 +506,22 @@ extern "C" int sbk_melenc_forward(sbk_textenc* e, const float* x, const float* x
 }
 
 extern "C" int64_t sbk_textenc_last_launch_count(const sbk_textenc* e) { return e ? e->last_launches : 0; }
+
+extern "C" int sbk_textenc_debug_capture(sbk_textenc* e, int on) {
+    if (!e) return fail(SBK_ERR_ARG, "sbk_textenc_debug_capture: null handle");
+    e->snaps.on = on != 0;
+    return SBK_OK;
+}
+extern "C" int sbk_textenc_debug_num(const sbk_textenc* e) { return e ? (int)e->snaps.list.size() : 0; }
+extern "C" const char* sbk_textenc_debug_name(const sbk_textenc* e, int i) {
+    if (!e || i < 0 || i >= (int)e->snaps.list.size()) return nullptr;
+    return e->snaps.list[i].name.c_str();
+}
+extern "C" int sbk_textenc_debug_op_layout(const sbk_textenc* e, const char* name) {
+    const Snapshots::Snap* sn = e && name ? e->snaps.find(name) : nullptr;
+    return sn ? sn->fmt : -1;
+}
+extern "C" int sbk_textenc_debug_read(sbk_textenc* e, const char* name, void* dst, int64_t* numel) {
+    if (!e || !name) return fail(SBK_ERR_ARG, "sbk_textenc_debug_read: null argument");
+    return e->snaps.read(name, dst, numel, e->cfg.device, "sbk_textenc_debug_read");
+}

@@ -83,6 +83,13 @@ class TextEncEngine(_NativeHandle):
         P, I = C.c_void_p, C.c_int
         self.lib.sbk_textenc_forward.argtypes = [P, P, P, P, P, P, P, I, I, P]
         self.lib.sbk_melenc_forward.argtypes = [P, P, P, P, I, I, P]
+        self.lib.sbk_textenc_debug_capture.argtypes = [P, I]
+        self.lib.sbk_textenc_debug_num.argtypes = [P]
+        self.lib.sbk_textenc_debug_name.argtypes = [P, I]
+        self.lib.sbk_textenc_debug_name.restype = C.c_char_p
+        self.lib.sbk_textenc_debug_op_layout.argtypes = [P, C.c_char_p]
+        self.lib.sbk_textenc_debug_read.argtypes = [P, C.c_char_p, P, C.POINTER(C.c_int64)]
+        self._shape = None                               # (B, Tx) of the last forward
         cfg = SbkTextEncConfig(device, m.n_vocab, m.n_feats, m.n_channels, m.filter_channels, m.filter_channels_dp, m.n_heads,
                                m.n_layers, m.kernel_size, m.window_size, m.n_spks, m.spk_emb_dim, kind)
         _check(self._create(cfg), "sbk_textenc_create")
@@ -108,6 +115,7 @@ class TextEncEngine(_NativeHandle):
         with torch.cuda.device(x.device):
             _check(self.lib.sbk_textenc_forward(self.h, _ptr(x), _ptr(x_lengths), _ptr(spk), _ptr(mu), _ptr(logw), _ptr(mask),
                                                 B, Tx, self._stream()), "sbk_textenc_forward")
+        self._shape = (B, Tx)
         return mu, logw, mask
 
     def forward_mel(self, x, x_mask):
@@ -121,7 +129,30 @@ class TextEncEngine(_NativeHandle):
         out = torch.empty_like(x)
         with torch.cuda.device(x.device):
             _check(self.lib.sbk_melenc_forward(self.h, _ptr(x), _ptr(x_mask), _ptr(out), B, T, self._stream()), "sbk_melenc_forward")
+        self._shape = (B, T)
         return out
+
+    # ---- test hooks: the intermediates of the last forward run with capture on (sbk_textenc_debug_*)
+    def debug_capture(self, on=True):
+        _check(self.lib.sbk_textenc_debug_capture(self.h, 1 if on else 0), "sbk_textenc_debug_capture")
+
+    def debug_names(self):
+        """Tensors the last forward captured, in launch order (sbk.h: sbk_textenc_debug_capture)."""
+        return [self.lib.sbk_textenc_debug_name(self.h, i).decode() for i in range(self.lib.sbk_textenc_debug_num(self.h))]
+
+    def debug_read(self, name):
+        """One captured tensor on the CPU, fp32: token-major [B, Tx, C] (mask: [B, Tx, 1]), or [B, C, Tx] for mu, logw
+        and the mel encoder's out."""
+        fmt = int(self.lib.sbk_textenc_debug_op_layout(self.h, name.encode()))
+        if fmt < 0:
+            raise RuntimeError(f"debug_read: no captured tensor named '{name}'")
+        n = C.c_int64(0)
+        _check(self.lib.sbk_textenc_debug_read(self.h, name.encode(), None, C.byref(n)), "sbk_textenc_debug_read")
+        out = torch.empty(n.value, dtype=torch.float32)
+        _check(self.lib.sbk_textenc_debug_read(self.h, name.encode(), C.c_void_p(out.data_ptr()), C.byref(n)),
+               "sbk_textenc_debug_read")
+        B, T = self._shape
+        return out.view(B, T, -1) if fmt == 0 else out.view(B, -1, T)
 
 
 class MelEncoder(BaseModule):

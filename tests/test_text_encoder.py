@@ -36,7 +36,9 @@ def test_parameter_tree_is_the_reference_state_dict():
 
 def test_textenc_symbols_exported(sbk_lib):
     for sym in ("sbk_textenc_create", "sbk_textenc_destroy", "sbk_textenc_num_weights", "sbk_textenc_weight_name",
-                "sbk_textenc_set_weight", "sbk_textenc_pack", "sbk_textenc_forward", "sbk_textenc_last_launch_count"):
+                "sbk_textenc_set_weight", "sbk_textenc_pack", "sbk_textenc_forward", "sbk_textenc_last_launch_count",
+                "sbk_textenc_debug_capture", "sbk_textenc_debug_num", "sbk_textenc_debug_name", "sbk_textenc_debug_op_layout",
+                "sbk_textenc_debug_read"):
         assert hasattr(sbk_lib, sym), sym
 
 
