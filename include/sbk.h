@@ -108,7 +108,7 @@ int sbk_reverse_diffusion_lengths(sbk_handle* h, const float* z, const float* ma
                                   const float* noise, const int64_t* lengths, float* out, int B, int T, int n_timesteps,
                                   int stoc, void* stream);
 
-/* ---- rolling batches (Grad-TTS) -----------------------------------------------------------------------------
+/* ---- rolling batches (Grad-TTS; DiffVC through sbk_vc_rolling_reserve / sbk_vc_rolling_admit) ---------------
  * A slot plan of `capacity` rows (slots) at T = max_frames keeps running while requests join and leave it: slot b holds
  * one request - the arguments of one B = 1 Diffusion.forward call - at its own step i_b of its own n_timesteps N_b, and
  * runs as a ragged row of its T_b frames (sbk_estimator_lengths).  Step i_b uses t = 1 - (i_b + 0.5)/N_b and the
@@ -118,7 +118,9 @@ int sbk_reverse_diffusion_lengths(sbk_handle* h, const float* z, const float* ma
  * the request was admitted.  An empty slot runs as a 4-frame row of zeros and is read by no other row.
  * The schedule is deterministic: the caller knows when each slot finishes without reading device memory.
  * The plan is the handle's one plan: another sampler call on the handle replaces it, and the rolling entry points then fail
- * with SBK_ERR_STATE until the next sbk_rolling_reserve.  Grad-TTS handles only (SBK_ERR_ARG for DiffVC). */
+ * with SBK_ERR_STATE until the next sbk_rolling_reserve (sbk_vc_rolling_reserve).  sbk_rolling_reserve and sbk_rolling_admit
+ * take Grad-TTS handles only (SBK_ERR_ARG for DiffVC); sbk_rolling_advance / read / release serve the slot plans of both
+ * models. */
 /* (Re)build the slot plan at (capacity >= 1, max_frames a multiple of 4) with every slot empty. */
 int sbk_rolling_reserve(sbk_handle* h, int capacity, int max_frames, void* stream);
 /* Admit a request into an empty slot (SBK_ERR_STATE if it is busy): z, mu [1,n_feats,T_b], mask [1,1,T_b] (copied on the
@@ -135,6 +137,24 @@ int sbk_rolling_advance(sbk_handle* h, int steps, void* stream);
 int sbk_rolling_read(sbk_handle* h, int slot, float* out, void* stream);
 /* Empty a slot (finished or not) so that a new request can be admitted into it. */
 int sbk_rolling_release(sbk_handle* h, int slot, void* stream);
+
+/* Rolling DiffVC batches: the same slot plan on a DiffVC handle (SBK_ERR_ARG for Grad-TTS), advanced, read and released with
+ * sbk_rolling_advance / read / release.  Slot b holds the arguments of one B = 1 sbk_vc_reverse_diffusion call at its own
+ * step i_b of its own N_b: step i_b uses t = 1 - i_b/N_b, the {A, Bc, sigma} coefficients of every other DiffVC sampler call
+ * and row i_b of the request's own conditioning table, gathered into a [1][capacity] table and folded into the first
+ * ResnetBlock per slot.  A finished request's mel is, in every mode bit for bit, row b of a sbk_vc_reverse_diffusion_lengths
+ * call at (capacity, max_frames) with the same N_b, mode, cond rows and noise, whatever the other slots hold and whenever it
+ * was admitted; and its own B = 1 sbk_vc_reverse_diffusion where the two plans pick the same 3x3 tile layout (SBK_CONV3_ROWS
+ * pins it): bit for bit in tf32 and bf16, within fp32 rounding in fp32x3 and fp32. */
+/* (Re)build a DiffVC slot plan at (capacity >= 1, max_frames a multiple of 4) with every slot empty. */
+int sbk_vc_rolling_reserve(sbk_handle* h, int capacity, int max_frames, void* stream);
+/* Admit a request into an empty slot (SBK_ERR_STATE if it is busy): z, mean [1,n_feats,T_b], mask [1,1,T_b], T_b a multiple of
+ * 4 in [4, max_frames], n_timesteps >= 1, cond [n_timesteps][1][dim_cond] (sbk_vc_conditioning at B = 1), mode 0 pf, 1 em,
+ * 2 ml.  z, mask, mean and cond are copied on the stream.  For em / ml, noise [n_timesteps,1,n_feats,T_b], the reference's
+ * per-step draws, which the slot reads until it finishes: the caller keeps it alive until then; NULL for pf.  Only this
+ * slot's rows and schedule are written. */
+int sbk_vc_rolling_admit(sbk_handle* h, int slot, const float* z, const float* mask, const float* mean, const float* cond,
+                         const float* noise, int T_b, int n_timesteps, int mode, void* stream);
 
 /* ---- DiffVC (SBK_MODEL_DIFFVC) ------------------------------------------------------------------------------
  * GradLogPEstimator.forward (DiffVC/model/diffusion.py:61-106) with the xt-independent conditioning vector

@@ -23,6 +23,7 @@ EXPORTS = [
     "sbk_estimator_lengths", "sbk_reverse_diffusion_lengths", "sbk_reverse_steps_lengths",
     "sbk_vc_estimator_lengths", "sbk_vc_reverse_diffusion_lengths", "sbk_vc_conditioning_lengths",
     "sbk_rolling_reserve", "sbk_rolling_admit", "sbk_rolling_advance", "sbk_rolling_read", "sbk_rolling_release",
+    "sbk_vc_rolling_reserve", "sbk_vc_rolling_admit",
 ]
 
 
@@ -68,6 +69,8 @@ def load_library() -> C.CDLL:
     lib.sbk_rolling_advance.argtypes = [P, I, P]
     lib.sbk_rolling_read.argtypes = [P, I, F, P]
     lib.sbk_rolling_release.argtypes = [P, I, P]
+    lib.sbk_vc_rolling_reserve.argtypes = [P, I, I, P]
+    lib.sbk_vc_rolling_admit.argtypes = [P, I, F, F, F, F, F, I, I, I, P]
     lib.sbk_last_host_launches.argtypes = [P]
     lib.sbk_debug_read.argtypes = [P, C.c_char_p, F, C.POINTER(C.c_int64)]
     lib.sbk_debug_num.argtypes = [P]
@@ -454,6 +457,18 @@ class Engine(_NativeHandle):
         _check(self.lib.sbk_rolling_admit(self.h, int(slot), _ptr(z), _ptr(mask), _ptr(mu), _ptr(spk), _ptr(noise),
                                           int(z.shape[-1]), int(n_timesteps), 1 if stoc else 0, self._stream()),
                "sbk_rolling_admit")
+
+    def vc_rolling_reserve(self, capacity, max_frames):
+        self._call(self.lib.sbk_vc_rolling_reserve, "sbk_vc_rolling_reserve", self.h, int(capacity), int(max_frames),
+                   self._stream())
+
+    def vc_rolling_admit(self, slot, z, mask, mean, cond, n_timesteps, mode, noise=None):
+        """DiffVC: z, mean [1,n_feats,T_b], mask [1,1,T_b], cond [N,1,dim_cond], noise [N,1,n_feats,T_b] for 'em' / 'ml', None
+        for 'pf': contiguous fp32 on this engine's device.  The slot reads `noise` until it finishes; the caller keeps it
+        alive.  Advanced, read and released with rolling_advance / rolling_read / rolling_release."""
+        _check(self.lib.sbk_vc_rolling_admit(self.h, int(slot), _ptr(z), _ptr(mask), _ptr(mean), _ptr(cond), _ptr(noise),
+                                             int(z.shape[-1]), int(n_timesteps), self.VC_MODES[mode], self._stream()),
+               "sbk_vc_rolling_admit")
 
     def rolling_advance(self, steps):
         _check(self.lib.sbk_rolling_advance(self.h, int(steps), self._stream()), "sbk_rolling_advance")

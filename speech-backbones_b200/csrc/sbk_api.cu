@@ -85,7 +85,7 @@ struct Rolling {
     SlotSched* sched = nullptr;             // device [capacity]
     SlotStep* cur = nullptr;                // device [capacity], gathered by k_slot_begin every step
     std::vector<SlotSched> host;            // host copies of sched (i advanced by sbk_rolling_advance as the device does)
-    std::vector<void*> tab;                 // per slot: device [cap] float4 coef, then [cap] float t
+    std::vector<void*> tab;                 // per slot: device table of up to cap steps (slot_tab_floats)
     std::vector<int> tab_cap;
 };
 
@@ -828,7 +828,9 @@ static int run_ops(sbk_handle* h, cudaStream_t s) {
     StepBeginParams sb{pl.stats, pl.n_stat_doubles, pl.step_cur, pl.step_next};
     int n = launch_step_begin(sb, s);
     for (auto& op : pl.ops) {
-        const int k = pl.rolling && op.kind == OP_FINAL ? launch_final_slot(op.fn, h->roll.cur, h->roll.sched, s) : launch_op(op, s);
+        const int k = pl.rolling && op.kind == OP_FINAL
+                          ? launch_final_slot(op.fn, h->roll.cur, h->roll.sched, h->cfg.model == SBK_MODEL_DIFFVC, s)
+                          : launch_op(op, s);
         if (k < 0) { fail(SBK_ERR_CUDA, "launch of '%s' was refused (device attribute / layout)", op.name.c_str()); return -1; }
         n += k;
         if (h->capture && op.dbg_ptr && op.dbg_numel > 0) {
@@ -1155,6 +1157,9 @@ extern "C" int sbk_reverse_diffusion_host(sbk_handle* h, const float* z, const f
 // ------------------------------------------------------------------------------------------------
 // rolling batches: a slot plan whose rows (slots) each run one request's Euler(-Maruyama) loop at its own step
 // ------------------------------------------------------------------------------------------------
+static void vc_step_coefs(const sbk_config& c, int N, int i, int mode, float* t_out, float4* cf);
+static int cond_fold(sbk_handle* h, int rows, int B, cudaStream_t s);
+
 static int rolling_state(sbk_handle* h, const char* what) {
     if (!h) return fail(SBK_ERR_ARG, "%s: null handle", what);
     if (!h->plan.rolling)
@@ -1175,11 +1180,10 @@ static int slot_rows(sbk_handle* h, int b, const float* z, const float* mu, cons
     return n;
 }
 
-extern "C" int sbk_rolling_reserve(sbk_handle* h, int capacity, int max_frames, void* stream) {
-    if (!h) return fail(SBK_ERR_ARG, "sbk_rolling_reserve: null handle");
-    if (h->cfg.model != SBK_MODEL_GRADTTS) return fail(SBK_ERR_ARG, "sbk_rolling_reserve: this handle is a DiffVC model (rolling batches are Grad-TTS only)");
+// the slot plan of either model (the caller has checked the handle's model): its update is the model's (set_mode, run_ops)
+static int rolling_reserve(sbk_handle* h, int capacity, int max_frames, void* stream, const char* what) {
     if (capacity < 1 || max_frames < 4 || max_frames % 4 != 0)
-        return fail(SBK_ERR_ARG, "sbk_rolling_reserve: capacity must be >= 1 and max_frames a positive multiple of 4, got %d, %d", capacity, max_frames);
+        return fail(SBK_ERR_ARG, "%s: capacity must be >= 1 and max_frames a positive multiple of 4, got %d, %d", what, capacity, max_frames);
     if (!h->is_packed) return fail(SBK_ERR_STATE, "weights not packed: call sbk_set_weight for every key, then sbk_pack");
     CU(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
@@ -1203,23 +1207,73 @@ extern "C" int sbk_rolling_reserve(sbk_handle* h, int capacity, int max_frames, 
     int64_t n = 0;
     for (int b = 0; b < capacity; ++b) n += slot_rows(h, b, nullptr, nullptr, nullptr, 4, s);
     set_ragged(pl, true);
-    set_mode(pl, 1, true, pl.xt);               // time rows per sample (row b = slot b); the update's mode is per slot
+    // time rows (and DiffVC's folded conditioning rows) per sample, row b = slot b; the update's mode is per slot
+    set_mode(pl, h->cfg.model == SBK_MODEL_DIFFVC ? 3 : 1, true, pl.xt);
     pl.rolling = true;
     CU(cudaGetLastError());
     h->last_launches = n;
     return SBK_OK;
 }
 
+extern "C" int sbk_rolling_reserve(sbk_handle* h, int capacity, int max_frames, void* stream) {
+    if (!h) return fail(SBK_ERR_ARG, "sbk_rolling_reserve: null handle");
+    if (h->cfg.model != SBK_MODEL_GRADTTS) return fail(SBK_ERR_ARG, "sbk_rolling_reserve: this handle is a DiffVC model (use sbk_vc_rolling_reserve)");
+    return rolling_reserve(h, capacity, max_frames, stream, "sbk_rolling_reserve");
+}
+
+extern "C" int sbk_vc_rolling_reserve(sbk_handle* h, int capacity, int max_frames, void* stream) {
+    if (!h) return fail(SBK_ERR_ARG, "sbk_vc_rolling_reserve: null handle");
+    if (h->cfg.model != SBK_MODEL_DIFFVC) return fail(SBK_ERR_ARG, "sbk_vc_rolling_reserve: this handle is not a DiffVC model (use sbk_rolling_reserve)");
+    return rolling_reserve(h, capacity, max_frames, stream, "sbk_vc_rolling_reserve");
+}
+
+// the checks every admission makes (`what`: the entry point, for the message)
+static int admit_check(sbk_handle* h, int slot, const float* z, const float* mask, const float* mu, int T_b, int n_timesteps,
+                       const char* what) {
+    const Rolling& r = h->roll;
+    if (!z || !mask || !mu) return fail(SBK_ERR_ARG, "%s: null argument", what);
+    if (slot < 0 || slot >= r.capacity) return fail(SBK_ERR_ARG, "%s: slot %d out of range [0, %d)", what, slot, r.capacity);
+    if (r.host[slot].n != 0) return fail(SBK_ERR_STATE, "%s: slot %d is busy (release it first)", what, slot);
+    if (T_b < 4 || T_b > r.max_frames || T_b % 4 != 0)
+        return fail(SBK_ERR_ARG, "%s: T_b must be a multiple of 4 in [4, %d] (fix_len_compatibility), got %d", what, r.max_frames, T_b);
+    if (n_timesteps < 1) return fail(SBK_ERR_ARG, "%s: n_timesteps must be >= 1", what);
+    return SBK_OK;
+}
+
+// write slot b's table (its t and coefficient rows `tab`, then for DiffVC the cond rows [N][dim_cond] copied from the
+// device) and its schedule, then its rows; *launches gets the kernels it launched
+static int admit_slot(sbk_handle* h, int slot, const float* z, const float* mask, const float* mu, const float* noise,
+                      const std::vector<float4>& tab, const float* cond, int T_b, int N, int stoc, cudaStream_t s,
+                      int64_t* launches) {
+    Rolling& r = h->roll;
+    const int dc = cond ? h->cfg.dim_cond : 0;
+    if (r.tab_cap[slot] < N) {
+        if (r.tab[slot]) CU(cudaFreeAsync(r.tab[slot], s));
+        r.tab[slot] = nullptr;
+        r.tab_cap[slot] = 0;
+        CU(cudaMallocAsync(&r.tab[slot], slot_tab_floats(N, dc) * sizeof(float), s));
+        r.tab_cap[slot] = N;
+    }
+    // pageable-source async copies are staged before returning, so the host vectors may die at scope exit
+    CU(cudaMemcpyAsync(r.tab[slot], tab.data(), tab.size() * sizeof(float4), cudaMemcpyHostToDevice, s));
+    SlotSched e;
+    e.n = N; e.i = 0; e.stoc = stoc ? 1 : 0; e.T = T_b; e.noise = stoc ? noise : nullptr;
+    e.coef_tab = static_cast<const float4*>(r.tab[slot]);
+    e.t_tab = reinterpret_cast<const float*>(e.coef_tab + N);
+    if (cond)
+        CU(cudaMemcpyAsync(const_cast<float*>(slot_cond_rows(e.coef_tab, N)), cond, (size_t)N * dc * sizeof(float),
+                           cudaMemcpyDeviceToDevice, s));
+    CU(cudaMemcpyAsync(r.sched + slot, &e, sizeof(e), cudaMemcpyHostToDevice, s));
+    *launches = slot_rows(h, slot, z, mu, mask, T_b, s);
+    r.host[slot] = e;
+    return SBK_OK;
+}
+
 extern "C" int sbk_rolling_admit(sbk_handle* h, int slot, const float* z, const float* mask, const float* mu, const float* spk,
                                  const float* noise, int T_b, int n_timesteps, int stoc, void* stream) {
+    if (h && h->cfg.model != SBK_MODEL_GRADTTS) return fail(SBK_ERR_ARG, "sbk_rolling_admit: this handle is a DiffVC model (use sbk_vc_rolling_admit)");
     TRY(rolling_state(h, "sbk_rolling_admit"));
-    Rolling& r = h->roll;
-    if (!z || !mask || !mu) return fail(SBK_ERR_ARG, "sbk_rolling_admit: null argument");
-    if (slot < 0 || slot >= r.capacity) return fail(SBK_ERR_ARG, "sbk_rolling_admit: slot %d out of range [0, %d)", slot, r.capacity);
-    if (r.host[slot].n != 0) return fail(SBK_ERR_STATE, "sbk_rolling_admit: slot %d is busy (release it first)", slot);
-    if (T_b < 4 || T_b > r.max_frames || T_b % 4 != 0)
-        return fail(SBK_ERR_ARG, "sbk_rolling_admit: T_b must be a multiple of 4 in [4, %d] (fix_len_compatibility), got %d", r.max_frames, T_b);
-    if (n_timesteps < 1) return fail(SBK_ERR_ARG, "sbk_rolling_admit: n_timesteps must be >= 1");
+    TRY(admit_check(h, slot, z, mask, mu, T_b, n_timesteps, "sbk_rolling_admit"));
     if (stoc && !noise) return fail(SBK_ERR_ARG, "sbk_rolling_admit: stoc=1 needs a noise buffer");
     if (h->cfg.n_spks > 1 && !spk) return fail(SBK_ERR_ARG, "sbk_rolling_admit: spk is required when n_spks > 1");
     cudaStream_t s = (cudaStream_t)stream;
@@ -1229,21 +1283,8 @@ extern "C" int sbk_rolling_admit(sbk_handle* h, int slot, const float* z, const 
     std::vector<float4> tab((size_t)N + (N + 3) / 4);
     float* tr = reinterpret_cast<float*>(tab.data() + N);
     for (int i = 0; i < N; ++i) step_coefs(h->cfg, N, i, &tr[i], &tab[i]);
-    if (r.tab_cap[slot] < N) {
-        if (r.tab[slot]) CU(cudaFreeAsync(r.tab[slot], s));
-        r.tab[slot] = nullptr;
-        r.tab_cap[slot] = 0;
-        CU(cudaMallocAsync(&r.tab[slot], tab.size() * sizeof(float4), s));
-        r.tab_cap[slot] = N;
-    }
-    // pageable-source async copies are staged before returning, so the host vectors may die at scope exit
-    CU(cudaMemcpyAsync(r.tab[slot], tab.data(), tab.size() * sizeof(float4), cudaMemcpyHostToDevice, s));
-    SlotSched e;
-    e.n = N; e.i = 0; e.stoc = stoc ? 1 : 0; e.T = T_b; e.noise = stoc ? noise : nullptr;
-    e.coef_tab = static_cast<const float4*>(r.tab[slot]);
-    e.t_tab = reinterpret_cast<const float*>(e.coef_tab + N);
-    CU(cudaMemcpyAsync(r.sched + slot, &e, sizeof(e), cudaMemcpyHostToDevice, s));
-    int64_t n = slot_rows(h, slot, z, mu, mask, T_b, s);
+    int64_t n = 0;
+    TRY(admit_slot(h, slot, z, mask, mu, noise, tab, nullptr, T_b, N, stoc, s, &n));
     if (h->cfg.n_spks > 1) {
         SpkParams p; p.spk = spk; p.B = 1; p.E = h->cfg.spk_emb_dim; p.n_feats = h->cfg.n_feats;
         p.out = pl.spk_s + (size_t)slot * h->cfg.n_feats;
@@ -1252,16 +1293,22 @@ extern "C" int sbk_rolling_admit(sbk_handle* h, int slot, const float* z, const 
         n += launch_spk(p, s);
     }
     CU(cudaGetLastError());
-    r.host[slot] = e;
     h->last_launches = n;
     return SBK_OK;
 }
 
-// one rolling step: every slot's t, coefficients and noise slab, the time table of those rows, the U-Net and the update
+// one rolling step: every slot's t, coefficients and noise slab (DiffVC: and its conditioning row, folded as a [1][B]
+// table), the time table of those rows, the U-Net and the update
 static int rolling_step(sbk_handle* h, cudaStream_t s) {
     Plan& pl = h->plan;
     SlotBeginParams p{h->roll.sched, h->roll.cur, pl.t_rows, pl.coef, pl.B, h->cfg.n_feats};
-    int n = launch_slot_begin(p, s);
+    int n;
+    if (h->cfg.model == SBK_MODEL_DIFFVC) {
+        n = launch_vc_slot_begin(VcSlotBeginParams{p, pl.vc_cond, h->cfg.dim_cond}, s);
+        n += cond_fold(h, 1, pl.B, s);
+    } else {
+        n = launch_slot_begin(p, s);
+    }
     n += time_table(h, pl.B, s);
     const int k = run_ops(h, s);
     return k < 0 ? -1 : n + k;
@@ -1284,7 +1331,8 @@ extern "C" int sbk_rolling_advance(sbk_handle* h, int steps, void* stream) {
         k_set_int<<<1, 1, 0, s>>>(pl.step_next, 0);
         k_set_int<<<1, 1, 0, s>>>(pl.step_end, steps);
         CU(cudaGraphLaunch(pl.groll, s));
-        n += 3 + (int64_t)steps * (pl.launches_per_step + 3);
+        // per step: the prologue (+ DiffVC's fold), the time table, the step's ops and k_loop_cond
+        n += 3 + (int64_t)steps * (pl.launches_per_step + (h->cfg.model == SBK_MODEL_DIFFVC ? 4 : 3));
         h->last_host_launches = 1;
     } else {
         for (int i = 0; i < steps; ++i) {
@@ -1295,6 +1343,26 @@ extern "C" int sbk_rolling_advance(sbk_handle* h, int steps, void* stream) {
     }
     CU(cudaGetLastError());
     for (SlotSched& e : h->roll.host) e.i = std::min(e.n, e.i + steps);
+    h->last_launches = n;
+    return SBK_OK;
+}
+
+extern "C" int sbk_vc_rolling_admit(sbk_handle* h, int slot, const float* z, const float* mask, const float* mean,
+                                    const float* cond, const float* noise, int T_b, int n_timesteps, int mode, void* stream) {
+    if (h && h->cfg.model != SBK_MODEL_DIFFVC) return fail(SBK_ERR_ARG, "sbk_vc_rolling_admit: this handle is not a DiffVC model (use sbk_rolling_admit)");
+    TRY(rolling_state(h, "sbk_vc_rolling_admit"));
+    TRY(admit_check(h, slot, z, mask, mean, T_b, n_timesteps, "sbk_vc_rolling_admit"));
+    if (!cond) return fail(SBK_ERR_ARG, "sbk_vc_rolling_admit: null argument");
+    if (mode < 0 || mode > 2) return fail(SBK_ERR_ARG, "sbk_vc_rolling_admit: mode must be 0 (pf), 1 (em) or 2 (ml)");
+    if (mode != 0 && !noise) return fail(SBK_ERR_ARG, "sbk_vc_rolling_admit: modes em/ml need a noise buffer");
+    const int N = n_timesteps;
+    // the request's t and {A, Bc, sigma} rows, computed as every other DiffVC sampler call computes them (vc_step_coefs)
+    std::vector<float4> tab((size_t)N + (N + 3) / 4);
+    float* tr = reinterpret_cast<float*>(tab.data() + N);
+    for (int i = 0; i < N; ++i) vc_step_coefs(h->cfg, N, i, mode, &tr[i], &tab[i]);
+    int64_t n = 0;
+    TRY(admit_slot(h, slot, z, mask, mean, noise, tab, cond, T_b, N, mode != 0, (cudaStream_t)stream, &n));
+    CU(cudaGetLastError());
     h->last_launches = n;
     return SBK_OK;
 }
@@ -1391,15 +1459,20 @@ static void vc_step_coefs(const sbk_config& c, int N, int i, int mode, float* t_
     *cf = make_float4((float)A, (float)Bc, (float)sigma, 0.f);
 }
 
-static int vc_fold(sbk_handle* h, const float* cond, int rows, int B, cudaStream_t s) {
+// fold the plan's conditioning table pl.vc_cond [rows][B] into the first ResnetBlock's extra weights
+static int cond_fold(sbk_handle* h, int rows, int B, cudaStream_t s) {
     Plan& pl = h->plan;
     const sbk_config& c = h->cfg;
-    CU(cudaMemcpyAsync(pl.vc_cond, cond, (size_t)rows * B * c.dim_cond * sizeof(float), cudaMemcpyDeviceToDevice, s));
     CondFoldParams p;
     p.cond = pl.vc_cond; p.w1 = h->w.get("estimator.downs.0.0.block1.block.0.weight");
     p.wres = h->w.get("estimator.downs.0.0.res_conv.weight");
     p.w_extra = pl.vc_wextra; p.r_extra = pl.vc_rextra; p.rows = rows; p.B = B; p.dc = c.dim_cond; p.C = c.dim;
     return launch_cond_fold(p, s);
+}
+
+static int vc_fold(sbk_handle* h, const float* cond, int rows, int B, cudaStream_t s) {
+    CU(cudaMemcpyAsync(h->plan.vc_cond, cond, (size_t)rows * B * h->cfg.dim_cond * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    return cond_fold(h, rows, B, s);
 }
 
 extern "C" int sbk_vc_estimator(sbk_handle* h, const float* x, const float* mask, const float* mean, const float* cond,

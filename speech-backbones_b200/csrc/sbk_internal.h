@@ -353,8 +353,10 @@ int launch_prior_expand(const PriorExpandParams& p, cudaStream_t s);
 
 struct StepBeginParams { double* stats; int n_doubles; int* step_cur; int* step_next; };
 
-// ---- a rolling Grad-TTS batch (sbk_rolling_*): every row (slot) runs its own request at its own step --------------------
+// ---- a rolling batch (sbk_rolling_*, sbk_vc_rolling_*): every row (slot) runs its own request at its own step ------------
 // The schedule of slot b, in device memory.  Written whole by the host at admission and release; k_final_slot advances i.
+// A DiffVC slot uses the same record: stoc is 1 for 'em' / 'ml' (the sampler mode itself only picks the host's
+// vc_step_coefs), and its conditioning rows follow the t rows in the slot's table (slot_cond_rows).
 struct SlotSched {
     int n;                      // the request's n_timesteps; 0: the slot is empty
     int i;                      // the step it runs next (the request has finished when i == n)
@@ -362,8 +364,14 @@ struct SlotSched {
     int T;                      // its frames T_b (the row stride of its noise)
     const float* noise;         // stoc: [n][n_feats][T_b], the request's draws; else nullptr
     const float* t_tab;         // [n] t of each step, and
-    const float4* coef_tab;     // [n] its coefficients, both from the host's step_coefs
+    const float4* coef_tab;     // [n] its coefficients, both from the host's step_coefs (DiffVC: vc_step_coefs)
 };
+// A slot's table, one allocation: [n] float4 coefficients, [n] float t padded to whole float4s, then for DiffVC the
+// request's [n][dim_cond] conditioning rows
+__host__ __device__ inline size_t slot_tab_floats(int n, int dc) { return 4 * ((size_t)n + (n + 3) / 4) + (size_t)n * dc; }
+__host__ __device__ inline const float* slot_cond_rows(const float4* coef_tab, int n) {
+    return reinterpret_cast<const float*>(coef_tab + n + (n + 3) / 4);
+}
 // What k_slot_begin gathers for the step about to run: mode 0 (idle or finished: the row is not updated), 1 (Euler) or
 // 2 (Euler-Maruyama, noise = this step's slab of the request's draws)
 struct SlotStep { const float* noise; int i; int mode; };
@@ -371,10 +379,15 @@ struct SlotBeginParams { const SlotSched* sched; SlotStep* cur; float* t_rows; f
 // admission / release of one slot: the plan's rows xt = z * mask, mu and mask over the plan's T frames, 0 from T_b on
 // (z, mu, mask [H][T_b] of the request; nullptr: the row is cleared)
 struct SlotWriteParams { const float* z; const float* mu; const float* mask; float* xt; float* mu_out; float* mask_out; int H, T, Tb; };
+// DiffVC: k_slot_begin's gather, plus each slot's conditioning row of its step into cond[b][dc] (0 for an idle slot), the
+// [1][B] table k_cond_fold then folds
+struct VcSlotBeginParams { SlotBeginParams s; float* cond; int dc; };
 int launch_slot_begin(const SlotBeginParams& p, cudaStream_t s);
+int launch_vc_slot_begin(const VcSlotBeginParams& p, cudaStream_t s);
 int launch_slot_write(const SlotWriteParams& p, cudaStream_t s);
-// k_final over a rolling batch: row b's mode and coefficients are its slot's (cur[b], p.coef[b]); advances sched[b].i
-int launch_final_slot(const FinalParams& p, const SlotStep* cur, SlotSched* sched, cudaStream_t s);
+// k_final over a rolling batch: row b's mode and coefficients are its slot's (cur[b], p.coef[b]); advances sched[b].i.
+// vc: DiffVC's update (k_final's mode 3) in place of Grad-TTS's
+int launch_final_slot(const FinalParams& p, const SlotStep* cur, SlotSched* sched, bool vc, cudaStream_t s);
 
 // launchers (all asynchronous on `s`); return the number of kernels launched
 int launch_igemm(const IgemmParams& p, cudaStream_t s);

@@ -998,10 +998,25 @@ __device__ __forceinline__ void slot_update(const FinalParams& p, const SlotStep
     p.xt_out[idx] = (xt - dxt) * mk;
 }
 
-// SLOT: a rolling batch (launch_final_slot) - row b takes its mode, coefficients and noise from its slot (slot_update), an
-// idle row is left as it is, and the row's step counter advances.  SLOT = false is the dense and ragged k_final: its code is
-// the part outside the `if constexpr (SLOT)` blocks, and its SASS is that of the kernel before the template.
-template <bool SLOT>
+// The DiffVC update of one element of a rolling batch's row b: k_final's mode 3, in its order, with the slot's coefficients
+// cf = {A, Bc, sigma} and, when sigma != 0, the request's own draws [n_feats][T_b]
+__device__ __forceinline__ void vc_slot_update(const FinalParams& p, const SlotStep& c, const float4 cf, int b, long long idx,
+                                               float mk, float est) {
+    const float xt = p.xt_in[idx], mu = __ldg(p.mu + idx);
+    float dxt = (mu - xt) * cf.x - est * cf.y;
+    if (cf.z != 0.f) {
+        const int m = (int)(idx - (long long)b * p.H * p.T), h = m / p.T;
+        dxt += __ldg(c.noise + (long long)h * unet_frames(p.lengths, b, p.T) + (m - h * p.T)) * cf.z;
+    }
+    p.xt_out[idx] = (xt - dxt) * mk;
+}
+
+// SLOT: FINAL_PLAN is the dense and ragged k_final: its code is the part outside the `if constexpr (SLOT)` blocks, and its
+// SASS is that of the kernel before the template.  FINAL_SLOT / FINAL_VC_SLOT: a rolling batch (launch_final_slot) - row b
+// takes its mode, coefficients and noise from its slot (slot_update for Grad-TTS, vc_slot_update for DiffVC), an idle row is
+// left as it is, and the row's step counter advances.
+enum FinalKind : int { FINAL_PLAN = 0, FINAL_SLOT = 1, FINAL_VC_SLOT = 2 };
+template <int SLOT>
 __global__ void __launch_bounds__(256) k_final(const FinalParams p, const SlotStep* slot, SlotSched* sched) {
     extern __shared__ __align__(16) float sm[];
     float* mean = sm; float* scale = mean + p.C; float* beta = scale + p.C; float* wf = beta + p.C;
@@ -1021,7 +1036,10 @@ __global__ void __launch_bounds__(256) k_final(const FinalParams p, const SlotSt
     if (!SLOT && p.mode != 0) { srow = *p.step; cf = p.coef[srow]; }
     auto update = [&](long long idx, float mk, float dot) {
         const float est = mk != 0.f ? dot + bf : 0.f;
-        if constexpr (SLOT) {
+        if constexpr (SLOT == FINAL_VC_SLOT) {
+            vc_slot_update(p, slot[b], p.coef[b], b, idx, mk, est);
+            return;
+        } else if constexpr (SLOT) {
             slot_update(p, slot[b], p.coef[b], b, idx, mk, est);
             return;
         }
@@ -1102,12 +1120,14 @@ static int final_grid(const FinalParams& p) {
 }
 
 int launch_final(const FinalParams& p, cudaStream_t s) {
-    k_final<false><<<dim3(final_grid(p), p.B), 256, 4 * p.C * sizeof(float), s>>>(p, nullptr, nullptr);
+    k_final<FINAL_PLAN><<<dim3(final_grid(p), p.B), 256, 4 * p.C * sizeof(float), s>>>(p, nullptr, nullptr);
     return 1;
 }
 
-int launch_final_slot(const FinalParams& p, const SlotStep* cur, SlotSched* sched, cudaStream_t s) {
-    k_final<true><<<dim3(final_grid(p), p.B), 256, 4 * p.C * sizeof(float), s>>>(p, cur, sched);
+int launch_final_slot(const FinalParams& p, const SlotStep* cur, SlotSched* sched, bool vc, cudaStream_t s) {
+    const dim3 grid(final_grid(p), p.B);
+    if (vc) k_final<FINAL_VC_SLOT><<<grid, 256, 4 * p.C * sizeof(float), s>>>(p, cur, sched);
+    else k_final<FINAL_SLOT><<<grid, 256, 4 * p.C * sizeof(float), s>>>(p, cur, sched);
     return 1;
 }
 
@@ -1129,6 +1149,32 @@ __global__ void k_slot_begin(const SlotBeginParams p) {
 
 int launch_slot_begin(const SlotBeginParams& p, cudaStream_t s) {
     k_slot_begin<<<(p.B + 127) / 128, 128, 0, s>>>(p);
+    return 1;
+}
+
+// k_slot_begin for a DiffVC slot plan, one block per slot: mode 1 for a live slot (vc_slot_update reads the noise slab only
+// when sigma != 0, so pf needs none), and the slot's conditioning row of step i into cond[b] - zeros for an idle slot, whose
+// folded row then adds nothing.  Each (row, sample) of k_cond_fold is computed on its own, so slot b's folded row has the
+// bits of the same cond row folded in a [N][B] table.
+__global__ void __launch_bounds__(128) k_vc_slot_begin(const VcSlotBeginParams p) {
+    const int b = blockIdx.x;
+    const SlotSched s = p.s.sched[b];
+    const bool live = s.i < s.n;
+    if (threadIdx.x == 0) {
+        SlotStep c;
+        c.i = s.i;
+        c.mode = live ? 1 : 0;
+        c.noise = live && s.stoc ? s.noise + (long long)s.i * p.s.H * s.T : nullptr;
+        p.s.cur[b] = c;
+        p.s.t_rows[b] = live ? s.t_tab[s.i] : 0.5f;
+        p.s.coef[b] = live ? s.coef_tab[s.i] : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    const float* row = live ? slot_cond_rows(s.coef_tab, s.n) + (long long)s.i * p.dc : nullptr;
+    for (int j = threadIdx.x; j < p.dc; j += 128) p.cond[(long long)b * p.dc + j] = live ? row[j] : 0.f;
+}
+
+int launch_vc_slot_begin(const VcSlotBeginParams& p, cudaStream_t s) {
+    k_vc_slot_begin<<<p.s.B, 128, 0, s>>>(p);
     return 1;
 }
 

@@ -24,6 +24,7 @@ import torch.nn.functional as F
 from .binding import Engine
 from .gradtts import (BaseModule, Mish, SinusoidalPosEmb, _ConvGNMish, _Gate, _LinAttn, _Resample, _Skip, _TimeResBlock)
 from .postnet import PostNet
+from .rolling import VcRollingSampler
 from .text_encoder import MelEncoder
 
 
@@ -140,24 +141,45 @@ class Diffusion(BaseModule):
         return (x0 * w + mean * (1.0 - w)) * mask
 
     # ---- engine ------------------------------------------------------------------------------
-    def engine(self) -> Engine:
+    def _device(self):
         dev = next(self.parameters()).device
         if dev.type != "cuda":
             raise RuntimeError("DiffVC sampling runs only on a CUDA device (sm_90a); move the module with .cuda() "
                                "first - there is no CPU fallback")
+        return dev
+
+    def _new_engine(self, dev) -> Engine:
+        return Engine(self.n_feats, self.dim_unet, 1, 64, self.beta_min, self.beta_max, 1000.0, device=dev.index,
+                      precision=self.precision, use_graph=self.use_graph, model="diffvc", dim_cond=self.dim_spk,
+                      use_ref_t=self.use_ref_t)
+
+    def engine(self) -> Engine:
+        dev = self._device()
         sig = (dev.index,) + tuple((p.data_ptr(), p._version) for p in self.estimator.parameters())
         if self._engine is None or self._engine.device != dev.index:
             if self._engine is not None:
                 self._engine.close()
-            self._engine = Engine(self.n_feats, self.dim_unet, 1, 64, self.beta_min, self.beta_max, 1000.0,
-                                  device=dev.index, precision=self.precision, use_graph=self.use_graph,
-                                  model="diffvc", dim_cond=self.dim_spk, use_ref_t=self.use_ref_t)
+            self._engine = self._new_engine(dev)
             self._engine_sig = None
         if sig != self._engine_sig:
             with torch.cuda.device(dev):
                 self._engine.load_state_dict({"estimator." + k: v for k, v in self.estimator.state_dict().items()})
             self._engine_sig = sig
         return self._engine
+
+    def rolling(self, capacity, max_frames):
+        """A VcRollingSampler (rolling.py) of `capacity` slots at up to `max_frames` frames with this module's configuration,
+        precision and current weights: utterances join and leave a running batch at any step.  The slot plan is a native
+        plan of its own, so the sampler holds an engine of its own and this module's `forward` calls stay usable alongside
+        it; weights changed later are not seen by the sampler."""
+        return self._rolling(VcRollingSampler, capacity, max_frames)
+
+    def _rolling(self, sampler, capacity, max_frames, *args):
+        dev = self._device()
+        eng = self._new_engine(dev)
+        with torch.cuda.device(dev):
+            eng.load_state_dict({"estimator." + k: v for k, v in self.estimator.state_dict().items()})
+            return sampler(*args, eng, capacity, max_frames)
 
     # ---- sampling (diffusion.py:164-205) ------------------------------------------------------
     @torch.no_grad()
@@ -220,22 +242,9 @@ def fix_len_compatibility(length, num_downsamplings_in_unet=2):
 
 
 @torch.no_grad()
-def convert_from_encoder(decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode="ml", *,
-                         ragged=False, x_ref_lengths=None):
-    """Drop-in for DiffVC/model/vc.py:107,110-127 - what `DiffVC.forward` does once `mean = self.encoder(x, x_mask)` and
-    `mean_ref = self.encoder(x_ref, x_ref_mask)` exist:
-
-        return convert_from_encoder(self.decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode)
-
-    The reference re-pads `mean` and `mean_x` to a length the U-Net accepts with a Python loop over the batch that indexes
-    `x_lengths[i]` on the host: 2B slice copies and B device-to-host synchronisations per call (vc.py:118-120).  Here the same
-    tensors are one masked pad each (bit-identical: a copy of the valid prefix into zeros), the only synchronisation left is
-    `int(x_lengths.max())`, which fixes the SHAPE of the returned tensor, and the noise draw is the reference's own call
-    (`randn_like` of a contiguous [B,n_feats,T'] tensor), so the generator stream is unchanged.  Returns (mean_x, y).
-
-    ragged=True (keyword only): the decoder samples row b on its own fix_len_compatibility(x_lengths[b]) frames and runs the
-    conditioning branch on its own x_ref_lengths[b] reference frames (the sum of x_ref_mask's row when not given), so each
-    row is the reference's B = 1 call on that utterance given the same draws; y is 0 past x_lengths[b]'s U-Net grid."""
+def decoder_inputs(decoder, x, x_lengths, mean):
+    """DiffVC/model/vc.py:104,107,111-123: (mean_x, z, x_mask_new, mean_new, max_length) - the decoder's inputs, with z's
+    draw (randn_like of the re-padded mean_x), as convert_from_encoder passes them to the decoder."""
     b, n_feats, t_in = x.shape
     max_length = int(x_lengths.max())                                              # :111 (host sync: output shape)
     if t_in != max_length:                                                         # the reference's x_mask (:104) has max_length frames
@@ -254,6 +263,27 @@ def convert_from_encoder(decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_re
     mean_new, mean_x_new = repad(mean), repad(mean_x)
     z = mean_x_new
     z += torch.randn_like(mean_x_new, device=mean_x_new.device)                    # :122-123
+    return mean_x, z, x_mask_new, mean_new, max_length
+
+
+@torch.no_grad()
+def convert_from_encoder(decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode="ml", *,
+                         ragged=False, x_ref_lengths=None):
+    """Drop-in for DiffVC/model/vc.py:107,110-127 - what `DiffVC.forward` does once `mean = self.encoder(x, x_mask)` and
+    `mean_ref = self.encoder(x_ref, x_ref_mask)` exist:
+
+        return convert_from_encoder(self.decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode)
+
+    The reference re-pads `mean` and `mean_x` to a length the U-Net accepts with a Python loop over the batch that indexes
+    `x_lengths[i]` on the host: 2B slice copies and B device-to-host synchronisations per call (vc.py:118-120).  Here the same
+    tensors are one masked pad each (bit-identical: a copy of the valid prefix into zeros), the only synchronisation left is
+    `int(x_lengths.max())`, which fixes the SHAPE of the returned tensor, and the noise draw is the reference's own call
+    (`randn_like` of a contiguous [B,n_feats,T'] tensor), so the generator stream is unchanged.  Returns (mean_x, y).
+
+    ragged=True (keyword only): the decoder samples row b on its own fix_len_compatibility(x_lengths[b]) frames and runs the
+    conditioning branch on its own x_ref_lengths[b] reference frames (the sum of x_ref_mask's row when not given), so each
+    row is the reference's B = 1 call on that utterance given the same draws; y is 0 past x_lengths[b]'s U-Net grid."""
+    mean_x, z, x_mask_new, mean_new, max_length = decoder_inputs(decoder, x, x_lengths, mean)
     if ragged:
         if x_ref_lengths is None:
             x_ref_lengths = x_ref_mask.sum((1, 2)).round().to(torch.int64)
@@ -334,9 +364,54 @@ class DiffVC(BaseModule):
         return convert_from_encoder(self.decoder, x, x_lengths, mean, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode,
                                     ragged=True, x_ref_lengths=x_ref_lengths)
 
+    def rolling(self, capacity, max_frames):
+        """A DiffVCRollingSampler: voice conversion of single utterances through a rolling decoder batch of `capacity` slots
+        at up to `max_frames` U-Net frames (a multiple of 4).  submit(x, x_ref, c, n_timesteps, mode="ml") takes one
+        utterance's B = 1 `forward` arguments; each result is that call's (mean_x, y)."""
+        return self.decoder._rolling(DiffVCRollingSampler, capacity, max_frames, self)
+
     def compute_loss(self, x, x_lengths, x_ref, c):                                 # :129-144
         x, x_lengths, x_ref, c = self.relocate_input([x, x_lengths, x_ref, c])
         x_mask = sequence_mask(x_lengths).unsqueeze(1).to(x.dtype)
         mean = self.encoder(x, x_mask).detach()
         mean_ref = self.encoder(x_ref, x_mask).detach()                            # the reference uses x_mask here (:142)
         return self.decoder.compute_loss(x, x_mask, mean, x_ref, mean_ref, c)
+
+
+class DiffVCRollingSampler(VcRollingSampler):
+    """`DiffVC.rolling`: one utterance per request through a rolling batch of the model's decoder.
+
+    submit(x [1, n_feats, L], x_ref [1, n_feats, R], c [1, 256], n_timesteps, mode="ml") runs the encoder on x and x_ref
+    and forms the decoder's inputs as `DiffVC.forward` does at B = 1 (decoder_inputs: mean_x, the re-padded mean, and z's
+    draw), then queues the decoder request, whose step noise is drawn after z, in `forward`'s order.  advance / drain return
+    {id: (mean_x [1, n_feats, L], y [1, n_feats, L])}."""
+
+    def __init__(self, model, engine, capacity, max_frames):
+        self.model = model
+        self._mean_x = {}
+        super().__init__(engine, capacity, max_frames)
+
+    def submit(self, x, x_ref, c, n_timesteps, mode="ml") -> int:
+        F = self.engine.n_feats
+        for name, v in (("x", x), ("x_ref", x_ref)):
+            if not isinstance(v, torch.Tensor) or v.dim() != 3 or v.shape[-1] < 1:
+                raise ValueError(f"{name}: expected a [1, {F}, frames] tensor, got {getattr(v, 'shape', type(v).__name__)}")
+        L, R = x.shape[-1], x_ref.shape[-1]
+        x, x_ref = self._tensor("x", x, (1, F, L)), self._tensor("x_ref", x_ref, (1, F, R))
+        c = self._tensor("c", c, (1, 256))
+        if fix_len_compatibility(L) > self.max_frames:
+            raise ValueError(f"x has {L} frames: the decoder runs {fix_len_compatibility(L)} > max_frames = {self.max_frames}")
+        self._steps(n_timesteps)
+        if mode not in ("pf", "em", "ml"):
+            raise ValueError(f"mode must be one of ['pf', 'em', 'ml'], got {mode!r}")
+        x_mask, x_ref_mask = torch.ones(1, 1, L, device=self.device), torch.ones(1, 1, R, device=self.device)
+        mean = self.model.encoder(x, x_mask)
+        mean_ref = self.model.encoder(x_ref, x_ref_mask)
+        mean_x, z, x_mask_new, mean_new, _ = decoder_inputs(self.model.decoder, x, torch.tensor([L], device=self.device), mean)
+        rid = super().submit(z, x_mask_new, mean_new, x_ref, x_ref_mask, mean_ref, c, n_timesteps, mode)
+        self._mean_x[rid] = mean_x
+        return rid
+
+    def _result(self, r, mel):
+        mean_x = self._mean_x.pop(r.rid)
+        return mean_x, mel[:, :, :mean_x.shape[-1]]
