@@ -124,7 +124,7 @@ def reverse_diffusion(p, cfg, z, mask, mean, ref, ref_mask, mean_ref, c, n_times
     xt = z * mask
     for i in range(n_timesteps):
         t, A, Bc, sigma, g0t = step_coefficients(cfg, n_timesteps, i, mode)
-        time = t * torch.ones(z.shape[0], dtype=z.dtype)
+        time = t * torch.ones(z.shape[0], dtype=z.dtype, device=z.device)
         xt_ref = ((ref * g0t + mean_ref * (1.0 - g0t)) * ref_mask)[:, None]          # compute_diffused_mean, :151-155
         est = estimator(p, cfg, xt, mask, mean, xt_ref, ref_mask, c, time)
         if mode == "pf":

@@ -706,8 +706,9 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                     }
                 }
                 if (!SIDE && p.ostats) {
-                    // GroupNorm partials of this 32-column chunk: 8-channel sub-sums first (static register indexing),
-                    // then merged to the group width cpg (8 -> 4 groups, 16 -> 2 groups, >= 32 -> 1 group)
+                    // GroupNorm partials of this 32-column chunk: 8-channel sub-sums first (static register indexing; cpg is
+                    // a multiple of 8, so none straddles a group), then merged as far as no merged partial straddles one:
+                    // the chunk starts at a multiple of 32, so cpg % 32 == 0 -> 1 partial, cpg % 16 == 0 -> 2, else 4
                     float s8[4], q8[4];
 #pragma unroll
                     for (int k = 0; k < 4; ++k) {
@@ -716,7 +717,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         for (int i = 0; i < 8; ++i) { const float x = valid ? v[8 * k + i] : 0.f; s += x; q = fmaf(x, x, q); }
                         s8[k] = s; q8[k] = q;
                     }
-                    const int ngrp = cpg == 8 ? 4 : (cpg == 16 ? 2 : 1);
+                    const int ngrp = cpg % 32 == 0 ? 1 : (cpg % 16 == 0 ? 2 : 4);
                     if (ngrp == 2) { s8[0] += s8[1]; q8[0] += q8[1]; s8[1] = s8[2] + s8[3]; q8[1] = q8[2] + q8[3]; }
                     if (ngrp == 1) { s8[0] += s8[1] + s8[2] + s8[3]; q8[0] += q8[1] + q8[2] + q8[3]; }
 #pragma unroll
@@ -737,7 +738,9 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
             }
             if (GEOM != G_PW && p.ostats) {
                 asm volatile("bar.sync 1, 256;" ::: "memory");
-                const int gb = n0 / cpg, ng = (NT + cpg - 1) / cpg;
+                // every group the tile's columns n0 .. n0 + NT - 1 touch (a tile may start inside a group; <= 8 under
+                // conv_tc_ntile, the slots per warp)
+                const int gb = n0 / cpg, ng = (n0 + NT - 1) / cpg - gb + 1;
                 const int r = tid / (ng * 2), e = tid - r * (ng * 2);       // output row of the tile, (group, sum | squares)
                 if (tid < ng * 2 * ROWS) {
                     double tot = 0.0;

@@ -363,7 +363,7 @@ __global__ void __launch_bounds__(IG_THREADS, 3) k_igemm(const IgemmParams p) {
         atomicAdd(&s_st[(g1 - gb) * 2 + 0], (double)st_s[1]);
         atomicAdd(&s_st[(g1 - gb) * 2 + 1], (double)st_q[1]);
         __syncthreads();
-        const int ng = (IG_TN + cpg - 1) / cpg;   // groups this N tile touches (cpg >= 8 -> <= 8)
+        const int ng = (n0 + IG_TN - 1) / cpg - gb + 1;   // groups this N tile touches (it may start inside one; <= 8)
         if (tid < ng * 2) {
             const int g = gb + (tid >> 1);
             atomicAdd(&p.ostats[((long long)b * kGroups + g) * 2 + (tid & 1)], s_st[tid]);
@@ -501,7 +501,7 @@ __device__ __forceinline__ void first_conv_body(const FirstConvParams& p) {
         }
     }
     __syncthreads();
-    const int ng = (64 + cpg - 1) / cpg;
+    const int ng = (n0 + 63) / cpg - gb + 1;       // groups the 64 channels touch (the tile may start inside one)
     if (p.ostats && tid < ng * 2) atomicAdd(&p.ostats[((long long)b * kGroups + gb + (tid >> 1)) * 2 + (tid & 1)], s_st[tid]);
 }
 __global__ void __launch_bounds__(256) k_first_conv(const FirstConvParams p) { first_conv_body<false>(p); }
