@@ -40,6 +40,12 @@ enum { SBK_PREC_FP32 = 0,   /* CUDA-core FFMA, fp32 operands (bit-faithful class
                                that are summed in round-to-nearest fp32 (the tensor core truncates its accumulator);
                                softmax / Mish / GN exact fp32.  The default of the drop-in modules: matches the
                                reference's fp32 CPU arithmetic to 2-3e-6 per estimator call                   */
+enum { SBK_PREC_F16 = 4 };  /* wgmma f16 on fp16 operand tensors: SBK_PREC_BF16's layout, tiling and launches with
+                               fp16 elements (11 significant bits, tf32's, instead of bf16's 8), rounded to nearest
+                               even and saturated to +-65504; fp32 accumulate, raw conv outputs, GN statistics,
+                               softmax and sampler state fp32.  tf32-class error at bf16's operand bytes and MMA
+                               rate.  Both models' samplers (DiffVC's RefBlock branch runs tf32 operands, as in the
+                               bf16 mode) and the PostNet (tf32 operands); the vocoder refuses it               */
 
 enum { SBK_MODEL_GRADTTS = 0, SBK_MODEL_DIFFVC = 1 };
 
@@ -269,8 +275,8 @@ int sbk_debug_capture(sbk_handle* h, int on);
  * 1 = channel-chunk planar [B][H][C/4][W][4] (tensor-core modes) */
 int sbk_debug_layout(const sbk_handle* h);
 /* test hook: layout of ONE named intermediate (the bf16 mode mixes fp32 raw outputs with bf16 operand tensors):
- * 0 / 1 as above, 2 = [B][H][C/8][W][8] stored as bf16 (sbk_debug_read widens it to fp32; dst must be host memory),
- * -1 = unknown name */
+ * 0 / 1 as above, 2 = [B][H][C/8][W][8] stored as bf16, 4 = the same stored as fp16 (sbk_debug_read widens both to fp32;
+ * dst must be host memory), -1 = unknown name */
 int sbk_debug_op_layout(const sbk_handle* h, const char* name);
 /* test hook: enumerate intermediate names */
 int sbk_debug_num(const sbk_handle* h);
@@ -287,6 +293,7 @@ const char* sbk_debug_name(const sbk_handle* h, int i);
  *   SBK_PREC_TF32 (a fresh handle)  tf32 operands;
  *   SBK_PREC_FP32X3 (and FP32, which maps to it)  fp32-class: x*w = x_hi*w_hi + one f16 correction MMA, chunked accumulation;
  *   SBK_PREC_BF16  bf16 weights and bf16 conv inputs (the LeakyReLU operands); the residual stream stays fp32.
+ *   SBK_PREC_F16 is a sampler mode: the vocoder refuses it (SBK_ERR_UNSUPPORTED).
  * In every mode conv_post + tanh, the transposed convs' overlap-add, the MRF mean and the waveform are fp32, and the forward
  * makes the same launches. */
 typedef struct sbk_vocoder sbk_vocoder;
@@ -418,7 +425,7 @@ typedef struct sbk_postnet_config {
     int32_t device;
     int32_t dim;          /* PostNet(dim) (vc.py:34; DiffVC enc_dim = 128): 64, 128 or a multiple of 256                  */
     int32_t groups;       /* GroupNorm groups (postnet.py:16,27,41, default 8): must be 8                                       */
-    int32_t precision;    /* SBK_PREC_*: FP32X3 and FP32 run the fp32x3 split, TF32 and BF16 run tf32 operands            */
+    int32_t precision;    /* SBK_PREC_*: FP32X3 and FP32 run the fp32x3 split, TF32, BF16 and F16 run tf32 operands      */
 } sbk_postnet_config;
 /* PostNet.__init__ (postnet.py:41-45).  SBK_ERR_UNSUPPORTED for any other dim / groups. */
 int sbk_postnet_create(const sbk_postnet_config* cfg, sbk_postnet** out);

@@ -16,11 +16,11 @@ import __graft_entry__ as ge  # noqa: E402
 ge.build()
 from helpers import case_id, case_inputs, rel_l2, stoc_noise  # noqa: E402
 from oracle import gradtts_oracle as O  # noqa: E402
-from oracle.precision_model import operand_rounding  # noqa: E402
+from precision_model_fp16 import operand_rounding  # noqa: E402  (oracle/precision_model.py + the fp16 mode)
 from speech_backbones_b200.binding import Engine  # noqa: E402
 
 golden = torch.load(os.path.join(ROOT, "tests", "golden", "gradtts_golden.pt"), weights_only=False)
-for mode in ("tf32", "bf16", "fp32x3"):
+for mode in ("tf32", "bf16", "fp16", "fp32x3"):
     eng = None
     for c in golden["cases"]:
         if c["n_spks"] != 1 or (c["kind"] == "traj" and mode == "fp32x3"):

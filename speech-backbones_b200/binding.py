@@ -10,7 +10,10 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsbk.so")
 
-PREC = {"fp32": 0, "tf32": 1, "bf16": 2, "fp32x3": 3}
+PREC = {"fp32": 0, "tf32": 1, "bf16": 2, "fp32x3": 3}          # every engine's modes, the vocoder's included
+# The samplers' modes (Engine, and the PostNet that DiffVC builds with the sampler's mode): PREC and "fp16" (sbk.h
+# SBK_PREC_F16), which the vocoder has no kernels for (hifigan.py refuses it) and the PostNet runs as tf32, like "bf16"
+SAMPLER_PREC = dict(PREC, fp16=4)
 MODEL = {"gradtts": 0, "diffvc": 1}
 
 EXPORTS = [
@@ -100,9 +103,9 @@ def _ptr(t):
     return None if t is None else C.c_void_p(t.data_ptr())
 
 
-def _check_precision(precision):
-    if precision not in PREC:
-        raise ValueError(f"precision must be one of {sorted(PREC)}, got {precision!r}")
+def _check_precision(precision, names=PREC):
+    if precision not in names:
+        raise ValueError(f"precision must be one of {sorted(names)}, got {precision!r}")
     return precision
 
 
@@ -242,7 +245,7 @@ class Engine(_NativeHandle):
                  use_ref_t=True):
         super().__init__()
         self.cfg = SbkConfig(MODEL[model], n_feats, dim, n_spks, spk_emb_dim, beta_min, beta_max, pe_scale,
-                             device, PREC[precision], 1 if use_graph else 0, dim_cond, 1 if use_ref_t else 0)
+                             device, SAMPLER_PREC[precision], 1 if use_graph else 0, dim_cond, 1 if use_ref_t else 0)
         self.model = model
         self.dim_cond = dim_cond
         _check(self._create(self.cfg), "sbk_create")
@@ -499,7 +502,8 @@ class Engine(_NativeHandle):
         _check(self.lib.sbk_debug_capture(self.h, 1 if on else 0), "sbk_debug_capture")
 
     def debug_layout(self, name=None):
-        """0: [B][H][W][C]; 1: [B][H][C/4][W][4]; 2: [B][H][C/8][W][8] (bf16 operand tensor, widened to fp32 by debug_read)."""
+        """0: [B][H][W][C]; 1: [B][H][C/4][W][4]; 2 / 4: [B][H][C/8][W][8] (bf16 / fp16 operand tensor, widened to fp32 by
+        debug_read)."""
         if name is not None:
             return int(self.lib.sbk_debug_op_layout(self.h, name.encode()))
         return int(self.lib.sbk_debug_layout(self.h))

@@ -42,7 +42,8 @@ struct Op {
     OpKind kind; std::string name;
     FirstConvParams fc; IgemmParams ig; ConvTcParams tc; GnActParams ga; ResFinalParams rf; AttnCtxParams cx; AttnMixParams mx; FinalParams fn;
     const float* dbg_ptr = nullptr; int64_t dbg_numel = 0;
-    int dbg_fmt = 0;               // layout of the named output: 0 NHWC fp32, 1 [B][H][C/4][W][4] fp32, 2 [B][H][C/8][W][8] bf16
+    int dbg_fmt = 0;               // layout of the named output: 0 NHWC fp32, 1 [B][H][C/4][W][4] fp32, 2 [B][H][C/8][W][8] bf16,
+                                   // 4 [B][H][C/8][W][8] fp16
     double flops = 0, bytes = 0;   // algorithmic work of this launch
     float* dbg_copy = nullptr;     // snapshot taken right after the launch when debug capture is on
 };
@@ -231,7 +232,7 @@ extern "C" int sbk_create(const sbk_config* cfg, sbk_handle** out) {
     if (cfg->dim <= 0 || cfg->dim % 64 != 0) return fail(SBK_ERR_ARG, "sbk_create: dim must be a positive multiple of 64 (got %d)", cfg->dim);
     if (cfg->n_feats <= 0 || cfg->n_feats % 4 != 0) return fail(SBK_ERR_ARG, "sbk_create: n_feats must be a multiple of 4 (two stride-2 levels), got %d", cfg->n_feats);
     if (cfg->n_spks < 1 || cfg->spk_emb_dim <= 0) return fail(SBK_ERR_ARG, "sbk_create: bad speaker configuration");
-    if (cfg->precision < SBK_PREC_FP32 || cfg->precision > SBK_PREC_FP32X3) return fail(SBK_ERR_ARG, "sbk_create: unknown precision %d", cfg->precision);
+    if (cfg->precision < SBK_PREC_FP32 || cfg->precision > SBK_PREC_F16) return fail(SBK_ERR_ARG, "sbk_create: unknown precision %d", cfg->precision);
     sbk_handle* h = new sbk_handle();
     h->cfg = *cfg;
     build_spec(h);
@@ -371,7 +372,8 @@ extern "C" int sbk_pack(sbk_handle* h) {
         }
         TRY(repack(h, "estimator.final_block.block.0.weight", "estimator.final_block.w", (size_t)h->cfg.dim * h->cfg.dim * 9, conv_pack));
     } else {
-        const int form = h->cfg.precision == SBK_PREC_BF16 ? FORM_BF16 : (x3 ? FORM_X3 : FORM_TF32);
+        const int form = h->cfg.precision == SBK_PREC_BF16 ? FORM_BF16 : h->cfg.precision == SBK_PREC_F16 ? FORM_F16
+                       : (x3 ? FORM_X3 : FORM_TF32);
         for (size_t k = 0; k < h->resnets.size(); ++k) {
             const ResnetInfo& r = h->resnets[k];
             if (k != 0) TRY(pack_tc(h, r.prefix + ".block1.block.0.weight", r.prefix + ".block1.wtc", r.cout, r.cin, G_C3, form));
@@ -396,7 +398,7 @@ extern "C" int sbk_pack(sbk_handle* h) {
         for (int k = 0; k < 5; ++k) {
             const std::string q = std::string("estimator.ref_block.") + nm[k];
             // the hoisted RefBlock branch (sbk_vc_conditioning) runs once per call outside the loop, on the tensor cores in
-            // every precision: tf32 operands with fp32 activations for the tf32 / bf16 handles, (w_hi, correction) image pairs for
+            // every precision: tf32 operands with fp32 activations for the tf32 / bf16 / fp16 handles, (w_hi, correction) image pairs for
             // the fp32-class handles (fp32x3 and the CUDA-core fp32 mode, whose U-Net kernels have no InstanceNorm/GLU path)
             TRY(pack_tc(h, q + ".0.weight", q + ".wtc", co[k], ci[k], G_C3, prec_runs_x3(h->cfg.precision) ? FORM_X3 : FORM_TF32));
         }
@@ -436,8 +438,9 @@ static size_t layout(const sbk_handle* h, int B, int T, int tb_rows, Arena& ar, 
     const size_t P[3] = {(size_t)H * T, (size_t)(H / 2) * (T / 2), (size_t)(H / 4) * (T / 4)};
     const int C[3] = {dim, dim * 2, dim * 4};
     auto f = [&](size_t n) { return (float*)ar.take(n * sizeof(float)); };
-    // operand-form tensors (conv inputs): fp32, or bf16 in the bf16 mode; A[] holds the raw conv outputs (always fp32)
-    const size_t osz = c.precision == SBK_PREC_BF16 ? 2 : 4;
+    // operand-form tensors (conv inputs): fp32, or bf16 / fp16 in the bf16 / fp16 modes; A[] holds the raw conv outputs
+    // (always fp32)
+    const size_t osz = c.precision == SBK_PREC_BF16 || c.precision == SBK_PREC_F16 ? 2 : 4;
     const bool x3 = c.precision == SBK_PREC_FP32X3;
     Bufs b{};
     // (fp32x3 keeps no correction twin of these: the conv kernels derive the correction operand in shared memory)
@@ -527,10 +530,11 @@ static int build_plan(sbk_handle* h, int B, int T, int tb_rows) {
     const int num_sms = device_sm_count();
     const char* rows_env = getenv("SBK_CONV3_ROWS");
     const int conv_rows_env = rows_env ? atoi(rows_env) : 0;
-    const bool b16 = c.precision == SBK_PREC_BF16;          // operand tensors in bf16 [B][H][C/8][W][8]
+    const bool f16 = c.precision == SBK_PREC_F16;
+    const bool b16 = c.precision == SBK_PREC_BF16 || f16;   // operand tensors in bf16 / fp16 [B][H][C/8][W][8]
     const double osz = b16 ? 2.0 : 4.0;                     // bytes per operand-tensor element
-    const int fmt_raw = use_tc ? 1 : 0, fmt_opnd = b16 ? 2 : fmt_raw;
-    const int form = b16 ? FORM_BF16 : (x3 ? FORM_X3 : (use_tc ? FORM_TF32 : FORM_NHWC));
+    const int fmt_raw = use_tc ? 1 : 0, fmt_opnd = f16 ? 4 : (b16 ? 2 : fmt_raw);
+    const int form = f16 ? FORM_F16 : b16 ? FORM_BF16 : (x3 ? FORM_X3 : (use_tc ? FORM_TF32 : FORM_NHWC));
     auto push = [&](Op& op, const float* dbg, int64_t numel) {
         op.dbg_ptr = dbg; op.dbg_numel = numel;
         // raw Block-conv outputs (and the attention contexts) are fp32; every other named output is an operand tensor
@@ -1714,8 +1718,8 @@ extern "C" int sbk_debug_capture(sbk_handle* h, int on) {
     return SBK_OK;
 }
 extern "C" int sbk_debug_layout(const sbk_handle* h) { return (h && h->cfg.precision != SBK_PREC_FP32) ? 1 : 0; }
-// layout of one named intermediate: 0 [B][H][W][C] fp32, 1 [B][H][C/4][W][4] fp32, 2 [B][H][C/8][W][8] (bf16 in HBM;
-// sbk_debug_read widens it to fp32), -1 unknown name
+// layout of one named intermediate: 0 [B][H][W][C] fp32, 1 [B][H][C/4][W][4] fp32, 2 / 4 [B][H][C/8][W][8] (bf16 / fp16
+// in HBM; sbk_debug_read widens it to fp32), -1 unknown name
 extern "C" int sbk_debug_op_layout(const sbk_handle* h, const char* name) {
     if (!h || !name) return -1;
     for (auto& op : h->plan.ops) if (op.name == name) return op.dbg_fmt;

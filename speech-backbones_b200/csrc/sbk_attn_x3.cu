@@ -10,7 +10,9 @@
 // blocks are kept).  Per item and head one partial {max[32], sum[32], S[32][32]} is written, merged by k_attn_ctx.
 //
 // Precision modes.  tf32: tf32 projection, fp32 softmax, tf32 context (P and V fp32 in shared memory, read as tf32).
-// bf16: the activations and weights are bf16 (a stage carries 64 channels), the rest as tf32.  fp32x3: every product is
+// bf16 / fp16: the activations and weights are bf16 / fp16 (a stage carries 64 channels), the rest as tf32: the
+// projection's result k, v is fp32 in registers whatever the operand type, so the softmax and P V^T run exactly as in the
+// bf16 mode and nothing past the projection is stored in fp16 (no saturation point past it).  fp32x3: every product is
 // fp32-class: each 32-channel K stage runs as an f16 correction sub-stage on the packed fp16 chunks ({x_lo, x*2^-12} x
 // {w, w_lo*2^12}, sbk_internal.h: corr_chunk) followed by the tf32 main sub-stage (x_hi * w_hi), and the context adds
 //     [ P_lo V^T + P V_lo^T ]  from  Pc = {P_lo*2^8, P*2^-4},  Vc = {V*2^-8, V_lo*2^4}  (fp16 images)
@@ -41,7 +43,7 @@ static_assert(SMEM <= 227 * 1024, "shared memory budget");
 static_assert(XS <= OPI && STAGES == 2, "fp32x3: the converted x fits a context image; a K stage is the whole ring");
 }
 
-// MODE: 0 = tf32, 1 = bf16, 2 = fp32x3.  p.in0: x (fp32x3: its correction chunks are derived here: the loader brings x with the main sub-stage only and the consumers convert it into the idle Pc / Vc images, alternating
+// MODE: 0 = tf32, 1 = bf16, 2 = fp32x3, 3 = fp16.  p.in0: x (fp32x3: its correction chunks are derived here: the loader brings x with the main sub-stage only and the consumers convert it into the idle Pc / Vc images, alternating
 // between them per K stage so that one warpgroup may still read the last stage's chunks); p.c0 = C; p.wpk: the k|v rows
 // of to_qkv as per-stage images [k|v][chunk][row][16 B] (fp32x3: [32-channel stage][hi | correction][k|v]...,
 // sbk_conv_tc.cu attn_kv_pack_image);
@@ -54,8 +56,8 @@ template <int MODE, bool RAG = false>
 __global__ void __launch_bounds__(kx3::THREADS, 1) k_attn_kv_wg(const ConvTcParams p) {
     using namespace kx3;
     constexpr bool X3 = MODE == 2;
-    constexpr int EPC = MODE == 1 ? 8 : 4;                         // channels per 16-byte chunk
-    constexpr int KMAIN = MODE == 1 ? K_BF16 : K_TF32;
+    constexpr int EPC = MODE == 1 || MODE == 3 ? 8 : 4;            // channels per 16-byte chunk
+    constexpr int KMAIN = MODE == 1 ? K_BF16 : MODE == 3 ? K_F16 : K_TF32;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* sS = smem;                                            // [STAGES][X | Wk | Wv]
     uint8_t* kp = sS + STAGES * STAGE;                             // K, then P (fp32)
@@ -281,7 +283,7 @@ static int launch_kv(const ConvTcParams& p, cudaStream_t s) {
     static DevCache cache;
     const int num_sms = cache.get(reinterpret_cast<const void*>(k_attn_kv_wg<MODE, RAG>));
     if (num_sms <= 0) return -1;
-    if (p.c0 % (kx3::KCH * (MODE == 1 ? 8 : 4)) != 0) return -1;
+    if (p.c0 % (kx3::KCH * (MODE == 1 || MODE == 3 ? 8 : 4)) != 0) return -1;
     const long long total = (long long)p.B * ((p.H * p.W + kx3::PX - 1) / kx3::PX);
     const int grid = (int)(total < num_sms ? total : num_sms);
     k_attn_kv_wg<MODE, RAG><<<grid, kx3::THREADS, kx3::SMEM, s>>>(p);
@@ -292,7 +294,8 @@ static int launch_kv(const ConvTcParams& p, cudaStream_t s) { return p.lengths ?
 
 int attn_kv_tile_pixels() { return kx3::PX; }
 int launch_attn_kv(const ConvTcParams& p, cudaStream_t s) {
-    return p.form == FORM_X3 ? launch_kv<2>(p, s) : p.form == FORM_BF16 ? launch_kv<1>(p, s) : launch_kv<0>(p, s);
+    return p.form == FORM_X3 ? launch_kv<2>(p, s) : p.form == FORM_BF16 ? launch_kv<1>(p, s)
+         : p.form == FORM_F16 ? launch_kv<3>(p, s) : launch_kv<0>(p, s);
 }
 
 }  // namespace sbk

@@ -1,6 +1,6 @@
 // Warpgroup-MMA (wgmma) implicit-GEMM convolutions for sm_90a: the 3x3 Block convs (81.5 % of the step's MACs), the
 // 1x1 channel mixes (res_conv, attention apply), Downsample / Upsample, the vocoder's dilated Conv1d and the 7x7 convs of
-// DiffVC's PostNet (G_C7: one kernel row per ring stage, see Geo<G_C7>).  tf32 (or bf16)
+// DiffVC's PostNet (G_C7: one kernel row per ring stage, see Geo<G_C7>).  tf32 (or bf16 / fp16)
 // operands from shared memory, fp32 accumulation in registers.
 //
 //   D[pixel][cout] (fp32, registers) += A[pixel][tap, cin] (smem) * W[cout][tap, cin] (smem)
@@ -141,9 +141,14 @@ template <int GEOM, int NT, int R> constexpr bool x3_depth_ok = Depth<GEOM, NT, 
 // RAG: a ragged batch (ConvTcParams::lengths non-null): each sample's strips (Conv1d) or images (the U-Net geometries) end at
 // its own edge, inputs at or past it read as zero and its tiles wholly past it are not visited.  A dense batch runs the
 // RAG = false kernels.
-template <int GEOM, bool BF16, int NT, bool RES, bool X3, bool VOC = false, int R = 1, bool RAG = false>
+//
+// KIND: the MMA kind of the operands, K_TF32 (4-byte operands: tf32, fp32x3) or a 16-bit one, K_BF16 / K_F16 (FORM_BF16 /
+// FORM_F16: the same layout and tiling, E16<KIND> converts).
+template <int GEOM, int KIND, int NT, bool RES, bool X3, bool VOC = false, int R = 1, bool RAG = false>
 __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
-    static_assert(!(X3 && BF16), "fp32x3 runs on tf32 operands");
+    constexpr bool H16 = KIND != K_TF32;                   // 16-bit operand tensors and weights
+    using E = E16<H16 ? KIND : K_BF16>;
+    static_assert(!(X3 && H16), "fp32x3 runs on tf32 operands");
     using G = Geo<GEOM, R>;
     using D = Depth<GEOM, NT, R>;
     constexpr int NACC = G::NACC, ROWS = G::ROWS;
@@ -163,22 +168,22 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
     constexpr int STAGES = D::STAGES, LDS = D::LDS;
     constexpr int LAG = STAGES >= 3 ? STAGES - 2 : 0;      // G_DOWN only: cp.async groups in flight behind the newest
     constexpr int HR = G::HR, PXP = G::PXP, TAPS = G::TAPS, KCH = G::KCH;
-    constexpr int EPC = BF16 ? 8 : 4;                      // elements per 16-byte channel chunk
+    constexpr int EPC = H16 ? 8 : 4;                       // elements per 16-byte channel chunk
     constexpr int CPS = KCH * EPC;                         // input channels per stage
     constexpr bool C1 = geom_is_c1(GEOM);                  // Conv1d strip geometry
     constexpr bool RAG2 = RAG && !C1;                      // a ragged Grad-TTS batch (unet_edge)
-    // bf16 mode: the raw Block-conv outputs (GroupNorm inputs) stay fp32 [C/4]; every other output is an operand tensor
-    // of a later tensor-core kernel and is written as bf16 [B][H][C/8][W][8].  The vocoder's forms (VF16) instead pick
-    // the dtype per output: bf16 for an activated output (act_out) and the second output act, fp32 for the others.
-    constexpr bool VF16 = BF16 && (C1 || VOC);
-    constexpr bool OUT16 = BF16 && GEOM != G_C3 && !VF16;
+    // bf16 / fp16 modes: the raw Block-conv outputs (GroupNorm inputs) stay fp32 [C/4]; every other output is an operand
+    // tensor of a later tensor-core kernel and is written as 16-bit [B][H][C/8][W][8].  The vocoder's forms (VF16) instead
+    // pick the dtype per output: bf16 for an activated output (act_out) and the second output act, fp32 for the others.
+    constexpr bool VF16 = H16 && (C1 || VOC);
+    constexpr bool OUT16 = H16 && GEOM != G_C3 && !VF16;
     constexpr int PLANE = HR * PXP * 16;                   // bytes between K chunks of the A tile
     constexpr int A_STAGE_BYTES = KCH * PLANE;
     constexpr int B_STAGE_BYTES = TAPS * KCH * NT * 16;
     constexpr bool BULK = GEOM != G_DOWN;                  // A tile = contiguous runs -> cp.async.bulk (no LSU work)
     constexpr int SPAN = TPX;                              // output pixels per tile along W
     constexpr int FR = NW / 2;                             // accumulator registers per thread and accumulator
-    constexpr int KMAIN = BF16 ? K_BF16 : K_TF32;
+    constexpr int KMAIN = KIND;
 
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* sA = smem;                                            // [STAGES][KCH][HR][PXP][16]
@@ -642,8 +647,8 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
 #pragma unroll
                         for (int j = 0; j < 4; ++j) {
                             const uint4 a = __ldg(ap + (long long)j * Wo);
-                            v[8 * j + 0] += bf16_lo(a.x); v[8 * j + 1] += bf16_hi(a.x); v[8 * j + 2] += bf16_lo(a.y); v[8 * j + 3] += bf16_hi(a.y);
-                            v[8 * j + 4] += bf16_lo(a.z); v[8 * j + 5] += bf16_hi(a.z); v[8 * j + 6] += bf16_lo(a.w); v[8 * j + 7] += bf16_hi(a.w);
+                            v[8 * j + 0] += E::lo(a.x); v[8 * j + 1] += E::hi(a.x); v[8 * j + 2] += E::lo(a.y); v[8 * j + 3] += E::hi(a.y);
+                            v[8 * j + 4] += E::lo(a.z); v[8 * j + 5] += E::hi(a.z); v[8 * j + 6] += E::lo(a.w); v[8 * j + 7] += E::hi(a.w);
                         }
                     } else {
                         const float* ap = p.addin + obase + (cb / 4) * cstride;
@@ -667,8 +672,8 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
                         uint4* op = reinterpret_cast<uint4*>(p.out) + ochunk + (long long)(cb / 8) * Wo;
 #pragma unroll
                         for (int j = 0; j < 4; ++j)
-                            op[(long long)j * Wo] = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
-                                                               pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
+                            op[(long long)j * Wo] = make_uint4(E::pack(v[8 * j], v[8 * j + 1]), E::pack(v[8 * j + 2], v[8 * j + 3]),
+                                                               E::pack(v[8 * j + 4], v[8 * j + 5]), E::pack(v[8 * j + 6], v[8 * j + 7]));
                     } else if constexpr (VF16) {
                         // bf16 [C/8] chunks of the activated operand (out, or lrelu(out) through act); fp32 x / Z otherwise
                         auto st16 = [&](void* base, float sl) {
@@ -924,34 +929,43 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p) {
 
 template <int GEOM, bool BF16, int NT, bool RES = false, int R = 1>
 __global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc(const ConvTcParams p) {
-    conv_tc_body<GEOM, BF16, NT, RES, false, false, R>(p);
+    conv_tc_body<GEOM, BF16 ? K_BF16 : K_TF32, NT, RES, false, false, R>(p);
+}
+// fp16 operands (FORM_F16): FORM_BF16's kernels with the f16 MMA and conversions
+template <int GEOM, int NT, bool RES = false, int R = 1>
+__global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc_f16(const ConvTcParams p) {
+    conv_tc_body<GEOM, K_F16, NT, RES, false, false, R>(p);
 }
 template <int GEOM, int NT, bool RES = false, int R = 1>
 __global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc_x3(const ConvTcParams p) {
-    conv_tc_body<GEOM, false, NT, RES, true, false, R>(p);
+    conv_tc_body<GEOM, K_TF32, NT, RES, true, false, R>(p);
 }
-// a ragged U-Net batch (ConvTcParams::lengths): tf32 / bf16, and fp32x3
+// a ragged U-Net batch (ConvTcParams::lengths): tf32 / bf16, fp16, and fp32x3
 template <int GEOM, bool BF16, int NT, bool RES = false, int R = 1>
 __global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc_ragged(const ConvTcParams p) {
-    conv_tc_body<GEOM, BF16, NT, RES, false, false, R, true>(p);
+    conv_tc_body<GEOM, BF16 ? K_BF16 : K_TF32, NT, RES, false, false, R, true>(p);
+}
+template <int GEOM, int NT, bool RES = false, int R = 1>
+__global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc_ragged_f16(const ConvTcParams p) {
+    conv_tc_body<GEOM, K_F16, NT, RES, false, false, R, true>(p);
 }
 template <int GEOM, int NT, bool RES = false, int R = 1>
 __global__ void __launch_bounds__(NTHREADS, 1) k_conv_tc_ragged_x3(const ConvTcParams p) {
-    conv_tc_body<GEOM, false, NT, RES, true, false, R, true>(p);
+    conv_tc_body<GEOM, K_TF32, NT, RES, true, false, R, true>(p);
 }
 // a ragged Conv1d batch (ConvTcParams::lengths): tf32 / bf16, and fp32x3
 template <int GEOM, bool BF16, int NT>
 __global__ void __launch_bounds__(NTHREADS, 1) k_conv1d_ragged(const ConvTcParams p) {
-    conv_tc_body<GEOM, BF16, NT, false, false, false, 1, true>(p);
+    conv_tc_body<GEOM, BF16 ? K_BF16 : K_TF32, NT, false, false, false, 1, true>(p);
 }
 template <int GEOM, int NT>
 __global__ void __launch_bounds__(NTHREADS, 1) k_conv1d_ragged_x3(const ConvTcParams p) {
-    conv_tc_body<GEOM, false, NT, false, true, false, 1, true>(p);
+    conv_tc_body<GEOM, K_TF32, NT, false, true, false, 1, true>(p);
 }
 // the vocoder's transposed-conv GEMM in bf16 mode: bf16 operands, fp32 output Z (ConvTcParams::voc)
 template <int NT>
 __global__ void __launch_bounds__(NTHREADS, 1) k_gemm_voc_bf16(const ConvTcParams p) {
-    conv_tc_body<G_PW, true, NT, false, false, true>(p);
+    conv_tc_body<G_PW, K_BF16, NT, false, false, true>(p);
 }
 
 // the kernel of one launch configuration; VOC: the vocoder's bf16 GEMM; RAG: a ragged Conv1d or U-Net batch
@@ -959,10 +973,12 @@ template <int GEOM, int FORM, int NT, bool RES, int R, bool VOC, bool RAG>
 constexpr auto tc_kernel() {
     if constexpr (VOC) return k_gemm_voc_bf16<NT>;
     else if constexpr (RAG && !geom_is_c1(GEOM) && FORM == FORM_X3) return k_conv_tc_ragged_x3<GEOM, NT, RES, R>;
+    else if constexpr (RAG && !geom_is_c1(GEOM) && FORM == FORM_F16) return k_conv_tc_ragged_f16<GEOM, NT, RES, R>;
     else if constexpr (RAG && !geom_is_c1(GEOM)) return k_conv_tc_ragged<GEOM, FORM == FORM_BF16, NT, RES, R>;
     else if constexpr (RAG && FORM == FORM_X3) return k_conv1d_ragged_x3<GEOM, NT>;
     else if constexpr (RAG) return k_conv1d_ragged<GEOM, FORM == FORM_BF16, NT>;
     else if constexpr (FORM == FORM_X3) return k_conv_tc_x3<GEOM, NT, RES, R>;
+    else if constexpr (FORM == FORM_F16) return k_conv_tc_f16<GEOM, NT, RES, R>;
     else return k_conv_tc<GEOM, FORM == FORM_BF16, NT, RES, R>;
 }
 
@@ -970,6 +986,7 @@ template <int GEOM, int FORM, int NT, bool RES = false, int R = 1, bool VOC = fa
 static int launch_tc(const ConvTcParams& p, cudaStream_t s) {
     using D = Depth<GEOM, NT, R>;
     static_assert(!VOC || (GEOM == G_PW && FORM == FORM_BF16 && !RES), "VOC selects the bf16 GEMM with fp32 output");
+    static_assert(FORM != FORM_F16 || !geom_is_c1(GEOM), "fp16 runs the U-Net geometries only");
     constexpr auto kernel = tc_kernel<GEOM, FORM, NT, RES, R, VOC, RAG>();
     // the dynamic-shared-memory opt-in is a per-device function attribute and the persistent grid is sized from the
     // current device's SM count: both are cached per device ordinal (a process may drive several GPUs through several handles)
@@ -999,7 +1016,7 @@ int conv_tc_ntile(int geom, int Cout, int form) {
 
 // one launch configuration: geometry, operand form, N tile, output rows per tile, ResnetBlock tail, vocoder GEMM
 static constexpr int tc_key(int geom, int form, int nt, int rows = 1, bool res = false, bool voc = false) {
-    return ((((geom * 4 + form) * 256 + nt) * 2 + rows - 1) * 2 + (res ? 1 : 0)) * 2 + (voc ? 1 : 0);
+    return ((((geom * 8 + form) * 256 + nt) * 2 + rows - 1) * 2 + (res ? 1 : 0)) * 2 + (voc ? 1 : 0);
 }
 
 // Conv1d (vocoder): tf32 and bf16 at N tiles 128 / 64 / 32, fp32x3 at 64 / 32 (conv_tc_ntile); a dense or a ragged batch
@@ -1028,7 +1045,7 @@ static int launch_unet(const ConvTcParams& p, cudaStream_t s) {
 }
 
 int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
-    if (p.form < FORM_TF32 || p.form > FORM_BF16 || p.nt <= 0 || p.nt > 128 || p.Cout % p.nt != 0) return -1;
+    if (p.form < FORM_TF32 || p.form > FORM_F16 || p.nt <= 0 || p.nt > 128 || p.Cout % p.nt != 0) return -1;
     if (p.geom == G_PW && p.epi == EPI_KV) return launch_attn_kv(p, s);   // fused projection + softmax + context (sbk_attn_x3.cu)
     if (geom_is_c1(p.geom) && (p.dil < 1 || p.pad < 0 || 2 * p.pad > conv_tc_c1_halo(p.geom))) return -1;   // the strip's halo
     switch (p.geom) {                                // Conv1d (vocoder): K = 3, 5, 7, 11, each with the 64- and the 128-sample-halo strip
@@ -1045,7 +1062,7 @@ int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
     const int rows = p.geom == G_C3 && p.rows == 2 ? 2 : 1;
     const bool res = p.geom == G_PW && p.epi == EPI_RES;
     const bool voc = p.voc && p.geom == G_PW && p.form == FORM_BF16;     // the vocoder's GEMM: fp32 Z from bf16 operands
-    constexpr int T = FORM_TF32, X = FORM_X3, B = FORM_BF16;
+    constexpr int T = FORM_TF32, X = FORM_X3, B = FORM_BF16, F = FORM_F16;
     switch (tc_key(p.geom, p.form, p.nt, rows, res, voc)) {
         // 3x3: one-row tiles, and two-row tiles 64 channels wide
         case tc_key(G_C3, T, 128):                  return launch_unet<G_C3, T, 128>(p, s);
@@ -1057,6 +1074,9 @@ int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
         case tc_key(G_C3, X, 128):                  return launch_unet<G_C3, X, 128>(p, s);
         case tc_key(G_C3, X, 64):                   return launch_unet<G_C3, X, 64>(p, s);
         case tc_key(G_C3, X, 64, 2):                return launch_unet<G_C3, X, 64, false, 2>(p, s);
+        case tc_key(G_C3, F, 128):                  return launch_unet<G_C3, F, 128>(p, s);
+        case tc_key(G_C3, F, 64):                   return launch_unet<G_C3, F, 64>(p, s);
+        case tc_key(G_C3, F, 64, 2):                return launch_unet<G_C3, F, 64, false, 2>(p, s);
         // 1x1: plain, the ResnetBlock tail, and the vocoder's bf16 GEMM
         case tc_key(G_PW, T, 128):                  return launch_unet<G_PW, T, 128>(p, s);
         case tc_key(G_PW, T, 64):                   return launch_unet<G_PW, T, 64>(p, s);
@@ -1072,13 +1092,19 @@ int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
         case tc_key(G_PW, X, 64):                   return launch_unet<G_PW, X, 64>(p, s);
         case tc_key(G_PW, X, 128, 1, true):         return launch_unet<G_PW, X, 128, true>(p, s);
         case tc_key(G_PW, X, 64, 1, true):          return launch_unet<G_PW, X, 64, true>(p, s);
+        case tc_key(G_PW, F, 128):                  return launch_unet<G_PW, F, 128>(p, s);
+        case tc_key(G_PW, F, 64):                   return launch_unet<G_PW, F, 64>(p, s);
+        case tc_key(G_PW, F, 128, 1, true):         return launch_unet<G_PW, F, 128, true>(p, s);
+        case tc_key(G_PW, F, 64, 1, true):          return launch_unet<G_PW, F, 64, true>(p, s);
         // Downsample, Upsample
         case tc_key(G_DOWN, T, 64):                 return launch_unet<G_DOWN, T, 64>(p, s);
         case tc_key(G_DOWN, B, 64):                 return launch_unet<G_DOWN, B, 64>(p, s);
         case tc_key(G_DOWN, X, 64):                 return launch_unet<G_DOWN, X, 64>(p, s);
+        case tc_key(G_DOWN, F, 64):                 return launch_unet<G_DOWN, F, 64>(p, s);
         case tc_key(G_UP, T, 64):                   return launch_unet<G_UP, T, 64>(p, s);
         case tc_key(G_UP, B, 64):                   return launch_unet<G_UP, B, 64>(p, s);
         case tc_key(G_UP, X, 64):                   return launch_unet<G_UP, X, 64>(p, s);
+        case tc_key(G_UP, F, 64):                   return launch_unet<G_UP, F, 64>(p, s);
         // 7x7 (PostNet): tf32 and fp32x3, a dense or a ragged batch
         case tc_key(G_C7, T, 128):                  return launch_unet<G_C7, T, 128>(p, s);
         case tc_key(G_C7, T, 64):                   return launch_unet<G_C7, T, 64>(p, s);
@@ -1106,12 +1132,12 @@ static uint16_t f32_to_bf16_rn(float x) {
     u += 0x7FFFu + ((u >> 16) & 1u);
     return (uint16_t)(u >> 16);
 }
-// weight w -> its element of image g: tf32 (RNA), bf16 (RNE), or FORM_X3's w_hi = tf32(w) in the main stage and
-// {w, (w - w_hi) * 2^12} in the correction stage
+// weight w -> its element of image g: tf32 (RNA), bf16 (RNE), fp16 (RNE, saturating), or FORM_X3's w_hi = tf32(w) in the
+// main stage and {w, (w - w_hi) * 2^12} in the correction stage
 static void wimg_put(uint8_t* img, const ConvTcWImg& g, int co, int ks, int tap, int ch, int e, float w) {
     const size_t i = conv_tc_wimg_index(g, co, ks, tap, ch, e);
-    if (g.form == FORM_BF16) {
-        reinterpret_cast<uint16_t*>(img)[i] = f32_to_bf16_rn(w);
+    if (form_16bit(g.form)) {
+        reinterpret_cast<uint16_t*>(img)[i] = g.form == FORM_F16 ? f32_to_f16_rn(w) : f32_to_bf16_rn(w);
         return;
     }
     const uint32_t uh = f32_to_tf32_rna(w);

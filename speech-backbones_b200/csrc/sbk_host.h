@@ -4,6 +4,7 @@
 #include "../../include/sbk.h"
 #include "sbk_internal.h"
 
+#include <math.h>
 #include <string.h>
 
 #include <map>
@@ -131,17 +132,29 @@ struct Workspace {
     Arena arena() const { Arena a; a.base = (char*)mem; return a; }
 };
 
-// Element size of a debug-snapshot layout: 2 = bf16, 3 = float64, every other layout fp32.
-inline size_t snap_elem_bytes(int fmt) { return fmt == 2 ? 2 : (fmt == 3 ? 8 : 4); }
+// Element size of a debug-snapshot layout: 2 = bf16, 4 = fp16 (both [B][H][C/8][W][8]), 3 = float64, every other layout fp32.
+inline size_t snap_elem_bytes(int fmt) { return fmt == 2 || fmt == 4 ? 2 : (fmt == 3 ? 8 : 4); }
 
-// Copy `numel` elements of layout `fmt` from device memory to `dst` (host or device); bf16 is widened to fp32 (exact),
-// element order unchanged.
+// IEEE binary16 bits -> fp32 (exact)
+inline float f16_bits_to_f32(uint16_t h) {
+    const uint32_t s = (uint32_t)(h & 0x8000u) << 16, e = (h >> 10) & 0x1Fu, m = h & 0x3FFu;
+    if (e == 0) { const float f = ldexpf((float)m, -24); return s ? -f : f; }       // zero / subnormal
+    const uint32_t u = s | (e == 31 ? 0x7F800000u : (e + 112) << 23) | (m << 13);
+    float f; memcpy(&f, &u, 4);
+    return f;
+}
+
+// Copy `numel` elements of layout `fmt` from device memory to `dst` (host or device); bf16 and fp16 are widened to fp32
+// (exact), element order unchanged.
 inline int read_widened(void* dst, const void* src, size_t numel, int fmt) {
-    if (fmt != 2) { CU(cudaMemcpy(dst, src, numel * snap_elem_bytes(fmt), cudaMemcpyDefault)); return SBK_OK; }
+    if (fmt != 2 && fmt != 4) { CU(cudaMemcpy(dst, src, numel * snap_elem_bytes(fmt), cudaMemcpyDefault)); return SBK_OK; }
     std::vector<uint16_t> h16(numel);
     CU(cudaMemcpy(h16.data(), src, numel * 2, cudaMemcpyDeviceToHost));
     std::vector<float> h32(numel);
-    for (size_t i = 0; i < numel; ++i) { const uint32_t u = (uint32_t)h16[i] << 16; memcpy(&h32[i], &u, 4); }
+    for (size_t i = 0; i < numel; ++i) {
+        if (fmt == 4) { h32[i] = f16_bits_to_f32(h16[i]); continue; }
+        const uint32_t u = (uint32_t)h16[i] << 16; memcpy(&h32[i], &u, 4);
+    }
     CU(cudaMemcpy(dst, h32.data(), numel * sizeof(float), cudaMemcpyDefault));
     return SBK_OK;
 }

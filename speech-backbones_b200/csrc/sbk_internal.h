@@ -103,23 +103,27 @@ enum Form {
     FORM_TF32 = 1,              // fp32 [B][H][C/4][W][4]; the Block activation is rounded to tf32 (cvt.rna), fast Mish
     FORM_X3 = 2,                // fp32 [B][H][C/4][W][4], exact Mish; the convs derive the correction operand (corr_chunk)
     FORM_BF16 = 3,              // bf16 [B][H][C/8][W][8], fast Mish
+    FORM_F16 = 4,               // fp16 [B][H][C/8][W][8] (FORM_BF16's layout), RNE saturating to +-65504, fast Mish
 };
+// the forms whose operand tensors and weight images hold 16-bit elements, 8 per 16-byte chunk
+__host__ __device__ constexpr bool form_16bit(int form) { return form == FORM_BF16 || form == FORM_F16; }
 
 // Tensor-core (wgmma) convolution (sbk_conv_tc.cu).  Inputs are operand-form tensors: already masked / activated, so the
 // kernel's A path is a pure copy.  geom = G_C3 (3x3, pad 1) or G_PW (1x1 over the flattened image).
 struct ConvTcParams {
     int geom;
-    int form;                                       // operand form: FORM_TF32 | FORM_X3 | FORM_BF16
-    const void* in0; const void* in1; int c0, c1;   // channel concat of two operand tensors: fp32 [B][H][C/4][W][4], or bf16
-                                                    // [B][H][C/8][W][8] in FORM_BF16 (16-byte channel chunks either way)
+    int form;                                       // operand form: FORM_TF32 | FORM_X3 | FORM_BF16 | FORM_F16
+    const void* in0; const void* in1; int c0, c1;   // channel concat of two operand tensors: fp32 [B][H][C/4][W][4], or bf16 /
+                                                    // fp16 [B][H][C/8][W][8] in FORM_BF16 / FORM_F16 (16-byte channel chunks
+                                                    // either way)
     int H, W, B;                                    // input grid
     int Ho, Wo;                                     // output grid (G_DOWN: ~H/2 x W/2, G_UP: 2H x 2W; else = H, W)
     const void* wpk; long long w_bstride_bytes;     // weight image conv_tc_pack_image(.., nt, ..) (+ per-sample stride)
     const float* bias; long long bias_bstride;      // per-sample bias stride, 0 in every engine.  Kept: dropping the term
                                                     // reschedules every conv kernel, and bench.py's fp32x3 rate fell 0.4 %
                                                     // without it (H100 80GB HBM3, 700 W)
-    float* out; int Cout;                           // FORM_BF16: G_C3 still writes fp32 raw [C/4] (GroupNorm input); the other
-                                                    // geometries write bf16 operand tensors [C/8] through this pointer
+    float* out; int Cout;                           // FORM_BF16 / FORM_F16: G_C3 still writes fp32 raw [C/4] (GroupNorm input);
+                                                    // the other geometries write 16-bit operand tensors [C/8] through this pointer
     int epi;                                        // EPI_PLAIN | EPI_RES | EPI_KV
     double* ostats;                                 // EPI_PLAIN: GroupNorm statistics of the raw output (nullable)
     const float* mask; int T; int lvl; int out_mask;   // out_mask: multiply the stored output by mask[b][wo << lvl]
@@ -169,12 +173,12 @@ __device__ __forceinline__ int ragged_edge(const int64_t* lengths, long long b, 
 // ---- the wgmma conv's weight image: per N tile and K stage exactly the stage's shared-memory image --------------------
 //   [ntile][kstage][main | correction][tap][16-byte chunk][co % nt][e]
 // A K stage holds `taps` taps (7x7: the 7 of one kernel row) x `kch` 16-byte chunks of input channels, e = 4 tf32 elements
-// per chunk (8 bf16).  FORM_X3 streams a (main, correction) stage pair per K stage: the main stage holds w_hi = tf32(w)
+// per chunk (8 bf16 or fp16).  FORM_X3 streams a (main, correction) stage pair per K stage: the main stage holds w_hi = tf32(w)
 // (RNA), the correction stage per chunk the 8 fp16 {w[c0..c3], (w - w_hi)[c0..c3] * 2^12} that pair with the
 // activations' corr_chunk in one f16 MMA.  The other forms have no correction stage.
 struct ConvTcWImg { int form, nt, ksteps, taps, kch; };        // ksteps: K stages per N tile
 
-__host__ __device__ constexpr int form_epc(int form) { return form == FORM_BF16 ? 8 : 4; }      // elements per 16-byte chunk
+__host__ __device__ constexpr int form_epc(int form) { return form_16bit(form) ? 8 : 4; }      // elements per 16-byte chunk
 __host__ __device__ constexpr int conv_tc_taps(int geom) {
     return geom == G_PW ? 1 : geom == G_UP ? 16 : geom == G_C1K3 || geom == G_C1K3W ? 3 : geom == G_C1K5 || geom == G_C1K5W ? 5
          : geom == G_C1K7 || geom == G_C1K7W ? 7 : geom == G_C1K11 || geom == G_C1K11W ? 11 : geom == G_C7 ? 49 : 9;
@@ -189,13 +193,13 @@ __host__ __device__ inline ConvTcWImg conv_tc_wimg(int geom, int form, int nt, i
 // elements of one (main or correction) stage
 __host__ __device__ inline size_t conv_tc_wimg_stage(const ConvTcWImg& g) { return (size_t)g.taps * g.kch * g.nt * form_epc(g.form); }
 // index of element e of chunk ch of output channel co at tap `tap` of K stage ks, in elements of the main stage (4 bytes,
-// bf16: 2); corr = 1: the same chunk's place in the correction stage, in 4-byte units
+// bf16 / fp16: 2); corr = 1: the same chunk's place in the correction stage, in 4-byte units
 __host__ __device__ inline size_t conv_tc_wimg_index(const ConvTcWImg& g, int co, int ks, int tap, int ch, int e, int corr = 0) {
     return (((size_t)(co / g.nt) * g.ksteps + ks) * (g.form == FORM_X3 ? 2 : 1) + corr) * conv_tc_wimg_stage(g) +
            (((size_t)tap * g.kch + ch) * g.nt + co % g.nt) * form_epc(g.form) + e;
 }
 __host__ __device__ inline size_t conv_tc_wimg_bytes(const ConvTcWImg& g, int cout) {
-    return (size_t)(cout / g.nt) * g.ksteps * (g.form == FORM_X3 ? 2 : 1) * conv_tc_wimg_stage(g) * (g.form == FORM_BF16 ? 2 : 4);
+    return (size_t)(cout / g.nt) * g.ksteps * (g.form == FORM_X3 ? 2 : 1) * conv_tc_wimg_stage(g) * (form_16bit(g.form) ? 2 : 4);
 }
 
 // Block activation between the two convs of a ResnetBlock, written once in operand form (diffusion.py:57,76):
@@ -204,7 +208,7 @@ struct GnActParams {          // (a ragged batch: gn.lengths, edge rule gn.exact
     const float* raw; GnRef gn; const float* tb; int tb_stride; int tb_per_sample; const int* step;
     const float* mask; int T; int lvl;
     float* out; int B, H, W, C;
-    int form;                   // FORM_TF32 | FORM_X3 | FORM_BF16
+    int form;                   // FORM_TF32 | FORM_X3 | FORM_BF16 | FORM_F16
 };
 
 struct FirstConvParams {        // Block.conv of downs.0.0.block1 on the planar stack([mu, xt(, s)]) * mask

@@ -10,6 +10,7 @@
 // epilogue (fp64 atomics of per-CTA fp32 partials), and the consumer applies
 // (x-mean)*rstd*gamma+beta -> Mish -> mask (+ time projection) in its operand prologue.
 #include "sbk_internal.h"
+#include "sbk_tc.cuh"
 
 #include <math.h>
 #include <type_traits>
@@ -616,8 +617,8 @@ __global__ void __launch_bounds__(256) k_resfinal_nhwc(const ResFinalParams p) {
 // A CTA owns ONE output channel chunk, whose GN / time / residual parameters live in registers for the whole kernel, and
 // walks mel bins 4 at a time; a thread owns frame(s) w, so the mask is read once and every index is 32-bit and
 // division-free (a generic flat loop was issue-bound on 64-bit divisions).  In the fp32 forms a chunk is 4 channels and a
-// lane owns a frame.  In bf16 a chunk is 8 channels and a LANE PAIR owns a frame: lane half h handles the fp32 raw chunk
-// 2*ch+h (the same register footprint as the fp32 forms) and writes its 8-byte half of the 16-byte bf16 chunk, so loads are
+// lane owns a frame.  In bf16 / fp16 a chunk is 8 channels and a LANE PAIR owns a frame: lane half h handles the fp32 raw
+// chunk 2*ch+h (the same register footprint as the fp32 forms) and writes its 8-byte half of the 16-byte chunk, so loads are
 // two interleaved 256-byte runs per warp and stores one contiguous 256-byte run.
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t pack_bf16x2_f(float lo, float hi) {
@@ -625,10 +626,12 @@ __device__ __forceinline__ uint32_t pack_bf16x2_f(float lo, float hi) {
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
     return d;
 }
-__device__ __forceinline__ float bf16_lo_f(uint32_t u) { return __uint_as_float(u << 16); }
-__device__ __forceinline__ float bf16_hi_f(uint32_t u) { return __uint_as_float(u & 0xFFFF0000u); }
-__device__ __forceinline__ float4 opnd_f32(float4 v) { return v; }
-__device__ __forceinline__ float4 opnd_f32(uint2 v) { return make_float4(bf16_lo_f(v.x), bf16_hi_f(v.x), bf16_lo_f(v.y), bf16_hi_f(v.y)); }
+// 4 channels of an operand tensor of form FORM -> fp32 (exact)
+template <int FORM> __device__ __forceinline__ float4 opnd_f32(float4 v) { return v; }
+template <int FORM> __device__ __forceinline__ float4 opnd_f32(uint2 v) {
+    using E = tc::E16<tc::form_kind16(FORM)>;
+    return make_float4(E::lo(v.x), E::hi(v.x), E::lo(v.y), E::hi(v.y));
+}
 __device__ __forceinline__ float rna_tf32(float x) {
     uint32_t t;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t) : "f"(x));
@@ -636,7 +639,7 @@ __device__ __forceinline__ float rna_tf32(float x) {
 }
 
 enum Tail { TAIL_ACT, TAIL_ID, TAIL_PLANAR };
-__host__ __device__ constexpr int lanes_per_frame(int form) { return form == FORM_BF16 ? 2 : 1; }
+__host__ __device__ constexpr int lanes_per_frame(int form) { return form_16bit(form) ? 2 : 1; }
 
 // grid.x = (channel chunks) x (mel-bin groups); a 256-thread CTA covers min(W, F) frames x F / min(W, F) bin sub-groups
 // (F = 256 / lanes per frame), each walking 4 bins per pass, ~2 passes per thread
@@ -652,7 +655,7 @@ static int planar_ew_grid(int form, int H, int W, int C) {
 // reader of this output looks at them.  (A template flag: the edge in a register would cost the dense loop a spill.)
 template <int FORM, int TAIL, bool RAG, class P>
 __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
-    constexpr bool B16 = FORM == FORM_BF16, X3 = FORM == FORM_X3;
+    constexpr bool B16 = form_16bit(FORM), X3 = FORM == FORM_X3;
     constexpr int LPF = lanes_per_frame(FORM), F = 256 / LPF;
     constexpr int U = 4;                         // independent 16-byte loads in flight per thread
     using Unit = typename std::conditional<B16, uint2, float4>::type;   // a thread's 4 channels of an operand tensor
@@ -694,7 +697,7 @@ __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
         if (p.r_extra) rx = ldg4(p.r_extra + ((long long)(p.extra_per_sample_row ? 0 : *p.step) * p.B + b) * p.C + c4 * 4);
         has_spk = p.cin > 2 && !p.r_extra;      // = a third real weight row
     }
-    // this chunk's res_conv bias and weight rows: bf16, whose launch bounds leave room, holds them in registers; the fp32
+    // this chunk's res_conv bias and weight rows: bf16 / fp16, whose launch bounds leave room, holds them in registers; the fp32
     // forms re-read them from shared memory per element (broadcast loads), which keeps them under the registers of the
     // fp32 kernels this walk replaced
     float4 wb = z4, w0 = z4, w1 = z4, w2 = z4;
@@ -742,7 +745,7 @@ __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
                     if (p.out_mask) { o.x *= mk; o.y *= mk; o.z *= mk; o.w *= mk; }
                 } else if (mk != 0.f) {
                     float4 a;
-                    if constexpr (TAIL == TAIL_ACT) a = pt; else a = opnd_f32(xv[u]);
+                    if constexpr (TAIL == TAIL_ACT) a = pt; else a = opnd_f32<FORM>(xv[u]);
                     o.x = mish_sel<X3>((r[u].x - pm.x) * ps.x + pb.x) + a.x;
                     o.y = mish_sel<X3>((r[u].y - pm.y) * ps.y + pb.y) + a.y;
                     o.z = mish_sel<X3>((r[u].z - pm.z) * ps.z + pb.z) + a.z;
@@ -751,7 +754,8 @@ __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
                 }
                 const long long oi = obase + (long long)(h0 + u) * ohs + w * LPF;
                 if constexpr (B16) {
-                    reinterpret_cast<uint2*>(p.out)[oi] = make_uint2(pack_bf16x2_f(o.x, o.y), pack_bf16x2_f(o.z, o.w));
+                    using E = tc::E16<tc::form_kind16(FORM)>;
+                    reinterpret_cast<uint2*>(p.out)[oi] = make_uint2(E::pack(o.x, o.y), E::pack(o.z, o.w));
                 } else {
                     reinterpret_cast<float4*>(p.out)[oi] = o;
                 }
@@ -763,9 +767,9 @@ __device__ __forceinline__ void planar_ew(const P& p, const float* raw) {
 template <int FORM, bool RAG>
 __global__ void __launch_bounds__(256) k_gn_act(const GnActParams p) { planar_ew<FORM, TAIL_ACT, RAG>(p, p.raw); }
 
-// the bf16 identity tail keeps to 64 registers for 4 CTAs per SM; its planar-input tail needs more and runs 2 (0: no minimum)
+// the 16-bit identity tail keeps to 64 registers for 4 CTAs per SM; its planar-input tail needs more and runs 2 (0: no minimum)
 template <int FORM, bool PLANAR, bool RAG>
-__global__ void __launch_bounds__(256, FORM == FORM_BF16 ? (PLANAR ? 2 : 4) : 0) k_resfinal(const ResFinalParams p) {
+__global__ void __launch_bounds__(256, form_16bit(FORM) ? (PLANAR ? 2 : 4) : 0) k_resfinal(const ResFinalParams p) {
     planar_ew<FORM, PLANAR ? TAIL_PLANAR : TAIL_ID, RAG>(p, p.h2raw);
 }
 
@@ -782,6 +786,7 @@ int launch_gn_act(const GnActParams& p, cudaStream_t s) {
         case FORM_TF32: launch_gn_act_form<FORM_TF32>(p, s); return 1;
         case FORM_X3:   launch_gn_act_form<FORM_X3>(p, s); return 1;
         case FORM_BF16: launch_gn_act_form<FORM_BF16>(p, s); return 1;
+        case FORM_F16:  launch_gn_act_form<FORM_F16>(p, s); return 1;
     }
     return -1;
 }
@@ -812,6 +817,7 @@ int launch_resfinal(const ResFinalParams& p, cudaStream_t s) {
         case FORM_TF32: launch_resfinal_planar<FORM_TF32>(p, sm, s); return 1;
         case FORM_X3:   launch_resfinal_planar<FORM_X3>(p, sm, s); return 1;
         case FORM_BF16: launch_resfinal_planar<FORM_BF16>(p, sm, s); return 1;
+        case FORM_F16:  launch_resfinal_planar<FORM_F16>(p, sm, s); return 1;
     }
     return -1;
 }
@@ -950,6 +956,8 @@ __global__ void __launch_bounds__(256) k_attn_mix(const AttnMixParams p) {
                     cb16[4 + e] = (unsigned short)(f16x2_sat((v - __uint_as_float(uh)) * kCorrUp, 0.f) & 0xFFFFu);
                 } else if (p.form == FORM_BF16) {
                     reinterpret_cast<unsigned short*>(wb)[idx] = (unsigned short)(pack_bf16x2_f(v, 0.f) & 0xFFFFu);
+                } else if (p.form == FORM_F16) {
+                    reinterpret_cast<unsigned short*>(wb)[idx] = (unsigned short)(f16x2_sat(v, 0.f) & 0xFFFFu);
                 } else {
                     uint32_t u; asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v));
                     reinterpret_cast<float*>(wb)[idx] = __uint_as_float(u);

@@ -112,8 +112,8 @@ size_t pn_carve(int B, int H, int C, int T, Arena& ar, PnBufs* o) {
 }  // namespace
 
 struct sbk_postnet {
-    // precision: the fp32-class modes run the fp32x3 path (prec_runs_x3), tf32 and bf16 the tf32 path (bf16 operands are not
-    // implemented for the 7x7 geometry)
+    // precision: the fp32-class modes run the fp32x3 path (prec_runs_x3), tf32, bf16 and fp16 the tf32 path (16-bit operands
+    // are not implemented for the 7x7 geometry)
     sbk_postnet_config cfg;
     WeightSet w;                             // raw: reference layout; packed: tensor-core stage images
     float* zero = nullptr;                   // zero page: A-tile borders, and k_gn_act's (absent) time bias
@@ -133,7 +133,7 @@ extern "C" int sbk_postnet_create(const sbk_postnet_config* cfg, sbk_postnet** o
     const int d = cfg->dim;
     if (d <= 0 || d % 64 != 0 || (d > 128 && d % 256 != 0))
         return fail(SBK_ERR_UNSUPPORTED, "sbk_postnet_create: dim = %d; supported: 64, 128 and multiples of 256", d);
-    if (cfg->precision < SBK_PREC_FP32 || cfg->precision > SBK_PREC_FP32X3)
+    if (cfg->precision < SBK_PREC_FP32 || cfg->precision > SBK_PREC_F16)
         return fail(SBK_ERR_ARG, "sbk_postnet_create: unknown precision %d", cfg->precision);
     sbk_postnet* p = new sbk_postnet();
     p->cfg = *cfg;

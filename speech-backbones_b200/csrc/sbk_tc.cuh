@@ -4,6 +4,7 @@
 #include "sbk_internal.h"
 
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <math.h>
 #include <stdint.h>
 
@@ -163,6 +164,24 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
     return d;
 }
+__device__ __forceinline__ float f16_lo(uint32_t u) { return __half2float(__ushort_as_half((unsigned short)(u & 0xFFFFu))); }
+__device__ __forceinline__ float f16_hi(uint32_t u) { return __half2float(__ushort_as_half((unsigned short)(u >> 16))); }
+
+// The 16-bit operand element of an MMA kind (K_BF16 or K_F16): pack two floats (RNE; fp16 saturates to +-65504 instead of
+// overflowing to inf) and widen the low / high half of a packed pair.  Every 16-bit operand path is written once over it.
+template <int KIND> struct E16;
+template <> struct E16<K_BF16> {
+    static __device__ __forceinline__ uint32_t pack(float lo, float hi) { return pack_bf16x2(lo, hi); }
+    static __device__ __forceinline__ float lo(uint32_t u) { return bf16_lo(u); }
+    static __device__ __forceinline__ float hi(uint32_t u) { return bf16_hi(u); }
+};
+template <> struct E16<K_F16> {
+    static __device__ __forceinline__ uint32_t pack(float lo, float hi) { return f16x2_sat(lo, hi); }
+    static __device__ __forceinline__ float lo(uint32_t u) { return f16_lo(u); }
+    static __device__ __forceinline__ float hi(uint32_t u) { return f16_hi(u); }
+};
+// the MMA kind of a 16-bit operand form
+__host__ __device__ constexpr int form_kind16(int form) { return form == FORM_F16 ? K_F16 : K_BF16; }
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");

@@ -266,6 +266,9 @@ extern "C" void sbk_vocoder_destroy(sbk_vocoder* v) {
 // Host logic only (no device work): the mode's tiling rules, then the packed state is dropped.
 extern "C" int sbk_vocoder_set_precision(sbk_vocoder* v, int32_t precision) {
     if (!v) return fail(SBK_ERR_ARG, "sbk_vocoder_set_precision: null handle");
+    if (precision == SBK_PREC_F16)
+        return fail(SBK_ERR_UNSUPPORTED, "sbk_vocoder_set_precision: fp16 is a sampler mode; the vocoder has no fp16 kernels "
+                                         "(use tf32, bf16 or fp32x3)");
     if (precision < SBK_PREC_FP32 || precision > SBK_PREC_FP32X3) return fail(SBK_ERR_ARG, "sbk_vocoder_set_precision: unknown precision %d", precision);
     if (prec_bf16(precision)) {
         // bf16 K stages hold 16 input channels (Conv1d) and 64 (GEMM, sbk_conv_tc.cu conv_tc_stage_channels).  Every stage

@@ -190,7 +190,8 @@ class Diffusion(BaseModule):
     """Score-based decoder.  `precision`/`use_graph` are extra, keyword-only engine knobs.  The default precision
     "fp32x3" is fp32-class arithmetic on the tensor cores (tf32 main product + one fp16 correction product per MAC, exact fp32 everywhere else): it matches
     the reference's fp32 path to ~1e-6 per estimator call.  "tf32" is what PyTorch's own GPU convs compute by default
-    (~1.5e-3 per call), "bf16" is config 3's arithmetic, "fp32" the CUDA-core FFMA path."""
+    (~1.5e-3 per call), "bf16" is config 3's arithmetic, "fp16" runs bf16's operand bytes and MMA rate with fp16 operands
+    (tf32-class error; operands saturate at +-65504), "fp32" the CUDA-core FFMA path."""
 
     def __init__(self, n_feats, dim, n_spks=1, spk_emb_dim=64, beta_min=0.05, beta_max=20, pe_scale=1000,
                  *, precision="fp32x3", use_graph=True):

@@ -25,7 +25,8 @@ them.  The Conv1d work past each utterance's end is skipped, so a ragged batch c
 
 `Generator(h, precision=...)` picks the operand arithmetic of those convs (the binding's PREC names): "tf32" (the default),
 "fp32x3" ("fp32" maps to it: fp32-class results on the tensor cores) or "bf16".  In the bf16 mode `forward` also takes a
-bfloat16 mel (widened to float32 first); the waveform is float32 in every mode.
+bfloat16 mel (widened to float32 first); the waveform is float32 in every mode.  "fp16" is a sampler mode only: the vocoder
+has no fp16 kernels, and asking for it raises ValueError.
 """
 from __future__ import annotations
 
@@ -36,6 +37,14 @@ import torch.nn as nn
 from torch.nn.utils import remove_weight_norm, weight_norm
 
 from .binding import PREC, _check, _check_precision, _NativeHandle, _ptr, check_lengths
+
+
+def _check_vocoder_precision(precision):
+    """one of the binding's PREC names; the samplers' "fp16" is refused with its reason (sbk_vocoder_set_precision)"""
+    if precision == "fp16":
+        raise ValueError('precision "fp16" is a sampler mode: the vocoder has no fp16 kernels '
+                         '(use "tf32", "bf16" or "fp32x3")')
+    return _check_precision(precision)
 
 
 class SbkVocoderConfig(C.Structure):
@@ -95,7 +104,7 @@ class VocoderEngine(_NativeHandle):
     STATE_DICT = "the vocoder state_dict"
 
     def __init__(self, h, device, precision="tf32"):
-        self.precision = _check_precision(precision)
+        self.precision = _check_vocoder_precision(precision)
         super().__init__()
         P, I = C.c_void_p, C.c_int
         self.lib.sbk_vocoder_set_precision.argtypes = [P, C.c_int32]
@@ -219,7 +228,7 @@ class Generator(nn.Module):
     def __init__(self, h, *, precision="tf32"):
         super().__init__()
         self.h = h
-        self.precision = _check_precision(precision)
+        self.precision = _check_vocoder_precision(precision)
         rates, ks = list(_get(h, "upsample_rates")), list(_get(h, "upsample_kernel_sizes"))
         rk, rd = list(_get(h, "resblock_kernel_sizes")), [list(d) for d in _get(h, "resblock_dilation_sizes")]
         c0 = int(_get(h, "upsample_initial_channel"))

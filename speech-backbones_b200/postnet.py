@@ -6,8 +6,8 @@ unchanged, and the same `forward(x, mask)` -> [B, n_feats, T].  The modules belo
 libsbk.so (`sbk_postnet_forward`: the two 7x7 convs on wgmma, csrc/sbk_postnet.cu).  Inference only: there is no CPU path
 and no autograd through this module.  `forward(x, mask, lengths=...)` runs a ragged batch, each row exactly its own call.
 
-`precision`: "fp32x3" (default; "fp32" maps to it) runs the fp32-class tf32 + fp16-correction split, "tf32" ("bf16" maps to
-it) plain tf32 operands.  The mapping lives in the library (sbk_postnet.cu)."""
+`precision`: "fp32x3" (default; "fp32" maps to it) runs the fp32-class tf32 + fp16-correction split, "tf32" ("bf16" and
+"fp16" map to it) plain tf32 operands.  The mapping lives in the library (sbk_postnet.cu)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -15,7 +15,7 @@ import ctypes as C
 import torch
 import torch.nn as nn
 
-from .binding import PREC, _check, _check_precision, _NativeHandle, _ptr, check_lengths
+from .binding import SAMPLER_PREC, _check, _check_precision, _NativeHandle, _ptr, check_lengths
 from .gradtts import BaseModule, Mish
 
 
@@ -58,7 +58,7 @@ class PostNetEngine(_NativeHandle):
         self.lib.sbk_postnet_debug_name.restype = C.c_char_p
         self.lib.sbk_postnet_debug_op_layout.argtypes = [P, C.c_char_p]
         self.lib.sbk_postnet_debug_read.argtypes = [P, C.c_char_p, P, C.POINTER(C.c_int64)]
-        rc = self._create(SbkPostNetConfig(device, dim, groups, PREC[precision]))
+        rc = self._create(SbkPostNetConfig(device, dim, groups, SAMPLER_PREC[precision]))
         if rc == _SBK_ERR_UNSUPPORTED:
             raise ValueError(self.lib.sbk_last_error().decode())
         _check(rc, "sbk_postnet_create")
@@ -115,7 +115,7 @@ class PostNetEngine(_NativeHandle):
 class PostNet(BaseModule):
     def __init__(self, dim, groups=8, *, precision="fp32x3"):
         super().__init__()
-        _check_precision(precision)
+        _check_precision(precision, SAMPLER_PREC)
         PostNetEngine(dim, groups, precision=precision).close()     # the library's config check (host logic): ValueError
         self.dim, self.groups, self.precision = dim, groups, precision
         self.init_conv = nn.Conv2d(1, dim, 1)

@@ -2,8 +2,8 @@
 
 Each slot holds one request - the arguments of one B = 1 `Diffusion.forward` call - at its own step of its own
 n_timesteps.  When a request finishes, its mel is read out and its slot freed, and the next queued request takes the slot
-at the next step boundary.  A finished mel equals `Diffusion.forward` on that utterance alone (bit for bit in tf32 and
-bf16, within fp32 rounding in fp32x3 and fp32), whatever the other slots hold and whenever it was admitted (sbk.h:
+at the next step boundary.  A finished mel equals `Diffusion.forward` on that utterance alone (bit for bit in tf32,
+bf16 and fp16, within fp32 rounding in fp32x3 and fp32), whatever the other slots hold and whenever it was admitted (sbk.h:
 sbk_rolling_*).
 
 The queue and the schedule live here, in Python.  The schedule is deterministic, so the host knows when each slot finishes
