@@ -467,6 +467,39 @@ int sbk_postnet_debug_op_layout(const sbk_postnet* p, const char* name);
  * through *numel; dst may be NULL to query it */
 int sbk_postnet_debug_read(sbk_postnet* p, const char* name, void* dst, int64_t* numel);
 
+/* ---- DiffVC's inference front end (DiffVC/inference.ipynb: get_mel, mel_spectral_subtraction) ----------------------------
+ * A handle without weights: the windowed-DFT basis and the Slaney filterbank are built on the host from the notebook's
+ * constants (22050 Hz, n_fft 1024, hop 256, 80 mels, 0 - 8000 Hz).  Creating a handle and sizing its workspace are host logic
+ * (no GPU work); the first call uploads the basis to cfg.device. */
+typedef struct sbk_frontend sbk_frontend;
+typedef struct sbk_frontend_config {
+    int32_t device;
+} sbk_frontend_config;
+int sbk_frontend_create(const sbk_frontend_config* cfg, sbk_frontend** out);
+void sbk_frontend_destroy(sbk_frontend* h);
+/* bins 0 .. n - 1 the DFT computes: up to the filterbank's last nonzero bin (371 at 8 kHz) */
+int sbk_frontend_dft_bins(const sbk_frontend* h);
+/* device workspace of a log-mel call of B utterances and T frames (allocated by the calls, grow-only); it also covers a
+ * spectral subtraction of [B, n_mels, T] */
+size_t sbk_frontend_workspace_bytes(const sbk_frontend* h, int B, int T);
+/* get_mel without decoding or resampling: wav [B, L] fp32 at 22050 Hz -> out [B, 80, T] fp32.  lengths (device int64 [B],
+ * NULL = every utterance L samples): utterance b is wav[b, :lengths[b]], truncated to T_b = lengths[b] / 256 whole hops and
+ * reflect-padded by 384 samples at its own edges; out[b, :, :T_b] is log(max(mel_basis @ |STFT|, 1e-5)) and out[b, :, T_b:]
+ * is 0.  Samples at or past lengths[b] are not read.  The DFT runs on wgmma in the fp32x3 split.  Callers validate the
+ * lengths (each in 512 .. L) and pass T = max_b T_b (<= L / 256); the kernels clamp a length to [0, L] and write zeros for an
+ * utterance of fewer than 2 hops.  Each row is bit for bit the B = 1 call on its own samples.  Asynchronous on `stream`. */
+int sbk_logmel_forward_lengths(sbk_frontend* h, const float* wav, const int64_t* lengths, float* out, int B, int L, int T,
+                               void* stream);
+/* mel_spectral_subtraction(mel_synth, mel_source, spectral_floor, silence_window, smoothing_window) on [B, n_mels, T] fp32,
+ * one utterance per CTA: row b is the function on its first lengths[b] frames (device int64 [B], clamped to [1, T]; NULL =
+ * all T) followed by zeros.  Window energies accumulate in fp64; smoothing_window = -1 skips noise_median_smoothing.
+ * SBK_ERR_ARG for silence_window < 1 or smoothing_window = 0 or < -1. */
+int sbk_spectral_subtraction_lengths(sbk_frontend* h, const float* mel_synth, const float* mel_source, const int64_t* lengths,
+                                     float* out, int B, int n_mels, int T, float spectral_floor, int silence_window,
+                                     int smoothing_window, void* stream);
+/* kernel launches the last call enqueued */
+int64_t sbk_frontend_last_launch_count(const sbk_frontend* h);
+
 const char* sbk_last_error(void);
 const char* sbk_version(void);
 

@@ -27,6 +27,8 @@ EXPORTS = [
     "sbk_vc_estimator_lengths", "sbk_vc_reverse_diffusion_lengths", "sbk_vc_conditioning_lengths",
     "sbk_rolling_reserve", "sbk_rolling_admit", "sbk_rolling_advance", "sbk_rolling_read", "sbk_rolling_release",
     "sbk_vc_rolling_reserve", "sbk_vc_rolling_admit",
+    "sbk_frontend_create", "sbk_frontend_destroy", "sbk_frontend_dft_bins", "sbk_frontend_workspace_bytes",
+    "sbk_logmel_forward_lengths", "sbk_spectral_subtraction_lengths", "sbk_frontend_last_launch_count",
 ]
 
 
@@ -35,6 +37,10 @@ class SbkConfig(C.Structure):
                 ("spk_emb_dim", C.c_int32), ("beta_min", C.c_float), ("beta_max", C.c_float),
                 ("pe_scale", C.c_float), ("device", C.c_int32), ("precision", C.c_int32),
                 ("use_graph", C.c_int32), ("dim_cond", C.c_int32), ("use_ref_t", C.c_int32)]
+
+
+class SbkFrontendConfig(C.Structure):
+    _fields_ = [("device", C.c_int32)]
 
 
 _lib = None
@@ -88,6 +94,16 @@ def load_library() -> C.CDLL:
     lib.sbk_vc_cond_debug_op_layout.argtypes = [P, C.c_char_p]
     lib.sbk_vc_cond_debug_read.argtypes = [P, C.c_char_p, F, C.POINTER(C.c_int64)]
     lib.sbk_profile_ops.argtypes = [P, F, F, F, I, C.POINTER(C.c_int)]
+    lib.sbk_frontend_create.argtypes = [C.POINTER(SbkFrontendConfig), C.POINTER(C.c_void_p)]
+    lib.sbk_frontend_destroy.argtypes = [P]
+    lib.sbk_frontend_destroy.restype = None
+    lib.sbk_frontend_dft_bins.argtypes = [P]
+    lib.sbk_frontend_workspace_bytes.argtypes = [P, I, I]
+    lib.sbk_frontend_workspace_bytes.restype = C.c_size_t
+    lib.sbk_logmel_forward_lengths.argtypes = [P, F, P, F, I, I, I, P]
+    lib.sbk_spectral_subtraction_lengths.argtypes = [P, F, F, P, F, I, I, I, C.c_float, I, I, P]
+    lib.sbk_frontend_last_launch_count.argtypes = [P]
+    lib.sbk_frontend_last_launch_count.restype = C.c_int64
     lib.sbk_last_error.restype = C.c_char_p
     lib.sbk_version.restype = C.c_char_p
     _lib = lib
